@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- image-pairs/sec of the UniMatch matching path on B200 (BASELINE.json metric).
+"""bench.py -- image-pairs/sec of the UniMatch matching path on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload config4|config2|config3|config5]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -12,6 +13,8 @@ Prints ONE JSON line (rank 0).  `value`: inputs resident in HBM; `e2e`: host pin
 the timed region.  `--impl reference` times the CPU oracle port of the reference path on the host's physical cores.
 `epe_vs_reference` compares pair 0 of the GPU output with the oracle (== reference) and carries its tolerance and a pass flag;
 a failing parity check makes the process exit non-zero after printing the line.
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (the final flow / disparity / depth of the
+batch, float32) as DIR/<name>.npy, so that two builds can be compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -43,7 +46,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], tflops=d["bf16_tflops_sustained"], tflops_burst=d["bf16_tflops"], source="measured")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, tflops_burst=1590.0, source="fallback")
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_burst=989.0, source="data sheet")
 
 
 def physical_cores():
@@ -73,7 +77,7 @@ def physical_cores():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -148,6 +152,8 @@ def main():
     ap.add_argument("--no-ref-gpu", action="store_true", help="skip the reference-eager-on-this-GPU line (oracle port on cuda, TF32 off)")
     ap.add_argument("--profile", action="store_true", help="1 warm-up + K steps of the resident path only (for ncu launch lists)")
     ap.add_argument("--graph", action="store_true", help="replay the forward as a CUDA graph")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -165,7 +171,7 @@ def main():
     config = {"workload": "%s %dx%d, %d pairs/GPU (BASELINE configs[%d])" % (wl_name, H, W, Bp, cfg_idx),
               "global_batch": Bp * world, "parallelism": "dp%d (pairs sharded, no data-path collective; NCCL all_gather of outputs off the critical path)" % world,
               "weights": "synthetic seed 326, well-conditioned set %s (same shapes / arithmetic as random init; reference self-noise 2e-5 px, tools/self_noise.py)" % json.dumps(BENCH_WEIGHTS),
-              "l2": "per-step working set >> 126 MB L2 (activations of the batch), no flush needed"}
+              "l2": "per-step working set >> 50 MB L2 (activations of the batch), no flush needed"}
     ARITHMETIC = ("fp32-faithful: tensor-core products as fp16 (hi, lo) split operands (hi*hi + hi*lo + lo*hi, fp32 accumulate), "
                   "everything else fp32 on CUDA cores; no TF32 / BF16 single-pass products")
 
@@ -266,9 +272,12 @@ def main():
                 pending[i].wait()
                 pending[i] = None
 
+    last = [None]
+
     def step_resident():
         flow = forward()
         gather_async(flow)
+        last[0] = flow
         return flow
 
     # End-to-end path: every step's inputs come from pinned host memory and its result goes back to pinned host memory,
@@ -366,6 +375,13 @@ def main():
         step_resident()
     gather_drain()
     ms, launches_r, clocks, (ms_own, steps_ms) = timed(step_resident, args.steps, sample_clocks=True, per_step=True)
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        name = {"flow": "flow", "stereo": "disparity", "depth": "depth"}[task]
+        out = last[0].detach().float()
+        keep = max(1, min(out.shape[0], (64 << 20) // (out[0].numel() * 4)))   # at most 64 MB: the leading pairs of the batch
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), out[:keep].cpu().numpy())
     # kernel-level timers and the launch counter live in the eager path: a separate pass (events around every launch group
     # perturb the host side, so this pass is not the one `value` is taken from)
     timer = {}
@@ -410,17 +426,6 @@ def main():
 
     # ---- rooflines: the fused attention kernel (tensor-bound) and the convolution / Linear family (tensor-bound)
     pk = peaks()
-    traffic, traffic_detail = None, None
-    tp = os.path.join(ROOT, "profiles", "r02_ncu_kernels.json")
-    if os.path.exists(tp):                                  # dram bytes per launch from the committed ncu --set full capture
-        try:
-            items = [d for d in json.load(open(tp)) if "attention" in d.get("label", "")]
-            traffic_detail = {d["label"]: d["dram__bytes_read.sum"] + d["dram__bytes_write.sum"] for d in items}
-            if traffic_detail:
-                traffic = sum(traffic_detail.values()) / len(traffic_detail)
-        except Exception:
-            traffic = None
-
     def roof(prefix, label):
         sel = {k: v for k, v in timer.items() if k.startswith(prefix)}
         if not sel:
@@ -431,19 +436,16 @@ def main():
         ach = tot_fl / (tot_ms / 1e3) / 1e12
         return {"kernel": label % (n_l // max(args.steps, 1)), "bound": "tensor", "achieved": ach, "peak": pk["tflops"],
                 "unit": "TFLOP/s", "frac": ach / pk["tflops"],
-                "peak_source": pk["source"] + " bf16 sustained (kernels timed inside a long step)",
+                "peak_source": pk["source"] + " dense fp16 (kernels timed inside a long step)",
                 "share_of_step": tot_ms / ms_timed, "avg_launch_ms": tot_ms / max(n_l, 1),
                 "algorithmic_gflop_per_step": tot_fl / 1e9 / args.steps,
                 "per_class": {k: {"ms_per_launch": round(v[0] / v[1], 4), "launches_per_step": v[1] // args.steps,
                                   "tflops": round(v[2] / (v[0] / 1e3) / 1e12, 1)} for k, v in sel.items()}}
 
-    roofline = roof("attn:", "um_window_attention_planes (fused QK^T.softmax.V on tcgen05, %d launches/step)")
+    roofline = roof("attn:", "um_window_attention_planes (fused QK^T.softmax.V on wgmma, %d launches/step)")
     if roofline:
-        roofline["traffic"] = traffic
-        roofline["traffic_unit"] = "bytes/launch (dram read+write, mean over the launch classes; profiles/r02_ncu_kernels.md)"
-        roofline["traffic_per_class"] = traffic_detail
         roofline["ceiling_note"] = "fp32-faithful products need 3 fp16 MMAs each: the path's tensor ceiling is peak/3 (frac 0.333)"
-    roofline_conv = roof("conv", "um_conv2d_tc + um_ffn_tc (implicit-GEMM convolutions, Linear layers and the fused FFN on tcgen05, %d launches/step)")
+    roofline_conv = roof("conv", "um_conv2d_tc + um_ffn_tc (implicit-GEMM convolutions, Linear layers and the FFN on wgmma, %d launches/step)")
     roofline_simt = roof("attn_simt:", "um_window_attention (CUDA-core kernel: 1-D / small windows, %d launches/step)")
 
     result = {"metric": metric, "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps,
@@ -469,7 +471,7 @@ def main():
                                       "reference_self_noise": "2e-5 px mean / 1.3e-4 px max under a 1e-7 relative input perturbation (tools/self_noise.py --bench-set)",
                                       "note": "GPU output vs CPU oracle (== reference bit-for-bit, tests/golden) on pair 0 of this batch"}
         if not args.no_ref_gpu:
-            # like-for-like GPU baseline (SURVEY.md section 8d): the reference's eager op sequence on this B200, fp32, TF32 off
+            # like-for-like GPU baseline (SURVEY.md section 8d): the reference's eager op sequence on this GPU, fp32, TF32 off
             try:
                 torch.backends.cuda.matmul.allow_tf32 = False
                 torch.backends.cudnn.allow_tf32 = False

@@ -1,4 +1,4 @@
-/* unimatch_sm100.h -- C ABI of libunimatch_sm100.so (B200 / sm_100a kernels for the UniMatch matching path).
+/* unimatch_sm100.h -- C ABI of libunimatch_sm100.so (H100 / sm_90a kernels for the UniMatch matching path).
  *
  * The reference (autonomousvision/unimatch) is pure Python/PyTorch and has no FFI of its own; these entry
  * points are what a binding for its hot-path functions would call.  Each declaration cites the reference
@@ -64,7 +64,7 @@ int um_window_attention(const float* q, const float* k, const float* v, float* o
                         int64_t ldq, int64_t ldk, int64_t ldv, int64_t ldo,
                         const um_attn_geom* geom, void* workspace, int64_t workspace_bytes, int32_t flags,
                         void* stream);
-/* Dense 2-D windows of >= 128 tokens run on the tcgen05 tensor cores (fp16 hi/lo split operands, fp32
+/* Dense 2-D windows of >= 128 tokens run on the Hopper tensor cores (wgmma, fp16 hi/lo split operands, fp32
  * accumulation, fp32-faithful); they need a device scratch buffer of um_window_attention_workspace() bytes for the
  * window-major operand planes (0 = this geometry runs on CUDA cores and needs none).  flags: */
 #define UM_ATTN_FORCE_CUDA_CORES 1   /* diagnostic: use the exact-fp32 CUDA-core kernel for every shape */
@@ -105,8 +105,8 @@ int um_softmax_expectation(const float* q, const float* k, const float* values, 
                            int64_t ldq, int64_t ldk, int32_t vdim, int32_t value_mode, int32_t post_op,
                            const um_attn_geom* geom, void* workspace, int64_t workspace_bytes, int32_t flags,
                            void* stream);
-/* Global (one window = the whole map) problems of >= 128 tokens run on the tcgen05 tensor cores: S = Q K^T tiles in
- * TMEM, softmax and sum_k p_k value_k in registers.  Scratch bytes (0 = CUDA-core path, none needed); flags as above. */
+/* Global (one window = the whole map) problems of >= 128 tokens run on the Hopper tensor cores: S = Q K^T tiles in
+ * registers, softmax and sum_k p_k value_k in registers.  Scratch bytes (0 = CUDA-core path, none needed); flags as above. */
 int64_t um_softmax_expectation_workspace(const um_attn_geom* geom, int32_t n_total, int32_t value_mode);
 
 /* ---- local (windowed, HBM/L2-bound) matching --------------------------------------------------------------
@@ -217,10 +217,8 @@ typedef struct um_conv_desc {
   const void* weights;
   const float* bias;          /* [cout] or NULL */
   int32_t kh, kw, pad_h, pad_w;
-  int32_t cout, cout_p, bn;   /* bn = output-channel tile (16, 64, 96, 128, 192 or 256); cout_p % bn == 0.  Long-K launches
-                               * (K >= 192, bn >= 64) over an even number of 16 x 8 pixel tiles run on CTA pairs
-                               * (cta_group::2: two SMs share every MMA and each stages half of the weight tile);
-                               * bn = 96 exists only as such a launch (Linear + ReLU).  UM_CONV_PAIR=0 disables pairs. */
+  int32_t cout, cout_p, bn;   /* bn = output-channel tile (16, 64, 96, 128, 192 or 256); cout_p % bn == 0.  bn = 256 / 192 run
+                               * as two 128- / 96-wide tiles (register accumulators of two warpgroups). */
   int32_t mode, act;
   float* out_f32;             /* [B,H,W,*] row stride ld_f32 floats, written at channel offset off_f32; or NULL */
   int64_t ld_f32;
@@ -260,9 +258,9 @@ int um_conv2d_tc(const um_conv_desc* desc, void* stream);
  * src0 / src1: fp16 (hi, lo) planes [2][>= rows][128] (source, message), planes src_plane_stride halves apart;
  * w1: prepared planes [2][hidden][256] (K ordered source | message), w2: [2][128][hidden] (um_conv2d_tc weight layout);
  * residual: fp32 rows (row stride ld_res) or NULL; out_f32 (row stride ld_f32) and/or out_split planes [2][>= rows][128].
- * The hidden activation (4 KB per row as split planes) never leaves the SM: one CTA-pair kernel, hidden channels produced
- * 128 at a time into TMEM, GELU'd in place and consumed as the A operand of the second GEMM.
- * rows must be a multiple of 256 (pairs of 128-row tiles; callers with other row counts use two um_conv2d_tc launches),
+ * The hidden activation never leaves the SM: one kernel, hidden channels produced 64 at a time into register accumulators,
+ * GELU'd, split and consumed as the register A operand of the second GEMM.
+ * rows must be a multiple of 256 (callers with other row counts use two um_conv2d_tc launches),
  * hidden a multiple of 128. */
 typedef struct um_ffn_desc {
   const void* src[2];

@@ -211,17 +211,15 @@ CONV_CASES = [
     ("linear_ln_residual", [128], 128, 1, 1, 128, "ln", 0, (40, 16)),            # token rows as a [rows/16, 16] grid
     ("ffn1_two_sources_gelu", [128, 128], 1024, 1, 1, 128, "lin", ops.ACT_GELU, (24, 16)),
     ("ffn2_k1024_ln", [1024], 128, 1, 1, 128, "ln", 0, (24, 16)),
-    ("many_tiles_persistent", [128], 640, 1, 1, 128, "lin", ops.ACT_NONE, (400, 16)),   # 250 tiles > 148 SMs
-    # wide tiles (BN = 192 / 256: two 96 KB stages, one TMEM accumulator buffer)
+    ("many_tiles_persistent", [128], 640, 1, 1, 128, "lin", ops.ACT_NONE, (400, 16)),   # 250 tiles > 132 SMs
+    # wide tiles (BN = 192 / 256: run as two 96- / 128-wide tiles)
     ("convc2_3x3_bn192", [256], 192, 3, 3, 192, "lin", ops.ACT_RELU, (20, 33)),
     ("gru_zr_1x5_bn256", [128, 256], 256, 1, 5, 256, "zr", 0, (12, 40)),
     ("flow_head1_3x3_bn256", [128], 256, 3, 3, 256, "lin", ops.ACT_RELU, (24, 40)),
     ("convc1_1x1_bn256", [81], 256, 1, 1, 256, "lin", ops.ACT_RELU, (16, 32)),
     ("wide_many_tiles", [128], 256, 3, 3, 256, "lin", ops.ACT_RELU, (160, 128)),        # 320 tiles: several per CTA
     ("ffn1_two_sources_gelu_bn256", [128, 128], 1024, 1, 1, 256, "lin", ops.ACT_GELU, (24, 16)),
-    # CTA-pair kernels (cta_group::2; taken for long-K launches with an even number of pixel tiles -- most cases above with
-    # batch 2 already are): LayerNorm epilogue on a pair, several tiles per pair with G = 2 / G = 4, an odd tile count per
-    # CTA pair on the last round (76 pair tiles on 74 clusters)
+    # long-K launches: LayerNorm epilogue, several tiles per CTA with G = 2 / G = 4, a last round with fewer tiles than CTAs
     ("ffn2_k1024_ln_pair", [1024], 128, 1, 1, 128, "ln", 0, (32, 16)),
     ("ffn2_k1024_ln_pair_many", [1024], 128, 1, 1, 128, "ln", 0, (2432, 16)),
     ("pair_many_tiles_bn128", [256], 128, 3, 3, 128, "lin", ops.ACT_RELU, (160, 128)),
@@ -279,8 +277,8 @@ def test_conv2d_tc(name, cins, cout, kh, kw, bn, mode, act, hw):
 @pytest.mark.parametrize("rows,hidden,outs", [(256, 128, "both"), (512, 1024, "both"), (256 * 77, 1024, "both"),
                                               (256 * 150, 256, "split"), (1024, 1024, "f32")])
 def test_ffn_tc(rows, hidden, outs):
-    """Fused FFN (CTA-pair kernel, hidden activation in tensor memory) vs the two GEMM launches it replaces, stated on CPU
-    (tests/refops.py): one chunk, the module's 8 chunks, more tile pairs than clusters (77 and 150 on 74)."""
+    """Fused FFN (hidden activation in registers) vs the two GEMM launches it replaces, stated on CPU
+    (tests/refops.py): one chunk, the module's 8 chunks, more 128-row tiles than SMs (154 and 300 on 132)."""
     gen = g(7000 + rows % 997 + hidden)
     w1 = torch.randn((hidden, 256, 1, 1), generator=gen) * (2.0 / 256) ** 0.5
     w2 = torch.randn((128, hidden, 1, 1), generator=gen) * (1.0 / hidden) ** 0.5
@@ -303,7 +301,7 @@ def test_ffn_tc(rows, hidden, outs):
                 (out_s[0].float() + out_s[1].float()).cpu() if out_s is not None else None)
 
     ref_f, ref_s = run("cpu", refops.ffn_tc, refops.split_planes)
-    for rep in range(2):                                                   # twice: barrier phases / TMEM state carry nothing over
+    for rep in range(2):                                                   # twice: barrier phases carry nothing over
         got_f, got_s = run("cuda", OPS.ffn_tc, OPS.split_planes)
         if ref_f is not None:
             close(got_f, ref_f, 3e-5)
@@ -371,7 +369,7 @@ def test_conv2d_tc_backbone_shapes(cin, cout, k, stride, hw):
     close(got, y.contiguous(), 2e-5)
 
 
-@pytest.mark.parametrize("hw", [(40, 56), (200, 330)])     # the larger one: 312 tiles > 2 CTAs x 148 SMs (persistent loop)
+@pytest.mark.parametrize("hw", [(40, 56), (200, 330)])     # the larger one: 312 tiles > 2 CTAs x 132 SMs (persistent loop)
 def test_conv7x7_stem_with_folded_normalisation(hw):
     gen = g(3200)
     H, W = hw

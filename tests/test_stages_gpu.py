@@ -1,4 +1,4 @@
-"""Parity where the metric lives: `unimatch_b200.UniMatch` on the B200 against the oracle (== reference) at the BASELINE
+"""Parity where the metric lives: `unimatch_b200.UniMatch` on the GPU against the oracle (== reference) at the BASELINE
 shape -- one 480x832 pair, gmflow-scale2-regrefine6 -- stage by stage with teacher forcing (every stage fed the oracle's
 inputs for it, so errors neither hide nor compound; reference unimatch/unimatch.py:136-354), then free-running end to end.
 The oracle runs on the box's CPU (~15-30 s).  Tolerances: tests/stage_checks.py."""

@@ -1,4 +1,4 @@
-"""unimatch_b200 -- B200-native (sm_100a) implementation of the UniMatch matching inference path.
+"""unimatch_b200 -- H100-native (sm_90a) implementation of the UniMatch matching inference path.
 
     from unimatch_b200 import UniMatch      # drop-in for reference unimatch.unimatch.UniMatch (inference)
 

@@ -1,4 +1,4 @@
-"""Build libunimatch_sm100.so in-tree with nvcc for sm_100a (no JIT cache, the .so travels with the repo).
+"""Build libunimatch_sm100.so in-tree with nvcc for sm_90a (no JIT cache, the .so travels with the repo).
 
     python unimatch_b200/csrc/build.py [--force] [-v]     (or: from unimatch_b200.csrc.build import build; build())
 
@@ -14,8 +14,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 LIB = os.path.join(os.path.dirname(HERE), "libunimatch_sm100.so")
-SOURCES = ["um_api.cu", "um_attention_simt.cu", "um_attention_tc.cu", "um_attention_tc2.cu", "um_conv_tc.cu", "um_ffn_tc.cu", "um_local.cu", "um_local_stencil.cu", "um_misc.cu", "um_norm.cu", "um_stem.cu"]
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+SOURCES = ["um_api.cu", "um_attention_simt.cu", "um_attention_tc.cu", "um_conv_tc.cu", "um_ffn_tc.cu", "um_local.cu", "um_local_stencil.cu", "um_misc.cu", "um_norm.cu", "um_stem.cu"]
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-I", os.path.join(ROOT, "include"), "-I", HERE]
 
 
@@ -32,10 +32,6 @@ def have_nvcc():
         return True
     except RuntimeError:
         return False
-
-
-if os.environ.get("UM_ATTN_DEBUG_BUILD") == "1":      # diagnostics of the attention kernel (timeline, dump, timing experiments)
-    FLAGS = FLAGS + ["-DUM_ATTN_DEBUG=1"]
 
 
 def _stamp():

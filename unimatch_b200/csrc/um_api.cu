@@ -48,7 +48,7 @@ extern "C" {
 int um_abi_version(void) { return 3; }
 
 const char* um_build_info(void) {
-  return "libunimatch_sm100 abi=2 arch=sm_100a cuda=" UM_STR(CUDART_VERSION) " built " __DATE__ " " __TIME__;
+  return "libunimatch_sm100 abi=2 arch=sm_90a cuda=" UM_STR(CUDART_VERSION) " built " __DATE__ " " __TIME__;
 }
 
 const char* um_last_error(void) { return um::g_err; }

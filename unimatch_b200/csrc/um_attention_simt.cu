@@ -6,7 +6,7 @@
 // no roll / split / merge copies, no [K*K, Lw, Lw] mask tensor.
 //
 // This is the general-shape path (any window length, 1-D row windows, causal stereo mask).  The
-// tensor-core (tcgen05) path in um_attention_tc.cu takes over the large 2-D windows.
+// tensor-core (wgmma) path in um_attention_tc.cu takes over the large 2-D windows.
 //
 // Reference semantics: attention.py:8-16, :19-42, :45-104, :107-163; matching.py:7-36, :126-151;
 // attention.py:194-215.

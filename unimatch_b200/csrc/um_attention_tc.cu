@@ -1,22 +1,21 @@
-// Fused window attention on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), fp32-faithful.
+// Fused window attention on the Hopper tensor cores (wgmma + TMA), fp32-faithful.
 //
-//   out = softmax(Q K^T / sqrt(C) + mask) V   per Swin window; the Lw x Lw scores live only in TMEM / registers.
+//   out = softmax(Q K^T / sqrt(C) + mask) V   per Swin window; the Lw x Lw scores live only in registers.
 //
 // Precision: operands are fp32 values split into (hi, lo) fp16 pairs (same bytes as fp32); every product is
-// formed as hi*hi + hi*lo + lo*hi on kind::f16 MMAs with fp32 accumulation in TMEM ("3xFP16", error ~2^-22 per
-// product, i.e. the accuracy of an fp32 dot product) -- one-pass TF32/BF16 moves the final flow by whole pixels
-// on this network (SURVEY.md §7.2 #1), so it is not an option for parity.
+// formed as hi*hi + hi*lo + lo*hi on fp16 MMAs with fp32 accumulation ("3xFP16", error ~2^-22 per product, i.e. the
+// accuracy of an fp32 dot product) -- one-pass TF32/BF16 moves the final flow by whole pixels on this network
+// (SURVEY.md §7.2 #1), so it is not an option for parity.
 //
 // Data flow
 //   1. um_split_windows: q/k/v fp32 token rows -> window-major, cyclically shifted, zero-padded fp16 hi/lo planes
 //      [part][stream][window][Lp][128] (Lp = Lw rounded up to 128), so every tile is a dense 2-D TMA box.
 //   2. attn_tc_kernel: one CTA per (128-query tile, window, stream); warp-specialised:
-//        warp 0     TMA producer      Q once; K/V tiles of 64 keys through a 2-stage mbarrier ring
-//        warp 1     MMA issuer        S_j = Q K_j^T (24 UMMAs 128x64x16) into a double-buffered TMEM tile,
-//                                     O += P_j V_j (12 UMMAs 128x128x16, V as MN-major B operand)
-//        warps 2-5  softmax           tcgen05.ld S -> registers, scale/mask, online softmax with lazy rescale,
-//                                     P -> fp16 hi/lo in 128B-swizzled smem, O correction via tcgen05.ld/st,
-//                                     epilogue O / l -> smem transpose -> coalesced rows at the un-shifted tokens
+//        warp 0          TMA producer   Q once; K and V tiles of 64 keys through two 2-stage mbarrier rings
+//        warpgroups 1-2  consumers      64 query rows each: S_j = Q K_j^T (24 wgmma 64x64x16) into registers, scale /
+//                                       mask, online softmax with lazy rescale, P as fp16 (hi, lo) register operands
+//                                       and O += P_j V_j (12 wgmma 64x128x16, V as MN-major B operand) into registers;
+//                                       epilogue O / l -> smem transpose -> coalesced rows at the un-shifted tokens
 //   3. the ragged last query tile (Lw mod 128 rows) runs the same code on zero-padded rows whose stores are masked.
 //
 // Reference semantics: attention.py:45-104 (split / roll / mask / softmax / merge / roll back), utils.py:84-108.
@@ -32,19 +31,19 @@ using namespace tc;
 namespace {
 
 constexpr int BM = 128, BN = 64;
-constexpr int NTHREADS = 320;                  // TMA warp + MMA warp + 8 softmax warps (2 per TMEM lane quarter)
-constexpr int NSOFT = 256;
+// 2 consumer warpgroups (warps 0-7) + one TMA producer warp (warp 8)
+constexpr int NTHREADS = 288;
+constexpr int PRODUCER = 8;
 constexpr uint32_t Q_BYTES = 4 * 16384;          // (hi, lo) x (ch 0-63, 64-127) x [128 rows x 128 B]
 constexpr uint32_t KV_STAGE_BYTES = 4 * 8192;    // (hi, lo) x (2 halves) x [64 rows x 128 B]
 constexpr uint32_t OFF_Q = 0;
 constexpr uint32_t OFF_K = OFF_Q + Q_BYTES;                  // 2 stages
 constexpr uint32_t OFF_V = OFF_K + 2 * KV_STAGE_BYTES;       // 2 stages
-constexpr uint32_t OFF_P = OFF_V + 2 * KV_STAGE_BYTES;       // (hi, lo) x [128 rows x 128 B]
-constexpr uint32_t OFF_BAR = OFF_P + 2 * 16384;              // 229376
+constexpr uint32_t OFF_X = OFF_V + 2 * KV_STAGE_BYTES;       // softmax-expectation key values [2][64][2] fp32
+constexpr uint32_t OFF_BAR = OFF_X + 1024;
 constexpr uint32_t OFF_KREG = OFF_BAR + 256;
 constexpr int MAX_LP = 2048;
-constexpr uint32_t SMEM_BYTES = OFF_KREG + MAX_LP;           // 231680 <= 232448
-constexpr uint32_t TMEM_COLS = 256;                          // S0 [0,64) S1 [64,128) O [128,256)
+constexpr uint32_t SMEM_BYTES = OFF_KREG + MAX_LP;           // 200960
 constexpr float SQRT_C = 11.313708498984761f;
 constexpr float EXP_SCALE = 1.4426950408889634f / 11.313708498984761f;   // log2(e) / sqrt(128)
 constexpr float LAZY_THRESH = 8.0f / EXP_SCALE;              // raw-logit units: rescale when the max grows by > 2^8
@@ -68,7 +67,7 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
 // HAS_V = true : fused attention, O = softmax(S) V through a second MMA chain.
 // HAS_V = false: softmax expectation (global correlation soft-argmax, matching.py:7-36; global flow propagation,
 //                attention.py:194-215): the values are 1-2 numbers per key, so sum_k p_k value_k is accumulated in
-//                registers straight from the S tile -- no P tile, no V tile, no second MMA.
+//                registers straight from the S tile -- no V tile, no second MMA.
 template <bool HAS_V>
 __global__ void __launch_bounds__(NTHREADS, 1)
 attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_k,
@@ -78,13 +77,8 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
   uint64_t* q_full = bars + 0;
   uint64_t* k_full = bars + 1;      // [2]   K and V tiles travel through SEPARATE rings: a K slot is free as soon as
   uint64_t* k_empty = bars + 3;     // [2]   S_j = Q K_j^T has been computed, long before P_j V_j releases the V slot
-  uint64_t* s_full = bars + 5;      // [2]
-  uint64_t* s_free = bars + 7;      // [2]
-  uint64_t* p_full = bars + 9;
-  uint64_t* pv_done = bars + 10;
-  uint64_t* v_full = bars + 11;     // [2]
-  uint64_t* v_empty = bars + 13;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
+  uint64_t* v_full = bars + 5;      // [2]
+  uint64_t* v_empty = bars + 7;     // [2]
   int8_t* kreg = reinterpret_cast<int8_t*>(smem + OFF_KREG);
 
   const Geom g = p.g;
@@ -98,18 +92,12 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
-      mbar_init(k_full + i, 1); mbar_init(k_empty + i, 1);
-      mbar_init(v_full + i, 1); mbar_init(v_empty + i, 1);
-      mbar_init(s_full + i, 1);  mbar_init(s_free + i, NSOFT);
+      mbar_init(k_full + i, 1); mbar_init(k_empty + i, 8);   // empty: one arrival per consumer warp
+      mbar_init(v_full + i, 1); mbar_init(v_empty + i, 8);
     }
-    mbar_init(p_full, NSOFT); mbar_init(pv_done, 1);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    if (lane == 0) { tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); }
-  } else if (warp == 1) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-  }
+  if (warp == PRODUCER && lane == 0) { tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_v); }
   // shift-region table of the keys of this window (utils.py:84-108); uniform windows skip masking altogether
   bool masked = false;
   if (g.mask_mode == UM_MASK_SWIN) {
@@ -122,342 +110,274 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
         kreg[t] = (int8_t)shift_region(g, yr, xr);
       }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER) {
     // =============================== TMA producer (converged warp, one elected lane issues) ===============================
-    {
-      const int qrow = (n * nwin + win) * lp + m0;
+    const int qrow = (n * nwin + win) * lp + m0;
+    if (elect_one()) {
+      mbar_arrive_expect_tx(q_full, Q_BYTES);
+#pragma unroll
+      for (int part = 0; part < 2; ++part)
+#pragma unroll
+        for (int half = 0; half < 2; ++half)
+          tma_load_2d(smem + OFF_Q + (part * 2 + half) * 16384, &map_q, q_full, half * 64, part * planes + qrow);
+    }
+    __syncwarp();
+    const int krow = (nk * nwin + win) * lp;
+    auto load_tile = [&](int j, const CUtensorMap* map, uint32_t off, uint64_t* full, uint64_t* empty) {
+      const int s = j & 1;
+      mbar_wait_inline(empty + s, ((j >> 1) & 1) ^ 1);
       if (elect_one()) {
-        mbar_arrive_expect_tx(q_full, Q_BYTES);
+        mbar_arrive_expect_tx(full + s, KV_STAGE_BYTES);
 #pragma unroll
         for (int part = 0; part < 2; ++part)
 #pragma unroll
           for (int half = 0; half < 2; ++half)
-            tma_load_2d(smem + OFF_Q + (part * 2 + half) * 16384, &map_q, q_full, half * 64, part * planes + qrow);
+            tma_load_2d(smem + off + s * KV_STAGE_BYTES + (part * 2 + half) * 8192, map, full + s, half * 64,
+                        part * planes + krow + j * BN);
       }
       __syncwarp();
-      const int krow = (nk * nwin + win) * lp;
-      auto load_tile = [&](int j, const CUtensorMap* map, uint32_t off, uint64_t* full, uint64_t* empty) {
-        const int s = j & 1;
-        mbar_wait(empty + s, ((j >> 1) & 1) ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(full + s, KV_STAGE_BYTES);
-#pragma unroll
-          for (int part = 0; part < 2; ++part)
-#pragma unroll
-            for (int half = 0; half < 2; ++half)
-              tma_load_2d(smem + off + s * KV_STAGE_BYTES + (part * 2 + half) * 8192, map, full + s, half * 64,
-                          part * planes + krow + j * BN);
-        }
-        __syncwarp();
-      };
-      // Issue order = the order in which the slots come free (MMA order is S0 S1 PV0 S2 PV1 S3 ...): K_{j+2} can be
-      // fetched as soon as S_j is done, i.e. a whole softmax + PV earlier than V_{j+1}.  With one combined K|V ring the
-      // K tile of S_{j+1} was only requested after PV_{j-1}, and the tensor pipe sat out the load latency every tile.
-      load_tile(0, &map_k, OFF_K, k_full, k_empty);
-      if (HAS_V) load_tile(0, &map_v, OFF_V, v_full, v_empty);
-      if (T > 1) {
-        load_tile(1, &map_k, OFF_K, k_full, k_empty);
-        if (HAS_V) load_tile(1, &map_v, OFF_V, v_full, v_empty);
-      }
-      for (int i = 2; i <= T; ++i) {
-        if (i < T) load_tile(i, &map_k, OFF_K, k_full, k_empty);
-        if (HAS_V && i - 1 >= 2) load_tile(i - 1, &map_v, OFF_V, v_full, v_empty);
-      }
+    };
+    // K_{j+1} is requested before V_j: the K slot comes free (S_{j-1} done) a whole softmax earlier than the V slot
+    load_tile(0, &map_k, OFF_K, k_full, k_empty);
+    for (int j = 0; j < T; ++j) {
+      if (j + 1 < T) load_tile(j + 1, &map_k, OFF_K, k_full, k_empty);
+      if (HAS_V) load_tile(j, &map_v, OFF_V, v_full, v_empty);
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer (converged warp: descriptors stay in uniform registers) ===============================
-    {
-      constexpr uint32_t IDESC_S = idesc_f16(BM, BN, 0, 0);
-      constexpr uint32_t IDESC_PV = idesc_f16(BM, 128, 0, 1);
-      const uint32_t q_base = smem_u32(smem + OFF_Q), p_base = smem_u32(smem + OFF_P);
-      auto issue_s = [&](int j) {
-        const int s = j & 1;
-        mbar_wait(k_full + s, (j >> 1) & 1);
-        mbar_wait(s_free + s, ((j >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t k_base = smem_u32(smem + OFF_K + s * KV_STAGE_BYTES);
-        const uint32_t d = tmem + s * BN;
-        // (q part, k part): lo*hi, hi*lo, hi*hi
-        const int qa[3] = {1, 0, 0}, kb[3] = {0, 1, 0};
-        if (elect_one()) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-#pragma unroll
-            for (int half = 0; half < 2; ++half)
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks) {
-                const uint64_t da = desc_kmajor(q_base + (qa[c] * 2 + half) * 16384 + ks * 32);
-                const uint64_t db = desc_kmajor(k_base + (kb[c] * 2 + half) * 8192 + ks * 32);
-                umma_f16(d, da, db, IDESC_S, (c | half | ks) != 0);
-              }
-          umma_commit(s_full + s);
-          umma_commit(k_empty + s);                          // the K slot is free once S_j has been computed
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int j) {
-        const int s = j & 1;
-        mbar_wait(v_full + s, (j >> 1) & 1);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint32_t v_base = smem_u32(smem + OFF_V + s * KV_STAGE_BYTES);
-        const uint32_t d = tmem + 2 * BN;
-        const int pa[3] = {1, 0, 0}, vb[3] = {0, 1, 0};
-        if (elect_one()) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint64_t da = desc_kmajor(p_base + pa[c] * 16384 + ks * 32);
-              const uint64_t db = desc_mnmajor(v_base + vb[c] * 16384 + ks * 2048, 8192);
-              umma_f16(d, da, db, IDESC_PV, (j > 0) || (c | ks) != 0);
-            }
-          umma_commit(pv_done);
-          umma_commit(v_empty + s);
-        }
-        __syncwarp();
-      };
-      mbar_wait(q_full, 0);
-      if (HAS_V) {
-        issue_s(0);
-        for (int j = 0; j < T; ++j) {
-          if (j + 1 < T) issue_s(j + 1);
-          issue_pv(j);
-        }
-      } else {
-        for (int j = 0; j < T; ++j) issue_s(j);
-      }
-    }
-  } else {
-    // =============================== softmax / correction / epilogue ===============================
-    // Two warps per TMEM lane quarter: both read the whole 64-column S row (the row max needs it and TMEM reads are
-    // cheap) but each exponentiates / converts / stores only its own 32 columns, halving the softmax critical path.
-    const int quarter = warp & 3;                           // TMEM lanes [32*quarter, +32) are this warp's
-    const int half = (warp - 2) >> 2;                       // which 32 key columns of a tile this thread owns
-    const int r = quarter * 32 + lane;                      // query row inside the tile
-    const uint32_t lane_addr = tmem + ((uint32_t)(quarter * 32) << 16);
-    const int tq = m0 + r;                                  // rows >= lw of the last tile are zero padding
-    const bool row_valid = tq < g.lw;
-    int yr = 0, xr = 0;
-    const int tok = row_valid ? window_token(g, win, tq, &yr, &xr) : -1;
-    const int rq = masked ? shift_region(g, yr, xr) : 0;
-    float m_run = -CUDART_INF_F, l_run = 0.f;
-    uint8_t* p_hi = smem + OFF_P;
-    uint8_t* p_lo = smem + OFF_P + 16384;
+    return;
+  }
 
-    if (!HAS_V) {
-      // ---------------- softmax expectation: per-key values staged in shared memory, sums kept in registers ----------------
-      float* vals = reinterpret_cast<float*>(smem + OFF_P);  // [2 buffers][64 keys][2]
-      const int et = threadIdx.x - 64;
-      const long long L = (long long)g.h * g.w;
-      float a0 = 0.f, a1 = 0.f;
-      for (int j = 0; j < T; ++j) {
-        const int s = j & 1;
-        const int n0 = j * BN;
-        if (et < BN) {                                       // value of key n0 + et (keys of the key stream nk)
-          float v0 = 0.f, v1 = 0.f;
-          const int t = n0 + et;
-          if (t < g.lw) {
-            const int ktok = window_token(g, win, t);
-            if (p.value_mode == UM_VALUE_TENSOR) {
-              const float* vp = p.values + ((long long)nk * L + ktok) * p.vdim;
-              v0 = __ldg(vp); v1 = (p.vdim > 1) ? __ldg(vp + 1) : 0.f;
-            } else {
-              const int ky = ktok / g.w;
-              v0 = (float)(ktok - ky * g.w); v1 = (float)ky;
-            }
+  // =============================== consumers: softmax / PV / epilogue ===============================
+  const int cw = warp;                                      // consumer warp 0..7
+  const int wg = cw >> 2;                                   // query rows [64 wg, 64 wg + 64) of the tile
+  const int fr = wg * 64 + (cw & 3) * 16 + (lane >> 2);     // this thread's rows fr and fr + 8 (MMA fragment layout)
+  const int fc = 2 * (lane & 3);                            // ... and columns 8 j + fc + {0, 1}
+  int rq[2] = {0, 0}, tok[2];
+  bool row_valid[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int tq = m0 + fr + 8 * h;                         // rows >= lw of the last tile are zero padding
+    row_valid[h] = tq < g.lw;
+    int yr = 0, xr = 0;
+    tok[h] = row_valid[h] ? window_token(g, win, tq, &yr, &xr) : -1;
+    if (masked) rq[h] = shift_region(g, yr, xr);
+  }
+  float m_run[2] = {-CUDART_INF_F, -CUDART_INF_F}, l_run[2] = {0.f, 0.f};
+  const uint32_t q_base = smem_u32(smem + OFF_Q) + wg * 8192;
+  auto consumers_sync = [&]() { asm volatile("bar.sync 1, 256;" ::: "memory"); };
+
+  // S_j = Q K_j^T for this warpgroup's 64 rows; the K slot is released as soon as the MMAs are complete
+  auto compute_s = [&](int j, float (&sv)[32]) {
+    const int s = j & 1;
+    mbar_wait_inline(k_full + s, (j >> 1) & 1);
+    const uint32_t k_base = smem_u32(smem + OFF_K + s * KV_STAGE_BYTES);
+    const int qa[3] = {1, 0, 0}, kb[3] = {0, 1, 0};        // (q part, k part): lo*hi, hi*lo, hi*hi
+    fence_acc(sv);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int half = 0; half < 2; ++half)
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          wgmma_ss<BN>(sv, desc_kmajor(q_base + (qa[c] * 2 + half) * 16384 + ks * 32),
+                       desc_kmajor(k_base + (kb[c] * 2 + half) * 8192 + ks * 32), (c | half | ks) != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(sv);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(k_empty + s);
+  };
+  mbar_wait_inline(q_full, 0);
+
+  if (!HAS_V) {
+    // ---------------- softmax expectation: per-key values staged in shared memory, sums kept in registers ----------------
+    float* vals = reinterpret_cast<float*>(smem + OFF_X);  // [2 buffers][64 keys][2]
+    const int et = threadIdx.x;
+    const long long L = (long long)g.h * g.w;
+    float a0[2] = {0.f, 0.f}, a1[2] = {0.f, 0.f};
+    for (int j = 0; j < T; ++j) {
+      const int s = j & 1;
+      const int n0 = j * BN;
+      if (et < BN) {                                       // value of key n0 + et (keys of the key stream nk)
+        float v0 = 0.f, v1 = 0.f;
+        const int t = n0 + et;
+        if (t < g.lw) {
+          const int ktok = window_token(g, win, t);
+          if (p.value_mode == UM_VALUE_TENSOR) {
+            const float* vp = p.values + ((long long)nk * L + ktok) * p.vdim;
+            v0 = __ldg(vp); v1 = (p.vdim > 1) ? __ldg(vp + 1) : 0.f;
+          } else {
+            const int ky = ktok / g.w;
+            v0 = (float)(ktok - ky * g.w); v1 = (float)ky;
           }
-          vals[(s * BN + et) * 2] = v0; vals[(s * BN + et) * 2 + 1] = v1;
         }
-        mbar_wait(s_full + s, (j >> 1) & 1);
-        tc_fence_after();
-        float sv[BN];
-        tmem_ld32(lane_addr + s * BN, sv);
-        tmem_ld32(lane_addr + s * BN + 32, sv + 32);
-        tmem_wait_ld();
-        tc_fence_before();
-        mbar_arrive(s_free + s);
-        asm volatile("bar.sync 1, 256;" ::: "memory");       // values of this tile are visible
-        if (n0 + BN > g.lw) {                                // ragged last key tile only
-#pragma unroll
-          for (int c = 0; c < BN; ++c)
-            if (n0 + c >= g.lw) sv[c] = -CUDART_INF_F;
-        }
-        float mx4[4] = {-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-        for (int c = 0; c < BN; c += 4) {
-          mx4[0] = fmaxf(mx4[0], sv[c]); mx4[1] = fmaxf(mx4[1], sv[c + 1]);
-          mx4[2] = fmaxf(mx4[2], sv[c + 2]); mx4[3] = fmaxf(mx4[3], sv[c + 3]);
-        }
-        const float m_new = fmaxf(m_run, fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3])));
-        const float alpha = exp2f((m_run - m_new) * EXP_SCALE);
-        m_run = m_new;
-        const float mscaled = m_run * EXP_SCALE;
-        float sum = 0.f, b0 = 0.f, b1 = 0.f;
-        const float2* vv = reinterpret_cast<const float2*>(vals + s * BN * 2) + half * 32;
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {                       // this thread's half of the keys
-          const float pe = ex2_approx(fmaf(half ? sv[32 + c] : sv[c], EXP_SCALE, -mscaled));
-          const float2 kv = vv[c];
-          sum += pe;
-          b0 = fmaf(pe, kv.x, b0);
-          b1 = fmaf(pe, kv.y, b1);
-        }
-        l_run = l_run * alpha + sum;
-        a0 = a0 * alpha + b0;
-        a1 = a1 * alpha + b1;
+        vals[(s * BN + et) * 2] = v0; vals[(s * BN + et) * 2 + 1] = v1;
       }
-      // combine the two halves of every row (same running max in both threads)
-      float* comb = reinterpret_cast<float*>(smem + OFF_P + 4096);
-      if (half == 1) { comb[r * 3] = l_run; comb[r * 3 + 1] = a0; comb[r * 3 + 2] = a1; }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (half == 0) { l_run += comb[r * 3]; a0 += comb[r * 3 + 1]; a1 += comb[r * 3 + 2]; }
-      if (row_valid && half == 0) {
-        float r0 = a0 / l_run, r1 = a1 / l_run;
-        const int oy = tok / g.w, ox = tok - oy * g.w;
+      float sv[32];
+      compute_s(j, sv);
+      consumers_sync();                                     // values of this tile are visible
+      const float2* vv = reinterpret_cast<const float2*>(vals + s * BN * 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mx = -CUDART_INF_F;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float& x = sv[4 * jj + 2 * h + e];
+            if (n0 + 8 * jj + fc + e >= g.lw) x = -CUDART_INF_F;   // ragged last key tile
+            mx = fmaxf(mx, x);
+          }
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m_run[h], mx);
+        const float alpha = exp2f((m_run[h] - m_new) * EXP_SCALE);
+        m_run[h] = m_new;
+        const float mscaled = m_new * EXP_SCALE;
+        float sum = 0.f, b0 = 0.f, b1 = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float pe = ex2_approx(fmaf(sv[4 * jj + 2 * h + e], EXP_SCALE, -mscaled));
+            const float2 kv = vv[8 * jj + fc + e];
+            sum += pe;
+            b0 = fmaf(pe, kv.x, b0);
+            b1 = fmaf(pe, kv.y, b1);
+          }
+        l_run[h] = l_run[h] * alpha + sum;
+        a0[h] = a0[h] * alpha + b0;
+        a1[h] = a1[h] * alpha + b1;
+      }
+    }
+    // combine the four threads of every row (same running max in all of them)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int o = 1; o <= 2; o <<= 1) {
+        l_run[h] += __shfl_xor_sync(0xffffffffu, l_run[h], o);
+        a0[h] += __shfl_xor_sync(0xffffffffu, a0[h], o);
+        a1[h] += __shfl_xor_sync(0xffffffffu, a1[h], o);
+      }
+      if (row_valid[h] && (lane & 3) == 0) {
+        float r0 = a0[h] / l_run[h], r1 = a1[h] / l_run[h];
+        const int oy = tok[h] / g.w, ox = tok[h] - oy * g.w;
         if (p.post_op == UM_POST_MINUS_OWN) { r0 -= (float)ox; r1 -= (float)oy; }
         else if (p.post_op == UM_POST_OWN_MINUS) { r0 = (float)ox - r0; }
-        float* dst = p.out + ((long long)n * L + tok) * p.vdim;
+        float* dst = p.out + ((long long)n * L + tok[h]) * p.vdim;
         dst[0] = r0;
         if (p.vdim > 1) dst[1] = r1;
       }
-    } else {
-    for (int j = 0; j < T; ++j) {
-      const int s = j & 1;
-      mbar_wait(s_full + s, (j >> 1) & 1);
-      tc_fence_after();
-      float sv[BN];
-      tmem_ld32(lane_addr + s * BN, sv);
-      tmem_ld32(lane_addr + s * BN + 32, sv + 32);
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive(s_free + s);
-      if (p.dbg && j == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0)
-        for (int c = 0; c < BN; ++c) p.dbg[r * BN + c] = sv[c];
-
-      const int n0 = j * BN;
-      // The softmax warps are instruction-issue bound (8 warps x ~N instructions per tile on 4 schedulers must stay
-      // below the ~1500 tensor-pipe cycles of a tile): masks only where they can apply, one-instruction exp2, paired
-      // fp16 conversions.
-      if (masked) {                                          // CTA-uniform: window touches a shift-region boundary
-#pragma unroll
-        for (int c = 0; c < BN; ++c)
-          if (kreg[n0 + c] != rq) sv[c] -= 100.0f * SQRT_C;
-      }
-      if (n0 + BN > g.lw) {                                  // ragged last key tile only
-#pragma unroll
-        for (int c = 0; c < BN; ++c)
-          if (n0 + c >= g.lw) sv[c] = -CUDART_INF_F;
-      }
-      float mx4[4] = {-CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F, -CUDART_INF_F};
-#pragma unroll
-      for (int c = 0; c < BN; c += 4) {
-        mx4[0] = fmaxf(mx4[0], sv[c]); mx4[1] = fmaxf(mx4[1], sv[c + 1]);
-        mx4[2] = fmaxf(mx4[2], sv[c + 2]); mx4[3] = fmaxf(mx4[3], sv[c + 3]);
-      }
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      float alpha = 1.0f;
-      const bool rescale = mx > m_run + LAZY_THRESH;       // first tile: m_run = -inf -> true
-      if (rescale) {
-        alpha = exp2f((m_run - mx) * EXP_SCALE);             // exp2(-inf) = 0 on the first tile
-        m_run = mx;
-      }
-      float pe[32];                                          // this thread's 32 keys of the tile
-      float sum4[4] = {0.f, 0.f, 0.f, 0.f};
-      const float mscaled = m_run * EXP_SCALE;
-#pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        pe[c] = ex2_approx(fmaf(half ? sv[32 + c] : sv[c], EXP_SCALE, -mscaled));
-        sum4[c & 3] += pe[c];
-      }
-      l_run = l_run * alpha + ((sum4[0] + sum4[1]) + (sum4[2] + sum4[3]));   // partial row sum (combined in the epilogue)
-
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);                     // P buffer free, O quiescent
-        tc_fence_after();
-        // tcgen05.ld/st are warp-collective (.sync.aligned): the correction must be taken by the whole warp; the two
-        // warps of a quarter decide identically (same row maxima) and each rescales 64 of the 128 O columns
-        if (__any_sync(0xffffffffu, rescale)) {
-#pragma unroll 1
-          for (int c = half * 64; c < half * 64 + 64; c += 32) {
-            float ov[32];
-            tmem_ld32(lane_addr + 2 * BN + c, ov);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] *= alpha;
-            tmem_st32(lane_addr + 2 * BN + c, ov);
-          }
-          tmem_wait_st();
-        }
-      }
-      // P -> fp16 (hi, lo), K-major rows of 64 keys, 128B swizzle
-#pragma unroll
-      for (int ch4 = 0; ch4 < 4; ++ch4) {
-        const int ch = half * 4 + ch4;
-        uint32_t hi[4], lo[4];
-#pragma unroll
-        for (int e = 0; e < 4; ++e) split_f16x2(pe[ch4 * 8 + 2 * e], pe[ch4 * 8 + 2 * e + 1], &hi[e], &lo[e]);
-        const uint32_t off = sw128_offset(r, ch);
-        *reinterpret_cast<uint4*>(p_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(p_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-      }
-      fence_proxy_async();
-      tc_fence_before();
-      mbar_arrive(p_full);
     }
-
-    // ---- epilogue: O / l -> smem (reusing the Q region) -> coalesced 512-byte rows ----
-    mbar_wait(pv_done, (T - 1) & 1);
-    tc_fence_after();
-    float* lx = reinterpret_cast<float*>(smem + OFF_P);      // P is dead now: exchange the two partial row sums
-    lx[half * 128 + r] = l_run;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float inv = 1.0f / (lx[r] + lx[128 + r]);
-    float* osm = reinterpret_cast<float*>(smem + OFF_Q);     // [128][128] fp32, 16-byte chunks XOR-swizzled by row
-#pragma unroll 1
-    for (int c = half * 64; c < half * 64 + 64; c += 32) {
-      float ov[32];
-      tmem_ld32(lane_addr + 2 * BN + c, ov);
-      tmem_wait_ld();
-      if (p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0)
-        for (int i = 0; i < 32; ++i) p.dbg[BM * BN + r * 128 + c + i] = ov[i];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int chunk = (c >> 2) + i;
-        *reinterpret_cast<float4*>(osm + r * 128 + ((chunk ^ (r & 31)) << 2)) =
-            make_float4(ov[4 * i] * inv, ov[4 * i + 1] * inv, ov[4 * i + 2] * inv, ov[4 * i + 3] * inv);
-      }
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");          // every row was filled by the two warps of its quarter
-    float* obase = p.out + (long long)n * g.h * g.w * p.ldo;
-    for (int rr = half * 16; rr < half * 16 + 16; ++rr) {
-      const int row = quarter * 32 + rr;
-      const int tk = __shfl_sync(0xffffffffu, tok, rr);
-      if (tk < 0) continue;                                   // warp-uniform (tk is a broadcast)
-      const float4 v = *reinterpret_cast<const float4*>(osm + row * 128 + ((lane ^ (row & 31)) << 2));
-      if (p.out) *reinterpret_cast<float4*>(obase + (long long)tk * p.ldo + lane * 4) = v;
-      if (p.out_split) {
-        uint32_t h0, h1, l0, l1;
-        split_f16x2(v.x, v.y, &h0, &l0);
-        split_f16x2(v.z, v.w, &h1, &l1);
-        __half* d = p.out_split + ((long long)n * g.h * g.w + tk) * 128 + lane * 4;
-        *reinterpret_cast<uint2*>(d) = make_uint2(h0, h1);
-        *reinterpret_cast<uint2*>(d + p.split_plane) = make_uint2(l0, l1);
-      }
-    }
-    }   // HAS_V
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, TMEM_COLS);
+  float o[64];                                              // O: 64 rows x 128 channels of this warpgroup
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  const bool dump = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
+  for (int j = 0; j < T; ++j) {
+    const int s = j & 1;
+    const int n0 = j * BN;
+    float sv[32];
+    compute_s(j, sv);
+    if (dump && j == 0)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) p.dbg[(fr + 8 * ((i >> 1) & 1)) * BN + 8 * (i >> 2) + fc + (i & 1)] = sv[i];
+    uint32_t ph[16], pl[16];                                // P as fp16 (hi, lo) pairs, already in the A-operand layout
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // masks only where they can apply: windows touching a shift-region boundary, the ragged last key tile
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = n0 + 8 * jj + fc + e;
+          float& x = sv[4 * jj + 2 * h + e];
+          if (masked && kreg[col < g.lw ? col : 0] != rq[h]) x -= 100.0f * SQRT_C;
+          if (col >= g.lw) x = -CUDART_INF_F;
+        }
+      float mx = -CUDART_INF_F;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) mx = fmaxf(mx, fmaxf(sv[4 * jj + 2 * h], sv[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      float alpha = 1.0f;
+      if (mx > m_run[h] + LAZY_THRESH) {                    // first tile: m_run = -inf -> true
+        alpha = exp2f((m_run[h] - mx) * EXP_SCALE);         // exp2(-inf) = 0 on the first tile
+        m_run[h] = mx;
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) { o[4 * jj + 2 * h] *= alpha; o[4 * jj + 2 * h + 1] *= alpha; }
+      }
+      const float mscaled = m_run[h] * EXP_SCALE;
+      float sum = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const float p0 = ex2_approx(fmaf(sv[4 * jj + 2 * h], EXP_SCALE, -mscaled));
+        const float p1 = ex2_approx(fmaf(sv[4 * jj + 2 * h + 1], EXP_SCALE, -mscaled));
+        sum += p0 + p1;
+        split_f16x2(p0, p1, &ph[2 * jj + h], &pl[2 * jj + h]);
+      }
+      l_run[h] = l_run[h] * alpha + sum;                    // partial row sum (combined in the epilogue)
+    }
+    // O += P V: A = P from registers (16 keys per MMA), B = V tile, MN-major
+    mbar_wait_inline(v_full + s, (j >> 1) & 1);
+    const uint32_t v_base = smem_u32(smem + OFF_V + s * KV_STAGE_BYTES);
+    fence_acc(o);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint32_t* pp = c == 0 ? pl : ph;              // lo*hi, hi*lo, hi*hi
+        const uint32_t a[4] = {pp[4 * ks], pp[4 * ks + 1], pp[4 * ks + 2], pp[4 * ks + 3]};
+        wgmma_rs_n128_tb(o, a, desc_mnmajor(v_base + (c == 1 ? 16384 : 0) + ks * 2048, 8192), true);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(v_empty + s);
+  }
+
+  // ---- epilogue: O / l -> smem (reusing the Q region once both warpgroups are done with it) -> coalesced 512-byte rows ----
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    inv[h] = 1.0f / l;
+  }
+  consumers_sync();
+  float* osm = reinterpret_cast<float*>(smem + OFF_Q);     // [128][128] fp32, 16-byte chunks XOR-swizzled by row
+#pragma unroll
+  for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = fr + 8 * h, col = 8 * jj + fc;
+      if (dump) { p.dbg[BM * BN + row * 128 + col] = o[4 * jj + 2 * h]; p.dbg[BM * BN + row * 128 + col + 1] = o[4 * jj + 2 * h + 1]; }
+      *reinterpret_cast<float2*>(osm + row * 128 + (((col >> 2) ^ (row & 31)) << 2) + (col & 3)) =
+          make_float2(o[4 * jj + 2 * h] * inv[h], o[4 * jj + 2 * h + 1] * inv[h]);
+    }
+  consumers_sync();
+  float* obase = p.out + (long long)n * g.h * g.w * p.ldo;
+  for (int row = cw * 16; row < cw * 16 + 16; ++row) {
+    const int tq = m0 + row;
+    if (tq >= g.lw) break;                                  // warp-uniform
+    const int tk = window_token(g, win, tq);
+    const float4 v = *reinterpret_cast<const float4*>(osm + row * 128 + ((lane ^ (row & 31)) << 2));
+    if (p.out) *reinterpret_cast<float4*>(obase + (long long)tk * p.ldo + lane * 4) = v;
+    if (p.out_split) {
+      uint32_t h0, h1, l0, l1;
+      split_f16x2(v.x, v.y, &h0, &l0);
+      split_f16x2(v.z, v.w, &h1, &l1);
+      __half* d = p.out_split + ((long long)n * g.h * g.w + tk) * 128 + lane * 4;
+      *reinterpret_cast<uint2*>(d) = make_uint2(h0, h1);
+      *reinterpret_cast<uint2*>(d + p.split_plane) = make_uint2(l0, l1);
+    }
   }
 }
 
@@ -555,11 +475,8 @@ int split_windows_launch(const float* q, const float* k, const float* v, long lo
 }
 
 // the fused attention kernel on window-major operand planes [2][n_streams][nwin][lp][128] (one buffer per operand)
-int attention_planes_launch(const __half* wq, const __half* wk, const __half* wv, float* out, long long ldo, __half* out_split,
-                            long long split_plane, int n_streams, int kv_shift, const Geom& g, float* dbg, cudaStream_t st);
 
-// first-generation kernel (one query tile per CTA): kept behind UM_ATTN_V1=1 as the A/B baseline of um_attention_tc2.cu
-int attention_planes_launch_v1(const __half* wq, const __half* wk, const __half* wv, float* out, long long ldo, __half* out_split,
+int attention_planes_launch(const __half* wq, const __half* wk, const __half* wv, float* out, long long ldo, __half* out_split,
                                long long split_plane, int n_streams, int kv_shift, const Geom& g, float* dbg, cudaStream_t st) {
   const int lp = padded_lw(g.lw);
   int rc;
@@ -575,7 +492,7 @@ int attention_planes_launch_v1(const __half* wq, const __half* wk, const __half*
   p.out_split = out_split; p.split_plane = split_plane;
   const int qtiles = (g.lw + BM - 1) / BM;                  // the ragged last tile is masked in the epilogue
   attn_tc_kernel<true><<<dim3(qtiles, g.nwin, n_streams), NTHREADS, SMEM_BYTES, st>>>(mq, mk, mv, p);
-  return check_launch("um_window_attention(tcgen05)");
+  return check_launch("um_window_attention(wgmma)");
 }
 
 // fp32 token rows in: split pass + kernel.  Returns the number of query rows per window that were handled.
@@ -613,7 +530,7 @@ int softmax_expectation_tc(const float* q, const float* k, const float* values, 
   p.values = values; p.vdim = vdim; p.value_mode = value_mode; p.post_op = post_op;
   const int qtiles = (g.lw + BM - 1) / BM;
   attn_tc_kernel<false><<<dim3(qtiles, g.nwin, n_streams), NTHREADS, SMEM_BYTES, st>>>(mq, mk, mk, p);
-  return check_launch("um_softmax_expectation(tcgen05)");
+  return check_launch("um_softmax_expectation(wgmma)");
 }
 
 }  // namespace um

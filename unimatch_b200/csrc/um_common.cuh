@@ -1,4 +1,4 @@
-// Shared helpers for libunimatch_sm100 (sm_100a only).
+// Shared helpers for libunimatch_sm100 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -55,7 +55,7 @@ inline int device_sm_count() {
   if (!sms[d]) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
-    sms[d] = n > 0 ? n : 148;
+    sms[d] = n > 0 ? n : 132;
   }
   return sms[d];
 }

@@ -1,18 +1,18 @@
-// Implicit-GEMM convolution / Linear layer on the tcgen05 tensor cores, fp32-faithful (fp16 hi/lo split operands).
+// Implicit-GEMM convolution / Linear layer on the Hopper tensor cores (wgmma), fp32-faithful (fp16 hi/lo split operands).
 //
 //   out[b,y,x,co] = post( bias[co] + sum_{src,ky,kx,ci} in_src[b, y+ky-ph, x+kx-pw, ci] * W[co, (src,ky,kx,ci)] )
 //
 // * Activations are channel-last fp16 (hi, lo) planes [2][B][H][W][Cp] (Cp multiple of 64).  One 4-D TMA box
-//   (64 channels x 16 x 8 pixels) per filter tap lands directly in the 128B-swizzled K-major layout UMMA reads:
+//   (64 channels x 16 x 8 pixels) per filter tap lands directly in the 128B-swizzled K-major layout wgmma reads:
 //   im2col is nothing but shifted box coordinates, and the zero padding of the convolution is TMA's out-of-bounds
 //   fill.  Up to two input tensors are summed in the same accumulator, so torch.cat([h, x]) of the GRU never exists.
 // * Weights are prepared once as [2][Cout_p][Ktot] fp16 planes, K ordered (src, tap, ci).
-// * Persistent CTAs (one per SM) loop over tiles of 128 output pixels (16 x 8) x BN output channels (BN = 16 ... 256);
-//   warp 0 = TMA producer (2-3 stage mbarrier ring that keeps running across tiles), warp 1 = MMA issuer (3 split
-//   terms x 4 K-steps of 128xBNx16 per stage) into a DOUBLE-BUFFERED TMEM accumulator (single for the widest tiles),
-//   warps 2-9 = epilogue straight out of TMEM (thread = pixel, two groups interleaved over the 32-channel chunks)
-//   overlapping the next tile's MMAs: bias, activation, fused GRU gate math or LayerNorm(+residual), fp32 and/or
-//   fp16-split channel-last bulk-tensor stores at a channel offset of a wider buffer (free concatenation).
+// * Persistent CTAs (one per SM) loop over tiles of 128 output pixels (16 x 8) x BN output channels (BN = 16 ... 128);
+//   warp 0 = TMA producer (2-3 stage mbarrier ring that keeps running across tiles), warpgroups 1 and 2 = consumers:
+//   each runs the MMAs of 64 of the tile's pixels (3 split terms x 4 K-steps of wgmma 64xBNx16 per stage) into register
+//   accumulators, then both hand the tile through shared memory to the epilogue (thread = pixel, two groups interleaved
+//   over the 32-channel chunks): bias, activation, fused GRU gate math or LayerNorm(+residual), fp32 and/or fp16-split
+//   channel-last bulk-tensor stores at a channel offset of a wider buffer (free concatenation).
 //
 // Replaces the fp32 convolutions of BasicUpdateBlock (reg_refine.py:6-119), refine_proj (unimatch.py:315), the CNN
 // encoder (backbone.py:49-86) and the transformer's Linear layers (1x1 "convolution" over a [rows/16, 16] pixel grid).
@@ -28,15 +28,20 @@ using namespace tc;
 namespace {
 
 constexpr int TW = 16, TH = 8;                 // spatial tile = 128 pixels
-// operand ring depth: three 64 KB stages, or two when the stages are wide (BN > 128: 80-96 KB) or when the kernel trades
-// a stage for more epilogue staging buffers (NSB = 3: the short-K, store-bound Linear layers)
-__host__ __device__ constexpr int stages_for(int bn, int nsb) { return (bn > 128 || nsb > 1) ? 2 : 3; }
-// CTA-pair kernels hold half of the weight tile per CTA: stage = 32 KB of A + bn x 128 B of B
-__host__ __device__ constexpr int stages_pair(int bn, int nsb = 1) { return nsb > 1 ? 2 : (bn > 128 ? 3 : 4); }
-constexpr int NTHREADS = 320;              // TMA warp + MMA warp + 8 epilogue warps
+// operand ring depth: three stages, or two for the widest tiles (BN >= 96: 56-64 KB a stage next to their accumulator tile)
+__host__ __device__ constexpr int stages_for(int bn) { return bn >= 96 ? 2 : 3; }
+// 2 consumer warpgroups (warps 0-7) + one TMA producer warp (warp 8)
+constexpr int NTHREADS = 288;
+constexpr int PRODUCER = 8;
 constexpr uint32_t A_BYTES = 2 * 16384;        // hi + lo, [128 x 64] fp16 each
 constexpr uint32_t STAGING_UNIT = 16384;       // one epilogue staging buffer: [128 rows x 32 floats]
-constexpr uint32_t TAIL_BYTES = 256 + 2048;    // barriers + TMEM slot, then bias[2][128] | gamma[128] | beta[128]
+constexpr uint32_t STAGING_BYTES = 2 * STAGING_UNIT;
+constexpr uint32_t TAIL_BYTES = 256 + 2048;    // barriers, then bias[2][128] | gamma[128] | beta[128]
+// accumulator tile handed from the MMA layout to the epilogue: [chunk of 32 channels][128 rows][32 floats]
+__host__ __device__ constexpr uint32_t acc_bytes(int bn) { return (bn < 32 ? 32 : bn) * 128 * 4; }
+__host__ __device__ constexpr uint32_t conv_smem_bytes(int bn) {
+  return stages_for(bn) * (A_BYTES + 2 * bn * 128) + acc_bytes(bn) + STAGING_BYTES + TAIL_BYTES;
+}
 
 struct ConvParams {
   int B, H, W, tiles_x, tiles_y;
@@ -69,65 +74,39 @@ __device__ __forceinline__ uint32_t pack_h2(__half a, __half b) {
   return (uint32_t)__half_as_ushort(a) | ((uint32_t)__half_as_ushort(b) << 16);
 }
 
-// sum of the G partial accumulators of 32 consecutive output channels (fp32 round-to-nearest adds)
-template <int BN, int G>
-__device__ __forceinline__ void load_acc32(uint32_t taddr, int gused, float* v) {
-  tmem_ld32(taddr, v);
-  tmem_wait_ld();
-  if (G > 1) {
-#pragma unroll 1
-    for (int g = 1; g < gused; ++g) {
-      float t[32];
-      tmem_ld32(taddr + g * BN, t);
-      tmem_wait_ld();
+// 32 consecutive output channels [c0, c0 + 32) of accumulator row r (16-byte pieces XOR-swizzled by row)
+__device__ __forceinline__ void load_acc32(const float* accs, int r, int c0, float* v) {
+  const float* row = accs + (c0 >> 5) * 4096 + r * 32;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] += t[i];
-    }
+  for (int i = 0; i < 8; ++i) {
+    const float4 x = *reinterpret_cast<const float4*>(row + ((i ^ (r & 7)) << 2));
+    v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
   }
 }
 
-// G = number of TMEM accumulators the K loop is dealt across (round robin over stages).  Tensor-core fp32 accumulation
-// rounds toward zero at every accumulate step; G accumulators see G x fewer, G x smaller additions each and are summed
-// with ordinary fp32 adds in the epilogue, which cuts the truncation error of long-K convolutions by ~G.
-// MODE / ACT >= 0 compile the epilogue for exactly that fused post-operation (a short straight-line loop: with the
-// run-time switch over every mode the four epilogue warps spent most of their time in instruction-fetch stalls on
-// far branches and were slower than the MMA loop of the short-K Linear layers); -1 = decided at run time.
-// NSB = staging buffers per epilogue group (bulk stores in flight per group = NSB - 1 while the next chunk is staged).
-//
-// PAIR = true: the CTAs of a 2-cluster run every MMA together (cta_group::2, M = 256: each CTA its own 128-pixel tile, the
-// same BN output channels).  Each CTA stages its own A tile and HALF of the weight tile (BN/2 rows); the leader (cluster
-// rank 0) issues the MMAs and its commits arrive on the barriers of both CTAs.  Per SM the operand stream out of shared
-// memory drops from (4 + BN/32) KB to (4 + BN/64) KB per K step: a 128 x N x 16 SS-form MMA takes N/2 tensor cycles and
-// (4096 + 32 N) / 128 cycles of operand reads -- N = 64 is operand bound (48 vs 32), N = 128 balanced, N = 256 math bound.
-// With half the B tile per CTA the 64-wide launches gain directly, and two 128-wide (or 96-wide) tiles with
-// double-buffered accumulators replace the 256-wide (192-wide) single-buffer tile (DESIGN.md 3.2.1).
-template <int BN, int G, int MODE, int ACT, int NSB = 1, bool WIN = false, bool PAIR = false>
+// G > 1: every K stage (12 MMAs) is accumulated into a fresh register accumulator and added to the tile's running sum
+// with ordinary round-to-nearest fp32 adds.  Tensor-core fp32 accumulation truncates at every accumulate step; the long-K
+// convolutions (K >= 512) see one such step per stage instead of one per MMA.
+// MODE / ACT >= 0 compile the epilogue for exactly that fused post-operation (a short straight-line loop instead of a
+// run-time switch over every mode); -1 = decided at run time.
+template <int BN, int G, int MODE, int ACT, bool WIN = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant__ CUtensorMap map_a1,
                const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_of,
                const __grid_constant__ CUtensorMap map_os, ConvParams p) {
-  static_assert(!PAIR || (!WIN && BN >= 64), "CTA-pair kernels: plain convolutions with BN >= 64");
-  constexpr int BROWS = PAIR ? BN / 2 : BN;                // weight rows staged by this CTA
-  constexpr uint32_t B_BYTES = 2 * BROWS * 128;            // hi + lo, [BROWS x 64] fp16 each
+  static_assert(BN == 16 || BN == 64 || BN == 96 || BN == 128, "tile widths 16, 64, 96, 128");
+  constexpr int NSB = 1;                                   // staging buffers per epilogue group
+  constexpr uint32_t B_BYTES = 2 * BN * 128;               // hi + lo, [BN x 64] fp16 each
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-  constexpr int STAGES = PAIR ? stages_pair(BN, NSB) : stages_for(BN, NSB);
-  constexpr uint32_t STAGING_BYTES = 2 * NSB * STAGING_UNIT;
-  constexpr uint32_t ACC_COLS = G * BN;                        // one buffer = G accumulators side by side
-  // two accumulator buffers (the epilogue of tile t overlaps the MMAs of tile t+1) whenever they fit the 512 columns;
-  // the wide tiles (BN = 192 / 256 with G = 2) keep one: their K loops are long and the epilogue is a small share
-  constexpr int NACC = 2 * ACC_COLS <= 512 ? 2 : 1;
-  constexpr uint32_t TMEM_NEED = NACC * ACC_COLS;
-  constexpr uint32_t TMEM_COLS = TMEM_NEED <= 32 ? 32 : TMEM_NEED <= 64 ? 64 : TMEM_NEED <= 128 ? 128 : TMEM_NEED <= 256 ? 256 : 512;
-  static_assert(TMEM_COLS <= 512 && (TMEM_COLS & (TMEM_COLS - 1)) == 0, "TMEM allocation must be a power of two <= 512");
+  constexpr int STAGES = stages_for(BN);
+  constexpr uint32_t ACC_BYTES = acc_bytes(BN);
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* stage_buf = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);      // 2 x [128 rows x 32 cols] fp32
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + STAGING_BYTES);
+  float* accs = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  float* stage_buf = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + ACC_BYTES);   // 2 x [128 rows x 32 cols] fp32
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + ACC_BYTES + STAGING_BYTES);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
-  uint64_t* acc_full = bars + 2 * STAGES; // [2]
-  uint64_t* acc_empty = acc_full + 2;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* coef = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES + STAGING_BYTES + 256);
+  float* coef = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
   const int mode = MODE >= 0 ? MODE : p.mode;
   const int act = ACT >= 0 ? ACT : p.act;
 
@@ -136,167 +115,130 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   int nk = 0;
   for (int s = 0; s < p.nsrc; ++s) nk += taps * (p.cin_p[s] >> 6);
 
-  // work distribution: CTA (or CTA pair) `cid` of `ncid` walks the tiles cid, cid + ncid, ...; a pair tile is two
-  // consecutive pixel tiles (one per CTA) x the same BN channels
-  const int rank = PAIR ? (int)cluster_ctarank() : 0;
-  const int cid = PAIR ? (int)cluster_id_x() : (int)blockIdx.x;
-  const int ncid = PAIR ? (int)cluster_count_x() : (int)gridDim.x;
+  // work distribution: CTA `cid` of `ncid` walks the tiles cid, cid + ncid, ...
+  const int cid = (int)blockIdx.x;
+  const int ncid = (int)gridDim.x;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, PAIR ? 512 : 256); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 8); }   // empty: one arrival per consumer warp
     fence_barrier_init();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER && lane == 0) {
     tma_prefetch_desc(&map_a0); tma_prefetch_desc(&map_w);
     if (p.nsrc > 1) tma_prefetch_desc(&map_a1);
   }
-  if (warp == 1) {
-    if (PAIR) tmem_alloc_pair(tmem_slot, TMEM_COLS);
-    else tmem_alloc(tmem_slot, TMEM_COLS);
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();            // the peer's barriers are initialised before anybody signals them
-  else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  // the accumulator buffer goes back to the MMA warp -- of the leader CTA when two CTAs share the MMAs
-  const uint32_t acc_empty_leader = PAIR ? smem_of_cta(acc_empty, 0) : 0u;
-  auto acc_release = [&](int buf) {
-    if (PAIR) mbar_arrive_remote(acc_empty_leader + buf * 8);
-    else mbar_arrive(acc_empty + buf);
-  };
+  __syncthreads();
 
-  // Producer and MMA warps run CONVERGED (all 32 lanes execute the loops, one elected lane issues the TMA / MMA
-  // instructions): addresses and descriptors are then provably warp-uniform and live in uniform registers.  Guarding the
-  // whole role with `if (lane == 0)` made every UTCHMMA pay ~20 instructions of ELECT / R2UR.BROADCAST glue (~100+ cycles
-  // per MMA, more than the MMA itself).
-  if (warp == 0) {
-    {
-      int it = 0;
-      const uint32_t full_leader = PAIR ? smem_of_cta(full, 0) : 0u;
-      for (int t = cid; t < p.ntiles; t += ncid) {
-        const int n0 = (t % p.tiles_n) * BN;
-        int tile = t / p.tiles_n;
-        if (PAIR) tile = 2 * tile + rank;
-        const int x0 = (tile % p.tiles_x) * TW; tile /= p.tiles_x;
-        const int y0 = (tile % p.tiles_y) * TH;
-        const int b = tile / p.tiles_y;
-        // K stages are visited in a per-CTA rotated order: all CTAs need the same weight tiles, and walking them in
-        // lock step makes every SM hit the same L2 lines at the same time
-        const int chunks0 = p.cin_p[0] >> 6;
-        const int nk0 = taps * chunks0;
-        const int rot = (int)((unsigned)cid % (unsigned)nk);
-        for (int kk = 0; kk < nk; ++kk, ++it) {
-          int k = kk + rot; if (k >= nk) k -= nk;
-          const int sidx = (k >= nk0) ? 1 : 0;
-          const int kl = sidx ? k - nk0 : k;
-          const int chunks = sidx ? (p.cin_p[1] >> 6) : chunks0;
-          const int tap = kl / chunks, kc = kl - tap * chunks;
-          const int ky = tap / p.KW, kx = tap - ky * p.KW;
-          const CUtensorMap* ma = sidx ? &map_a1 : &map_a0;
-          const int st = it % STAGES;
-          mbar_wait(empty + st, ((it / STAGES) & 1) ^ 1);
-          uint8_t* sa = smem + st * STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          const int kcol = (sidx ? taps * p.cin_p[0] : 0) + tap * p.cin_p[sidx] + kc * 64;
-          if (elect_one()) {
-            if (PAIR) {
-              // both CTAs' bytes are counted on the leader's barrier (the peer's may land before the leader arms it: the
-              // phase cannot complete while the leader's arrival is pending)
-              if (rank == 0) mbar_arrive_expect_tx(full + st, 2 * STAGE_BYTES);
-              const uint32_t fb = full_leader + st * 8;
-#pragma unroll
-              for (int part = 0; part < 2; ++part) {
-                tma_load_4d_pair(sa + part * 16384, ma, fb, kc * 64, x0 * p.stride + kx - p.PW, y0 * p.stride + ky - p.PH, part * p.B + b);
-                tma_load_2d_pair(sb + part * (BROWS * 128), &map_w, fb, kcol, part * p.cout_p + n0 + rank * BROWS);
-              }
-            } else {
-              mbar_arrive_expect_tx(full + st, STAGE_BYTES);
-#pragma unroll
-              for (int part = 0; part < 2; ++part) {
-                tma_load_4d(sa + part * 16384, ma, full + st, kc * 64, x0 * p.stride + kx - p.PW, y0 * p.stride + ky - p.PH, part * p.B + b);
-                tma_load_2d(sb + part * (BN * 128), &map_w, full + st, kcol, part * p.cout_p + n0);
-              }
-            }
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (!PAIR || rank == 0) {
-      constexpr uint32_t IDESC = idesc_f16(PAIR ? 256 : 128, BN, 0, 0);
-      int it = 0, lt = 0;
-      for (int t = cid; t < p.ntiles; t += ncid, ++lt) {
-        const int buf = NACC == 2 ? (lt & 1) : 0;
-        mbar_wait(acc_empty + buf, (((NACC == 2 ? (lt >> 1) : lt) & 1) ^ 1));
-        tc_fence_after();
-        const uint32_t dbase = tmem + buf * ACC_COLS;
-        int mcount = 0;                                        // MMAs issued for this tile
-        for (int k = 0; k < nk; ++k, ++it) {
-          const int st = it % STAGES;
-          mbar_wait(full + st, (it / STAGES) & 1);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + st * STAGE_BYTES);
-          const uint32_t b_base = a_base + A_BYTES;
-          const int pa[3] = {1, 0, 0}, pb[3] = {0, 1, 0};      // lo*hi, hi*lo, hi*hi
-          if (elect_one()) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks) {
-                // consecutive MMAs go to different accumulators: each sees G x fewer truncating additions
-                const int mi = mcount + c * 4 + ks;
-                const uint32_t d = dbase + (mi % G) * BN;
-                if (PAIR)
-                  umma_f16_pair(d, desc_kmajor(a_base + pa[c] * 16384 + ks * 32), desc_kmajor(b_base + pb[c] * (BROWS * 128) + ks * 32),
-                                IDESC, mi >= G);
-                else
-                  umma_f16(d, desc_kmajor(a_base + pa[c] * 16384 + ks * 32), desc_kmajor(b_base + pb[c] * (BN * 128) + ks * 32),
-                           IDESC, mi >= G);
-              }
-            if (PAIR) umma_commit_pair(empty + st);
-            else umma_commit(empty + st);
-          }
-          __syncwarp();
-          mcount += 12;
-        }
+  // The producer warp runs CONVERGED (all 32 lanes execute the loops, one elected lane issues the TMA instructions):
+  // addresses are then provably warp-uniform and live in uniform registers.
+  if (warp == PRODUCER) {
+    int it = 0;
+    for (int t = cid; t < p.ntiles; t += ncid) {
+      const int n0 = (t % p.tiles_n) * BN;
+      int tile = t / p.tiles_n;
+      const int x0 = (tile % p.tiles_x) * TW; tile /= p.tiles_x;
+      const int y0 = (tile % p.tiles_y) * TH;
+      const int b = tile / p.tiles_y;
+      // K stages are visited in a per-CTA rotated order: all CTAs need the same weight tiles, and walking them in
+      // lock step makes every SM hit the same L2 lines at the same time
+      const int chunks0 = p.cin_p[0] >> 6;
+      const int nk0 = taps * chunks0;
+      const int rot = (int)((unsigned)cid % (unsigned)nk);
+      for (int kk = 0; kk < nk; ++kk, ++it) {
+        int k = kk + rot; if (k >= nk) k -= nk;
+        const int sidx = (k >= nk0) ? 1 : 0;
+        const int kl = sidx ? k - nk0 : k;
+        const int chunks = sidx ? (p.cin_p[1] >> 6) : chunks0;
+        const int tap = kl / chunks, kc = kl - tap * chunks;
+        const int ky = tap / p.KW, kx = tap - ky * p.KW;
+        const CUtensorMap* ma = sidx ? &map_a1 : &map_a0;
+        const int st = it % STAGES;
+        mbar_wait_inline(empty + st, ((it / STAGES) & 1) ^ 1);
+        uint8_t* sa = smem + st * STAGE_BYTES;
+        uint8_t* sb = sa + A_BYTES;
+        const int kcol = (sidx ? taps * p.cin_p[0] : 0) + tap * p.cin_p[sidx] + kc * 64;
         if (elect_one()) {
-          if (PAIR) umma_commit_pair(acc_full + buf);
-          else umma_commit(acc_full + buf);
+          mbar_arrive_expect_tx(full + st, STAGE_BYTES);
+#pragma unroll
+          for (int part = 0; part < 2; ++part) {
+            tma_load_4d(sa + part * 16384, ma, full + st, kc * 64, x0 * p.stride + kx - p.PW, y0 * p.stride + ky - p.PH, part * p.B + b);
+            tma_load_2d(sb + part * (BN * 128), &map_w, full + st, kcol, part * p.cout_p + n0);
+          }
         }
+        __syncwarp();
       }
     }
   } else {
-    // ---- epilogue: 8 warps = 2 groups x 4 TMEM lane quarters; thread = output pixel (accumulator row).  Group g owns
-    //      the 32-channel chunks g, g+2, ... of the tile: two warps per scheduler hide each other's TMEM / global /
+    // ---- consumers.  MMA: warpgroup grp computes pixels [64 grp, 64 grp + 64) of the tile.
+    //      Epilogue: 8 warps = 2 groups x 4 row quarters; thread = output pixel (accumulator row).  Group g owns
+    //      the 32-channel chunks g, g+2, ... of the tile: two warps per scheduler hide each other's shared / global /
     //      MUFU latencies, and the per-chunk math (GELU, gates, LayerNorm) is spread over twice the issue slots.
     //      Results are staged in shared memory in TMA box layout (16 KB per group) and ONE thread per group issues
-    //      bulk tensor stores; everything overlaps the MMAs of the next tile (other TMEM buffer). ----
+    //      bulk tensor stores, which overlap the MMAs of the next tile. ----
     const int quarter = warp & 3;
-    const int grp = (warp - 2) >> 2;
+    const int grp = warp >> 2;
     const int r = quarter * 32 + lane;
-    const int eg = ((warp - 2) & 3) * 32 + lane;           // 0..127 inside the group
+    const int eg = (warp & 3) * 32 + lane;           // 0..127 inside the group
+    const int frow = grp * 64 + quarter * 16 + (lane >> 2); // first accumulator row of this thread's MMA fragment (+ 8)
+    const int fcol = 2 * (lane & 3);
     const bool leader = eg == 0;
     int sctr = 0;                                          // staging passes issued by this group (buffer ring position)
     auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); };
     auto all_sync = [&]() { asm volatile("bar.sync 3, 256;" ::: "memory"); };
     if (mode == UM_CONV_LN && grp == 0) { coef[256 + eg] = __ldg(p.gamma + eg); coef[384 + eg] = __ldg(p.beta + eg); }
-    int lt = 0;
+    int lt = 0, it = 0;
     for (int t = cid; t < p.ntiles; t += ncid, ++lt) {
-      const int buf = NACC == 2 ? (lt & 1) : 0;
-      const int acc_par = (NACC == 2 ? (lt >> 1) : lt) & 1;
+      // ---- MMAs of this warpgroup's 64 rows ----
+      float acc[BN / 2], part[BN / 2];
+      for (int k = 0; k < nk; ++k, ++it) {
+        const int st = it % STAGES;
+        mbar_wait_inline(full + st, (it / STAGES) & 1);
+        const uint32_t a_base = smem_u32(smem + st * STAGE_BYTES) + grp * 8192;
+        const uint32_t b_base = smem_u32(smem + st * STAGE_BYTES) + A_BYTES;
+        const int pa[3] = {1, 0, 0}, pb[3] = {0, 1, 0};        // lo*hi, hi*lo, hi*hi
+        if (G > 1) fence_acc(part); else fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+#pragma unroll
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint64_t da = desc_kmajor(a_base + pa[c] * 16384 + ks * 32);
+            const uint64_t db = desc_kmajor(b_base + pb[c] * (BN * 128) + ks * 32);
+            if (G > 1) wgmma_ss<BN>(part, da, db, (c | ks) != 0);
+            else wgmma_ss<BN>(acc, da, db, k > 0 || (c | ks) != 0);
+          }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (G > 1) fence_acc(part); else fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty + st);                  // this warp is done with the stage
+        if (G > 1) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = k ? acc[i] + part[i] : part[i];
+        }
+      }
+      // ---- accumulator tile -> shared memory (the previous tile's epilogue has finished reading it) ----
+      all_sync();
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + fcol;
+        float* chunk = accs + (col >> 5) * 4096;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = frow + 8 * h;
+          *reinterpret_cast<float2*>(chunk + row * 32 + ((((col & 31) >> 2) ^ (row & 7)) << 2) + (col & 3)) =
+              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+      }
+      all_sync();
+
       const int n0 = (t % p.tiles_n) * BN;
       int tile = t / p.tiles_n;
-      if (PAIR) tile = 2 * tile + rank;
       const int x0 = (tile % p.tiles_x) * TW; tile /= p.tiles_x;
       const int y0 = (tile % p.tiles_y) * TH;
       const int b = tile / p.tiles_y;
       const long long pix_r = ((long long)b * p.H + (y0 + (r >> 4))) * p.W + x0 + (r & 15);
       const bool valid_r = (y0 + (r >> 4) < p.H) && (x0 + (r & 15) < p.W);
-      const uint32_t lane_addr = tmem + ((uint32_t)(quarter * 32) << 16) + buf * ACC_COLS;
-      const int gused = (nk * 12 < G) ? nk * 12 : G;
 
       // One 32-channel chunk of the tile -> global memory.  The group's staging buffer was last read by the bulk store
       // this group issued for its previous chunk: that read must be over before anybody overwrites it (checking only
@@ -389,14 +331,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
               a1[4 * i] = u4.x; a1[4 * i + 1] = u4.y; a1[4 * i + 2] = u4.z; a1[4 * i + 3] = u4.w;
             }
           }
-          all_sync();                                        // everybody is done with the previous tile's exchange slots
-          mbar_wait(acc_full + buf, acc_par);
-          tc_fence_after();
           float v0[32], v1[32];
-          load_acc32<BN, G>(lane_addr + ca, gused, v0);
-          load_acc32<BN, G>(lane_addr + cb, gused, v1);
-          tc_fence_before();
-          acc_release(buf);
+          load_acc32(accs, r, ca, v0);
+          load_acc32(accs, r, cb, v1);
           float* xs = coef;                                  // [2 groups][128 rows] (LN has no bias: the slots are free)
           float sum = 0.f;
 #pragma unroll
@@ -438,7 +375,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
       }
 
       // bias slice of this tile -> shared memory (read back as broadcast float4; double-buffered by tile parity)
-      float* sbias = coef + (lt & 1) * (BN > 128 ? 256 : 128);
+      float* sbias = coef + (lt & 1) * 128;
       if (grp == 0) {
         for (int i = eg; i < BN; i += 128) sbias[i] = (p.bias && n0 + i < p.cout) ? __ldg(p.bias + n0 + i) : 0.f;
         if (WIN) {                                           // destination row of every token of this tile (eg = row)
@@ -459,13 +396,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         }
       }
       all_sync();
-      mbar_wait(acc_full + buf, acc_par);
-      tc_fence_after();
-      if (grp * 32 >= BN) {                                  // narrow tiles: the second group has no chunk
-        tc_fence_before();
-        acc_release(buf);
-        continue;
-      }
+      if (grp * 32 >= BN) continue;                          // narrow tiles: the second group has no chunk
 
       constexpr int CH = BN < 32 ? BN : 32;
 #pragma unroll 1
@@ -502,11 +433,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(pp + i); px[4 * i] = t4.x; px[4 * i + 1] = t4.y; px[4 * i + 2] = t4.z; px[4 * i + 3] = t4.w; }
         }
         float v[32];
-        load_acc32<BN, G>(lane_addr + c0, gused, v);       // BN = 16: the upper 16 columns are unused
-        if (c0 + 64 >= BN) {               // this thread's last read of the accumulator: hand it back to the MMA warp
-          tc_fence_before();
-          acc_release(buf);
-        }
+        load_acc32(accs, r, c0, v);                          // BN = 16: the upper 16 columns are unused
         if (!live) continue;
         // ---- per-pixel math on the thread's own row ----
         if (p.bias) {
@@ -589,15 +516,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
     }
     if (leader) bulk_wait_all();                             // shared memory must outlive the last bulk stores
   }
-
-  tc_fence_before();
-  if (PAIR) cluster_sync_all();            // nobody leaves while the peer may still signal its barriers / read its operands
-  else __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem, TMEM_COLS);
-    else tmem_dealloc(tmem, TMEM_COLS);
-  }
 }
 
 // fp32 rows [rows, C] (row stride ld) -> fp16 (hi, lo) planes at channel offset `off` of a [rows, cp] buffer
@@ -663,47 +581,17 @@ int make_map_out(CUtensorMap* map, void* base, int elem_bytes, uint64_t cout, ui
 
 namespace {
 
-template <int BN, int G, int MODE, int ACT, int NSB = 1, bool WIN = false>
+template <int BN, int G, int MODE, int ACT, bool WIN = false>
 int launch_conv(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mof,
                 const CUtensorMap& mos, const ConvParams& p, cudaStream_t st) {
-  constexpr uint32_t smem = stages_for(BN, NSB) * (A_BYTES + 2 * BN * 128) + 2 * NSB * STAGING_UNIT + TAIL_BYTES;
+  constexpr uint32_t smem = conv_smem_bytes(BN);
   static_assert(smem <= 232448, "shared memory budget");
   static PerDeviceBytes configured;
-  if (int rc = ensure_smem(configured, conv_tc_kernel<BN, G, MODE, ACT, NSB, WIN>, smem, "conv_tc")) return rc;
+  if (int rc = ensure_smem(configured, conv_tc_kernel<BN, G, MODE, ACT, WIN>, smem, "conv_tc")) return rc;
   const int num_sms = device_sm_count();
   const int grid = p.ntiles < num_sms ? p.ntiles : num_sms;      // persistent: one CTA per SM
-  conv_tc_kernel<BN, G, MODE, ACT, NSB, WIN><<<grid, NTHREADS, smem, st>>>(m0, m1, mw, mof, mos, p);
+  conv_tc_kernel<BN, G, MODE, ACT, WIN><<<grid, NTHREADS, smem, st>>>(m0, m1, mw, mof, mos, p);
   return check_launch("um_conv2d_tc");
-}
-
-// CTA-pair launch: clusters of two CTAs (one TPC), one cluster per pair tile or as many as the device holds at once.
-// p.ntiles counts PAIR tiles; mw is the weight map with a box of BN / 2 rows.
-template <int BN, int G, int MODE, int ACT, int NSB = 1>
-int launch_conv_pair(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& mw, const CUtensorMap& mof,
-                     const CUtensorMap& mos, const ConvParams& p, cudaStream_t st) {
-  constexpr uint32_t smem = stages_pair(BN, NSB) * (A_BYTES + BN * 128) + 2 * NSB * STAGING_UNIT + TAIL_BYTES;
-  static_assert(smem <= 232448, "shared memory budget");
-  auto kernel = conv_tc_kernel<BN, G, MODE, ACT, NSB, false, true>;
-  static PerDeviceBytes configured;
-  if (int rc = ensure_smem(configured, kernel, smem, "conv_tc(pair)")) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st; cfg.attrs = attr; cfg.numAttrs = 1;
-  static int max_clusters[kMaxDevices] = {};
-  const int dev = current_device();
-  if (!max_clusters[dev]) {
-    int n = 0;
-    cfg.gridDim = dim3(2 * (device_sm_count() / 2));
-    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess || n <= 0) { cudaGetLastError(); n = device_sm_count() / 2; }
-    max_clusters[dev] = n;
-  }
-  const int clusters = p.ntiles < max_clusters[dev] ? p.ntiles : max_clusters[dev];
-  cfg.gridDim = dim3(2 * clusters);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, m0, m1, mw, mof, mos, p);
-  if (e != cudaSuccess) { set_error("um_conv2d_tc(pair): %s", cudaGetErrorString(e)); cudaGetLastError(); return UM_ECUDA; }
-  return check_launch("um_conv2d_tc(pair)");
 }
 
 }  // namespace
@@ -773,8 +661,6 @@ int um_conv2d_tc(const um_conv_desc* d, void* stream) {
   p.aux0 = d->aux0; p.ld_aux0 = d->ld_aux0; p.aux1 = d->aux1; p.ld_aux1 = d->ld_aux1;
   p.gamma = d->gamma; p.beta = d->beta;
   p.pre = d->pre; p.ld_pre = d->ld_pre;
-  p.tiles_n = d->cout_p / d->bn;
-  p.ntiles = p.tiles_x * p.tiles_y * p.B * p.tiles_n;
   if (d->split_plane_stride) p.plane_split = d->split_plane_stride;
   if (win) {
     p.win_dst = reinterpret_cast<__half*>(d->win_dst);
@@ -786,34 +672,20 @@ int um_conv2d_tc(const um_conv_desc* d, void* stream) {
 
   long long ktot = 0;
   for (int s = 0; s < d->nsrc; ++s) ktot += (long long)d->kh * d->kw * d->cin_p[s];
-  // long K loops are dealt across several accumulators (see conv_tc_kernel); short ones (Linear layers) need one
+  // long K loops sum per-stage partial accumulators with fp32 adds (see conv_tc_kernel); short ones (Linear layers) need none
   const long long nk = ktot / 64;
   const bool multi = nk >= 8;
-  // CTA pairs (see conv_tc_kernel, PAIR): the operand-stream-bound launches, i.e. everything but the one- or two-stage
-  // Linear layers (store bound) and the 16-wide heads.  Needs an even number of pixel tiles (one per CTA of a pair).
-  static int pair_env = -1;
-  if (pair_env < 0) { const char* e = getenv("UM_CONV_PAIR"); pair_env = (e && e[0] == '0') ? 0 : 1; }
-  const int pixel_tiles = p.tiles_x * p.tiles_y * p.B;
-  bool pair = pair_env && !win && d->bn >= 64 && nk >= 3 && (pixel_tiles % 2 == 0);
-  if (pair) {
-    // only the instantiations below exist as pair kernels
-    const bool lin = d->mode == UM_CONV_LINEAR;
-    const bool relu = lin && d->act == UM_ACT_RELU, none = lin && d->act == UM_ACT_NONE, gelu = lin && d->act == UM_ACT_GELU;
-    if (d->bn == 256) pair = multi ? (d->mode == UM_CONV_GRU_ZR || relu) : (relu || gelu);
-    else if (d->bn == 192 || d->bn == 96) pair = multi && relu;
-    else if (d->bn == 128) pair = multi && (none || relu || d->mode == UM_CONV_GRU_ZR || d->mode == UM_CONV_GRU_Q || d->mode == UM_CONV_LN);
-    else pair = multi && (none || relu);
-  }
-  // 96-wide tiles (192 output channels as 2 x 96 with double-buffered accumulators) exist as a CTA-pair kernel only
-  UM_REQUIRE(d->bn != 96 || pair, "um_conv2d_tc: bn 96 needs a CTA-pair launch (long-K Linear + ReLU, even number of 16 x 8 pixel tiles)");
-  if (pair) p.ntiles = (pixel_tiles / 2) * p.tiles_n;
+  // the accumulator tile lives in registers of two warpgroups: 256- and 192-wide channel tiles run as two 128- / 96-wide ones
+  const int bn = d->bn == 256 ? 128 : d->bn == 192 ? 96 : d->bn;
+  p.tiles_n = d->cout_p / bn;
+  p.ntiles = p.tiles_x * p.tiles_y * p.B * p.tiles_n;
   CUtensorMap m0, m1, mw;
   int rc;
   const uint64_t sps = (uint64_t)d->src_plane_stride;
   if ((rc = make_map_4d_f16(&m0, d->src[0], d->cin_p[0], d->w, d->h, 2ull * d->batch, d->stride, sps))) return rc;
   if (d->nsrc > 1) { if ((rc = make_map_4d_f16(&m1, d->src[1], d->cin_p[1], d->w, d->h, 2ull * d->batch, d->stride, sps))) return rc; }
   else m1 = m0;
-  if ((rc = make_map_2d_f16(&mw, d->weights, 2ull * d->cout_p, (uint64_t)ktot, (uint32_t)(pair ? d->bn / 2 : d->bn)))) return rc;
+  if ((rc = make_map_2d_f16(&mw, d->weights, 2ull * d->cout_p, (uint64_t)ktot, (uint32_t)bn))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   CUtensorMap mof = m0, mos = m0;
   if (d->bn >= 32) {
@@ -832,38 +704,11 @@ int um_conv2d_tc(const um_conv_desc* d, void* stream) {
   }
   // the post-operations the matching path uses get their own epilogue instantiation; anything else runs the generic one
 #define UM_CONV_CASE(BN_, G_, MODE_, ACT_)                                                   \
-  if (d->bn == BN_ && multi == (G_ > 1) && d->mode == MODE_ && ((MODE_) != UM_CONV_LINEAR || d->act == (ACT_))) \
+  if (bn == BN_ && multi == (G_ > 1) && d->mode == MODE_ && ((MODE_) != UM_CONV_LINEAR || d->act == (ACT_))) \
     return launch_conv<BN_, G_, MODE_, (MODE_) == UM_CONV_LINEAR ? (ACT_) : 0>(m0, m1, mw, mof, mos, p, st);
-#define UM_CONV_PAIR_CASE(BN_, G_, MODE_, ACT_)                                              \
-  if (d->bn == BN_ && multi == (G_ > 1) && d->mode == MODE_ && ((MODE_) != UM_CONV_LINEAR || d->act == (ACT_))) \
-    return launch_conv_pair<BN_, G_, MODE_, (MODE_) == UM_CONV_LINEAR ? (ACT_) : 0>(m0, m1, mw, mof, mos, p, st);
-  if (pair) {
-    UM_CONV_PAIR_CASE(256, 2, UM_CONV_GRU_ZR, 0)
-    UM_CONV_PAIR_CASE(256, 2, UM_CONV_LINEAR, UM_ACT_RELU)
-    UM_CONV_PAIR_CASE(256, 1, UM_CONV_LINEAR, UM_ACT_RELU)
-    UM_CONV_PAIR_CASE(256, 1, UM_CONV_LINEAR, UM_ACT_GELU)
-    UM_CONV_PAIR_CASE(192, 2, UM_CONV_LINEAR, UM_ACT_RELU)
-    UM_CONV_PAIR_CASE(96, 2, UM_CONV_LINEAR, UM_ACT_RELU)
-    UM_CONV_PAIR_CASE(128, 2, UM_CONV_LINEAR, UM_ACT_NONE)
-    UM_CONV_PAIR_CASE(128, 2, UM_CONV_LINEAR, UM_ACT_RELU)
-    UM_CONV_PAIR_CASE(128, 2, UM_CONV_GRU_ZR, 0)
-    UM_CONV_PAIR_CASE(128, 2, UM_CONV_GRU_Q, 0)
-    UM_CONV_PAIR_CASE(128, 2, UM_CONV_LN, 0)
-    UM_CONV_PAIR_CASE(64, 4, UM_CONV_LINEAR, UM_ACT_NONE)
-    UM_CONV_PAIR_CASE(64, 4, UM_CONV_LINEAR, UM_ACT_RELU)
-    set_error("um_conv2d_tc: no CTA-pair instantiation for this launch (internal)");
-    return UM_EINVAL;
-  }
-#undef UM_CONV_PAIR_CASE
-  // one- or two-stage K loops (the K = 128 Linear layers) are store-bound: a 2-stage ring and 3 staging buffers per group
   if (win) {
     UM_REQUIRE(nk <= 2, "um_conv2d_tc: window-plane output is built for K <= 128");
-    return launch_conv<128, 1, UM_CONV_LINEAR, UM_ACT_NONE, 3, true>(m0, m1, mw, mof, mos, p, st);
-  }
-  if (d->bn == 128 && nk <= 2) {
-    if (d->mode == UM_CONV_LINEAR && d->act == UM_ACT_NONE) return launch_conv<128, 1, UM_CONV_LINEAR, UM_ACT_NONE, 3>(m0, m1, mw, mof, mos, p, st);
-    if (d->mode == UM_CONV_LINEAR && d->act == UM_ACT_RELU) return launch_conv<128, 1, UM_CONV_LINEAR, UM_ACT_RELU, 3>(m0, m1, mw, mof, mos, p, st);
-    if (d->mode == UM_CONV_LN) return launch_conv<128, 1, UM_CONV_LN, 0, 3>(m0, m1, mw, mof, mos, p, st);
+    return launch_conv<128, 1, UM_CONV_LINEAR, UM_ACT_NONE, true>(m0, m1, mw, mof, mos, p, st);
   }
   UM_CONV_CASE(128, 1, UM_CONV_LINEAR, UM_ACT_NONE)
   UM_CONV_CASE(128, 1, UM_CONV_LINEAR, UM_ACT_RELU)
@@ -874,18 +719,13 @@ int um_conv2d_tc(const um_conv_desc* d, void* stream) {
   UM_CONV_CASE(128, 2, UM_CONV_LINEAR, UM_ACT_RELU)
   UM_CONV_CASE(128, 2, UM_CONV_GRU_ZR, 0)
   UM_CONV_CASE(128, 2, UM_CONV_GRU_Q, 0)
-  UM_CONV_CASE(256, 2, UM_CONV_GRU_ZR, 0)
-  UM_CONV_CASE(256, 2, UM_CONV_LINEAR, UM_ACT_RELU)
-  UM_CONV_CASE(256, 1, UM_CONV_LINEAR, UM_ACT_RELU)
-  UM_CONV_CASE(256, 1, UM_CONV_LINEAR, UM_ACT_GELU)
-  UM_CONV_CASE(192, 2, UM_CONV_LINEAR, UM_ACT_RELU)
+  UM_CONV_CASE(96, 2, UM_CONV_LINEAR, UM_ACT_RELU)
   UM_CONV_CASE(64, 4, UM_CONV_LINEAR, UM_ACT_NONE)
   UM_CONV_CASE(64, 4, UM_CONV_LINEAR, UM_ACT_RELU)
 #undef UM_CONV_CASE
-  if (d->bn == 256) return multi ? launch_conv<256, 2, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<256, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
-  if (d->bn == 192) return multi ? launch_conv<192, 2, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<192, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
-  if (d->bn == 128) return multi ? launch_conv<128, 2, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<128, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
-  if (d->bn == 64) return multi ? launch_conv<64, 4, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<64, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
+  if (bn == 128) return multi ? launch_conv<128, 2, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<128, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
+  if (bn == 96) return multi ? launch_conv<96, 2, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<96, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
+  if (bn == 64) return multi ? launch_conv<64, 4, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<64, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
   return multi ? launch_conv<16, 4, -1, -1>(m0, m1, mw, mof, mos, p, st) : launch_conv<16, 1, -1, -1>(m0, m1, mw, mof, mos, p, st);
 }
 

@@ -1,31 +1,18 @@
-// Fused transformer FFN on the tcgen05 tensor cores (CTA pairs), fp32-faithful (fp16 hi/lo split operands):
+// Fused transformer FFN on the Hopper tensor cores (wgmma + TMA), fp32-faithful (fp16 hi/lo split operands):
 //
 //   out = residual + LayerNorm( GELU( [source | message] W1^T ) W2^T )            transformer.py:137-144
 //
-// The two-launch version (um_conv2d_tc: FFN1 256 -> 1024 + GELU, then FFN2 1024 -> 128 + LN) writes the 1024-wide hidden
-// activation as fp16 (hi, lo) planes -- 4 KB per token row, 1.6 GB at 8 pairs of 480x832 -- and reads it back through HBM
-// (FFN2: 72 % DRAM throughput; ncu, profiles/r02_ncu_conv.md).  Here the hidden activation of a 128-row tile never leaves
-// the SM: it is produced 128 channels at a time into a TMEM accumulator, GELU'd and split by the epilogue warps IN PLACE
-// (fp16 pairs over the fp32 columns they came from, the way the attention kernel keeps P), and consumed from TMEM as the
-// A operand of the second GEMM, whose 128 x 128 accumulator lives in TMEM across the 8 chunks.
+// Run as two GEMM launches (um_conv2d_tc: FFN1 256 -> 1024 + GELU, then FFN2 1024 -> 128 + LN), the 1024-wide hidden
+// activation travels through HBM as fp16 (hi, lo) planes -- 4 KB per token row, 1.6 GB at 8 pairs of 480x832.  Here it
+// never leaves the registers: one CTA per 128-row tile, warp-specialised:
 //
-// Two CTAs of a cluster (one TPC) share every MMA (cta_group::2, M = 256: each CTA its own 128 rows): the weight tiles --
-// 1.5 MB per row tile, the whole operand stream of this kernel -- are staged half per CTA.
-//
-//   warp 0      TMA producer: the row tile's [source | message] planes (128 KB, resident for the tile) and a 4-slot ring
-//               of 16 KB weight tiles in the order the MMA warp consumes them:
-//               W1(0) W1(1) W2(0) W1(2) W2(1) ... W1(7) W2(6) W2(7)    (W1(c): 4 K-slices, W2(c): 2 K-halves)
-//   warp 1      MMA issuer (leader CTA only): H_c = X W1_c^T (48 MMAs 256x128x16, SS), issued one chunk AHEAD of
-//               O += P_c W2_c^T (24 MMAs, A = P_c from TMEM) so the pipe has work while the epilogue runs GELU on chunk c
-//   warps 2-9   epilogue: group g (4 warps = 4 TMEM lane quarters) owns hidden columns [64 g, 64 g + 64) of every chunk:
-//               tcgen05.ld -> exact-erf GELU -> (hi, lo) fp16 pairs -> tcgen05.st over the same columns -> arrive;
-//               after the last chunk: LayerNorm (two-pass statistics) + residual on O, fp32 rows and fp16 planes out
-//               through shared-memory staging and bulk tensor stores.
-//
-// TMEM (per CTA, 512 columns allocated): H0 [0,128)  H1 [128,256)  O [256,384).
-// SMEM: X 128 KB | ring 4 x 16 KB | staging 2 x 16 KB | barriers + LN coefficients.
-#include <stdlib.h>
-
+//   warp 8          TMA producer: the tile's [source | message] planes (128 KB, resident for the tile), then a 5-slot ring
+//                   of 16 KB weight tiles in the order the consumers use them: W1(c) as 4 K-slices, W2(c) as 2 row halves
+//   warpgroups 0-1  consumers, 64 rows each, for every 64-wide hidden chunk c:
+//                   H_c = X W1_c^T (48 wgmma 64x64x16, both operands in shared memory) into registers -> exact-erf GELU ->
+//                   (hi, lo) fp16 pairs, which are already the register A operand of O += P_c W2_c^T (24 wgmma 64x64x16);
+//                   after the last chunk: LayerNorm (two-pass statistics over the 4 threads of a row) + residual on O,
+//                   fp32 rows and / or fp16 planes out.
 #include "um_common.cuh"
 #include "um_tc.cuh"
 
@@ -35,352 +22,187 @@ using namespace tc;
 
 namespace {
 
-constexpr int NTHREADS = 320;
-constexpr uint32_t X_BYTES = 4 * 32768;              // 4 K-chunks x (hi, lo) x [128 rows x 64 ch]
+constexpr int NTHREADS = 288;                        // 2 consumer warpgroups (warps 0-7) + one TMA producer warp (warp 8)
+constexpr int PRODUCER = 8;
+constexpr int HC = 64;                               // hidden channels per chunk
+constexpr uint32_t X_BYTES = 4 * 32768;              // 4 K-slices x (hi, lo) x [128 rows x 64 ch]
 constexpr uint32_t SLOT_BYTES = 16384;               // (hi, lo) x [64 weight rows x 64 k]
-constexpr int NSLOT = 4;
+constexpr int NSLOT = 5;
 constexpr uint32_t OFF_RING = X_BYTES;
-constexpr uint32_t OFF_STAGE = OFF_RING + NSLOT * SLOT_BYTES;       // 196608
-constexpr uint32_t OFF_BAR = OFF_STAGE + 2 * 16384;                 // 229376
-constexpr uint32_t OFF_COEF = OFF_BAR + 256;                        // xs[2][128] | gamma[128] | beta[128]
-constexpr uint32_t SMEM_BYTES = OFF_COEF + 2048;                    // 231680
+constexpr uint32_t OFF_BAR = OFF_RING + NSLOT * SLOT_BYTES;        // 212992
+constexpr uint32_t SMEM_BYTES = OFF_BAR + 256;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t COL_O = 256;
 
 struct FfnParams {
-  int npair_tiles;         // pairs of 128-row tiles
-  int nchunk;              // hidden / 128
-  int hidden;
+  int nchunk, hidden;
   const float* residual; long long ld_res;
   const float* gamma; const float* beta;
-  float* out_f32;
-  __half* out_split;
-  long long rows;
+  float* out_f32; long long ld_f32;
+  __half* out_split; long long split_plane;
 };
 
-// D[tmem, both CTAs] (+)= A[tmem of each CTA: fp16 pairs] * B[smem: N/2 rows per CTA]; leader thread only
-__device__ __forceinline__ void umma_f16_ts_pair(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, bool accumulate) {
-  uint32_t acc = accumulate ? 1u : 0u;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(acc)
-      : "memory");
-}
-
-__device__ __forceinline__ void tmem_st16u(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-      ::"r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(taddr)
-      : "memory");
-}
-
-// (320 threads are allocated as 12 warps -- one more per scheduler -- so 168 registers per thread is the most a CTA of this
-// shape can have: __maxnreg__(192) compiles and then fails to launch)
 __global__ void __launch_bounds__(NTHREADS, 1)
 ffn_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant__ CUtensorMap map_x1,
-              const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2,
-              const __grid_constant__ CUtensorMap map_of, const __grid_constant__ CUtensorMap map_os, FfnParams p) {
+              const __grid_constant__ CUtensorMap map_w1, const __grid_constant__ CUtensorMap map_w2, FfnParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* x_full = bars + 0;         // leader's counts the bytes of both CTAs
-  uint64_t* x_free = bars + 1;         // last H MMAs of the tile complete (multicast commit)
-  uint64_t* w_full = bars + 2;         // [4] leader's
-  uint64_t* w_empty = bars + 6;        // [4] own (multicast commit)
-  uint64_t* h_full = bars + 10;        // [2] H_c complete in buffer c & 1 (multicast commit)
-  uint64_t* p_full = bars + 12;        // [2] leader's: GELU'd operand written by the 2 x 256 epilogue threads
-  uint64_t* o_full = bars + 14;        // O complete (multicast commit)
-  uint64_t* o_free = bars + 15;        // leader's: O read out by the 2 x 256 epilogue threads
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  float* coef = reinterpret_cast<float*>(smem + OFF_COEF);
-  float* stage_buf = reinterpret_cast<float*>(smem + OFF_STAGE);
-
+  uint64_t* x_full = bars;
+  uint64_t* full = bars + 1;                 // [NSLOT]
+  uint64_t* empty = bars + 1 + NSLOT;        // [NSLOT]: one arrival per consumer warp
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rank = (int)cluster_ctarank();
-  const int cid = (int)cluster_id_x(), ncid = (int)cluster_count_x();
-  const int NC = p.nchunk;
+  const int tile = blockIdx.x;               // rows [128 tile, 128 tile + 128)
 
   if (threadIdx.x == 0) {
-    mbar_init(x_full, 1); mbar_init(x_free, 1); mbar_init(o_full, 1); mbar_init(o_free, 512);
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(w_full + i, 1); mbar_init(w_empty + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(h_full + i, 1); mbar_init(p_full + i, 512); }
+    mbar_init(x_full, 1);
+    for (int i = 0; i < NSLOT; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 8); }
     fence_barrier_init();
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == PRODUCER && lane == 0) {
     tma_prefetch_desc(&map_x0); tma_prefetch_desc(&map_x1); tma_prefetch_desc(&map_w1); tma_prefetch_desc(&map_w2);
   }
-  if (warp == 1) tmem_alloc_pair(tmem_slot, TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  __syncthreads();
 
-  if (warp == 0) {
-    // =============================== TMA producer (both CTAs; bytes counted on the leader's barriers) ===============================
-    const uint32_t x_full_l = smem_of_cta(x_full, 0), w_full_l = smem_of_cta(w_full, 0);
-    int it = 0, lt = 0;
-    auto load_w = [&](const CUtensorMap* map, int col, int row) {            // one ring slot: (hi, lo) x [64 rows x 64 k]
-      const int s = it % NSLOT;
-      mbar_wait(w_empty + s, ((it / NSLOT) & 1) ^ 1);
-      if (elect_one()) {
-        if (rank == 0) mbar_arrive_expect_tx(w_full + s, 2 * SLOT_BYTES);
-        uint8_t* dst = smem + OFF_RING + s * SLOT_BYTES;
-        tma_load_2d_pair(dst, map, w_full_l + s * 8, col, row);
-        tma_load_2d_pair(dst + 8192, map, w_full_l + s * 8, col, (map == &map_w1 ? p.hidden : 128) + row);
-      }
-      __syncwarp();
-      ++it;
-    };
-    auto load_w1 = [&](int c) { for (int k = 0; k < 4; ++k) load_w(&map_w1, k * 64, c * 128 + rank * 64); };
-    auto load_w2 = [&](int c) { for (int hf = 0; hf < 2; ++hf) load_w(&map_w2, c * 128 + hf * 64, rank * 64); };
-    for (int t = cid; t < p.npair_tiles; t += ncid, ++lt) {
-      const int y0 = (2 * t + rank) * 8;                       // rows as a [rows/16, 16] grid: tile = 8 grid rows
-      mbar_wait(x_free, (lt & 1) ^ 1);
-      if (elect_one()) {
-        if (rank == 0) mbar_arrive_expect_tx(x_full, 2 * X_BYTES);
+  if (warp == PRODUCER) {
+    if (elect_one()) {
+      mbar_arrive_expect_tx(x_full, X_BYTES);
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
+      for (int kc = 0; kc < 4; ++kc)                 // K slice kc: source kc / 2, channels 64 (kc % 2) ...
 #pragma unroll
-          for (int part = 0; part < 2; ++part)
-            tma_load_4d_pair(smem + k * 32768 + part * 16384, k < 2 ? &map_x0 : &map_x1, x_full_l, (k & 1) * 64, 0, y0, part);
-      }
-      __syncwarp();
-      load_w1(0);
-      for (int c = 0; c < NC; ++c) {
-        if (c + 1 < NC) load_w1(c + 1);
-        load_w2(c);
-      }
+        for (int part = 0; part < 2; ++part)
+          tma_load_4d(smem + (kc * 2 + part) * 16384, kc < 2 ? &map_x0 : &map_x1, x_full, (kc & 1) * 64, 0, tile * 8, part);
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer (leader CTA) ===============================
-    if (rank == 0) {
-      constexpr uint32_t IDESC = idesc_f16(256, 128, 0, 0);
-      int it = 0, lt = 0;
-      long long gc = 0;                                        // chunks issued so far (H / P buffer = gc & 1)
-      const uint32_t x_base = smem_u32(smem);
-      auto issue_h = [&](long long g, bool last) {            // H(g & 1) = X W1_c^T
-        const uint32_t d = tmem + (uint32_t)(g & 1) * 128;
-#pragma unroll 1
-        for (int k = 0; k < 4; ++k, ++it) {
-          const int s = it % NSLOT;
-          mbar_wait(w_full + s, (it / NSLOT) & 1);
-          tc_fence_after();
-          const uint32_t w_base = smem_u32(smem + OFF_RING + s * SLOT_BYTES);
-          if (elect_one()) {
-#pragma unroll 1
-            for (int c3 = 0; c3 < 3; ++c3) {                   // (x part, w part): lo*hi, hi*lo, hi*hi
-              const uint32_t xo = (c3 == 0 ? 16384u : 0u), wo = (c3 == 1 ? 8192u : 0u);
-#pragma unroll
-              for (int ks = 0; ks < 4; ++ks)
-                umma_f16_pair(d, desc_kmajor(x_base + k * 32768 + xo + ks * 32), desc_kmajor(w_base + wo + ks * 32), IDESC,
-                              (k | c3 | ks) != 0);
-            }
-            umma_commit_pair(w_empty + s);
-          }
-          __syncwarp();
-        }
+    __syncwarp();
+    int it = 0;
+    for (int c = 0; c < p.nchunk; ++c)
+      for (int q = 0; q < 6; ++q, ++it) {
+        const int s = it % NSLOT;
+        mbar_wait_inline(empty + s, ((it / NSLOT) & 1) ^ 1);
+        uint8_t* slot = smem + OFF_RING + s * SLOT_BYTES;
         if (elect_one()) {
-          umma_commit_pair(h_full + (g & 1));
-          if (last) umma_commit_pair(x_free);                  // X has been read for the last time
+          mbar_arrive_expect_tx(full + s, SLOT_BYTES);
+#pragma unroll
+          for (int part = 0; part < 2; ++part) {
+            if (q < 4) tma_load_2d(slot + part * 8192, &map_w1, full + s, q * 64, part * p.hidden + c * HC);
+            else tma_load_2d(slot + part * 8192, &map_w2, full + s, c * HC, part * 128 + (q - 4) * 64);
+          }
         }
         __syncwarp();
-      };
-      auto issue_pv = [&](long long g, bool first, bool last) {   // O (+)= P(g & 1) W2_c^T, P read from TMEM
-        const int hb = (int)(g & 1);
-        mbar_wait(p_full + hb, (uint32_t)((g >> 1) & 1));
-        if (first) mbar_wait(o_free, (lt & 1) ^ 1);            // the previous tile's O has left TMEM
-        tc_fence_after();
-        const uint32_t a = tmem + hb * 128;
-#pragma unroll 1
-        for (int hf = 0; hf < 2; ++hf, ++it) {
-          const int s = it % NSLOT;
-          mbar_wait(w_full + s, (it / NSLOT) & 1);
-          tc_fence_after();
-          const uint32_t w_base = smem_u32(smem + OFF_RING + s * SLOT_BYTES);
-          if (elect_one()) {
-#pragma unroll 1
-            for (int c3 = 0; c3 < 3; ++c3) {                   // (p part, w part): lo*hi, hi*lo, hi*hi
-              // P columns of K step j (16 hidden channels) inside the 64-column half: 32 (j >> 1) + 8 (j & 1), lo pairs + 16
-              const uint32_t po = (c3 == 0 ? 16u : 0u), wo = (c3 == 1 ? 8192u : 0u);
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                umma_f16_ts_pair(tmem + COL_O, a + 64 * hf + 32 * (j >> 1) + po + 8 * (j & 1), desc_kmajor(w_base + wo + j * 32),
-                                 IDESC, !(first && hf == 0 && c3 == 0 && j == 0));
-            }
-            umma_commit_pair(w_empty + s);
-          }
-          __syncwarp();
-        }
-        if (last) {
-          if (elect_one()) umma_commit_pair(o_full);
-          __syncwarp();
-        }
-      };
-      for (int t = cid; t < p.npair_tiles; t += ncid, ++lt) {
-        mbar_wait(x_full, lt & 1);
-        tc_fence_after();
-        issue_h(gc, NC == 1);
-#pragma unroll 1
-        for (int c = 0; c < NC; ++c) {
-          if (c + 1 < NC) issue_h(gc + c + 1, c + 2 == NC);
-          issue_pv(gc + c, c == 0, c + 1 == NC);
-        }
-        gc += NC;
       }
-    }
-  } else {
-    // =============================== epilogue: GELU in place, then LayerNorm + residual ===============================
-    const int quarter = warp & 3;
-    const int grp = (warp - 2) >> 2;
-    const int r = quarter * 32 + lane;
-    const int eg = ((warp - 2) & 3) * 32 + lane;
-    const bool leader = eg == 0;
-    const uint32_t lane_addr = tmem + ((uint32_t)(quarter * 32) << 16);
-    const uint32_t p_full_l = smem_of_cta(p_full, 0), o_free_l = smem_of_cta(o_free, 0);
-    auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); };
-    auto all_sync = [&]() { asm volatile("bar.sync 3, 256;" ::: "memory"); };
-    if (grp == 0) { coef[256 + eg] = __ldg(p.gamma + eg); coef[384 + eg] = __ldg(p.beta + eg); }
-    long long gc = 0;
-    int lt = 0;
-    for (int t = cid; t < p.npair_tiles; t += ncid, ++lt) {
-      const int y0 = (2 * t + rank) * 8;
-      const long long row = (long long)(y0 + (r >> 4)) * 16 + (r & 15);
-      const bool valid_r = row < p.rows;
-
-#pragma unroll 1
-      for (int c = 0; c < NC; ++c, ++gc) {
-        const int hb = (int)(gc & 1);
-        mbar_wait(h_full + hb, (uint32_t)((gc >> 1) & 1));
-        tc_fence_after();
-        // 32 hidden channels at a time, each block rewritten in place: k = 64 grp + 32 q + (2i, 2i+1) -> column
-        // 64 grp + 32 q + i (hi pairs), + 16 (lo pairs).
-        // A rolled loop keeps the role's code small (both blocks loaded up front + straight-line code: 0.767 vs 0.753 ms).
-#pragma unroll 1
-        for (int q = 0; q < 2; ++q) {
-          const uint32_t addr = lane_addr + hb * 128 + 64 * grp + 32 * q;
-          float sv[32];
-          tmem_ld32(addr, sv);
-          tmem_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) sv[i] = act_gelu(sv[i]);
-          uint32_t hi[16], lo[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) split_f16x2(sv[2 * i], sv[2 * i + 1], &hi[i], &lo[i]);
-          tmem_st16u(addr, hi);
-          tmem_st16u(addr + 16, lo);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive_remote(p_full_l + hb * 8);                 // (one arrival per warp instead of per thread: measured 5 % slower)
-      }
-
-      // ---- LayerNorm over the 128 output channels (+ residual): each group keeps 64 channels in registers ----
-      const int ca = grp * 32, cb = 64 + grp * 32;
-      float a0[32], a1[32];
-      const bool need_a = valid_r && p.residual;
-      if (need_a) {
-        const float4* pa = reinterpret_cast<const float4*>(p.residual + row * p.ld_res + ca);
-        const float4* pb = reinterpret_cast<const float4*>(p.residual + row * p.ld_res + cb);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float4 t4 = __ldg(pa + i), u4 = __ldg(pb + i);
-          a0[4 * i] = t4.x; a0[4 * i + 1] = t4.y; a0[4 * i + 2] = t4.z; a0[4 * i + 3] = t4.w;
-          a1[4 * i] = u4.x; a1[4 * i + 1] = u4.y; a1[4 * i + 2] = u4.z; a1[4 * i + 3] = u4.w;
-        }
-      }
-      all_sync();                                              // everybody is done with the previous tile's exchange slots
-      mbar_wait(o_full, lt & 1);
-      tc_fence_after();
-      float v0[32], v1[32];
-      tmem_ld32(lane_addr + COL_O + ca, v0);
-      tmem_ld32(lane_addr + COL_O + cb, v1);
-      tmem_wait_ld();
-      tc_fence_before();
-      mbar_arrive_remote(o_free_l);
-      float* xs = coef;                                        // [2 groups][128 rows]
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) sum += v0[i];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) sum += v1[i];
-      xs[grp * 128 + r] = sum;
-      all_sync();
-      const float mean = (xs[r] + xs[128 + r]) * (1.0f / 128.0f);
-      all_sync();
-      float sq = 0.f;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) { const float dd = v0[i] - mean; sq = fmaf(dd, dd, sq); }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) { const float dd = v1[i] - mean; sq = fmaf(dd, dd, sq); }
-      xs[grp * 128 + r] = sq;
-      all_sync();
-      const float rstd = rsqrtf((xs[r] + xs[128 + r]) * (1.0f / 128.0f) + 1e-5f);
-      const float4* g4a = reinterpret_cast<const float4*>(coef + 256 + ca);
-      const float4* b4a = reinterpret_cast<const float4*>(coef + 384 + ca);
-      const float4* g4b = reinterpret_cast<const float4*>(coef + 256 + cb);
-      const float4* b4b = reinterpret_cast<const float4*>(coef + 384 + cb);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float4 ga = g4a[i], ba = b4a[i], gb = g4b[i], bb = b4b[i];
-        v0[4 * i] = (v0[4 * i] - mean) * rstd * ga.x + ba.x;             v1[4 * i] = (v1[4 * i] - mean) * rstd * gb.x + bb.x;
-        v0[4 * i + 1] = (v0[4 * i + 1] - mean) * rstd * ga.y + ba.y;     v1[4 * i + 1] = (v1[4 * i + 1] - mean) * rstd * gb.y + bb.y;
-        v0[4 * i + 2] = (v0[4 * i + 2] - mean) * rstd * ga.z + ba.z;     v1[4 * i + 2] = (v1[4 * i + 2] - mean) * rstd * gb.z + bb.z;
-        v0[4 * i + 3] = (v0[4 * i + 3] - mean) * rstd * ga.w + ba.w;     v1[4 * i + 3] = (v1[4 * i + 3] - mean) * rstd * gb.w + bb.w;
-      }
-      if (need_a) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) { v0[i] += a0[i]; v1[i] += a1[i]; }
-      }
-      // 32 channels of the tile -> global memory through the group's staging buffer (TMA box layout) and bulk tensor stores;
-      // the buffer was last read by the bulk store this group issued before: that read must be over before it is overwritten
-      auto emit = [&](const float (&v)[32], int co) {
-        if (p.out_f32) {                                       // [128 rows][32 floats], 128B swizzle
-          float* my_stage = stage_buf + grp * 4096;
-          if (leader) bulk_wait_read<0>();
-          group_sync();
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            *reinterpret_cast<float4*>(my_stage + r * 32 + ((i ^ (r & 7)) << 2)) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          fence_proxy_async();
-          group_sync();
-          if (leader) { tma_store_4d(&map_of, my_stage, co, 0, y0, 0); bulk_commit(); }
-        }
-        if (p.out_split) {                                     // hi then lo: [128 rows][32 halves], 64-byte rows, 64B swizzle
-          uint8_t* sbs = reinterpret_cast<uint8_t*>(stage_buf + grp * 4096);
-          if (leader) bulk_wait_read<0>();
-          group_sync();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            uint32_t hw[4], lw[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) split_f16x2(v[8 * i + 2 * e], v[8 * i + 2 * e + 1], &hw[e], &lw[e]);
-            const int off = r * 64 + ((i ^ ((r >> 1) & 3)) << 4);
-            *reinterpret_cast<uint4*>(sbs + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-            *reinterpret_cast<uint4*>(sbs + 8192 + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-          }
-          fence_proxy_async();
-          group_sync();
-          if (leader) {
-            tma_store_4d(&map_os, sbs, co, 0, y0, 0);
-            tma_store_4d(&map_os, sbs + 8192, co, 0, y0, 1);
-            bulk_commit();
-          }
-        }
-      };
-      emit(v0, ca);
-      emit(v1, cb);
-    }
-    if (leader) bulk_wait_all();                               // shared memory must outlive the last bulk stores
+    return;
   }
 
-  tc_fence_before();
-  cluster_sync_all();                      // nobody leaves while the peer may still signal its barriers / read its operands
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem, TMEM_COLS);
+  // =============================== consumers ===============================
+  const int wg = warp >> 2;
+  const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows fr and fr + 8 (MMA fragment layout)
+  const int fc = 2 * (lane & 3);                            // ... and columns 8 j + fc + {0, 1}
+  const uint32_t x_base = smem_u32(smem) + wg * 8192;
+  const int pa[3] = {1, 0, 0}, pb[3] = {0, 1, 0};          // lo*hi, hi*lo, hi*hi
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  mbar_wait_inline(x_full, 0);
+  int it = 0;
+  for (int c = 0; c < p.nchunk; ++c) {
+    // ---- H_c = X W1_c^T: 64 rows x 64 hidden channels, K = 256 in 4 slots ----
+    float h[32];
+    int sl[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      sl[q] = (it + q) % NSLOT;
+      mbar_wait_inline(full + sl[q], ((it + q) / NSLOT) & 1);
+    }
+    fence_acc(h);
+    wgmma_fence();
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const uint32_t sb = smem_u32(smem + OFF_RING + sl[q] * SLOT_BYTES);
+#pragma unroll
+      for (int cc = 0; cc < 3; ++cc)
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+          wgmma_ss<64>(h, desc_kmajor(x_base + (q * 2 + pa[cc]) * 16384 + ks * 32), desc_kmajor(sb + pb[cc] * 8192 + ks * 32),
+                       (q | cc | ks) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(h);
+    __syncwarp();
+    if (lane == 0)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) mbar_arrive(empty + sl[q]);
+    it += 4;
+    // ---- GELU -> fp16 (hi, lo) pairs in the A-operand layout of the next MMA ----
+    uint32_t ph[16], pl[16];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+        split_f16x2(act_gelu(h[4 * jj + 2 * hh]), act_gelu(h[4 * jj + 2 * hh + 1]), &ph[2 * jj + hh], &pl[2 * jj + hh]);
+    // ---- O += P_c W2_c^T: output channels [0, 64) and [64, 128) from one slot each ----
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      sl[q] = (it + q) % NSLOT;
+      mbar_wait_inline(full + sl[q], ((it + q) / NSLOT) & 1);
+    }
+    fence_acc(o);
+    wgmma_fence();
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const uint32_t sb = smem_u32(smem + OFF_RING + sl[q] * SLOT_BYTES);
+      float (&oq)[32] = *reinterpret_cast<float (*)[32]>(o + 32 * q);
+#pragma unroll
+      for (int cc = 0; cc < 3; ++cc)
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint32_t* pp = cc == 0 ? pl : ph;
+          const uint32_t a[4] = {pp[4 * ks], pp[4 * ks + 1], pp[4 * ks + 2], pp[4 * ks + 3]};
+          wgmma_rs_n64(oq, a, desc_kmajor(sb + (cc == 1 ? 8192 : 0) + ks * 32), true);
+        }
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_acc(o);
+    __syncwarp();
+    if (lane == 0) { mbar_arrive(empty + sl[0]); mbar_arrive(empty + sl[1]); }
+    it += 2;
+  }
+
+  // ---- LayerNorm (+ residual) on the thread's two rows; a row's 128 channels are spread over 4 lanes ----
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const long long row = (long long)tile * 128 + fr + 8 * hh;
+    float sum = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) sum += o[4 * jj + 2 * hh] + o[4 * jj + 2 * hh + 1];
+    sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+    sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+    const float mean = sum * (1.0f / 128.0f);
+    float sq = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const float d0 = o[4 * jj + 2 * hh] - mean, d1 = o[4 * jj + 2 * hh + 1] - mean;
+      sq = fmaf(d0, d0, fmaf(d1, d1, sq));
+    }
+    sq += __shfl_xor_sync(0xffffffffu, sq, 1);
+    sq += __shfl_xor_sync(0xffffffffu, sq, 2);
+    const float rstd = rsqrtf(sq * (1.0f / 128.0f) + 1e-5f);
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int col = 8 * jj + fc;
+      float y0 = (o[4 * jj + 2 * hh] - mean) * rstd * __ldg(p.gamma + col) + __ldg(p.beta + col);
+      float y1 = (o[4 * jj + 2 * hh + 1] - mean) * rstd * __ldg(p.gamma + col + 1) + __ldg(p.beta + col + 1);
+      if (p.residual) {
+        const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + row * p.ld_res + col));
+        y0 += r.x; y1 += r.y;
+      }
+      if (p.out_f32) *reinterpret_cast<float2*>(p.out_f32 + row * p.ld_f32 + col) = make_float2(y0, y1);
+      if (p.out_split) {
+        uint32_t hi, lo;
+        split_f16x2(y0, y1, &hi, &lo);
+        *reinterpret_cast<uint32_t*>(p.out_split + row * 128 + col) = hi;
+        *reinterpret_cast<uint32_t*>(p.out_split + p.split_plane + row * 128 + col) = lo;
+      }
+    }
   }
 }
 
@@ -390,7 +212,6 @@ ffn_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant_
 extern "C" {
 
 int um_ffn_tc(const um_ffn_desc* d, void* stream) {
-  using namespace um;
   UM_REQUIRE(d && d->src[0] && d->src[1] && d->w1 && d->w2 && d->gamma && d->beta, "um_ffn_tc: null descriptor / operand");
   UM_REQUIRE(d->rows > 0 && d->rows % 256 == 0, "um_ffn_tc: rows must be a positive multiple of 256 (pairs of 128-row tiles)");
   UM_REQUIRE(d->hidden >= 128 && d->hidden % 128 == 0, "um_ffn_tc: hidden must be a multiple of 128");
@@ -407,41 +228,22 @@ int um_ffn_tc(const um_ffn_desc* d, void* stream) {
     UM_REQUIRE(d->split_plane_stride >= d->rows * 128 && d->split_plane_stride % 8 == 0 &&
                    (reinterpret_cast<uintptr_t>(d->out_split) & 15) == 0,
                "um_ffn_tc: output plane stride must cover rows * 128 halves (multiple of 8), 16-byte aligned planes");
+  using namespace um;
   const uint64_t gh = (uint64_t)d->rows / 16;                   // rows as a [rows/16, 16] pixel grid, 128 channels
-  CUtensorMap mx0, mx1, mw1, mw2, mof, mos;
+  CUtensorMap mx0, mx1, mw1, mw2;
   int rc;
   if ((rc = make_map_4d_f16(&mx0, d->src[0], 128, 16, gh, 2, 1, (uint64_t)d->src_plane_stride))) return rc;
   if ((rc = make_map_4d_f16(&mx1, d->src[1], 128, 16, gh, 2, 1, (uint64_t)d->src_plane_stride))) return rc;
   if ((rc = make_map_2d_f16(&mw1, d->w1, 2ull * d->hidden, 256, 64))) return rc;
   if ((rc = make_map_2d_f16(&mw2, d->w2, 2ull * 128, (uint64_t)d->hidden, 64))) return rc;
-  mof = mx0; mos = mx0;
-  if (d->out_f32 && (rc = make_map_out(&mof, d->out_f32, 4, 128, (uint64_t)d->ld_f32, 16, gh, 1))) return rc;
-  if (d->out_split && (rc = make_map_out(&mos, d->out_split, 2, 128, 128, 16, gh, 2, (uint64_t)d->split_plane_stride))) return rc;
   FfnParams p{};
-  p.npair_tiles = (int)(d->rows / 256); p.nchunk = d->hidden / 128; p.hidden = d->hidden;
+  p.nchunk = d->hidden / HC; p.hidden = d->hidden;
   p.residual = d->residual; p.ld_res = d->ld_res; p.gamma = d->gamma; p.beta = d->beta;
-  p.out_f32 = d->out_f32; p.out_split = reinterpret_cast<__half*>(d->out_split); p.rows = d->rows;
-
-  auto kernel = ffn_tc_kernel;
+  p.out_f32 = d->out_f32; p.ld_f32 = d->ld_f32;
+  p.out_split = reinterpret_cast<__half*>(d->out_split); p.split_plane = d->split_plane_stride;
   static PerDeviceBytes configured;
-  if ((rc = ensure_smem(configured, kernel, SMEM_BYTES, "ffn_tc"))) return rc;
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.blockDim = dim3(NTHREADS); cfg.dynamicSmemBytes = SMEM_BYTES; cfg.stream = (cudaStream_t)stream; cfg.attrs = attr; cfg.numAttrs = 1;
-  static int max_clusters[kMaxDevices] = {};
-  const int dev = current_device();
-  if (!max_clusters[dev]) {
-    int n = 0;
-    cfg.gridDim = dim3(2 * (device_sm_count() / 2));
-    if (cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess || n <= 0) { cudaGetLastError(); n = device_sm_count() / 2; }
-    max_clusters[dev] = n;
-  }
-  const int clusters = p.npair_tiles < max_clusters[dev] ? p.npair_tiles : max_clusters[dev];
-  cfg.gridDim = dim3(2 * clusters);
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, mx0, mx1, mw1, mw2, mof, mos, p);
-  if (e != cudaSuccess) { set_error("um_ffn_tc: %s", cudaGetErrorString(e)); cudaGetLastError(); return UM_ECUDA; }
+  if ((rc = ensure_smem(configured, ffn_tc_kernel, SMEM_BYTES, "ffn_tc"))) return rc;
+  ffn_tc_kernel<<<(unsigned)(d->rows / 128), NTHREADS, SMEM_BYTES, (cudaStream_t)stream>>>(mx0, mx1, mw1, mw2, p);
   return check_launch("um_ffn_tc");
 }
 

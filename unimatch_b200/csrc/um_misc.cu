@@ -178,7 +178,7 @@ __global__ void __launch_bounds__(256) gru_update_kernel(const float* __restrict
 
 inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
-  const long long cap = 148LL * 16;      // 148 SMs x 16 resident CTAs, grid-stride beyond that
+  const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
   return (int)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 

@@ -143,7 +143,7 @@ int um_instance_norm_apply(const float* a, int64_t ld_a, const float* stats_a, i
   p.split = reinterpret_cast<__half*>(out_split); p.cp = cp; p.off = off; p.plane = (long long)n * hw * cp;
   p.hw = hw; p.C = c; p.total4 = (long long)n * hw * (c / 4);
   long long blocks = (p.total4 + 255) / 256;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > 132LL * 32) blocks = 132LL * 32;
   in_apply_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(p);
   return um::check_launch("um_instance_norm_apply");
 }

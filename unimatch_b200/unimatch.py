@@ -1,6 +1,6 @@
 """Drop-in `UniMatch(nn.Module)`: the reference's constructor, `forward()` signature, `state_dict` layout and
 `{'flow_preds': [...]}` output (reference `unimatch/unimatch.py:17-26, :95-111, :365-367`), with the matching
-path executed by libunimatch_sm100 (hand-written sm_100a kernels) instead of eager PyTorch ops.
+path executed by libunimatch_sm100 (hand-written sm_90a kernels) instead of eager PyTorch ops.
 
 Host side = plain PyTorch orchestration:
   * parameters live in a module tree generated from `spec.param_spec` (same keys/shapes as the reference);
@@ -11,9 +11,9 @@ Host side = plain PyTorch orchestration:
   * loop-invariant / dead work of the refinement loop is hoisted (`refine_proj`, unimatch.py:315-320) or skipped
     (mask head on non-final iterations, unimatch.py:333,351) -- results are unchanged.
 Every Linear layer, the CNN backbone, the update-block convolutions, the `upsampler` head and the propagation
-projections run on the library's tcgen05 implicit-GEMM kernel (`um_conv2d_tc`, fp32-faithful split-fp16 operands);
-attention / correlation on the tcgen05 attention kernels.  There is no cuDNN / cuBLAS call on the path and no
-alternative backend in this module (A/B harnesses against the libraries live in tools/ab_paths.py).
+projections run on the library's wgmma implicit-GEMM kernel (`um_conv2d_tc`, fp32-faithful split-fp16 operands);
+attention / correlation on the wgmma attention kernel.  There is no cuDNN / cuBLAS call on the path and no
+alternative backend in this module.
 
 The forward pass is a sequence of `_stage_*` methods (encoder, position + warp, transformer, correlation,
 propagation, refinement iteration, upsampling) so that the parity tests can teacher-force every stage with the
@@ -38,11 +38,9 @@ _FUSED_FFN = _os.environ.get("UM_FUSED_FFN", "1") != "0"      # A/B switch of th
 
 
 def _bn256(b, h, w):
-    """Output-channel tile of the 256-channel update-block convolutions (GRU z|r, flow / mask heads).  With an even number of
-    16 x 8 pixel tiles the launch runs on CTA pairs (um_conv_tc.cu, PAIR): two 128-wide tiles with double-buffered TMEM
-    accumulators (the epilogue overlaps the next tile's MMAs; measured 16.3 -> 15.3 ms per step for the update block) beat
-    one 256-wide tile with a single buffer.  A lone CTA reads its A tile once per channel tile: the wide tile wins there."""
-    return 128 if (b * ((h + 7) // 8) * ((w + 15) // 16)) % 2 == 0 else 256
+    """Output-channel tile of the 256-channel update-block convolutions (GRU z|r, flow / mask heads): 128 (the
+    accumulator tile lives in the registers of two warpgroups)."""
+    return 128
 
 
 
@@ -270,7 +268,7 @@ class UniMatch(nn.Module):
 
     # ------------------------------------------------------------------------------------------ backbone
     def _stage_backbone(self, P, img0, img1, normalise):
-        """CNNEncoder (backbone.py:104-133) with every 3x3 / 1x1 convolution on the tcgen05 implicit-GEMM kernel and
+        """CNNEncoder (backbone.py:104-133) with every 3x3 / 1x1 convolution on the wgmma implicit-GEMM kernel and
         InstanceNorm + ReLU + residual as fused bandwidth passes that emit the next convolution's fp16 planes.
         The 7x7 stem (3 input channels) is the direct fp32 kernel `um_conv7x7_small` with `normalize_img` folded into its load.
         Returns the feature maps low -> high resolution, each [2B, h, w, 128] (first views, then second views)."""
@@ -387,7 +385,7 @@ class UniMatch(nn.Module):
 
     def _stage_transformer(self, P, x, h, w, attn_type, splits, tag="s0"):
         """FeatureTransformer.forward (transformer.py:226-294) on tokens x [N, L, 128], N = 2 x pairs.  Every Linear is a
-        tcgen05 GEMM over token rows (activations travel as fp16 (hi, lo) planes [2, rows, C] between GEMMs); LayerNorm
+        wgmma GEMM over token rows (activations travel as fp16 (hi, lo) planes [2, rows, C] between GEMMs); LayerNorm
         (+residual) / GELU are GEMM epilogues; `cat([source, message])` of the FFN (transformer.py:141) is a second GEMM
         source.  Where the window geometry runs on the tensor-core attention kernel, the q|k|v projections write the
         kernel's window-major operand planes directly (no fp32 q/k/v, no split pass) and the attention writes the merge
@@ -405,8 +403,8 @@ class UniMatch(nn.Module):
         hid = P["blocks"][0]["hid"]
         x_f, xo_f, x1_f = f32(c), f32(c), f32(c)
         x_s, xo_s, x1_s, msg_s, m_s = planes(c), planes(c), planes(c), planes(c), planes(c)
-        # FFN: one fused CTA-pair kernel (the 1024-wide hidden activation stays in tensor memory) when the rows are a whole
-        # number of tile pairs; else two GEMM launches around hidden planes in HBM
+        # FFN: one fused kernel (the 1024-wide hidden activation stays in registers) when the rows are a multiple of 256;
+        # else two GEMM launches around hidden planes in HBM
         fused_ffn = _FUSED_FFN and ops.ffn_tc_supported(rp)
         hid_s = None if fused_ffn else planes(hid)
         x_f[:rows] = x.reshape(rows, c)
@@ -445,9 +443,6 @@ class UniMatch(nn.Module):
                 _OPS.split_planes(msg.view(rows, c), msg_s, 0)
             G(msg_s, None, blk["tc_m_c"], None, 1, 1, 0, 0, c, 128, LN, 0, None, 0, m_s, 0, None, None, blk["g_c1"], blk["b_c1"], 1, rp)
             # ---- FFN on cat([source, message]) + LayerNorm + residual
-            # (Measured and not kept: FFN1 / FFN2 slab by slab over a hidden buffer that fits the L2 -- 22 x 2 launches of 71
-            # CTA-pair tiles instead of 2: transformer_s1 15.0 -> 18.5 ms; launch gaps and partial waves cost more than the
-            # 3.2 GB round trip of the hidden planes.)
             if fused_ffn:
                 self._timed("conv", 2.0 * rp * hid * (2 * c + c), _OPS.ffn_tc, x1_s, m_s, blk["tc_w1"], blk["tc_w2"], x1_f,
                             blk["g_c2"], blk["b_c2"], xo_f, xo_s, rp)
@@ -501,7 +496,7 @@ class UniMatch(nn.Module):
     def _stage_propagation(self, P, x_s, flow, nb, h, wd, prop_r):
         """SelfAttnPropagation.forward (attention.py:184-253) on the first `nb` streams of the transformer output planes
         x_s [2, rows_padded, 128]: q = Wq x + bq; global: k = Wk q + bk, out = softmax(q k^T / sqrt(C)) flow;
-        local (radius r): k = Wk x + bk, 3x3 zero-padded window.  Both projections are tcgen05 GEMMs."""
+        local (radius r): k = Wk x + bk, 3x3 zero-padded window.  Both projections are wgmma GEMMs."""
         dev = flow.device
         L = h * wd
         rows = nb * L
