@@ -184,6 +184,23 @@ int um_upsample2x(const float* flow, float* out, int32_t batch, int32_t h, int32
 int um_resize_bilinear(const float* in, float* out, int32_t batch, int32_t channels, int32_t h_in, int32_t w_in,
                        int32_t h_out, int32_t w_out, const float* scale, int32_t flip_x, void* stream);
 
+/* Video frames to model input: frames = DEVICE uint8 [n, h, w, 3] channel-last (what decoders produce) -> out fp32 planar
+ * [n, 3, h_out, w_out], bit-identical to um_resize_bilinear of the float-converted planar frames.  transpose != 0 reads each
+ * frame as its transpose [3, w, h] first (the portrait rule of evaluate_flow.py:713-717), so (h_out, w_out) is the size of
+ * the transposed image.  At (h_out, w_out) equal to the source size the pass is an exact conversion.  Replaces the host-side
+ * `torch.from_numpy(image).permute(2, 0, 1).float()`, transpose and F.interpolate of evaluate_flow.py:710-733. */
+int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t transpose,
+                        int32_t h_out, int32_t w_out, void* stream);
+
+/* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
+ * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
+ * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the
+ * maximum radius is a float32 reduction, the rest float64, as numpy evaluates the reference; zero flow is white.
+ * max_scratch: DEVICE buffer of n floats (receives the per-image maximum radius).
+ * Replaces flow_to_image (utils/flow_viz.py:240-275; called at evaluate_flow.py:768 for videos). */
+int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
+                     int32_t n, int32_t h, int32_t w, void* stream);
+
 /* GRU gate fusions of SepConvGRU (reg_refine.py:37-52): rows of 128 hidden channels, independent row strides
  * (floats, multiples of 4) so the z|r pre-activations may live side by side in one fused conv output.
  *   um_gru_rh:     rh = sigmoid(r_pre) * h

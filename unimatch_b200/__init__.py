@@ -20,10 +20,14 @@ _LAZY = {
     "infer_stereo": (".inference", "infer_stereo"),
     "infer_depth": (".inference", "infer_depth"),
     "BatchedFlowRunner": (".inference", "BatchedFlowRunner"),
+    "infer_flow_video": (".inference", "infer_flow_video"),
+    "VideoFlowRunner": (".inference", "VideoFlowRunner"),
+    "flow_to_image": (".inference", "flow_to_image"),
 }
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
-           "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check"]
+           "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
+           "flow_to_image"]
 
 
 def __getattr__(name):

@@ -6,11 +6,17 @@ resize-to-multiple / resize-back / rescale logic of `inference_flow` (evaluate_f
 `inference_depth` (evaluate_depth.py:297-419), and the forward-backward consistency check (geometry.py:75-96,
 evaluate_flow.py:774-792) -- but on BATCHES of pairs that are already device tensors, with every resize (flow-component /
 disparity rescale and flips folded in) as one `um_resize_bilinear` launch and the occlusion test as one fused kernel
-(`um_fb_consistency`).  File IO, visualisation and video handling stay out of scope.
+(`um_fb_consistency`).
 
 `BatchedFlowRunner` is the serving-side driver (evaluate_flow.py:686-760 runs one frame pair at a time): frames are padded to a
 fixed bucket, host batches are staged through two pinned buffers and copied on a side stream while the previous batch
 computes, and the fixed-shape forward is replayed as a CUDA graph.
+
+Video (`main_flow.py --inference_video`, evaluate_flow.py:642-831): `infer_flow_video` runs the consecutive pairs of a frame
+sequence with every frame encoded ONCE (pair (t, t+1) and pair (t+1, t+2) share frame t+1's feature pyramid; the encoder is
+per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 summation order), `VideoFlowRunner` streams host uint8 frames through the same
+path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
+colouring of utils/flow_viz.py on the device.  Decoding and writing files (frames, PNG, .flo, mp4) stay out of scope.
 """
 import math
 
@@ -73,20 +79,28 @@ def infer_flow(model, image1, image2, *, padding_factor, inference_size=None, pr
     multiple of `padding_factor` (or to `inference_size`), the flow is resized back and its components rescaled.
     Returns {'flow': [B,2,H,W]} plus 'flow_bwd' when `pred_bidir_flow` and 'fwd_occ' / 'bwd_occ' ([B,H,W], 1 = occluded)
     when `fwd_bwd_consistency_check`.  `model_kwargs` are forwarded to `model(...)` (attn_type, attn_splits_list, ...)."""
-    if fwd_bwd_consistency_check and not pred_bidir_flow:
-        raise ValueError("fwd_bwd_consistency_check needs pred_bidir_flow=True (evaluate_flow.py:774-792)")
+    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, "infer_flow")
     transposed = image1.size(-2) > image1.size(-1)
     if transposed:
         image1, image2 = image1.transpose(-2, -1), image2.transpose(-2, -1)
     ori = tuple(image1.shape[-2:])
     size = _inference_size(ori, padding_factor, inference_size)
-    resized = size != ori
-    if resized:
+    if size != ori:
         image1, image2 = _resize(image1, size), _resize(image2, size)
-    if model_kwargs.setdefault("task", "flow") != "flow":
-        raise ValueError("infer_flow drives the flow task only")
     flow = model(image1.contiguous(), image2.contiguous(), pred_bidir_flow=pred_bidir_flow, **model_kwargs)["flow_preds"][-1]
-    if resized:                                          # resize back + rescale (u, v) by the size ratios, one launch
+    return _flow_outputs(flow, ori, size, transposed, pred_bidir_flow, fwd_bwd_consistency_check)
+
+
+def _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, name):
+    if fwd_bwd_consistency_check and not pred_bidir_flow:
+        raise ValueError("fwd_bwd_consistency_check needs pred_bidir_flow=True (evaluate_flow.py:774-792)")
+    if model_kwargs.setdefault("task", "flow") != "flow":
+        raise ValueError("%s drives the flow task only" % name)
+
+
+def _flow_outputs(flow, ori, size, transposed, pred_bidir_flow, fwd_bwd_consistency_check):
+    """The model's flow at the inference size -> the driver's outputs at the original size (evaluate_flow.py:750-792)."""
+    if size != ori:                                      # resize back + rescale (u, v) by the size ratios, one launch
         flow = _resize(flow, ori, [ori[1] / size[1], ori[0] / size[0]])
     if transposed:
         flow = flow.transpose(-2, -1)       # axes only -- the reference leaves the (u, v) components in place (evaluate_flow.py:757-758)
@@ -97,6 +111,57 @@ def infer_flow(model, image1, image2, *, padding_factor, inference_size=None, pr
         if fwd_bwd_consistency_check:
             out["fwd_occ"], out["bwd_occ"] = forward_backward_consistency_check(out["flow"], out["flow_bwd"])
     return out
+
+
+def flow_to_image(flow, out=None):
+    """utils/flow_viz.py:240-275 (`flow_to_image`, what the video driver paints, evaluate_flow.py:768) on the device for a
+    batch: planar flow [N,2,H,W] -> uint8 RGB [N,H,W,3], per-image normalisation by the largest radius.  `out` may be a view
+    into larger pictures ([N,H,W,3] with 3-byte pixels and any row / image stride), e.g. the flow half of a frame + flow
+    picture.  One max-reduction pass and one colouring pass."""
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise ValueError("flow_to_image expects planar flows [N,2,H,W]")
+    n, _, h, w = flow.shape
+    if out is None:
+        out = torch.empty((n, h, w, 3), device=flow.device, dtype=torch.uint8)
+    _OPS.flow_to_image(flow.float().contiguous(), out)
+    return out
+
+
+def _frame_geometry(h, w, padding_factor, inference_size):
+    """(transposed, original size as the model sees it, inference size) of a frame sequence (evaluate_flow.py:713-723)."""
+    transposed = h > w
+    ori = (w, h) if transposed else (h, w)
+    return transposed, ori, _inference_size(ori, padding_factor, inference_size)
+
+
+def _frames_to_model(frames, transposed, size):
+    """[T,H,W,3] uint8 (one fused kernel) or [T,3,H,W] float frames -> planar float32 [T,3,*size] model input."""
+    if frames.dtype == torch.uint8:
+        return _OPS.frames_to_planar(frames.contiguous(), int(size[0]), int(size[1]), bool(transposed))
+    if transposed:
+        frames = frames.transpose(-2, -1)
+    return _resize(frames, size) if tuple(frames.shape[-2:]) != tuple(size) else frames.float().contiguous()
+
+
+@torch.no_grad()
+def infer_flow_video(model, frames, *, padding_factor, inference_size=None, pred_bidir_flow=False, pred_bwd_flow=False,
+                     fwd_bwd_consistency_check=False, **model_kwargs):
+    """`inference_flow(..., inference_video=...)` (evaluate_flow.py:686-792) on a device frame sequence: `frames` is
+    uint8 [T,H,W,3] (channel-last, as decoded) or float [T,3,H,W] in [0,255].  Returns what
+    `infer_flow(model, frames[:-1], frames[1:], ...)` returns for the T-1 consecutive pairs, with every frame encoded once
+    (equal up to fp32 summation order, see `UniMatch.encode_frames`).
+    `pred_bwd_flow`: each pair runs in swapped order (evaluate_flow.py:735-736), i.e. the flow from frame t+1 to frame t."""
+    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, "infer_flow_video")
+    if frames.dim() != 4 or frames.shape[0] < 2:
+        raise ValueError("infer_flow_video needs at least two frames [T>=2, H, W, 3] or [T>=2, 3, H, W]")
+    h, w = (frames.shape[1], frames.shape[2]) if frames.dtype == torch.uint8 else (frames.shape[2], frames.shape[3])
+    transposed, ori, size = _frame_geometry(h, w, padding_factor, inference_size)
+    feats = model.encode_frames(_frames_to_model(frames, transposed, size))
+    first, second = [f[:-1] for f in feats], [f[1:] for f in feats]
+    if pred_bwd_flow:
+        first, second = second, first
+    flow = model.forward_encoded(first, second, pred_bidir_flow=pred_bidir_flow, **model_kwargs)["flow_preds"][-1]
+    return _flow_outputs(flow, ori, size, transposed, pred_bidir_flow, fwd_bwd_consistency_check)
 
 
 @torch.no_grad()
@@ -155,7 +220,98 @@ def infer_depth(model, img_ref, img_tgt, intrinsics, pose, *, padding_factor=16,
     return {"depth": depth}
 
 
-class BatchedFlowRunner:
+class _PipelinedRunner:
+    """Two staging slots, host->device copies on a side stream, one CUDA graph per slot, device->host copies behind the step.
+
+    Subclasses provide `_stage_host(slot, chunk)` (fill the slot's pinned buffers and enqueue their H2D copies on the current
+    stream, which is the copy stream), `_reset_inputs(slot)`, `_step(slot)` (the fixed-shape device work -> dict of device
+    tensors), `_download(slot, out)` (enqueue the D2H copies of a step's outputs) and `_results(slot, n)` (the host results)."""
+
+    def _init_pipeline(self, device, use_graph):
+        self.dev = torch.device(device)
+        self.copy_stream = torch.cuda.Stream(device=self.dev)
+        self.graphs = [None, None]
+        self.static_out = [None, None]
+        self.use_graph = use_graph
+
+    def _capture(self):
+        with torch.cuda.device(self.dev):
+            side = torch.cuda.Stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                for _ in range(2):            # eager warm-up: builds the module's cached operand planes outside the capture
+                    for slot in range(2):
+                        self._reset_inputs(slot)
+                        self._step(slot)
+            torch.cuda.current_stream().wait_stream(side)
+            torch.cuda.synchronize()
+            for slot in range(2):
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    self.static_out[slot] = self._step(slot)
+                self.graphs[slot] = g
+            torch.cuda.synchronize()
+
+    def _stage(self, slot, chunk):
+        """host side of one batch, then the H2D copies on the side stream; returns their completion event"""
+        with torch.cuda.stream(self.copy_stream):
+            self._stage_host(slot, chunk)
+            ev = torch.cuda.Event()
+            ev.record(self.copy_stream)
+        return ev
+
+    def _pipeline(self, items, start=None):
+        """Yields the results of `items` taken `self.batch` at a time.  `start()` runs (eagerly, on the main stream) before
+        the first step, after the graphs exist."""
+        if self.use_graph and self.graphs[0] is None:
+            self._capture()
+        it = iter(items)
+
+        def next_chunk():
+            chunk = []
+            for p in it:
+                chunk.append(p)
+                if len(chunk) == self.batch:
+                    break
+            return chunk
+
+        cur = next_chunk()
+        if not cur:
+            return
+        main = torch.cuda.current_stream()
+        if start is not None:
+            start()
+        self.copy_stream.wait_stream(main)
+        ready = self._stage(0, cur)
+        slot = 0
+        done_ev, done_n = None, 0
+        while cur:
+            main.wait_event(ready)
+            if self.use_graph:
+                self.graphs[slot].replay()
+                out = self.static_out[slot]
+            else:
+                out = self._step(slot)
+            fwd_done = torch.cuda.Event()
+            fwd_done.record(main)
+            nxt = next_chunk()
+            if nxt:                                        # stage the next batch while this one computes
+                ready = self._stage(slot ^ 1, nxt)
+            if done_ev is not None:                        # hand out the previous batch's results
+                done_ev.synchronize()
+                yield from self._results(slot ^ 1, done_n)
+            with torch.cuda.stream(self.copy_stream):      # D2H of this batch's results behind its step
+                self.copy_stream.wait_event(fwd_done)
+                self._download(slot, out)
+                done_ev = torch.cuda.Event()
+                done_ev.record(self.copy_stream)
+            done_n = len(cur)
+            cur, slot = nxt, slot ^ 1
+        done_ev.synchronize()
+        yield from self._results(slot ^ 1, done_n)
+
+
+class BatchedFlowRunner(_PipelinedRunner):
     """Fixed-bucket, double-buffered, graph-replayed flow inference for a stream of host frame pairs.
 
     * bucket: every pair is replicate-padded (`InputPadder`, mode 'sintel') from `frame_size` up to a multiple of
@@ -170,7 +326,8 @@ class BatchedFlowRunner:
     (CPU, pinned staging reused -- copy them if you keep them)."""
 
     def __init__(self, model, frame_size, batch, device, padding_factor=32, use_graph=True, **model_kwargs):
-        self.model, self.kw, self.batch, self.dev = model, dict(model_kwargs), int(batch), torch.device(device)
+        self.model, self.kw, self.batch = model, dict(model_kwargs), int(batch)
+        self._init_pipeline(device, use_graph)
         self.kw.setdefault("task", "flow")
         self.padder = InputPadder(frame_size, mode="sintel", padding_factor=padding_factor)
         h, w = frame_size
@@ -180,92 +337,138 @@ class BatchedFlowRunner:
         self.pin = [[torch.empty(shape).pin_memory() for _ in range(2)] for _ in range(2)]       # [slot][view]
         self.dev_in = [[torch.empty(shape, device=self.dev) for _ in range(2)] for _ in range(2)]
         self.out_pin = [torch.empty((self.batch, 2, self.hp, self.wp)).pin_memory() for _ in range(2)]
-        self.copy_stream = torch.cuda.Stream(device=self.dev)
-        self.graphs = [None, None]
-        self.static_out = [None, None]
-        self.use_graph = use_graph
 
-    def _forward(self, slot):
+    def _step(self, slot):
         a, b = self.dev_in[slot]
         return self.model(a, b, **self.kw)["flow_preds"][-1]
 
-    def _capture(self):
-        with torch.cuda.device(self.dev):
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                for _ in range(2):
-                    for slot in range(2):
-                        self.dev_in[slot][0].zero_(); self.dev_in[slot][1].zero_()
-                        self._forward(slot)
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            for slot in range(2):
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self.static_out[slot] = self._forward(slot)
-                self.graphs[slot] = g
-            torch.cuda.synchronize()
+    _forward = _step
 
-    def _stage(self, slot, chunk):
-        """host side of one batch: pad into the pinned buffers, then enqueue the H2D copy on the side stream"""
+    def _reset_inputs(self, slot):
+        self.dev_in[slot][0].zero_(); self.dev_in[slot][1].zero_()
+
+    def _stage_host(self, slot, chunk):
+        """pad into the pinned buffers, then enqueue the H2D copies"""
         for i in range(self.batch):
             img1, img2 = chunk[min(i, len(chunk) - 1)]
             p1, p2 = self.padder.pad(img1[None].float(), img2[None].float())
             self.pin[slot][0][i].copy_(p1[0]); self.pin[slot][1][i].copy_(p2[0])
-        with torch.cuda.stream(self.copy_stream):
-            for v in range(2):
-                self.dev_in[slot][v].copy_(self.pin[slot][v], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self.copy_stream)
-        return ev
+        for v in range(2):
+            self.dev_in[slot][v].copy_(self.pin[slot][v], non_blocking=True)
+
+    def _download(self, slot, flow):
+        self.out_pin[slot].copy_(flow, non_blocking=True)
+
+    def _results(self, slot, n):
+        for i in range(n):
+            yield self.padder.unpad(self.out_pin[slot][i])
 
     @torch.no_grad()
     def run(self, pairs):
         with torch.cuda.device(self.dev):
-            if self.use_graph and self.graphs[0] is None:
-                self._capture()
-            it = iter(pairs)
+            yield from self._pipeline(pairs)
 
-            def next_chunk():
-                chunk = []
-                for p in it:
-                    chunk.append(p)
-                    if len(chunk) == self.batch:
-                        break
-                return chunk
 
-            cur = next_chunk()
-            if not cur:
+class VideoFlowRunner(_PipelinedRunner):
+    """Streaming optical flow over a video: consecutive pairs of host uint8 frames, every frame uploaded and encoded once.
+
+    * upload: each step copies `batch` NEW frames, uint8 [H,W,3] as decoded, through pinned double buffers on a side stream
+      (1.2 MB per 480x832 frame, against 9.6 MB for the two float32 images of a pair);
+    * device work of a step (one CUDA graph per staging slot): `um_frames_to_planar` (uint8 -> float planes, portrait
+      transpose and resize to the inference size in one pass), the encoder on the new frames, the matching path on the
+      `batch` pairs (previous step's last frame, new frames), the flow resized back; the last frame's pyramid is carried into
+      the next step, so nothing is encoded twice.  A short last step is filled with repeats of its last frame and the extra
+      results are dropped;
+    * download: the flow (and flow_bwd / fwd_occ / bwd_occ when asked) and, with `visualize`, the uint8 Middlebury picture
+      (`flow_to_image`; with `concat_frame` the frame and its picture side by side, stacked as the reference's
+      `concat_flow_img` does, evaluate_flow.py:818-825).  `return_flow=False` with `visualize` sends back only the picture.
+
+    Sizes, transpose and rescale semantics are those of `infer_flow_video` (and `infer_flow`); the flows equal
+    `infer_flow_video` on the whole sequence up to fp32 summation order.  `run(frames)` takes an iterable of host uint8 frames [H,W,3] (numpy arrays or
+    tensors) and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy what you keep)."""
+
+    def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
+                 visualize=False, concat_frame=False, pred_bidir_flow=False, fwd_bwd_consistency_check=False,
+                 return_flow=True, **model_kwargs):
+        self.model, self.kw, self.batch = model, dict(model_kwargs), int(batch)
+        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "VideoFlowRunner")
+        if concat_frame and not visualize:
+            raise ValueError("concat_frame needs visualize=True")
+        if not return_flow and not visualize:
+            raise ValueError("nothing to return: return_flow=False needs visualize=True")
+        self._init_pipeline(device, use_graph)
+        self.h, self.w = int(frame_size[0]), int(frame_size[1])
+        self.transposed, self.ori, self.size = _frame_geometry(self.h, self.w, padding_factor, inference_size)
+        self.bidir, self.check = bool(pred_bidir_flow), bool(fwd_bwd_consistency_check)
+        self.visualize, self.concat, self.return_flow = bool(visualize), bool(concat_frame), bool(return_flow)
+        self.concat_axis = 0 if self.h < self.w else 1                                  # evaluate_flow.py:822
+        shape = (self.batch, self.h, self.w, 3)
+        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.carry_frame = torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev)
+        self.carry = None                                  # last frame's feature pyramid, [1,h,w,128] per scale
+        self.out_pin = [None, None]
+
+    # ---- device side
+    def _encode(self, frames_u8):
+        return self.model.encode_frames(_OPS.frames_to_planar(frames_u8, self.size[0], self.size[1], self.transposed))
+
+    def _step(self, slot):
+        new = self._encode(self.dev_in[slot])
+        first = [torch.cat((c, f[:-1]), dim=0) for c, f in zip(self.carry, new)]
+        flow = self.model.forward_encoded(first, new, pred_bidir_flow=self.bidir, **self.kw)["flow_preds"][-1]
+        out = _flow_outputs(flow, self.ori, self.size, self.transposed, self.bidir, self.check)
+        if self.visualize:
+            b, h, w = self.batch, self.h, self.w
+            if self.concat:
+                pics = torch.empty((b, 2 * h, w, 3) if self.concat_axis == 0 else (b, h, 2 * w, 3), dtype=torch.uint8,
+                                   device=self.dev)
+                frame_half, flow_half = (pics[:, :h], pics[:, h:]) if self.concat_axis == 0 else (pics[:, :, :w], pics[:, :, w:])
+                frame_half.copy_(torch.cat((self.carry_frame, self.dev_in[slot][:-1]), dim=0))   # first frame of each pair
+            else:
+                pics = flow_half = torch.empty((b, h, w, 3), dtype=torch.uint8, device=self.dev)
+            flow_to_image(out["flow"], flow_half)
+            out["vis"] = pics
+            if not self.return_flow:
+                del out["flow"]
+        for c, f in zip(self.carry, new):                # carry the last frame into the next step
+            c.copy_(f[-1:])
+        self.carry_frame.copy_(self.dev_in[slot][-1:])
+        return out
+
+    def _reset_inputs(self, slot):
+        self.dev_in[slot].zero_()
+
+    # ---- host side
+    def _stage_host(self, slot, chunk):
+        for i in range(self.batch):
+            self.pin[slot][i].copy_(torch.as_tensor(chunk[min(i, len(chunk) - 1)]))
+        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
+
+    def _download(self, slot, out):
+        if self.out_pin[slot] is None:
+            self.out_pin[slot] = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in out.items()}
+        for k, v in out.items():
+            self.out_pin[slot][k].copy_(v, non_blocking=True)
+
+    def _results(self, slot, n):
+        for i in range(n):
+            yield {k: v[i] for k, v in self.out_pin[slot].items()}
+
+    def _prime(self, frame):
+        """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
+        f = torch.as_tensor(frame).to(self.dev)[None].contiguous()
+        for c, g in zip(self.carry, self._encode(f)):
+            c.copy_(g)
+        self.carry_frame.copy_(f)
+
+    @torch.no_grad()
+    def run(self, frames):
+        with torch.cuda.device(self.dev):
+            it = iter(frames)
+            first = next(it, None)
+            if first is None:
                 return
-            main = torch.cuda.current_stream()
-            self.copy_stream.wait_stream(main)
-            ready = self._stage(0, cur)
-            slot = 0
-            done_ev, done_n = None, 0
-            while cur:
-                main.wait_event(ready)
-                if self.use_graph:
-                    self.graphs[slot].replay()
-                    flow = self.static_out[slot]
-                else:
-                    flow = self._forward(slot)
-                fwd_done = torch.cuda.Event()
-                fwd_done.record(main)
-                nxt = next_chunk()
-                if nxt:                                        # stage the next batch while this one computes
-                    ready = self._stage(slot ^ 1, nxt)
-                if done_ev is not None:                        # hand out the previous batch's flows
-                    done_ev.synchronize()
-                    for i in range(done_n):
-                        yield self.padder.unpad(self.out_pin[slot ^ 1][i])
-                with torch.cuda.stream(self.copy_stream):      # D2H of this batch's flows behind its forward
-                    self.copy_stream.wait_event(fwd_done)
-                    self.out_pin[slot].copy_(flow, non_blocking=True)
-                    done_ev = torch.cuda.Event()
-                    done_ev.record(self.copy_stream)
-                done_n = len(cur)
-                cur, slot = nxt, slot ^ 1
-            done_ev.synchronize()
-            for i in range(done_n):
-                yield self.padder.unpad(self.out_pin[slot ^ 1][i])
+            if self.carry is None:                       # eager runs: allocate the carried pyramid
+                self.carry = [f.clone() for f in self._encode(torch.as_tensor(first).to(self.dev)[None].contiguous())]
+            yield from self._pipeline(it, start=lambda: self._prime(first))

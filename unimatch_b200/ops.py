@@ -19,6 +19,7 @@ SYMBOLS = [
     "um_window_attention", "um_window_attention_workspace", "um_attention_planes_lp", "um_window_attention_planes", "um_debug_set_dump", "um_softmax_expectation", "um_softmax_expectation_workspace",
     "um_local_corr_softmax", "um_local_corr_volume", "um_flow_warp", "um_fb_consistency", "um_propagate_local", "um_depth_corr_softmax",
     "um_conv2d_tc", "um_ffn_tc", "um_conv7x7_small", "um_split_planes", "um_instance_norm_scratch_floats", "um_instance_norm_stats", "um_instance_norm_apply", "um_add_position", "um_layernorm_residual", "um_convex_upsample", "um_upsample2x", "um_resize_bilinear", "um_gru_rh", "um_gru_update",
+    "um_frames_to_planar", "um_flow_to_image",
 ]
 
 MASK_NONE, MASK_SWIN, MASK_CAUSAL = 0, 1, 2
@@ -125,6 +126,10 @@ def _load():
     lib.um_instance_norm_apply.restype = ctypes.c_int
     lib.um_resize_bilinear.argtypes = [P, P, I, I, I, I, I, I, FP, I, P]
     lib.um_resize_bilinear.restype = ctypes.c_int
+    lib.um_frames_to_planar.argtypes = [P, P, I, I, I, I, I, I, P]
+    lib.um_frames_to_planar.restype = ctypes.c_int
+    lib.um_flow_to_image.argtypes = [P, P, L, L, P, I, I, I, P]
+    lib.um_flow_to_image.restype = ctypes.c_int
     lib.um_debug_set_dump.argtypes = [P]
     lib.um_debug_set_dump.restype = None
     for name, argtypes in sig.items():
@@ -418,6 +423,36 @@ def _resize_bilinear(x, h_out, w_out, scale, flip_x):
 
 
 resize_bilinear = _define("resize_bilinear(Tensor x, int h_out, int w_out, float[]? scale, bool flip_x) -> Tensor", _resize_bilinear)
+
+
+def _frames_to_planar(frames, h_out, w_out, transpose):
+    if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3 or not frames.is_contiguous():
+        raise RuntimeError("frames_to_planar: expected contiguous CUDA uint8 frames [T, H, W, 3]")
+    t, h, w, _ = frames.shape
+    out = torch.empty((t, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
+    _check(LIB.um_frames_to_planar(_p(frames), _p(out), t, h, w, int(transpose), h_out, w_out, _stream()), "um_frames_to_planar")
+    return out
+
+
+frames_to_planar = _define("frames_to_planar(Tensor frames, int h_out, int w_out, bool transpose) -> Tensor", _frames_to_planar)
+
+
+def _flow_to_image(flow, out):
+    """flow: planar [N, 2, H, W] fp32; out: uint8 [N, H, W, 3] whose pixels are 3 contiguous bytes -- rows and images may be
+    strided (a view into a larger picture)."""
+    _f32c(flow, "flow")
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise RuntimeError("flow_to_image: expected planar flow [N, 2, H, W]")
+    n, _, h, w = flow.shape
+    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
+            or out.device != flow.device:
+        raise RuntimeError("flow_to_image: out must be uint8 [N, H, W, 3] on the flow's device with 3-byte pixels")
+    scratch = torch.empty((n,), device=flow.device, dtype=torch.float32)
+    _check(LIB.um_flow_to_image(_p(flow), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
+           "um_flow_to_image")
+
+
+flow_to_image = _define("flow_to_image(Tensor flow, Tensor(a!) out) -> ()", _flow_to_image)
 
 
 def _gru_rh(r_pre, h):

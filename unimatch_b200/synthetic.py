@@ -103,6 +103,21 @@ def synthetic_batch(task, batch, h, w, first_index=0, seed=1234):
     return {k: torch.cat([it[k] for it in items], dim=0) for k in items[0]}
 
 
+def synthetic_video(T, h, w, seed=1234, step=3):
+    """T frames uint8 [T,H,W,3] (channel-last, as a decoder returns them) cropped from one box-blurred noise canvas along a
+    seeded path that moves up to `step` px per frame and axis, so consecutive frames have a true match."""
+    g = torch.Generator().manual_seed(seed)
+    m = step * max(T - 1, 0) + 1
+    canvas = _texture(g, h + 2 * m, w + 2 * m)[0].round().clamp(0, 255).to(torch.uint8).permute(1, 2, 0)
+    moves = torch.randint(-step, step + 1, (max(T - 1, 0), 2), generator=g)
+    y = x = m
+    frames = [canvas[y:y + h, x:x + w]]
+    for dy, dx in moves.tolist():
+        y, x = y + dy, x + dx
+        frames.append(canvas[y:y + h, x:x + w])
+    return torch.stack(frames, 0).contiguous()
+
+
 def noise_batch(task, batch, h, w, seed=99):
     """Cheap pure-noise batch for throughput runs (no match structure; same arithmetic)."""
     g = torch.Generator().manual_seed(seed)

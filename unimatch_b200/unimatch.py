@@ -274,7 +274,7 @@ class UniMatch(nn.Module):
         Returns the feature maps low -> high resolution, each [2B, h, w, 128] (first views, then second views)."""
         T = P["tcb"]
         dev = img0.device
-        nb = img0.shape[0] + img1.shape[0]
+        nb = img0.shape[0] + (img1.shape[0] if img1 is not None else 0)
         C, IS, IA = self._conv, _OPS.instance_norm_stats, _OPS.instance_norm_apply
         pad64 = lambda c: (c + 63) // 64 * 64
 
@@ -664,13 +664,52 @@ class UniMatch(nn.Module):
         B = img0.shape[0]
         with self._section("backbone"):                                           # [2B,h,w,128] low -> high res
             feats = self._stage_backbone(P, img0.float().contiguous(), img1.float().contiguous(), task == "flow")
+        return self._forward_encoded(P, [f[:B] for f in feats], [f[B:] for f in feats], attn_type, attn_splits_list,
+                                     corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, intrinsics,
+                                     pose, min_depth, max_depth, num_depth_candidates, depth_from_argmax, pred_bidir_depth)
 
+    # ------------------------------------------------------------------------------------------ video: encode frames once
+    def encode_frames(self, frames):
+        """CNN encoder on a set of frames [T,3,H,W] in [0,255] (flow task: normalize_img folded in).  Returns the feature
+        pyramid low -> high resolution, each [T,h,w,128].  Every encoder kernel works per image (convolutions per pixel,
+        InstanceNorm per image over a fixed chunking), so a frame's features do not depend on its partner or on the batch and
+        consecutive pairs of a video can share one encoding per frame.  They are equal up to fp32 summation order, not bit
+        for bit: um_conv2d_tc walks the K chunks of an output tile in an order rotated by the index of the CTA that owns the
+        tile (to spread the weight reads over L2), and the tile-to-CTA assignment follows the launch's tile count, so the
+        same frame in a batch of a different size can round differently in the last bits."""
+        if self.training:
+            raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
+        with torch.no_grad():
+            P = self._prepared()
+            with self._section("backbone"):
+                return self._stage_backbone(P, frames.float().contiguous(), None, True)
+
+    def forward_encoded(self, feats0, feats1, attn_type=None, attn_splits_list=None, corr_radius_list=None,
+                        prop_radius_list=None, num_reg_refine=1, pred_bidir_flow=False, task="flow", **kwargs):
+        """Everything of `forward` after the encoder, on per-scale features of the first and second views ([B,h,w,128] each,
+        low -> high resolution, e.g. slices `f[:-1]`, `f[1:]` of `encode_frames`).  Flow task; returns {'flow_preds': [...]}
+        exactly as `forward` does for the images those features were encoded from."""
+        if self.training:
+            raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
+        if task != "flow":
+            raise ValueError("forward_encoded drives the flow task only (stereo / depth encode both views per pair)")
+        if len(feats0) != self.num_scales or len(feats1) != self.num_scales:
+            raise ValueError("forward_encoded needs one feature map per scale (%d)" % self.num_scales)
+        assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
+        with torch.no_grad():
+            return self._forward_encoded(self._prepared(), list(feats0), list(feats1), attn_type, attn_splits_list,
+                                         corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, "flow", None,
+                                         None, None, None, None, False, False)
+
+    def _forward_encoded(self, P, feats0, feats1, attn_type, attn_splits_list, corr_radius_list, prop_radius_list,
+                         num_reg_refine, pred_bidir_flow, task, intrinsics, pose, min_depth, max_depth, num_depth_candidates,
+                         depth_from_argmax, pred_bidir_depth):
+        """The matching path after the encoder (unimatch.py:127-367); feats0 / feats1: per-scale [B,h,w,128] views."""
         flow = None            # [Bp, h, w, fd] channel-last
         preds = []
         for s in range(self.num_scales):
-            f = feats[s]
-            _, h, wd, c = f.shape
-            f0, f1 = f[:B], f[B:]
+            f0, f1 = feats0[s], feats1[s]
+            _, h, wd, c = f0.shape
             if pred_bidir_flow and s > 0:                                         # unimatch.py:139-141
                 f0, f1 = torch.cat((f0, f1), dim=0), torch.cat((f1, f0), dim=0)
             f0_ori, f1_ori = f0, f1
