@@ -7,12 +7,14 @@
 //   im2col is nothing but shifted box coordinates, and the zero padding of the convolution is TMA's out-of-bounds
 //   fill.  Up to two input tensors are summed in the same accumulator, so torch.cat([h, x]) of the GRU never exists.
 // * Weights are prepared once as [2][Cout_p][Ktot] fp16 planes, K ordered (src, tap, ci).
-// * Persistent CTAs (one per SM) loop over tiles of 128 output pixels (16 x 8) x BN output channels (BN = 16 ... 128);
-//   warp 0 = TMA producer (2-3 stage mbarrier ring that keeps running across tiles), warpgroups 1 and 2 = consumers:
-//   each runs the MMAs of 64 of the tile's pixels (3 split terms x 4 K-steps of wgmma 64xBNx16 per stage) into register
-//   accumulators, then both hand the tile through shared memory to the epilogue (thread = pixel, two groups interleaved
-//   over the 32-channel chunks): bias, activation, fused GRU gate math or LayerNorm(+residual), fp32 and/or fp16-split
-//   channel-last bulk-tensor stores at a channel offset of a wider buffer (free concatenation).
+// * Persistent CTAs (one per SM) loop over tiles of 128 output pixels (16 x 8) x BN output channels (BN = 16 ... 128),
+//   warp-specialised: one TMA producer warp (2-3 stage mbarrier ring that keeps running across tiles); two MMA
+//   warpgroups, each running the MMAs of 64 of the tile's pixels (3 split terms x 4 K-steps of wgmma 64xBNx16 per stage)
+//   into register accumulators, which they hand to the epilogue through a shared-memory tile (acc_full / acc_empty
+//   mbarriers) before going on with the next tile's K loop; one epilogue warpgroup (thread = pixel): bias, activation,
+//   fused GRU gate math or LayerNorm(+residual), fp32 and/or fp16-split channel-last bulk-tensor stores at a channel
+//   offset of a wider buffer (free concatenation).  The epilogue of tile i thus runs under the MMAs of tile i + 1, and
+//   neither role's registers count against the other's.
 //
 // Replaces the fp32 convolutions of BasicUpdateBlock (reg_refine.py:6-119), refine_proj (unimatch.py:315), the CNN
 // encoder (backbone.py:49-86) and the transformer's Linear layers (1x1 "convolution" over a [rows/16, 16] pixel grid).
@@ -30,9 +32,15 @@ namespace {
 constexpr int TW = 16, TH = 8;                 // spatial tile = 128 pixels
 // operand ring depth: three stages, or two for the widest tiles (BN >= 96: 56-64 KB a stage next to their accumulator tile)
 __host__ __device__ constexpr int stages_for(int bn) { return bn >= 96 ? 2 : 3; }
-// 2 consumer warpgroups (warps 0-7) + one TMA producer warp (warp 8)
-constexpr int NTHREADS = 288;
-constexpr int PRODUCER = 8;
+// 2 MMA warpgroups (warps 0-7) + one epilogue warpgroup (warps 8-11) + the TMA producer's warpgroup (warp 12 works,
+// warps 13-15 leave at once)
+constexpr int NTHREADS = 512;
+constexpr int EPILOGUE = 8;
+constexpr int PRODUCER = 12;
+// per-thread registers of each role (setmaxnreg): 32 + 2 x 168 + 144 = 512 over the four warpgroups = the 64 K register
+// file.  The MMA warpgroups hold acc and part (BN = 128, G > 1: 128 registers), the epilogue up to three 32-float
+// arrays; the producer loop does not fit in 24.
+constexpr int REGS_PRODUCER = 32, REGS_MMA = 168, REGS_EPI = 144;
 constexpr uint32_t A_BYTES = 2 * 16384;        // hi + lo, [128 x 64] fp16 each
 constexpr uint32_t STAGING_UNIT = 16384;       // one epilogue staging buffer: [128 rows x 32 floats]
 constexpr uint32_t STAGING_BYTES = 2 * STAGING_UNIT;
@@ -95,7 +103,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
                const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_of,
                const __grid_constant__ CUtensorMap map_os, ConvParams p) {
   static_assert(BN == 16 || BN == 64 || BN == 96 || BN == 128, "tile widths 16, 64, 96, 128");
-  constexpr int NSB = 1;                                   // staging buffers per epilogue group
+  constexpr int NSB = 2;                                   // staging buffers of the epilogue's bulk-store ring
   constexpr uint32_t B_BYTES = 2 * BN * 128;               // hi + lo, [BN x 64] fp16 each
   constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
   constexpr int STAGES = stages_for(BN);
@@ -106,21 +114,26 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + ACC_BYTES + STAGING_BYTES);
   uint64_t* full = bars;                  // [STAGES]
   uint64_t* empty = bars + STAGES;        // [STAGES]
+  uint64_t* acc_full = bars + 2 * STAGES; // the tile's accumulators are in accs (one arrival per MMA thread)
+  uint64_t* acc_empty = acc_full + 1;     // the epilogue has read accs (one arrival per epilogue thread)
   float* coef = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);
   const int mode = MODE >= 0 ? MODE : p.mode;
   const int act = ACT >= 0 ? ACT : p.act;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int taps = p.KH * p.KW;
-  int nk = 0;
-  for (int s = 0; s < p.nsrc; ++s) nk += taps * (p.cin_p[s] >> 6);
-
-  // work distribution: CTA `cid` of `ncid` walks the tiles cid, cid + ncid, ...
-  const int cid = (int)blockIdx.x;
-  const int ncid = (int)gridDim.x;
+  // Work distribution: CTA `cid` of `ncid` walks the tiles cid, cid + ncid, ...  These and the number of K stages (64
+  // input channels each) are formed by each role after its setmaxnreg: ptxas keeps a value that is live across that
+  // instruction in local memory.
+  auto k_stages = [&]() {
+    int n = 0;
+    for (int s = 0; s < p.nsrc; ++s) n += p.KH * p.KW * (p.cin_p[s] >> 6);
+    return n;
+  };
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 8); }   // empty: one arrival per consumer warp
+    for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 8); }   // empty: one arrival per MMA warp
+    mbar_init(acc_full, 256);
+    mbar_init(acc_empty, 128);
     fence_barrier_init();
   }
   if (warp == PRODUCER && lane == 0) {
@@ -129,9 +142,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
   }
   __syncthreads();
 
-  // The producer warp runs CONVERGED (all 32 lanes execute the loops, one elected lane issues the TMA instructions):
-  // addresses are then provably warp-uniform and live in uniform registers.
-  if (warp == PRODUCER) {
+  if (warp >= PRODUCER) {
+    setmaxnreg_dec<REGS_PRODUCER>();
+    if (warp != PRODUCER) return;
+    const int cid = (int)blockIdx.x, ncid = (int)gridDim.x;
+    const int taps = p.KH * p.KW;
+    const int nk = k_stages();
+    // The producer warp runs CONVERGED (all 32 lanes execute the loops, one elected lane issues the TMA instructions):
+    // addresses are then provably warp-uniform and live in uniform registers.
     int it = 0;
     for (int t = cid; t < p.ntiles; t += ncid) {
       const int n0 = (t % p.tiles_n) * BN;
@@ -168,27 +186,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         __syncwarp();
       }
     }
-  } else {
-    // ---- consumers.  MMA: warpgroup grp computes pixels [64 grp, 64 grp + 64) of the tile.
-    //      Epilogue: 8 warps = 2 groups x 4 row quarters; thread = output pixel (accumulator row).  Group g owns
-    //      the 32-channel chunks g, g+2, ... of the tile: two warps per scheduler hide each other's shared / global /
-    //      MUFU latencies, and the per-chunk math (GELU, gates, LayerNorm) is spread over twice the issue slots.
-    //      Results are staged in shared memory in TMA box layout (16 KB per group) and ONE thread per group issues
-    //      bulk tensor stores, which overlap the MMAs of the next tile. ----
+  } else if (warp < EPILOGUE) {
+    // ---- MMA warpgroups: warpgroup grp computes pixels [64 grp, 64 grp + 64) of the tile, hands the accumulators to
+    //      the epilogue through accs and goes on with the next tile's K loop ----
+    setmaxnreg_inc<REGS_MMA>();
+    const int cid = (int)blockIdx.x, ncid = (int)gridDim.x;
+    const int nk = k_stages();
     const int quarter = warp & 3;
     const int grp = warp >> 2;
-    const int r = quarter * 32 + lane;
-    const int eg = (warp & 3) * 32 + lane;           // 0..127 inside the group
     const int frow = grp * 64 + quarter * 16 + (lane >> 2); // first accumulator row of this thread's MMA fragment (+ 8)
     const int fcol = 2 * (lane & 3);
-    const bool leader = eg == 0;
-    int sctr = 0;                                          // staging passes issued by this group (buffer ring position)
-    auto group_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(1 + grp) : "memory"); };
-    auto all_sync = [&]() { asm volatile("bar.sync 3, 256;" ::: "memory"); };
-    if (mode == UM_CONV_LN && grp == 0) { coef[256 + eg] = __ldg(p.gamma + eg); coef[384 + eg] = __ldg(p.beta + eg); }
     int lt = 0, it = 0;
     for (int t = cid; t < p.ntiles; t += ncid, ++lt) {
-      // ---- MMAs of this warpgroup's 64 rows ----
       float acc[BN / 2], part[BN / 2];
       for (int k = 0; k < nk; ++k, ++it) {
         const int st = it % STAGES;
@@ -217,8 +226,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           for (int i = 0; i < BN / 2; ++i) acc[i] = k ? acc[i] + part[i] : part[i];
         }
       }
-      // ---- accumulator tile -> shared memory (the previous tile's epilogue has finished reading it) ----
-      all_sync();
+      mbar_wait_inline(acc_empty, (lt & 1) ^ 1);               // the previous tile's epilogue has read accs
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int col = 8 * j + fcol;
@@ -230,8 +238,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
               make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
-      all_sync();
-
+      mbar_arrive(acc_full);
+    }
+  } else {
+    // ---- epilogue warpgroup: thread = output pixel (accumulator row), walking the tile's 32-channel chunks.  Results
+    //      are staged in shared memory in TMA box layout (a ring of two 16 KB buffers) and ONE thread issues bulk tensor
+    //      stores, which overlap the next chunk's math. ----
+    setmaxnreg_inc<REGS_EPI>();
+    const int cid = (int)blockIdx.x, ncid = (int)gridDim.x;
+    const int r = threadIdx.x - EPILOGUE * 32;
+    const bool leader = r == 0;
+    int sctr = 0;                                          // staging passes issued (buffer ring position)
+    auto epi_sync = [&]() { asm volatile("bar.sync 1, 128;" ::: "memory"); };
+    if (mode == UM_CONV_LN) { coef[256 + r] = __ldg(p.gamma + r); coef[384 + r] = __ldg(p.beta + r); }
+    epi_sync();
+    int lt = 0;
+    for (int t = cid; t < p.ntiles; t += ncid, ++lt) {
       const int n0 = (t % p.tiles_n) * BN;
       int tile = t / p.tiles_n;
       const int x0 = (tile % p.tiles_x) * TW; tile /= p.tiles_x;
@@ -240,15 +262,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
       const long long pix_r = ((long long)b * p.H + (y0 + (r >> 4))) * p.W + x0 + (r & 15);
       const bool valid_r = (y0 + (r >> 4) < p.H) && (x0 + (r & 15) < p.W);
 
-      // One 32-channel chunk of the tile -> global memory.  The group's staging buffer was last read by the bulk store
-      // this group issued for its previous chunk: that read must be over before anybody overwrites it (checking only
-      // after the writes, as an earlier version did, let fast epilogues corrupt rows the TMA unit was still reading).
+      // One 32-channel chunk of the tile -> global memory.  A staging buffer was last read by the bulk store issued two
+      // passes earlier: that read must be over before anybody overwrites it (checking only after the writes, as an
+      // earlier version did, let fast epilogues corrupt rows the TMA unit was still reading).
       auto emit = [&](const float (&v)[32], int co_out, bool to_f32, bool to_split, bool to_win = false) {
         if (WIN && to_win) {                                 // hi then lo rows staged like to_split, scattered row by row
-          uint8_t* sbs = reinterpret_cast<uint8_t*>(stage_buf + (grp * NSB + sctr % NSB) * 4096);
+          uint8_t* sbs = reinterpret_cast<uint8_t*>(stage_buf + (sctr % NSB) * 4096);
           ++sctr;
-          if (leader) bulk_wait_read<NSB - 1>();             // the ring is shared with the bulk-store paths
-          group_sync();
+          if (leader) bulk_wait_read<0>();                   // this pass commits no bulk group: drain the ring
+          epi_sync();
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint32_t hw[4], lw[4];
@@ -258,14 +280,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
             *reinterpret_cast<uint4*>(sbs + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
             *reinterpret_cast<uint4*>(sbs + 8192 + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
           }
-          group_sync();
+          epi_sync();
           const int wc = co_out - p.win_c0;                  // channel inside the window-plane range
           __half* obase = p.win_dst + (long long)(wc >> 7) * 2 * p.win_plane + (wc & 127);
           const int* rowdst = reinterpret_cast<const int*>(coef + 256) + (lt & 1) * 128;
-          const int piece = eg & 3;
+          const int piece = r & 3;
 #pragma unroll
           for (int itr = 0; itr < 4; ++itr) {
-            const int row = itr * 32 + (eg >> 2);
+            const int row = itr * 32 + (r >> 2);
             const int drow = rowdst[row];
             if (drow < 0) continue;
             const int soff = row * 64 + ((piece ^ ((row >> 1) & 3)) << 4);
@@ -278,22 +300,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           return;
         }
         if (to_f32) {                                        // [128 rows][32 floats], 128B swizzle
-          float* my_stage = stage_buf + (grp * NSB + sctr % NSB) * 4096;
+          float* my_stage = stage_buf + (sctr % NSB) * 4096;
           ++sctr;
           if (leader) bulk_wait_read<NSB - 1>();
-          group_sync();
+          epi_sync();
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             *reinterpret_cast<float4*>(my_stage + r * 32 + ((i ^ (r & 7)) << 2)) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
           fence_proxy_async();
-          group_sync();
+          epi_sync();
           if (leader) { tma_store_4d(&map_of, my_stage, co_out, x0, y0, b); bulk_commit(); }
         }
         if (to_split) {                                      // hi then lo: [128 rows][32 halves], 64-byte rows, 64B swizzle
-          uint8_t* sbs = reinterpret_cast<uint8_t*>(stage_buf + (grp * NSB + sctr % NSB) * 4096);
+          uint8_t* sbs = reinterpret_cast<uint8_t*>(stage_buf + (sctr % NSB) * 4096);
           ++sctr;
           if (leader) bulk_wait_read<NSB - 1>();
-          group_sync();
+          epi_sync();
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             uint32_t hw[4], lw[4];
@@ -304,7 +326,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
             *reinterpret_cast<uint4*>(sbs + 8192 + off) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
           }
           fence_proxy_async();
-          group_sync();
+          epi_sync();
           if (leader) {
             tma_store_4d(&map_os, sbs, co_out, x0, y0, b);
             tma_store_4d(&map_os, sbs + 8192, co_out, x0, y0, p.B + b);
@@ -315,94 +337,96 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
 
       if constexpr (BN == 128) {
         if (mode == UM_CONV_LN) {
-          // LayerNorm over the 128 channels of the row (+ residual): each group keeps its 64 channels in registers;
-          // row sums are exchanged through shared memory (mean first, then the centred sum of squares: two-pass
-          // statistics like the reference's, not E[x^2] - mean^2)
-          const int ca = grp * 32, cb = 64 + grp * 32;
-          float a0[32], a1[32];
+          // LayerNorm over the 128 channels of the row (+ residual), two-pass statistics like the reference's (mean first,
+          // then the centred sum of squares, not E[x^2] - mean^2).  Each statistic is the sum of two partial sums, over
+          // channels {0-31, 64-95} and {32-63, 96-127}, each accumulated in that channel order: the rounding the kernel
+          // has always had.  The row is re-read from accs for every pass instead of being held in registers.
+          mbar_wait_inline(acc_full, lt & 1);
+          float sum0 = 0.f, sum1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+#pragma unroll 1
+          for (int h = 0; h < 2; ++h) {
+            float v0[32], v1[32];
+            load_acc32(accs, r, 32 * h, v0);
+            load_acc32(accs, r, 64 + 32 * h, v1);
+            float sum = 0.f;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) sum += v0[i];
+#pragma unroll
+            for (int i = 0; i < 32; ++i) sum += v1[i];
+            if (h == 0) sum0 = sum; else sum1 = sum;
+          }
+          const float mean = (sum0 + sum1) * (1.0f / 128.0f);
+#pragma unroll 1
+          for (int h = 0; h < 2; ++h) {
+            float v0[32], v1[32];
+            load_acc32(accs, r, 32 * h, v0);
+            load_acc32(accs, r, 64 + 32 * h, v1);
+            float sq = 0.f;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { const float dd = v0[i] - mean; sq = fmaf(dd, dd, sq); }
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { const float dd = v1[i] - mean; sq = fmaf(dd, dd, sq); }
+            if (h == 0) sq0 = sq; else sq1 = sq;
+          }
+          const float rstd = rsqrtf((sq0 + sq1) * (1.0f / 128.0f) + 1e-5f);
           const bool need_a = valid_r && p.aux0;
-          if (need_a) {                                      // residual: fetched while the MMAs of this tile still run
-            const float4* pa = reinterpret_cast<const float4*>(p.aux0 + pix_r * p.ld_aux0 + ca);
-            const float4* pb = reinterpret_cast<const float4*>(p.aux0 + pix_r * p.ld_aux0 + cb);
+#pragma unroll 1
+          for (int c0 = 0; c0 < 128; c0 += 32) {
+            float a[32];
+            if (need_a) {                                    // residual
+              const float4* pa = reinterpret_cast<const float4*>(p.aux0 + pix_r * p.ld_aux0 + c0);
+#pragma unroll
+              for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(pa + i); a[4 * i] = t4.x; a[4 * i + 1] = t4.y; a[4 * i + 2] = t4.z; a[4 * i + 3] = t4.w; }
+            }
+            float v[32];
+            load_acc32(accs, r, c0, v);
+            if (c0 == 96) mbar_arrive(acc_empty);            // the tile's last read of accs
+            const float4* g4 = reinterpret_cast<const float4*>(coef + 256 + c0);
+            const float4* b4 = reinterpret_cast<const float4*>(coef + 384 + c0);
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-              const float4 t4 = __ldg(pa + i), u4 = __ldg(pb + i);
-              a0[4 * i] = t4.x; a0[4 * i + 1] = t4.y; a0[4 * i + 2] = t4.z; a0[4 * i + 3] = t4.w;
-              a1[4 * i] = u4.x; a1[4 * i + 1] = u4.y; a1[4 * i + 2] = u4.z; a1[4 * i + 3] = u4.w;
+              const float4 g = g4[i], bb = b4[i];
+              v[4 * i] = (v[4 * i] - mean) * rstd * g.x + bb.x;
+              v[4 * i + 1] = (v[4 * i + 1] - mean) * rstd * g.y + bb.y;
+              v[4 * i + 2] = (v[4 * i + 2] - mean) * rstd * g.z + bb.z;
+              v[4 * i + 3] = (v[4 * i + 3] - mean) * rstd * g.w + bb.w;
             }
+            if (need_a) {
+#pragma unroll
+              for (int i = 0; i < 32; ++i) v[i] += a[i];
+            }
+            emit(v, c0, p.out_f32 != nullptr, p.out_split != nullptr);
           }
-          float v0[32], v1[32];
-          load_acc32(accs, r, ca, v0);
-          load_acc32(accs, r, cb, v1);
-          float* xs = coef;                                  // [2 groups][128 rows] (LN has no bias: the slots are free)
-          float sum = 0.f;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) sum += v0[i];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) sum += v1[i];
-          xs[grp * 128 + r] = sum;
-          all_sync();
-          const float mean = (xs[r] + xs[128 + r]) * (1.0f / 128.0f);
-          all_sync();
-          float sq = 0.f;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) { const float dd = v0[i] - mean; sq = fmaf(dd, dd, sq); }
-#pragma unroll
-          for (int i = 0; i < 32; ++i) { const float dd = v1[i] - mean; sq = fmaf(dd, dd, sq); }
-          xs[grp * 128 + r] = sq;
-          all_sync();
-          const float rstd = rsqrtf((xs[r] + xs[128 + r]) * (1.0f / 128.0f) + 1e-5f);
-          const float4* g4a = reinterpret_cast<const float4*>(coef + 256 + ca);
-          const float4* b4a = reinterpret_cast<const float4*>(coef + 384 + ca);
-          const float4* g4b = reinterpret_cast<const float4*>(coef + 256 + cb);
-          const float4* b4b = reinterpret_cast<const float4*>(coef + 384 + cb);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 ga = g4a[i], ba = b4a[i], gb = g4b[i], bb = b4b[i];
-            v0[4 * i] = (v0[4 * i] - mean) * rstd * ga.x + ba.x;             v1[4 * i] = (v1[4 * i] - mean) * rstd * gb.x + bb.x;
-            v0[4 * i + 1] = (v0[4 * i + 1] - mean) * rstd * ga.y + ba.y;     v1[4 * i + 1] = (v1[4 * i + 1] - mean) * rstd * gb.y + bb.y;
-            v0[4 * i + 2] = (v0[4 * i + 2] - mean) * rstd * ga.z + ba.z;     v1[4 * i + 2] = (v1[4 * i + 2] - mean) * rstd * gb.z + bb.z;
-            v0[4 * i + 3] = (v0[4 * i + 3] - mean) * rstd * ga.w + ba.w;     v1[4 * i + 3] = (v1[4 * i + 3] - mean) * rstd * gb.w + bb.w;
-          }
-          if (need_a) {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) { v0[i] += a0[i]; v1[i] += a1[i]; }
-          }
-          emit(v0, ca, p.out_f32 != nullptr, p.out_split != nullptr);
-          emit(v1, cb, p.out_f32 != nullptr, p.out_split != nullptr);
           continue;
         }
       }
 
       // bias slice of this tile -> shared memory (read back as broadcast float4; double-buffered by tile parity)
       float* sbias = coef + (lt & 1) * 128;
-      if (grp == 0) {
-        for (int i = eg; i < BN; i += 128) sbias[i] = (p.bias && n0 + i < p.cout) ? __ldg(p.bias + n0 + i) : 0.f;
-        if (WIN) {                                           // destination row of every token of this tile (eg = row)
-          const int yy = y0 + (eg >> 4), xx = x0 + (eg & 15);
-          const long long token = ((long long)b * p.H + yy) * p.W + xx;
-          int drow = -1;
-          if (yy < p.H && xx < p.W && token < p.win_tokens) {
-            const Geom& g = p.win_g;
-            const int n = (int)(token / p.win_L);
-            const int t = (int)(token - (long long)n * p.win_L);
-            const int ty = t / g.w, tx = t - ty * g.w;
-            int yr = ty - g.sh; if (yr < 0) yr += g.h;       // rolled[yr, xr] = orig[(yr + sh) % h, (xr + sw) % w]
-            int xr = tx - g.sw; if (xr < 0) xr += g.w;
-            const int wy = yr / g.wh, wx = xr / g.ww;
-            drow = (n * g.nwin + wy * g.kw + wx) * p.win_lp + (yr - wy * g.wh) * g.ww + (xr - wx * g.ww);
-          }
-          reinterpret_cast<int*>(coef + 256)[(lt & 1) * 128 + eg] = drow;
+      if (r < BN) sbias[r] = (p.bias && n0 + r < p.cout) ? __ldg(p.bias + n0 + r) : 0.f;
+      if (WIN) {                                             // destination row of every token of this tile (r = row)
+        const int yy = y0 + (r >> 4), xx = x0 + (r & 15);
+        const long long token = ((long long)b * p.H + yy) * p.W + xx;
+        int drow = -1;
+        if (yy < p.H && xx < p.W && token < p.win_tokens) {
+          const Geom& g = p.win_g;
+          const int n = (int)(token / p.win_L);
+          const int t = (int)(token - (long long)n * p.win_L);
+          const int ty = t / g.w, tx = t - ty * g.w;
+          int yr = ty - g.sh; if (yr < 0) yr += g.h;         // rolled[yr, xr] = orig[(yr + sh) % h, (xr + sw) % w]
+          int xr = tx - g.sw; if (xr < 0) xr += g.w;
+          const int wy = yr / g.wh, wx = xr / g.ww;
+          drow = (n * g.nwin + wy * g.kw + wx) * p.win_lp + (yr - wy * g.wh) * g.ww + (xr - wx * g.ww);
         }
+        reinterpret_cast<int*>(coef + 256)[(lt & 1) * 128 + r] = drow;
       }
-      all_sync();
-      if (grp * 32 >= BN) continue;                          // narrow tiles: the second group has no chunk
+      epi_sync();
 
       constexpr int CH = BN < 32 ? BN : 32;
 #pragma unroll 1
-      for (int c0 = grp * 32; c0 < BN; c0 += 64) {
+      for (int c0 = 0; c0 < BN; c0 += 32) {
         const int co0 = n0 + c0;
-        const bool live = co0 < p.cout;                      // group-uniform
+        const bool live = co0 < p.cout;                      // warpgroup-uniform
         bool to_f32 = p.out_f32 != nullptr, to_split = p.out_split != nullptr;
         int co_out = co0;
         if (mode == UM_CONV_GRU_ZR) {                        // z -> fp32, r*h -> split planes
@@ -411,20 +435,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         }
         bool to_win = false;
         if (WIN && co0 >= p.win_c0 && co0 < p.win_c1) { to_win = true; to_f32 = to_split = false; }
-        // operands of the fused gate math that do not depend on the accumulator: fetch them first
-        float ax[32], bx[32];
-        const bool need_a = live && valid_r && p.aux0 && (mode == UM_CONV_GRU_Q || (mode == UM_CONV_GRU_ZR && co0 >= 128));
-        const bool need_b = live && valid_r && mode == UM_CONV_GRU_Q;
-        if (need_a) {
-          const float4* ap = reinterpret_cast<const float4*>(p.aux0 + pix_r * p.ld_aux0 + (mode == UM_CONV_GRU_ZR ? co0 - 128 : co0));
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(ap + i); ax[4 * i] = t4.x; ax[4 * i + 1] = t4.y; ax[4 * i + 2] = t4.z; ax[4 * i + 3] = t4.w; }
-        }
-        if (need_b) {
-          const float4* bp = reinterpret_cast<const float4*>(p.aux1 + pix_r * p.ld_aux1 + co0);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(bp + i); bx[4 * i] = t4.x; bx[4 * i + 1] = t4.y; bx[4 * i + 2] = t4.z; bx[4 * i + 3] = t4.w; }
-        }
+        // the pre-accumulated part does not depend on the accumulator: fetched before waiting for it
         float px[32];
         const bool need_p = live && valid_r && p.pre;        // loop-invariant part of the convolution, computed once by the caller
         if (need_p) {
@@ -433,7 +444,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(pp + i); px[4 * i] = t4.x; px[4 * i + 1] = t4.y; px[4 * i + 2] = t4.z; px[4 * i + 3] = t4.w; }
         }
         float v[32];
+        mbar_wait_inline(acc_full, lt & 1);
         load_acc32(accs, r, c0, v);                          // BN = 16: the upper 16 columns are unused
+        if (c0 + 32 >= BN) mbar_arrive(acc_empty);           // the tile's last read of accs
         if (!live) continue;
         // ---- per-pixel math on the thread's own row ----
         if (p.bias) {
@@ -447,6 +460,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         if (need_p) {
 #pragma unroll
           for (int i = 0; i < CH; ++i) v[i] += px[i];
+        }
+        // operands of the fused gate math, fetched once px is consumed: at most three 32-float arrays are live, which
+        // keeps the epilogue inside its register budget
+        float ax[32], bx[32];
+        const bool need_a = valid_r && p.aux0 && (mode == UM_CONV_GRU_Q || (mode == UM_CONV_GRU_ZR && co0 >= 128));
+        const bool need_b = valid_r && mode == UM_CONV_GRU_Q;
+        if (need_a) {
+          const float4* ap = reinterpret_cast<const float4*>(p.aux0 + pix_r * p.ld_aux0 + (mode == UM_CONV_GRU_ZR ? co0 - 128 : co0));
+#pragma unroll
+          for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(ap + i); ax[4 * i] = t4.x; ax[4 * i + 1] = t4.y; ax[4 * i + 2] = t4.z; ax[4 * i + 3] = t4.w; }
+        }
+        if (need_b) {
+          const float4* bp = reinterpret_cast<const float4*>(p.aux1 + pix_r * p.ld_aux1 + co0);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) { const float4 t4 = __ldg(bp + i); bx[4 * i] = t4.x; bx[4 * i + 1] = t4.y; bx[4 * i + 2] = t4.z; bx[4 * i + 3] = t4.w; }
         }
         if (mode == UM_CONV_GRU_ZR) {
 #pragma unroll
@@ -478,16 +506,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
         } else {
           // BN = 16 (flow / disparity heads, 1-2 live channels): plain predicated stores through a staging transpose
           const int nvalid = min(CH, p.cout - co0);
-          float* sb = stage_buf + grp * NSB * 4096;
-          group_sync();                                      // the previous tile's readers are done with the buffer
+          float* sb = stage_buf;
+          epi_sync();                                        // the previous tile's readers are done with the buffer
 #pragma unroll
           for (int i = 0; i < CH / 4; ++i)
             *reinterpret_cast<float4*>(sb + r * 32 + ((i ^ (r & 7)) << 2)) = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          group_sync();
+          epi_sync();
           if (to_f32) {
 #pragma unroll 1
             for (int itr = 0; itr < 8; ++itr) {
-              const int row = itr * 16 + (eg >> 3), piece = eg & 7;
+              const int row = itr * 16 + (r >> 3), piece = r & 7;
               const int yy = y0 + (row >> 4), xx = x0 + (row & 15);
               if (yy >= p.H || xx >= p.W || piece * 4 >= nvalid) continue;
               const float4 val = *reinterpret_cast<const float4*>(sb + row * 32 + ((piece ^ (row & 7)) << 2));
@@ -499,7 +527,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a0, const __grid_constant
           if (to_split) {
 #pragma unroll 1
             for (int itr = 0; itr < 4; ++itr) {
-              const int row = itr * 32 + (eg >> 2), piece = eg & 3;          // piece = 8 channels
+              const int row = itr * 32 + (r >> 2), piece = r & 3;            // piece = 8 channels
               const int yy = y0 + (row >> 4), xx = x0 + (row & 15);
               if (yy >= p.H || xx >= p.W || piece * 8 >= nvalid) continue;
               const float4 a4 = *reinterpret_cast<const float4*>(sb + row * 32 + (((2 * piece) ^ (row & 7)) << 2));

@@ -114,6 +114,12 @@ __device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr, uint32_t mn_gro
   return smem_desc_sw128(saddr, mn_group_stride, 1024);
 }
 
+// per-warpgroup register budget of a warp-specialised kernel (executed by all warps of the warpgroup)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
