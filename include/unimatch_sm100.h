@@ -192,6 +192,16 @@ int um_resize_bilinear(const float* in, float* out, int32_t batch, int32_t chann
 int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t transpose,
                         int32_t h_out, int32_t w_out, void* stream);
 
+/* Depth-sequence frames to model input: frames = DEVICE uint8 [n, h, w, 3] channel-last -> out fp32 planar
+ * [n, 3, h_out, w_out], ImageNet-normalised.  mean, std = HOST arrays of 3 floats.  Each source sample is normalised as
+ * the depth data pipeline does it, three correctly rounded fp32 operations in this order: x / 255, - mean[c], / std[c];
+ * the normalised samples are then resampled with align_corners=True.  The result is bit-identical to um_resize_bilinear of
+ * the normalised planar frames, and at (h_out, w_out) = (h, w) it is exactly those frames.  No transpose.
+ * Replaces the host-side ToTensor / Normalize (dataloader/depth/augmentation.py:30, 56-61) and the F.interpolate of
+ * evaluate_depth.py:372-376. */
+int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t h_out,
+                                   int32_t w_out, const float* mean, const float* std, void* stream);
+
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the

@@ -1,16 +1,20 @@
 #!/usr/bin/env python
-"""Video optical flow against pairwise inference on the same consecutive pairs, on one GPU.
+"""Video inference against pairwise inference on the same consecutive pairs, on one GPU.
 
-    python tools/video_bench.py [--workload config4|config2] [--steps K] [--warmup W] [--pairs-per-step B]
+    python tools/video_bench.py [--workload config4|config2|config5] [--steps K] [--warmup W] [--pairs-per-step B]
 
-The timed video step is what `unimatch_b200.VideoFlowRunner` does per step: B new synthetic uint8 frames are copied from pinned
-memory, converted on the device (`um_frames_to_planar`), encoded, paired with the previous step's last frame (its feature
-pyramid is carried, not re-encoded) and run as B pairs; the flow goes back to pinned memory.  The pairwise step is
-`UniMatch.forward` on the same B pairs, uploaded as two float32 images per pair and downloaded the same way.  The two steps
-alternate in one process, eager on both sides, and the workloads, sizes and weights are those of bench.py.  Prints ONE JSON
-line: pairs/s of each path, the encoder ("backbone") section time of each, H2D / D2H bytes per step, and how far the two
-outputs are apart (they are not bit-identical: see `UniMatch.encode_frames`).  Exits non-zero beyond 1e-4 of the largest flow.
-Writes nothing to the tree.
+Flow workloads (config4, config2): the timed video step is what `unimatch_b200.VideoFlowRunner` does per step: B new synthetic
+uint8 frames are copied from pinned memory, converted on the device (`um_frames_to_planar`), encoded, paired with the previous
+step's last frame (its feature pyramid is carried, not re-encoded) and run as B pairs; the flow goes back to pinned memory.
+The pairwise step is `UniMatch.forward` on the same B pairs, uploaded as two float32 images per pair and downloaded the same way.
+Depth workload (config5): the timed sequence step is what `unimatch_b200.DepthSequenceRunner` does per step: B new uint8 frames
+of a synthetic posed sequence and their B relative poses are copied from pinned memory, normalised and converted on the device
+(`um_frames_to_planar_normalized`), encoded and run as B pairs with the carried frame; the pairwise step is `UniMatch.forward`
+on the same B pairs as ImageNet-normalised float32 images, with their intrinsics and relative poses.
+The two steps alternate in one process, eager on both sides, and the workloads, sizes and weights are those of bench.py.
+Prints ONE JSON line: pairs/s of each path, the encoder ("backbone") section time of each, H2D / D2H bytes per step, and how
+far the two outputs are apart (they are not bit-identical: see `UniMatch.encode_frames`).  Exits non-zero beyond 1e-4 of the
+largest output value.  Writes nothing to the tree.
 """
 import argparse
 import json
@@ -27,7 +31,7 @@ from bench import BENCH_WORKLOADS  # noqa: E402
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="config4", choices=["config4", "config2"])
+    ap.add_argument("--workload", default="config4", choices=["config4", "config2", "config5"])
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--pairs-per-step", type=int, default=0, help="B (default: the workload's pairs per GPU in bench.py)")
@@ -36,42 +40,22 @@ def main():
 
 
 def run(args):
-    """One VideoFlowRunner step (B new synthetic uint8 frames uploaded from pinned memory, the previous step's last
-    frame carried, B pairs, flow back to pinned memory) against `UniMatch.forward` on the same B pairs as float32 images
-    (uploaded and downloaded the same way), alternating step by step in one process, eager on both sides."""
+    """One runner step (B new synthetic uint8 frames uploaded from pinned memory, the previous step's last frame carried, B
+    pairs, output back to pinned memory) against `UniMatch.forward` on the same B pairs as float32 images (uploaded and
+    downloaded the same way), alternating step by step in one process, eager on both sides."""
     from unimatch_b200 import UniMatch, ops
-    from unimatch_b200.inference import VideoFlowRunner
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
     wl_name, H, W, ppg, cfg_idx, _, _ = BENCH_WORKLOADS[args.workload]
     cfg = WORKLOADS[wl_name]
-    if cfg["model"]["task"] != "flow":
-        raise SystemExit("video inference runs the flow workloads only (config4, config2)")
     B = args.pairs_per_step or ppg
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     model = UniMatch(**cfg["model"]).eval()
     model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
     model = model.to(dev)
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    frames = synthetic_video(B + 1, H, W, seed=77)                          # frame 0 = carried, frames 1..B = new
-    runner = VideoFlowRunner(model, (H, W), B, dev, padding_factor=cfg["pad"], use_graph=False, **call)
-    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(dev))]
-    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
-    pin_new = frames[1:].contiguous().pin_memory()
-    planar = frames.permute(0, 3, 1, 2).float()
-    pin0, pin1 = planar[:-1].contiguous().pin_memory(), planar[1:].contiguous().pin_memory()
-    out_v, out_p = torch.empty((B, 2, H, W)).pin_memory(), torch.empty((B, 2, H, W)).pin_memory()
-
-    def video_step():
-        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
-            c.copy_(f)
-        runner.dev_in[0].copy_(pin_new, non_blocking=True)
-        out_v.copy_(runner._step(0)["flow"], non_blocking=True)
-
-    def pair_step():
-        a, b = pin0.to(dev, non_blocking=True), pin1.to(dev, non_blocking=True)
-        out_p.copy_(model(a, b, **cfg["call"])["flow_preds"][-1], non_blocking=True)
+    setup = _flow_steps if cfg["model"]["task"] == "flow" else _depth_steps
+    video_step, pair_step, out_v, out_p, io, notes = setup(model, cfg, H, W, B, dev)
 
     for _ in range(max(args.warmup, 2)):
         video_step(); pair_step()
@@ -103,24 +87,94 @@ def run(args):
                 acc[tag[4:]] = acc.get(tag[4:], 0.0) + a.elapsed_time(b)
         sections[name] = {k: round(v / args.steps, 3) for k, v in acc.items()}
     props = torch.cuda.get_device_properties(dev)
-    res = {"metric": "pairs/s of consecutive video pairs @%dx%d %s, video path vs pairwise forward" % (H, W, wl_name),
+    res = {"metric": "pairs/s of consecutive %s pairs @%dx%d %s, %s path vs pairwise forward" % (notes["kind"], H, W, wl_name,
+                                                                                                  notes["kind"]),
            "device": props.name, "workload": "%s %dx%d, %d pairs per step (BASELINE configs[%d])" % (wl_name, H, W, B, cfg_idx),
-           "steps": args.steps, "warmup": max(args.warmup, 2), "data": "synthetic_video seed 77", "cuda_graph": False,
+           "steps": args.steps, "warmup": max(args.warmup, 2), "data": notes["data"], "cuda_graph": False,
            "video": {"pairs_per_s": B / (ms_v / 1e3), "ms_per_step": round(ms_v, 3),
                      "sections_ms_per_step": {"backbone": sections["video"].get("backbone")},
-                     "h2d_bytes_per_step": int(pin_new.numel()), "d2h_bytes_per_step": int(out_v.numel() * 4),
+                     "h2d_bytes_per_step": io[0], "d2h_bytes_per_step": int(out_v.numel() * 4),
                      "note": "B new frames encoded, the carried frame's pyramid reused (restored to frame 0's by a device copy "
                              "inside the step so that every step runs the same pairs)"},
            "pairwise": {"pairs_per_s": B / (ms_p / 1e3), "ms_per_step": round(ms_p, 3),
                         "sections_ms_per_step": {"backbone": sections["pairwise"].get("backbone")},
-                        "h2d_bytes_per_step": int((pin0.numel() + pin1.numel()) * 4), "d2h_bytes_per_step": int(out_p.numel() * 4)},
-           "speedup": ms_p / ms_v, "outputs_bit_identical": identical, "max_abs_diff_rel_to_max_flow": rel_diff,
+                        "h2d_bytes_per_step": io[1], "d2h_bytes_per_step": int(out_p.numel() * 4)},
+           "speedup": ms_p / ms_v, "outputs_bit_identical": identical, "max_abs_diff_rel_to_max_" + notes["value"]: rel_diff,
            "identity_note": "um_conv2d_tc sums a tile's K chunks in an order rotated by the CTA owning the tile; encoding B frames "
-                            "instead of 2B changes the tile-to-CTA map, hence the last bits (tolerance 1e-4 of the largest flow)",
+                            "instead of 2B changes the tile-to-CTA map, hence the last bits (tolerance 1e-4 of the largest %s)"
+                            % notes["value"],
            "launches_per_process": ops.launch_count()}
     print(json.dumps(res))
     if rel_diff > 1e-4:
         sys.exit(1)
+
+
+def _flow_steps(model, cfg, H, W, B, dev):
+    """VideoFlowRunner step and pairwise forward on the same B pairs of a synthetic video"""
+    from unimatch_b200.inference import VideoFlowRunner
+    from unimatch_b200.synthetic import synthetic_video
+    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    frames = synthetic_video(B + 1, H, W, seed=77)                          # frame 0 = carried, frames 1..B = new
+    runner = VideoFlowRunner(model, (H, W), B, dev, padding_factor=cfg["pad"], use_graph=False, **call)
+    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(dev))]
+    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
+    pin_new = frames[1:].contiguous().pin_memory()
+    planar = frames.permute(0, 3, 1, 2).float()
+    pin0, pin1 = planar[:-1].contiguous().pin_memory(), planar[1:].contiguous().pin_memory()
+    out_v, out_p = torch.empty((B, 2, H, W)).pin_memory(), torch.empty((B, 2, H, W)).pin_memory()
+
+    def video_step():
+        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
+            c.copy_(f)
+        runner.dev_in[0].copy_(pin_new, non_blocking=True)
+        out_v.copy_(runner._step(0)["flow"], non_blocking=True)
+
+    def pair_step():
+        a, b = pin0.to(dev, non_blocking=True), pin1.to(dev, non_blocking=True)
+        out_p.copy_(model(a, b, **cfg["call"])["flow_preds"][-1], non_blocking=True)
+
+    io = (int(pin_new.numel()), int((pin0.numel() + pin1.numel()) * 4))
+    return video_step, pair_step, out_v, out_p, io, dict(kind="video", data="synthetic_video seed 77", value="flow")
+
+
+def _depth_steps(model, cfg, H, W, B, dev):
+    """DepthSequenceRunner step and pairwise forward on the same B pairs of a synthetic posed sequence.  bench.py's call
+    gives the model's inverse-depth range; the runner takes the metric one."""
+    from unimatch_b200.inference import DepthSequenceRunner, _relative_poses
+    from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_posed_sequence
+    call = cfg["call"]
+    kw = {k: v for k, v in call.items() if k not in ("task", "min_depth", "max_depth", "num_depth_candidates")}
+    frames, K, poses = synthetic_posed_sequence(B + 1, H, W, seed=77)     # frame 0 = carried, frames 1..B = new
+    runner = DepthSequenceRunner(model, (H, W), B, dev, K, padding_factor=cfg["pad"], use_graph=False,
+                                 min_depth=1.0 / call["max_depth"], max_depth=1.0 / call["min_depth"],
+                                 num_depth_candidates=call["num_depth_candidates"], **kw)
+    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(dev))]
+    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
+    pin_new = frames[1:].contiguous().pin_memory()
+    rel = torch.from_numpy(_relative_poses([p for p in poses.numpy()], False))
+    pin_pose = rel.contiguous().pin_memory()
+    mean, std = torch.tensor(IMAGENET_MEAN).view(1, 3, 1, 1), torch.tensor(IMAGENET_STD).view(1, 3, 1, 1)
+    planar = (frames.permute(0, 3, 1, 2).float() / 255. - mean) / std
+    pin0, pin1 = planar[:-1].contiguous().pin_memory(), planar[1:].contiguous().pin_memory()
+    pin_k = K[None].repeat(B, 1, 1).contiguous().pin_memory()
+    out_v, out_p = torch.empty((B, H, W)).pin_memory(), torch.empty((B, H, W)).pin_memory()
+
+    def video_step():
+        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
+            c.copy_(f)
+        runner.dev_in[0].copy_(pin_new, non_blocking=True)
+        runner.pose_dev[0].copy_(pin_pose, non_blocking=True)
+        out_v.copy_(runner._step(0)["depth"], non_blocking=True)
+
+    def pair_step():
+        a, b = pin0.to(dev, non_blocking=True), pin1.to(dev, non_blocking=True)
+        k, p = pin_k.to(dev, non_blocking=True), pin_pose.to(dev, non_blocking=True)
+        out_p.copy_(model(a, b, intrinsics=k, pose=p, **call)["flow_preds"][-1], non_blocking=True)
+
+    io = (int(pin_new.numel() + pin_pose.numel() * 4),
+          int((pin0.numel() + pin1.numel() + pin_k.numel() + pin_pose.numel()) * 4))
+    return video_step, pair_step, out_v, out_p, io, dict(kind="depth-sequence", data="synthetic_posed_sequence seed 77",
+                                                        value="depth")
 
 
 if __name__ == "__main__":

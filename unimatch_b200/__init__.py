@@ -23,11 +23,13 @@ _LAZY = {
     "infer_flow_video": (".inference", "infer_flow_video"),
     "VideoFlowRunner": (".inference", "VideoFlowRunner"),
     "flow_to_image": (".inference", "flow_to_image"),
+    "infer_depth_sequence": (".inference", "infer_depth_sequence"),
+    "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
 }
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "flow_to_image"]
+           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner"]
 
 
 def __getattr__(name):

@@ -176,6 +176,34 @@ __global__ void __launch_bounds__(256) frames_to_planar_kernel(const uint8_t* __
   }
 }
 
+// ---- depth frames -> model input: uint8 [T,H,W,3] -> ImageNet-normalised fp32 planar [T,3,ho,wo] ----------------------
+// = resize_bilinear of the frames normalised the way the depth data pipeline does it on the host
+// (dataloader/depth/augmentation.py:30, 56-61): every SOURCE sample is x / 255, then - mean_c, then / std_c, each one
+// correctly rounded fp32 operation in that order, and the normalised samples are resampled.  No transpose: the depth
+// drivers have no portrait rule.
+__global__ void __launch_bounds__(256) frames_to_planar_normalized_kernel(const uint8_t* __restrict__ frames,
+                                                                          float* __restrict__ out, int H, int W, int ho, int wo,
+                                                                          float m0, float m1, float m2, float s0, float s1,
+                                                                          float s2, long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int X = (int)(i % wo);
+  const int Y = (int)((i / wo) % ho);
+  const long long t = i / ((long long)ho * wo);
+  const uint8_t* base = frames + t * (long long)H * W * 3;
+  const long long plane = (long long)ho * wo;
+  float* o = out + t * 3 * plane + (long long)Y * wo + X;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float mean = c == 0 ? m0 : (c == 1 ? m1 : m2), std = c == 0 ? s0 : (c == 1 ? s1 : s2);
+    const auto load = [&](int y, int x) {
+      const float v = (float)__ldg(base + ((long long)y * W + x) * 3 + c);
+      return __fdiv_rn(__fsub_rn(__fdiv_rn(v, 255.0f), mean), std);
+    };
+    o[c * plane] = bilinear_align_corners(load, H, W, ho, wo, Y, X);
+  }
+}
+
 // ---- Middlebury flow colouring: flow_to_image of utils/flow_viz.py:240-275 (the VCN variant) --------------------------
 // Precision follows numpy on float32 flow: |u| or |v| > 1e7 (UNKNOWN_FLOW_THRESH, :140) -> zeroed and painted black;
 // rad = sqrt(u*u + v*v) and its per-image maximum in FLOAT32 (:264-265); everything after that in FLOAT64, because
@@ -355,6 +383,16 @@ int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h,
   frames_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(frames, out, h, w, transpose ? 1 : 0,
                                                                                            h_out, w_out, total);
   return um::check_launch("um_frames_to_planar");
+}
+
+int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t h_out,
+                                   int32_t w_out, const float* mean, const float* std, void* stream) {
+  UM_REQUIRE(frames && out && mean && std && n > 0 && h > 0 && w > 0 && h_out > 0 && w_out > 0,
+             "um_frames_to_planar_normalized: bad arguments (positive sizes, non-null buffers, 3 means and stds)");
+  const long long total = (long long)n * h_out * w_out;
+  frames_to_planar_normalized_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      frames, out, h, w, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2], total);
+  return um::check_launch("um_frames_to_planar_normalized");
 }
 
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,

@@ -17,13 +17,20 @@ sequence with every frame encoded ONCE (pair (t, t+1) and pair (t+1, t+2) share 
 per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 summation order), `VideoFlowRunner` streams host uint8 frames through the same
 path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
 colouring of utils/flow_viz.py on the device.  Decoding and writing files (frames, PNG, .flo, mp4) stay out of scope.
+
+Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
+sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
+does; `DepthSequenceRunner` streams host (uint8 frame, pose) items through the same path, replayed as a CUDA graph.  Colouring
+depth maps (matplotlib's `plasma`, evaluate_depth.py:403-417) stays out of scope.
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
 from . import ops  # noqa: F401  (registers torch.ops.unimatch_sm100.*)
+from .synthetic import IMAGENET_MEAN, IMAGENET_STD
 
 _OPS = torch.ops.unimatch_sm100
 
@@ -212,7 +219,12 @@ def infer_depth(model, img_ref, img_tgt, intrinsics, pose, *, padding_factor=16,
     depth = model(img_ref.float().contiguous(), img_tgt.float().contiguous(), intrinsics=intrinsics, pose=pose,
                   min_depth=1.0 / max_depth, max_depth=1.0 / min_depth, num_depth_candidates=num_depth_candidates,
                   depth_from_argmax=depth_from_argmax, pred_bidir_depth=pred_bidir_depth, **model_kwargs)["flow_preds"][-1]
-    if resized:
+    return _depth_outputs(depth, ori, size, pred_bidir_depth)
+
+
+def _depth_outputs(depth, ori, size, pred_bidir_depth):
+    """The model's depth at the inference size -> the driver's outputs at the original size (evaluate_depth.py:397-417)."""
+    if size != ori:
         depth = _resize(depth.unsqueeze(1), ori).squeeze(1)
     if pred_bidir_depth:
         half = depth.shape[0] // 2
@@ -220,12 +232,99 @@ def infer_depth(model, img_ref, img_tgt, intrinsics, pose, *, padding_factor=16,
     return {"depth": depth}
 
 
+# ---------------------------------------------------------------------------------------------- depth over posed sequences
+def _depth_task_kwargs(model_kwargs, name):
+    if model_kwargs.pop("task", "depth") != "depth":
+        raise ValueError("%s drives the depth task only" % name)
+    return model_kwargs
+
+
+def _intrinsics33(intrinsics, name):
+    """The sequence's one intrinsics matrix (the reference reads one file per sequence, evaluate_depth.py:331, :343) as float32 [3,3]."""
+    if not (torch.is_tensor(intrinsics) or isinstance(intrinsics, np.ndarray)) or tuple(intrinsics.shape) != (3, 3):
+        raise ValueError("%s: intrinsics must be one [3,3] matrix (tensor or numpy array)" % name)
+    if not (intrinsics.dtype.is_floating_point if torch.is_tensor(intrinsics) else np.issubdtype(intrinsics.dtype, np.floating)):
+        raise ValueError("%s: intrinsics must be floating point" % name)
+    return torch.as_tensor(intrinsics).float()
+
+
+def _pose44(pose, name):
+    """An absolute camera pose on the host as float32 [4,4], as the reference loads it (np.loadtxt(...).astype(np.float32))."""
+    if torch.is_tensor(pose) and pose.is_cuda:
+        raise ValueError("%s: camera poses are host arrays (numpy or CPU tensors)" % name)
+    p = np.asarray(pose)
+    if p.shape != (4, 4) or not np.issubdtype(p.dtype, np.floating):
+        raise ValueError("%s: a camera pose must be a floating-point [4,4] matrix" % name)
+    return p.astype(np.float32)
+
+
+def _relative_poses(poses, bidir):
+    """Relative poses of the consecutive pairs of a list of absolute float32 poses [4,4], computed on the host with the
+    reference's own expression, pair by pair (evaluate_depth.py:344-350): inv(pose[t+1]) @ pose[t] in numpy float32.  With
+    `bidir` the inverses of those (np.linalg.inv) follow, for the backward streams: float32 [n,4,4] or [2n,4,4], the layout
+    `UniMatch.depth_cameras` takes."""
+    rel = [np.linalg.inv(poses[t + 1]) @ poses[t] for t in range(len(poses) - 1)]
+    if bidir:
+        rel += [np.linalg.inv(r) for r in rel]
+    return np.stack(rel).astype(np.float32)
+
+
+def _depth_frames_to_model(frames, size):
+    """[T,H,W,3] uint8 (one fused kernel: ImageNet normalisation and resize) or [T,3,H,W] normalised float frames ->
+    planar float32 [T,3,*size] model input (evaluate_depth.py:353-376)."""
+    if frames.dtype == torch.uint8:
+        return _OPS.frames_to_planar_normalized(frames.contiguous(), int(size[0]), int(size[1]), list(IMAGENET_MEAN),
+                                                list(IMAGENET_STD))
+    return _resize(frames, size) if tuple(frames.shape[-2:]) != tuple(size) else frames.float().contiguous()
+
+
+@torch.no_grad()
+def infer_depth_sequence(model, frames, intrinsics, poses, *, padding_factor=16, inference_size=None, min_depth=0.5,
+                         max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
+                         **model_kwargs):
+    """`inference_depth` (evaluate_depth.py:297-419) on a posed frame sequence with every frame encoded once.
+
+    `frames`: device uint8 [T,H,W,3] as decoded (normalised and resized by one kernel) or ImageNet-normalised float
+    [T,3,H,W]; `intrinsics`: the sequence's [3,3] matrix (not rescaled when the frames are resized, as in the reference);
+    `poses`: the absolute camera poses [T,4,4] on the host.  The T-1 consecutive pairs (t, t+1) get the relative pose
+    inv(pose[t+1]) @ pose[t], computed on the host in numpy float32 as the reference does (and its inverse there too when
+    `pred_bidir_depth`).  Returns what `infer_depth` returns on those pairs: {'depth': [T-1,H,W]} (+ 'depth_bwd'), equal up to
+    fp32 summation order (see `UniMatch.encode_frames`)."""
+    model_kwargs = _depth_task_kwargs(model_kwargs, "infer_depth_sequence")
+    if not torch.is_tensor(frames) or frames.dim() != 4 or frames.shape[0] < 2:
+        raise ValueError("infer_depth_sequence needs at least two frames [T>=2, H, W, 3] uint8 or [T>=2, 3, H, W] float")
+    if frames.dtype == torch.uint8:
+        if frames.shape[-1] != 3:
+            raise ValueError("infer_depth_sequence: uint8 frames are channel-last [T, H, W, 3]")
+        ori = (int(frames.shape[1]), int(frames.shape[2]))
+    elif frames.dtype.is_floating_point and frames.shape[1] == 3:
+        ori = (int(frames.shape[2]), int(frames.shape[3]))
+    else:
+        raise ValueError("infer_depth_sequence: frames must be uint8 [T, H, W, 3] or float [T, 3, H, W]")
+    T = frames.shape[0]
+    if len(poses) != T:
+        raise ValueError("infer_depth_sequence: %d frames need %d poses, got %d" % (T, T, len(poses)))
+    abs_poses = [_pose44(p, "infer_depth_sequence") for p in poses]
+    K = _intrinsics33(intrinsics, "infer_depth_sequence")
+    size = _inference_size(ori, padding_factor, inference_size)
+    dev = frames.device
+    feats = model.encode_frames(_depth_frames_to_model(frames, size), task="depth")
+    rel = torch.from_numpy(_relative_poses(abs_poses, pred_bidir_depth)).to(dev)
+    cams = model.depth_cameras(K.to(dev)[None].repeat(T - 1, 1, 1), rel, model.upsample_factor, 1.0 / max_depth,
+                               1.0 / min_depth, num_depth_candidates, pred_bidir_depth)
+    depth = model.forward_encoded([f[:-1] for f in feats], [f[1:] for f in feats], task="depth", cameras=cams,
+                                  min_depth=1.0 / max_depth, max_depth=1.0 / min_depth, depth_from_argmax=depth_from_argmax,
+                                  pred_bidir_depth=pred_bidir_depth, **model_kwargs)["flow_preds"][-1]
+    return _depth_outputs(depth, ori, size, pred_bidir_depth)
+
+
 class _PipelinedRunner:
     """Two staging slots, host->device copies on a side stream, one CUDA graph per slot, device->host copies behind the step.
 
     Subclasses provide `_stage_host(slot, chunk)` (fill the slot's pinned buffers and enqueue their H2D copies on the current
-    stream, which is the copy stream), `_reset_inputs(slot)`, `_step(slot)` (the fixed-shape device work -> dict of device
-    tensors), `_download(slot, out)` (enqueue the D2H copies of a step's outputs) and `_results(slot, n)` (the host results)."""
+    stream, which is the copy stream), `_reset_inputs(slot)` and `_step(slot)` (the fixed-shape device work).  When `_step`
+    returns a dict of device tensors whose first axis is the batch, the default `_download(slot, out)` (enqueue the D2H
+    copies of a step's outputs into pinned buffers) and `_results(slot, n)` (one dict of host tensors per item) apply."""
 
     def _init_pipeline(self, device, use_graph):
         self.dev = torch.device(device)
@@ -233,6 +332,17 @@ class _PipelinedRunner:
         self.graphs = [None, None]
         self.static_out = [None, None]
         self.use_graph = use_graph
+        self.out_pin = [None, None]
+
+    def _download(self, slot, out):
+        if self.out_pin[slot] is None:
+            self.out_pin[slot] = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in out.items()}
+        for k, v in out.items():
+            self.out_pin[slot][k].copy_(v, non_blocking=True)
+
+    def _results(self, slot, n):
+        for i in range(n):
+            yield {k: v[i] for k, v in self.out_pin[slot].items()}
 
     def _capture(self):
         with torch.cuda.device(self.dev):
@@ -407,7 +517,6 @@ class VideoFlowRunner(_PipelinedRunner):
         self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
         self.carry_frame = torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev)
         self.carry = None                                  # last frame's feature pyramid, [1,h,w,128] per scale
-        self.out_pin = [None, None]
 
     # ---- device side
     def _encode(self, frames_u8):
@@ -445,16 +554,6 @@ class VideoFlowRunner(_PipelinedRunner):
             self.pin[slot][i].copy_(torch.as_tensor(chunk[min(i, len(chunk) - 1)]))
         self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
 
-    def _download(self, slot, out):
-        if self.out_pin[slot] is None:
-            self.out_pin[slot] = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in out.items()}
-        for k, v in out.items():
-            self.out_pin[slot][k].copy_(v, non_blocking=True)
-
-    def _results(self, slot, n):
-        for i in range(n):
-            yield {k: v[i] for k, v in self.out_pin[slot].items()}
-
     def _prime(self, frame):
         """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
         f = torch.as_tensor(frame).to(self.dev)[None].contiguous()
@@ -472,3 +571,104 @@ class VideoFlowRunner(_PipelinedRunner):
             if self.carry is None:                       # eager runs: allocate the carried pyramid
                 self.carry = [f.clone() for f in self._encode(torch.as_tensor(first).to(self.dev)[None].contiguous())]
             yield from self._pipeline(it, start=lambda: self._prime(first))
+
+
+class DepthSequenceRunner(_PipelinedRunner):
+    """Streaming depth over a posed frame sequence: consecutive pairs of host (uint8 frame, absolute pose) items, every frame
+    uploaded and encoded once -- the depth counterpart of `VideoFlowRunner`.
+
+    * upload: each step copies `batch` NEW frames, uint8 [H,W,3] as decoded, and the `batch` relative poses of its pairs
+      (followed by their inverses when `pred_bidir_depth`), computed on the host with the reference's numpy expression,
+      through pinned double buffers on a side stream (0.59 MB per 384x512 frame, against 4.72 MB for the two float32
+      images of a pair);
+    * device work of a step (one CUDA graph per staging slot): `um_frames_to_planar_normalized` (uint8 -> ImageNet-normalised
+      planes at the inference size), the encoder on the new frames, the depth matching path on the `batch` pairs (previous
+      step's last frame, new frames) and the depth resized back.  The camera operands that depend on the intrinsics only
+      (`UniMatch.depth_cameras`) are built once, eagerly, before any capture; the per-step poses are static device buffers that
+      the upload fills.  The last frame's pyramid stays on the device for the next step and its pose on the host.  A short
+      last step is filled with repeats of its last item and the extra results are dropped;
+    * download: 'depth' (and 'depth_bwd') [H,W] per pair.
+
+    Sizes and semantics are those of `infer_depth_sequence` (and `infer_depth`): `min_depth` / `max_depth` are metric,
+    the intrinsics [3,3] are not rescaled with the frames.  `run(items)` takes an iterable of (uint8 frame [H,W,3], pose [4,4])
+    host items and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy what you keep)."""
+
+    def __init__(self, model, frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None, min_depth=0.5,
+                 max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False, use_graph=True,
+                 **model_kwargs):
+        self.model, self.batch = model, int(batch)
+        self.kw = _depth_task_kwargs(dict(model_kwargs), "DepthSequenceRunner")
+        if self.batch < 1:
+            raise ValueError("DepthSequenceRunner: batch must be positive")
+        K = _intrinsics33(intrinsics, "DepthSequenceRunner")
+        self._init_pipeline(device, use_graph)
+        self.h, self.w = int(frame_size[0]), int(frame_size[1])
+        self.ori = (self.h, self.w)
+        self.size = _inference_size(self.ori, padding_factor, inference_size)
+        self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
+        self.inv_range = (1.0 / max_depth, 1.0 / min_depth)                      # the model works on inverse depth
+        shape = (self.batch, self.h, self.w, 3)
+        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        npose = (2 if self.bidir else 1) * self.batch
+        self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
+        self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
+        Kb = K.to(self.dev)[None].repeat(self.batch, 1, 1)
+        # cams[slot]["pose"] IS pose_dev[slot] (a float32 pose of 2B matrices is taken as it is), so the upload updates it
+        self.cams = [model.depth_cameras(Kb, self.pose_dev[s], model.upsample_factor, *self.inv_range, num_depth_candidates,
+                                         self.bidir) for s in range(2)]
+        self.carry = None                                  # last frame's feature pyramid, [1,h,w,128]
+        self.prev_pose = None                              # last frame's absolute pose, float32 [4,4] on the host
+
+    # ---- device side
+    def _encode(self, frames_u8):
+        planar = _OPS.frames_to_planar_normalized(frames_u8, self.size[0], self.size[1], list(IMAGENET_MEAN),
+                                                  list(IMAGENET_STD))
+        return self.model.encode_frames(planar, task="depth")
+
+    def _step(self, slot):
+        new = self._encode(self.dev_in[slot])
+        first = [torch.cat((c, f[:-1]), dim=0) for c, f in zip(self.carry, new)]
+        depth = self.model.forward_encoded(first, new, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
+                                           max_depth=self.inv_range[1], depth_from_argmax=self.from_argmax,
+                                           pred_bidir_depth=self.bidir, **self.kw)["flow_preds"][-1]
+        out = _depth_outputs(depth, self.ori, self.size, self.bidir)
+        for c, f in zip(self.carry, new):                # carry the last frame into the next step
+            c.copy_(f[-1:])
+        return out
+
+    def _reset_inputs(self, slot):
+        self.dev_in[slot].zero_()
+        self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
+
+    # ---- host side
+    def _stage_host(self, slot, chunk):
+        poses = [self.prev_pose]
+        for i in range(self.batch):
+            frame, pose = chunk[min(i, len(chunk) - 1)]
+            self.pin[slot][i].copy_(torch.as_tensor(frame))
+            poses.append(_pose44(pose, "DepthSequenceRunner"))
+        self.pose_pin[slot].copy_(torch.from_numpy(_relative_poses(poses, self.bidir)))
+        self.prev_pose = poses[-1]
+        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
+        self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
+
+    def _prime(self, frame):
+        """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
+        for c, g in zip(self.carry, self._encode(torch.as_tensor(frame).to(self.dev)[None].contiguous())):
+            c.copy_(g)
+
+    @torch.no_grad()
+    def run(self, items):
+        with torch.cuda.device(self.dev):
+            it = iter(items)
+            first = next(it, None)
+            if first is None:
+                return
+            frame0, pose0 = first
+            if tuple(torch.as_tensor(frame0).shape) != (self.h, self.w, 3):
+                raise ValueError("DepthSequenceRunner: frames must be uint8 [%d, %d, 3]" % (self.h, self.w))
+            self.prev_pose = _pose44(pose0, "DepthSequenceRunner")
+            if self.carry is None:                       # eager runs: allocate the carried pyramid
+                self.carry = [f.clone() for f in self._encode(torch.as_tensor(frame0).to(self.dev)[None].contiguous())]
+            yield from self._pipeline(it, start=lambda: self._prime(frame0))

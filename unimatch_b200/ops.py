@@ -19,7 +19,7 @@ SYMBOLS = [
     "um_window_attention", "um_window_attention_workspace", "um_attention_planes_lp", "um_window_attention_planes", "um_debug_set_dump", "um_softmax_expectation", "um_softmax_expectation_workspace",
     "um_local_corr_softmax", "um_local_corr_volume", "um_flow_warp", "um_fb_consistency", "um_propagate_local", "um_depth_corr_softmax",
     "um_conv2d_tc", "um_ffn_tc", "um_conv7x7_small", "um_split_planes", "um_instance_norm_scratch_floats", "um_instance_norm_stats", "um_instance_norm_apply", "um_add_position", "um_layernorm_residual", "um_convex_upsample", "um_upsample2x", "um_resize_bilinear", "um_gru_rh", "um_gru_update",
-    "um_frames_to_planar", "um_flow_to_image",
+    "um_frames_to_planar", "um_flow_to_image", "um_frames_to_planar_normalized",
 ]
 
 MASK_NONE, MASK_SWIN, MASK_CAUSAL = 0, 1, 2
@@ -128,6 +128,8 @@ def _load():
     lib.um_resize_bilinear.restype = ctypes.c_int
     lib.um_frames_to_planar.argtypes = [P, P, I, I, I, I, I, I, P]
     lib.um_frames_to_planar.restype = ctypes.c_int
+    lib.um_frames_to_planar_normalized.argtypes = [P, P, I, I, I, I, I, FP, FP, P]
+    lib.um_frames_to_planar_normalized.restype = ctypes.c_int
     lib.um_flow_to_image.argtypes = [P, P, L, L, P, I, I, I, P]
     lib.um_flow_to_image.restype = ctypes.c_int
     lib.um_debug_set_dump.argtypes = [P]
@@ -435,6 +437,25 @@ def _frames_to_planar(frames, h_out, w_out, transpose):
 
 
 frames_to_planar = _define("frames_to_planar(Tensor frames, int h_out, int w_out, bool transpose) -> Tensor", _frames_to_planar)
+
+
+def _frames_to_planar_normalized(frames, h_out, w_out, mean, std):
+    """mean / std: 3 per-channel constants each, passed to the kernel rounded to float32"""
+    if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3 or not frames.is_contiguous():
+        raise RuntimeError("frames_to_planar_normalized: expected contiguous CUDA uint8 frames [T, H, W, 3]")
+    if len(mean) != 3 or len(std) != 3:
+        raise RuntimeError("frames_to_planar_normalized: expected 3 means and 3 stds")
+    t, h, w, _ = frames.shape
+    out = torch.empty((t, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
+    m, s = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
+    _check(LIB.um_frames_to_planar_normalized(_p(frames), _p(out), t, h, w, h_out, w_out, m, s, _stream()),
+           "um_frames_to_planar_normalized")
+    return out
+
+
+frames_to_planar_normalized = _define(
+    "frames_to_planar_normalized(Tensor frames, int h_out, int w_out, float[] mean, float[] std) -> Tensor",
+    _frames_to_planar_normalized)
 
 
 def _flow_to_image(flow, out):

@@ -118,6 +118,29 @@ def synthetic_video(T, h, w, seed=1234, step=3):
     return torch.stack(frames, 0).contiguous()
 
 
+def synthetic_posed_sequence(T, h, w, seed=1234, step=3, plane_depth=2.0):
+    """A posed frame sequence for depth inference: T frames uint8 [T,H,W,3] of a fronto-parallel textured plane at depth
+    `plane_depth`, the intrinsics K [3,3] (focal 0.9 W, centred principal point) and the absolute camera-to-world poses
+    [T,4,4] (float32, as the reference loads pose files).  The camera moves along x only, by seeded whole-pixel amounts of up
+    to `step` px per frame: the frames are crops of one box-blurred noise canvas at matching integer x-shifts, so every
+    consecutive pair has a true match with depth `plane_depth` everywhere."""
+    g = torch.Generator().manual_seed(seed)
+    m = step * max(T - 1, 0) + 1
+    canvas = _texture(g, h, w + 2 * m)[0].round().clamp(0, 255).to(torch.uint8).permute(1, 2, 0)
+    shifts = torch.randint(-step, step + 1, (max(T - 1, 0),), generator=g).tolist()
+    focal = 0.9 * w
+    K = torch.tensor([[focal, 0.0, w / 2.0], [0.0, focal, h / 2.0], [0.0, 0.0, 1.0]])
+    frames, poses, x = [], [], 0
+    for t in range(T):
+        if t > 0:
+            x += shifts[t - 1]
+        frames.append(canvas[:, m + x:m + x + w])          # camera moved right by x px -> the crop moves right by x px
+        pose = torch.eye(4, dtype=torch.float64)
+        pose[0, 3] = x * plane_depth / focal
+        poses.append(pose)
+    return torch.stack(frames, 0).contiguous(), K, torch.stack(poses, 0).float()
+
+
 def noise_batch(task, batch, h, w, seed=99):
     """Cheap pure-noise batch for throughput runs (no match structure; same arithmetic)."""
     g = torch.Generator().manual_seed(seed)

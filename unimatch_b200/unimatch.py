@@ -102,6 +102,7 @@ class UniMatch(nn.Module):
         self._prep_key = None
         self._prep = None
         self._tables = {}
+        self._cands = {}             # depth candidate vectors, per (min, max, n, device)
         self._attn_ws = {}           # window-major attention operand planes, cached per (device, streams, geometry)
         self._pad_ws = {}            # zero-padded plane buffers, cached per (use, shape)
         self.training = False        # inference-only module: starts (and stays) in eval mode
@@ -465,19 +466,15 @@ class UniMatch(nn.Module):
 
     def _stage_correlation(self, tok, Bp, h, wd, task, radius, pred_bidir_flow=False, depth=None):
         """Correlation + softmax (unimatch.py:186-216) on the transformer outputs tok [2Bp, L, 128] -> [ns, h, w, fd]."""
-        dev = tok.device
         t0, t1 = tok[:Bp], tok[Bp:]
         if task == "depth":
-            Ks, pose, min_depth, max_depth, ncand, from_argmax, bidir = depth
-            cand = torch.linspace(min_depth, max_depth, ncand).float().to(dev)                         # :190
+            cams, from_argmax, bidir = depth                                 # cams: `depth_cameras`
             if bidir:
                 q0, q1 = torch.cat((t0, t1), 0).contiguous(), torch.cat((t1, t0), 0).contiguous()
-                Kc = Ks.repeat(2, 1, 1)
-                pc = torch.cat((pose, torch.inverse(pose)), dim=0).float()
             else:
-                q0, q1, Kc, pc = t0.contiguous(), t1.contiguous(), Ks, pose.float()
-            return _OPS.depth_corr_softmax(q0, q1, Kc.contiguous(), torch.inverse(Kc).contiguous(), pc.contiguous(), cand,
-                                           h, wd, bool(from_argmax))
+                q0, q1 = t0.contiguous(), t1.contiguous()
+            return _OPS.depth_corr_softmax(q0, q1, cams["K"].contiguous(), cams["K_inv"].contiguous(),
+                                           cams["pose"].contiguous(), cams["cand"], h, wd, bool(from_argmax))
         if radius == -1:
             if task == "flow":
                 ns = 2 * Bp if pred_bidir_flow else Bp
@@ -588,8 +585,8 @@ class UniMatch(nn.Module):
         pre-transformer features, update block, residual update.  Returns (flow, mask or None)."""
         h, wd = flow.shape[1], flow.shape[2]
         if task == "depth":
-            Kr, pr, min_depth, max_depth = depth
-            cflow = self._rigid_flow(flow, Kr.float(), pr.float(), h, wd)
+            cams, min_depth, max_depth = depth
+            cflow = self._rigid_flow(flow, cams["K"].float(), cams["K_inv"].float(), cams["pose"].float(), h, wd)
         else:
             cflow = flow.contiguous()                                       # disparity handled in-kernel
         with self._section("refine_corr_volume"):
@@ -621,15 +618,16 @@ class UniMatch(nn.Module):
         return _OPS.convex_upsample(flow2.contiguous(), m, factor, float(mult))
 
     @staticmethod
-    def _rigid_flow(inv_depth, K, pose, h, w):
-        """compute_flow_with_depth_pose(1/inv_depth, K, pose) (geometry.py:99-195) on [B,h,w,1] -> [B,h,w,2]."""
+    def _rigid_flow(inv_depth, K, K_inv, pose, h, w):
+        """compute_flow_with_depth_pose(1/inv_depth, K, pose) (geometry.py:99-195) on [B,h,w,1] -> [B,h,w,2];
+        K_inv = torch.inverse(K), taken once per forward by `depth_cameras`."""
         b = inv_depth.shape[0]
         dev = inv_depth.device
         ys, xs = torch.meshgrid(torch.arange(h, device=dev, dtype=torch.float32),
                                 torch.arange(w, device=dev, dtype=torch.float32), indexing="ij")
         grid = torch.stack([xs, ys, torch.ones_like(xs)], dim=0).view(1, 3, -1).expand(b, 3, h * w)
         depth = (1.0 / inv_depth.view(b, 1, h * w))
-        pts = torch.inverse(K).bmm(grid) * depth
+        pts = K_inv.bmm(grid) * depth
         pts = torch.bmm(pose[:, :3, :3], pts) + pose[:, :3, -1:]
         proj = torch.bmm(K, pts)
         z = proj[:, 2:3].clamp(min=1e-3)
@@ -664,13 +662,46 @@ class UniMatch(nn.Module):
         B = img0.shape[0]
         with self._section("backbone"):                                           # [2B,h,w,128] low -> high res
             feats = self._stage_backbone(P, img0.float().contiguous(), img1.float().contiguous(), task == "flow")
+        cams = None
+        if task == "depth":
+            cams = self.depth_cameras(intrinsics, pose, self.upsample_factor, min_depth, max_depth, num_depth_candidates,
+                                      pred_bidir_depth)
         return self._forward_encoded(P, [f[:B] for f in feats], [f[B:] for f in feats], attn_type, attn_splits_list,
-                                     corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, intrinsics,
-                                     pose, min_depth, max_depth, num_depth_candidates, depth_from_argmax, pred_bidir_depth)
+                                     corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, cams,
+                                     min_depth, max_depth, depth_from_argmax, pred_bidir_depth)
+
+    # ------------------------------------------------------------------------------------------ depth cameras
+    def depth_cameras(self, intrinsics, pose, up, min_depth, max_depth, num_depth_candidates, pred_bidir_depth):
+        """The camera operands of the depth task (unimatch.py:176-190, geometry.py:99-195), as a dict of device tensors:
+          'Ks'     intrinsics [B,3,3] at the feature resolution (rows 0-1 divided by `up`, the upsample factor);
+          'K'      intrinsics of the matched streams: Ks, repeated for the backward streams when `pred_bidir_depth`;
+          'K_inv'  torch.inverse(K), read by the depth correlation and by the rigid flow of the refinement;
+          'pose'   relative poses of the matched streams: `pose` [B,4,4], with `torch.inverse(pose)` appended when
+                   `pred_bidir_depth`; a `pose` of 2B matrices is taken to hold those inverses already (e.g. computed on the
+                   host) and is used as it is;
+          'cand'   the inverse-depth candidates linspace(min_depth, max_depth, n), built once per (min, max, n, device).
+        `forward` builds them after the encoder with the same calls it always made, so its results do not change.  The
+        stages only read them: given `cameras`, `forward_encoded` issues no host synchronisation and no pageable copy and can
+        be captured in a CUDA graph.  `torch.inverse` checks its result on the host, so build the cameras outside a capture."""
+        dev = intrinsics.device
+        Ks = intrinsics.clone().float()
+        Ks[:, :2] = Ks[:, :2] / up
+        B = Ks.shape[0]
+        if pred_bidir_depth:
+            K = Ks.repeat(2, 1, 1)
+            pc = pose.float() if pose.shape[0] == 2 * B else torch.cat((pose, torch.inverse(pose)), dim=0).float()
+        else:
+            K, pc = Ks, pose.float()
+        key = (float(min_depth), float(max_depth), int(num_depth_candidates), str(dev))
+        cand = self._cands.get(key)
+        if cand is None:
+            cand = self._cands[key] = torch.linspace(min_depth, max_depth, num_depth_candidates).float().to(dev)   # :190
+        return {"Ks": Ks, "K": K, "K_inv": torch.inverse(K), "pose": pc, "cand": cand}
 
     # ------------------------------------------------------------------------------------------ video: encode frames once
-    def encode_frames(self, frames):
-        """CNN encoder on a set of frames [T,3,H,W] in [0,255] (flow task: normalize_img folded in).  Returns the feature
+    def encode_frames(self, frames, task="flow"):
+        """CNN encoder on a set of frames [T,3,H,W]: in [0,255] for the flow task (normalize_img folded into the stem), already
+        ImageNet-normalised for stereo and depth, as `forward` takes them for each task.  Returns the feature
         pyramid low -> high resolution, each [T,h,w,128].  Every encoder kernel works per image (convolutions per pixel,
         InstanceNorm per image over a fixed chunking), so a frame's features do not depend on its partner or on the batch and
         consecutive pairs of a video can share one encoding per frame.  They are equal up to fp32 summation order, not bit
@@ -679,32 +710,53 @@ class UniMatch(nn.Module):
         same frame in a batch of a different size can round differently in the last bits."""
         if self.training:
             raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
+        if task not in ("flow", "stereo", "depth"):
+            raise ValueError("encode_frames: unknown task %r" % (task,))
         with torch.no_grad():
             P = self._prepared()
             with self._section("backbone"):
-                return self._stage_backbone(P, frames.float().contiguous(), None, True)
+                return self._stage_backbone(P, frames.float().contiguous(), None, task == "flow")
 
     def forward_encoded(self, feats0, feats1, attn_type=None, attn_splits_list=None, corr_radius_list=None,
-                        prop_radius_list=None, num_reg_refine=1, pred_bidir_flow=False, task="flow", **kwargs):
+                        prop_radius_list=None, num_reg_refine=1, pred_bidir_flow=False, task="flow", cameras=None,
+                        intrinsics=None, pose=None, min_depth=1. / 0.5, max_depth=1. / 10, num_depth_candidates=64,
+                        depth_from_argmax=False, pred_bidir_depth=False, **kwargs):
         """Everything of `forward` after the encoder, on per-scale features of the first and second views ([B,h,w,128] each,
-        low -> high resolution, e.g. slices `f[:-1]`, `f[1:]` of `encode_frames`).  Flow task; returns {'flow_preds': [...]}
-        exactly as `forward` does for the images those features were encoded from."""
+        low -> high resolution, e.g. slices `f[:-1]`, `f[1:]` of `encode_frames`).  Returns {'flow_preds': [...]} exactly as
+        `forward` does for the images those features were encoded from (encoded with `encode_frames(..., task)`).
+        Flow and depth.  Depth: `cameras` = `depth_cameras(...)` for these B pairs (then `intrinsics`, `pose` and
+        `num_depth_candidates` are not read, and nothing here synchronises with the host), or `intrinsics` and `pose` as
+        `forward` takes them.  Stereo is not offered: its pairs share no view, so there is no encoding to reuse."""
         if self.training:
             raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
-        if task != "flow":
-            raise ValueError("forward_encoded drives the flow task only (stereo / depth encode both views per pair)")
+        if task not in ("flow", "depth"):
+            raise ValueError("forward_encoded drives the flow and depth tasks only (each stereo pair encodes two distinct views)")
         if len(feats0) != self.num_scales or len(feats1) != self.num_scales:
             raise ValueError("forward_encoded needs one feature map per scale (%d)" % self.num_scales)
-        assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
+        if task == "depth":
+            assert self.num_scales == 1 and not pred_bidir_flow
+            assert len(attn_splits_list) == len(prop_radius_list) == 1
+            B = feats0[0].shape[0]
+            if cameras is None:
+                if intrinsics is None or pose is None:
+                    raise ValueError("forward_encoded(task='depth') needs cameras= or intrinsics= and pose=")
+                cameras = self.depth_cameras(intrinsics, pose, self.upsample_factor, min_depth, max_depth,
+                                             num_depth_candidates, pred_bidir_depth)
+            if cameras["K"].shape[0] != (2 if pred_bidir_depth else 1) * B or cameras["pose"].shape[0] != cameras["K"].shape[0]:
+                raise ValueError("forward_encoded: cameras were built for another batch or pred_bidir_depth setting")
+        else:
+            assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
+            cameras, pred_bidir_depth, depth_from_argmax = None, False, False
         with torch.no_grad():
             return self._forward_encoded(self._prepared(), list(feats0), list(feats1), attn_type, attn_splits_list,
-                                         corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, "flow", None,
-                                         None, None, None, None, False, False)
+                                         corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, cameras,
+                                         min_depth, max_depth, depth_from_argmax, pred_bidir_depth)
 
     def _forward_encoded(self, P, feats0, feats1, attn_type, attn_splits_list, corr_radius_list, prop_radius_list,
-                         num_reg_refine, pred_bidir_flow, task, intrinsics, pose, min_depth, max_depth, num_depth_candidates,
-                         depth_from_argmax, pred_bidir_depth):
-        """The matching path after the encoder (unimatch.py:127-367); feats0 / feats1: per-scale [B,h,w,128] views."""
+                         num_reg_refine, pred_bidir_flow, task, cams, min_depth, max_depth, depth_from_argmax,
+                         pred_bidir_depth):
+        """The matching path after the encoder (unimatch.py:127-367); feats0 / feats1: per-scale [B,h,w,128] views;
+        cams: `depth_cameras` (depth task) or None."""
         flow = None            # [Bp, h, w, fd] channel-last
         preds = []
         for s in range(self.num_scales):
@@ -714,11 +766,6 @@ class UniMatch(nn.Module):
                 f0, f1 = torch.cat((f0, f1), dim=0), torch.cat((f1, f0), dim=0)
             f0_ori, f1_ori = f0, f1
             Bp = f0.shape[0]
-            up = self.upsample_factor * (2 ** (self.num_scales - 1 - s))
-            Ks = None
-            if task == "depth":
-                Ks = intrinsics.clone().float()
-                Ks[:, :2] = Ks[:, :2] / up
             if s > 0:
                 flow = _OPS.upsample2x(flow.contiguous(), 2.0)                    # unimatch.py:154
             splits = attn_splits_list[s]
@@ -729,8 +776,7 @@ class UniMatch(nn.Module):
 
             # ---- correlation + softmax (unimatch.py:186-216) ----
             with self._section("correlation_s%d" % s):
-                dargs = (Ks, pose, min_depth, max_depth, num_depth_candidates, depth_from_argmax, pred_bidir_depth) \
-                    if task == "depth" else None
+                dargs = (cams, depth_from_argmax, pred_bidir_depth) if task == "depth" else None
                 pred = self._stage_correlation(tok, Bp, h, wd, task, None if task == "depth" else corr_radius_list[s],
                                                pred_bidir_flow, dargs)
             flow = flow + pred if flow is not None else pred
@@ -764,12 +810,9 @@ class UniMatch(nn.Module):
             g0, g1 = f0_ori.contiguous(), f1_ori.contiguous()
             drefine = None
             if task == "depth":
-                Kr, pr = Ks, pose
                 if pred_bidir_depth:
-                    Kr = Ks.repeat(2, 1, 1)
-                    pr = torch.cat((pose, torch.inverse(pose)), dim=0).float()
                     g0, g1 = torch.cat((g0, g1), dim=0), torch.cat((g1, g0), dim=0)
-                drefine = (Kr, pr, min_depth, max_depth)
+                drefine = (cams, min_depth, max_depth)
             rst = self._stage_refine_setup(P, feat0.contiguous(), nb, h, wd)
             for it in range(num_reg_refine):
                 last = it == num_reg_refine - 1
