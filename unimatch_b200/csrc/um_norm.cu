@@ -1,5 +1,5 @@
 // InstanceNorm2d (eps 1e-5, no affine, biased variance; backbone.py:7,41) on channel-last fp32 maps, as three
-// bandwidth-bound passes: per-(image, channel) partial sums -> mean / rstd -> fused normalise (+ReLU) (+residual,
+// bandwidth-bound passes: per-(image, channel) pivot-shifted partial sums -> mean / rstd -> fused normalise (+ReLU) (+residual,
 // itself optionally normalised) (+ReLU) writing fp32 and/or the fp16 (hi, lo) planes the tensor-core convolution reads.
 #include "um_common.cuh"
 #include "um_tc.cuh"
@@ -8,7 +8,21 @@ namespace {
 
 constexpr int CHUNKS = 64;
 
-// grid (CHUNKS, N); 256 threads = (C/4 float4 lanes) x row lanes.  partial[n][chunk][2][C]
+// Per-(image, channel) pivot: the fp32 mean of the first min(hw, 16) pixels, summed in pixel order.  The partial sums are
+// of x - pivot, so E[x^2] - mean^2 no longer cancels when |mean| >> std (a channel with |mean| / std = 100 would otherwise
+// lose ~1e-4 of rstd to the fp32 sums).  Both kernels form it with the same instructions, so they agree to the bit.
+__device__ __forceinline__ float4 in_pivot(const float* __restrict__ x, long long ld, int hw, int n, int c4) {
+  const int np = hw < 16 ? hw : 16;
+  float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int r = 0; r < np; ++r) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(x + ((long long)n * hw + r) * ld) + c4);
+    p.x += v.x; p.y += v.y; p.z += v.z; p.w += v.w;
+  }
+  const float inv = 1.0f / (float)np;
+  return make_float4(p.x * inv, p.y * inv, p.z * inv, p.w * inv);
+}
+
+// grid (CHUNKS, N); 256 threads = (C/4 float4 lanes) x row lanes.  partial[n][chunk][2][C]: sums of x - pivot and of its square
 __global__ void __launch_bounds__(256) in_partial_kernel(const float* __restrict__ x, long long ld, int hw, int C,
                                                          float* __restrict__ partial) {
   extern __shared__ float sm[];                 // [2][rows_per_iter][C]
@@ -19,12 +33,15 @@ __global__ void __launch_bounds__(256) in_partial_kernel(const float* __restrict
   const int rows_per_chunk = (hw + CHUNKS - 1) / CHUNKS;
   const int r0 = chunk * rows_per_chunk, r1 = min(hw, r0 + rows_per_chunk);
   float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (rl < rlanes)
+  if (rl < rlanes) {
+    const float4 pv = in_pivot(x, ld, hw, n, c4);
     for (int r = r0 + rl; r < r1; r += rlanes) {
-      const float4 v = __ldg(reinterpret_cast<const float4*>(x + ((long long)n * hw + r) * ld) + c4);
+      float4 v = __ldg(reinterpret_cast<const float4*>(x + ((long long)n * hw + r) * ld) + c4);
+      v.x -= pv.x; v.y -= pv.y; v.z -= pv.z; v.w -= pv.w;
       s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
       q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
     }
+  }
   float* ss = sm;
   float* qs = sm + rlanes * C;
   if (rl < rlanes) {
@@ -42,19 +59,22 @@ __global__ void __launch_bounds__(256) in_partial_kernel(const float* __restrict
 }
 
 // stats[n][0][c] = mean, stats[n][1][c] = rstd; final combination in double
-__global__ void in_finalize_kernel(const float* __restrict__ partial, float* __restrict__ stats, int hw, int C, int total) {
+__global__ void in_finalize_kernel(const float* __restrict__ x, long long ld, const float* __restrict__ partial,
+                                   float* __restrict__ stats, int hw, int C, int total) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const int n = i / C, c = i - n * C;
+  const float4 pv = in_pivot(x, ld, hw, n, c >> 2);
+  const float piv = (c & 3) == 0 ? pv.x : (c & 3) == 1 ? pv.y : (c & 3) == 2 ? pv.z : pv.w;
   double s = 0.0, q = 0.0;
   for (int k = 0; k < CHUNKS; ++k) {
     const float* p = partial + (((long long)n * CHUNKS + k) * 2) * C;
     s += (double)p[c]; q += (double)p[C + c];
   }
-  const double mean = s / hw;
-  double var = q / hw - mean * mean;
+  const double dm = s / hw;                      // mean - pivot
+  double var = q / hw - dm * dm;
   if (var < 0.0) var = 0.0;
-  stats[((long long)n * 2) * C + c] = (float)mean;
+  stats[((long long)n * 2) * C + c] = (float)((double)piv + dm);
   stats[((long long)n * 2 + 1) * C + c] = (float)(1.0 / sqrt(var + 1e-5));
 }
 
@@ -124,7 +144,7 @@ int um_instance_norm_stats(const float* x, int64_t ld, int32_t n, int32_t hw, in
   int rc = um::check_launch("um_instance_norm_stats(partial)");
   if (rc) return rc;
   const int total = n * c;
-  in_finalize_kernel<<<(total + 127) / 128, 128, 0, st>>>(scratch, stats, hw, c, total);
+  in_finalize_kernel<<<(total + 127) / 128, 128, 0, st>>>(x, ld, scratch, stats, hw, c, total);
   return um::check_launch("um_instance_norm_stats(finalize)");
 }
 
