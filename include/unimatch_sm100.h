@@ -30,6 +30,7 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info. */
+#define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
 const char* um_last_error(void);
@@ -69,9 +70,6 @@ int um_window_attention(const float* q, const float* k, const float* v, float* o
  * window-major operand planes (0 = this geometry runs on CUDA cores and needs none).  flags: */
 #define UM_ATTN_FORCE_CUDA_CORES 1   /* diagnostic: use the exact-fp32 CUDA-core kernel for every shape */
 int64_t um_window_attention_workspace(const um_attn_geom* geom, int32_t n_streams);
-/* Diagnostic: device buffer (>= 128*64 + 128*128 floats) that receives the raw S tile and the un-normalised O tile
- * of CTA (0,0,0) of the next tensor-core attention launches; NULL disables. */
-void um_debug_set_dump(float* device_buffer);
 
 /* The same attention on operands that are ALREADY window-major fp16 (hi, lo) planes [2][n_streams][kh*kw][lp][128]
  * (lp = um_attention_planes_lp(geom): the window length rounded up to 128; rows [lw, lp) of every window must be zero):
@@ -159,11 +157,6 @@ int um_depth_corr_softmax(const float* f0, const float* f1, const float* Kmat, c
 int um_add_position(const float* x, const float* table, float* out,
                     int32_t n_streams, int32_t h, int32_t w, int32_t wh, int32_t ww, void* stream);
 
-/* out = residual + LayerNorm(x) * gamma + beta over the last dim (128), eps 1e-5; residual may be NULL.
- * Replaces norm1/norm2 + the residual add of TransformerLayer.forward (transformer.py:137-144). */
-int um_layernorm_residual(const float* x, const float* residual, const float* gamma, const float* beta,
-                          float* out, int64_t rows, int64_t ldx, int64_t ldr, int64_t ldo, void* stream);
-
 /* Convex upsampling: up[b, c, y*F+ky, x*F+kx] = sum_t softmax_t(mask[b,y,x, t*F*F + ky*F + kx]) * mult*flow[b, nb_t, c],
  * 3x3 zero-padded neighbourhood.  mask channel-last [B,h,w,9*F*F]; flow [B,h,w,fd]; up is PLANAR [B, fd, h*F, w*F]
  * (the layout the reference returns).  Replaces upsample_flow_with_mask (utils.py:134-152). */
@@ -210,15 +203,6 @@ int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n,
  * Replaces flow_to_image (utils/flow_viz.py:240-275; called at evaluate_flow.py:768 for videos). */
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
                      int32_t n, int32_t h, int32_t w, void* stream);
-
-/* GRU gate fusions of SepConvGRU (reg_refine.py:37-52): rows of 128 hidden channels, independent row strides
- * (floats, multiples of 4) so the z|r pre-activations may live side by side in one fused conv output.
- *   um_gru_rh:     rh = sigmoid(r_pre) * h
- *   um_gru_update: h_out = (1 - sigmoid(z_pre)) * h + sigmoid(z_pre) * tanh(q_pre)                          */
-int um_gru_rh(const float* r_pre, int64_t ldr, const float* h, int64_t ldh, float* rh, int64_t ldo, int64_t rows,
-              void* stream);
-int um_gru_update(const float* z_pre, int64_t ldz, const float* q_pre, int64_t ldq, const float* h, int64_t ldh,
-                  float* h_out, int64_t ldo, int64_t rows, void* stream);
 
 /* ---- tensor-core implicit-GEMM convolution / Linear layer (fp16 hi/lo split operands, fp32 accumulate) ----------
  * Replaces the nn.Conv2d calls of BasicUpdateBlock (reg_refine.py:6-119), refine_proj (unimatch.py:315) and, as a

@@ -131,11 +131,6 @@ def add_position(x, table, h, w):
     return x + table.repeat(h // wh, w // ww, 1)[None]
 
 
-def layernorm_residual(x, residual, gamma, beta):
-    y = torch.nn.functional.layer_norm(x, (C,), gamma, beta)
-    return y if residual is None else residual + y
-
-
 def convex_upsample(flow, mask, factor, mult):
     return O.convex_upsample(_nchw(flow), _nchw(mask), factor, is_depth=(mult == 1.0))
 
@@ -149,15 +144,6 @@ def resize_bilinear(x, h_out, w_out, scale, flip_x):
     if scale is not None:
         y = y * torch.tensor(list(scale)).view(1, -1, 1, 1)
     return torch.flip(y, dims=[-1]) if flip_x else y
-
-
-def gru_rh(r_pre, h):
-    return torch.sigmoid(r_pre) * h
-
-
-def gru_update(z_pre, q_pre, h):
-    z = torch.sigmoid(z_pre)
-    return (1 - z) * h + z * torch.tanh(q_pre)
 
 
 def split_planes(src, dst, off):
@@ -337,8 +323,7 @@ def ffn_tc(src0, src1, w1, w2, residual, gamma, beta, out_f32, out_split, rows):
 
 
 ALL = ["split_planes", "conv7x7_small", "conv2d_tc", "ffn_tc", "instance_norm_stats", "instance_norm_apply", "window_attention", "window_attention_planes", "softmax_expectation", "local_corr_softmax", "local_corr_volume", "flow_warp", "fb_consistency",
-       "propagate_local", "depth_corr_softmax", "add_position", "layernorm_residual", "convex_upsample", "upsample2x", "resize_bilinear",
-       "gru_rh", "gru_update"]
+       "propagate_local", "depth_corr_softmax", "add_position", "convex_upsample", "upsample2x", "resize_bilinear"]
 
 _registered = []
 

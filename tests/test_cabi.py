@@ -23,10 +23,14 @@ def test_header_symbols_exported():
     assert sorted(ops.SYMBOLS) == names
 
 
-def test_abi_version_and_build_info():
-    assert ops.LIB.um_abi_version() == 3
+def test_abi_version_matches_header_and_build_info():
+    text = open(os.path.join(ROOT, "include", "unimatch_sm100.h")).read()
+    declared = int(re.search(r"#define UM_ABI_VERSION (\d+)", text).group(1))
+    assert declared == 4
+    assert ops.LIB.um_abi_version() == declared
     info = ops.build_info()
     assert "sm_90a" in info
+    assert "abi=%d " % declared in info
 
 
 def test_bad_arguments_are_reported_without_a_gpu():

@@ -163,17 +163,6 @@ def test_sine_table_is_the_reference_encoding():
     assert (ref - _sine_table(5, 7)).abs().max().item() <= 1e-6
 
 
-@pytest.mark.parametrize("with_res", [False, True])
-def test_layernorm_residual(with_res):
-    gen = g(900)
-    x = torch.randn((2, 37, C), generator=gen) * 3 + 0.5
-    res = torch.randn((2, 37, C), generator=gen) if with_res else None
-    gamma, beta = torch.randn(C, generator=gen), torch.randn(C, generator=gen)
-    ref = refops.layernorm_residual(x, res, gamma, beta)
-    got = OPS.layernorm_residual(x.cuda(), None if res is None else res.cuda(), gamma.cuda(), beta.cuda())
-    close(got, ref, 1e-5)
-
-
 @pytest.mark.parametrize("fd,factor,mult", [(2, 4, 4.0), (2, 8, 8.0), (2, 8, 1.0)])
 def test_convex_upsample(fd, factor, mult):
     gen = g(1000 + factor)
@@ -186,16 +175,6 @@ def test_convex_upsample(fd, factor, mult):
 def test_upsample2x(fd):
     flow = torch.randn((2, 7, 9, fd), generator=g(1100)) * 5
     close(OPS.upsample2x(flow.cuda(), 2.0), refops.upsample2x(flow, 2.0), 1e-5)
-
-
-def test_gru_gates():
-    gen = g(1200)
-    zr = torch.randn((2, 5, 6, 256), generator=gen) * 2
-    q = torch.randn((2, 5, 6, C), generator=gen) * 2
-    h = torch.tanh(torch.randn((2, 5, 6, C), generator=gen))
-    d = zr.cuda()
-    close(OPS.gru_rh(d[..., 128:], h.cuda()), refops.gru_rh(zr[..., 128:], h), 1e-5)
-    close(OPS.gru_update(d[..., :128], q.cuda(), h.cuda()), refops.gru_update(zr[..., :128], q, h), 1e-5)
 
 
 CONV_CASES = [

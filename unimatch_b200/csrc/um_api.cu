@@ -22,21 +22,19 @@ void set_error(const char* fmt, ...) {
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
 int window_attention_simt(const float* q, const float* k, const float* v, float* out, int n_streams, int kv_shift,
-                          long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, int m_begin,
-                          cudaStream_t st);
+                          long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, cudaStream_t st);
 bool attention_tc_supported(const Geom& g);
 size_t attention_tc_workspace_bytes(const Geom& g, int n_streams);
 int window_attention_tc(const float* q, const float* k, const float* v, float* out, int n_streams, int kv_shift,
                         long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, void* workspace,
-                        float* dbg, cudaStream_t st, int* rows_done);
+                        cudaStream_t st);
 int attention_planes_launch(const __half* wq, const __half* wk, const __half* wv, float* out, long long ldo, __half* out_split,
-                            long long split_plane, int n_streams, int kv_shift, const Geom& g, float* dbg, cudaStream_t st);
+                            long long split_plane, int n_streams, int kv_shift, const Geom& g, cudaStream_t st);
 bool expectation_tc_supported(const Geom& g, int value_mode);
 size_t expectation_tc_workspace_bytes(const Geom& g, int n_total);
 int softmax_expectation_tc(const float* q, const float* k, const float* values, float* out, int n_streams, int n_total,
                            int kv_shift, long long ldq, long long ldk, int vdim, int value_mode, int post_op,
                            const Geom& g, void* workspace, cudaStream_t st);
-static float* g_dump = nullptr;
 int softmax_expectation_simt(const float* q, const float* k, const float* values, float* out, int n_streams,
                              int n_total, int kv_shift, long long ldq, long long ldk, int vdim, int value_mode,
                              int post_op, const Geom& g, cudaStream_t st);
@@ -45,10 +43,11 @@ int softmax_expectation_simt(const float* q, const float* k, const float* values
 
 extern "C" {
 
-int um_abi_version(void) { return 3; }
+int um_abi_version(void) { return UM_ABI_VERSION; }
 
 const char* um_build_info(void) {
-  return "libunimatch_sm100 abi=2 arch=sm_90a cuda=" UM_STR(CUDART_VERSION) " built " __DATE__ " " __TIME__;
+  return "libunimatch_sm100 abi=" UM_STR(UM_ABI_VERSION) " arch=sm_90a cuda=" UM_STR(CUDART_VERSION) " built " __DATE__ " "
+         __TIME__;
 }
 
 const char* um_last_error(void) { return um::g_err; }
@@ -60,8 +59,6 @@ int64_t um_window_attention_workspace(const um_attn_geom* geom, int32_t n_stream
   if (!um::make_geom(geom, &g) || n_streams <= 0 || !um::attention_tc_supported(g)) return 0;
   return (int64_t)um::attention_tc_workspace_bytes(g, n_streams);
 }
-
-void um_debug_set_dump(float* device_buffer) { um::g_dump = device_buffer; }
 
 int32_t um_attention_planes_lp(const um_attn_geom* geom) {
   um::Geom g;
@@ -87,7 +84,7 @@ int um_window_attention_planes(const void* q_planes, const void* k_planes, const
              "um_window_attention_planes: planes must be 16-byte aligned");
   return um::attention_planes_launch(reinterpret_cast<const __half*>(q_planes), reinterpret_cast<const __half*>(k_planes),
                                      reinterpret_cast<const __half*>(v_planes), out, ldo, reinterpret_cast<__half*>(out_split),
-                                     split_plane_stride, n_streams, kv_shift, g, um::g_dump, (cudaStream_t)stream);
+                                     split_plane_stride, n_streams, kv_shift, g, (cudaStream_t)stream);
 }
 
 int um_window_attention(const float* q, const float* k, const float* v, float* out, int32_t n_streams,
@@ -103,17 +100,13 @@ int um_window_attention(const float* q, const float* k, const float* v, float* o
              "um_window_attention: row strides must be >= 128 and multiples of 4 floats");
   UM_REQUIRE(g.mask_mode >= UM_MASK_NONE && g.mask_mode <= UM_MASK_CAUSAL, "um_window_attention: bad mask_mode");
   cudaStream_t st = (cudaStream_t)stream;
-  int m_begin = 0;
   if (!(flags & UM_ATTN_FORCE_CUDA_CORES) && um::attention_tc_supported(g)) {
     UM_REQUIRE(workspace && workspace_bytes >= (int64_t)um::attention_tc_workspace_bytes(g, n_streams),
                "um_window_attention: workspace too small (%lld bytes needed, see um_window_attention_workspace)",
                (long long)um::attention_tc_workspace_bytes(g, n_streams));
-    int rc = um::window_attention_tc(q, k, v, out, n_streams, kv_shift, ldq, ldk, ldv, ldo, g, workspace, um::g_dump,
-                                     st, &m_begin);
-    if (rc) return rc;
-    if (m_begin >= g.lw) return UM_OK;
+    return um::window_attention_tc(q, k, v, out, n_streams, kv_shift, ldq, ldk, ldv, ldo, g, workspace, st);
   }
-  return um::window_attention_simt(q, k, v, out, n_streams, kv_shift, ldq, ldk, ldv, ldo, g, m_begin, st);
+  return um::window_attention_simt(q, k, v, out, n_streams, kv_shift, ldq, ldk, ldv, ldo, g, st);
 }
 
 int64_t um_softmax_expectation_workspace(const um_attn_geom* geom, int32_t n_total, int32_t value_mode) {

@@ -27,7 +27,7 @@ constexpr float SQRT_C = 11.313708498984761f;   // 128 ** 0.5
 struct Params {
   const float* q; const float* k; const float* v; float* out;
   long long ldq, ldk, ldv, ldo;
-  int n_total, kv_shift, m_begin;
+  int n_total, kv_shift;
   um::Geom g;
   const float* values; int vdim, value_mode, post_op;
 };
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(NT) attn_simt_kernel(Params p) {
   const int win = blockIdx.y, n = blockIdx.z;
   const int nk = (n + p.kv_shift) % p.n_total;
   const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  const int m0 = p.m_begin + blockIdx.x * BM;
+  const int m0 = blockIdx.x * BM;
   const long long L = (long long)g.h * g.w;
 
   if (tid < BM) {
@@ -252,7 +252,7 @@ template <bool FEAT>
 int launch(const Params& p, int n_streams, cudaStream_t st) {
   static um::PerDeviceBytes configured;
   if (int rc = um::ensure_smem(configured, attn_simt_kernel<FEAT>, smem_bytes<FEAT>(), "attn_simt")) return rc;
-  dim3 grid((p.g.lw - p.m_begin + BM - 1) / BM, p.g.nwin, n_streams);
+  dim3 grid((p.g.lw + BM - 1) / BM, p.g.nwin, n_streams);
   attn_simt_kernel<FEAT><<<grid, NT, smem_bytes<FEAT>(), st>>>(p);
   return um::check_launch(FEAT ? "um_window_attention(simt)" : "um_softmax_expectation(simt)");
 }
@@ -262,12 +262,11 @@ int launch(const Params& p, int n_streams, cudaStream_t st) {
 namespace um {
 
 int window_attention_simt(const float* q, const float* k, const float* v, float* out, int n_streams, int kv_shift,
-                          long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, int m_begin,
-                          cudaStream_t st) {
+                          long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, cudaStream_t st) {
   Params p{};
   p.q = q; p.k = k; p.v = v; p.out = out;
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.ldo = ldo;
-  p.n_total = n_streams; p.kv_shift = kv_shift; p.g = g; p.m_begin = m_begin;
+  p.n_total = n_streams; p.kv_shift = kv_shift; p.g = g;
   return launch<true>(p, n_streams, st);
 }
 

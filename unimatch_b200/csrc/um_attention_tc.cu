@@ -54,7 +54,6 @@ struct TcParams {
   Geom g;
   // softmax-expectation variant (HAS_V = false): out[n, t, 0..vdim) = post(sum_k p_k value_k)
   const float* values; int vdim, value_mode, post_op;
-  float* dbg;          // optional: raw S of the first key tile [128 x 64] then un-normalised O [128 x 128] of CTA (0,0,0)
   // optional second output: the same rows as fp16 (hi, lo) planes [2][rows][128] (token order), i.e. the operand planes of the
   // merge Linear layer -- saves the separate fp32 -> planes pass
   __half* out_split; long long split_plane;
@@ -277,15 +276,11 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
   float o[64];                                              // O: 64 rows x 128 channels of this warpgroup
 #pragma unroll
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
-  const bool dump = p.dbg && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
   for (int j = 0; j < T; ++j) {
     const int s = j & 1;
     const int n0 = j * BN;
     float sv[32];
     compute_s(j, sv);
-    if (dump && j == 0)
-#pragma unroll
-      for (int i = 0; i < 32; ++i) p.dbg[(fr + 8 * ((i >> 1) & 1)) * BN + 8 * (i >> 2) + fc + (i & 1)] = sv[i];
     uint32_t ph[16], pl[16];                                // P as fp16 (hi, lo) pairs, already in the A-operand layout
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -358,7 +353,6 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int row = fr + 8 * h, col = 8 * jj + fc;
-      if (dump) { p.dbg[BM * BN + row * 128 + col] = o[4 * jj + 2 * h]; p.dbg[BM * BN + row * 128 + col + 1] = o[4 * jj + 2 * h + 1]; }
       *reinterpret_cast<float2*>(osm + row * 128 + (((col >> 2) ^ (row & 31)) << 2) + (col & 3)) =
           make_float2(o[4 * jj + 2 * h] * inv[h], o[4 * jj + 2 * h + 1] * inv[h]);
     }
@@ -477,7 +471,7 @@ int split_windows_launch(const float* q, const float* k, const float* v, long lo
 // the fused attention kernel on window-major operand planes [2][n_streams][nwin][lp][128] (one buffer per operand)
 
 int attention_planes_launch(const __half* wq, const __half* wk, const __half* wv, float* out, long long ldo, __half* out_split,
-                               long long split_plane, int n_streams, int kv_shift, const Geom& g, float* dbg, cudaStream_t st) {
+                               long long split_plane, int n_streams, int kv_shift, const Geom& g, cudaStream_t st) {
   const int lp = padded_lw(g.lw);
   int rc;
   CUtensorMap mq, mk, mv;
@@ -488,17 +482,17 @@ int attention_planes_launch(const __half* wq, const __half* wk, const __half* wv
   static PerDeviceBytes configured;
   if ((rc = ensure_smem(configured, attn_tc_kernel<true>, SMEM_BYTES, "attn_tc"))) return rc;
   TcParams p{};
-  p.out = out; p.ldo = ldo; p.n_streams = n_streams; p.kv_shift = kv_shift; p.lp = lp; p.g = g; p.dbg = dbg;
+  p.out = out; p.ldo = ldo; p.n_streams = n_streams; p.kv_shift = kv_shift; p.lp = lp; p.g = g;
   p.out_split = out_split; p.split_plane = split_plane;
   const int qtiles = (g.lw + BM - 1) / BM;                  // the ragged last tile is masked in the epilogue
   attn_tc_kernel<true><<<dim3(qtiles, g.nwin, n_streams), NTHREADS, SMEM_BYTES, st>>>(mq, mk, mv, p);
   return check_launch("um_window_attention(wgmma)");
 }
 
-// fp32 token rows in: split pass + kernel.  Returns the number of query rows per window that were handled.
+// fp32 token rows in: split pass + kernel
 int window_attention_tc(const float* q, const float* k, const float* v, float* out, int n_streams, int kv_shift,
                         long long ldq, long long ldk, long long ldv, long long ldo, const Geom& g, void* workspace,
-                        float* dbg, cudaStream_t st, int* rows_done) {
+                        cudaStream_t st) {
   const int lp = padded_lw(g.lw);
   const size_t plane_elems = (size_t)2 * n_streams * g.nwin * lp * 128;
   __half* wq = reinterpret_cast<__half*>(workspace);
@@ -506,8 +500,7 @@ int window_attention_tc(const float* q, const float* k, const float* v, float* o
   __half* wv = wk + plane_elems;
   int rc = split_windows_launch(q, k, v, ldq, ldk, ldv, wq, wk, wv, n_streams, g, st, "um_window_attention(split)");
   if (rc) return rc;
-  *rows_done = g.lw;
-  return attention_planes_launch(wq, wk, wv, out, ldo, nullptr, 0, n_streams, kv_shift, g, dbg, st);
+  return attention_planes_launch(wq, wk, wv, out, ldo, nullptr, 0, n_streams, kv_shift, g, st);
 }
 
 int softmax_expectation_tc(const float* q, const float* k, const float* values, float* out, int n_streams, int n_total,
@@ -526,7 +519,7 @@ int softmax_expectation_tc(const float* q, const float* k, const float* values, 
   static PerDeviceBytes configured;
   if ((rc = ensure_smem(configured, attn_tc_kernel<false>, SMEM_BYTES, "expect_tc"))) return rc;
   TcParams p{};
-  p.out = out; p.ldo = vdim; p.n_streams = n_total; p.kv_shift = kv_shift; p.lp = lp; p.g = g; p.dbg = nullptr;
+  p.out = out; p.ldo = vdim; p.n_streams = n_total; p.kv_shift = kv_shift; p.lp = lp; p.g = g;
   p.values = values; p.vdim = vdim; p.value_mode = value_mode; p.post_op = post_op;
   const int qtiles = (g.lw + BM - 1) / BM;
   attn_tc_kernel<false><<<dim3(qtiles, g.nwin, n_streams), NTHREADS, SMEM_BYTES, st>>>(mq, mk, mk, p);

@@ -1,5 +1,5 @@
-// Small fused glue kernels on the matching path: position add, LayerNorm(+residual), convex upsampling,
-// x2 bilinear flow upsampling, GRU gate math.  All channel-last, all bandwidth-bound, all vectorised (float4).
+// Small fused glue kernels on the matching path: position add, convex upsampling, x2 bilinear flow upsampling.
+// All channel-last, all bandwidth-bound, all vectorised (float4).
 #include "um_common.cuh"
 
 namespace {
@@ -20,32 +20,6 @@ __global__ void __launch_bounds__(256) add_position_kernel(const float4* __restr
     v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
     out[i] = v;
   }
-}
-
-// ---- LayerNorm over 128 channels + residual (transformer.py:137-144): one warp per row -------------------
-__global__ void __launch_bounds__(256) layernorm_residual_kernel(const float* __restrict__ x, const float* __restrict__ res,
-                                                                 const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                                 float* __restrict__ out, long long rows, long long ldx,
-                                                                 long long ldr, long long ldo) {
-  const int lane = threadIdx.x & 31;
-  const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
-  if (row >= rows) return;
-  const float4 v = __ldg(reinterpret_cast<const float4*>(x + row * ldx) + lane);
-  float s = (v.x + v.y) + (v.z + v.w);
-  s = um::warp_sum(s);
-  const float mean = s * (1.0f / 128.0f);
-  const float dx = v.x - mean, dy = v.y - mean, dz = v.z - mean, dw = v.w - mean;
-  float q = (dx * dx + dy * dy) + (dz * dz + dw * dw);
-  q = um::warp_sum(q);
-  const float rstd = rsqrtf(q * (1.0f / 128.0f) + 1e-5f);
-  const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + lane);
-  const float4 b = __ldg(reinterpret_cast<const float4*>(beta) + lane);
-  float4 o = make_float4(dx * rstd * g.x + b.x, dy * rstd * g.y + b.y, dz * rstd * g.z + b.z, dw * rstd * g.w + b.w);
-  if (res) {
-    const float4 r = __ldg(reinterpret_cast<const float4*>(res + row * ldr) + lane);
-    o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
-  }
-  reinterpret_cast<float4*>(out + row * ldo)[lane] = o;
 }
 
 // ---- convex upsampling (utils.py:134-152) ---------------------------------------------------------------
@@ -278,43 +252,6 @@ __global__ void __launch_bounds__(256) flow_color_kernel(const float* __restrict
   }
 }
 
-// ---- SepConvGRU gate math (reg_refine.py:37-52) -------------------------------------------------------------
-__device__ __forceinline__ float sigmoidf(float x) { return 1.0f / (1.0f + expf(-x)); }
-
-// rows of 128 channels with independent row strides (the z|r pre-activations come out of one fused conv)
-__global__ void __launch_bounds__(256) gru_rh_kernel(const float* __restrict__ r, long long ldr, const float* __restrict__ hh,
-                                                     long long ldh, float* __restrict__ rh, long long ldo, long long rows) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < rows * 32; i += stride) {
-    const long long row = i >> 5; const int c4 = (int)(i & 31);
-    const float4 a = __ldg(reinterpret_cast<const float4*>(r + row * ldr) + c4);
-    const float4 b = __ldg(reinterpret_cast<const float4*>(hh + row * ldh) + c4);
-    reinterpret_cast<float4*>(rh + row * ldo)[c4] =
-        make_float4(sigmoidf(a.x) * b.x, sigmoidf(a.y) * b.y, sigmoidf(a.z) * b.z, sigmoidf(a.w) * b.w);
-  }
-}
-
-__device__ __forceinline__ float gru_mix(float z, float q, float h) {
-  const float s = sigmoidf(z);
-  return (1.0f - s) * h + s * tanhf(q);
-}
-
-__global__ void __launch_bounds__(256) gru_update_kernel(const float* __restrict__ z, long long ldz, const float* __restrict__ q,
-                                                         long long ldq, const float* __restrict__ hh, long long ldh,
-                                                         float* __restrict__ out, long long ldo, long long rows) {
-  long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  for (; i < rows * 32; i += stride) {
-    const long long row = i >> 5; const int c4 = (int)(i & 31);
-    const float4 a = __ldg(reinterpret_cast<const float4*>(z + row * ldz) + c4);
-    const float4 b = __ldg(reinterpret_cast<const float4*>(q + row * ldq) + c4);
-    const float4 c = __ldg(reinterpret_cast<const float4*>(hh + row * ldh) + c4);
-    reinterpret_cast<float4*>(out + row * ldo)[c4] =
-        make_float4(gru_mix(a.x, b.x, c.x), gru_mix(a.y, b.y, c.y), gru_mix(a.z, b.z, c.z), gru_mix(a.w, b.w, c.w));
-  }
-}
-
 inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
   const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
@@ -334,15 +271,6 @@ int um_add_position(const float* x, const float* table, float* out, int32_t n_st
       reinterpret_cast<const float4*>(x), reinterpret_cast<const float4*>(table), reinterpret_cast<float4*>(out), h, w,
       wh, ww, total4);
   return um::check_launch("um_add_position");
-}
-
-int um_layernorm_residual(const float* x, const float* residual, const float* gamma, const float* beta, float* out,
-                          int64_t rows, int64_t ldx, int64_t ldr, int64_t ldo, void* stream) {
-  UM_REQUIRE(x && gamma && beta && out && rows > 0, "um_layernorm_residual: bad arguments");
-  UM_REQUIRE(ldx % 4 == 0 && ldo % 4 == 0 && (!residual || ldr % 4 == 0), "um_layernorm_residual: strides must be multiples of 4");
-  layernorm_residual_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, (cudaStream_t)stream>>>(x, residual, gamma, beta, out,
-                                                                                         rows, ldx, ldr, ldo);
-  return um::check_launch("um_layernorm_residual");
 }
 
 int um_convex_upsample(const float* flow, const float* mask, float* up, int32_t batch, int32_t h, int32_t w,
@@ -412,21 +340,6 @@ int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_
   flow_color_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(flow, reinterpret_cast<const unsigned*>(max_scratch), out, w,
                                                                      hw, row_stride, image_stride, total);
   return um::check_launch("um_flow_to_image");
-}
-
-int um_gru_rh(const float* r_pre, int64_t ldr, const float* h, int64_t ldh, float* rh, int64_t ldo, int64_t rows,
-              void* stream) {
-  UM_REQUIRE(r_pre && h && rh && rows > 0 && ldr % 4 == 0 && ldh % 4 == 0 && ldo % 4 == 0, "um_gru_rh: bad arguments");
-  gru_rh_kernel<<<ew_grid(rows * 32), 256, 0, (cudaStream_t)stream>>>(r_pre, ldr, h, ldh, rh, ldo, rows);
-  return um::check_launch("um_gru_rh");
-}
-
-int um_gru_update(const float* z_pre, int64_t ldz, const float* q_pre, int64_t ldq, const float* h, int64_t ldh,
-                  float* h_out, int64_t ldo, int64_t rows, void* stream) {
-  UM_REQUIRE(z_pre && q_pre && h && h_out && rows > 0 && ldz % 4 == 0 && ldq % 4 == 0 && ldh % 4 == 0 && ldo % 4 == 0,
-             "um_gru_update: bad arguments");
-  gru_update_kernel<<<ew_grid(rows * 32), 256, 0, (cudaStream_t)stream>>>(z_pre, ldz, q_pre, ldq, h, ldh, h_out, ldo, rows);
-  return um::check_launch("um_gru_update");
 }
 
 }  // extern "C"

@@ -13,15 +13,6 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libunimatch_sm100.so")
 
-# every symbol include/unimatch_sm100.h declares (checked by tests/test_cabi.py)
-SYMBOLS = [
-    "um_abi_version", "um_build_info", "um_last_error", "um_launch_count",
-    "um_window_attention", "um_window_attention_workspace", "um_attention_planes_lp", "um_window_attention_planes", "um_debug_set_dump", "um_softmax_expectation", "um_softmax_expectation_workspace",
-    "um_local_corr_softmax", "um_local_corr_volume", "um_flow_warp", "um_fb_consistency", "um_propagate_local", "um_depth_corr_softmax",
-    "um_conv2d_tc", "um_ffn_tc", "um_conv7x7_small", "um_split_planes", "um_instance_norm_scratch_floats", "um_instance_norm_stats", "um_instance_norm_apply", "um_add_position", "um_layernorm_residual", "um_convex_upsample", "um_upsample2x", "um_resize_bilinear", "um_gru_rh", "um_gru_update",
-    "um_frames_to_planar", "um_flow_to_image", "um_frames_to_planar_normalized",
-]
-
 MASK_NONE, MASK_SWIN, MASK_CAUSAL = 0, 1, 2
 VALUE_TENSOR, VALUE_COORDS, VALUE_XCOORD = 0, 1, 2
 POST_NONE, POST_MINUS_OWN, POST_OWN_MINUS = 0, 1, 2
@@ -70,6 +61,45 @@ class FfnDesc(ctypes.Structure):
                 ("split_plane_stride", ctypes.c_int64)]
 
 
+_P, _I, _L, _F = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
+_G, _FP, _RC = ctypes.POINTER(AttnGeom), ctypes.POINTER(ctypes.c_float), ctypes.c_int
+
+# name -> (restype, argtypes) of every function include/unimatch_sm100.h declares
+_SIGNATURES = {
+    "um_abi_version": (_RC, []),
+    "um_build_info": (ctypes.c_char_p, []),
+    "um_last_error": (ctypes.c_char_p, []),
+    "um_launch_count": (_L, []),
+    "um_window_attention": (_RC, [_P, _P, _P, _P, _I, _I, _L, _L, _L, _L, _G, _P, _L, _I, _P]),
+    "um_window_attention_workspace": (_L, [_G, _I]),
+    "um_attention_planes_lp": (_I, [_G]),
+    "um_window_attention_planes": (_RC, [_P, _P, _P, _P, _L, _P, _L, _I, _I, _G, _P]),
+    "um_softmax_expectation": (_RC, [_P, _P, _P, _P, _I, _I, _I, _L, _L, _I, _I, _I, _G, _P, _L, _I, _P]),
+    "um_softmax_expectation_workspace": (_L, [_G, _I, _I]),
+    "um_local_corr_softmax": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "um_local_corr_volume": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "um_flow_warp": (_RC, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    "um_fb_consistency": (_RC, [_P, _P, _F, _F, _P, _P, _I, _I, _I, _P]),
+    "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
+    "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "um_convex_upsample": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    "um_upsample2x": (_RC, [_P, _P, _I, _I, _I, _I, _F, _P]),
+    "um_resize_bilinear": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _FP, _I, _P]),
+    "um_frames_to_planar": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
+    "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
+    "um_ffn_tc": (_RC, [ctypes.POINTER(FfnDesc), _P]),
+    "um_conv7x7_small": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _FP, _FP, _P, _L, _P, _I, _P]),
+    "um_instance_norm_scratch_floats": (_L, [_I, _I]),
+    "um_instance_norm_stats": (_RC, [_P, _L, _I, _I, _I, _P, _P, _P]),
+    "um_instance_norm_apply": (_RC, [_P, _L, _P, _I, _P, _L, _P, _I, _P, _L, _P, _I, _I, _I, _I, _I, _P]),
+    "um_split_planes": (_RC, [_P, _L, _I, _L, _P, _I, _I, _L, _P]),
+}
+SYMBOLS = list(_SIGNATURES)
+
+
 def _load():
     from .csrc.build import build, have_nvcc
     if have_nvcc():
@@ -80,64 +110,9 @@ def _load():
     missing = [s for s in SYMBOLS if not hasattr(lib, s)]
     if missing:
         raise ImportError("libunimatch_sm100.so lacks symbols %s (stale build? run python unimatch_b200/csrc/build.py --force)" % missing)
-    lib.um_build_info.restype = ctypes.c_char_p
-    lib.um_last_error.restype = ctypes.c_char_p
-    lib.um_launch_count.restype = ctypes.c_int64
-    P, I, L, F = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
-    G = ctypes.POINTER(AttnGeom)
-    sig = {
-        "um_window_attention": [P, P, P, P, I, I, L, L, L, L, G, P, L, I, P],
-        "um_softmax_expectation": [P, P, P, P, I, I, I, L, L, I, I, I, G, P, L, I, P],
-        "um_local_corr_softmax": [P, P, P, I, I, I, I, I, I, P],
-        "um_local_corr_volume": [P, P, P, P, I, I, I, I, I, P],
-        "um_flow_warp": [P, P, P, I, I, I, I, P],
-        "um_fb_consistency": [P, P, F, F, P, P, I, I, I, P],
-        "um_propagate_local": [P, P, P, P, I, I, I, I, I, L, L, P],
-        "um_depth_corr_softmax": [P, P, P, P, P, P, P, I, I, I, I, I, P],
-        "um_add_position": [P, P, P, I, I, I, I, I, P],
-        "um_layernorm_residual": [P, P, P, P, P, L, L, L, L, P],
-        "um_convex_upsample": [P, P, P, I, I, I, I, I, F, P],
-        "um_upsample2x": [P, P, I, I, I, I, F, P],
-        "um_gru_rh": [P, L, P, L, P, L, L, P],
-        "um_gru_update": [P, L, P, L, P, L, P, L, L, P],
-    }
-    lib.um_window_attention_workspace.argtypes = [G, I]
-    lib.um_window_attention_workspace.restype = ctypes.c_int64
-    lib.um_softmax_expectation_workspace.argtypes = [G, I, I]
-    lib.um_softmax_expectation_workspace.restype = ctypes.c_int64
-    lib.um_conv2d_tc.argtypes = [ctypes.POINTER(ConvDesc), P]
-    lib.um_conv2d_tc.restype = ctypes.c_int
-    lib.um_ffn_tc.argtypes = [ctypes.POINTER(FfnDesc), P]
-    lib.um_ffn_tc.restype = ctypes.c_int
-    lib.um_split_planes.argtypes = [P, L, I, L, P, I, I, L, P]
-    lib.um_attention_planes_lp.argtypes = [G]
-    lib.um_attention_planes_lp.restype = ctypes.c_int32
-    lib.um_window_attention_planes.argtypes = [P, P, P, P, L, P, L, I, I, G, P]
-    lib.um_window_attention_planes.restype = ctypes.c_int
-    lib.um_split_planes.restype = ctypes.c_int
-    FP = ctypes.POINTER(ctypes.c_float)
-    lib.um_conv7x7_small.argtypes = [P, P, I, I, I, I, I, I, I, P, P, I, I, FP, FP, P, L, P, I, P]
-    lib.um_conv7x7_small.restype = ctypes.c_int
-    lib.um_instance_norm_scratch_floats.argtypes = [I, I]
-    lib.um_instance_norm_scratch_floats.restype = ctypes.c_int64
-    lib.um_instance_norm_stats.argtypes = [P, L, I, I, I, P, P, P]
-    lib.um_instance_norm_stats.restype = ctypes.c_int
-    lib.um_instance_norm_apply.argtypes = [P, L, P, I, P, L, P, I, P, L, P, I, I, I, I, I, P]
-    lib.um_instance_norm_apply.restype = ctypes.c_int
-    lib.um_resize_bilinear.argtypes = [P, P, I, I, I, I, I, I, FP, I, P]
-    lib.um_resize_bilinear.restype = ctypes.c_int
-    lib.um_frames_to_planar.argtypes = [P, P, I, I, I, I, I, I, P]
-    lib.um_frames_to_planar.restype = ctypes.c_int
-    lib.um_frames_to_planar_normalized.argtypes = [P, P, I, I, I, I, I, FP, FP, P]
-    lib.um_frames_to_planar_normalized.restype = ctypes.c_int
-    lib.um_flow_to_image.argtypes = [P, P, L, L, P, I, I, I, P]
-    lib.um_flow_to_image.restype = ctypes.c_int
-    lib.um_debug_set_dump.argtypes = [P]
-    lib.um_debug_set_dump.restype = None
-    for name, argtypes in sig.items():
+    for name, (restype, argtypes) in _SIGNATURES.items():
         fn = getattr(lib, name)
-        fn.argtypes = argtypes
-        fn.restype = ctypes.c_int
+        fn.restype, fn.argtypes = restype, argtypes
     return lib
 
 
@@ -369,27 +344,6 @@ def _add_position(x, table, h, w):
 add_position = _define("add_position(Tensor x, Tensor table, int h, int w) -> Tensor", _add_position)
 
 
-def _layernorm_residual(x, residual, gamma, beta):
-    _f32c(x, "x", rows_ok=True), _f32c(gamma, "gamma"), _f32c(beta, "beta")
-    if x.shape[-1] != 128:
-        raise RuntimeError("layernorm_residual: expected rows of 128 channels")
-    x2 = x.flatten(0, -2)
-    rows = x2.shape[0]
-    out = torch.empty((rows, 128), device=x.device, dtype=torch.float32)
-    ldr, r2 = 0, None
-    if residual is not None:
-        _f32c(residual, "residual", rows_ok=True)
-        r2 = residual.flatten(0, -2)
-        ldr = r2.stride(0)
-    _check(LIB.um_layernorm_residual(_p(x2), _p(r2), _p(gamma), _p(beta), _p(out), rows, x2.stride(0), ldr, 128,
-                                     _stream()), "um_layernorm_residual")
-    return out.view(x.shape)
-
-
-layernorm_residual = _define("layernorm_residual(Tensor x, Tensor? residual, Tensor gamma, Tensor beta) -> Tensor",
-                             _layernorm_residual)
-
-
 def _convex_upsample(flow, mask, factor, mult):
     _f32c(flow, "flow"), _f32c(mask, "mask")
     b, h, w, fd = flow.shape
@@ -476,32 +430,6 @@ def _flow_to_image(flow, out):
 flow_to_image = _define("flow_to_image(Tensor flow, Tensor(a!) out) -> ()", _flow_to_image)
 
 
-def _gru_rh(r_pre, h):
-    _f32c(r_pre, "r_pre", rows_ok=True), _f32c(h, "h", rows_ok=True)
-    r2, h2 = r_pre.flatten(0, -2), h.flatten(0, -2)
-    rows = h2.shape[0]
-    out = torch.empty((rows, 128), device=h.device, dtype=torch.float32)
-    _check(LIB.um_gru_rh(_p(r2), r2.stride(0), _p(h2), h2.stride(0), _p(out), 128, rows, _stream()), "um_gru_rh")
-    return out.view(h.shape)
-
-
-gru_rh = _define("gru_rh(Tensor r_pre, Tensor h) -> Tensor", _gru_rh)
-
-
-def _gru_update(z_pre, q_pre, h):
-    for t, n in ((z_pre, "z_pre"), (q_pre, "q_pre"), (h, "h")):
-        _f32c(t, n, rows_ok=True)
-    z2, q2, h2 = z_pre.flatten(0, -2), q_pre.flatten(0, -2), h.flatten(0, -2)
-    rows = h2.shape[0]
-    out = torch.empty((rows, 128), device=h.device, dtype=torch.float32)
-    _check(LIB.um_gru_update(_p(z2), z2.stride(0), _p(q2), q2.stride(0), _p(h2), h2.stride(0), _p(out), 128, rows,
-                             _stream()), "um_gru_update")
-    return out.view(h.shape)
-
-
-gru_update = _define("gru_update(Tensor z_pre, Tensor q_pre, Tensor h) -> Tensor", _gru_update)
-
-
 # ---- tensor-core convolution / Linear ---------------------------------------------------------------------------
 def prep_conv_weight(w, cin_splits, cout_p):
     """[Cout, sum(cin_splits), KH, KW] fp32 -> fp16 planes [2, cout_p, ktot], K ordered (source, tap, ci) with every
@@ -518,9 +446,7 @@ def prep_conv_weight(w, cin_splits, cout_p):
     m = torch.nn.functional.pad(m, (0, 0, 0, cout_p - cout)).float()
     hi = m.half()
     lo = (m - hi.float()).half()
-    out = torch.stack((hi, lo), dim=0).contiguous()
-    out.k_true = int(w.shape[1] * kh * kw)          # real (unpadded) reduction length: algorithmic FLOPs of the layer
-    return out
+    return torch.stack((hi, lo), dim=0).contiguous()
 
 
 def split_buffer(batch, h, w, cp, device):

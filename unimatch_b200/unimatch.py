@@ -22,6 +22,7 @@ oracle's intermediate tensors at the BASELINE shapes (tests/test_stages_gpu.py).
 Inference only (the reference's callers use eval()/no_grad, evaluate_flow.py:19,33); `train()` mode raises.
 """
 import math
+from collections import namedtuple
 from contextlib import contextmanager
 
 import torch
@@ -33,15 +34,23 @@ from .spec import param_spec
 _OPS = torch.ops.unimatch_sm100
 
 
-import os as _os
-_FUSED_FFN = _os.environ.get("UM_FUSED_FFN", "1") != "0"      # A/B switch of the fused FFN kernel (tools / profiling)
+class _Layer(namedtuple("_Layer", "weights bias kh kw pad_h pad_w stride cout bn mode act gamma beta k")):
+    """A tensor-core convolution / Linear layer for um_conv2d_tc: weight planes (`ops.prep_conv_weight`, cout padded to a
+    multiple of the output-channel tile bn), 'same' zero padding, default stride, epilogue (mode, act, LayerNorm gamma / beta)
+    and k = cin * kh * kw, the real (unpadded) reduction length: 2 k FLOPs per output value."""
+    __slots__ = ()
+
+    def out_hw(self, h, w, stride):
+        return (h + 2 * self.pad_h - self.kh) // stride + 1, (w + 2 * self.pad_w - self.kw) // stride + 1
 
 
-def _bn256(b, h, w):
-    """Output-channel tile of the 256-channel update-block convolutions (GRU z|r, flow / mask heads): 128 (the
-    accumulator tile lives in the registers of two warpgroups)."""
-    return 128
-
+def _layer(w, cin_splits, bn, bias=None, act=ops.ACT_NONE, mode=ops.CONV_LINEAR, gamma=None, beta=None, stride=1):
+    """_Layer of the fp32 weight [cout, cin, kh, kw] or [cout, cin] (Linear), input channels from sources of cin_splits."""
+    if w.dim() == 2:
+        w = w[:, :, None, None]
+    cout, cin, kh, kw = w.shape
+    return _Layer(ops.prep_conv_weight(w, cin_splits, (cout + bn - 1) // bn * bn), bias, kh, kw, kh // 2, kw // 2, stride,
+                  cout, bn, mode, act, gamma, beta, cin * kh * kw)
 
 
 class _Node(nn.Module):
@@ -129,14 +138,13 @@ class UniMatch(nn.Module):
 
     # ------------------------------------------------------------------------------------------ weights
     def _prepared(self):
-        """fp16 (hi, lo) weight planes of every layer (`ops.prep_conv_weight`), rebuilt when a parameter changes."""
+        """`_Layer`s of every tensor-core layer, rebuilt when a parameter changes."""
         params = dict(self.named_parameters())
         key = (tuple((p._version, p.data_ptr()) for p in params.values()),)
         if self._prep_key == key:
             return self._prep
         w = {k: v.detach() for k, v in params.items()}
-        prep = ops.prep_conv_weight
-        lin = lambda m: m[:, :, None, None]
+        LN = ops.CONV_LN
         P = {"raw": w, "blocks": []}
         for i in range(self.num_transformer_layers):
             sk, ck = "transformer.layers.%d.self_attn." % i, "transformer.layers.%d.cross_attn_ffn." % i
@@ -144,82 +152,82 @@ class UniMatch(nn.Module):
                               w[ck + "k_proj.weight"], w[ck + "v_proj.weight"]], dim=0)        # [640, 128]
             hid = w[ck + "mlp.0.weight"].shape[0]
             P["blocks"].append(dict(
-                tc_in=prep(lin(w_in), [128], 640),
-                tc_m_s=prep(lin(w[sk + "merge.weight"]), [128], 128), g_s=w[sk + "norm1.weight"], b_s=w[sk + "norm1.bias"],
-                tc_q_c=prep(lin(w[ck + "q_proj.weight"]), [128], 128),
-                tc_m_c=prep(lin(w[ck + "merge.weight"]), [128], 128), g_c1=w[ck + "norm1.weight"], b_c1=w[ck + "norm1.bias"],
-                tc_w1=prep(lin(w[ck + "mlp.0.weight"]), [128, 128], hid),
-                tc_w2=prep(lin(w[ck + "mlp.2.weight"]), [hid], 128), g_c2=w[ck + "norm2.weight"], b_c2=w[ck + "norm2.bias"],
-                hid=hid))
-        P["tcb"] = self._prepare_backbone(w)
+                tc_in=_layer(w_in, [128], 128),
+                tc_m_s=_layer(w[sk + "merge.weight"], [128], 128, mode=LN, gamma=w[sk + "norm1.weight"], beta=w[sk + "norm1.bias"]),
+                tc_q_c=_layer(w[ck + "q_proj.weight"], [128], 128),
+                tc_m_c=_layer(w[ck + "merge.weight"], [128], 128, mode=LN, gamma=w[ck + "norm1.weight"], beta=w[ck + "norm1.bias"]),
+                # the two-launch FFN; the fused FFN kernel reads the same weight planes, gamma and beta
+                tc_w1=_layer(w[ck + "mlp.0.weight"], [128, 128], 256, act=ops.ACT_GELU),
+                tc_w2=_layer(w[ck + "mlp.2.weight"], [hid], 128, mode=LN, gamma=w[ck + "norm2.weight"], beta=w[ck + "norm2.bias"])))
+        P["tcb"] = self._prepare_backbone(w, self.num_scales)
         # SelfAttnPropagation projections (attention.py:177-178, :204-205, :227-232)
         qw, qb = w["feature_flow_attn.q_proj.weight"], w["feature_flow_attn.q_proj.bias"]
         kw, kb = w["feature_flow_attn.k_proj.weight"], w["feature_flow_attn.k_proj.bias"]
-        P["prop_q"] = (prep(lin(qw), [128], 128), qb.contiguous())
-        P["prop_k"] = (prep(lin(kw), [128], 128), kb.contiguous())
-        P["prop_qk"] = (prep(lin(torch.cat([qw, kw], 0)), [128], 256), torch.cat([qb, kb]).contiguous())
+        P["prop_q"] = _layer(qw, [128], 128, qb.contiguous())
+        P["prop_k"] = _layer(kw, [128], 128, kb.contiguous())
+        P["prop_qk"] = _layer(torch.cat([qw, kw], 0), [128], 128, torch.cat([qb, kb]).contiguous())
         if self.reg_refine:
             P["tc"] = self._prepare_refine(w)
         if "upsampler.0.weight" in w:                                           # unimatch.py:47-52
             w0 = w["upsampler.0.weight"]                                        # [256, 2 + 128, 3, 3], input = cat(flow, feature)
             w0 = torch.cat([w0[:, 2:], w0[:, :2]], dim=1)                       # our planes hold [feature | flow]
-            nm = w["upsampler.2.weight"].shape[0]
-            bn2 = 192 if nm % 192 == 0 else 64
-            P["up"] = dict(c0=(prep(w0, [130], 256), w["upsampler.0.bias"]),
-                           c2=(prep(w["upsampler.2.weight"], [256], (nm + bn2 - 1) // bn2 * bn2), w["upsampler.2.bias"]),
-                           nm=nm, bn2=bn2)
+            w2 = w["upsampler.2.weight"]
+            P["up"] = dict(c0=_layer(w0, [130], 128, w["upsampler.0.bias"], act=ops.ACT_RELU),
+                           c2=_layer(w2, [256], 192 if w2.shape[0] % 192 == 0 else 64, w["upsampler.2.bias"]))
         self._prep_key, self._prep = key, P
         return P
 
     @staticmethod
-    def _prepare_backbone(w):
-        """fp16 (hi, lo) weight planes of the CNN encoder convolutions (backbone.py:49-86) for um_conv2d_tc."""
+    def _prepare_backbone(w, num_scales):
+        """`_Layer`s of the CNN encoder convolutions (backbone.py:49-86); layer2 and layer3 (one scale) start at stride 2."""
+        first_stride = {"layer2": 2, "layer3": 2 if num_scales == 1 else 1}
         T = {}
         for key, wt in w.items():
             if not key.startswith("backbone.") or not key.endswith(".weight") or key == "backbone.conv1.weight":
                 continue
-            cout, cin = wt.shape[0], wt.shape[1]
-            bn = 128 if cout > 64 else 64          # 96 channels: one padded 128-wide tile beats two 64-wide (A is read once)
-            T[key[:-7]] = (ops.prep_conv_weight(wt, [cin], (cout + bn - 1) // bn * bn), w.get(key[:-7] + ".bias"), bn)
+            name = key[:-7]
+            part = name.split(".")                  # backbone.layer<i>.<block>.conv1 | .conv2 | .downsample.0
+            stride = first_stride.get(part[1], 1) if part[2:3] == ["0"] and part[3] in ("conv1", "downsample") else 1
+            bn = 128 if wt.shape[0] > 64 else 64    # 96 channels: one padded 128-wide tile beats two 64-wide (A is read once)
+            T[name] = _layer(wt, [wt.shape[1]], bn, w.get(name + ".bias"), stride=stride)
         return T
 
     @staticmethod
     def _prepare_refine(w):
-        """fp16 (hi, lo) weight planes for um_conv2d_tc, K ordered (source, tap, ci); see ops.prep_conv_weight."""
-        prep = ops.prep_conv_weight
-        fd = w["refine.flow_head.conv2.weight"].shape[0]
-        T = {"fd": fd}
+        """`_Layer`s of the refinement: refine_proj and the update block (reg_refine.py:6-119)."""
+        R = ops.ACT_RELU
+        T = {}
         pw, pb = w["refine_proj.weight"], w["refine_proj.bias"]
-        T["proj_net"] = (prep(pw[:128], [128], 128), pb[:128].contiguous())
-        T["proj_inp"] = (prep(pw[128:], [128], 128), pb[128:].contiguous())
+        T["proj_net"] = _layer(pw[:128], [128], 128, pb[:128].contiguous(), act=ops.ACT_TANH)
+        T["proj_inp"] = _layer(pw[128:], [128], 128, pb[128:].contiguous(), act=R)
         e = "refine.encoder."
-        T["convc1"] = (prep(w[e + "convc1.weight"], [81], 256), w[e + "convc1.bias"])
-        T["convc2"] = (prep(w[e + "convc2.weight"], [256], 192), w[e + "convc2.bias"])
-        T["convf2"] = (prep(w[e + "convf2.weight"], [128], 64), w[e + "convf2.bias"])
-        T["conv"] = (prep(w[e + "conv.weight"], [256], 128), w[e + "conv.bias"])
+        T["convc1"] = _layer(w[e + "convc1.weight"], [81], 256, w[e + "convc1.bias"], act=R)
+        T["convc2"] = _layer(w[e + "convc2.weight"], [256], 96, w[e + "convc2.bias"], act=R)
+        T["convf2"] = _layer(w[e + "convf2.weight"], [128], 64, w[e + "convf2.bias"], act=R)
+        T["conv"] = _layer(w[e + "conv.weight"], [256], 128, w[e + "conv.bias"], act=R)
         # SepConvGRU (reg_refine.py:22-52) over hx = cat[h, inp, motion | flow] (128 + 128 + 128 channels).  `inp` is the same in
         # every refinement iteration and so is `h` of the first half (net is not carried between iterations, unimatch.py:315-333):
         # their share of each convolution is computed ONCE per forward ("_fix" weights -> a fp32 tensor the per-iteration
         # convolution adds to its accumulator) and only the channels that changed are convolved per iteration ("_var").
         g = "refine.gru.conv"
+        Z, Q = ops.CONV_GRU_ZR, ops.CONV_GRU_Q
         for sfx in ("1", "2"):
             wzr = torch.cat([w[g + "z%s.weight" % sfx], w[g + "r%s.weight" % sfx]], 0)           # [256, 384, kh, kw]
             bzr = torch.cat([w[g + "z%s.bias" % sfx], w[g + "r%s.bias" % sfx]])
             wq, bq = w[g + "q%s.weight" % sfx], w[g + "q%s.bias" % sfx]                           # [128, 384, kh, kw]
             if sfx == "1":
-                T["zr1_fix"] = (prep(wzr[:, :256], [128, 128], 256), bzr)                         # h0 | inp
-                T["zr1_var"] = prep(wzr[:, 256:], [128], 256)                                     # motion | flow
+                T["zr1_fix"] = _layer(wzr[:, :256], [128, 128], 128, bzr)                          # h0 | inp
+                T["zr1_var"] = _layer(wzr[:, 256:], [128], 128, mode=Z)                            # motion | flow
             else:
-                T["zr2_fix"] = (prep(wzr[:, 128:256], [128], 256), bzr)                           # inp
-                T["zr2_var"] = prep(torch.cat([wzr[:, :128], wzr[:, 256:]], 1), [128, 128], 256)  # h1 | motion
-            T["q%s_fix" % sfx] = (prep(wq[:, 128:256], [128], 128), bq)                           # inp
-            T["q%s_var" % sfx] = prep(torch.cat([wq[:, :128], wq[:, 256:]], 1), [128, 128], 128)  # r*h | motion
-        T["fh1"] = (prep(w["refine.flow_head.conv1.weight"], [128], 256), w["refine.flow_head.conv1.bias"])
-        T["fh2"] = (prep(w["refine.flow_head.conv2.weight"], [256], 16), w["refine.flow_head.conv2.bias"])
+                T["zr2_fix"] = _layer(wzr[:, 128:256], [128], 128, bzr)                            # inp
+                T["zr2_var"] = _layer(torch.cat([wzr[:, :128], wzr[:, 256:]], 1), [128, 128], 128, mode=Z)  # h1 | motion
+            T["q%s_fix" % sfx] = _layer(wq[:, 128:256], [128], 128, bq)                            # inp
+            T["q%s_var" % sfx] = _layer(torch.cat([wq[:, :128], wq[:, 256:]], 1), [128, 128], 128, mode=Q)  # r*h | motion
+        T["fh1"] = _layer(w["refine.flow_head.conv1.weight"], [128], 128, w["refine.flow_head.conv1.bias"], act=R)
+        T["fh2"] = _layer(w["refine.flow_head.conv2.weight"], [256], 16, w["refine.flow_head.conv2.bias"])
         if "refine.mask.0.weight" in w:
-            T["mask0"] = (prep(w["refine.mask.0.weight"], [128], 256), w["refine.mask.0.bias"])
-            nm = w["refine.mask.2.weight"].shape[0]
-            T["mask2"] = (prep(w["refine.mask.2.weight"], [256], (nm + 63) // 64 * 64), w["refine.mask.2.bias"])
+            T["mask0"] = _layer(w["refine.mask.0.weight"], [128], 128, w["refine.mask.0.bias"], act=R)
+            T["mask2"] = _layer(w["refine.mask.2.weight"], [256], 64, w["refine.mask.2.bias"])
         return T
 
     def _pos_table(self, wh, ww, device):
@@ -253,19 +261,21 @@ class UniMatch(nn.Module):
         t.setdefault("_events", []).append((tag, e0, e1, flops))
         return out
 
-    def _conv(self, src0, src1, weights, bias, kh, kw, ph, pw, cout, *rest, **kwargs):
-        """um_conv2d_tc; under the bench timer also records 2 x output pixels x cout x real K as the layer's algorithmic FLOPs."""
+    def _conv(self, layer, src0, src1=None, stride=None, rows=0, out_f32=None, off_f32=0, out_split=None, off_split=0,
+              aux0=None, aux1=None, **kw):
+        """um_conv2d_tc of the `_Layer` on src0 (| src1); the other arguments are those of `ops.conv2d_tc`, and `stride`
+        overrides the layer's.  Under the bench timer also records 2 x output pixels x cout x k as algorithmic FLOPs."""
+        stride = layer.stride if stride is None else stride
+
+        def launch():
+            _OPS.conv2d_tc(src0=src0, src1=src1, weights=layer.weights, bias=layer.bias, kh=layer.kh, kw=layer.kw,
+                           pad_h=layer.pad_h, pad_w=layer.pad_w, cout=layer.cout, bn=layer.bn, mode=layer.mode, act=layer.act,
+                           out_f32=out_f32, off_f32=off_f32, out_split=out_split, off_split=off_split, aux0=aux0, aux1=aux1,
+                           gamma=layer.gamma, beta=layer.beta, stride=stride, rows=rows, **kw)
         if self.kernel_timer is None:
-            return _OPS.conv2d_tc(src0, src1, weights, bias, kh, kw, ph, pw, cout, *rest, **kwargs)
-        stride = rest[11] if len(rest) > 11 else 1
-        rows = rest[12] if len(rest) > 12 else 0
-        if rows:
-            pix = rows
-        else:
-            _, b, h, w, _ = src0.shape
-            pix = b * ((h + 2 * ph - kh) // stride + 1) * ((w + 2 * pw - kw) // stride + 1)
-        flops = 2.0 * pix * cout * getattr(weights, "k_true", kh * kw * src0.shape[-1])
-        return self._timed("conv", flops, lambda: _OPS.conv2d_tc(src0, src1, weights, bias, kh, kw, ph, pw, cout, *rest, **kwargs))
+            return launch()
+        pix = rows or src0.shape[1] * math.prod(layer.out_hw(src0.shape[2], src0.shape[3], stride))
+        return self._timed("conv", 2.0 * pix * layer.cout * layer.k, launch)
 
     # ------------------------------------------------------------------------------------------ backbone
     def _stage_backbone(self, P, img0, img1, normalise):
@@ -288,13 +298,10 @@ class UniMatch(nn.Module):
             nplanes[0] += 1                                  # distinct live buffers of one forward get distinct cache slots
             return self._zero_padded("backbone%d" % nplanes[0], (2, nb, h, w, cp), dev)
 
-        def conv(src_s, name, k, stride, cout, hw_in):
-            wt, bias, bn = T[name]
-            h, w = hw_in
-            ho, wo = (h + 2 * (k // 2) - k) // stride + 1, (w + 2 * (k // 2) - k) // stride + 1
-            out = torch.empty((nb, ho, wo, cout), device=dev)
-            C(src_s, None, wt, bias, k, k, k // 2, k // 2, cout, bn, ops.CONV_LINEAR, ops.ACT_NONE, out, 0, None, 0, None,
-              None, None, None, stride)
+        def conv(src_s, name, h, w, stride=None):
+            layer = T[name]
+            out = torch.empty((nb, *layer.out_hw(h, w, layer.stride if stride is None else stride), layer.cout), device=dev)
+            C(layer, src_s, out_f32=out, stride=stride)
             return out
 
         hh, ww = img0.shape[2], img0.shape[3]
@@ -310,17 +317,16 @@ class UniMatch(nn.Module):
         cur_f = torch.empty((nb, h, w, 64), device=dev)
         cur_s = planes(h, w, 64)
         IA(a, IS(a), True, None, None, False, cur_f, cur_s, 0)
-        for li, cout, stride in ((1, 64, 1), (2, 96, 2), (3, 128, 2 if self.num_scales == 1 else 1)):
+        for li in (1, 2, 3):
             for bi in range(2):
                 pf = "backbone.layer%d.%d." % (li, bi)
-                st = stride if bi == 0 else 1
-                a1 = conv(cur_s, pf + "conv1", 3, st, cout, (h, w))
-                ho, wo = a1.shape[1], a1.shape[2]
+                a1 = conv(cur_s, pf + "conv1", h, w)
+                _, ho, wo, cout = a1.shape
                 t_s = planes(ho, wo, cout)
                 IA(a1, IS(a1), True, None, None, False, None, t_s, 0)
-                a2 = conv(t_s, pf + "conv2", 3, 1, cout, (ho, wo))
+                a2 = conv(t_s, pf + "conv2", ho, wo)
                 if (pf + "downsample.0") in T:
-                    res = conv(cur_s, pf + "downsample.0", 1, st, cout, (h, w))
+                    res = conv(cur_s, pf + "downsample.0", h, w)
                     st_res = IS(res)
                 else:
                     res, st_res = cur_f, None
@@ -328,14 +334,13 @@ class UniMatch(nn.Module):
                 out_s = planes(ho, wo, cout)
                 IA(a2, IS(a2), True, res, st_res, True, out_f, out_s, 0)
                 cur_f, cur_s, h, w = out_f, out_s, ho, wo
-        wt, bias, bn = T["backbone.conv2"]
         x6 = torch.empty((nb, h, w, 128), device=dev)
         x6_s = planes(h, w, 128) if self.num_scales > 1 else None
-        C(cur_s, None, wt, bias, 1, 1, 0, 0, 128, bn, ops.CONV_LINEAR, ops.ACT_NONE, x6, 0, x6_s, 0, None, None)
+        C(T["backbone.conv2"], cur_s, out_f32=x6, out_split=x6_s)
         if self.num_scales == 1:
             return [x6]
         strides = (1, 2, 4, 8)[:self.num_scales]                               # trident_conv.py:64-70
-        feats = [conv(x6_s, "backbone.trident_conv", 3, s, 128, (h, w)) for s in strides]
+        feats = [conv(x6_s, "backbone.trident_conv", h, w, stride=s) for s in strides]
         return feats[::-1]
 
     # ------------------------------------------------------------------------------------------ transformer
@@ -396,17 +401,17 @@ class UniMatch(nn.Module):
         rows = n * l
         rp = _ceil16(rows)
         dev = x.device
-        G, LN, LIN, NONE = self._conv, ops.CONV_LN, ops.CONV_LINEAR, ops.ACT_NONE
+        G = self._conv
         mk = torch.empty if rp == rows else torch.zeros
         planes = lambda cp: mk((2, rp, cp), device=dev, dtype=torch.float16)
         f32 = lambda cols: mk((rp, cols), device=dev)
         tok = lambda t, c0, c1: t[:rows].view(n, l, t.shape[-1])[:, :, c0:c1]
-        hid = P["blocks"][0]["hid"]
+        hid = P["blocks"][0]["tc_w1"].cout
         x_f, xo_f, x1_f = f32(c), f32(c), f32(c)
         x_s, xo_s, x1_s, msg_s, m_s = planes(c), planes(c), planes(c), planes(c), planes(c)
         # FFN: one fused kernel (the 1024-wide hidden activation stays in registers) when the rows are a multiple of 256;
         # else two GEMM launches around hidden planes in HBM
-        fused_ffn = _FUSED_FFN and ops.ffn_tc_supported(rp)
+        fused_ffn = ops.ffn_tc_supported(rp)
         hid_s = None if fused_ffn else planes(hid)
         x_f[:rows] = x.reshape(rows, c)
         _OPS.split_planes(x_f, x_s, 0)
@@ -421,8 +426,8 @@ class UniMatch(nn.Module):
             win_c1 = 640 if lp_c else (384 if lp_s else 0)
             if win_c1 < 640 and y is None:
                 y = f32(5 * c)
-            G(x_s, None, blk["tc_in"], None, 1, 1, 0, 0, 5 * c, 128, LIN, NONE, y if win_c1 < 640 else None, 0, None, 0, None,
-              None, None, None, 1, rp, ws[:win_c1 // 128] if win_c1 else None, gs if win_c1 else None, 0, win_c1, n)
+            G(blk["tc_in"], x_s, rows=rp, out_f32=y if win_c1 < 640 else None, win_dst=ws[:win_c1 // 128] if win_c1 else None,
+              win_geom=gs if win_c1 else None, win_c1=win_c1, win_streams=n)
             # ---- self-attention -> merge + LayerNorm + residual (transformer.py:137-144, no FFN: :157-161)
             fl_s, fl_c = (4.0 * (l // (g[0] * g[1])) * l * 128 * n for g in (geo_s, geo_c))   # 4 Lw^2 C per window per stream
             if lp_s:
@@ -430,26 +435,26 @@ class UniMatch(nn.Module):
             else:
                 msg = self._timed("attn_simt:" + tag, fl_s, _OPS.window_attention, tok(y, 0, 128), tok(y, 128, 256), tok(y, 256, 384), 0, *gs)
                 _OPS.split_planes(msg.view(rows, c), msg_s, 0)
-            G(msg_s, None, blk["tc_m_s"], None, 1, 1, 0, 0, c, 128, LN, 0, x1_f, 0, x1_s, 0, x_f, None, blk["g_s"], blk["b_s"], 1, rp)
+            G(blk["tc_m_s"], msg_s, rows=rp, out_f32=x1_f, out_split=x1_s, aux0=x_f)
             # ---- cross-attention: q from the updated stream, k / v from the partner stream's projections
             if lp_c:
-                G(x1_s, None, blk["tc_q_c"], None, 1, 1, 0, 0, c, 128, LIN, NONE, None, 0, None, 0, None, None, None, None, 1, rp,
-                  ws[5:6], gc, 0, 128, n)
+                G(blk["tc_q_c"], x1_s, rows=rp, win_dst=ws[5:6], win_geom=gc, win_c1=128, win_streams=n)
                 self._timed("attn:" + tag, fl_c, _OPS.window_attention_planes, ws[5], ws[3], ws[4], n, half, *gc, None, msg_s)
             else:
                 if q_f is None:
                     q_f = f32(c)
-                G(x1_s, None, blk["tc_q_c"], None, 1, 1, 0, 0, c, 128, LIN, NONE, q_f, 0, None, 0, None, None, None, None, 1, rp)
+                G(blk["tc_q_c"], x1_s, rows=rp, out_f32=q_f)
                 msg = self._timed("attn_simt:" + tag, fl_c, _OPS.window_attention, tok(q_f, 0, 128), tok(y, 384, 512), tok(y, 512, 640), half, *gc)
                 _OPS.split_planes(msg.view(rows, c), msg_s, 0)
-            G(msg_s, None, blk["tc_m_c"], None, 1, 1, 0, 0, c, 128, LN, 0, None, 0, m_s, 0, None, None, blk["g_c1"], blk["b_c1"], 1, rp)
+            G(blk["tc_m_c"], msg_s, rows=rp, out_split=m_s)
             # ---- FFN on cat([source, message]) + LayerNorm + residual
+            w1, w2 = blk["tc_w1"], blk["tc_w2"]
             if fused_ffn:
-                self._timed("conv", 2.0 * rp * hid * (2 * c + c), _OPS.ffn_tc, x1_s, m_s, blk["tc_w1"], blk["tc_w2"], x1_f,
-                            blk["g_c2"], blk["b_c2"], xo_f, xo_s, rp)
+                self._timed("conv", 2.0 * rp * hid * (2 * c + c), _OPS.ffn_tc, x1_s, m_s, w1.weights, w2.weights, x1_f,
+                            w2.gamma, w2.beta, xo_f, xo_s, rp)
             else:
-                G(x1_s, m_s, blk["tc_w1"], None, 1, 1, 0, 0, hid, 256, LIN, ops.ACT_GELU, None, 0, hid_s, 0, None, None, None, None, 1, rp)
-                G(hid_s, None, blk["tc_w2"], None, 1, 1, 0, 0, c, 128, LN, 0, xo_f, 0, xo_s, 0, x1_f, None, blk["g_c2"], blk["b_c2"], 1, rp)
+                G(w1, x1_s, m_s, rows=rp, out_split=hid_s)
+                G(w2, hid_s, rows=rp, out_f32=xo_f, out_split=xo_s, aux0=x1_f)
             x_f, xo_f, x_s, xo_s = xo_f, x_f, xo_s, x_s
         return x_f[:rows].view(n, l, c), x_s
 
@@ -498,19 +503,19 @@ class UniMatch(nn.Module):
         L = h * wd
         rows = nb * L
         rq = rows if rows % 16 == 0 else x_s.shape[1]            # the GEMM runs over a multiple of 16 rows
-        G, LIN, NONE = self._conv, ops.CONV_LINEAR, ops.ACT_NONE
+        G = self._conv
         fd = flow.shape[-1]
         flow = flow.contiguous()
         if prop_r > 0:
             qk = torch.empty((rq, 256), device=dev)
-            G(x_s, None, *P["prop_qk"], 1, 1, 0, 0, 256, 128, LIN, NONE, qk, 0, None, 0, None, None, None, None, 1, rq)
+            G(P["prop_qk"], x_s, rows=rq, out_f32=qk)
             qk = qk[:rows].view(nb, L, 256)
             return _OPS.propagate_local(qk[:, :, :128], qk[:, :, 128:], flow, h, wd, prop_r)
         q = torch.empty((rq, 128), device=dev)
         q_s = torch.empty((2, rq, 128), device=dev, dtype=torch.float16)
         k = torch.empty((rq, 128), device=dev)
-        G(x_s, None, *P["prop_q"], 1, 1, 0, 0, 128, 128, LIN, NONE, q, 0, q_s, 0, None, None, None, None, 1, rq)
-        G(q_s, None, *P["prop_k"], 1, 1, 0, 0, 128, 128, LIN, NONE, k, 0, None, 0, None, None, None, None, 1, rq)
+        G(P["prop_q"], x_s, rows=rq, out_f32=q, out_split=q_s)
+        G(P["prop_k"], q_s, rows=rq, out_f32=k)
         return _OPS.softmax_expectation(q[:rows].view(nb, L, 128), k[:rows].view(nb, L, 128), flow.view(nb, L, fd), nb, 0, fd,
                                         ops.VALUE_TENSOR, ops.POST_NONE, h, wd, 1, 1, ops.MASK_NONE).view(nb, h, wd, fd)
 
@@ -533,51 +538,46 @@ class UniMatch(nn.Module):
         _OPS.split_planes(feat0, f0_s, 0)
         f32 = lambda cc: torch.empty((b, h, w, cc), device=dev)
         st.net0, st.z, st.h1, st.h2 = f32(128), f32(128), f32(128), f32(128)
-        C, LIN, NONE = self._conv, ops.CONV_LINEAR, ops.ACT_NONE
-        C(f0_s, None, *T["proj_net"], 1, 1, 0, 0, 128, 128, LIN, ops.ACT_TANH, st.net0, 0, st.h0_s, 0, None, None)
-        C(f0_s, None, *T["proj_inp"], 1, 1, 0, 0, 128, 128, LIN, ops.ACT_RELU, None, 0, st.inp_s, 0, None, None)
+        C = self._conv
+        C(T["proj_net"], f0_s, out_f32=st.net0, out_split=st.h0_s)
+        C(T["proj_inp"], f0_s, out_split=st.inp_s)
         # loop-invariant shares of the four GRU convolutions (bias included), fp32
         st.pre_zr1, st.pre_q1, st.pre_zr2, st.pre_q2 = f32(256), f32(128), f32(256), f32(128)
-        bn_zr = _bn256(b, h, w)
-        C(st.h0_s, st.inp_s, *T["zr1_fix"], 1, 5, 0, 2, 256, bn_zr, LIN, NONE, st.pre_zr1, 0, None, 0, None, None)
-        C(st.inp_s, None, *T["q1_fix"], 1, 5, 0, 2, 128, 128, LIN, NONE, st.pre_q1, 0, None, 0, None, None)
-        C(st.inp_s, None, *T["zr2_fix"], 5, 1, 2, 0, 256, bn_zr, LIN, NONE, st.pre_zr2, 0, None, 0, None, None)
-        C(st.inp_s, None, *T["q2_fix"], 5, 1, 2, 0, 128, 128, LIN, NONE, st.pre_q2, 0, None, 0, None, None)
+        C(T["zr1_fix"], st.h0_s, st.inp_s, out_f32=st.pre_zr1)
+        C(T["q1_fix"], st.inp_s, out_f32=st.pre_q1)
+        C(T["zr2_fix"], st.inp_s, out_f32=st.pre_zr2)
+        C(T["q2_fix"], st.inp_s, out_f32=st.pre_q2)
         return st
 
     def _update_block(self, P, st, corr, flow, want_mask):
         """BasicUpdateBlock.forward (reg_refine.py:106-119) as 11 tensor-core convolutions: activations live as fp16 (hi, lo)
         planes, the concatenations are channel offsets / second sources, the GRU gate math is the conv epilogue."""
         T, w = P["tc"], P["raw"]
-        fd = T["fd"]
-        C, L, R = self._conv, ops.CONV_LINEAR, ops.ACT_RELU
+        fd = T["fh2"].cout
+        C = self._conv
         b, h, wd, _ = corr.shape
         dev = corr.device
-        bn_zr = bn_fh = _bn256(b, h, wd)
         _OPS.split_planes(corr, st.corr_s, 0)
-        C(st.corr_s, None, *T["convc1"], 1, 1, 0, 0, 256, 256, L, R, None, 0, st.cor1_s, 0, None, None)
-        C(st.cor1_s, None, *T["convc2"], 3, 3, 1, 1, 192, 96 if bn_zr == 128 else 192, L, R, None, 0, st.cf_s, 0, None, None)
+        C(T["convc1"], st.corr_s, out_split=st.cor1_s)
+        C(T["convc2"], st.cor1_s, out_split=st.cf_s)
         _OPS.conv7x7_small(flow, None, False, w["refine.encoder.convf1.weight"], w["refine.encoder.convf1.bias"], 1, True,
                            None, None, None, st.flo1_s)        # 7x7 on 1-2 channels: direct fp32 kernel -> fp16 planes
-        C(st.flo1_s, None, *T["convf2"], 3, 3, 1, 1, 64, 64, L, R, None, 0, st.cf_s, 192, None, None)
-        C(st.cf_s, None, *T["conv"], 3, 3, 1, 1, 128 - fd, 128, L, R, None, 0, st.mfx_s, 0, None, None)
+        C(T["convf2"], st.flo1_s, out_split=st.cf_s, off_split=192)
+        C(T["conv"], st.cf_s, out_split=st.mfx_s)
         _OPS.split_planes(flow, st.mfx_s, 128 - fd)                              # mfx = [motion features | flow]
         # SepConvGRU (reg_refine.py:37-52): horizontal 1x5 then vertical 5x1; the invariant input channels come in through `pre`
-        Z, Q = ops.CONV_GRU_ZR, ops.CONV_GRU_Q
-        kw = dict(gamma=None, beta=None, stride=1, rows=0, win_dst=None, win_geom=None, win_c0=0, win_c1=0, win_streams=0)
-        C(st.mfx_s, None, T["zr1_var"], None, 1, 5, 0, 2, 256, bn_zr, Z, 0, st.z, 0, st.rh_s, 0, st.net0, None, pre=st.pre_zr1, **kw)
-        C(st.rh_s, st.mfx_s, T["q1_var"], None, 1, 5, 0, 2, 128, 128, Q, 0, st.h1, 0, st.h1_s, 0, st.net0, st.z, pre=st.pre_q1, **kw)
-        C(st.h1_s, st.mfx_s, T["zr2_var"], None, 5, 1, 2, 0, 256, bn_zr, Z, 0, st.z, 0, st.rh_s, 0, st.h1, None, pre=st.pre_zr2, **kw)
-        C(st.rh_s, st.mfx_s, T["q2_var"], None, 5, 1, 2, 0, 128, 128, Q, 0, st.h2, 0, st.h2_s, 0, st.h1, st.z, pre=st.pre_q2, **kw)
-        C(st.h2_s, None, *T["fh1"], 3, 3, 1, 1, 256, bn_fh, L, R, None, 0, st.fh_s, 0, None, None)
+        C(T["zr1_var"], st.mfx_s, out_f32=st.z, out_split=st.rh_s, aux0=st.net0, pre=st.pre_zr1)
+        C(T["q1_var"], st.rh_s, st.mfx_s, out_f32=st.h1, out_split=st.h1_s, aux0=st.net0, aux1=st.z, pre=st.pre_q1)
+        C(T["zr2_var"], st.h1_s, st.mfx_s, out_f32=st.z, out_split=st.rh_s, aux0=st.h1, pre=st.pre_zr2)
+        C(T["q2_var"], st.rh_s, st.mfx_s, out_f32=st.h2, out_split=st.h2_s, aux0=st.h1, aux1=st.z, pre=st.pre_q2)
+        C(T["fh1"], st.h2_s, out_split=st.fh_s)
         delta = torch.empty((b, h, wd, fd), device=dev)
-        C(st.fh_s, None, *T["fh2"], 3, 3, 1, 1, fd, 16, L, ops.ACT_NONE, delta, 0, None, 0, None, None)
+        C(T["fh2"], st.fh_s, out_f32=delta)
         mask = None
         if want_mask and "mask0" in T:
-            C(st.h2_s, None, *T["mask0"], 3, 3, 1, 1, 256, bn_fh, L, R, None, 0, st.fh_s, 0, None, None)
-            nm = w["refine.mask.2.weight"].shape[0]
-            mask = torch.empty((b, h, wd, nm), device=dev)
-            C(st.fh_s, None, *T["mask2"], 1, 1, 0, 0, nm, 64, L, ops.ACT_NONE, mask, 0, None, 0, None, None)
+            C(T["mask0"], st.h2_s, out_split=st.fh_s)
+            mask = torch.empty((b, h, wd, T["mask2"].cout), device=dev)
+            C(T["mask2"], st.fh_s, out_f32=mask)
         return st.h2, mask, delta
 
     def _stage_refine_iter(self, P, rst, g0, g1, flow, task, want_mask, depth=None):
@@ -607,14 +607,13 @@ class UniMatch(nn.Module):
         U = P["up"]
         b, h, w, _ = feat.shape
         dev = feat.device
-        C = self._conv
         src = self._zero_padded("upsampler", (2, b, h, w, 192), dev)                # [feature 0..127 | flow 128..129 | 0]
         _OPS.split_planes(feat.contiguous(), src, 0)
         _OPS.split_planes(flow2.contiguous(), src, 128)
         mid = torch.empty((2, b, h, w, 256), device=dev, dtype=torch.float16)
-        C(src, None, *U["c0"], 3, 3, 1, 1, 256, _bn256(b, h, w), ops.CONV_LINEAR, ops.ACT_RELU, None, 0, mid, 0, None, None)
-        m = torch.empty((b, h, w, U["nm"]), device=dev)
-        C(mid, None, *U["c2"], 1, 1, 0, 0, U["nm"], U["bn2"], ops.CONV_LINEAR, ops.ACT_NONE, m, 0, None, 0, None, None)
+        self._conv(U["c0"], src, out_split=mid)
+        m = torch.empty((b, h, w, U["c2"].cout), device=dev)
+        self._conv(U["c2"], mid, out_f32=m)
         return _OPS.convex_upsample(flow2.contiguous(), m, factor, float(mult))
 
     @staticmethod
