@@ -204,6 +204,62 @@ int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n,
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
                      int32_t n, int32_t h, int32_t w, void* stream);
 
+/* ---- evaluation statistics -----------------------------------------------------------------------------------
+ * One pass from a batch of predictions at ground-truth resolution to a [batch, S] float64 table of per-sample sufficient
+ * statistics (pixel counts, counts over thresholds, fp64 sums), from which the host forms the metrics of the reference's
+ * validate_* loops (evaluate_flow.py:160-638, evaluate_stereo.py:302-708, evaluate_depth.py:22-293).
+ *   pred: [B, C, h, w] read through element strides (pred_sb, pred_sc, pred_sy, pred_sx) -- e.g. the unpadded window of the
+ *         padded model output; C = 2 for flow (pred_sc = distance between the u and v planes), 1 otherwise (pred_sc unused);
+ *   gt: contiguous [B, C, h, w]; valid, noc_valid: contiguous [B, h, w] or NULL;
+ *   scratch: DEVICE buffer of batch * UM_EVAL_PARTS * S doubles; out: DEVICE [batch, S] doubles.
+ * Per-pixel values are correctly rounded fp32 in the reference's order of operations, so every count is the reference's
+ * count on the same prediction (logf may differ from numpy's float32 log by 1 ulp: the log-error sum only).  One caveat: the
+ * reference's flow epe / |gt| come from torch's CPU float sqrt, which is not correctly rounded (torch 2.11: one ulp off on
+ * about 0.7% of inputs); a flow count can then differ only where such a value lies within one ulp of a threshold.  Sums are
+ * reduced in a fixed order over a fixed grid (UM_EVAL_PARTS CTAs per sample, then one ordered pass): bit-reproducible,
+ * no host synchronisation.  Threshold constants are the reference's python scalars rounded to float32, as torch / numpy
+ * compare them with float32 arrays. */
+#define UM_EVAL_FLOW 0
+#define UM_EVAL_STEREO 1
+#define UM_EVAL_DEPTH 2
+#define UM_EVAL_PARTS 128
+/* Flow, mask_mode selects the evaluation mask M; epe = sqrt(du*du + dv*dv), mag the same of the GT: */
+#define UM_EVAL_MASK_ALL 0         /* every pixel (Sintel, Chairs)                                                   */
+#define UM_EVAL_MASK_VALID 1       /* valid >= 0.5 (KITTI)                                                           */
+#define UM_EVAL_MASK_VALID_MAX 2   /* valid * (mag < max_val) >= 0.5 (Things, evaluate_flow.py:298-303)              */
+enum um_eval_flow_cols {
+  UM_EVF_N = 0,          /* pixels in M                                                                               */
+  UM_EVF_EPE,            /* sum of epe over M                                                                         */
+  UM_EVF_1PX, UM_EVF_3PX, UM_EVF_5PX,   /* counts of epe > 1, 3, 5                                                   */
+  UM_EVF_OUTLIER,        /* KITTI outliers: epe > 3 & epe / mag > 0.05 (evaluate_flow.py:593)                         */
+  UM_EVF_S0_10_N, UM_EVF_S0_10_EPE,     /* (n, sum epe) with mag < 10                                                */
+  UM_EVF_S10_40_N, UM_EVF_S10_40_EPE,   /* 10 <= mag <= 40                                                           */
+  UM_EVF_S40_N, UM_EVF_S40_EPE,         /* mag > 40                                                                  */
+  UM_EVF_MATCHED_N, UM_EVF_MATCHED_EPE, /* noc_valid given: noc_valid > 0.5 & in-image (compute_out_of_boundary_mask) */
+  UM_EVF_UNMATCHED_N, UM_EVF_UNMATCHED_EPE,   /* the rest of M                                                       */
+  UM_EVAL_FLOW_COLS
+};
+/* Stereo: e = |gt - pred|, M = gt > 0 (& gt < max_val when max_val > 0). */
+enum um_eval_stereo_cols {
+  UM_EVS_N = 0, UM_EVS_ABS,               /* n, sum e                                                                */
+  UM_EVS_D1,                              /* e > 3 & e / gt > 0.05 (loss/stereo_metric.py:d1_metric)                 */
+  UM_EVS_1PX, UM_EVS_2PX, UM_EVS_3PX,     /* e > 1, 2, 3                                                             */
+  UM_EVAL_STEREO_COLS
+};
+/* Depth: d = gt - pred, M = gt > eval_min & gt < eval_max (& valid > 0.5 when valid is given); loss/depth_loss.py:compute_errors. */
+enum um_eval_depth_cols {
+  UM_EVD_N = 0,
+  UM_EVD_ABS_REL,        /* sum |d| / gt                                                                              */
+  UM_EVD_SQ_REL,         /* sum d^2 / gt                                                                              */
+  UM_EVD_SQ,             /* sum d^2                                                                                   */
+  UM_EVD_LOG_SQ,         /* sum (log gt - log pred)^2                                                                 */
+  UM_EVD_A1, UM_EVD_A2, UM_EVD_A3,        /* max(gt/pred, pred/gt) < 1.25, 1.25^2, 1.25^3                            */
+  UM_EVAL_DEPTH_COLS
+};
+int um_eval_stats(const float* pred, int64_t pred_sb, int64_t pred_sc, int64_t pred_sy, int64_t pred_sx, const float* gt,
+                  const float* valid, const float* noc_valid, int32_t task, int32_t mask_mode, float max_val, float eval_min,
+                  float eval_max, int32_t batch, int32_t h, int32_t w, double* scratch, double* out, void* stream);
+
 /* ---- tensor-core implicit-GEMM convolution / Linear layer (fp16 hi/lo split operands, fp32 accumulate) ----------
  * Replaces the nn.Conv2d calls of BasicUpdateBlock (reg_refine.py:6-119), refine_proj (unimatch.py:315) and, as a
  * 1x1 convolution over a [rows/16, 16] grid, nn.Linear (transformer.py:58-60,137,141).

@@ -27,6 +27,17 @@ def set_force_cuda_cores(flag):
     _force_cuda_cores = bool(flag)
 
 
+EVAL_FLOW, EVAL_STEREO, EVAL_DEPTH = 0, 1, 2
+EVAL_MASK_ALL, EVAL_MASK_VALID, EVAL_MASK_VALID_MAX = 0, 1, 2
+EVAL_PARTS = 128                      # UM_EVAL_PARTS: partial rows per sample in the scratch buffer
+# columns of the [B, S] statistics table (include/unimatch_sm100.h, enum um_eval_*_cols)
+EVAL_FLOW_COLS = ("n", "epe", "1px", "3px", "5px", "outlier", "s0_10_n", "s0_10_epe", "s10_40_n", "s10_40_epe", "s40_n",
+                  "s40_epe", "matched_n", "matched_epe", "unmatched_n", "unmatched_epe")
+EVAL_STEREO_COLS = ("n", "abs", "d1", "1px", "2px", "3px")
+EVAL_DEPTH_COLS = ("n", "abs_rel", "sq_rel", "sq", "log_sq", "a1", "a2", "a3")
+EVAL_COLS = {EVAL_FLOW: EVAL_FLOW_COLS, EVAL_STEREO: EVAL_STEREO_COLS, EVAL_DEPTH: EVAL_DEPTH_COLS}
+
+
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_SIGMOID, ACT_GELU = 0, 1, 2, 3, 4
 CONV_LINEAR, CONV_GRU_ZR, CONV_GRU_Q, CONV_LN = 0, 1, 2, 3
 
@@ -89,6 +100,7 @@ _SIGNATURES = {
     "um_frames_to_planar": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_eval_stats": (_RC, [_P, _L, _L, _L, _L, _P, _P, _P, _I, _I, _F, _F, _F, _I, _I, _I, _P, _P, _P]),
     "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
     "um_ffn_tc": (_RC, [ctypes.POINTER(FfnDesc), _P]),
     "um_conv7x7_small": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _I, _I, _FP, _FP, _P, _L, _P, _I, _P]),
@@ -428,6 +440,41 @@ def _flow_to_image(flow, out):
 
 
 flow_to_image = _define("flow_to_image(Tensor flow, Tensor(a!) out) -> ()", _flow_to_image)
+
+
+def _eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, eval_max):
+    """pred: flow [B, 2, h, w] or disparity / depth [B, h, w], fp32 with any non-overlapping strides (e.g. the unpadded view
+    of the padded model output); gt: contiguous, same shape; valid / noc_valid: contiguous [B, h, w] or None.
+    Returns the [B, S] float64 statistics table, columns EVAL_COLS[task]."""
+    if task not in EVAL_COLS:
+        raise RuntimeError("eval_stats: unknown task %d" % task)
+    nd = 4 if task == EVAL_FLOW else 3
+    if pred.dim() != nd or (nd == 4 and pred.shape[1] != 2):
+        raise RuntimeError("eval_stats: expected pred [B, 2, h, w] for flow and [B, h, w] otherwise")
+    if not pred.is_cuda or pred.dtype != torch.float32:
+        raise RuntimeError("eval_stats: pred must be a float32 CUDA tensor")
+    _f32c(gt, "gt")
+    if gt.shape != pred.shape or gt.device != pred.device:
+        raise RuntimeError("eval_stats: gt must have the prediction's shape and device")
+    b, h, w = pred.shape[0], pred.shape[-2], pred.shape[-1]
+    for t, name in ((valid, "valid"), (noc_valid, "noc_valid")):
+        if t is not None:
+            _f32c(t, name)
+            if tuple(t.shape) != (b, h, w) or t.device != pred.device:
+                raise RuntimeError("eval_stats: %s must be [B, h, w] on the prediction's device" % name)
+    sb, sy, sx = pred.stride(0), pred.stride(-2), pred.stride(-1)
+    sc = pred.stride(1) if nd == 4 else 0
+    cols = len(EVAL_COLS[task])
+    scratch = torch.empty((b * EVAL_PARTS * cols,), device=pred.device, dtype=torch.float64)
+    out = torch.empty((b, cols), device=pred.device, dtype=torch.float64)
+    _check(LIB.um_eval_stats(_p(pred), sb, sc, sy, sx, _p(gt), _p(valid), _p(noc_valid), task, mask_mode, float(max_val),
+                             float(eval_min), float(eval_max), b, h, w, _p(scratch), _p(out), _stream()), "um_eval_stats")
+    return out
+
+
+eval_stats = _define(
+    "eval_stats(Tensor pred, Tensor gt, Tensor? valid, Tensor? noc_valid, int task, int mask_mode, float max_val, "
+    "float eval_min, float eval_max) -> Tensor", _eval_stats)
 
 
 # ---- tensor-core convolution / Linear ---------------------------------------------------------------------------
