@@ -41,6 +41,7 @@ SPLIT_OUT = (2.0 ** -21, 2.0 ** -24)   # fp32 value stored as fp16 (hi, lo) plan
 ACT_ABS = {"tanh": 1e-6, "sigmoid": 5e-7, "gelu": 5e-7}   # fast-intrinsic epilogue functions, absolute error
 ACT_SLOPE = {"none": 1.0, "relu": 1.0, "tanh": 1.0, "sigmoid": 0.25, "gelu": 1.13}
 L_SUM = 4.0                # fp32 sums of the softmax weights: L_SUM * 2^-24 * sqrt(keys) relative
+UFLOW = 2.0 ** -100        # absolute error of a weight that underflows fp32 (peaked or saturated logits), per |value|
 
 ACT_NAMES = {0: "none", 1: "relu", 2: "tanh", 3: "sigmoid", 4: "gelu"}
 MASK_NONE, MASK_SWIN, MASK_CAUSAL = 0, 1, 2
@@ -193,28 +194,34 @@ def _logit_bound(qw, kw_):
     return s, G0 * a + gemm_steps(C) * U_STEP * (s.abs() + WALK * r) + rep
 
 
+def _pv(p, vals):
+    """p [M, N] times vals: [N, d] shared by every row, or [M, N, d] per row."""
+    return p @ vals if vals.dim() == 2 else torch.einsum("mn,mnd->md", p, vals)
+
+
 def softmax_weighted(s, ds, vals, v_rep=None, tc_pv=True):
-    """s: [M, N] scaled logits (-inf = excluded), ds: their bound, vals: [N, d] float64.  Returns (o, bound) [M, d].
-    tc_pv: P V on the tensor cores (P split into fp16 (hi, lo), truncating accumulation over 64-key tiles); otherwise fp32
-    CUDA-core sums of p * value."""
+    """s: [M, N] scaled logits (-inf = excluded), ds: their bound, vals: [N, d] (or [M, N, d]: values per row) float64.
+    Returns (o, bound) [M, d].  tc_pv: P V on the tensor cores (P split into fp16 (hi, lo), truncating accumulation over
+    64-key tiles); otherwise fp32 CUDA-core sums of p * value."""
     smax = s.max(-1, keepdim=True).values
     e = torch.exp(s - smax)
     l = e.sum(-1, keepdim=True)
     p = e / l
-    o = p @ vals
+    o = _pv(p, vals)
     va = vals.abs()
-    pv = p @ va
+    pv = _pv(p, va)
     n = s.shape[-1]
     ds = torch.where(torch.isfinite(s), ds + U_STEP * (s.abs() + smax.abs()), torch.zeros_like(ds))
     pds = p * ds
-    b = pds @ va + pds.sum(-1, keepdim=True) * o.abs()                   # sum_k p_k ds_k |v_k - o|
+    b = _pv(pds, va) + pds.sum(-1, keepdim=True) * o.abs()               # sum_k p_k ds_k |v_k - o|
     b = b + 2 * G0 * pv + 2 * U32 * o.abs() + L_SUM * U32 * math.sqrt(n) * (o.abs() + pv)
+    b = b + UFLOW * _pv(torch.ones_like(p), va)                          # weights near and below the fp32 underflow
     if tc_pv:
         tiles = (n + 63) // 64
         b = b + 12 * tiles * U_STEP * (o.abs() + WALK * torch.sqrt((p * p) @ (vals * vals)))
         b = b + 2.0 ** -22 * pv + 2.0 ** -25 / l * va.sum(0, keepdim=True)
     if v_rep is not None:
-        b = b + p @ v_rep
+        b = b + _pv(p, v_rep)
     return o, b
 
 
@@ -294,6 +301,344 @@ def instance_norm_stats64(x):
     mean = v.mean(1)
     var = ((v - mean[:, None]) ** 2).mean(1)
     return mean, 1.0 / torch.sqrt(var + EPS_IN), torch.sqrt(var)
+
+
+# ---- matching-path kernels on the CUDA cores (um_local.cu, um_local_stencil.cu, um_misc.cu, um_stem.cu) ------------
+# These run fp32 FMAs (no fp16 split, no fast math), so the bounds are the classical ones:
+#   dot product over n sequential roundings     gamma_n * sum |a||b|, gamma_n = n u / (1 - n u), u = 2^-24
+#     gather kernels: 16 FMAs per lane + 3 shuffle adds (n = 19); the stencil: one FMA chain over 128 channels
+#   bilinear blend of 4 taps with fp32 weights   BLEND_N more roundings on the blend of |values|
+#   coordinates                                  the kernels form positions in fp32 the way the reference does (normalise
+#                                                to [-1, 1], un-normalise with align_corners=True), which moves a tap by a
+#                                                few ulps of (size - 1) and of the position itself: COORD_REL * (size - 1 +
+#                                                |p|).  The output moves by |d out / d x| dx + |d out / d y| dy, with the
+#                                                derivative bounded by the largest finite difference of the four-tap cells
+#                                                the rounding can reach (the cell of the position and its neighbours).
+#   online softmax                               softmax_weighted(..., tc_pv=False)
+SQRT_C = math.sqrt(C)
+DOT_N_GATHER = 19
+DOT_N_STENCIL = 128
+BLEND_N = 6
+COORD_REL = 2.0 ** -21
+
+
+def gamma(n):
+    return n * U32 / (1 - n * U32)
+
+
+def coord_err(p, size):
+    return COORD_REL * ((size - 1) + p.abs())
+
+
+def bilerp(val, ix, iy):
+    """Bilinear interpolation at float64 positions (ix, iy) [P, K] of val(yy, xx) -> [P, K, ...] (values at integer pixels,
+    padding done by val), with the weights of the kernels' make_tap.  Returns (out, |d/dx| bound, |d/dy| bound, blend of
+    |values|)."""
+    x0, y0 = torch.floor(ix), torch.floor(iy)
+    wx, wy = ix - x0, iy - y0
+    x0, y0 = x0.long(), y0.long()
+    V = [[val(y0 + j, x0 + i) for i in range(-1, 3)] for j in range(-1, 3)]
+    ex = lambda t: t.view(t.shape + (1,) * (V[0][0].dim() - t.dim()))
+    wx, wy = ex(wx), ex(wy)
+    ws = ((1 - wx) * (1 - wy), wx * (1 - wy), (1 - wx) * wy, wx * wy)
+    taps = (V[1][1], V[1][2], V[2][1], V[2][2])
+    out = sum(w_ * t for w_, t in zip(ws, taps))
+    mag = sum(w_ * t.abs() for w_, t in zip(ws, taps))
+    gx = torch.stack([(V[j][i + 1] - V[j][i]).abs() for j in range(4) for i in range(3)]).amax(0)
+    gy = torch.stack([(V[j + 1][i] - V[j][i]).abs() for j in range(3) for i in range(4)]).amax(0)
+    return out, gx, gy, mag
+
+
+def _zero_pad(img, b):
+    """val(yy, xx) of bilerp on channel-last float64 images img [B, h, w, c] (query p in image b[p]), zeros outside."""
+    h, w = img.shape[1], img.shape[2]
+
+    def val(yy, xx):
+        ok = (yy >= 0) & (yy < h) & (xx >= 0) & (xx < w)
+        v = img[b.view(-1, *([1] * (yy.dim() - 1))).expand_as(yy), yy.clamp(0, h - 1), xx.clamp(0, w - 1)]
+        return v * ok.unsqueeze(-1)
+    return val
+
+
+def _dot_val(a, img, b):
+    """val(yy, xx) -> (a_p . img[b_p, yy, xx], sum |a_p||img|) stacked on the last dim, zeros outside the image."""
+    sample = _zero_pad(img, b)
+
+    def val(yy, xx):
+        v = sample(yy, xx)
+        return torch.stack((torch.einsum("pc,pkc->pk", a, v), torch.einsum("pc,pkc->pk", a.abs(), v.abs())), -1)
+    return val
+
+
+def _chunks(n, size=256):
+    return [slice(i, min(i + size, n)) for i in range(0, n, size)]
+
+
+def _logits(a, img, b, ix, iy, exact_coords, dot_n, h, w):
+    """Scaled correlation logits a . bilinear(img, (ix, iy)) / sqrt(C) [P, K] and their bound."""
+    v, gx, gy, mag = bilerp(_dot_val(a, img, b), ix, iy)
+    s, A = v[..., 0] / SQRT_C, mag[..., 1] / SQRT_C
+    ds = gamma(dot_n + (0 if exact_coords else BLEND_N)) * A + 2 * U32 * s.abs()
+    if not exact_coords:
+        ds = ds + (gx[..., 0] * coord_err(ix, w) + gy[..., 0] * coord_err(iy, h)) / SQRT_C
+    return s, ds
+
+
+def window_offsets(ry, rx):
+    dy, dx = torch.meshgrid(torch.arange(-ry, ry + 1), torch.arange(-rx, rx + 1), indexing="ij")
+    return dy.reshape(-1), dx.reshape(-1)
+
+
+def local_corr_softmax64(f0, f1, ry, rx, stereo, pix, stencil):
+    """local_correlation_softmax / _stereo (matching.py): softmax over the integer window (out-of-image taps excluded, weight
+    exp(-1e9)) of f0 . f1 / sqrt(C), expectation of the tap coordinates minus the pixel's own; stereo returns x - E[x].
+    f0, f1: [B, h, w, C] fp32, pix = (b, y, x) of the query pixels.  stencil: integer taps on exact coordinates and one FMA
+    chain per dot product (um_local_stencil.cu); otherwise the gather kernel.  Returns (out, bound) [P, 2 or 1]."""
+    B, h, w, _ = f0.shape
+    f0d, f1d = f0.double(), f1.double()
+    b, y, x = pix
+    dy, dx = window_offsets(ry, rx)
+    outs, bnds = [], []
+    for sl in _chunks(b.numel()):
+        bb, yy, xx = b[sl], y[sl], x[sl]
+        sy, sx = yy[:, None] + dy, xx[:, None] + dx
+        s, ds = _logits(f0d[bb, yy, xx], f1d, bb, sx.double(), sy.double(), stencil,
+                        DOT_N_STENCIL if stencil else DOT_N_GATHER, h, w)
+        valid = (sx >= 0) & (sx < w) & (sy >= 0) & (sy < h)
+        s = torch.where(valid, s, torch.full_like(s, -math.inf))
+        vals = torch.stack((sx, sy), -1).double()[..., :1 if stereo else 2]
+        o, bd = softmax_weighted(s, ds, vals, tc_pv=False)
+        own = torch.stack((xx, yy), -1).double()[:, :o.shape[-1]]
+        o = own - o if stereo else o - own
+        outs.append(o)
+        bnds.append(bd + U32 * o.abs())
+    return torch.cat(outs), torch.cat(bnds)
+
+
+def as_flow2(flow):
+    """[..., 2] flow or [..., 1] disparity -> float64 (u, v); a disparity d moves a pixel by (-d, 0)."""
+    flow = flow.double()
+    return flow if flow.shape[-1] == 2 else torch.cat((-flow, torch.zeros_like(flow)), -1)
+
+
+def local_corr_volume64(f0, f1, flow, radius, pix):
+    """local_correlation_with_flow (matching.py): f0 . bilinear(f1, (x + dx + u, y + dy + v)) / sqrt(C) for the (2r+1)^2
+    offsets, zeros padding, exact coordinates.  The kernel blends all taps with the centre tap's weights, which is the same
+    function of the same positions up to the coordinate rounding the bound carries.  Returns (out, bound) [P, (2r+1)^2]."""
+    B, h, w, _ = f0.shape
+    f0d, f1d, fl = f0.double(), f1.double(), as_flow2(flow)
+    b, y, x = pix
+    dy, dx = window_offsets(radius, radius)
+    outs, bnds = [], []
+    for sl in _chunks(b.numel()):
+        bb, yy, xx = b[sl], y[sl], x[sl]
+        u = fl[bb, yy, xx]
+        ix = (xx.double() + u[:, 0])[:, None] + dx
+        iy = (yy.double() + u[:, 1])[:, None] + dy
+        s, ds = _logits(f0d[bb, yy, xx], f1d, bb, ix, iy, False, DOT_N_GATHER, h, w)
+        outs.append(s)
+        bnds.append(ds)
+    return torch.cat(outs), torch.cat(bnds)
+
+
+def flow_warp64(f, flow, pix):
+    """bilinear_sample of f [B, h, w, C] at (x + u, y + v) (geometry.py: zeros padding, align_corners=True) -> (out, bound)
+    [P, C]."""
+    B, h, w, _ = f.shape
+    fd, fl = f.double(), as_flow2(flow)
+    b, y, x = pix
+    outs, bnds = [], []
+    for sl in _chunks(b.numel()):
+        bb, yy, xx = b[sl], y[sl], x[sl]
+        u = fl[bb, yy, xx]
+        ix, iy = (xx.double() + u[:, 0])[:, None], (yy.double() + u[:, 1])[:, None]
+        v, gx, gy, mag = bilerp(_zero_pad(fd, bb), ix, iy)
+        bd = gamma(BLEND_N) * mag + gx * coord_err(ix, w)[..., None] + gy * coord_err(iy, h)[..., None]
+        outs.append(v[:, 0])
+        bnds.append(bd[:, 0])
+    return torch.cat(outs), torch.cat(bnds)
+
+
+def propagate_local64(q, k, flow, radius, pix):
+    """SelfAttnPropagation.forward_local_window_attn (attention.py) on projected q / k [B, h, w, C] (any strides): softmax
+    over the (2r+1)^2 window of q . k / sqrt(C), zero-padded unfold, so an out-of-image key is a zero vector with logit 0 and
+    value 0.  Returns (out, bound) [P, fd]."""
+    B, h, w, _ = q.shape
+    qd, kd, fl = q.double(), k.double(), flow.double()
+    b, y, x = pix
+    dy, dx = window_offsets(radius, radius)
+    outs, bnds = [], []
+    for sl in _chunks(b.numel()):
+        bb, yy, xx = b[sl], y[sl], x[sl]
+        sy, sx = yy[:, None] + dy, xx[:, None] + dx
+        kv = _zero_pad(kd, bb)(sy, sx)
+        a = qd[bb, yy, xx]
+        s = torch.einsum("pc,pkc->pk", a, kv) / SQRT_C
+        ds = gamma(DOT_N_GATHER) * torch.einsum("pc,pkc->pk", a.abs(), kv.abs()) / SQRT_C + 2 * U32 * s.abs()
+        o, bd = softmax_weighted(s, ds, _zero_pad(fl, bb)(sy, sx), tc_pv=False)
+        outs.append(o)
+        bnds.append(bd)
+    return torch.cat(outs), torch.cat(bnds)
+
+
+def _project64(K, Kinv, pose, x, y, depth):
+    """warp_with_pose_depth_candidates (matching.py) in float64 on the fp32 camera matrices: pixel (x, y) [P] at depths
+    [P, D] -> image positions (u, v) [P, D] (z clamped at 1e-3) and a bound of their fp32 rounding."""
+    X = Kinv[:, :, 0] * x[:, None] + Kinv[:, :, 1] * y[:, None] + Kinv[:, :, 2]                       # [P, 3]
+    Xa = Kinv[:, :, 0].abs() * x[:, None].abs() + Kinv[:, :, 1].abs() * y[:, None].abs() + Kinv[:, :, 2].abs()
+    R, t = pose[:, :3, :3], pose[:, :3, 3]
+    Xr = torch.einsum("prc,pc->pr", R, X)
+    Xra = torch.einsum("prc,pc->pr", R.abs(), Xa)
+    eXr = 6 * U32 * Xra                                                                               # two 3-term FMA chains
+    Pt = Xr[:, None, :] * depth[..., None] + t[:, None, :]                                            # [P, D, 3]
+    Pta = Xra[:, None, :] * depth[..., None] + t[:, None, :].abs()
+    ePt = eXr[:, None, :] * depth[..., None] + 4 * U32 * Pta                                          # 1 / c, * and +
+    pr = torch.einsum("prc,pdc->pdr", K, Pt)
+    pra = torch.einsum("prc,pdc->pdr", K.abs(), Pta)
+    epr = torch.einsum("prc,pdc->pdr", K.abs(), ePt) + 3 * U32 * pra
+    z = pr[..., 2].clamp(min=1e-3)
+    ez = torch.where(pr[..., 2] + epr[..., 2] >= 1e-3, epr[..., 2], torch.zeros_like(z))
+    u, v = pr[..., 0] / z, pr[..., 1] / z
+    eu = (epr[..., 0] + u.abs() * ez) / (z - ez).clamp(min=1e-3) + U32 * u.abs()
+    ev = (epr[..., 1] + v.abs() * ez) / (z - ez).clamp(min=1e-3) + U32 * v.abs()
+    return u, v, eu, ev
+
+
+def depth_corr64(f0, f1, K, Kinv, pose, cand, pix):
+    """correlation_softmax_depth (matching.py): f0 . bilinear(f1, project(pixel, 1 / c)) / sqrt(C) for every inverse-depth
+    candidate c (zeros padding: a candidate projecting outside has logit 0), softmax over the candidates and the expected
+    candidate.  Returns (softmax out [P], bound [P], logits [P, D], their bound [P, D])."""
+    B, h, w, _ = f0.shape
+    f0d, f1d = f0.double(), f1.double()
+    Kd, Kid, Pd, cd = K.double(), Kinv.double(), pose.double(), cand.double()
+    b, y, x = pix
+    outs, bnds, ss, dss = [], [], [], []
+    for sl in _chunks(b.numel(), 128):
+        bb, yy, xx = b[sl], y[sl], x[sl]
+        depth = (1.0 / cd)[None].expand(bb.numel(), -1)
+        u, v, eu, ev = _project64(Kd[bb], Kid[bb], Pd[bb], xx.double(), yy.double(), depth)
+        val, gx, gy, mag = bilerp(_dot_val(f0d[bb, yy, xx], f1d, bb), u, v)
+        s, A = val[..., 0] / SQRT_C, mag[..., 1] / SQRT_C
+        ds = (gamma(DOT_N_GATHER + BLEND_N) * A + 2 * U32 * s.abs() +
+              (gx[..., 0] * (eu + coord_err(u, w)) + gy[..., 0] * (ev + coord_err(v, h))) / SQRT_C)
+        o, bd = softmax_weighted(s, ds, cd[:, None], tc_pv=False)
+        outs.append(o[:, 0])
+        bnds.append(bd[:, 0])
+        ss.append(s)
+        dss.append(ds)
+    return torch.cat(outs), torch.cat(bnds), torch.cat(ss), torch.cat(dss)
+
+
+def argmax_admissible(s, ds):
+    """[P, D] bool: the candidates a first-maximum argmax over logits within ds of s may return.  d qualifies if no earlier
+    candidate is surely >= it and no later one surely > it; where the top two differ by more than their bounds only the
+    true argmax qualifies."""
+    lo, hi = s - ds, s + ds
+    neg = torch.full_like(lo[:, :1], -math.inf)
+    before = torch.cat((neg, torch.cummax(lo, 1).values[:, :-1]), 1)
+    after = torch.cat((torch.cummax(lo.flip(1), 1).values.flip(1)[:, 1:], neg), 1)
+    return (before < hi) & (after <= hi)
+
+
+def check_argmax(name, got, cand, s, ds):
+    """got [P] candidate values the kernel returned; every one must be admissible.  Prints how many were decided exactly."""
+    got = got.detach().double().cpu().view(-1, 1)
+    hit = got == cand.double().view(1, -1)
+    assert (hit.sum(1) == 1).all(), "%s: output is not one of the candidates" % name
+    adm = argmax_admissible(s, ds)
+    ok = (hit & adm).any(1)
+    exact = adm.sum(1) == 1
+    print("%-60s argmax: %d of %d pixels decided exactly, %d near-tied" % (name, int(exact.sum()), got.shape[0],
+                                                                          int((~exact).sum())))
+    if not ok.all():
+        i = int((~ok).nonzero()[0])
+        raise AssertionError("%s: pixel %d chose candidate %d, admissible %s" % (
+            name, i, int(hit[i].nonzero()), adm[i].nonzero().view(-1).tolist()))
+
+
+def convex_upsample64(flow, mask, factor, mult, rows=None):
+    """upsample_flow_with_mask (utils.py): softmax over the 9 mask logits of each sub-pixel, convex combination of the 3x3
+    neighbourhood of mult * flow (zero-padded unfold, the softmax still over all 9).  flow [B, h, w, fd], mask
+    [B, h, w, 9 F F] (logit t * F * F + ky * F + kx).  rows: low-resolution rows to evaluate.  Returns (out, bound)
+    [B, fd, len(rows) * F, w * F]."""
+    B, h, w, fd = flow.shape
+    rows = torch.arange(h) if rows is None else rows
+    F_ = factor
+    m = mask.double()[:, rows].view(B, len(rows), w, 9, F_ * F_)
+    e = torch.exp(m - m.amax(3, keepdim=True))
+    p = e / e.sum(3, keepdim=True)
+    fl = torch.nn.functional.pad(flow.double() * mult, (0, 0, 1, 1, 1, 1))                     # [B, h+2, w+2, fd]
+    nb = torch.stack([fl[:, rows + ty][:, :, tx:tx + w] for ty in range(3) for tx in range(3)], 3)   # [B, R, w, 9, fd]
+    o = torch.einsum("brwts,brwtd->brwsd", p, nb)
+    pv = torch.einsum("brwts,brwtd->brwsd", p, nb.abs())
+    dev = (nb[:, :, :, :, None, :] - o[:, :, :, None]).abs()                                  # [B, R, w, 9, FF, fd]
+    arg = (m - m.amax(3, keepdim=True)).abs()
+    bd = 24 * U32 * pv + torch.einsum("brwts,brwtsd->brwsd", p * (4 * U32 + U32 * arg), dev)
+    bd = bd + UFLOW * nb.abs().sum(3, keepdim=True)                # weights near and below the fp32 underflow
+    fix = lambda t: t.view(B, len(rows), w, F_, F_, fd).permute(0, 5, 1, 3, 2, 4).reshape(B, fd, len(rows) * F_, w * F_)
+    return fix(o), fix(bd)
+
+
+def upsample2x64(flow, mult):
+    """F.interpolate(scale_factor=2, bilinear, align_corners=True) * mult of channel-last flow [B, h, w, fd] -> (out,
+    bound) [B, 2h, 2w, fd]."""
+    B, h, w, fd = flow.shape
+    H, W = 2 * h, 2 * w
+    fy = torch.arange(H, dtype=torch.float64) * ((h - 1) / (H - 1) if H > 1 else 0.0)
+    fx = torch.arange(W, dtype=torch.float64) * ((w - 1) / (W - 1) if W > 1 else 0.0)
+    iy, ix = (t.reshape(-1, 1) for t in torch.meshgrid(fy, fx, indexing="ij"))
+    img = flow.double()
+
+    def val(yy, xx):                                               # ATen clamps the second tap at the last row / column
+        return img[:, yy.clamp(0, h - 1), xx.clamp(0, w - 1)].permute(1, 2, 0, 3)          # [H W, 1, B, fd]
+    out, gx, gy, mag = (t.view(H, W, B, fd).permute(2, 0, 1, 3) for t in bilerp(val, ix, iy))
+    bd = 6 * U32 * mag + gx * COORD_REL * (w - 1) + gy * COORD_REL * (h - 1)
+    return out * mult, (bd + U32 * out.abs()) * abs(mult)
+
+
+def add_position_ref(x, table, h, w):
+    """feature_add_position: x + table[y mod wh, x mod ww] -- one fp32 addition per element, so the result is exact."""
+    wh, ww = table.shape[0], table.shape[1]
+    return x + table.repeat(h // wh, w // ww, 1)[None]
+
+
+def conv7x7_64(x, weight, bias, stride, relu, scale=None, shift=None):
+    """The 7x7 stem / flow-encoder convolution, padding 3, on planar [N, cin, H, W] input: x * scale + shift per channel
+    inside the image (the folded ImageNet normalisation), zeros outside, then + bias and ReLU.  The kernel is one fp32 FMA
+    chain of 49 cin products per output.  Returns (out, bound) channel-last [N, Ho, Wo, cout]."""
+    xd = x.double()
+    if scale is not None:
+        xd = xd * torch.tensor(scale, dtype=torch.float32).double().view(1, -1, 1, 1) + \
+             torch.tensor(shift, dtype=torch.float32).double().view(1, -1, 1, 1)
+    wd = weight.double()
+    y = torch.nn.functional.conv2d(xd, wd, None, stride=stride, padding=3)
+    a = torch.nn.functional.conv2d(xd.abs(), wd.abs(), None, stride=stride, padding=3)
+    e = gamma(49 * x.shape[1] + 3) * a
+    if bias is not None:
+        y = y + bias.double().view(1, -1, 1, 1)
+        e = e + gamma(49 * x.shape[1] + 3) * bias.double().abs().view(1, -1, 1, 1)
+    if relu:
+        y = torch.relu(y)
+    return y.permute(0, 2, 3, 1), e.permute(0, 2, 3, 1)
+
+
+def pixel_subset(B, h, w, gen, seam_x=(), seam_y=(), n_seam=2000, n_rand=300):
+    """(b, y, x) of the pixels a reference is evaluated on: every border pixel, up to n_seam pixels on the columns / rows
+    x mod sx in (0, sx - 1), y mod sy in (0, sy - 1) of the given tile seams, and n_rand random pixels."""
+    ys, xs = torch.meshgrid(torch.arange(h), torch.arange(w), indexing="ij")
+    border = (ys == 0) | (ys == h - 1) | (xs == 0) | (xs == w - 1)
+    seam = torch.zeros_like(border)
+    for s in seam_x:
+        seam |= (xs % s == 0) | (xs % s == s - 1)
+    for s in seam_y:
+        seam |= (ys % s == 0) | (ys % s == s - 1)
+    seam &= ~border
+    idx = [border.reshape(-1).nonzero().view(-1)]
+    si = seam.reshape(-1).nonzero().view(-1)
+    idx.append(si[torch.randperm(si.numel(), generator=gen)[:n_seam]])
+    idx = torch.cat(idx)
+    flat = torch.cat([idx + i * h * w for i in range(B)] + [torch.randperm(B * h * w, generator=gen)[:n_rand]]).unique()
+    return flat // (h * w), (flat % (h * w)) // w, flat % w
 
 
 # ---- the assertion ------------------------------------------------------------------------------------------------

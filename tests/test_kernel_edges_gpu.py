@@ -10,6 +10,7 @@ import pytest
 import torch
 
 import ref64
+import test_matching_edges_gpu as M
 from unimatch_b200 import ops
 
 pytestmark = pytest.mark.gpu
@@ -389,7 +390,7 @@ def covered_keys():
         keys.add(attn_key(h, w, kh, kw, sh, sw, mask))
     for name, nt, ns, kvs, h, w, vdim, vm, post, kh, kw, mask, _ in EXP_EDGE:
         keys.add(expect_key(h, w, kh, kw, mask, nt, vm))
-    return keys
+    return keys | M.covered_keys()                                          # tests/test_matching_edges_gpu.py
 
 
 def test_case_tables_reach_every_conv_instantiation():
@@ -437,19 +438,49 @@ class _Census:
     def _key_softmax_expectation(self, q, k, values, ns, kvs, vdim, vm, post, h, w, kh, kw, mask):
         return expect_key(h, w, kh, kw, mask, q.shape[0], vm)
 
+    def _key_local_corr_softmax(self, f0, f1, h, w, ry, rx, stereo):
+        return M.lcs_key(ry, rx, stereo)
+
+    def _key_local_corr_volume(self, f0, f1, flow, h, w, radius):
+        return M.corr_volume_key(flow.shape[-1])
+
+    def _key_flow_warp(self, f, flow, h, w):
+        return M.flow_warp_key(flow.shape[-1])
+
+    def _key_propagate_local(self, q, k, flow, h, w, radius):
+        return M.propagate_key(radius, q.stride(-2), k.stride(-2), flow.shape[-1])
+
+    def _key_depth_corr_softmax(self, f0, f1, K, Kinv, pose, cand, h, w, from_argmax):
+        return M.depth_key(cand.numel(), from_argmax)
+
+    def _key_convex_upsample(self, flow, mask, factor, mult):
+        return M.convex_key(factor, flow.shape[-1], mult)
+
+    def _key_upsample2x(self, flow, mult):
+        return M.upsample2x_key(flow.shape[-1])
+
+    def _key_add_position(self, x, table, h, w):
+        return M.add_position_key()
+
+    def _key_conv7x7_small(self, in0, in1, nchw, weight, bias, stride, relu, scale, shift, out_f32, out_split):
+        return M.conv7x7_key(weight.shape[1], stride, nchw, in1 is not None, scale is not None, out_f32 is not None,
+                             out_split is not None)
+
+
+CENSUS_RES = {"flow": (480, 832), "stereo": (544, 960), "depth": (384, 512)}
+
 
 def test_launch_census_of_bench_workloads(monkeypatch):
-    """One pair of every bench.py workload at its real resolution; every conv / attention / expectation dispatch key it
-    launches must be one the case tables above test."""
+    """One pair of every workload in spec.WORKLOADS at its real resolution; every conv / attention / expectation /
+    matching-path dispatch key it launches must be one the case tables here or in tests/test_matching_edges_gpu.py test."""
     import unimatch_b200.unimatch as um
     from unimatch_b200 import UniMatch
     from unimatch_b200.spec import WORKLOADS
     from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict
     census = _Census(um._OPS)
     monkeypatch.setattr(um, "_OPS", census)
-    for wl, H, W in (("gmflow-scale1", 480, 832), ("gmstereo-scale2", 544, 960), ("gmflow-scale2-regrefine6", 480, 832),
-                     ("gmdepth-scale1-regrefine1", 384, 512)):
-        cfg = WORKLOADS[wl]
+    for wl, cfg in WORKLOADS.items():
+        H, W = CENSUS_RES[cfg["model"]["task"]]
         model = UniMatch(**cfg["model"]).eval()
         model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
         model = model.cuda()
@@ -457,6 +488,7 @@ def test_launch_census_of_bench_workloads(monkeypatch):
         with torch.no_grad():
             model(inp["img0"], inp["img1"], intrinsics=inp.get("intrinsics"), pose=inp.get("pose"), **cfg["call"])
         torch.cuda.synchronize()
+        print("census: ran", wl, H, W)
     for key in sorted(census.keys, key=str):
         print("census:", key)
     missing = census.keys - covered_keys()

@@ -332,3 +332,499 @@ def test_instance_norm_stats_need_shifted_sums(ratio):
     if ratio >= 100:
         _, r_bad = emu_in_stats(x, False)
         assert abs(r_bad / rstd.item() - 1) > 1e-6
+
+
+# ---- matching-path kernels: fp32 emulations of um_local.cu / um_local_stencil.cu / um_misc.cu / um_stem.cu ---------
+F32 = torch.float32
+SQRT_C32 = torch.tensor(math.sqrt(C), dtype=F32)
+
+
+def fma(a, b, c):
+    """fmaf: the exact product plus c, rounded once to fp32."""
+    return (a.double() * b.double() + c.double()).float()
+
+
+def norm_window(p, size):
+    c = torch.tensor(float(size - 1), dtype=F32) / 2.0
+    return (p - c) / c
+
+
+def norm_sample(p, size):
+    return 2.0 * p / torch.tensor(float(size - 1), dtype=F32) - 1.0
+
+
+def unnorm(g, size):
+    return ((g + 1.0) / 2.0) * torch.tensor(float(size - 1), dtype=F32)
+
+
+def emu_taps(img, b, ix, iy, defect=None):
+    """sample() of um_local.cu on fp32 img [B, h, w, C] at fp32 positions [P, K]: make_tap weights, the four taps in ATen
+    order as FMAs, zeros outside (defect "replicate": border taps clamped)."""
+    h, w = img.shape[1], img.shape[2]
+    fx, fy = torch.floor(ix), torch.floor(iy)
+    x0, y0 = fx.long(), fy.long()
+    xe, ye = fx + 1.0, fy + 1.0
+    wts = ((xe - ix) * (ye - iy), (ix - fx) * (ye - iy), (xe - ix) * (iy - fy), (ix - fx) * (iy - fy))
+    acc = torch.zeros(ix.shape + (img.shape[-1],), dtype=F32)
+    bb = b.view(-1, *([1] * (ix.dim() - 1))).expand_as(x0)
+    for wt, (dy, dx) in zip(wts, ((0, 0), (0, 1), (1, 0), (1, 1))):
+        yy, xx = y0 + dy, x0 + dx
+        ok = (yy >= 0) & (yy < h) & (xx >= 0) & (xx < w)
+        if defect == "replicate":
+            ok = torch.ones_like(ok)
+        v = img[bb, yy.clamp(0, h - 1), xx.clamp(0, w - 1)]
+        acc = torch.where(ok[..., None], fma(wt[..., None], v, acc), acc)
+    return acc
+
+
+def emu_dot8(a, v):
+    """dot_partial + reduce8: lane `sub` chains 16 FMAs over channels sub*4 + 32 i + j, then three xor-shuffle adds.
+    a [P, C], v [P, K, C] fp32 -> [P, K]."""
+    va = v.view(*v.shape[:-1], 4, 8, 4)                                  # [.., i, sub, j]
+    aa = a.view(a.shape[0], 1, 4, 8, 4).expand_as(va)
+    s = torch.zeros(va.shape[:-3] + (8,), dtype=F32)
+    for i in range(4):
+        for j in range(4):
+            s = fma(aa[..., i, :, j], va[..., i, :, j], s)
+    for m in (4, 2, 1):
+        s = s + s[..., torch.arange(8) ^ m]
+    return s[..., 0]
+
+
+def emu_online(logits, vals):
+    """The kernels' online softmax over the taps in order: m, l and the value sums in fp32 with FMA rescales.
+    logits [P, K], vals [P, K, d] -> (l, sums [P, d], m)."""
+    P, K = logits.shape
+    m = torch.full((P,), -math.inf)
+    l = torch.zeros(P)
+    acc = torch.zeros((P, vals.shape[-1]))
+    for k in range(K):
+        s = logits[:, k]
+        mn = torch.maximum(m, s)
+        al, p = torch.exp(m - mn), torch.exp(s - mn)
+        l = fma(l, al, p)
+        acc = fma(acc, al[:, None], (p[:, None] * vals[:, k]))
+        m = mn
+    return l, acc, m
+
+
+def emu_merge(parts):
+    l, acc, m = parts[0]
+    for l2, a2, m2 in parts[1:]:
+        mn = torch.maximum(m, m2)
+        a0, a1 = torch.exp(m - mn), torch.exp(m2 - mn)
+        l, acc, m = fma(l, a0, l2 * a1), fma(acc, a0[:, None], a2 * a1[:, None]), mn
+    return l, acc, m
+
+
+def emu_local_corr_softmax(f0, f1, ry, rx, stereo, pix, stencil, defect=None):
+    B, h, w, _ = f0.shape
+    b, y, x = pix
+    dy, dx = ref64.window_offsets(ry, rx)
+    sy, sx = y[:, None] + dy, x[:, None] + dx
+    valid = (sx >= 0) & (sx < w) & (sy >= 0) & (sy < h)
+    a = f0[b, y, x]
+    if stencil:                                          # integer taps, one FMA chain over the 128 channels
+        v = f1[b[:, None].expand_as(sx), sy.clamp(0, h - 1), sx.clamp(0, w - 1)] * valid[..., None]
+        if defect == "drop_halo_col":                   # the last halo column of the 32-wide tile is never staged
+            v = v * (sx != (x // 32 * 32 + 35)[:, None])[..., None]
+        s = torch.zeros(sx.shape, dtype=F32)
+        for c in range(C):
+            s = fma(a[:, None, c], v[..., c], s)
+    else:
+        ix = unnorm(norm_window(sx.float(), w), w)
+        iy = unnorm(norm_window(sy.float(), h), h)
+        s = emu_dot8(a, emu_taps(f1, b, ix, iy))
+    s = s / SQRT_C32
+    if defect != "oob_logit0":
+        s = torch.where(valid, s, torch.full_like(s, -1e9))
+    vals = torch.stack((sx, sy), -1).float()
+    if stencil:
+        nrow = 2 * rx + 1
+        rows = [(0, 1), (2, 3), (4, 5), (6, 7), (8,)]
+        if defect == "drop_last_row":
+            rows = rows[:-1]
+        parts = [emu_online(s[:, r[0] * nrow:(r[-1] + 1) * nrow], vals[:, r[0] * nrow:(r[-1] + 1) * nrow]) for r in rows]
+        l, acc, _ = emu_merge(parts)
+    else:
+        l, acc, _ = emu_online(s, vals)
+    o = acc / l[:, None] - torch.stack((x, y), -1).float()
+    return -o[:, :1] if stereo else o
+
+
+def _feat(B, h, w, seed, scale=1.5):
+    gen = g(seed)
+    return torch.randn((B, h, w, C), generator=gen) * scale, torch.randn((B, h, w, C), generator=gen) * scale
+
+
+def _sub(B, h, w, seed, tx=(), ty=()):
+    return ref64.pixel_subset(B, h, w, g(seed), tx, ty, n_seam=400, n_rand=200)
+
+
+LCS_CPU = [
+    # name, B, h, w, ry, rx, stereo, stencil
+    ("stencil_18x70", 2, 18, 70, 4, 4, False, True),
+    ("gather_flow_r3", 1, 14, 23, 3, 3, False, False),
+    ("gather_stereo", 2, 10, 40, 0, 4, True, False),
+]
+
+
+@pytest.mark.parametrize("name,B,h,w,ry,rx,stereo,stencil", LCS_CPU)
+def test_local_corr_softmax64_matches_oracle_and_emulation(name, B, h, w, ry, rx, stereo, stencil):
+    f0, f1 = _feat(B, h, w, 200 + w)
+    pix = _sub(B, h, w, 201, (32,), (8,))
+    ref, bnd = ref64.local_corr_softmax64(f0, f1, ry, rx, stereo, pix, stencil)
+    oracle = refops.local_corr_softmax(f0, f1, h, w, ry, rx, stereo)[pix]
+    _, bnd_g = ref64.local_corr_softmax64(f0, f1, ry, rx, stereo, pix, False)
+    ref64.check(name + " oracle", oracle, ref, bnd_g)                    # the oracle's taps go through grid_sample
+    r = ref64.check(name + " emulation", emu_local_corr_softmax(f0, f1, ry, rx, stereo, pix, stencil), ref, bnd)
+    assert r < 0.5
+
+
+@pytest.mark.parametrize("defect,case", [("drop_last_row", "stencil_18x70"), ("drop_halo_col", "stencil_18x70"),
+                                         ("oob_logit0", "stencil_18x70"), ("oob_logit0", "gather_stereo")])
+def test_local_corr_softmax64_rejects_defects(defect, case):
+    name, B, h, w, ry, rx, stereo, stencil = next(c for c in LCS_CPU if c[0] == case)
+    f0, f1 = _feat(B, h, w, 200 + w)
+    pix = _sub(B, h, w, 201, (32,), (8,))
+    ref, bnd = ref64.local_corr_softmax64(f0, f1, ry, rx, stereo, pix, stencil)
+    rejects(name + " " + defect, emu_local_corr_softmax(f0, f1, ry, rx, stereo, pix, stencil, defect), ref, bnd)
+
+
+def test_local_corr_softmax64_translation_property():
+    """f1 = f0 shifted by (dx, dy): away from the border the window's peak is the shift (peaked features)."""
+    B, h, w = 1, 24, 40
+    f0, _ = _feat(B, h, w, 210, 4.0)
+    f1 = torch.roll(f0, (2, -3), (1, 2))                  # f1[y + 2, x - 3] = f0[y, x]
+    ys, xs = torch.meshgrid(torch.arange(6, h - 6), torch.arange(6, w - 6), indexing="ij")
+    pix = (torch.zeros(ys.numel(), dtype=torch.long), ys.reshape(-1), xs.reshape(-1))
+    ref, bnd = ref64.local_corr_softmax64(f0, f1, 4, 4, False, pix, True)
+    assert torch.allclose(ref, torch.tensor([-3.0, 2.0], dtype=torch.float64).expand_as(ref), atol=1e-9)
+
+
+def emu_corr_volume(f0, f1, flow, radius, pix, defect=None):
+    B, h, w, _ = f0.shape
+    b, y, x = pix
+    fl = flow[b, y, x].float()
+    u, v = (fl[:, 0], fl[:, 1]) if fl.shape[-1] == 2 else ((fl[:, 0] if defect == "disp_plus" else -fl[:, 0]), 0 * fl[:, 0])
+    cx = unnorm(norm_window(x.float() + u, w), w)
+    cy = unnorm(norm_window(y.float() + v, h), h)
+    fx, fy = torch.floor(cx), torch.floor(cy)
+    xe, ye = fx + 1.0, fy + 1.0
+    wnw, wne, wsw, wse = (xe - cx) * (ye - cy), (cx - fx) * (ye - cy), (xe - cx) * (cy - fy), (cx - fx) * (cy - fy)
+    if defect == "nesw_swap":
+        wne, wsw = wsw, wne
+    G = 2 * radius + 2
+    gy, gx = torch.meshgrid(torch.arange(G), torch.arange(G), indexing="ij")
+    yy = fy.long()[:, None] - radius + gy.reshape(-1)
+    xx = fx.long()[:, None] - radius + gx.reshape(-1)
+    ok = (yy >= 0) & (yy < h) & (xx >= 0) & (xx < w)
+    if defect == "replicate":
+        ok = torch.ones_like(ok)
+    rows = f1[b[:, None].expand_as(yy), yy.clamp(0, h - 1), xx.clamp(0, w - 1)] * ok[..., None]
+    d = emu_dot8(f0[b, y, x], rows).view(-1, G, G)
+    n = 2 * radius + 1
+    r = d[:, :n, :n] * wnw[:, None, None]
+    r = fma(d[:, :n, 1:], wne[:, None, None], r)
+    r = fma(d[:, 1:, :n], wsw[:, None, None], r)
+    r = fma(d[:, 1:, 1:], wse[:, None, None], r)
+    return (r / SQRT_C32).reshape(-1, n * n)
+
+
+def _flows(kind, B, h, w, fd, seed):
+    gen = g(seed)
+    shp = (B, h, w, fd)
+    if kind == "sigma12":
+        return torch.randn(shp, generator=gen) * 12
+    if kind == "frac":
+        return torch.randint(-6, 7, shp, generator=gen).float() + torch.rand(shp, generator=gen) * 0.8 + 0.1
+    if kind == "half":
+        return torch.randint(-3, 4, shp, generator=gen).float() + 0.5
+    if kind == "near_int":
+        return torch.randint(-4, 5, shp, generator=gen).float() + (torch.rand(shp, generator=gen) - 0.5) * 2e-6
+    raise ValueError(kind)
+
+
+CV_CPU = [("sigma12", 2), ("frac", 2), ("frac", 1), ("near_int", 2)]
+
+
+@pytest.mark.parametrize("kind,fd", CV_CPU)
+def test_corr_volume64_and_flow_warp64_match_oracle_and_emulation(kind, fd):
+    B, h, w = 2, 14, 40
+    f0, f1 = _feat(B, h, w, 220 + fd)
+    fl = _flows(kind, B, h, w, fd, 221)
+    pix = _sub(B, h, w, 222)
+    ref, bnd = ref64.local_corr_volume64(f0, f1, fl, 4, pix)
+    ref64.check("corr volume %s fd %d oracle" % (kind, fd), refops.local_corr_volume(f0, f1, fl, h, w, 4)[pix], ref, bnd)
+    r = ref64.check("corr volume %s fd %d emulation" % (kind, fd), emu_corr_volume(f0, f1, fl, 4, pix), ref, bnd)
+    assert r < 0.5
+    ref, bnd = ref64.flow_warp64(f1, fl, pix)
+    ref64.check("flow warp %s fd %d oracle" % (kind, fd), refops.flow_warp(f1, fl, h, w)[pix], ref, bnd)
+    r = ref64.check("flow warp %s fd %d emulation" % (kind, fd), emu_flow_warp(f1, fl, pix), ref, bnd)
+    assert r < 0.5
+
+
+def emu_flow_warp(f, flow, pix, defect=None):
+    B, h, w, _ = f.shape
+    b, y, x = pix
+    fl = flow[b, y, x].float()
+    u, v = (fl[:, 0], fl[:, 1]) if fl.shape[-1] == 2 else ((fl[:, 0] if defect == "disp_plus" else -fl[:, 0]), 0 * fl[:, 0])
+    ix = unnorm(norm_sample(x.float() + u, w), w)[:, None]
+    iy = unnorm(norm_sample(y.float() + v, h), h)[:, None]
+    return emu_taps(f, b, ix, iy, defect)[:, 0]
+
+
+@pytest.mark.parametrize("defect,kind,fd", [("replicate", "sigma12", 2), ("nesw_swap", "frac", 2),
+                                            ("disp_plus", "frac", 1)])
+def test_corr_volume64_and_flow_warp64_reject_defects(defect, kind, fd):
+    B, h, w = 2, 14, 40
+    f0, f1 = _feat(B, h, w, 220 + fd)
+    fl = _flows(kind, B, h, w, fd, 221)
+    pix = _sub(B, h, w, 222)
+    ref, bnd = ref64.local_corr_volume64(f0, f1, fl, 4, pix)
+    rejects("corr volume " + defect, emu_corr_volume(f0, f1, fl, 4, pix, defect), ref, bnd)
+    if defect != "nesw_swap":
+        ref, bnd = ref64.flow_warp64(f1, fl, pix)
+        rejects("flow warp " + defect, emu_flow_warp(f1, fl, pix, defect), ref, bnd)
+
+
+def emu_propagate(q, k, flow, radius, pix, defect=None):
+    B, h, w, _ = q.shape
+    b, y, x = pix
+    dy, dx = ref64.window_offsets(radius, radius)
+    sy, sx = y[:, None] + dy, x[:, None] + dx
+    ok = (sx >= 0) & (sx < w) & (sy >= 0) & (sy < h)
+    bb = b[:, None].expand_as(sy)
+    kv = k[bb, sy.clamp(0, h - 1), sx.clamp(0, w - 1)] * ok[..., None]
+    s = emu_dot8(q[b, y, x].contiguous(), kv) / SQRT_C32
+    s = torch.where(ok, s, torch.full_like(s, -1e9) if defect == "exclude_oob" else torch.zeros_like(s))
+    vals = flow[bb, sy.clamp(0, h - 1), sx.clamp(0, w - 1)] * ok[..., None]
+    l, acc, _ = emu_online(s, vals)
+    return acc / l[:, None]
+
+
+@pytest.mark.parametrize("fd", [1, 2])
+def test_propagate_local64_matches_oracle_and_emulation(fd):
+    B, h, w = 2, 12, 30
+    gen = g(230 + fd)
+    qk = torch.randn((B, h * w, 256), generator=gen) * 1.5
+    q, k = qk[..., :128].reshape(B, h, w, C), qk[..., 128:].reshape(B, h, w, C)
+    fl = torch.randn((B, h, w, fd), generator=gen) * 5
+    pix = _sub(B, h, w, 231)
+    ref, bnd = ref64.propagate_local64(q, k, fl, 1, pix)
+    oracle = refops.propagate_local(q.contiguous(), k.contiguous(), fl, h, w, 1)[pix]
+    ref64.check("propagate fd %d oracle" % fd, oracle, ref, bnd)
+    r = ref64.check("propagate fd %d emulation" % fd, emu_propagate(q, k, fl, 1, pix), ref, bnd)
+    assert r < 0.5
+    rejects("propagate exclude out-of-image keys", emu_propagate(q, k, fl, 1, pix, "exclude_oob"), ref, bnd)
+
+
+def depth_setup(B, h, w, seed, kind="bidir", neg=False):
+    """Features, cameras built by UniMatch.depth_cameras (at 1/8 resolution, bidirectional) and the workloads' 64
+    inverse-depth candidates.  kind: "bidir" (small motion), "rotated", "forward" (2 units forward: near candidates project
+    behind the camera)."""
+    import types
+    from unimatch_b200 import UniMatch
+    gen = g(seed)
+    f0 = torch.randn((B, h, w, C), generator=gen) * 1.5
+    f1 = torch.randn((B, h, w, C), generator=gen) * 1.5
+    if neg:                                                 # every in-image correlation negative: ties at logit 0 decide
+        f0, f1 = f0.abs(), -f1.abs()
+    n = (B + 1) // 2
+    intr = torch.tensor([[500.0, 0, 8 * w / 2 - 3], [0, 490.0, 8 * h / 2 + 2], [0, 0, 1]]).repeat(n, 1, 1)
+    pose = torch.eye(4).repeat(n, 1, 1)
+    ang = 0.15 if kind == "rotated" else 0.02
+    ca, sa = math.cos(ang), math.sin(ang)
+    pose[:, 0, 0], pose[:, 0, 2], pose[:, 2, 0], pose[:, 2, 2] = ca, sa, -sa, ca
+    # "forward": the mirror image of a point behind the camera lands inside the image, so only the z clamp keeps it out
+    pose[:, :3, 3] = torch.tensor([0.0, 0.0, -2.0] if kind == "forward" else [0.3, -0.05, 0.1])
+    cams = UniMatch.depth_cameras(types.SimpleNamespace(_cands={}), intr, pose, 8, 1.0 / 10, 1.0 / 0.5, 64, True)
+    return f0, f1, cams
+
+
+def emu_depth(f0, f1, cams, pix, from_argmax, defect=None):
+    B, h, w, _ = f0.shape
+    b, y, x = pix
+    Ki, Kb, Pm, cand = cams["K_inv"][b], cams["K"][b], cams["pose"][b], cams["cand"]
+    fx, fy = x.float(), y.float()
+    X = [fma(Ki[:, r, 2], torch.ones(()), fma(Ki[:, r, 1], fy, Ki[:, r, 0] * fx)) for r in range(3)]
+    Xr = [fma(Pm[:, r, 2], X[2], fma(Pm[:, r, 1], X[1], Pm[:, r, 0] * X[0])) for r in range(3)]
+    a = f0[b, y, x]
+    logits = []
+    for d in range(cand.numel()):
+        depth = 1.0 / cand[d]
+        Pt = [fma(Xr[r], depth, Pm[:, r, 3]) for r in range(3)]
+        pr = [fma(Kb[:, r, 2], Pt[2], fma(Kb[:, r, 1], Pt[1], Kb[:, r, 0] * Pt[0])) for r in range(3)]
+        z = pr[2] if defect == "no_zclamp" else torch.clamp(pr[2], min=1e-3)
+        ix = unnorm(norm_sample(pr[0] / z, w), w)[:, None]
+        iy = unnorm(norm_sample(pr[1] / z, h), h)[:, None]
+        logits.append(emu_dot8(a, emu_taps(f1, b, ix, iy))[:, 0] / SQRT_C32)
+    s = torch.stack(logits, 1)
+    if from_argmax:
+        best = torch.zeros(s.shape[0])
+        m = torch.full((s.shape[0],), -math.inf)
+        for d in range(cand.numel()):
+            better = s[:, d] >= m if defect == "last_max" else s[:, d] > m
+            best = torch.where(better, cand[d], best)
+            m = torch.maximum(m, s[:, d])
+        return best
+    l, acc, _ = emu_online(s, cand.view(1, -1, 1).expand(s.shape[0], -1, 1))
+    return (acc / l[:, None])[:, 0]
+
+
+@pytest.mark.parametrize("kind", ["bidir", "rotated", "forward"])
+def test_depth_corr64_matches_oracle_and_emulation(kind):
+    B, h, w = 2, 12, 16
+    f0, f1, cams = depth_setup(B, h, w, 240, kind)
+    pix = _sub(B, h, w, 241)
+    ref, bnd, s, ds = ref64.depth_corr64(f0, f1, cams["K"], cams["K_inv"], cams["pose"], cams["cand"], pix)
+    args = (f0, f1, cams["K"], cams["K_inv"], cams["pose"], cams["cand"], h, w)
+    ref64.check("depth %s oracle" % kind, refops.depth_corr_softmax(*args, False)[pix][:, 0], ref, bnd)
+    r = ref64.check("depth %s emulation" % kind, emu_depth(f0, f1, cams, pix, False), ref, bnd)
+    assert r < 0.5
+    ref64.check_argmax("depth %s oracle argmax" % kind, refops.depth_corr_softmax(*args, True)[pix][:, 0], cams["cand"], s,
+                       ds)
+    ref64.check_argmax("depth %s emulation argmax" % kind, emu_depth(f0, f1, cams, pix, True), cams["cand"], s, ds)
+    if kind == "forward":
+        rejects("depth without the z clamp", emu_depth(f0, f1, cams, pix, False, "no_zclamp"), ref, bnd)
+
+
+def test_depth_corr64_argmax_rejects_last_maximum():
+    """Negative in-image correlations: candidates projecting outside (logit exactly 0) tie for the maximum, and
+    torch.argmax takes the first of them."""
+    B, h, w = 2, 12, 16
+    f0, f1, cams = depth_setup(B, h, w, 250, "forward", neg=True)
+    pix = _sub(B, h, w, 251)
+    _, _, s, ds = ref64.depth_corr64(f0, f1, cams["K"], cams["K_inv"], cams["pose"], cams["cand"], pix)
+    ref64.check_argmax("depth argmax ties", emu_depth(f0, f1, cams, pix, True), cams["cand"], s, ds)
+    with pytest.raises(AssertionError):
+        ref64.check_argmax("depth argmax last max", emu_depth(f0, f1, cams, pix, True, "last_max"), cams["cand"], s, ds)
+
+
+def emu_convex(flow, mask, factor, mult, defect=None):
+    B, h, w, fd = flow.shape
+    FF = factor * factor
+    m = mask.view(B, h, w, 9, FF)
+    e = torch.exp(m - m.amax(3, keepdim=True))
+    fl = torch.nn.functional.pad(flow * mult, (0, 0, 1, 1, 1, 1))
+    inside = torch.nn.functional.pad(torch.ones((B, h, w, 1)), (0, 0, 1, 1, 1, 1))
+    nb = torch.stack([fl[:, ty:ty + h, tx:tx + w] for ty in range(3) for tx in range(3)], 3)      # [B, h, w, 9, fd]
+    ins = torch.stack([inside[:, ty:ty + h, tx:tx + w] for ty in range(3) for tx in range(3)], 3)
+    den = torch.zeros((B, h, w, FF))
+    for t in range(9):
+        den = den + e[:, :, :, t] * (ins[:, :, :, t] if defect == "inimage_norm" else 1.0)
+    acc = torch.zeros((B, h, w, FF, fd))
+    for t in range(9):
+        acc = fma((e[:, :, :, t] / den)[..., None], nb[:, :, :, t, None, :], acc)
+    return acc.view(B, h, w, factor, factor, fd).permute(0, 5, 1, 3, 2, 4).reshape(B, fd, h * factor, w * factor)
+
+
+@pytest.mark.parametrize("factor,fd,mult,scale", [(4, 2, 4, 3.0), (8, 1, 1, 3.0), (4, 2, 4, 60.0)])
+def test_convex_upsample64_matches_oracle_and_emulation(factor, fd, mult, scale):
+    B, h, w = 2, 5, 7
+    gen = g(260 + factor + fd)
+    fl = torch.randn((B, h, w, fd), generator=gen) * 4
+    mask = torch.randn((B, h, w, 9 * factor * factor), generator=gen) * scale
+    ref, bnd = ref64.convex_upsample64(fl, mask, factor, mult)
+    name = "convex F %d fd %d mult %d scale %g" % (factor, fd, mult, scale)
+    ref64.check(name + " oracle", refops.convex_upsample(fl, mask, factor, float(mult)), ref, bnd)
+    assert ref64.check(name + " emulation", emu_convex(fl, mask, factor, mult), ref, bnd) < 0.5
+    rejects(name + " in-image normalisation", emu_convex(fl, mask, factor, mult, "inimage_norm"), ref, bnd)
+
+
+def emu_upsample2x(flow, mult, defect=None):
+    B, h, w, fd = flow.shape
+    H, W = 2 * h, 2 * w
+    f32 = lambda v: torch.tensor(float(v), dtype=F32)
+    Y, X = torch.arange(H).float(), torch.arange(W).float()
+    if defect == "align_false":
+        fy, fx = ((Y + 0.5) * 0.5 - 0.5).clamp(min=0), ((X + 0.5) * 0.5 - 0.5).clamp(min=0)
+    else:
+        fy = (f32(h - 1) / f32(H - 1) if H > 1 else f32(0)) * Y
+        fx = (f32(w - 1) / f32(W - 1) if W > 1 else f32(0)) * X
+    y0, x0 = fy.long(), fx.long()
+    y1, x1 = y0 + (y0 < h - 1).long(), x0 + (x0 < w - 1).long()
+    ly, lx = (fy - y0.float())[:, None, None], (fx - x0.float())[None, :, None]
+    hy, hx = 1.0 - ly, 1.0 - lx
+    v = lambda yy, xx: flow[:, yy][:, :, xx]
+    return (hy * (hx * v(y0, x0) + lx * v(y0, x1)) + ly * (hx * v(y1, x0) + lx * v(y1, x1))) * mult
+
+
+@pytest.mark.parametrize("h,w,fd", [(6, 9, 2), (1, 12, 1), (7, 5, 1)])
+def test_upsample2x64_matches_oracle_and_emulation(h, w, fd):
+    fl = torch.randn((2, h, w, fd), generator=g(270 + h)) * 6
+    ref, bnd = ref64.upsample2x64(fl, 2.0)
+    ref64.check("upsample2x %dx%d oracle" % (h, w), refops.upsample2x(fl, 2.0), ref, bnd)
+    assert ref64.check("upsample2x %dx%d emulation" % (h, w), emu_upsample2x(fl, 2.0), ref, bnd) < 0.5
+    rejects("upsample2x align_corners=False", emu_upsample2x(fl, 2.0, "align_false"), ref, bnd)
+
+
+def test_add_position_ref_matches_refops():
+    gen = g(280)
+    x = torch.randn((3, 12, 20, C), generator=gen)
+    table = torch.randn((6, 5, C), generator=gen)
+    want = torch.empty_like(x)
+    for yy in range(12):
+        for xx in range(20):
+            want[:, yy, xx] = x[:, yy, xx] + table[yy % 6, xx % 5]
+    assert torch.equal(ref64.add_position_ref(x, table, 12, 20), want)
+    assert torch.equal(refops.add_position(x, table, 12, 20), want)
+
+
+STEM_SCALE = [1.0 / (255.0 * s_) for s_ in (0.229, 0.224, 0.225)]
+STEM_SHIFT = [-m_ / s_ for m_, s_ in zip((0.485, 0.456, 0.406), (0.229, 0.224, 0.225))]
+
+
+def stem_images(n, H, W, seed):
+    """Raw pixels in [0, 255] with saturated 0 and 255 blocks."""
+    gen = g(seed)
+    x = torch.rand((n, 3, H, W), generator=gen) * 255
+    x[:, :, :H // 3, :W // 4] = 0.0
+    x[:, :, H // 2:, W // 2:W // 2 + W // 5] = 255.0
+    return x.round()
+
+
+def emu_stem(x, weight, bias, stride, relu, scale, shift, defect=None):
+    F_ = torch.nn.functional
+    if scale is not None:
+        sc, sh = torch.tensor(scale).view(1, -1, 1, 1), torch.tensor(shift).view(1, -1, 1, 1)
+        if defect == "pad_shift":                           # normalising after the zero padding
+            v = F_.pad(x, (3, 3, 3, 3)) * sc + sh
+            y = F_.conv2d(v, weight, bias, stride=stride)
+        else:
+            y = F_.conv2d(fma(x, sc.expand_as(x), sh.expand_as(x)), weight, bias, stride=stride, padding=3)
+    else:
+        y = F_.conv2d(x, weight, bias, stride=stride, padding=3)
+    y = torch.relu(y) if relu else y
+    return y.permute(0, 2, 3, 1)
+
+
+@pytest.mark.parametrize("norm", [True, False])
+def test_conv7x7_64_stem_matches_oracle_and_emulation(norm):
+    x = stem_images(2, 37, 54, 290)
+    if not norm:
+        x = x / 255.0
+    wt = torch.randn((64, 3, 7, 7), generator=g(291)) * (2.0 / 147) ** 0.5
+    sc, sh = (STEM_SCALE, STEM_SHIFT) if norm else (None, None)
+    ref, bnd = ref64.conv7x7_64(x, wt, None, 2, False, sc, sh)
+    out = torch.empty(ref.shape, dtype=F32)
+    refops.conv7x7_small(x[:1], x[1:], True, wt, None, 2, False, sc, sh, out, None)
+    ref64.check("stem norm %s oracle" % norm, out, ref, bnd)
+    assert ref64.check("stem norm %s emulation" % norm, emu_stem(x, wt, None, 2, False, sc, sh), ref, bnd) < 0.5
+    if norm:
+        rejects("stem padded with the shift", emu_stem(x, wt, None, 2, False, sc, sh, "pad_shift"), ref, bnd)
+
+
+@pytest.mark.parametrize("cin", [1, 2])
+def test_conv7x7_64_flow_encoder_matches_oracle(cin):
+    gen = g(295 + cin)
+    fl = torch.randn((2, 15, 22, cin), generator=gen) * 20
+    wt = torch.randn((128, cin, 7, 7), generator=gen) * (2.0 / (49 * cin)) ** 0.5
+    bias = torch.randn(128, generator=gen) * 0.1
+    ref, bnd = ref64.conv7x7_64(fl.permute(0, 3, 1, 2), wt, bias, 1, True)
+    out = torch.empty(ref.shape, dtype=F32)
+    split = torch.empty((2,) + ref.shape, dtype=torch.float16)
+    refops.conv7x7_small(fl, None, False, wt, bias, 1, True, None, None, out, split)
+    ref64.check("flow encoder cin %d oracle" % cin, out, ref, bnd)
+    ref64.check("flow encoder cin %d oracle split" % cin, split[0].double() + split[1].double(), ref,
+                ref64.split_out_bound(ref, bnd))
