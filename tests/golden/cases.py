@@ -3,6 +3,7 @@ and `tests/test_oracle_golden.py` (runs the ORACLE against the stored reference 
 
 Every case: seeded inputs (regenerated, never stored) -> reference output (stored in golden.pt).
 """
+import math
 import os
 import sys
 
@@ -211,6 +212,75 @@ E2E_NOISE_FACTOR = 8.0    # stated tolerance: mean error <= 8 x self-noise (+ 1e
 
 def e2e_tolerance(name):
     return E2E_NOISE_FACTOR * E2E_NOISE[name] + 1e-4
+
+
+def distinct_cameras(B, h, w, seed=5):
+    """Per-pair cameras for images of h x w: intrinsics [B,3,3] whose focal length, aspect ratio and principal point all
+    differ between pairs, and relative poses [B,4,4] with a rotation about all three axes (up to 3 degrees each) and a
+    translation, different for every pair."""
+    g = _g(seed)
+    K, pose = torch.zeros((B, 3, 3)), torch.eye(4).repeat(B, 1, 1)
+    for b in range(B):
+        r = torch.rand(4, generator=g)
+        fx = w * (0.7 + 0.5 * r[0].item())
+        K[b] = torch.tensor([[fx, 0.0, w * (0.4 + 0.2 * r[2].item())],
+                             [0.0, fx * (0.85 + 0.3 * r[1].item()), h * (0.4 + 0.2 * r[3].item())], [0.0, 0.0, 1.0]])
+        ax, ay, az = ((torch.rand(3, generator=g) * 2 - 1) * 0.05).tolist()
+        rx = torch.tensor([[1.0, 0, 0], [0, math.cos(ax), -math.sin(ax)], [0, math.sin(ax), math.cos(ax)]])
+        ry = torch.tensor([[math.cos(ay), 0, math.sin(ay)], [0, 1.0, 0], [-math.sin(ay), 0, math.cos(ay)]])
+        rz = torch.tensor([[math.cos(az), -math.sin(az), 0], [math.sin(az), math.cos(az), 0], [0, 0, 1.0]])
+        pose[b, :3, :3] = rz @ ry @ rx
+        pose[b, :3, 3] = torch.tensor([0.05 + 0.1 * b / max(B - 1, 1), 0.0, 0.0]) + (torch.rand(3, generator=g) * 2 - 1) * 0.03
+    return K, pose
+
+
+# ---- batch 3 cases: distinct pairs, bidirectional modes and per-pair cameras ------------------------------------------
+# (workload, H, W, extra forward kwargs); the depth cases get the cameras of `distinct_cameras`
+BATCH3_CASES = {
+    "b3_gmflow_s1_bidir": ("gmflow-scale1", 64, 96, dict(pred_bidir_flow=True)),
+    "b3_gmflow_s2_rr6_bidir": ("gmflow-scale2-regrefine6", 64, 128, dict(pred_bidir_flow=True)),
+    "b3_gmstereo_s2": ("gmstereo-scale2", 128, 192, {}),
+    "b3_gmstereo_s2_rr3": ("gmstereo-scale2-regrefine3", 128, 192, {}),
+    "b3_gmdepth_s1": ("gmdepth-scale1", 128, 192, {}),
+    "b3_gmdepth_s1_rr1": ("gmdepth-scale1-regrefine1", 128, 192, {}),
+    "b3_gmdepth_s1_bidir": ("gmdepth-scale1", 96, 128, dict(pred_bidir_depth=True)),
+    "b3_gmdepth_s1_rr1_bidir": ("gmdepth-scale1-regrefine1", 96, 128, dict(pred_bidir_depth=True)),
+    "b3_gmdepth_s1_argmax": ("gmdepth-scale1", 96, 128, dict(depth_from_argmax=True)),
+}
+
+# Self-noise of the reference on these batches (tools/self_noise.py's `threads` probe: 1 against 8 CPU threads), largest
+# per-pair mean error; the tolerance of a pair is E2E_NOISE_FACTOR x this + 1e-4, as for E2E_CASES.
+BATCH3_NOISE = {
+    "b3_gmflow_s1_bidir": 9.7e-5,
+    "b3_gmflow_s2_rr6_bidir": 1.5e-2,
+    "b3_gmstereo_s2": 4.9e-4,
+    "b3_gmstereo_s2_rr3": 2.5e-3,
+    "b3_gmdepth_s1": 3.4e-6,
+    "b3_gmdepth_s1_rr1": 2.6e-6,
+    "b3_gmdepth_s1_bidir": 3.8e-6,
+    "b3_gmdepth_s1_rr1_bidir": 3.3e-6,
+    "b3_gmdepth_s1_argmax": 5.8e-6,
+}
+
+
+def batch3_setup(name, h=None, w=None):
+    """(cfg, state_dict, batch of 3 distinct pairs, call kwargs) of a BATCH3_CASES entry, optionally at another size."""
+    wl, h0, w0, extra = BATCH3_CASES[name]
+    h, w = h or h0, w or w0
+    cfg = WORKLOADS[wl]
+    sd = synthetic_state_dict(seed=326, damp=E2E_DAMP, **cfg["model"])
+    batch = synthetic_batch(cfg["model"]["task"], 3, h, w, first_index=7)
+    if cfg["model"]["task"] == "depth":
+        batch["intrinsics"], batch["pose"] = distinct_cameras(3, h, w)
+    call = dict(cfg["call"])
+    call.update(extra)
+    return cfg, sd, batch, call
+
+
+def oracle_forward(cfg, sd, batch, call):
+    mk = {k: cfg["model"][k] for k in ("num_scales", "upsample_factor", "reg_refine")}
+    return O.forward(sd, batch["img0"], batch["img1"], intrinsics=batch.get("intrinsics"), pose=batch.get("pose"),
+                     **mk, **call)["flow_preds"][-1]
 
 
 def epe(a, b):

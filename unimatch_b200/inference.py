@@ -333,6 +333,7 @@ class _PipelinedRunner:
         self.static_out = [None, None]
         self.use_graph = use_graph
         self.out_pin = [None, None]
+        self._held_buffers = []
 
     def _download(self, slot, out):
         if self.out_pin[slot] is None:
@@ -360,6 +361,9 @@ class _PipelinedRunner:
                 with torch.cuda.graph(g):
                     self.static_out[slot] = self._step(slot)
                 self.graphs[slot] = g
+            # the graphs hold the raw addresses of the module's cached planes; calls at other shapes may evict them from
+            # the module's caches, so the runner keeps them alive for as long as it may replay
+            self._held_buffers = self.model.cached_buffers()
             torch.cuda.synchronize()
 
     def _stage(self, slot, chunk):

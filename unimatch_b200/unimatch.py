@@ -389,6 +389,13 @@ class UniMatch(nn.Module):
             self._attn_ws[key] = buf
         return buf
 
+    def cached_buffers(self):
+        """The device buffers this module keeps between calls: the window-major attention operand planes and the zero-padded
+        plane buffers.  Each cache drops its entries once enough other shapes come along, and the caching allocator then hands
+        that memory to the next allocation.  A CUDA graph captured around a forward holds their raw addresses, so whoever
+        replays it must hold these tensors, taken just after the capture, for as long as the graph lives."""
+        return list(self._attn_ws.values()) + list(self._pad_ws.values())
+
     def _stage_transformer(self, P, x, h, w, attn_type, splits, tag="s0"):
         """FeatureTransformer.forward (transformer.py:226-294) on tokens x [N, L, 128], N = 2 x pairs.  Every Linear is a
         wgmma GEMM over token rows (activations travel as fp16 (hi, lo) planes [2, rows, C] between GEMMs); LayerNorm
@@ -725,7 +732,10 @@ class UniMatch(nn.Module):
         `forward` does for the images those features were encoded from (encoded with `encode_frames(..., task)`).
         Flow and depth.  Depth: `cameras` = `depth_cameras(...)` for these B pairs (then `intrinsics`, `pose` and
         `num_depth_candidates` are not read, and nothing here synchronises with the host), or `intrinsics` and `pose` as
-        `forward` takes them.  Stereo is not offered: its pairs share no view, so there is no encoding to reuse."""
+        `forward` takes them.  Stereo is not offered: its pairs share no view, so there is no encoding to reuse.
+        A caller who captures this call (or `forward`) in a CUDA graph of their own must keep the tensors of
+        `cached_buffers()`, taken just after the capture, for as long as they replay the graph: calls at other batch sizes or
+        shapes can evict them from the module's caches, and a replay would then write into memory another tensor owns."""
         if self.training:
             raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
         if task not in ("flow", "depth"):
