@@ -88,6 +88,8 @@ def test_infer_flow_video_argument_errors():
     frames = synthetic_video(3, 32, 48)
     with pytest.raises(ValueError):
         infer_flow_video(m, frames[:1], padding_factor=16, **kw)
+    with pytest.raises(ValueError):                                        # float frames must be planar [T,3,H,W]
+        infer_flow_video(m, frames.float(), padding_factor=16, **kw)
     with pytest.raises(ValueError):
         infer_flow_video(m, frames, padding_factor=16, fwd_bwd_consistency_check=True, **kw)
     with pytest.raises(ValueError):

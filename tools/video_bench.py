@@ -109,6 +109,23 @@ def run(args):
         sys.exit(1)
 
 
+def _video_step(runner, frames, out, key, pin_pose=None):
+    """(runner step on frames 1..B paired with frame 0, H2D bytes per step): B new uint8 frames (and, for depth, their
+    relative poses) copied from pinned memory, the step's `key` output copied back to `out`."""
+    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(runner.dev))]
+    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
+    pin_new = frames[1:].contiguous().pin_memory()
+
+    def step():
+        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
+            c.copy_(f)
+        runner.dev_in[0].copy_(pin_new, non_blocking=True)
+        if pin_pose is not None:
+            runner.pose_dev[0].copy_(pin_pose, non_blocking=True)
+        out.copy_(runner._step(0)[key], non_blocking=True)
+    return step, int(pin_new.numel() + (0 if pin_pose is None else pin_pose.numel() * 4))
+
+
 def _flow_steps(model, cfg, H, W, B, dev):
     """VideoFlowRunner step and pairwise forward on the same B pairs of a synthetic video"""
     from unimatch_b200.inference import VideoFlowRunner
@@ -116,24 +133,16 @@ def _flow_steps(model, cfg, H, W, B, dev):
     call = {k: v for k, v in cfg["call"].items() if k != "task"}
     frames = synthetic_video(B + 1, H, W, seed=77)                          # frame 0 = carried, frames 1..B = new
     runner = VideoFlowRunner(model, (H, W), B, dev, padding_factor=cfg["pad"], use_graph=False, **call)
-    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(dev))]
-    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
-    pin_new = frames[1:].contiguous().pin_memory()
     planar = frames.permute(0, 3, 1, 2).float()
     pin0, pin1 = planar[:-1].contiguous().pin_memory(), planar[1:].contiguous().pin_memory()
     out_v, out_p = torch.empty((B, 2, H, W)).pin_memory(), torch.empty((B, 2, H, W)).pin_memory()
-
-    def video_step():
-        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
-            c.copy_(f)
-        runner.dev_in[0].copy_(pin_new, non_blocking=True)
-        out_v.copy_(runner._step(0)["flow"], non_blocking=True)
+    video_step, io_v = _video_step(runner, frames, out_v, "flow")
 
     def pair_step():
         a, b = pin0.to(dev, non_blocking=True), pin1.to(dev, non_blocking=True)
         out_p.copy_(model(a, b, **cfg["call"])["flow_preds"][-1], non_blocking=True)
 
-    io = (int(pin_new.numel()), int((pin0.numel() + pin1.numel()) * 4))
+    io = (io_v, int((pin0.numel() + pin1.numel()) * 4))
     return video_step, pair_step, out_v, out_p, io, dict(kind="video", data="synthetic_video seed 77", value="flow")
 
 
@@ -148,9 +157,6 @@ def _depth_steps(model, cfg, H, W, B, dev):
     runner = DepthSequenceRunner(model, (H, W), B, dev, K, padding_factor=cfg["pad"], use_graph=False,
                                  min_depth=1.0 / call["max_depth"], max_depth=1.0 / call["min_depth"],
                                  num_depth_candidates=call["num_depth_candidates"], **kw)
-    runner.carry = [f.clone() for f in runner._encode(frames[:1].to(dev))]
-    saved = [c.clone() for c in runner.carry]                                # frame 0's pyramid
-    pin_new = frames[1:].contiguous().pin_memory()
     rel = torch.from_numpy(_relative_poses([p for p in poses.numpy()], False))
     pin_pose = rel.contiguous().pin_memory()
     mean, std = torch.tensor(IMAGENET_MEAN).view(1, 3, 1, 1), torch.tensor(IMAGENET_STD).view(1, 3, 1, 1)
@@ -158,21 +164,14 @@ def _depth_steps(model, cfg, H, W, B, dev):
     pin0, pin1 = planar[:-1].contiguous().pin_memory(), planar[1:].contiguous().pin_memory()
     pin_k = K[None].repeat(B, 1, 1).contiguous().pin_memory()
     out_v, out_p = torch.empty((B, H, W)).pin_memory(), torch.empty((B, H, W)).pin_memory()
-
-    def video_step():
-        for c, f in zip(runner.carry, saved):                                # same pairs every step: (0,1), (1,2), ...
-            c.copy_(f)
-        runner.dev_in[0].copy_(pin_new, non_blocking=True)
-        runner.pose_dev[0].copy_(pin_pose, non_blocking=True)
-        out_v.copy_(runner._step(0)["depth"], non_blocking=True)
+    video_step, io_v = _video_step(runner, frames, out_v, "depth", pin_pose)
 
     def pair_step():
         a, b = pin0.to(dev, non_blocking=True), pin1.to(dev, non_blocking=True)
         k, p = pin_k.to(dev, non_blocking=True), pin_pose.to(dev, non_blocking=True)
         out_p.copy_(model(a, b, intrinsics=k, pose=p, **call)["flow_preds"][-1], non_blocking=True)
 
-    io = (int(pin_new.numel() + pin_pose.numel() * 4),
-          int((pin0.numel() + pin1.numel() + pin_k.numel() + pin_pose.numel()) * 4))
+    io = (io_v, int((pin0.numel() + pin1.numel() + pin_k.numel() + pin_pose.numel()) * 4))
     return video_step, pair_step, out_v, out_p, io, dict(kind="depth-sequence", data="synthetic_posed_sequence seed 77",
                                                         value="depth")
 

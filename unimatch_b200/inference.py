@@ -134,16 +134,36 @@ def flow_to_image(flow, out=None):
     return out
 
 
-def _frame_geometry(h, w, padding_factor, inference_size):
-    """(transposed, original size as the model sees it, inference size) of a frame sequence (evaluate_flow.py:713-723)."""
-    transposed = h > w
+def _frames_hw(frames, name):
+    """(H, W) of a device sequence of T >= 2 frames: uint8 channel-last [T,H,W,3] as decoded, or float planar [T,3,H,W]."""
+    if not torch.is_tensor(frames) or frames.dim() != 4 or frames.shape[0] < 2:
+        raise ValueError("%s needs at least two frames [T>=2, H, W, 3] uint8 or [T>=2, 3, H, W] float" % name)
+    if frames.dtype == torch.uint8:
+        if frames.shape[-1] != 3:
+            raise ValueError("%s: uint8 frames are channel-last [T, H, W, 3]" % name)
+        return int(frames.shape[1]), int(frames.shape[2])
+    if frames.dtype.is_floating_point and frames.shape[1] == 3:
+        return int(frames.shape[2]), int(frames.shape[3])
+    raise ValueError("%s: frames must be uint8 [T, H, W, 3] or float [T, 3, H, W]" % name)
+
+
+def _frame_geometry(h, w, padding_factor, inference_size, task):
+    """(transposed, original size as the model sees it, inference size) of a frame sequence.  Portrait frames are transposed
+    for the flow model, which is trained with width > height (evaluate_flow.py:713-723); depth frames are not
+    (evaluate_depth.py:364-376)."""
+    transposed = task == "flow" and h > w
     ori = (w, h) if transposed else (h, w)
     return transposed, ori, _inference_size(ori, padding_factor, inference_size)
 
 
-def _frames_to_model(frames, transposed, size):
-    """[T,H,W,3] uint8 (one fused kernel) or [T,3,H,W] float frames -> planar float32 [T,3,*size] model input."""
+def _frames_to_model(frames, task, transposed, size):
+    """Frames -> planar float32 [T,3,*size] model input.  uint8 [T,H,W,3] as decoded: one fused kernel (transpose and resize
+    for flow; ImageNet normalisation and resize for depth, evaluate_depth.py:353-376).  Float [T,3,H,W], in [0,255] for flow
+    and normalised for depth: the resize kernel, or the frames as they are at the inference size."""
     if frames.dtype == torch.uint8:
+        if task == "depth":
+            return _OPS.frames_to_planar_normalized(frames.contiguous(), int(size[0]), int(size[1]), list(IMAGENET_MEAN),
+                                                    list(IMAGENET_STD))
         return _OPS.frames_to_planar(frames.contiguous(), int(size[0]), int(size[1]), bool(transposed))
     if transposed:
         frames = frames.transpose(-2, -1)
@@ -159,11 +179,9 @@ def infer_flow_video(model, frames, *, padding_factor, inference_size=None, pred
     (equal up to fp32 summation order, see `UniMatch.encode_frames`).
     `pred_bwd_flow`: each pair runs in swapped order (evaluate_flow.py:735-736), i.e. the flow from frame t+1 to frame t."""
     _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, "infer_flow_video")
-    if frames.dim() != 4 or frames.shape[0] < 2:
-        raise ValueError("infer_flow_video needs at least two frames [T>=2, H, W, 3] or [T>=2, 3, H, W]")
-    h, w = (frames.shape[1], frames.shape[2]) if frames.dtype == torch.uint8 else (frames.shape[2], frames.shape[3])
-    transposed, ori, size = _frame_geometry(h, w, padding_factor, inference_size)
-    feats = model.encode_frames(_frames_to_model(frames, transposed, size))
+    h, w = _frames_hw(frames, "infer_flow_video")
+    transposed, ori, size = _frame_geometry(h, w, padding_factor, inference_size, "flow")
+    feats = model.encode_frames(_frames_to_model(frames, "flow", transposed, size))
     first, second = [f[:-1] for f in feats], [f[1:] for f in feats]
     if pred_bwd_flow:
         first, second = second, first
@@ -269,15 +287,6 @@ def _relative_poses(poses, bidir):
     return np.stack(rel).astype(np.float32)
 
 
-def _depth_frames_to_model(frames, size):
-    """[T,H,W,3] uint8 (one fused kernel: ImageNet normalisation and resize) or [T,3,H,W] normalised float frames ->
-    planar float32 [T,3,*size] model input (evaluate_depth.py:353-376)."""
-    if frames.dtype == torch.uint8:
-        return _OPS.frames_to_planar_normalized(frames.contiguous(), int(size[0]), int(size[1]), list(IMAGENET_MEAN),
-                                                list(IMAGENET_STD))
-    return _resize(frames, size) if tuple(frames.shape[-2:]) != tuple(size) else frames.float().contiguous()
-
-
 @torch.no_grad()
 def infer_depth_sequence(model, frames, intrinsics, poses, *, padding_factor=16, inference_size=None, min_depth=0.5,
                          max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
@@ -291,24 +300,15 @@ def infer_depth_sequence(model, frames, intrinsics, poses, *, padding_factor=16,
     `pred_bidir_depth`).  Returns what `infer_depth` returns on those pairs: {'depth': [T-1,H,W]} (+ 'depth_bwd'), equal up to
     fp32 summation order (see `UniMatch.encode_frames`)."""
     model_kwargs = _depth_task_kwargs(model_kwargs, "infer_depth_sequence")
-    if not torch.is_tensor(frames) or frames.dim() != 4 or frames.shape[0] < 2:
-        raise ValueError("infer_depth_sequence needs at least two frames [T>=2, H, W, 3] uint8 or [T>=2, 3, H, W] float")
-    if frames.dtype == torch.uint8:
-        if frames.shape[-1] != 3:
-            raise ValueError("infer_depth_sequence: uint8 frames are channel-last [T, H, W, 3]")
-        ori = (int(frames.shape[1]), int(frames.shape[2]))
-    elif frames.dtype.is_floating_point and frames.shape[1] == 3:
-        ori = (int(frames.shape[2]), int(frames.shape[3]))
-    else:
-        raise ValueError("infer_depth_sequence: frames must be uint8 [T, H, W, 3] or float [T, 3, H, W]")
+    h, w = _frames_hw(frames, "infer_depth_sequence")
     T = frames.shape[0]
     if len(poses) != T:
         raise ValueError("infer_depth_sequence: %d frames need %d poses, got %d" % (T, T, len(poses)))
     abs_poses = [_pose44(p, "infer_depth_sequence") for p in poses]
     K = _intrinsics33(intrinsics, "infer_depth_sequence")
-    size = _inference_size(ori, padding_factor, inference_size)
+    _, ori, size = _frame_geometry(h, w, padding_factor, inference_size, "depth")
     dev = frames.device
-    feats = model.encode_frames(_depth_frames_to_model(frames, size), task="depth")
+    feats = model.encode_frames(_frames_to_model(frames, "depth", False, size), task="depth")
     rel = torch.from_numpy(_relative_poses(abs_poses, pred_bidir_depth)).to(dev)
     cams = model.depth_cameras(K.to(dev)[None].repeat(T - 1, 1, 1), rel, model.upsample_factor, 1.0 / max_depth,
                                1.0 / min_depth, num_depth_candidates, pred_bidir_depth)
@@ -456,8 +456,6 @@ class BatchedFlowRunner(_PipelinedRunner):
         a, b = self.dev_in[slot]
         return self.model(a, b, **self.kw)["flow_preds"][-1]
 
-    _forward = _step
-
     def _reset_inputs(self, slot):
         self.dev_in[slot][0].zero_(); self.dev_in[slot][1].zero_()
 
@@ -483,53 +481,114 @@ class BatchedFlowRunner(_PipelinedRunner):
             yield from self._pipeline(pairs)
 
 
-class VideoFlowRunner(_PipelinedRunner):
+class _SequenceRunner(_PipelinedRunner):
+    """Consecutive pairs of a stream of host items, each holding one uint8 frame [H,W,3] as decoded, with every frame uploaded
+    and encoded once: a step copies `batch` new frames through pinned double buffers on a side stream, converts and encodes
+    them on the device (one CUDA graph per staging slot) and runs `_match` on the `batch` pairs (previous step's last frame,
+    new frames); the last frame's pyramid (`carry`) is kept for the next step.  A short last step is filled with repeats of
+    its last item and the extra results are dropped.  Subclasses set `task` and provide `_match(slot, first, second)`, which
+    returns the step's dict of outputs; items with more than a frame override `_frame` and `_begin` (host state of the first
+    item) and extend `_stage_host` and `_reset_inputs`."""
+
+    def _init_sequence(self, model, frame_size, batch, device, use_graph, padding_factor, inference_size):
+        self.model, self.batch = model, int(batch)
+        if self.batch < 1:
+            raise ValueError("%s: batch must be positive" % type(self).__name__)
+        self._init_pipeline(device, use_graph)
+        self.h, self.w = int(frame_size[0]), int(frame_size[1])
+        self.transposed, self.ori, self.size = _frame_geometry(self.h, self.w, padding_factor, inference_size, self.task)
+        shape = (self.batch, self.h, self.w, 3)
+        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.carry = None                                  # last frame's feature pyramid, [1,h,w,128] per scale
+
+    @staticmethod
+    def _frame(item):
+        return item
+
+    def _begin(self, first):
+        pass
+
+    # ---- device side
+    def _encode(self, frames_u8):
+        return self.model.encode_frames(_frames_to_model(frames_u8, self.task, self.transposed, self.size), task=self.task)
+
+    def _step(self, slot):
+        new = self._encode(self.dev_in[slot])
+        out = self._match(slot, [torch.cat((c, f[:-1]), dim=0) for c, f in zip(self.carry, new)], new)
+        for c, f in zip(self.carry, new):                # carry the last frame into the next step
+            c.copy_(f[-1:])
+        return out
+
+    def _reset_inputs(self, slot):
+        self.dev_in[slot].zero_()
+
+    def _prime(self, frame):
+        """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
+        for c, g in zip(self.carry, self._encode(frame)):
+            c.copy_(g)
+
+    # ---- host side
+    def _stage_host(self, slot, chunk):
+        """the step's frames into the pinned buffer, then their H2D copy; returns the step's `batch` items"""
+        items = [chunk[min(i, len(chunk) - 1)] for i in range(self.batch)]
+        for i, item in enumerate(items):
+            self.pin[slot][i].copy_(torch.as_tensor(self._frame(item)))
+        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
+        return items
+
+    @torch.no_grad()
+    def run(self, items):
+        with torch.cuda.device(self.dev):
+            it = iter(items)
+            first = next(it, None)
+            if first is None:
+                return
+            frame0 = torch.as_tensor(self._frame(first))
+            if tuple(frame0.shape) != (self.h, self.w, 3):
+                raise ValueError("%s: frames must be uint8 [%d, %d, 3]" % (type(self).__name__, self.h, self.w))
+            self._begin(first)
+            frame0 = frame0.to(self.dev)[None].contiguous()
+            if self.carry is None:                       # eager runs: allocate the carried pyramid
+                self.carry = [f.clone() for f in self._encode(frame0)]
+            yield from self._pipeline(it, start=lambda: self._prime(frame0))
+
+
+class VideoFlowRunner(_SequenceRunner):
     """Streaming optical flow over a video: consecutive pairs of host uint8 frames, every frame uploaded and encoded once.
 
-    * upload: each step copies `batch` NEW frames, uint8 [H,W,3] as decoded, through pinned double buffers on a side stream
-      (1.2 MB per 480x832 frame, against 9.6 MB for the two float32 images of a pair);
-    * device work of a step (one CUDA graph per staging slot): `um_frames_to_planar` (uint8 -> float planes, portrait
-      transpose and resize to the inference size in one pass), the encoder on the new frames, the matching path on the
-      `batch` pairs (previous step's last frame, new frames), the flow resized back; the last frame's pyramid is carried into
-      the next step, so nothing is encoded twice.  A short last step is filled with repeats of its last frame and the extra
-      results are dropped;
+    * upload: each step copies `batch` NEW frames, uint8 [H,W,3] as decoded (1.2 MB per 480x832 frame, against 9.6 MB for
+      the two float32 images of a pair);
+    * device work of a step: `um_frames_to_planar` (uint8 -> float planes, portrait transpose and resize to the inference
+      size in one pass), the encoder on the new frames, the matching path on the `batch` pairs, the flow resized back;
     * download: the flow (and flow_bwd / fwd_occ / bwd_occ when asked) and, with `visualize`, the uint8 Middlebury picture
       (`flow_to_image`; with `concat_frame` the frame and its picture side by side, stacked as the reference's
       `concat_flow_img` does, evaluate_flow.py:818-825).  `return_flow=False` with `visualize` sends back only the picture.
 
     Sizes, transpose and rescale semantics are those of `infer_flow_video` (and `infer_flow`); the flows equal
-    `infer_flow_video` on the whole sequence up to fp32 summation order.  `run(frames)` takes an iterable of host uint8 frames [H,W,3] (numpy arrays or
-    tensors) and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy what you keep)."""
+    `infer_flow_video` on the whole sequence up to fp32 summation order.  `run(frames)` takes an iterable of host uint8 frames
+    [H,W,3] (numpy arrays or tensors) and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy
+    what you keep)."""
+
+    task = "flow"
 
     def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
                  visualize=False, concat_frame=False, pred_bidir_flow=False, fwd_bwd_consistency_check=False,
                  return_flow=True, **model_kwargs):
-        self.model, self.kw, self.batch = model, dict(model_kwargs), int(batch)
+        self.kw = dict(model_kwargs)
         _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "VideoFlowRunner")
         if concat_frame and not visualize:
             raise ValueError("concat_frame needs visualize=True")
         if not return_flow and not visualize:
             raise ValueError("nothing to return: return_flow=False needs visualize=True")
-        self._init_pipeline(device, use_graph)
-        self.h, self.w = int(frame_size[0]), int(frame_size[1])
-        self.transposed, self.ori, self.size = _frame_geometry(self.h, self.w, padding_factor, inference_size)
+        self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.check = bool(pred_bidir_flow), bool(fwd_bwd_consistency_check)
         self.visualize, self.concat, self.return_flow = bool(visualize), bool(concat_frame), bool(return_flow)
         self.concat_axis = 0 if self.h < self.w else 1                                  # evaluate_flow.py:822
-        shape = (self.batch, self.h, self.w, 3)
-        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
-        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
         self.carry_frame = torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev)
-        self.carry = None                                  # last frame's feature pyramid, [1,h,w,128] per scale
 
-    # ---- device side
-    def _encode(self, frames_u8):
-        return self.model.encode_frames(_OPS.frames_to_planar(frames_u8, self.size[0], self.size[1], self.transposed))
-
-    def _step(self, slot):
-        new = self._encode(self.dev_in[slot])
-        first = [torch.cat((c, f[:-1]), dim=0) for c, f in zip(self.carry, new)]
-        flow = self.model.forward_encoded(first, new, pred_bidir_flow=self.bidir, **self.kw)["flow_preds"][-1]
+    def _match(self, slot, first, second):
+        flow = self.model.forward_encoded(first, second, pred_bidir_flow=self.bidir, **self.kw)["flow_preds"][-1]
         out = _flow_outputs(flow, self.ori, self.size, self.transposed, self.bidir, self.check)
         if self.visualize:
             b, h, w = self.batch, self.h, self.w
@@ -544,76 +603,41 @@ class VideoFlowRunner(_PipelinedRunner):
             out["vis"] = pics
             if not self.return_flow:
                 del out["flow"]
-        for c, f in zip(self.carry, new):                # carry the last frame into the next step
-            c.copy_(f[-1:])
         self.carry_frame.copy_(self.dev_in[slot][-1:])
         return out
 
-    def _reset_inputs(self, slot):
-        self.dev_in[slot].zero_()
-
-    # ---- host side
-    def _stage_host(self, slot, chunk):
-        for i in range(self.batch):
-            self.pin[slot][i].copy_(torch.as_tensor(chunk[min(i, len(chunk) - 1)]))
-        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
-
     def _prime(self, frame):
-        """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
-        f = torch.as_tensor(frame).to(self.dev)[None].contiguous()
-        for c, g in zip(self.carry, self._encode(f)):
-            c.copy_(g)
-        self.carry_frame.copy_(f)
-
-    @torch.no_grad()
-    def run(self, frames):
-        with torch.cuda.device(self.dev):
-            it = iter(frames)
-            first = next(it, None)
-            if first is None:
-                return
-            if self.carry is None:                       # eager runs: allocate the carried pyramid
-                self.carry = [f.clone() for f in self._encode(torch.as_tensor(first).to(self.dev)[None].contiguous())]
-            yield from self._pipeline(it, start=lambda: self._prime(first))
+        super()._prime(frame)
+        self.carry_frame.copy_(frame)
 
 
-class DepthSequenceRunner(_PipelinedRunner):
+class DepthSequenceRunner(_SequenceRunner):
     """Streaming depth over a posed frame sequence: consecutive pairs of host (uint8 frame, absolute pose) items, every frame
     uploaded and encoded once -- the depth counterpart of `VideoFlowRunner`.
 
     * upload: each step copies `batch` NEW frames, uint8 [H,W,3] as decoded, and the `batch` relative poses of its pairs
-      (followed by their inverses when `pred_bidir_depth`), computed on the host with the reference's numpy expression,
-      through pinned double buffers on a side stream (0.59 MB per 384x512 frame, against 4.72 MB for the two float32
-      images of a pair);
-    * device work of a step (one CUDA graph per staging slot): `um_frames_to_planar_normalized` (uint8 -> ImageNet-normalised
-      planes at the inference size), the encoder on the new frames, the depth matching path on the `batch` pairs (previous
-      step's last frame, new frames) and the depth resized back.  The camera operands that depend on the intrinsics only
-      (`UniMatch.depth_cameras`) are built once, eagerly, before any capture; the per-step poses are static device buffers that
-      the upload fills.  The last frame's pyramid stays on the device for the next step and its pose on the host.  A short
-      last step is filled with repeats of its last item and the extra results are dropped;
+      (followed by their inverses when `pred_bidir_depth`), computed on the host with the reference's numpy expression
+      (0.59 MB per 384x512 frame, against 4.72 MB for the two float32 images of a pair);
+    * device work of a step: `um_frames_to_planar_normalized` (uint8 -> ImageNet-normalised planes at the inference size), the
+      encoder on the new frames, the depth matching path on the `batch` pairs and the depth resized back.  The camera operands
+      that depend on the intrinsics only (`UniMatch.depth_cameras`) are built once, eagerly, before any capture; the per-step
+      poses are static device buffers that the upload fills.  The last frame's pose stays on the host for the next step;
     * download: 'depth' (and 'depth_bwd') [H,W] per pair.
 
     Sizes and semantics are those of `infer_depth_sequence` (and `infer_depth`): `min_depth` / `max_depth` are metric,
     the intrinsics [3,3] are not rescaled with the frames.  `run(items)` takes an iterable of (uint8 frame [H,W,3], pose [4,4])
     host items and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy what you keep)."""
 
+    task = "depth"
+
     def __init__(self, model, frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None, min_depth=0.5,
                  max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False, use_graph=True,
                  **model_kwargs):
-        self.model, self.batch = model, int(batch)
         self.kw = _depth_task_kwargs(dict(model_kwargs), "DepthSequenceRunner")
-        if self.batch < 1:
-            raise ValueError("DepthSequenceRunner: batch must be positive")
         K = _intrinsics33(intrinsics, "DepthSequenceRunner")
-        self._init_pipeline(device, use_graph)
-        self.h, self.w = int(frame_size[0]), int(frame_size[1])
-        self.ori = (self.h, self.w)
-        self.size = _inference_size(self.ori, padding_factor, inference_size)
+        self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
         self.inv_range = (1.0 / max_depth, 1.0 / min_depth)                      # the model works on inverse depth
-        shape = (self.batch, self.h, self.w, 3)
-        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
-        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
         npose = (2 if self.bidir else 1) * self.batch
         self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
         self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
@@ -621,58 +645,28 @@ class DepthSequenceRunner(_PipelinedRunner):
         # cams[slot]["pose"] IS pose_dev[slot] (a float32 pose of 2B matrices is taken as it is), so the upload updates it
         self.cams = [model.depth_cameras(Kb, self.pose_dev[s], model.upsample_factor, *self.inv_range, num_depth_candidates,
                                          self.bidir) for s in range(2)]
-        self.carry = None                                  # last frame's feature pyramid, [1,h,w,128]
         self.prev_pose = None                              # last frame's absolute pose, float32 [4,4] on the host
 
-    # ---- device side
-    def _encode(self, frames_u8):
-        planar = _OPS.frames_to_planar_normalized(frames_u8, self.size[0], self.size[1], list(IMAGENET_MEAN),
-                                                  list(IMAGENET_STD))
-        return self.model.encode_frames(planar, task="depth")
+    @staticmethod
+    def _frame(item):
+        return item[0]
 
-    def _step(self, slot):
-        new = self._encode(self.dev_in[slot])
-        first = [torch.cat((c, f[:-1]), dim=0) for c, f in zip(self.carry, new)]
-        depth = self.model.forward_encoded(first, new, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
+    def _begin(self, first):
+        self.prev_pose = _pose44(first[1], "DepthSequenceRunner")
+
+    def _match(self, slot, first, second):
+        depth = self.model.forward_encoded(first, second, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
                                            max_depth=self.inv_range[1], depth_from_argmax=self.from_argmax,
                                            pred_bidir_depth=self.bidir, **self.kw)["flow_preds"][-1]
-        out = _depth_outputs(depth, self.ori, self.size, self.bidir)
-        for c, f in zip(self.carry, new):                # carry the last frame into the next step
-            c.copy_(f[-1:])
-        return out
+        return _depth_outputs(depth, self.ori, self.size, self.bidir)
 
     def _reset_inputs(self, slot):
-        self.dev_in[slot].zero_()
+        super()._reset_inputs(slot)
         self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
 
-    # ---- host side
     def _stage_host(self, slot, chunk):
-        poses = [self.prev_pose]
-        for i in range(self.batch):
-            frame, pose = chunk[min(i, len(chunk) - 1)]
-            self.pin[slot][i].copy_(torch.as_tensor(frame))
-            poses.append(_pose44(pose, "DepthSequenceRunner"))
+        """the frames, then the relative poses of the step's pairs, continuing from the carried pose"""
+        poses = [self.prev_pose] + [_pose44(pose, "DepthSequenceRunner") for _, pose in super()._stage_host(slot, chunk)]
         self.pose_pin[slot].copy_(torch.from_numpy(_relative_poses(poses, self.bidir)))
         self.prev_pose = poses[-1]
-        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
         self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
-
-    def _prime(self, frame):
-        """Encode the sequence's first frame (eagerly) as the carried frame of the first step."""
-        for c, g in zip(self.carry, self._encode(torch.as_tensor(frame).to(self.dev)[None].contiguous())):
-            c.copy_(g)
-
-    @torch.no_grad()
-    def run(self, items):
-        with torch.cuda.device(self.dev):
-            it = iter(items)
-            first = next(it, None)
-            if first is None:
-                return
-            frame0, pose0 = first
-            if tuple(torch.as_tensor(frame0).shape) != (self.h, self.w, 3):
-                raise ValueError("DepthSequenceRunner: frames must be uint8 [%d, %d, 3]" % (self.h, self.w))
-            self.prev_pose = _pose44(pose0, "DepthSequenceRunner")
-            if self.carry is None:                       # eager runs: allocate the carried pyramid
-                self.carry = [f.clone() for f in self._encode(torch.as_tensor(frame0).to(self.dev)[None].contiguous())]
-            yield from self._pipeline(it, start=lambda: self._prime(frame0))

@@ -647,34 +647,17 @@ class UniMatch(nn.Module):
                 pred_bidir_depth=False, **kwargs):
         if self.training:
             raise NotImplementedError("unimatch_b200.UniMatch is inference-only; call .eval()")
-        if pred_bidir_flow:
-            assert task == "flow"
-        if task == "depth":
-            assert self.num_scales == 1
-            assert len(attn_splits_list) == len(prop_radius_list) == self.num_scales == 1
-        else:
-            assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
         # no device check here: the unimatch_sm100 ops are registered for CUDA only, so CPU tensors fail loudly
         # in the dispatcher (there is no CPU path)
         with torch.no_grad():
-            return self._forward(img0, img1, attn_type, attn_splits_list, corr_radius_list, prop_radius_list,
-                                 num_reg_refine, pred_bidir_flow, task, intrinsics, pose, min_depth, max_depth,
-                                 num_depth_candidates, depth_from_argmax, pred_bidir_depth)
-
-    def _forward(self, img0, img1, attn_type, attn_splits_list, corr_radius_list, prop_radius_list, num_reg_refine,
-                 pred_bidir_flow, task, intrinsics, pose, min_depth, max_depth, num_depth_candidates,
-                 depth_from_argmax, pred_bidir_depth):
-        P = self._prepared()
-        B = img0.shape[0]
-        with self._section("backbone"):                                           # [2B,h,w,128] low -> high res
-            feats = self._stage_backbone(P, img0.float().contiguous(), img1.float().contiguous(), task == "flow")
-        cams = None
-        if task == "depth":
-            cams = self.depth_cameras(intrinsics, pose, self.upsample_factor, min_depth, max_depth, num_depth_candidates,
-                                      pred_bidir_depth)
-        return self._forward_encoded(P, [f[:B] for f in feats], [f[B:] for f in feats], attn_type, attn_splits_list,
-                                     corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, cams,
-                                     min_depth, max_depth, depth_from_argmax, pred_bidir_depth)
+            P = self._prepared()
+            B = img0.shape[0]
+            with self._section("backbone"):                                       # [2B,h,w,128] low -> high res
+                feats = self._stage_backbone(P, img0.float().contiguous(), img1.float().contiguous(), task == "flow")
+            return self._forward_encoded(P, [f[:B] for f in feats], [f[B:] for f in feats], attn_type, attn_splits_list,
+                                         corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, None,
+                                         intrinsics, pose, min_depth, max_depth, num_depth_candidates, depth_from_argmax,
+                                         pred_bidir_depth)
 
     # ------------------------------------------------------------------------------------------ depth cameras
     def depth_cameras(self, intrinsics, pose, up, min_depth, max_depth, num_depth_candidates, pred_bidir_depth):
@@ -742,30 +725,32 @@ class UniMatch(nn.Module):
             raise ValueError("forward_encoded drives the flow and depth tasks only (each stereo pair encodes two distinct views)")
         if len(feats0) != self.num_scales or len(feats1) != self.num_scales:
             raise ValueError("forward_encoded needs one feature map per scale (%d)" % self.num_scales)
-        if task == "depth":
-            assert self.num_scales == 1 and not pred_bidir_flow
-            assert len(attn_splits_list) == len(prop_radius_list) == 1
-            B = feats0[0].shape[0]
-            if cameras is None:
-                if intrinsics is None or pose is None:
-                    raise ValueError("forward_encoded(task='depth') needs cameras= or intrinsics= and pose=")
-                cameras = self.depth_cameras(intrinsics, pose, self.upsample_factor, min_depth, max_depth,
-                                             num_depth_candidates, pred_bidir_depth)
-            if cameras["K"].shape[0] != (2 if pred_bidir_depth else 1) * B or cameras["pose"].shape[0] != cameras["K"].shape[0]:
-                raise ValueError("forward_encoded: cameras were built for another batch or pred_bidir_depth setting")
-        else:
-            assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
-            cameras, pred_bidir_depth, depth_from_argmax = None, False, False
         with torch.no_grad():
             return self._forward_encoded(self._prepared(), list(feats0), list(feats1), attn_type, attn_splits_list,
                                          corr_radius_list, prop_radius_list, num_reg_refine, pred_bidir_flow, task, cameras,
-                                         min_depth, max_depth, depth_from_argmax, pred_bidir_depth)
+                                         intrinsics, pose, min_depth, max_depth, num_depth_candidates, depth_from_argmax,
+                                         pred_bidir_depth)
 
     def _forward_encoded(self, P, feats0, feats1, attn_type, attn_splits_list, corr_radius_list, prop_radius_list,
-                         num_reg_refine, pred_bidir_flow, task, cams, min_depth, max_depth, depth_from_argmax,
-                         pred_bidir_depth):
-        """The matching path after the encoder (unimatch.py:127-367); feats0 / feats1: per-scale [B,h,w,128] views;
-        cams: `depth_cameras` (depth task) or None."""
+                         num_reg_refine, pred_bidir_flow, task, cams, intrinsics, pose, min_depth, max_depth,
+                         num_depth_candidates, depth_from_argmax, pred_bidir_depth):
+        """The per-task argument checks of `forward` and `forward_encoded`, then the matching path after the encoder
+        (unimatch.py:127-367).  feats0 / feats1: per-scale [B,h,w,128] views; cams: `depth_cameras` for the depth task, or
+        None to build them here from `intrinsics` and `pose`."""
+        assert task == "flow" or not pred_bidir_flow
+        if task == "depth":
+            assert self.num_scales == 1 and len(attn_splits_list) == len(prop_radius_list) == 1
+            if cams is None:
+                if intrinsics is None or pose is None:
+                    raise ValueError("the depth task needs intrinsics= and pose= (or, in forward_encoded, cameras=)")
+                cams = self.depth_cameras(intrinsics, pose, self.upsample_factor, min_depth, max_depth, num_depth_candidates,
+                                          pred_bidir_depth)
+            streams = (2 if pred_bidir_depth else 1) * feats0[0].shape[0]
+            if cams["K"].shape[0] != streams or cams["pose"].shape[0] != streams:
+                raise ValueError("the depth cameras were built for another batch or pred_bidir_depth setting")
+        else:
+            assert len(attn_splits_list) == len(corr_radius_list) == len(prop_radius_list) == self.num_scales
+            cams, pred_bidir_depth, depth_from_argmax = None, False, False
         flow = None            # [Bp, h, w, fd] channel-last
         preds = []
         for s in range(self.num_scales):
@@ -801,39 +786,31 @@ class UniMatch(nn.Module):
                 continue
 
             feat0 = tok[:nb].reshape(nb, h, wd, c)                                # post-transformer feature0
-            if not self.reg_refine:                                               # unimatch.py:246-264
-                zeros = torch.zeros_like(flow)
-                if task == "stereo":
-                    out = -self._stage_upsample_learned(P, torch.cat((-flow, zeros), -1), feat0, self.upsample_factor,
-                                                        self.upsample_factor)[:, :1]
-                elif task == "depth":
-                    out = self._stage_upsample_learned(P, torch.cat((flow, zeros), -1), feat0, self.upsample_factor,
-                                                       1).clamp(min=min_depth, max=max_depth)[:, :1]
-                else:
-                    out = self._stage_upsample_learned(P, flow, feat0, self.upsample_factor, self.upsample_factor)
-                preds.append(out)
-                continue
-
             # ---- regression refinement (unimatch.py:272-354) ----
-            assert num_reg_refine > 0
-            g0, g1 = f0_ori.contiguous(), f1_ori.contiguous()
-            drefine = None
+            if self.reg_refine:
+                assert num_reg_refine > 0
+                g0, g1 = f0_ori.contiguous(), f1_ori.contiguous()
+                drefine = None
+                if task == "depth":
+                    if pred_bidir_depth:
+                        g0, g1 = torch.cat((g0, g1), dim=0), torch.cat((g1, g0), dim=0)
+                    drefine = (cams, min_depth, max_depth)
+                rst = self._stage_refine_setup(P, feat0.contiguous(), nb, h, wd)
+                for it in range(num_reg_refine):
+                    flow, mask = self._stage_refine_iter(P, rst, g0, g1, flow, task, it == num_reg_refine - 1, drefine)
+
+            # ---- upsampling to the input resolution (unimatch.py:246-264; after the refinement :335-354) ----
+            up = self.upsample_factor
             if task == "depth":
-                if pred_bidir_depth:
-                    g0, g1 = torch.cat((g0, g1), dim=0), torch.cat((g1, g0), dim=0)
-                drefine = (cams, min_depth, max_depth)
-            rst = self._stage_refine_setup(P, feat0.contiguous(), nb, h, wd)
-            for it in range(num_reg_refine):
-                last = it == num_reg_refine - 1
-                flow, mask = self._stage_refine_iter(P, rst, g0, g1, flow, task, last, drefine)
-                if last:
-                    if task == "depth":
-                        out = self._stage_upsample_learned(P, torch.cat((flow, torch.zeros_like(flow)), -1), feat0,
-                                                           self.upsample_factor, 1).clamp(min=min_depth, max=max_depth)[:, :1]
-                    else:
-                        out = _OPS.convex_upsample(flow.contiguous(), mask, self.upsample_factor,
-                                                   float(self.upsample_factor))
-                    preds.append(out)
+                out = self._stage_upsample_learned(P, torch.cat((flow, torch.zeros_like(flow)), -1), feat0, up,
+                                                   1).clamp(min=min_depth, max=max_depth)[:, :1]
+            elif self.reg_refine:
+                out = _OPS.convex_upsample(flow.contiguous(), mask, up, float(up))
+            elif task == "stereo":
+                out = -self._stage_upsample_learned(P, torch.cat((-flow, torch.zeros_like(flow)), -1), feat0, up, up)[:, :1]
+            else:
+                out = self._stage_upsample_learned(P, flow, feat0, up, up)
+            preds.append(out)
 
         if task == "stereo":
             preds = [p.squeeze(1) for p in preds]
