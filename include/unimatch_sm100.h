@@ -204,6 +204,17 @@ int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n,
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
                      int32_t n, int32_t h, int32_t w, void* stream);
 
+/* Disparity colouring of n contiguous fp32 disparities [n, h, w] -> uint8 BGR pictures (cv2's channel order), written at
+ * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES, as for um_flow_to_image).  Per image, as numpy
+ * evaluates vis_disparity on float32: g = uint8(((d - min) / (max - min)) * 255), each operation a correctly rounded fp32
+ * operation, truncated; the pixel is cv2's COLORMAP_INFERNO table at g.  A NaN normalised value gives g = 0, so a constant
+ * image, a NaN anywhere in the image or +-inf in it paints the whole image INFERNO[0].
+ * minmax_scratch: DEVICE buffer of 2n words (the per-image min / max keys; reset inside the call, graph-capturable).
+ * Replaces vis_disparity (utils/visualization.py:11-16), called on every predicted disparity by inference_stereo
+ * (evaluate_stereo.py:820-841). */
+int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,
+                          int32_t n, int32_t h, int32_t w, void* stream);
+
 /* ---- evaluation statistics -----------------------------------------------------------------------------------
  * One pass from a batch of predictions at ground-truth resolution to a [batch, S] float64 table of per-sample sufficient
  * statistics (pixel counts, counts over thresholds, fp64 sums), from which the host forms the metrics of the reference's

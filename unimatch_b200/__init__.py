@@ -25,6 +25,8 @@ _LAZY = {
     "flow_to_image": (".inference", "flow_to_image"),
     "infer_depth_sequence": (".inference", "infer_depth_sequence"),
     "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
+    "StereoRunner": (".inference", "StereoRunner"),
+    "disparity_to_image": (".inference", "disparity_to_image"),
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
@@ -32,7 +34,8 @@ _LAZY = {
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "validate_flow", "validate_stereo", "validate_depth"]
+           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "disparity_to_image", "validate_flow",
+           "validate_stereo", "validate_depth"]
 
 
 def __getattr__(name):

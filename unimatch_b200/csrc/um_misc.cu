@@ -252,6 +252,119 @@ __global__ void __launch_bounds__(256) flow_color_kernel(const float* __restrict
   }
 }
 
+// ---- disparity colouring: vis_disparity of utils/visualization.py:11-16 ------------------------------------------------
+// numpy on a float32 disparity: g = uint8(((d - min) / (max - min)) * 255) per image, three separately rounded fp32
+// operations (the build would otherwise contract and reorder them), truncated; a NaN result gives 0 (what numpy's cast
+// gives on x86-64), which covers constant images, NaN anywhere in the image (min / max propagate it) and +-inf.  The
+// picture is cv2's COLORMAP_INFERNO LUT at g, in cv2's BGR channel order (what cv2.imwrite writes).
+// Per-image min / max live in 2n words as order-preserving keys of the floats, so that unsigned atomicMax orders like the
+// values, negatives included: lo[i] = max of ~key (= ~min key), hi[i] = max of key.  A NaN sets hi[i] to 0xFFFFFFFF, the
+// key of a NaN that no other value has, and that flag paints the whole image INFERNO[0].  Both start at 0 (one memset).
+__device__ __forceinline__ unsigned float_key(float f) {
+  const unsigned u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+constexpr unsigned kNanKey = 0xffffffffu;
+
+// cv2.applyColorMap(np.arange(256, dtype=np.uint8)[:, None], cv2.COLORMAP_INFERNO): 256 x (B, G, R)
+__device__ const uint8_t kInferno[768] = {
+    4, 0, 0, 5, 0, 1, 6, 1, 1, 8, 1, 1, 10, 1, 2, 12, 2, 2, 14, 2, 2, 16, 2, 3,
+    18, 3, 4, 20, 3, 4, 23, 4, 5, 25, 4, 6, 27, 5, 7, 29, 5, 8, 31, 6, 9, 34, 7, 10,
+    36, 7, 11, 38, 8, 12, 41, 8, 13, 43, 9, 14, 45, 9, 16, 48, 10, 17, 50, 10, 18, 52, 11, 20,
+    55, 11, 21, 57, 11, 22, 60, 12, 24, 62, 12, 25, 65, 12, 27, 67, 12, 28, 69, 12, 30, 72, 12, 31,
+    74, 12, 33, 76, 12, 35, 79, 12, 36, 81, 12, 38, 83, 11, 40, 85, 11, 41, 87, 11, 43, 89, 11, 45,
+    91, 10, 47, 92, 10, 49, 94, 10, 50, 95, 10, 52, 97, 9, 54, 98, 9, 56, 99, 9, 57, 100, 9, 59,
+    101, 9, 61, 102, 9, 62, 103, 10, 64, 104, 10, 66, 104, 10, 68, 105, 10, 69, 106, 11, 71, 106, 11, 73,
+    107, 12, 74, 107, 12, 76, 108, 13, 77, 108, 13, 79, 108, 14, 81, 109, 14, 82, 109, 15, 84, 109, 15, 85,
+    110, 16, 87, 110, 16, 89, 110, 17, 90, 110, 18, 92, 110, 18, 93, 110, 19, 95, 110, 19, 97, 110, 20, 98,
+    110, 21, 100, 110, 21, 101, 110, 22, 103, 110, 22, 105, 110, 23, 106, 110, 24, 108, 110, 24, 109, 110, 25, 111,
+    110, 25, 113, 110, 26, 114, 110, 26, 116, 110, 27, 117, 109, 28, 119, 109, 28, 120, 109, 29, 122, 109, 29, 124,
+    109, 30, 125, 108, 30, 127, 108, 31, 128, 108, 32, 130, 107, 32, 132, 107, 33, 133, 107, 33, 135, 106, 34, 136,
+    106, 34, 138, 105, 35, 140, 105, 35, 141, 105, 36, 143, 104, 37, 144, 104, 37, 146, 103, 38, 147, 103, 38, 149,
+    102, 39, 151, 102, 39, 152, 101, 40, 154, 100, 41, 155, 100, 41, 157, 99, 42, 159, 99, 42, 160, 98, 43, 162,
+    97, 44, 163, 96, 44, 165, 96, 45, 166, 95, 46, 168, 94, 46, 169, 94, 47, 171, 93, 48, 173, 92, 48, 174,
+    91, 49, 176, 90, 50, 177, 90, 50, 179, 89, 51, 180, 88, 52, 182, 87, 53, 183, 86, 53, 185, 85, 54, 186,
+    84, 55, 188, 83, 56, 189, 82, 57, 191, 81, 58, 192, 80, 58, 193, 79, 59, 195, 78, 60, 196, 77, 61, 198,
+    76, 62, 199, 75, 63, 200, 74, 64, 202, 73, 65, 203, 72, 66, 204, 71, 67, 206, 70, 68, 207, 69, 69, 208,
+    68, 70, 210, 67, 71, 211, 66, 72, 212, 65, 74, 213, 63, 75, 215, 62, 76, 216, 61, 77, 217, 60, 78, 218,
+    59, 80, 219, 58, 81, 221, 56, 82, 222, 55, 83, 223, 54, 85, 224, 53, 86, 225, 52, 87, 226, 51, 89, 227,
+    49, 90, 228, 48, 92, 229, 47, 93, 230, 46, 94, 231, 45, 96, 232, 43, 97, 233, 42, 99, 234, 41, 100, 235,
+    40, 102, 235, 38, 103, 236, 37, 105, 237, 36, 106, 238, 35, 108, 239, 33, 110, 239, 32, 111, 240, 31, 113, 241,
+    29, 115, 241, 28, 116, 242, 27, 118, 243, 25, 120, 243, 24, 121, 244, 23, 123, 245, 21, 125, 245, 20, 126, 246,
+    19, 128, 246, 18, 130, 247, 16, 132, 247, 15, 133, 248, 14, 135, 248, 12, 137, 248, 11, 139, 249, 10, 140, 249,
+    9, 142, 249, 8, 144, 250, 7, 146, 250, 7, 148, 250, 6, 150, 251, 6, 151, 251, 6, 153, 251, 6, 155, 251,
+    7, 157, 251, 7, 159, 252, 8, 161, 252, 9, 163, 252, 10, 165, 252, 12, 166, 252, 13, 168, 252, 15, 170, 252,
+    17, 172, 252, 18, 174, 252, 20, 176, 252, 22, 178, 252, 24, 180, 252, 26, 182, 251, 29, 184, 251, 31, 186, 251,
+    33, 188, 251, 35, 190, 251, 38, 192, 250, 40, 194, 250, 42, 196, 250, 45, 198, 250, 47, 199, 249, 50, 201, 249,
+    53, 203, 249, 55, 205, 248, 58, 207, 248, 61, 209, 247, 64, 211, 247, 67, 213, 246, 70, 215, 246, 73, 217, 245,
+    76, 219, 245, 79, 221, 244, 83, 223, 244, 86, 225, 244, 90, 227, 243, 93, 229, 243, 97, 230, 242, 101, 232, 242,
+    105, 234, 242, 109, 236, 241, 113, 237, 241, 117, 239, 241, 121, 241, 241, 125, 242, 242, 130, 244, 242, 134, 245, 243,
+    138, 246, 243, 142, 248, 244, 146, 249, 245, 150, 250, 246, 154, 251, 248, 157, 252, 249, 161, 253, 250, 164, 255, 252,
+};
+
+// grid (x: CTAs over the pixels of one image, y: image); 4 loads in flight per thread and step
+__global__ void __launch_bounds__(256) disp_minmax_kernel(const float* __restrict__ disp, unsigned* __restrict__ lo,
+                                                          unsigned* __restrict__ hi, int hw) {
+  const int n = blockIdx.y;
+  const float* d = disp + (long long)n * hw;
+  unsigned l = 0, m = 0;
+  bool nan = false;
+  const int stride = gridDim.x * blockDim.x;
+  for (long long p0 = blockIdx.x * blockDim.x + threadIdx.x; p0 < hw; p0 += 4LL * stride) {
+    float v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long p = p0 + (long long)k * stride;
+      v[k] = p < hw ? __ldg(d + p) : __ldg(d + p0);     // out of range: repeat a value of this thread's, no effect
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      nan |= v[k] != v[k];
+      const unsigned key = float_key(v[k]);
+      l = max(l, ~key);
+      m = max(m, key);
+    }
+  }
+  if (nan) m = kNanKey;
+  l = __reduce_max_sync(0xffffffffu, l);
+  m = __reduce_max_sync(0xffffffffu, m);
+  __shared__ unsigned part[2][8];
+  if ((threadIdx.x & 31) == 0) { part[0][threadIdx.x >> 5] = l; part[1][threadIdx.x >> 5] = m; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < 8; ++i) { l = max(l, part[0][i]); m = max(m, part[1][i]); }
+    atomicMax(lo + n, l);
+    atomicMax(hi + n, m);
+  }
+}
+
+// grid (x: CTAs over the pixels of one image, y: image); the LUT is staged in shared memory once per CTA, because every
+// warp indexes it divergently (a __constant__ table would serialise those reads)
+__global__ void __launch_bounds__(256) disp_color_kernel(const float* __restrict__ disp, const unsigned* __restrict__ lo,
+                                                         const unsigned* __restrict__ hi, uint8_t* __restrict__ out, int w,
+                                                         int hw, long long row_stride, long long image_stride) {
+  __shared__ uint8_t lut[768];
+  for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kInferno[i];
+  __syncthreads();
+  const int n = blockIdx.y;
+  const unsigned hkey = __ldg(hi + n);
+  const bool flagged = hkey == kNanKey;
+  const float mn = key_float(~__ldg(lo + n)), mx = key_float(hkey);
+  const float range = __fsub_rn(mx, mn);
+  const float* d = disp + (long long)n * hw;
+  uint8_t* img = out + n * image_stride;
+  for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
+    const float q = __fmul_rn(__fdiv_rn(__fsub_rn(__ldg(d + p), mn), range), 255.0f);
+    const int g = (flagged || !(q >= 0.f)) ? 0 : min((int)q, 255);          // NaN -> 0; (int) truncates, as numpy's cast
+    const int y = (int)p / w, x = (int)p - y * w;
+    uint8_t* o = img + y * row_stride + 3LL * x;
+    o[0] = lut[3 * g]; o[1] = lut[3 * g + 1]; o[2] = lut[3 * g + 2];
+  }
+}
+
 inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
   const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
@@ -340,6 +453,29 @@ int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_
   flow_color_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(flow, reinterpret_cast<const unsigned*>(max_scratch), out, w,
                                                                      hw, row_stride, image_stride, total);
   return um::check_launch("um_flow_to_image");
+}
+
+int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,
+                          int32_t n, int32_t h, int32_t w, void* stream) {
+  UM_REQUIRE(disp && out && minmax_scratch && n > 0 && h > 0 && w > 0, "um_disparity_to_image: bad arguments");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_disparity_to_image: an image has at most 2^31 - 1 pixels");
+  UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
+             "um_disparity_to_image: row_stride must cover 3*w bytes and image_stride h rows");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int hw = h * w;
+  unsigned* lo = reinterpret_cast<unsigned*>(minmax_scratch);
+  unsigned* hi = lo + n;
+  if (cudaMemsetAsync(minmax_scratch, 0, sizeof(float) * 2 * n, st) != cudaSuccess)
+    return um::check_launch("um_disparity_to_image");
+  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
+  long long bx = ((long long)hw + 1023) / 1024;                                     // 4 pixels per thread and pass
+  bx = bx < per_image ? bx : per_image;
+  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(disp, lo, hi, hw);
+  if (int rc = um::check_launch("um_disparity_to_image")) return rc;
+  long long cx = ((long long)hw + 255) / 256;
+  cx = cx < 2 * per_image ? cx : 2 * per_image;
+  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(disp, lo, hi, out, w, hw, row_stride, image_stride);
+  return um::check_launch("um_disparity_to_image");
 }
 
 }  // extern "C"

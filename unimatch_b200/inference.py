@@ -22,6 +22,10 @@ Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_seq
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
 does; `DepthSequenceRunner` streams host (uint8 frame, pose) items through the same path, replayed as a CUDA graph.  Colouring
 depth maps (matplotlib's `plasma`, evaluate_depth.py:403-417) stays out of scope.
+
+Stereo (`inference_stereo`, evaluate_stereo.py:711-843): `StereoRunner` streams host uint8 (left, right) pairs, normalised and
+resized on the device, through the same path as `infer_stereo`, replayed as a CUDA graph; `disparity_to_image` is the
+reference's `vis_disparity` (min-max scaling, cv2's INFERNO map) on the device.  Writing files (PNG, PFM) stays out of scope.
 """
 import math
 
@@ -201,9 +205,15 @@ def infer_stereo(model, left, right, *, padding_factor=16, inference_size=None, 
         raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
     ori = tuple(left.shape[-2:])
     size = _inference_size(ori, padding_factor, inference_size)
-    resized = size != ori
-    if resized:
+    if size != ori:
         left, right = _resize(left, size), _resize(right, size)
+    return _stereo_outputs(model, left, right, ori, size, pred_bidir_disp, pred_right_disp, model_kwargs)
+
+
+def _stereo_outputs(model, left, right, ori, size, pred_bidir_disp, pred_right_disp, model_kwargs):
+    """Normalised pairs at the inference size -> the stereo driver's outputs at the original size: the hflip batching, the
+    forward, and the resize back with the width rescale and the flip back (evaluate_stereo.py:789-836)."""
+    resized = size != ori
     b = left.shape[0]
     if pred_bidir_disp:
         left, right = torch.cat((left, _hflip(right)), dim=0), torch.cat((right, _hflip(left)), dim=0)
@@ -220,6 +230,40 @@ def infer_stereo(model, left, right, *, padding_factor=16, inference_size=None, 
     if resized or pred_right_disp:
         disp = _resize(disp, ori, sc, flip=pred_right_disp)
     return {"disp": disp.squeeze(1)}
+
+
+@torch.no_grad()
+def _stereo_from_frames(model, frames_u8, *, padding_factor=16, inference_size=None, pred_bidir_disp=False,
+                        pred_right_disp=False, **model_kwargs):
+    """`infer_stereo` on B pairs given as 2B device uint8 frames [2B,H,W,3] as decoded, the B left frames then the B right
+    ones.  One `um_frames_to_planar_normalized` launch normalises them as the stereo data pipeline does
+    (dataloader/stereo/transforms.py:20-63: x / 255, - mean, / std in float32) and resizes them to the inference size, so the
+    model sees what `infer_stereo` sees on frames normalised on the host."""
+    ori = (int(frames_u8.shape[1]), int(frames_u8.shape[2]))
+    size = _inference_size(ori, padding_factor, inference_size)
+    planes = _OPS.frames_to_planar_normalized(frames_u8.contiguous(), int(size[0]), int(size[1]), list(IMAGENET_MEAN),
+                                              list(IMAGENET_STD))
+    b = frames_u8.shape[0] // 2
+    return _stereo_outputs(model, planes[:b], planes[b:], ori, size, pred_bidir_disp, pred_right_disp, model_kwargs)
+
+
+def disparity_to_image(disp, out=None):
+    """`vis_disparity` (utils/visualization.py:11-16, what the stereo driver paints, evaluate_stereo.py:820-841) on the device
+    for a batch: disparities [N,H,W] -> uint8 BGR pictures [N,H,W,3] (cv2's channel order, ready for cv2.imwrite), each image
+    min-max scaled to 0..255 and coloured with cv2's INFERNO map; a single disparity [H,W] gives one picture [H,W,3].  `out`
+    may be a view into larger pictures (3-byte pixels, any row / image stride).  One min / max pass and one colouring pass."""
+    if not torch.is_tensor(disp) or disp.dim() not in (2, 3) or not disp.dtype.is_floating_point or 0 in disp.shape:
+        raise ValueError("disparity_to_image expects float disparities [N,H,W] or [H,W]")
+    shape = tuple(disp.shape) + (3,)
+    if out is None:
+        out = torch.empty(shape, device=disp.device, dtype=torch.uint8)
+    elif not torch.is_tensor(out) or tuple(out.shape) != shape or out.dtype != torch.uint8:
+        raise ValueError("disparity_to_image: out must be uint8 %s" % (list(shape),))
+    if disp.dim() == 2:
+        _OPS.disparity_to_image(disp[None].float().contiguous(), out[None])
+    else:
+        _OPS.disparity_to_image(disp.float().contiguous(), out)
+    return out
 
 
 @torch.no_grad()
@@ -474,6 +518,79 @@ class BatchedFlowRunner(_PipelinedRunner):
     def _results(self, slot, n):
         for i in range(n):
             yield self.padder.unpad(self.out_pin[slot][i])
+
+    @torch.no_grad()
+    def run(self, pairs):
+        with torch.cuda.device(self.dev):
+            yield from self._pipeline(pairs)
+
+
+class StereoRunner(_PipelinedRunner):
+    """Streaming stereo inference over host (left, right) uint8 frame pairs: `inference_stereo` (evaluate_stereo.py:711-843)
+    as a stream.
+
+    * upload: a step stages `batch` pairs into one pinned uint8 [2B,H,W,3] buffer (the B left frames, then the B right ones,
+      as decoded) and copies it on a side stream while the previous step computes (3.1 MB per 544x960 pair, against 12.5 MB
+      for the two float32 images);
+    * device work of a step, captured once per staging slot in a CUDA graph: `_stereo_from_frames` (ImageNet normalisation
+      and resize to the inference size in one `um_frames_to_planar_normalized` launch, the hflip batching of
+      `pred_bidir_disp` / `pred_right_disp`, the forward, the resize back with the width rescale) and, with `visualize`,
+      `disparity_to_image` on 'disp' (and 'disp_right');
+    * download: 'disp' [H,W] (+ 'disp_right') and, with `visualize`, the uint8 BGR pictures 'vis' [H,W,3] (+ 'vis_right');
+      `return_disp=False` with `visualize` sends back only the pictures.
+
+    Sizes, padding, `inference_size` and the bidirectional / right-view semantics are those of `infer_stereo`.  The runner is
+    built for one frame size (the reference handles each file at its own size); a short last step is filled with repeats of
+    its last pair and the extra results are dropped.  `run(pairs)` takes an iterable of (left, right) host uint8 frames
+    [H,W,3] (numpy arrays or tensors, RGB as PIL decodes them) and yields one dict of CPU tensors per pair (pinned staging
+    reused -- copy what you keep)."""
+
+    def __init__(self, model, frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
+                 pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, **model_kwargs):
+        if pred_bidir_disp and pred_right_disp:
+            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
+        if not return_disp and not visualize:
+            raise ValueError("nothing to return: return_disp=False needs visualize=True")
+        self.kw = dict(model_kwargs)
+        if self.kw.pop("task", "stereo") != "stereo":
+            raise ValueError("StereoRunner drives the stereo task only")
+        self.model, self.batch = model, int(batch)
+        if self.batch < 1:
+            raise ValueError("StereoRunner: batch must be positive")
+        self.h, self.w = int(frame_size[0]), int(frame_size[1])
+        self.geometry = dict(padding_factor=padding_factor, inference_size=inference_size, pred_bidir_disp=bool(pred_bidir_disp),
+                             pred_right_disp=bool(pred_right_disp))
+        self.visualize, self.return_disp = bool(visualize), bool(return_disp)
+        self._init_pipeline(device, use_graph)
+        shape = (2 * self.batch, self.h, self.w, 3)
+        self.pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_in = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+
+    def _step(self, slot):
+        out = _stereo_from_frames(self.model, self.dev_in[slot], **self.geometry, **self.kw)
+        if self.visualize:
+            for k in [k for k in ("disp", "disp_right") if k in out]:
+                out[k.replace("disp", "vis")] = disparity_to_image(out[k])
+                if not self.return_disp:
+                    del out[k]
+        return out
+
+    def _reset_inputs(self, slot):
+        self.dev_in[slot].zero_()
+
+    def _frame(self, img):
+        f = torch.as_tensor(img)
+        if f.dtype != torch.uint8 or tuple(f.shape) != (self.h, self.w, 3):
+            raise ValueError("StereoRunner: frames must be uint8 [%d, %d, 3]" % (self.h, self.w))
+        return f
+
+    def _stage_host(self, slot, chunk):
+        """the step's left frames, then its right frames, into the pinned buffer; then their one H2D copy"""
+        for i in range(self.batch):
+            left, right = chunk[min(i, len(chunk) - 1)]
+            self.pin[slot][i].copy_(self._frame(left))
+            self.pin[slot][self.batch + i].copy_(self._frame(right))
+        self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
 
     @torch.no_grad()
     def run(self, pairs):

@@ -100,6 +100,7 @@ _SIGNATURES = {
     "um_frames_to_planar": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_eval_stats": (_RC, [_P, _L, _L, _L, _L, _P, _P, _P, _I, _I, _F, _F, _F, _I, _I, _I, _P, _P, _P]),
     "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
     "um_ffn_tc": (_RC, [ctypes.POINTER(FfnDesc), _P]),
@@ -440,6 +441,23 @@ def _flow_to_image(flow, out):
 
 
 flow_to_image = _define("flow_to_image(Tensor flow, Tensor(a!) out) -> ()", _flow_to_image)
+
+
+def _disparity_to_image(disp, out):
+    """disp: contiguous fp32 [N, H, W]; out: uint8 BGR [N, H, W, 3] with 3-byte pixels, rows and images may be strided."""
+    _f32c(disp, "disp")
+    if disp.dim() != 3:
+        raise RuntimeError("disparity_to_image: expected disparities [N, H, W]")
+    n, h, w = disp.shape
+    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
+            or out.device != disp.device:
+        raise RuntimeError("disparity_to_image: out must be uint8 [N, H, W, 3] on the disparity's device with 3-byte pixels")
+    scratch = torch.empty((2 * n,), device=disp.device, dtype=torch.float32)
+    _check(LIB.um_disparity_to_image(_p(disp), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
+           "um_disparity_to_image")
+
+
+disparity_to_image = _define("disparity_to_image(Tensor disp, Tensor(a!) out) -> ()", _disparity_to_image)
 
 
 def _eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, eval_max):

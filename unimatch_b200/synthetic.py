@@ -118,6 +118,19 @@ def synthetic_video(T, h, w, seed=1234, step=3):
     return torch.stack(frames, 0).contiguous()
 
 
+def synthetic_stereo_frames(n, h, w, seed=1234):
+    """n rectified stereo pairs as decoded: left and right uint8 frames [n,H,W,3] (channel-last), pair i cropped from band i
+    of one box-blurred noise canvas, the right view being the left shifted by a seeded whole-pixel disparity in [0, 32] --
+    the uint8 counterpart of `synthetic_pair("stereo")`."""
+    g = torch.Generator().manual_seed(seed)
+    m = 32
+    canvas = _texture(g, n * h, w + m)[0].round().clamp(0, 255).to(torch.uint8).permute(1, 2, 0)
+    disps = torch.randint(0, m + 1, (n,), generator=g).tolist()
+    lefts = [canvas[i * h:(i + 1) * h, m:m + w] for i in range(n)]
+    rights = [canvas[i * h:(i + 1) * h, m - d:m - d + w] for i, d in enumerate(disps)]      # right view = left shifted by +d px
+    return torch.stack(lefts, 0).contiguous(), torch.stack(rights, 0).contiguous()
+
+
 def synthetic_posed_sequence(T, h, w, seed=1234, step=3, plane_depth=2.0):
     """A posed frame sequence for depth inference: T frames uint8 [T,H,W,3] of a fronto-parallel textured plane at depth
     `plane_depth`, the intrinsics K [3,3] (focal 0.9 W, centred principal point) and the absolute camera-to-world poses
