@@ -215,6 +215,20 @@ int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_
 int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,
                           int32_t n, int32_t h, int32_t w, void* stream);
 
+/* Depth colouring of n contiguous fp32 depths [n, h, w] -> uint8 RGB pictures (PIL's channel order) of the inverse depth,
+ * written at out + i * image_stride + y * row_stride + 3 * x (strides in BYTES, as for um_flow_to_image).  Per image, as
+ * numpy 1.19 / matplotlib 3.5.1 evaluate viz_depth_tensor(1. / depth): inv = 1 / depth (correctly rounded fp32); vmin =
+ * min(inv); vmax = a * (1 - g) + b * g in float64, with a, b the exact order statistics of inv at ranks k and
+ * min(k + 1, N - 1), k = floor(0.95 * (N - 1)) and g its fraction (np.percentile(inv, 95)); t = (inv - vmin) /
+ * fp32(vmax - vmin) in fp32; the pixel is uint8(floor(255 * plasma[c])) at index trunc(256 * t), clamped to 0..255, and
+ * black for a NaN t.  vmax <= vmin gives index 0 everywhere; a NaN in the image, or a NaN vmax, paints it all black.
+ * scratch: DEVICE buffer of 2056 * n 32-bit words (per image four 512-bin radix-select histograms and the selection
+ * state; reset inside the call).  One memset and nine kernels whatever the data, no host synchronisation: graph-capturable.
+ * Replaces viz_depth_tensor (utils/visualization.py:92-107), called on every predicted depth (and the backward one with
+ * pred_bidir_depth) by inference_depth (evaluate_depth.py:403-417). */
+int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,
+                      int32_t h, int32_t w, void* stream);
+
 /* ---- evaluation statistics -----------------------------------------------------------------------------------
  * One pass from a batch of predictions at ground-truth resolution to a [batch, S] float64 table of per-sample sufficient
  * statistics (pixel counts, counts over thresholds, fp64 sums), from which the host forms the metrics of the reference's

@@ -365,6 +365,196 @@ __global__ void __launch_bounds__(256) disp_color_kernel(const float* __restrict
   }
 }
 
+// ---- depth colouring: viz_depth_tensor(1. / depth) of utils/visualization.py:92-107 ----------------------------------
+// Per image of N pixels, as numpy 1.19 / matplotlib 3.5.1 evaluate it (oracle/depth_viz.py states it step by step):
+// inv = 1 / depth (correctly rounded fp32); vmin = min(inv); vmax = a * (1 - g) + b * g in float64, where a and b are the
+// sorted inv at ranks k and min(k + 1, N - 1), k = floor(0.95 * (N - 1)) and g its fraction; t = (inv - vmin) /
+// fp32(vmax - vmin) in fp32; x = t * 256 indexes the plasma table, below 0 -> first colour, 255 and above -> last colour,
+// NaN -> black.  vmin == vmax (and vmin > vmax, where matplotlib raises; only float64 rounding with a = vmin gets there)
+// gives t = 0 everywhere; a NaN anywhere in the image (or a NaN vmax, +inf * 0 when b = +inf and g = 0) paints it black.
+// a and b are found exactly by a radix select on the order-preserving keys of inv, one byte per pass from the top: pass 0
+// fuses the reciprocal, the minimum and the NaN flag with the histogram of the top byte; passes 1-3 histogram the next
+// byte of the keys under rank k's prefix and, where it differs, rank k+1's.  Per image the scratch holds one 2 x 256-bin
+// histogram per pass and kDvState words of state, all zeroed by one memset; the launch count does not depend on the data.
+constexpr int kDvBins = 256;
+constexpr int kDvHistWords = 4 * 2 * kDvBins;
+enum : int { kDvLo, kDvNan, kDvPrefA, kDvPrefB, kDvRankA, kDvRankB, kDvRange, kDvMode, kDvState };
+constexpr int kDvWords = kDvHistWords + kDvState;          // = 2056, the per-image scratch size the header states
+enum : unsigned { kDvNormal = 0, kDvFlat = 1, kDvBlack = 2 };
+constexpr unsigned kNoBin = 0xffffffffu;
+
+// matplotlib's _plasma_data (CC0) as uint8(floor(float64(c) * 255)): 256 x (R, G, B)
+__device__ const uint8_t kPlasma[768] = {
+    12, 7, 134, 16, 7, 135, 19, 6, 137, 21, 6, 138, 24, 6, 139, 27, 6, 140, 29, 6, 141, 31, 5, 142,
+    33, 5, 143, 35, 5, 144, 37, 5, 145, 39, 5, 146, 41, 5, 147, 43, 5, 148, 45, 4, 148, 47, 4, 149,
+    49, 4, 150, 51, 4, 151, 52, 4, 152, 54, 4, 152, 56, 4, 153, 58, 4, 154, 59, 3, 154, 61, 3, 155,
+    63, 3, 156, 64, 3, 156, 66, 3, 157, 68, 3, 158, 69, 3, 158, 71, 2, 159, 73, 2, 159, 74, 2, 160,
+    76, 2, 161, 78, 2, 161, 79, 2, 162, 81, 1, 162, 82, 1, 163, 84, 1, 163, 86, 1, 163, 87, 1, 164,
+    89, 1, 164, 90, 0, 165, 92, 0, 165, 94, 0, 165, 95, 0, 166, 97, 0, 166, 98, 0, 166, 100, 0, 167,
+    101, 0, 167, 103, 0, 167, 104, 0, 167, 106, 0, 167, 108, 0, 168, 109, 0, 168, 111, 0, 168, 112, 0, 168,
+    114, 0, 168, 115, 0, 168, 117, 0, 168, 118, 1, 168, 120, 1, 168, 121, 1, 168, 123, 2, 168, 124, 2, 167,
+    126, 3, 167, 127, 3, 167, 129, 4, 167, 130, 4, 167, 132, 5, 166, 133, 6, 166, 134, 7, 166, 136, 7, 165,
+    137, 8, 165, 139, 9, 164, 140, 10, 164, 142, 12, 164, 143, 13, 163, 144, 14, 163, 146, 15, 162, 147, 16, 161,
+    149, 17, 161, 150, 18, 160, 151, 19, 160, 153, 20, 159, 154, 21, 158, 155, 23, 158, 157, 24, 157, 158, 25, 156,
+    159, 26, 155, 160, 27, 155, 162, 28, 154, 163, 29, 153, 164, 30, 152, 165, 31, 151, 167, 33, 151, 168, 34, 150,
+    169, 35, 149, 170, 36, 148, 172, 37, 147, 173, 38, 146, 174, 39, 145, 175, 40, 144, 176, 42, 143, 177, 43, 143,
+    178, 44, 142, 180, 45, 141, 181, 46, 140, 182, 47, 139, 183, 48, 138, 184, 50, 137, 185, 51, 136, 186, 52, 135,
+    187, 53, 134, 188, 54, 133, 189, 55, 132, 190, 56, 131, 191, 57, 130, 192, 59, 129, 193, 60, 128, 194, 61, 128,
+    195, 62, 127, 196, 63, 126, 197, 64, 125, 198, 65, 124, 199, 66, 123, 200, 68, 122, 201, 69, 121, 202, 70, 120,
+    203, 71, 119, 204, 72, 118, 205, 73, 117, 206, 74, 117, 207, 75, 116, 208, 77, 115, 209, 78, 114, 209, 79, 113,
+    210, 80, 112, 211, 81, 111, 212, 82, 110, 213, 83, 109, 214, 85, 109, 215, 86, 108, 215, 87, 107, 216, 88, 106,
+    217, 89, 105, 218, 90, 104, 219, 91, 103, 220, 93, 102, 220, 94, 102, 221, 95, 101, 222, 96, 100, 223, 97, 99,
+    223, 98, 98, 224, 100, 97, 225, 101, 96, 226, 102, 96, 227, 103, 95, 227, 104, 94, 228, 106, 93, 229, 107, 92,
+    229, 108, 91, 230, 109, 90, 231, 110, 90, 232, 112, 89, 232, 113, 88, 233, 114, 87, 234, 115, 86, 234, 116, 85,
+    235, 118, 84, 236, 119, 84, 236, 120, 83, 237, 121, 82, 237, 123, 81, 238, 124, 80, 239, 125, 79, 239, 126, 78,
+    240, 128, 77, 240, 129, 77, 241, 130, 76, 242, 132, 75, 242, 133, 74, 243, 134, 73, 243, 135, 72, 244, 137, 71,
+    244, 138, 71, 245, 139, 70, 245, 141, 69, 246, 142, 68, 246, 143, 67, 246, 145, 66, 247, 146, 65, 247, 147, 65,
+    248, 149, 64, 248, 150, 63, 248, 152, 62, 249, 153, 61, 249, 154, 60, 250, 156, 59, 250, 157, 58, 250, 159, 58,
+    250, 160, 57, 251, 162, 56, 251, 163, 55, 251, 164, 54, 252, 166, 53, 252, 167, 53, 252, 169, 52, 252, 170, 51,
+    252, 172, 50, 252, 173, 49, 253, 175, 49, 253, 176, 48, 253, 178, 47, 253, 179, 46, 253, 181, 45, 253, 182, 45,
+    253, 184, 44, 253, 185, 43, 253, 187, 43, 253, 188, 42, 253, 190, 41, 253, 192, 41, 253, 193, 40, 253, 195, 40,
+    253, 196, 39, 253, 198, 38, 252, 199, 38, 252, 201, 38, 252, 203, 37, 252, 204, 37, 252, 206, 37, 251, 208, 36,
+    251, 209, 36, 251, 211, 36, 250, 213, 36, 250, 214, 36, 250, 216, 36, 249, 217, 36, 249, 219, 36, 248, 221, 36,
+    248, 223, 36, 247, 224, 36, 247, 226, 37, 246, 228, 37, 246, 229, 37, 245, 231, 38, 245, 233, 38, 244, 234, 38,
+    243, 236, 38, 243, 238, 38, 242, 240, 38, 242, 241, 38, 241, 243, 38, 240, 245, 37, 240, 246, 35, 239, 248, 33,
+};
+
+// 0.95 * (N - 1) in float64, as numpy 1.19's percentile forms the index of q = 95 / 100
+__device__ __forceinline__ double p95_index(int hw) { return __dmul_rn(0.95, (double)(hw - 1)); }
+
+// grid (x: CTAs over the pixels of one image, y: image).  Pass 0 histograms the top byte of every key (bins 0-255); pass
+// p > 0 histograms byte 3 - p of the keys whose top p bytes equal rank k's prefix (bins 0-255) or else rank k+1's (bins
+// 256-511).  The loop bound is warp-uniform, so that a warp's equal bins are counted by one shared atomic
+// (__match_any_sync): a smooth depth map puts most of a warp into one bin, which would otherwise serialise the atomics.
+template <bool kFirst>
+__global__ void __launch_bounds__(256) depth_hist_kernel(const float* __restrict__ depth, unsigned* __restrict__ scratch,
+                                                         int hw, int pass) {
+  __shared__ unsigned hist[2 * kDvBins];
+  for (int i = threadIdx.x; i < 2 * kDvBins; i += blockDim.x) hist[i] = 0;
+  const int n = blockIdx.y, lane = threadIdx.x & 31;
+  unsigned* img = scratch + (long long)n * kDvWords;
+  unsigned* st = img + kDvHistWords;
+  const float* d = depth + (long long)n * hw;
+  const int shift = 32 - 8 * pass;                           // pass > 0: the prefix is the key's top 8 * pass bits
+  const unsigned pa = kFirst ? 0u : st[kDvPrefA], pb = kFirst ? 0u : st[kDvPrefB];
+  __syncthreads();
+  unsigned lo = 0;
+  bool nan = false;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long base = (long long)blockIdx.x * blockDim.x + (threadIdx.x & ~31); base < hw; base += 4 * stride) {
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const long long p = base + lane + j * stride;
+      v[j] = p < hw ? __ldg(d + p) : 0.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      unsigned bin = kNoBin;
+      if (base + lane + j * stride < hw) {
+        const float inv = __frcp_rn(v[j]);
+        const unsigned key = float_key(inv);
+        if (kFirst) {
+          nan |= inv != inv;
+          if (inv == inv) lo = max(lo, ~key);
+          bin = key >> 24;
+        } else {
+          const unsigned top = key >> shift, digit = (key >> (shift - 8)) & 255u;
+          bin = top == pa ? digit : top == pb ? kDvBins + digit : kNoBin;
+        }
+      }
+      const unsigned peers = __match_any_sync(0xffffffffu, bin);
+      if (bin != kNoBin && lane == __ffs(peers) - 1) atomicAdd(hist + bin, (unsigned)__popc(peers));
+    }
+  }
+  __syncthreads();
+  unsigned* gh = img + pass * 2 * kDvBins;
+  for (int i = threadIdx.x; i < 2 * kDvBins; i += blockDim.x)
+    if (hist[i]) atomicAdd(gh + i, hist[i]);
+  if (kFirst) {
+    lo = __reduce_max_sync(0xffffffffu, lo);
+    nan = __any_sync(0xffffffffu, nan);
+    if (lane == 0) {
+      if (lo) atomicMax(st + kDvLo, lo);
+      if (nan) atomicOr(st + kDvNan, 1u);
+    }
+  }
+}
+
+// one CTA of 256 threads per image, thread t owning bin t: a block-wide scan of the pass's histogram finds the bins that
+// hold ranks k and k+1 and appends them to both prefixes.  After the last pass the prefixes are the keys a and b, and
+// thread 0 forms vmax, the fp32 divisor and the image's mode, each float64 / fp32 operation rounded on its own.
+__global__ void __launch_bounds__(256) depth_select_kernel(unsigned* __restrict__ scratch, int hw, int pass) {
+  unsigned* img = scratch + (long long)blockIdx.x * kDvWords;
+  unsigned* st = img + kDvHistWords;
+  const unsigned* h = img + pass * 2 * kDvBins;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  unsigned pa = 0, pb = 0, ra, rb;
+  if (pass == 0) {
+    ra = (unsigned)(int)p95_index(hw);                         // floor of a non-negative index
+    rb = min(ra + 1, (unsigned)hw - 1);
+  } else {
+    pa = st[kDvPrefA]; pb = st[kDvPrefB]; ra = st[kDvRankA]; rb = st[kDvRankB];
+  }
+  const unsigned ca = h[t], cb = (pass == 0 || pa == pb) ? ca : h[kDvBins + t];
+  unsigned ia = ca, ib = cb;                                   // inclusive prefix sums over the bins
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned xa = __shfl_up_sync(0xffffffffu, ia, o), xb = __shfl_up_sync(0xffffffffu, ib, o);
+    if (lane >= o) { ia += xa; ib += xb; }
+  }
+  __shared__ unsigned wsum[2][8], sel[4];
+  if (lane == 31) { wsum[0][warp] = ia; wsum[1][warp] = ib; }
+  __syncthreads();
+  for (int i = 0; i < warp; ++i) { ia += wsum[0][i]; ib += wsum[1][i]; }
+  if (ia - ca <= ra && ra < ia) { sel[0] = (pa << 8) | t; sel[1] = ra - (ia - ca); }
+  if (ib - cb <= rb && rb < ib) { sel[2] = (pb << 8) | t; sel[3] = rb - (ib - cb); }
+  __syncthreads();
+  if (t != 0) return;
+  if (pass < 3) {
+    st[kDvPrefA] = sel[0]; st[kDvRankA] = sel[1]; st[kDvPrefB] = sel[2]; st[kDvRankB] = sel[3];
+    return;
+  }
+  const double idx = p95_index(hw), g = __dsub_rn(idx, (double)(int)idx);
+  const double a = key_float(sel[0]), b = key_float(sel[2]);
+  const double vmax = __dadd_rn(__dmul_rn(a, __dsub_rn(1.0, g)), __dmul_rn(b, g));
+  const double vmin = key_float(~st[kDvLo]);
+  unsigned mode = kDvNormal;
+  if (st[kDvNan] || vmax != vmax) mode = kDvBlack;
+  else if (!(vmin < vmax)) mode = kDvFlat;
+  else st[kDvRange] = __float_as_uint(__double2float_rn(__dsub_rn(vmax, vmin)));
+  st[kDvMode] = mode;
+}
+
+// grid (x: CTAs over the pixels of one image, y: image); the floor table is staged in shared memory as in disp_color_kernel
+__global__ void __launch_bounds__(256) depth_color_kernel(const float* __restrict__ depth, const unsigned* __restrict__ scratch,
+                                                          uint8_t* __restrict__ out, int w, int hw, long long row_stride,
+                                                          long long image_stride) {
+  __shared__ uint8_t lut[768];
+  for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kPlasma[i];
+  __syncthreads();
+  const int n = blockIdx.y;
+  const unsigned* st = scratch + (long long)n * kDvWords + kDvHistWords;
+  const unsigned mode = __ldg(st + kDvMode);
+  const float vmin = key_float(~__ldg(st + kDvLo)), range = __uint_as_float(__ldg(st + kDvRange));
+  const float* d = depth + (long long)n * hw;
+  uint8_t* img = out + n * image_stride;
+  for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
+    int i = mode == kDvFlat ? 0 : -1;                          // colour index, -1 = black
+    if (mode == kDvNormal) {
+      const float x = __fmul_rn(__fdiv_rn(__fsub_rn(__frcp_rn(__ldg(d + p)), vmin), range), 256.0f);
+      i = x != x ? -1 : x < 0.f ? 0 : x >= 255.f ? 255 : (int)x;
+    }
+    const int y = (int)p / w, xx = (int)p - y * w;
+    uint8_t* o = img + y * row_stride + 3LL * xx;
+    if (i < 0) {
+      o[0] = o[1] = o[2] = 0;
+    } else {
+      o[0] = lut[3 * i]; o[1] = lut[3 * i + 1]; o[2] = lut[3 * i + 2];
+    }
+  }
+}
+
 inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
   const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
@@ -476,6 +666,35 @@ int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, i
   cx = cx < 2 * per_image ? cx : 2 * per_image;
   disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(disp, lo, hi, out, w, hw, row_stride, image_stride);
   return um::check_launch("um_disparity_to_image");
+}
+
+int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,
+                      int32_t h, int32_t w, void* stream) {
+  UM_REQUIRE(depth && out && scratch && n > 0 && h > 0 && w > 0, "um_depth_to_image: bad arguments");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_depth_to_image: an image has at most 2^31 - 1 pixels");
+  UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
+             "um_depth_to_image: row_stride must cover 3*w bytes and image_stride h rows");
+  static_assert(kDvWords == 2056, "the header states the scratch size");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int hw = h * w;
+  unsigned* words = reinterpret_cast<unsigned*>(scratch);
+  if (cudaMemsetAsync(scratch, 0, sizeof(unsigned) * kDvWords * n, st) != cudaSuccess)
+    return um::check_launch("um_depth_to_image");
+  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
+  long long bx = ((long long)hw + 1023) / 1024;                                     // 4 pixels per thread and pass
+  bx = bx < per_image ? bx : per_image;
+  const dim3 grid((unsigned)(bx > 0 ? bx : 1), (unsigned)n);
+  for (int pass = 0; pass < 4; ++pass) {
+    if (pass == 0) depth_hist_kernel<true><<<grid, 256, 0, st>>>(depth, words, hw, pass);
+    else depth_hist_kernel<false><<<grid, 256, 0, st>>>(depth, words, hw, pass);
+    if (int rc = um::check_launch("um_depth_to_image")) return rc;
+    depth_select_kernel<<<(unsigned)n, 256, 0, st>>>(words, hw, pass);
+    if (int rc = um::check_launch("um_depth_to_image")) return rc;
+  }
+  long long cx = ((long long)hw + 255) / 256;
+  cx = cx < 2 * per_image ? cx : 2 * per_image;
+  depth_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(depth, words, out, w, hw, row_stride, image_stride);
+  return um::check_launch("um_depth_to_image");
 }
 
 }  // extern "C"

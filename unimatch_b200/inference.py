@@ -20,8 +20,9 @@ colouring of utils/flow_viz.py on the device.  Decoding and writing files (frame
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
-does; `DepthSequenceRunner` streams host (uint8 frame, pose) items through the same path, replayed as a CUDA graph.  Colouring
-depth maps (matplotlib's `plasma`, evaluate_depth.py:403-417) stays out of scope.
+does; `DepthSequenceRunner` streams host (uint8 frame, pose) items through the same path, replayed as a CUDA graph;
+`depth_to_image` is the reference's `viz_depth_tensor(1. / depth)` (inverse depth scaled by its exact 95th percentile,
+matplotlib's `plasma` map, evaluate_depth.py:403-417) on the device.  Writing files (PNG) stays out of scope.
 
 Stereo (`inference_stereo`, evaluate_stereo.py:711-843): `StereoRunner` streams host uint8 (left, right) pairs, normalised and
 resized on the device, through the same path as `infer_stereo`, replayed as a CUDA graph; `disparity_to_image` is the
@@ -282,6 +283,27 @@ def infer_depth(model, img_ref, img_tgt, intrinsics, pose, *, padding_factor=16,
                   min_depth=1.0 / max_depth, max_depth=1.0 / min_depth, num_depth_candidates=num_depth_candidates,
                   depth_from_argmax=depth_from_argmax, pred_bidir_depth=pred_bidir_depth, **model_kwargs)["flow_preds"][-1]
     return _depth_outputs(depth, ori, size, pred_bidir_depth)
+
+
+def depth_to_image(depth, out=None):
+    """`viz_depth_tensor(1. / depth)` (utils/visualization.py:92-107, what the depth driver paints, evaluate_depth.py:403-417)
+    on the device for a batch: depths [N,H,W] -> uint8 RGB pictures [N,H,W,3] (PIL's channel order) of the inverse depth,
+    scaled from its minimum to its exact 95th percentile (np.percentile's linear interpolation) and coloured with
+    matplotlib's `plasma`; a single depth [H,W] gives one picture [H,W,3].  `out` may be a view into larger pictures (3-byte
+    pixels, any row / image stride).  A radix select of the two order statistics, then one colouring pass; see
+    oracle/depth_viz.py for the arithmetic and the edge cases (NaN, zero or negative depths)."""
+    if not torch.is_tensor(depth) or depth.dim() not in (2, 3) or not depth.dtype.is_floating_point or 0 in depth.shape:
+        raise ValueError("depth_to_image expects float depths [N,H,W] or [H,W]")
+    shape = tuple(depth.shape) + (3,)
+    if out is None:
+        out = torch.empty(shape, device=depth.device, dtype=torch.uint8)
+    elif not torch.is_tensor(out) or tuple(out.shape) != shape or out.dtype != torch.uint8:
+        raise ValueError("depth_to_image: out must be uint8 %s" % (list(shape),))
+    if depth.dim() == 2:
+        _OPS.depth_to_image(depth[None].float().contiguous(), out[None])
+    else:
+        _OPS.depth_to_image(depth.float().contiguous(), out)
+    return out
 
 
 def _depth_outputs(depth, ori, size, pred_bidir_depth):
@@ -739,7 +761,9 @@ class DepthSequenceRunner(_SequenceRunner):
       encoder on the new frames, the depth matching path on the `batch` pairs and the depth resized back.  The camera operands
       that depend on the intrinsics only (`UniMatch.depth_cameras`) are built once, eagerly, before any capture; the per-step
       poses are static device buffers that the upload fills.  The last frame's pose stays on the host for the next step;
-    * download: 'depth' (and 'depth_bwd') [H,W] per pair.
+    * download: 'depth' (and 'depth_bwd') [H,W] per pair and, with `visualize`, the uint8 RGB pictures 'vis' [H,W,3]
+      (+ 'vis_bwd') that the reference writes for them (`depth_to_image`, painted inside the step's graph);
+      `return_depth=False` with `visualize` sends back only the pictures.
 
     Sizes and semantics are those of `infer_depth_sequence` (and `infer_depth`): `min_depth` / `max_depth` are metric,
     the intrinsics [3,3] are not rescaled with the frames.  `run(items)` takes an iterable of (uint8 frame [H,W,3], pose [4,4])
@@ -749,8 +773,11 @@ class DepthSequenceRunner(_SequenceRunner):
 
     def __init__(self, model, frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None, min_depth=0.5,
                  max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False, use_graph=True,
-                 **model_kwargs):
+                 visualize=False, return_depth=True, **model_kwargs):
+        if not return_depth and not visualize:
+            raise ValueError("nothing to return: return_depth=False needs visualize=True")
         self.kw = _depth_task_kwargs(dict(model_kwargs), "DepthSequenceRunner")
+        self.visualize, self.return_depth = bool(visualize), bool(return_depth)
         K = _intrinsics33(intrinsics, "DepthSequenceRunner")
         self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
@@ -775,7 +802,13 @@ class DepthSequenceRunner(_SequenceRunner):
         depth = self.model.forward_encoded(first, second, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
                                            max_depth=self.inv_range[1], depth_from_argmax=self.from_argmax,
                                            pred_bidir_depth=self.bidir, **self.kw)["flow_preds"][-1]
-        return _depth_outputs(depth, self.ori, self.size, self.bidir)
+        out = _depth_outputs(depth, self.ori, self.size, self.bidir)
+        if self.visualize:
+            for k in [k for k in ("depth", "depth_bwd") if k in out]:
+                out[k.replace("depth", "vis")] = depth_to_image(out[k])
+                if not self.return_depth:
+                    del out[k]
+        return out
 
     def _reset_inputs(self, slot):
         super()._reset_inputs(slot)

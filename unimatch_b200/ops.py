@@ -101,6 +101,7 @@ _SIGNATURES = {
     "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_depth_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_eval_stats": (_RC, [_P, _L, _L, _L, _L, _P, _P, _P, _I, _I, _F, _F, _F, _I, _I, _I, _P, _P, _P]),
     "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
     "um_ffn_tc": (_RC, [ctypes.POINTER(FfnDesc), _P]),
@@ -458,6 +459,25 @@ def _disparity_to_image(disp, out):
 
 
 disparity_to_image = _define("disparity_to_image(Tensor disp, Tensor(a!) out) -> ()", _disparity_to_image)
+
+DEPTH_TO_IMAGE_SCRATCH_WORDS = 2056      # per image, include/unimatch_sm100.h (um_depth_to_image)
+
+
+def _depth_to_image(depth, out):
+    """depth: contiguous fp32 [N, H, W]; out: uint8 RGB [N, H, W, 3] with 3-byte pixels, rows and images may be strided."""
+    _f32c(depth, "depth")
+    if depth.dim() != 3:
+        raise RuntimeError("depth_to_image: expected depths [N, H, W]")
+    n, h, w = depth.shape
+    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
+            or out.device != depth.device:
+        raise RuntimeError("depth_to_image: out must be uint8 [N, H, W, 3] on the depth's device with 3-byte pixels")
+    scratch = torch.empty((DEPTH_TO_IMAGE_SCRATCH_WORDS * n,), device=depth.device, dtype=torch.int32)
+    _check(LIB.um_depth_to_image(_p(depth), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
+           "um_depth_to_image")
+
+
+depth_to_image = _define("depth_to_image(Tensor depth, Tensor(a!) out) -> ()", _depth_to_image)
 
 
 def _eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, eval_max):
