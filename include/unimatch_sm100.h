@@ -229,6 +229,36 @@ int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, i
 int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,
                       int32_t h, int32_t w, void* stream);
 
+/* ---- leaderboard submission payloads -------------------------------------------------------------------------
+ * One launch from the model's planar output pred = DEVICE fp32 [batch, C, h, w] at the inference size (C = 2 flow, 1
+ * disparity) to each sample's file payload, without the header: sample i at out + i * sample_stride (bytes).  Geometry:
+ *   UM_SUBMIT_CROP:   value (Y, X) = pred[i, c, top + Y, left + X], the InputPadder unpad (top + out_h <= h, left + out_w <= w);
+ *   UM_SUBMIT_RESIZE: the align-corners bilinear resize to (out_h, out_w) of um_resize_bilinear, then the reference's two
+ *                     rounded steps (x * out_w) / w for u and disparity, (x * out_h) / h for v (evaluate_flow.py:67-70,
+ *                     evaluate_stereo.py:87); top / left unused.
+ * Formats (payload bytes per sample):
+ *   UM_SUBMIT_FLO             writeFlow (utils/frame_utils.py:70-99): interleaved (u, v) fp32 little-endian, row-major; 8 h w
+ *   UM_SUBMIT_KITTI_FLOW_PNG  writeFlowKITTI (:117-121): PNG scanlines of RGB uint16 big-endian, R = q(64 u + 32768),
+ *                             G = q(64 v + 32768), B = 1 (fp32 multiply, then fp32 add); (1 + 6 w) h
+ *   UM_SUBMIT_KITTI_DISP_PNG  (disp * 256.).astype(np.uint16) (evaluate_stereo.py:91): PNG scanlines of grey uint16
+ *                             big-endian, q(256 d) in fp32; (1 + 2 w) h
+ *   UM_SUBMIT_PFM             write_pfm (utils/file_io.py:98-127): fp32 little-endian, rows bottom to top; 4 h w
+ * q is numpy's float -> uint16 cast on x86-64: truncate toward zero to int32, NaN / +-inf / anything outside the int32
+ * range -> INT32_MIN, keep the low 16 bits (so 65536 -> 0, -1.5 -> 65535, NaN -> 0).  PNG scanlines carry the "Up" filter
+ * (each byte minus the byte above it, mod 256, filter byte 2; row 0 unfiltered, filter byte 0): the host only deflates.
+ * out_w / out_h are the sizes in the payload; every operation is a correctly rounded fp32 intrinsic (no contraction).  The
+ * crop copies values bit for bit; a NaN out of the resize arithmetic is the device's canonical 0x7fffffff.
+ * FLO needs 8-byte and PFM 4-byte alignment of out and sample_stride.  No host synchronisation: graph-capturable. */
+#define UM_SUBMIT_CROP 0
+#define UM_SUBMIT_RESIZE 1
+#define UM_SUBMIT_FLO 0
+#define UM_SUBMIT_KITTI_FLOW_PNG 1
+#define UM_SUBMIT_KITTI_DISP_PNG 2
+#define UM_SUBMIT_PFM 3
+int um_encode_submission(const float* pred, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t geometry,
+                         int32_t top, int32_t left, int32_t out_h, int32_t out_w, int32_t format, uint8_t* out,
+                         int64_t sample_stride, void* stream);
+
 /* ---- evaluation statistics -----------------------------------------------------------------------------------
  * One pass from a batch of predictions at ground-truth resolution to a [batch, S] float64 table of per-sample sufficient
  * statistics (pixel counts, counts over thresholds, fp64 sums), from which the host forms the metrics of the reference's

@@ -3,7 +3,7 @@
     from unimatch_b200 import UniMatch      # drop-in for reference unimatch.unimatch.UniMatch (inference)
 
 The C-ABI library (libunimatch_sm100.so) is loaded -- and built with nvcc when the in-tree copy is stale -- the first
-time `ops`, `UniMatch` or one of the inference / validation drivers is touched; `spec`, `synthetic` and `sharding` are plain Python and
+time `ops`, `UniMatch` or one of the inference / validation / submission drivers is touched; `spec`, `synthetic` and `sharding` are plain Python and
 import without it (the CPU reference arm of bench.py and the oracle tests never map the product library).
 There is no CPU / eager fallback for the `torch.ops.unimatch_sm100.*` ops.
 """
@@ -31,12 +31,14 @@ _LAZY = {
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
+    "create_flow_submission": (".submission", "create_flow_submission"),
+    "create_stereo_submission": (".submission", "create_stereo_submission"),
 }
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
            "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "disparity_to_image", "depth_to_image",
-           "validate_flow", "validate_stereo", "validate_depth"]
+           "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission"]
 
 
 def __getattr__(name):

@@ -555,6 +555,75 @@ __global__ void __launch_bounds__(256) depth_color_kernel(const float* __restric
   }
 }
 
+// ---- leaderboard submission payloads (evaluate_flow.py:19-156, evaluate_stereo.py:28-298) ---------------------------------
+struct SubmitGeom {
+  const float* pred;
+  int C, h, w, H, W, top, left, resize;
+};
+
+// Value of channel c at payload pixel (Y, X): the unpad crop, or the align-corners resize with the reference's two-step
+// rescale ((x * ori) / inf, two roundings; not x * (ori / inf)).
+__device__ __forceinline__ float submit_value(const SubmitGeom& g, long long b, int c, int Y, int X) {
+  const float* plane = g.pred + (b * g.C + c) * (long long)g.h * g.w;
+  if (!g.resize) return __ldg(plane + (long long)(Y + g.top) * g.w + (X + g.left));
+  const float v = bilinear_align_corners([&](int y, int x) { return __ldg(plane + (long long)y * g.w + x); }, g.h, g.w, g.H, g.W,
+                                         Y, X);
+  return c == 0 ? __fdiv_rn(__fmul_rn(v, (float)g.W), (float)g.w) : __fdiv_rn(__fmul_rn(v, (float)g.H), (float)g.h);
+}
+
+// numpy's float -> uint16 cast on x86-64 (cvttss2si, then the low 16 bits): truncation toward zero where the result fits
+// int32, INT32_MIN (low half 0) for NaN, +-inf and everything else.  __float2int_rz saturates instead, so the range test
+// comes first and the conversion only sees values it converts exactly.
+__device__ __forceinline__ unsigned numpy_u16(float x) {
+  const int t = (x >= -2147483648.0f && x < 2147483648.0f) ? __float2int_rz(x) : (-2147483647 - 1);
+  return (unsigned)t & 0xffffu;
+}
+
+// The uint16 samples of payload pixel (Y, X): 3 for KITTI flow (R, G, B), 1 for KITTI disparity.
+template <int FMT>
+__device__ __forceinline__ void submit_png_samples(const SubmitGeom& g, long long b, int Y, int X, unsigned* s) {
+  if (FMT == UM_SUBMIT_KITTI_FLOW_PNG) {
+    s[0] = numpy_u16(__fadd_rn(__fmul_rn(64.0f, submit_value(g, b, 0, Y, X)), 32768.0f));
+    s[1] = numpy_u16(__fadd_rn(__fmul_rn(64.0f, submit_value(g, b, 1, Y, X)), 32768.0f));
+    s[2] = 1u;
+  } else {
+    s[0] = numpy_u16(__fmul_rn(submit_value(g, b, 0, Y, X), 256.0f));
+  }
+}
+
+// One thread per payload pixel.  PNG formats: the pixel's big-endian bytes minus those of the pixel above (the "Up" filter),
+// which the thread recomputes, so rows stay independent; thread X = 0 writes the row's filter byte.
+template <int FMT>
+__global__ void __launch_bounds__(256) encode_submission_kernel(SubmitGeom g, uint8_t* __restrict__ out, long long sample_stride,
+                                                                long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int X = (int)(i % g.W);
+  const int Y = (int)((i / g.W) % g.H);
+  const long long b = i / ((long long)g.H * g.W);
+  uint8_t* dst = out + b * sample_stride;
+  if (FMT == UM_SUBMIT_FLO) {
+    reinterpret_cast<float2*>(dst)[(long long)Y * g.W + X] = make_float2(submit_value(g, b, 0, Y, X), submit_value(g, b, 1, Y, X));
+  } else if (FMT == UM_SUBMIT_PFM) {
+    reinterpret_cast<float*>(dst)[(long long)(g.H - 1 - Y) * g.W + X] = submit_value(g, b, 0, Y, X);
+  } else {
+    constexpr int NS = FMT == UM_SUBMIT_KITTI_FLOW_PNG ? 3 : 1;
+    unsigned cur[NS], up[NS];
+    submit_png_samples<FMT>(g, b, Y, X, cur);
+    if (Y > 0) submit_png_samples<FMT>(g, b, Y - 1, X, up);
+    uint8_t* row = dst + (long long)Y * (1 + 2 * NS * (long long)g.W);
+    if (X == 0) row[0] = Y > 0 ? 2 : 0;
+    uint8_t* px = row + 1 + 2 * NS * (long long)X;
+#pragma unroll
+    for (int k = 0; k < NS; ++k) {
+      unsigned hi = cur[k] >> 8, lo = cur[k] & 0xffu;
+      if (Y > 0) { hi -= up[k] >> 8; lo -= up[k] & 0xffu; }
+      px[2 * k] = (uint8_t)hi;
+      px[2 * k + 1] = (uint8_t)lo;
+    }
+  }
+}
+
 inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
   const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
@@ -695,6 +764,41 @@ int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int6
   cx = cx < 2 * per_image ? cx : 2 * per_image;
   depth_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(depth, words, out, w, hw, row_stride, image_stride);
   return um::check_launch("um_depth_to_image");
+}
+
+int um_encode_submission(const float* pred, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t geometry,
+                         int32_t top, int32_t left, int32_t out_h, int32_t out_w, int32_t format, uint8_t* out,
+                         int64_t sample_stride, void* stream) {
+  UM_REQUIRE(pred && out && batch > 0 && h > 0 && w > 0 && out_h > 0 && out_w > 0, "um_encode_submission: bad arguments");
+  UM_REQUIRE(format >= UM_SUBMIT_FLO && format <= UM_SUBMIT_PFM, "um_encode_submission: unknown format %d", format);
+  const bool flow = format == UM_SUBMIT_FLO || format == UM_SUBMIT_KITTI_FLOW_PNG;
+  UM_REQUIRE(channels == (flow ? 2 : 1), "um_encode_submission: format %d needs %d channels", format, flow ? 2 : 1);
+  UM_REQUIRE(geometry == UM_SUBMIT_RESIZE ||
+                 (geometry == UM_SUBMIT_CROP && top >= 0 && left >= 0 && top + out_h <= h && left + out_w <= w),
+             "um_encode_submission: the crop must lie inside the prediction");
+  const long long pixels = (long long)out_h * out_w;
+  const long long bytes = format == UM_SUBMIT_FLO ? 8 * pixels
+                        : format == UM_SUBMIT_PFM ? 4 * pixels
+                        : (long long)out_h * (1 + (format == UM_SUBMIT_KITTI_FLOW_PNG ? 6LL : 2LL) * out_w);
+  UM_REQUIRE(sample_stride >= bytes, "um_encode_submission: sample_stride must cover the %lld payload bytes", bytes);
+  const int align = format == UM_SUBMIT_FLO ? 8 : (format == UM_SUBMIT_PFM ? 4 : 1);
+  UM_REQUIRE((uintptr_t)out % align == 0 && sample_stride % align == 0,
+             "um_encode_submission: out and sample_stride must be %d-byte aligned for this format", align);
+  const SubmitGeom g{pred, channels, h, w, out_h, out_w, top, left, geometry == UM_SUBMIT_RESIZE ? 1 : 0};
+  const long long total = (long long)batch * pixels;
+  const unsigned grid = (unsigned)((total + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (format) {
+    case UM_SUBMIT_FLO: encode_submission_kernel<UM_SUBMIT_FLO><<<grid, 256, 0, st>>>(g, out, sample_stride, total); break;
+    case UM_SUBMIT_KITTI_FLOW_PNG:
+      encode_submission_kernel<UM_SUBMIT_KITTI_FLOW_PNG><<<grid, 256, 0, st>>>(g, out, sample_stride, total);
+      break;
+    case UM_SUBMIT_KITTI_DISP_PNG:
+      encode_submission_kernel<UM_SUBMIT_KITTI_DISP_PNG><<<grid, 256, 0, st>>>(g, out, sample_stride, total);
+      break;
+    default: encode_submission_kernel<UM_SUBMIT_PFM><<<grid, 256, 0, st>>>(g, out, sample_stride, total); break;
+  }
+  return um::check_launch("um_encode_submission");
 }
 
 }  // extern "C"

@@ -16,7 +16,8 @@ Video (`main_flow.py --inference_video`, evaluate_flow.py:642-831): `infer_flow_
 sequence with every frame encoded ONCE (pair (t, t+1) and pair (t+1, t+2) share frame t+1's feature pyramid; the encoder is
 per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 summation order), `VideoFlowRunner` streams host uint8 frames through the same
 path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
-colouring of utils/flow_viz.py on the device.  Decoding and writing files (frames, PNG, .flo, mp4) stay out of scope.
+colouring of utils/flow_viz.py on the device.  Decoding frames and writing videos (mp4) stay out of scope; the leaderboard
+files (.flo, PNG, PFM) are written by `submission.py`.
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference

@@ -102,6 +102,7 @@ _SIGNATURES = {
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_depth_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_encode_submission": (_RC, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
     "um_eval_stats": (_RC, [_P, _L, _L, _L, _L, _P, _P, _P, _I, _I, _F, _F, _F, _I, _I, _I, _P, _P, _P]),
     "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
     "um_ffn_tc": (_RC, [ctypes.POINTER(FfnDesc), _P]),
@@ -478,6 +479,45 @@ def _depth_to_image(depth, out):
 
 
 depth_to_image = _define("depth_to_image(Tensor depth, Tensor(a!) out) -> ()", _depth_to_image)
+
+# include/unimatch_sm100.h (um_encode_submission)
+SUBMIT_CROP, SUBMIT_RESIZE = 0, 1
+SUBMIT_FLO, SUBMIT_KITTI_FLOW_PNG, SUBMIT_KITTI_DISP_PNG, SUBMIT_PFM = 0, 1, 2, 3
+SUBMIT_CHANNELS = {SUBMIT_FLO: 2, SUBMIT_KITTI_FLOW_PNG: 2, SUBMIT_KITTI_DISP_PNG: 1, SUBMIT_PFM: 1}
+
+
+def submission_payload_bytes(fmt, h, w):
+    """Payload bytes of one (h, w) sample in format `fmt` (PNG formats: filtered scanlines, one filter byte per row)."""
+    if fmt == SUBMIT_FLO:
+        return 8 * h * w
+    if fmt == SUBMIT_PFM:
+        return 4 * h * w
+    if fmt == SUBMIT_KITTI_FLOW_PNG:
+        return h * (1 + 6 * w)
+    if fmt == SUBMIT_KITTI_DISP_PNG:
+        return h * (1 + 2 * w)
+    raise RuntimeError("encode_submission: unknown format %r" % (fmt,))
+
+
+def _encode_submission(pred, fmt, out_h, out_w, resize, top, left):
+    """pred: contiguous fp32 [B, C, h, w] at the inference size -> uint8 [B, bytes], each row one sample's file payload.
+    `resize`: align-corners resize to (out_h, out_w) with the two-step rescale; otherwise the crop at (top, left)."""
+    _f32c(pred, "pred")
+    if pred.dim() != 4:
+        raise RuntimeError("encode_submission: expected planar predictions [B, C, h, w]")
+    if fmt not in SUBMIT_CHANNELS or pred.shape[1] != SUBMIT_CHANNELS[fmt]:
+        raise RuntimeError("encode_submission: format %r needs [B, %s, h, w]" % (fmt, SUBMIT_CHANNELS.get(fmt, "?")))
+    b, c, h, w = pred.shape
+    nbytes = submission_payload_bytes(fmt, out_h, out_w)
+    out = torch.empty((b, nbytes), device=pred.device, dtype=torch.uint8)
+    _check(LIB.um_encode_submission(_p(pred), b, c, h, w, SUBMIT_RESIZE if resize else SUBMIT_CROP, top, left, out_h, out_w,
+                                    fmt, _p(out), nbytes, _stream()), "um_encode_submission")
+    return out
+
+
+encode_submission = _define(
+    "encode_submission(Tensor pred, int fmt, int out_h, int out_w, bool resize, int top, int left) -> Tensor",
+    _encode_submission)
 
 
 def _eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, eval_max):
