@@ -195,6 +195,45 @@ int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h,
 int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t h_out,
                                    int32_t w_out, const float* mean, const float* std, void* stream);
 
+/* ---- ragged batches: images of different sizes packed back to back ------------------------------------------
+ * Per-image geometry of the *_ragged entries, a DEVICE array of n items (read by the kernels, so a CUDA graph replay picks
+ * up whatever the table holds at that time).  offset: where image i starts in the packed buffer, in elements of that
+ * buffer (bytes for uint8 frames [h, w, 3]; floats for disparities [h, w], whose BGR pictures start at 3 * offset bytes);
+ * (h, w): its size; scale and flags: used by um_resize_bilinear_ragged only.  An item with h or w outside 1..capacity, or
+ * that does not fit in the packed buffer (numel / bytes arguments), is skipped: nothing of it is read or written.  Each
+ * entry validates its scalar arguments before any CUDA call, launches a grid sized by the capacity (h_max, w_max) or the
+ * uniform side, and never synchronises: graph-capturable.  n <= 65535. */
+typedef struct um_ragged_item {
+  int64_t offset;
+  int32_t h, w;
+  float scale;
+  int32_t flags;
+} um_ragged_item;
+#define UM_RAGGED_FLIP_X 1   /* um_resize_bilinear_ragged: mirror the item's output horizontally */
+
+/* um_frames_to_planar_normalized per frame: frame i = DEVICE uint8 [h_i, w_i, 3] at frames + items[i].offset (frames_bytes
+ * = size of the packed buffer) -> out fp32 planar [n, 3, h_out, w_out].  Image i is bit-identical to
+ * um_frames_to_planar_normalized of frame i alone (the same device code: three correctly rounded fp32 operations per
+ * sample, then the align-corners resample; a frame at the output size comes out as its normalised samples). */
+int um_frames_to_planar_normalized_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out,
+                                          int32_t n, int32_t h_max, int32_t w_max, int32_t h_out, int32_t w_out,
+                                          const float* mean, const float* std, void* stream);
+
+/* um_resize_bilinear per item: in = uniform planar [n, 1, h_in, w_in] fp32 -> item i at out + items[i].offset (out_numel
+ * floats in all), size (h_i, w_i), multiplied by items[i].scale unless it is 1.0f, mirrored with UM_RAGGED_FLIP_X.  Item i is
+ * bit-identical to um_resize_bilinear of image i alone with scale = &items[i].scale; an item at (h_in, w_in) without the flip
+ * is copied as it is (what the stereo driver does with a disparity it does not resize, evaluate_stereo.py:813-836).
+ * Replaces the resize back, disparity rescale and flip back of inference_stereo for pairs of different sizes. */
+int um_resize_bilinear_ragged(const float* in, float* out, int64_t out_numel, const um_ragged_item* items, int32_t n,
+                              int32_t h_in, int32_t w_in, int32_t h_max, int32_t w_max, void* stream);
+
+/* um_disparity_to_image per item: disparity i = fp32 [h_i, w_i] at disp + items[i].offset (numel floats in all) -> its BGR
+ * picture at out + 3 * items[i].offset bytes, rows of 3 w_i bytes.  Picture i is bit-identical to um_disparity_to_image of
+ * disparity i alone (NaN / constant / inf rule included).  minmax_scratch: DEVICE buffer of 2n words, reset inside the call.
+ * Replaces vis_disparity on each predicted disparity of inference_stereo (evaluate_stereo.py:820-841). */
+int um_disparity_to_image_ragged(const float* disp, int64_t numel, const um_ragged_item* items, uint8_t* out,
+                                 float* minmax_scratch, int32_t n, int32_t h_max, int32_t w_max, void* stream);
+
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the

@@ -108,22 +108,86 @@ __device__ __forceinline__ float bilinear_align_corners(const Load& load, int hi
   return __fmaf_rn(hy, row0, __fmul_rn(ly, row1));
 }
 
-// out[b,c,Y,X] = scale[c] * bilinear(in[b,c], ...).  `flip_x`: the OUTPUT is mirrored horizontally (torchvision hflip of
+// ---- per-image geometry of the ragged entries (um_ragged_item, read from device memory) ----------------------------------
+// An item is used only if it lies inside the capacity and inside the packed buffer; otherwise its thread writes nothing.
+__device__ __forceinline__ bool ragged_ok(const um_ragged_item& it, int h_max, int w_max, long long pixels_per_elem,
+                                          long long numel) {
+  return it.h > 0 && it.w > 0 && it.h <= h_max && it.w <= w_max && it.offset >= 0 &&
+         it.offset + pixels_per_elem * it.h * it.w <= numel;
+}
+
+// One output sample of a planar resize: source plane (hi, wi), destination plane (ho, wo), scale and flip.
+struct ResizeSample {
+  const float* src;
+  float* dst;
+  int ho, wo, Y, X;
+  float sc;
+  int flip_x, copy;
+};
+
+// Uniform batch [B, C, ho, wo]: one thread per output sample, channel c scaled by s_c.
+struct ResizeUniform {
+  const float* in;
+  float* out;
+  int C, hi, wi, ho, wo;
+  float s0, s1, s2;
+  int flip_x;
+  long long total;
+  __device__ __forceinline__ bool sample(ResizeSample& s) const {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return false;
+    s.X = (int)(i % wo);
+    s.Y = (int)((i / wo) % ho);
+    const long long bc = i / ((long long)ho * wo);
+    const int c = (int)(bc % C);
+    s.src = in + bc * (long long)hi * wi;
+    s.dst = out + bc * (long long)ho * wo;
+    s.ho = ho; s.wo = wo;
+    s.sc = c == 0 ? s0 : (c == 1 ? s1 : s2);
+    s.flip_x = flip_x;
+    s.copy = 0;
+    return true;
+  }
+};
+
+// Uniform single-channel batch [n, 1, hi, wi] -> item i at out + offset[i] at its own (h, w), scale and flip (grid y: item,
+// grid x: the capacity's pixels).  An item at the input size without a flip is copied as it is, as the stereo driver
+// leaves a disparity that needs no resize (the bilinear pass would turn a non-finite neighbour into NaN there).
+struct ResizeRagged {
+  const float* in;
+  float* out;
+  const um_ragged_item* items;
+  int hi, wi, h_max, w_max;
+  long long out_numel;
+  __device__ __forceinline__ bool sample(ResizeSample& s) const {
+    const int n = blockIdx.y;
+    const um_ragged_item it = items[n];
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (!ragged_ok(it, h_max, w_max, 1, out_numel) || q >= (long long)it.h * it.w) return false;
+    s.X = (int)(q % it.w);
+    s.Y = (int)(q / it.w);
+    s.src = in + (long long)n * hi * wi;
+    s.dst = out + it.offset;
+    s.ho = it.h; s.wo = it.w;
+    s.sc = it.scale;
+    s.flip_x = it.flags & UM_RAGGED_FLIP_X;
+    s.copy = !s.flip_x && it.h == hi && it.w == wi;
+    return true;
+  }
+};
+
+// out = scale * bilinear(in, ...).  `flip_x`: the OUTPUT is mirrored horizontally (torchvision hflip of
 // evaluate_stereo.py:789-796 folded into the same pass).
-__global__ void __launch_bounds__(256) resize_bilinear_kernel(const float* __restrict__ in, float* __restrict__ out, int C,
-                                                              int hi, int wi, int ho, int wo, float s0, float s1, float s2,
-                                                              int flip_x, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int X = (int)(i % wo);
-  const int Y = (int)((i / wo) % ho);
-  const long long bc = i / ((long long)ho * wo);
-  const int c = (int)(bc % C);
-  const float* base = in + bc * (long long)hi * wi;
-  const float v = bilinear_align_corners([&](int y, int x) { return __ldg(base + (long long)y * wi + x); }, hi, wi, ho, wo, Y, X);
-  const float sc = c == 0 ? s0 : (c == 1 ? s1 : s2);
-  const int Xo = flip_x ? wo - 1 - X : X;
-  out[(bc * ho + Y) * (long long)wo + Xo] = sc == 1.0f ? v : v * sc;
+template <class Geo>
+__global__ void __launch_bounds__(256) resize_bilinear_kernel(Geo geo, int hi, int wi) {
+  ResizeSample s;
+  if (!geo.sample(s)) return;
+  const float* base = s.src;
+  const float v = s.copy ? __ldg(base + (long long)s.Y * wi + s.X)
+                         : bilinear_align_corners([&](int y, int x) { return __ldg(base + (long long)y * wi + x); }, hi, wi,
+                                                  s.ho, s.wo, s.Y, s.X);
+  const int Xo = s.flip_x ? s.wo - 1 - s.X : s.X;
+  s.dst[(long long)s.Y * s.wo + Xo] = s.sc == 1.0f ? v : v * s.sc;
 }
 
 // ---- video frames -> model input: uint8 [T,H,W,3] channel-last -> fp32 planar [T,3,ho,wo] -------------------------------
@@ -154,19 +218,60 @@ __global__ void __launch_bounds__(256) frames_to_planar_kernel(const uint8_t* __
 // = resize_bilinear of the frames normalised the way the depth data pipeline does it on the host
 // (dataloader/depth/augmentation.py:30, 56-61): every SOURCE sample is x / 255, then - mean_c, then / std_c, each one
 // correctly rounded fp32 operation in that order, and the normalised samples are resampled.  No transpose: the depth
-// drivers have no portrait rule.
-__global__ void __launch_bounds__(256) frames_to_planar_normalized_kernel(const uint8_t* __restrict__ frames,
-                                                                          float* __restrict__ out, int H, int W, int ho, int wo,
+// drivers have no portrait rule.  `Geo` says where frame t lies and how large it is: one size for the whole batch
+// (FramesUniform), or each frame at its own offset and size in a packed buffer (FramesRagged); the output is uniform.
+struct FramePixel {
+  const uint8_t* base;
+  int H, W;
+  long long t;
+  int Y, X;
+};
+
+struct FramesUniform {
+  const uint8_t* frames;
+  int H, W, ho, wo;
+  long long total;
+  __device__ __forceinline__ bool pixel(FramePixel& p) const {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return false;
+    p.X = (int)(i % wo);
+    p.Y = (int)((i / wo) % ho);
+    p.t = i / ((long long)ho * wo);
+    p.base = frames + p.t * (long long)H * W * 3;
+    p.H = H; p.W = W;
+    return true;
+  }
+};
+
+// grid (x: output pixels, y: frame)
+struct FramesRagged {
+  const uint8_t* frames;
+  const um_ragged_item* items;
+  int h_max, w_max, ho, wo;
+  long long frames_bytes;
+  __device__ __forceinline__ bool pixel(FramePixel& p) const {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    p.t = blockIdx.y;
+    const um_ragged_item it = items[p.t];
+    if (i >= (long long)ho * wo || !ragged_ok(it, h_max, w_max, 3, frames_bytes)) return false;
+    p.X = (int)(i % wo);
+    p.Y = (int)(i / wo);
+    p.base = frames + it.offset;
+    p.H = it.h; p.W = it.w;
+    return true;
+  }
+};
+
+template <class Geo>
+__global__ void __launch_bounds__(256) frames_to_planar_normalized_kernel(Geo geo, float* __restrict__ out, int ho, int wo,
                                                                           float m0, float m1, float m2, float s0, float s1,
-                                                                          float s2, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int X = (int)(i % wo);
-  const int Y = (int)((i / wo) % ho);
-  const long long t = i / ((long long)ho * wo);
-  const uint8_t* base = frames + t * (long long)H * W * 3;
+                                                                          float s2) {
+  FramePixel p;
+  if (!geo.pixel(p)) return;
+  const int H = p.H, W = p.W, X = p.X, Y = p.Y;
+  const uint8_t* base = p.base;
   const long long plane = (long long)ho * wo;
-  float* o = out + t * 3 * plane + (long long)Y * wo + X;
+  float* o = out + p.t * 3 * plane + (long long)Y * wo + X;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     const float mean = c == 0 ? m0 : (c == 1 ? m1 : m2), std = c == 0 ? s0 : (c == 1 ? s1 : s2);
@@ -305,11 +410,46 @@ __device__ const uint8_t kInferno[768] = {
     138, 246, 243, 142, 248, 244, 146, 249, 245, 150, 250, 246, 154, 251, 248, 157, 252, 249, 161, 253, 250, 164, 255, 252,
 };
 
+// Where disparity image n and its picture lie: one size, contiguous disparities and strided pictures (DispUniform), or each
+// image at its own offset and size in a packed buffer, its picture at 3 * offset bytes with 3w-byte rows (DispRagged).
+// A ragged item that does not fit (ragged_ok) has hw = 0: it reads and writes nothing.
+struct DispImage {
+  const float* d;
+  uint8_t* img;
+  int w, hw;
+  long long row_stride;
+};
+
+struct DispUniform {
+  const float* disp;
+  uint8_t* out;
+  int w, hw;
+  long long row_stride, image_stride;
+  __device__ __forceinline__ DispImage image(int n) const {
+    return DispImage{disp + (long long)n * hw, out + n * image_stride, w, hw, row_stride};
+  }
+};
+
+struct DispRagged {
+  const float* disp;
+  uint8_t* out;
+  const um_ragged_item* items;
+  int h_max, w_max;
+  long long numel;
+  __device__ __forceinline__ DispImage image(int n) const {
+    const um_ragged_item it = items[n];
+    const bool ok = ragged_ok(it, h_max, w_max, 1, numel);
+    return DispImage{disp + (ok ? it.offset : 0), out + 3 * (ok ? it.offset : 0), it.w, ok ? it.h * it.w : 0, 3LL * it.w};
+  }
+};
+
 // grid (x: CTAs over the pixels of one image, y: image); 4 loads in flight per thread and step
-__global__ void __launch_bounds__(256) disp_minmax_kernel(const float* __restrict__ disp, unsigned* __restrict__ lo,
-                                                          unsigned* __restrict__ hi, int hw) {
+template <class Geo>
+__global__ void __launch_bounds__(256) disp_minmax_kernel(Geo geo, unsigned* __restrict__ lo, unsigned* __restrict__ hi) {
   const int n = blockIdx.y;
-  const float* d = disp + (long long)n * hw;
+  const DispImage im = geo.image(n);
+  const float* d = im.d;
+  const int hw = im.hw;
   unsigned l = 0, m = 0;
   bool nan = false;
   const int stride = gridDim.x * blockDim.x;
@@ -343,19 +483,22 @@ __global__ void __launch_bounds__(256) disp_minmax_kernel(const float* __restric
 
 // grid (x: CTAs over the pixels of one image, y: image); the LUT is staged in shared memory once per CTA, because every
 // warp indexes it divergently (a __constant__ table would serialise those reads)
-__global__ void __launch_bounds__(256) disp_color_kernel(const float* __restrict__ disp, const unsigned* __restrict__ lo,
-                                                         const unsigned* __restrict__ hi, uint8_t* __restrict__ out, int w,
-                                                         int hw, long long row_stride, long long image_stride) {
+template <class Geo>
+__global__ void __launch_bounds__(256) disp_color_kernel(Geo geo, const unsigned* __restrict__ lo,
+                                                         const unsigned* __restrict__ hi) {
   __shared__ uint8_t lut[768];
   for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kInferno[i];
   __syncthreads();
   const int n = blockIdx.y;
+  const DispImage im = geo.image(n);
+  const int w = im.w, hw = im.hw;
+  const long long row_stride = im.row_stride;
   const unsigned hkey = __ldg(hi + n);
   const bool flagged = hkey == kNanKey;
   const float mn = key_float(~__ldg(lo + n)), mx = key_float(hkey);
   const float range = __fsub_rn(mx, mn);
-  const float* d = disp + (long long)n * hw;
-  uint8_t* img = out + n * image_stride;
+  const float* d = im.d;
+  uint8_t* img = im.img;
   for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
     const float q = __fmul_rn(__fdiv_rn(__fsub_rn(__ldg(d + p), mn), range), 255.0f);
     const int g = (flagged || !(q >= 0.f)) ? 0 : min((int)q, 255);          // NaN -> 0; (int) truncates, as numpy's cast
@@ -670,9 +813,19 @@ int um_resize_bilinear(const float* in, float* out, int32_t batch, int32_t chann
   const long long total = (long long)batch * channels * h_out * w_out;
   const float s0 = scale ? scale[0] : 1.0f, s1 = (scale && channels > 1) ? scale[1] : 1.0f,
               s2 = (scale && channels > 2) ? scale[2] : 1.0f;
-  resize_bilinear_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(in, out, channels, h_in, w_in, h_out,
-                                                                                          w_out, s0, s1, s2, flip_x, total);
+  const ResizeUniform geo{in, out, channels, h_in, w_in, h_out, w_out, s0, s1, s2, flip_x, total};
+  resize_bilinear_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, h_in, w_in);
   return um::check_launch("um_resize_bilinear");
+}
+
+int um_resize_bilinear_ragged(const float* in, float* out, int64_t out_numel, const um_ragged_item* items, int32_t n,
+                              int32_t h_in, int32_t w_in, int32_t h_max, int32_t w_max, void* stream) {
+  UM_REQUIRE(in && out && items && n > 0 && n <= 65535 && h_in > 0 && w_in > 0 && h_max > 0 && w_max > 0 && out_numel > 0,
+             "um_resize_bilinear_ragged: bad arguments (1-65535 items, positive sizes, non-null buffers)");
+  const long long cap = (long long)h_max * w_max;
+  const ResizeRagged geo{in, out, items, h_in, w_in, h_max, w_max, out_numel};
+  resize_bilinear_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(geo, h_in, w_in);
+  return um::check_launch("um_resize_bilinear_ragged");
 }
 
 int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t transpose,
@@ -690,9 +843,24 @@ int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n,
   UM_REQUIRE(frames && out && mean && std && n > 0 && h > 0 && w > 0 && h_out > 0 && w_out > 0,
              "um_frames_to_planar_normalized: bad arguments (positive sizes, non-null buffers, 3 means and stds)");
   const long long total = (long long)n * h_out * w_out;
+  const FramesUniform geo{frames, h, w, h_out, w_out, total};
   frames_to_planar_normalized_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      frames, out, h, w, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2], total);
+      geo, out, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
   return um::check_launch("um_frames_to_planar_normalized");
+}
+
+int um_frames_to_planar_normalized_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out,
+                                          int32_t n, int32_t h_max, int32_t w_max, int32_t h_out, int32_t w_out,
+                                          const float* mean, const float* std, void* stream) {
+  UM_REQUIRE(frames && items && out && mean && std && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && h_out > 0 &&
+                 w_out > 0 && frames_bytes > 0,
+             "um_frames_to_planar_normalized_ragged: bad arguments (1-65535 frames, positive sizes, non-null buffers, 3 means "
+             "and stds)");
+  const long long plane = (long long)h_out * w_out;
+  const FramesRagged geo{frames, items, h_max, w_max, h_out, w_out, frames_bytes};
+  frames_to_planar_normalized_kernel<<<dim3((unsigned)((plane + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(
+      geo, out, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
+  return um::check_launch("um_frames_to_planar_normalized_ragged");
 }
 
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
@@ -729,12 +897,36 @@ int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, i
   const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
   long long bx = ((long long)hw + 1023) / 1024;                                     // 4 pixels per thread and pass
   bx = bx < per_image ? bx : per_image;
-  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(disp, lo, hi, hw);
+  const DispUniform geo{disp, out, w, hw, row_stride, image_stride};
+  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, lo, hi);
   if (int rc = um::check_launch("um_disparity_to_image")) return rc;
   long long cx = ((long long)hw + 255) / 256;
   cx = cx < 2 * per_image ? cx : 2 * per_image;
-  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(disp, lo, hi, out, w, hw, row_stride, image_stride);
+  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
   return um::check_launch("um_disparity_to_image");
+}
+
+int um_disparity_to_image_ragged(const float* disp, int64_t numel, const um_ragged_item* items, uint8_t* out,
+                                 float* minmax_scratch, int32_t n, int32_t h_max, int32_t w_max, void* stream) {
+  UM_REQUIRE(disp && items && out && minmax_scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && numel > 0,
+             "um_disparity_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
+  UM_REQUIRE((long long)h_max * w_max <= 0x7fffffffLL, "um_disparity_to_image_ragged: an image has at most 2^31 - 1 pixels");
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long cap = (long long)h_max * w_max;      // the grid is sized for the largest image; smaller ones stride less
+  unsigned* lo = reinterpret_cast<unsigned*>(minmax_scratch);
+  unsigned* hi = lo + n;
+  if (cudaMemsetAsync(minmax_scratch, 0, sizeof(float) * 2 * n, st) != cudaSuccess)
+    return um::check_launch("um_disparity_to_image_ragged");
+  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;
+  long long bx = (cap + 1023) / 1024;
+  bx = bx < per_image ? bx : per_image;
+  const DispRagged geo{disp, out, items, h_max, w_max, numel};
+  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, lo, hi);
+  if (int rc = um::check_launch("um_disparity_to_image_ragged")) return rc;
+  long long cx = (cap + 255) / 256;
+  cx = cx < 2 * per_image ? cx : 2 * per_image;
+  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
+  return um::check_launch("um_disparity_to_image_ragged");
 }
 
 int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,

@@ -25,10 +25,16 @@ does; `DepthSequenceRunner` streams host (uint8 frame, pose) items through the s
 `depth_to_image` is the reference's `viz_depth_tensor(1. / depth)` (inverse depth scaled by its exact 95th percentile,
 matplotlib's `plasma` map, evaluate_depth.py:403-417) on the device.  Writing files (PNG) stays out of scope.
 
-Stereo (`inference_stereo`, evaluate_stereo.py:711-843): `StereoRunner` streams host uint8 (left, right) pairs, normalised and
-resized on the device, through the same path as `infer_stereo`, replayed as a CUDA graph; `disparity_to_image` is the
-reference's `vis_disparity` (min-max scaling, cv2's INFERNO map) on the device.  Writing files (PNG, PFM) stays out of scope.
+Stereo (`inference_stereo`, evaluate_stereo.py:711-843): `StereoRunner` streams host uint8 (left, right) pairs of one frame
+size, normalised and resized on the device, through the same path as `infer_stereo`, replayed as a CUDA graph;
+`MixedSizeStereoRunner` does the same for pairs of any size, as the reference takes each file at its own size: pairs are
+batched by the size the model sees, and the input conversion, the resize back and the colouring read each pair's own size
+from a device descriptor table (the `*_ragged` kernels), so one CUDA graph per inference size serves every pair that maps
+to it.  `disparity_to_image` is the reference's `vis_disparity` (min-max scaling, cv2's INFERNO map) on the device.
+Writing files (PNG, PFM) stays out of scope.
 """
+import collections
+import itertools
 import math
 
 import numpy as np
@@ -71,6 +77,26 @@ def _inference_size(ori, padding_factor, inference_size):
     if inference_size is None:
         return (int(math.ceil(ori[0] / padding_factor)) * padding_factor, int(math.ceil(ori[1] / padding_factor)) * padding_factor)
     return (int(inference_size[0]), int(inference_size[1]))
+
+
+def _batches(samples, batch, shape_of, max_open=None):
+    """Lists of samples of equal `shape_of(sample)`, at most `batch` long: one open batch per shape, flushed when full and,
+    at the end, in the order the shapes were first opened.  With `max_open`, opening a batch that makes more than
+    `max_open` open flushes the oldest open batch first, so at most `max_open` partial batches are held."""
+    if batch < 1:
+        raise ValueError("batch must be positive")
+    if max_open is not None and max_open < 1:
+        raise ValueError("max_open must be positive")
+    open_batches = {}
+    for s in samples:
+        key = shape_of(s)
+        if key not in open_batches and max_open is not None and len(open_batches) >= max_open:
+            yield open_batches.pop(next(iter(open_batches)))
+        open_batches.setdefault(key, []).append(s)
+        if len(open_batches[key]) == batch:
+            yield open_batches.pop(key)
+    for key in list(open_batches):
+        yield open_batches.pop(key)
 
 
 def _resize(x, size, scale=None, flip=False):
@@ -212,18 +238,24 @@ def infer_stereo(model, left, right, *, padding_factor=16, inference_size=None, 
     return _stereo_outputs(model, left, right, ori, size, pred_bidir_disp, pred_right_disp, model_kwargs)
 
 
-def _stereo_outputs(model, left, right, ori, size, pred_bidir_disp, pred_right_disp, model_kwargs):
-    """Normalised pairs at the inference size -> the stereo driver's outputs at the original size: the hflip batching, the
-    forward, and the resize back with the width rescale and the flip back (evaluate_stereo.py:789-836)."""
-    resized = size != ori
-    b = left.shape[0]
+def _stereo_forward(model, left, right, pred_bidir_disp, pred_right_disp, model_kwargs):
+    """Normalised pairs at the inference size -> the model's disparities [B or 2B, 1, H, W] at that size: the hflip batching
+    of the right view (evaluate_stereo.py:789-796) and the forward."""
     if pred_bidir_disp:
         left, right = torch.cat((left, _hflip(right)), dim=0), torch.cat((right, _hflip(left)), dim=0)
     elif pred_right_disp:
         left, right = _hflip(right), _hflip(left)
     model_kwargs["task"] = "stereo"
     disp = model(left.float().contiguous(), right.float().contiguous(), **model_kwargs)["flow_preds"][-1]     # [B or 2B, H, W]
-    disp = disp.unsqueeze(1)
+    return disp.unsqueeze(1)
+
+
+def _stereo_outputs(model, left, right, ori, size, pred_bidir_disp, pred_right_disp, model_kwargs):
+    """Normalised pairs at the inference size -> the stereo driver's outputs at the original size: the hflip batching, the
+    forward, and the resize back with the width rescale and the flip back (evaluate_stereo.py:789-836)."""
+    resized = size != ori
+    b = left.shape[0]
+    disp = _stereo_forward(model, left, right, pred_bidir_disp, pred_right_disp, model_kwargs)
     sc = [ori[1] / float(size[1])] if resized else None
     if pred_bidir_disp:
         main = _resize(disp[:b], ori, sc) if resized else disp[:b]
@@ -391,7 +423,9 @@ class _PipelinedRunner:
     Subclasses provide `_stage_host(slot, chunk)` (fill the slot's pinned buffers and enqueue their H2D copies on the current
     stream, which is the copy stream), `_reset_inputs(slot)` and `_step(slot)` (the fixed-shape device work).  When `_step`
     returns a dict of device tensors whose first axis is the batch, the default `_download(slot, out)` (enqueue the D2H
-    copies of a step's outputs into pinned buffers) and `_results(slot, n)` (one dict of host tensors per item) apply."""
+    copies of a step's outputs into pinned buffers) and `_results(slot, n)` (one dict of host tensors per item) apply.
+    Runners whose steps are not all one shape override `_chunks` (how items form steps), `_prepare_graphs` and
+    `_device_step` (which graph replays a step)."""
 
     def _init_pipeline(self, device, use_graph):
         self.dev = torch.device(device)
@@ -401,6 +435,7 @@ class _PipelinedRunner:
         self.use_graph = use_graph
         self.out_pin = [None, None]
         self._held_buffers = []
+        self._staged = [None, None]                    # completion event of each slot's last H2D copies
 
     def _download(self, slot, out):
         if self.out_pin[slot] is None:
@@ -434,27 +469,47 @@ class _PipelinedRunner:
             torch.cuda.synchronize()
 
     def _stage(self, slot, chunk):
-        """host side of one batch, then the H2D copies on the side stream; returns their completion event"""
+        """host side of one batch, then the H2D copies on the side stream; returns their completion event.  The slot's
+        pinned buffers are refilled only once their previous copies have been read out (the copy stream may still be
+        queued behind earlier device work)."""
+        if self._staged[slot] is not None:
+            self._staged[slot].synchronize()
         with torch.cuda.stream(self.copy_stream):
             self._stage_host(slot, chunk)
             ev = torch.cuda.Event()
             ev.record(self.copy_stream)
+        self._staged[slot] = ev
         return ev
 
-    def _pipeline(self, items, start=None):
-        """Yields the results of `items` taken `self.batch` at a time.  `start()` runs (eagerly, on the main stream) before
-        the first step, after the graphs exist."""
+    def _prepare_graphs(self):
+        """Before the first step: the one-shape runners capture both slots' graphs here."""
         if self.use_graph and self.graphs[0] is None:
             self._capture()
+
+    def _chunks(self, items):
+        """The steps' items: `self.batch` at a time, read as each step is staged."""
         it = iter(items)
+        while True:
+            chunk = list(itertools.islice(it, self.batch))
+            if not chunk:
+                return
+            yield chunk
+
+    def _device_step(self, slot, chunk):
+        """Enqueue the device work of the step staged in `slot`; returns its outputs."""
+        if self.use_graph:
+            self.graphs[slot].replay()
+            return self.static_out[slot]
+        return self._step(slot)
+
+    def _pipeline(self, items, start=None):
+        """Yields the results of `items` taken one chunk (`_chunks`) at a time.  `start()` runs (eagerly, on the main
+        stream) before the first step, after `_prepare_graphs`."""
+        self._prepare_graphs()
+        chunks = self._chunks(items)
 
         def next_chunk():
-            chunk = []
-            for p in it:
-                chunk.append(p)
-                if len(chunk) == self.batch:
-                    break
-            return chunk
+            return next(chunks, [])
 
         cur = next_chunk()
         if not cur:
@@ -468,11 +523,7 @@ class _PipelinedRunner:
         done_ev, done_n = None, 0
         while cur:
             main.wait_event(ready)
-            if self.use_graph:
-                self.graphs[slot].replay()
-                out = self.static_out[slot]
-            else:
-                out = self._step(slot)
+            out = self._device_step(slot, cur)
             fwd_done = torch.cuda.Event()
             fwd_done.record(main)
             nxt = next_chunk()
@@ -619,6 +670,238 @@ class StereoRunner(_PipelinedRunner):
     def run(self, pairs):
         with torch.cuda.device(self.dev):
             yield from self._pipeline(pairs)
+
+
+# um_ragged_item (include/unimatch_sm100.h) as a numpy record, for building descriptor tables on the host
+RAGGED_ITEM = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("scale", "<f4"), ("flags", "<i4")])
+assert RAGGED_ITEM.itemsize == ops.RAGGED_ITEM_BYTES
+
+
+def _ragged_step_layout(sizes, batch, size, pred_bidir_disp, pred_right_disp):
+    """Descriptor tables of one stereo step of `batch` pairs at the inference size `size`, whose real pairs have the
+    original sizes `sizes` (1 <= len <= batch).  Returns (frames, outputs, frame_bytes, out_pixels, results):
+    * frames: 2*batch items over the packed uint8 frames -- the real pairs' left frames back to back, then their right
+      frames; the items of a short step's filler pairs point at its last pair's frames, so fillers upload nothing;
+    * outputs: batch items ('disp'), or 2*batch with `pred_bidir_disp` ('disp', then 'disp_right'), packed back to back in
+      that order; each scaled by the width ratio rounded to fp32 when its size differs from `size` (1 otherwise, as
+      `_stereo_outputs` does), flipped for the right view; fillers are empty items, which the kernels skip;
+    * frame_bytes / out_pixels: the used prefixes of the packed buffers;
+    * results: per real pair, the (key, offset, h, w) of each of its outputs."""
+    n = len(sizes)
+    frames = np.zeros(2 * batch, RAGGED_ITEM)
+    off = 0
+    for side in range(2):
+        for i, (h, w) in enumerate(sizes):
+            frames[side * batch + i] = (off, h, w, 1.0, 0)
+            off += 3 * h * w
+        frames[side * batch + n:(side + 1) * batch] = frames[side * batch + n - 1]
+    keys = ("disp", "disp_right") if pred_bidir_disp else ("disp",)
+    outputs = np.zeros(len(keys) * batch, RAGGED_ITEM)
+    results = [[] for _ in sizes]
+    used = 0
+    for k, key in enumerate(keys):
+        flags = ops.RAGGED_FLIP_X if (pred_right_disp or key == "disp_right") else 0
+        for i, (h, w) in enumerate(sizes):
+            scale = np.float32(w / float(size[1])) if (h, w) != tuple(size) else np.float32(1.0)
+            outputs[k * batch + i] = (used, h, w, scale, flags)
+            results[i].append((key, used, h, w))
+            used += h * w
+    return frames, outputs, off, used, results
+
+
+class MixedSizeStereoRunner(_PipelinedRunner):
+    """Streaming stereo inference over host (left, right) uint8 pairs of ANY size up to `max_frame_size`:
+    `inference_stereo` (evaluate_stereo.py:711-843), which takes each pair at its own size, as a stream.
+
+    * buckets: a pair's bucket is the size the model sees, its size rounded up to a multiple of `padding_factor` or
+      `inference_size` (so with `inference_size` every pair shares one bucket); a step holds up to `batch` pairs of one
+      bucket, formed as the submission drivers form batches (`_batches`: one open step per bucket, sent when full; opening
+      more than `max_buckets` sends the oldest open step early; the open steps are sent at the end);
+    * upload: each slot has one pinned uint8 buffer of 2 * batch * H_max * W_max * 3 bytes and a small descriptor table
+      (`um_ragged_item`); a step packs its left frames, then its right frames, back to back and copies only the used bytes
+      and the table on a side stream while the previous step computes; a short step's fillers repeat its last pair
+      without uploading it again and their results are dropped;
+    * device work of a step, one CUDA graph per bucket and staging slot, captured when the bucket first appears (the least
+      recently used bucket's graphs and held buffers are dropped when `max_buckets` buckets hold graphs): the ragged
+      conversion (`um_frames_to_planar_normalized_ragged`: ImageNet normalisation and resize of every frame from its own
+      size to the bucket's), the hflip batching and forward of `infer_stereo`, the ragged resize back with the width
+      rescale and the flip back (`um_resize_bilinear_ragged`) and, with `visualize`, the ragged colouring
+      (`um_disparity_to_image_ragged`); the descriptors live in device memory, so a replay reads each step's geometry;
+    * download: only the used prefix of the packed disparities (and pictures).
+
+    Sizes, padding, `inference_size` and the bidirectional / right-view semantics are those of `infer_stereo` on each pair.
+    `run(pairs)` takes an iterable of (left, right) host uint8 frames [h, w, 3] (numpy arrays or tensors, RGB as PIL decodes
+    them; both of a pair the same size) and yields (index, result) as steps complete -- completion order, not input order,
+    so a rare bucket does not hold back later results; `index` is the pair's position in the input, each exactly once.
+    `result` holds CPU views 'disp' [h, w] (+ 'disp_right') and, with `visualize`, the uint8 BGR pictures 'vis' [h, w, 3]
+    (+ 'vis_right'); `return_disp=False` with `visualize` sends back only the pictures.  The views point into reused pinned
+    staging -- copy what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
+
+    def __init__(self, model, max_frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
+                 pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, max_buckets=4, **model_kwargs):
+        if pred_bidir_disp and pred_right_disp:
+            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
+        if not return_disp and not visualize:
+            raise ValueError("nothing to return: return_disp=False needs visualize=True")
+        self.kw = dict(model_kwargs)
+        if self.kw.pop("task", "stereo") != "stereo":
+            raise ValueError("MixedSizeStereoRunner drives the stereo task only")
+        self.model, self.batch, self.max_buckets = model, int(batch), int(max_buckets)
+        if self.batch < 1 or self.max_buckets < 1:
+            raise ValueError("MixedSizeStereoRunner: batch and max_buckets must be positive")
+        self.hmax, self.wmax = int(max_frame_size[0]), int(max_frame_size[1])
+        if self.hmax < 1 or self.wmax < 1 or self.hmax * self.wmax > 0x7fffffff:
+            raise ValueError("MixedSizeStereoRunner: max_frame_size must be positive, at most 2^31 - 1 pixels")
+        self.padding_factor, self.inference_size = padding_factor, inference_size
+        self.bidir, self.right = bool(pred_bidir_disp), bool(pred_right_disp)
+        self.visualize, self.return_disp = bool(visualize), bool(return_disp)
+        self._init_pipeline(device, use_graph)
+        cap = self.hmax * self.wmax
+        nout = (2 if self.bidir else 1) * self.batch
+        ndesc = 2 * self.batch + nout
+        self.pin = [torch.empty((2 * self.batch * cap * 3,), dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_in = [torch.empty((2 * self.batch * cap * 3,), dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.desc_pin = [torch.empty((ndesc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_desc = [torch.zeros((ndesc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.out_pin = [{} for _ in range(2)]
+        for pins in self.out_pin:
+            if self.return_disp:
+                pins["disp"] = torch.empty((nout * cap,)).pin_memory()
+            if self.visualize:
+                pins["vis"] = torch.empty((3 * nout * cap,), dtype=torch.uint8).pin_memory()
+        self.meta = [None, None]                 # host layout of the step staged in each slot
+        self.out_meta = [None, None]             # host layout of the step downloaded into each slot's pinned outputs
+        self.buckets = collections.OrderedDict()  # inference size -> (graphs, outputs, held buffers), least recent first
+        self.stats = {"steps": 0, "pairs": 0, "captures": 0, "h2d_bytes": 0, "d2h_bytes": 0}
+
+    # ---- host side
+    def _pair(self, pair):
+        left, right = (torch.as_tensor(f) for f in pair)
+        for f in (left, right):
+            if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+                raise ValueError("MixedSizeStereoRunner: frames must be uint8 [h, w, 3]")
+        if left.shape != right.shape:
+            raise ValueError("MixedSizeStereoRunner: the left and right frames of a pair must have the same size")
+        if not (1 <= left.shape[0] <= self.hmax and 1 <= left.shape[1] <= self.wmax):
+            raise ValueError("MixedSizeStereoRunner: a %dx%d frame exceeds max_frame_size %dx%d"
+                             % (left.shape[0], left.shape[1], self.hmax, self.wmax))
+        return left, right
+
+    def _bucket(self, pair):
+        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+
+    def _chunks(self, items):
+        checked = ((i, self._pair(p)) for i, p in items)
+        return _batches(checked, self.batch, lambda s: self._bucket(s[1]), self.max_buckets)
+
+    def _stage_host(self, slot, chunk):
+        """the step's packed frames and descriptor table into pinned memory, then their H2D copies (used bytes only)"""
+        pairs = [p for _, p in chunk]
+        size = self._bucket(pairs[0])
+        frames, outputs, nbytes, used, results = _ragged_step_layout([tuple(p[0].shape[:2]) for p in pairs], self.batch, size,
+                                                                     self.bidir, self.right)
+        off = 0
+        for f in [p[0] for p in pairs] + [p[1] for p in pairs]:
+            self.pin[slot][off:off + f.numel()].copy_(f.reshape(-1))
+            off += f.numel()
+        table = np.concatenate((frames, outputs)).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES)
+        self.desc_pin[slot].copy_(torch.from_numpy(table))
+        self.dev_in[slot][:nbytes].copy_(self.pin[slot][:nbytes], non_blocking=True)
+        self.dev_desc[slot].copy_(self.desc_pin[slot], non_blocking=True)
+        self.meta[slot] = {"size": size, "used": used, "results": [(i, r) for (i, _), r in zip(chunk, results)]}
+        self.stats["steps"] += 1
+        self.stats["pairs"] += len(chunk)
+        self.stats["h2d_bytes"] += nbytes + table.nbytes
+
+    def _download(self, slot, out):
+        meta = self.out_meta[slot] = self.meta[slot]
+        for k, v in out.items():
+            n = meta["used"] * (3 if k == "vis" else 1)
+            self.out_pin[slot][k][:n].copy_(v[:n], non_blocking=True)
+            self.stats["d2h_bytes"] += n * v.element_size()
+
+    def _results(self, slot, n):
+        pins = self.out_pin[slot]
+        for index, outs in self.out_meta[slot]["results"][:n]:
+            r = {}
+            for key, off, h, w in outs:
+                if self.return_disp:
+                    r[key] = pins["disp"][off:off + h * w].view(h, w)
+                if self.visualize:
+                    r[key.replace("disp", "vis")] = pins["vis"][3 * off:3 * (off + h * w)].view(h, w, 3)
+            yield index, r
+
+    # ---- device side
+    def _step(self, slot, size):
+        b, nf = self.batch, 2 * self.batch
+        items = self.dev_desc[slot]
+        planes = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:nf], self.hmax, self.wmax, int(size[0]),
+                                                         int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
+        disp = _stereo_forward(self.model, planes[:b], planes[b:], self.bidir, self.right, dict(self.kw))
+        out_items = items[nf:]
+        packed = _OPS.resize_bilinear_ragged(disp.contiguous(), out_items, self.hmax, self.wmax,
+                                             out_items.shape[0] * self.hmax * self.wmax)
+        out = {}
+        if self.return_disp:
+            out["disp"] = packed
+        if self.visualize:
+            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
+            _OPS.disparity_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
+        return out
+
+    def _reset_inputs(self, slot):
+        """zero frames and a full-capacity descriptor table: valid for any bucket"""
+        full = [(self.hmax, self.wmax)] * self.batch
+        frames, outputs, _, _, _ = _ragged_step_layout(full, self.batch, (self.hmax, self.wmax), self.bidir, self.right)
+        table = np.concatenate((frames, outputs)).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES)
+        self.dev_in[slot].zero_()
+        self.dev_desc[slot].copy_(torch.from_numpy(table))
+
+    def _prepare_graphs(self):
+        pass                                       # graphs are captured per bucket, when it first appears
+
+    def _capture_bucket(self, slot, size):
+        """Both slots' graphs of bucket `size`, while `slot` holds a staged step of that bucket (its inputs are used as they
+        are for the eager warm-up) and the other slot is free (reset to valid descriptors)."""
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            self._reset_inputs(slot ^ 1)
+            for _ in range(2):                     # eager warm-up: builds the module's cached operand planes for this shape
+                for s in range(2):
+                    self._step(s, size)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        graphs, outs = [], []
+        for s in range(2):
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                outs.append(self._step(s, size))
+            graphs.append(g)
+        held = self.model.cached_buffers()         # see _PipelinedRunner._capture
+        torch.cuda.synchronize()
+        self.stats["captures"] += 1
+        return graphs, outs, held
+
+    def _device_step(self, slot, chunk):
+        size = self.meta[slot]["size"]
+        if not self.use_graph:
+            return self._step(slot, size)
+        entry = self.buckets.get(size)
+        if entry is None:
+            if len(self.buckets) >= self.max_buckets:
+                torch.cuda.synchronize()           # the evicted graphs' last outputs may still be on their way to the host
+                self.buckets.popitem(last=False)
+            entry = self.buckets[size] = self._capture_bucket(slot, size)
+        self.buckets.move_to_end(size)
+        graphs, outs, _ = entry
+        graphs[slot].replay()
+        return outs[slot]
+
+    @torch.no_grad()
+    def run(self, pairs):
+        with torch.cuda.device(self.dev):
+            yield from self._pipeline(enumerate(pairs))
 
 
 class _SequenceRunner(_PipelinedRunner):

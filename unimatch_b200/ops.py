@@ -64,6 +64,16 @@ class ConvDesc(ctypes.Structure):
                 ("pre", ctypes.c_void_p), ("ld_pre", ctypes.c_int64)]
 
 
+class RaggedItem(ctypes.Structure):
+    """um_ragged_item: one image of a ragged batch (offset in elements of the packed buffer, size, resize scale, flags)"""
+    _fields_ = [("offset", ctypes.c_int64), ("h", ctypes.c_int32), ("w", ctypes.c_int32), ("scale", ctypes.c_float),
+                ("flags", ctypes.c_int32)]
+
+
+RAGGED_FLIP_X = 1
+RAGGED_ITEM_BYTES = ctypes.sizeof(RaggedItem)      # 24
+
+
 class FfnDesc(ctypes.Structure):
     _fields_ = [("src", ctypes.c_void_p * 2), ("src_plane_stride", ctypes.c_int64), ("rows", ctypes.c_int64),
                 ("w1", ctypes.c_void_p), ("w2", ctypes.c_void_p), ("hidden", ctypes.c_int32),
@@ -99,6 +109,9 @@ _SIGNATURES = {
     "um_resize_bilinear": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _FP, _I, _P]),
     "um_frames_to_planar": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
+    "um_frames_to_planar_normalized_ragged": (_RC, [_P, _L, _P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
+    "um_resize_bilinear_ragged": (_RC, [_P, _P, _L, _P, _I, _I, _I, _I, _I, _P]),
+    "um_disparity_to_image_ragged": (_RC, [_P, _L, _P, _P, _P, _I, _I, _I, _P]),
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_depth_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
@@ -460,6 +473,69 @@ def _disparity_to_image(disp, out):
 
 
 disparity_to_image = _define("disparity_to_image(Tensor disp, Tensor(a!) out) -> ()", _disparity_to_image)
+
+
+# ---- ragged batches (include/unimatch_sm100.h, um_ragged_item) ---------------------------------------------------------
+def _ragged_items(items, name):
+    """items: the DEVICE descriptor table, uint8 [n, 24] (n um_ragged_item structs); returns n"""
+    if not items.is_cuda or items.dtype != torch.uint8 or items.dim() != 2 or items.shape[1] != RAGGED_ITEM_BYTES \
+            or not items.is_contiguous() or not 1 <= items.shape[0] <= 65535:
+        raise RuntimeError("%s: items must be a contiguous CUDA uint8 table [1..65535, %d]" % (name, RAGGED_ITEM_BYTES))
+    return items.shape[0]
+
+
+def _frames_to_planar_normalized_ragged(frames, items, h_max, w_max, h_out, w_out, mean, std):
+    """frames: contiguous CUDA uint8, the packed frames (frame i [h_i, w_i, 3] at byte items[i].offset) -> fp32 [n, 3, h_out,
+    w_out]; mean / std as for frames_to_planar_normalized"""
+    if not frames.is_cuda or frames.dtype != torch.uint8 or not frames.is_contiguous() or frames.numel() == 0:
+        raise RuntimeError("frames_to_planar_normalized_ragged: expected contiguous CUDA uint8 packed frames")
+    if len(mean) != 3 or len(std) != 3:
+        raise RuntimeError("frames_to_planar_normalized_ragged: expected 3 means and 3 stds")
+    n = _ragged_items(items, "frames_to_planar_normalized_ragged")
+    out = torch.empty((n, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
+    m, s = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
+    _check(LIB.um_frames_to_planar_normalized_ragged(_p(frames), frames.numel(), _p(items), _p(out), n, h_max, w_max, h_out,
+                                                     w_out, m, s, _stream()), "um_frames_to_planar_normalized_ragged")
+    return out
+
+
+frames_to_planar_normalized_ragged = _define(
+    "frames_to_planar_normalized_ragged(Tensor frames, Tensor items, int h_max, int w_max, int h_out, int w_out, float[] mean, "
+    "float[] std) -> Tensor", _frames_to_planar_normalized_ragged)
+
+
+def _resize_bilinear_ragged(x, items, h_max, w_max, out_numel):
+    """x: contiguous fp32 [n, 1, h, w] -> fp32 [out_numel], item i at items[i].offset (the rest left unwritten)"""
+    _f32c(x, "x")
+    if x.dim() != 4 or x.shape[1] != 1:
+        raise RuntimeError("resize_bilinear_ragged: expected planar [n, 1, H, W]")
+    n = _ragged_items(items, "resize_bilinear_ragged")
+    if x.shape[0] != n or out_numel < 1:
+        raise RuntimeError("resize_bilinear_ragged: one item per image and a positive output size")
+    out = torch.empty((out_numel,), device=x.device, dtype=torch.float32)
+    _check(LIB.um_resize_bilinear_ragged(_p(x), _p(out), out_numel, _p(items), n, x.shape[2], x.shape[3], h_max, w_max,
+                                         _stream()), "um_resize_bilinear_ragged")
+    return out
+
+
+resize_bilinear_ragged = _define("resize_bilinear_ragged(Tensor x, Tensor items, int h_max, int w_max, int out_numel) -> Tensor",
+                                 _resize_bilinear_ragged)
+
+
+def _disparity_to_image_ragged(disp, items, out, h_max, w_max):
+    """disp: contiguous fp32 packed disparities (item i at items[i].offset); out: contiguous uint8 of at least 3 disp.numel()
+    bytes, picture i at 3 items[i].offset"""
+    _f32c(disp, "disp")
+    if out.dtype != torch.uint8 or not out.is_contiguous() or out.device != disp.device or out.numel() < 3 * disp.numel():
+        raise RuntimeError("disparity_to_image_ragged: out must be contiguous uint8 of 3 bytes per disparity on its device")
+    n = _ragged_items(items, "disparity_to_image_ragged")
+    scratch = torch.empty((2 * n,), device=disp.device, dtype=torch.float32)
+    _check(LIB.um_disparity_to_image_ragged(_p(disp), disp.numel(), _p(items), _p(out), _p(scratch), n, h_max, w_max, _stream()),
+           "um_disparity_to_image_ragged")
+
+
+disparity_to_image_ragged = _define("disparity_to_image_ragged(Tensor disp, Tensor items, Tensor(a!) out, int h_max, int w_max) -> ()",
+                                    _disparity_to_image_ragged)
 
 DEPTH_TO_IMAGE_SCRATCH_WORDS = 2056      # per image, include/unimatch_sm100.h (um_depth_to_image)
 

@@ -27,7 +27,7 @@ import torch
 
 from . import ops
 from .evaluation import _upload
-from .inference import InputPadder, _resize, disparity_to_image, flow_to_image
+from .inference import InputPadder, _batches, _resize, disparity_to_image, flow_to_image
 
 _OPS = torch.ops.unimatch_sm100
 
@@ -72,22 +72,7 @@ def pfm_header(h, w):
     return b"Pf\n" + b"%d %d\n" % (w, h) + b"%f\n" % -1
 
 
-# ---- batching and the writer pool ------------------------------------------------------------------------------------------
-def _batches(samples, batch, shape_of):
-    """Lists of samples of equal `shape_of(sample)`, at most `batch` long: one open batch per shape, flushed when full and,
-    at the end, in the order the shapes were first opened."""
-    if batch < 1:
-        raise ValueError("batch must be positive")
-    open_batches = {}
-    for s in samples:
-        key = shape_of(s)
-        open_batches.setdefault(key, []).append(s)
-        if len(open_batches[key]) == batch:
-            yield open_batches.pop(key)
-    for key in list(open_batches):
-        yield open_batches.pop(key)
-
-
+# ---- the writer pool (samples are batched by `inference._batches`) -----------------------------------------------------------
 class _WriterPool:
     """Two pinned staging slots and a pool of writer threads.  `stage` waits for the writers of the batch that last used the
     slot (re-raising their errors), copies device tensors into the slot and records an event; jobs wait on that event."""
