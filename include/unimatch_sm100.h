@@ -199,7 +199,8 @@ int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n,
  * Per-image geometry of the *_ragged entries, a DEVICE array of n items (read by the kernels, so a CUDA graph replay picks
  * up whatever the table holds at that time).  offset: where image i starts in the packed buffer, in elements of that
  * buffer (bytes for uint8 frames [h, w, 3]; floats for disparities [h, w], whose BGR pictures start at 3 * offset bytes);
- * (h, w): its size; scale and flags: used by um_resize_bilinear_ragged only.  An item with h or w outside 1..capacity, or
+ * (h, w): its size as stored; scale: used by um_resize_bilinear_ragged only; flags: UM_RAGGED_*, each entry names the ones
+ * it reads and ignores the others.  An item with h or w outside 1..capacity, or
  * that does not fit in the packed buffer (numel / bytes arguments), is skipped: nothing of it is read or written.  Each
  * entry validates its scalar arguments before any CUDA call, launches a grid sized by the capacity (h_max, w_max) or the
  * uniform side, and never synchronises: graph-capturable.  n <= 65535. */
@@ -210,6 +211,10 @@ typedef struct um_ragged_item {
   int32_t flags;
 } um_ragged_item;
 #define UM_RAGGED_FLIP_X 1   /* um_resize_bilinear_ragged: mirror the item's output horizontally */
+/* A portrait item of the flow drivers, which run the model on the transposed (landscape) image (evaluate_flow.py:713-717,
+ * :757-758).  um_frames_to_planar_ragged: the frame [h, w, 3] is read as its transpose [w, h, 3].
+ * um_resize_bilinear_ragged: the item stored as [h, w] is the transpose of the (w, h) resize of the source. */
+#define UM_RAGGED_TRANSPOSE 2
 
 /* um_frames_to_planar_normalized per frame: frame i = DEVICE uint8 [h_i, w_i, 3] at frames + items[i].offset (frames_bytes
  * = size of the packed buffer) -> out fp32 planar [n, 3, h_out, w_out].  Image i is bit-identical to
@@ -219,11 +224,23 @@ int um_frames_to_planar_normalized_ragged(const uint8_t* frames, int64_t frames_
                                           int32_t n, int32_t h_max, int32_t w_max, int32_t h_out, int32_t w_out,
                                           const float* mean, const float* std, void* stream);
 
+/* um_frames_to_planar per frame: frame i = DEVICE uint8 [h_i, w_i, 3] at frames + items[i].offset (frames_bytes = size of the
+ * packed buffer) -> out fp32 planar [n, 3, h_out, w_out] in [0, 255].  Image i is bit-identical to um_frames_to_planar of
+ * frame i alone with transpose = (items[i].flags & UM_RAGGED_TRANSPOSE) (the same device code).  Replaces the host-side
+ * conversion, transpose and F.interpolate of inference_flow (evaluate_flow.py:710-733) for pairs of different sizes. */
+int um_frames_to_planar_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out, int32_t n,
+                               int32_t h_max, int32_t w_max, int32_t h_out, int32_t w_out, void* stream);
+
 /* um_resize_bilinear per item: in = uniform planar [n, 1, h_in, w_in] fp32 -> item i at out + items[i].offset (out_numel
  * floats in all), size (h_i, w_i), multiplied by items[i].scale unless it is 1.0f, mirrored with UM_RAGGED_FLIP_X.  Item i is
  * bit-identical to um_resize_bilinear of image i alone with scale = &items[i].scale; an item at (h_in, w_in) without the flip
  * is copied as it is (what the stereo driver does with a disparity it does not resize, evaluate_stereo.py:813-836).
- * Replaces the resize back, disparity rescale and flip back of inference_stereo for pairs of different sizes. */
+ * With UM_RAGGED_TRANSPOSE the item [h_i, w_i] is the transpose of um_resize_bilinear of image i to (w_i, h_i) (mirrored
+ * before the transpose when both flags are set), and it is copied, transposed, when (w_i, h_i) = (h_in, w_in).
+ * A flow batch [B, 2, H, W] is 2B images: pair i's u plane with scale = (float)(ori_w / size_w) and its v plane with
+ * (float)(ori_h / size_h), packed back to back, give the planar flow [2, h_i, w_i] of evaluate_flow.py:750-758.
+ * Replaces the resize back, disparity rescale and flip back of inference_stereo, and the resize back, flow rescale and
+ * transpose back of inference_flow, for pairs of different sizes. */
 int um_resize_bilinear_ragged(const float* in, float* out, int64_t out_numel, const um_ragged_item* items, int32_t n,
                               int32_t h_in, int32_t w_in, int32_t h_max, int32_t w_max, void* stream);
 
@@ -233,6 +250,24 @@ int um_resize_bilinear_ragged(const float* in, float* out, int64_t out_numel, co
  * Replaces vis_disparity on each predicted disparity of inference_stereo (evaluate_stereo.py:820-841). */
 int um_disparity_to_image_ragged(const float* disp, int64_t numel, const um_ragged_item* items, uint8_t* out,
                                  float* minmax_scratch, int32_t n, int32_t h_max, int32_t w_max, void* stream);
+
+/* um_flow_to_image per item: flow i = fp32 planar [2, h_i, w_i] at flow + flow_items[i].offset (offset in floats, flow_numel
+ * floats in all) -> its RGB picture at out + picture_items[i].offset (offset in BYTES, out_bytes in all), rows of 3 w_i
+ * bytes.  Picture i is bit-identical to um_flow_to_image of flow i alone (unknown-flow / NaN / all-zero rule included).
+ * An item is skipped unless both of its descriptors fit and have the same (h, w).  max_scratch: DEVICE buffer of n words,
+ * reset inside the call.  Replaces flow_to_image on each predicted flow of inference_flow (evaluate_flow.py:771, :784). */
+int um_flow_to_image_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, uint8_t* out,
+                            int64_t out_bytes, const um_ragged_item* picture_items, float* max_scratch, int32_t n,
+                            int32_t h_max, int32_t w_max, void* stream);
+
+/* um_fb_consistency per pair: flow_items and occ_items hold 2n items each, pair i's forward flow [2, h_i, w_i] (mask
+ * [h_i, w_i]) at index i and its backward one at index n + i; offsets in floats into flow (flow_numel floats in all) and
+ * occ (occ_numel).  The masks of pair i are bit-identical to um_fb_consistency of pair i alone.  A pair is skipped unless
+ * its four items fit and have one size of at least 2 x 2 (what um_fb_consistency accepts).  Replaces
+ * forward_backward_consistency_check on each pair of inference_flow, at its original size (evaluate_flow.py:789-792). */
+int um_fb_consistency_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, float alpha, float beta,
+                             float* occ, int64_t occ_numel, const um_ragged_item* occ_items, int32_t n, int32_t h_max,
+                             int32_t w_max, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -27,6 +27,7 @@ _LAZY = {
     "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
     "StereoRunner": (".inference", "StereoRunner"),
     "MixedSizeStereoRunner": (".inference", "MixedSizeStereoRunner"),
+    "MixedSizeFlowRunner": (".inference", "MixedSizeFlowRunner"),
     "disparity_to_image": (".inference", "disparity_to_image"),
     "depth_to_image": (".inference", "depth_to_image"),
     "validate_flow": (".evaluation", "validate_flow"),
@@ -38,7 +39,8 @@ _LAZY = {
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "MixedSizeStereoRunner", "disparity_to_image", "depth_to_image",
+           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "MixedSizeStereoRunner", "MixedSizeFlowRunner",
+           "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission"]
 
 

@@ -114,4 +114,12 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+// Per-image geometry of the ragged entries (um_ragged_item, read from device memory): an item is used only if it lies
+// inside the capacity and inside the packed buffer; otherwise its threads read and write nothing.
+__device__ __forceinline__ bool ragged_ok(const um_ragged_item& it, int h_max, int w_max, long long elems_per_pixel,
+                                          long long numel) {
+  return it.h > 0 && it.w > 0 && it.h <= h_max && it.w <= w_max && it.offset >= 0 &&
+         it.offset + elems_per_pixel * it.h * it.w <= numel;
+}
+
 }  // namespace um

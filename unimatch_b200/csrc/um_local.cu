@@ -342,17 +342,76 @@ __device__ __forceinline__ float2 sample_flow(const float* f, long long plane, i
   return r;
 }
 
-__global__ void __launch_bounds__(256) fb_consistency_kernel(const float* __restrict__ fwd, const float* __restrict__ bwd,
-                                                             float alpha, float beta, float* __restrict__ fwd_occ,
-                                                             float* __restrict__ bwd_occ, int h, int w, long long npix) {
-  const long long pix = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (pix >= npix) return;
+// Where one pixel's flow pair and occlusion outputs lie: a uniform batch (FbUniform, grid x over all pixels of the batch),
+// or pair n's flows [2, h, w] and masks [h, w] at their own offsets in packed buffers (FbRagged, grid x over the
+// capacity's pixels, grid y the pair).
+struct FbPixel {
+  const float* fb;
+  const float* bb;
+  float* fwd_occ;
+  float* bwd_occ;
+  int h, w, rem;
+};
+
+struct FbUniform {
+  const float* fwd;
+  const float* bwd;
+  float* fwd_occ;
+  float* bwd_occ;
+  int h, w;
+  long long npix;
+  __device__ __forceinline__ bool pixel(FbPixel& p) const {
+    const long long pix = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (pix >= npix) return false;
+    const long long plane = (long long)h * w;
+    const int b = (int)(pix / plane);
+    p.rem = (int)(pix - (long long)b * plane);
+    p.fb = fwd + (long long)b * 2 * plane;
+    p.bb = bwd + (long long)b * 2 * plane;
+    p.fwd_occ = fwd_occ + (long long)b * plane;
+    p.bwd_occ = bwd_occ + (long long)b * plane;
+    p.h = h; p.w = w;
+    return true;
+  }
+};
+
+// flow_items / occ_items: 2n items each, pair i's forward flow (mask) at [i] and its backward one at [n + i].  A pair is
+// used only if its four items have one size of at least 2 x 2 (the sampling grid divides by size - 1) and fit.
+struct FbRagged {
+  const float* flow;
+  float* occ;
+  const um_ragged_item* flow_items;
+  const um_ragged_item* occ_items;
+  int n, h_max, w_max;
+  long long flow_numel, occ_numel;
+  __device__ __forceinline__ bool pixel(FbPixel& p) const {
+    const int i = blockIdx.y;
+    const um_ragged_item f = flow_items[i], b = flow_items[n + i], of = occ_items[i], ob = occ_items[n + i];
+    const long long q = (long long)blockIdx.x * 256 + threadIdx.x;
+    const bool same = b.h == f.h && b.w == f.w && of.h == f.h && of.w == f.w && ob.h == f.h && ob.w == f.w;
+    if (!same || f.h < 2 || f.w < 2 || !um::ragged_ok(f, h_max, w_max, 2, flow_numel) ||
+        !um::ragged_ok(b, h_max, w_max, 2, flow_numel) || !um::ragged_ok(of, h_max, w_max, 1, occ_numel) ||
+        !um::ragged_ok(ob, h_max, w_max, 1, occ_numel) || q >= (long long)f.h * f.w)
+      return false;
+    p.rem = (int)q;
+    p.fb = flow + f.offset;
+    p.bb = flow + b.offset;
+    p.fwd_occ = occ + of.offset;
+    p.bwd_occ = occ + ob.offset;
+    p.h = f.h; p.w = f.w;
+    return true;
+  }
+};
+
+template <class Geo>
+__global__ void __launch_bounds__(256) fb_consistency_kernel(Geo geo, float alpha, float beta) {
+  FbPixel p;
+  if (!geo.pixel(p)) return;
+  const int h = p.h, w = p.w, rem = p.rem;
   const long long plane = (long long)h * w;
-  const int b = (int)(pix / plane);
-  const int rem = (int)(pix - (long long)b * plane);
   const int y = rem / w, x = rem - y * w;
-  const float* fb = fwd + (long long)b * 2 * plane;
-  const float* bb = bwd + (long long)b * 2 * plane;
+  const float* fb = p.fb;
+  const float* bb = p.bb;
   const float fu = __ldg(fb + rem), fv = __ldg(fb + plane + rem);
   const float bu = __ldg(bb + rem), bv = __ldg(bb + plane + rem);
   const float mag = sqrtf(fu * fu + fv * fv) + sqrtf(bu * bu + bv * bv);
@@ -360,8 +419,8 @@ __global__ void __launch_bounds__(256) fb_consistency_kernel(const float* __rest
   const float2 wf = sample_flow(fb, plane, h, w, (float)x + bu, (float)y + bv);   // flow_warp(fwd, bwd)
   const float dfx = fu + wb.x, dfy = fv + wb.y, dbx = bu + wf.x, dby = bv + wf.y;
   const float thr = alpha * mag + beta;
-  fwd_occ[pix] = sqrtf(dfx * dfx + dfy * dfy) > thr ? 1.0f : 0.0f;
-  bwd_occ[pix] = sqrtf(dbx * dbx + dby * dby) > thr ? 1.0f : 0.0f;
+  p.fwd_occ[rem] = sqrtf(dfx * dfx + dfy * dfy) > thr ? 1.0f : 0.0f;
+  p.bwd_occ[rem] = sqrtf(dbx * dbx + dby * dby) > thr ? 1.0f : 0.0f;
 }
 
 }  // namespace
@@ -381,9 +440,22 @@ int um_fb_consistency(const float* fwd_flow, const float* bwd_flow, float alpha,
                       float* bwd_occ, int32_t batch, int32_t h, int32_t w, void* stream) {
   UM_REQUIRE(fwd_flow && bwd_flow && fwd_occ && bwd_occ && batch > 0 && h > 1 && w > 1, "um_fb_consistency: bad arguments");
   const long long npix = (long long)batch * h * w;
-  fb_consistency_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream>>>(fwd_flow, bwd_flow, alpha, beta,
-                                                                                      fwd_occ, bwd_occ, h, w, npix);
+  const FbUniform geo{fwd_flow, bwd_flow, fwd_occ, bwd_occ, h, w, npix};
+  fb_consistency_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, alpha, beta);
   return um::check_launch("um_fb_consistency");
+}
+
+int um_fb_consistency_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, float alpha, float beta,
+                             float* occ, int64_t occ_numel, const um_ragged_item* occ_items, int32_t n, int32_t h_max,
+                             int32_t w_max, void* stream) {
+  UM_REQUIRE(flow && flow_items && occ && occ_items && n > 0 && n <= 65535 && h_max > 1 && w_max > 1 && flow_numel > 0 &&
+                 occ_numel > 0,
+             "um_fb_consistency_ragged: bad arguments (1-65535 pairs, capacity of at least 2 x 2, non-null buffers)");
+  UM_REQUIRE((long long)h_max * w_max <= 0x7fffffffLL, "um_fb_consistency_ragged: an image has at most 2^31 - 1 pixels");
+  const long long cap = (long long)h_max * w_max;
+  const FbRagged geo{flow, occ, flow_items, occ_items, n, h_max, w_max, flow_numel, occ_numel};
+  fb_consistency_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(geo, alpha, beta);
+  return um::check_launch("um_fb_consistency_ragged");
 }
 
 int um_local_corr_softmax(const float* f0, const float* f1, float* flow, int32_t batch, int32_t h, int32_t w,

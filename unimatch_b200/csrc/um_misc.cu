@@ -108,21 +108,16 @@ __device__ __forceinline__ float bilinear_align_corners(const Load& load, int hi
   return __fmaf_rn(hy, row0, __fmul_rn(ly, row1));
 }
 
-// ---- per-image geometry of the ragged entries (um_ragged_item, read from device memory) ----------------------------------
-// An item is used only if it lies inside the capacity and inside the packed buffer; otherwise its thread writes nothing.
-__device__ __forceinline__ bool ragged_ok(const um_ragged_item& it, int h_max, int w_max, long long pixels_per_elem,
-                                          long long numel) {
-  return it.h > 0 && it.w > 0 && it.h <= h_max && it.w <= w_max && it.offset >= 0 &&
-         it.offset + pixels_per_elem * it.h * it.w <= numel;
-}
+using um::ragged_ok;
 
-// One output sample of a planar resize: source plane (hi, wi), destination plane (ho, wo), scale and flip.
+// One output sample of a planar resize: source plane (hi, wi), destination plane (ho, wo), scale and flip; `transpose`:
+// the destination plane is stored transposed, as [wo, ho].
 struct ResizeSample {
   const float* src;
   float* dst;
   int ho, wo, Y, X;
   float sc;
-  int flip_x, copy;
+  int flip_x, copy, transpose;
 };
 
 // Uniform batch [B, C, ho, wo]: one thread per output sample, channel c scaled by s_c.
@@ -146,6 +141,7 @@ struct ResizeUniform {
     s.sc = c == 0 ? s0 : (c == 1 ? s1 : s2);
     s.flip_x = flip_x;
     s.copy = 0;
+    s.transpose = 0;
     return true;
   }
 };
@@ -153,6 +149,8 @@ struct ResizeUniform {
 // Uniform single-channel batch [n, 1, hi, wi] -> item i at out + offset[i] at its own (h, w), scale and flip (grid y: item,
 // grid x: the capacity's pixels).  An item at the input size without a flip is copied as it is, as the stereo driver
 // leaves a disparity that needs no resize (the bilinear pass would turn a non-finite neighbour into NaN there).
+// UM_RAGGED_TRANSPOSE: the item's (h, w) is its size as stored; it is the transpose of the (w, h) resize of the source, so
+// the "at the input size" rule compares the swapped size.  Consecutive threads write consecutive stored samples.
 struct ResizeRagged {
   const float* in;
   float* out;
@@ -164,14 +162,17 @@ struct ResizeRagged {
     const um_ragged_item it = items[n];
     const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (!ragged_ok(it, h_max, w_max, 1, out_numel) || q >= (long long)it.h * it.w) return false;
-    s.X = (int)(q % it.w);
-    s.Y = (int)(q / it.w);
+    s.transpose = (it.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0;
+    const int xs = (int)(q % it.w), ys = (int)(q / it.w);      // the sample as stored
+    s.X = s.transpose ? ys : xs;
+    s.Y = s.transpose ? xs : ys;
     s.src = in + (long long)n * hi * wi;
     s.dst = out + it.offset;
-    s.ho = it.h; s.wo = it.w;
+    s.ho = s.transpose ? it.w : it.h;
+    s.wo = s.transpose ? it.h : it.w;
     s.sc = it.scale;
     s.flip_x = it.flags & UM_RAGGED_FLIP_X;
-    s.copy = !s.flip_x && it.h == hi && it.w == wi;
+    s.copy = !s.flip_x && s.ho == hi && s.wo == wi;
     return true;
   }
 };
@@ -187,42 +188,15 @@ __global__ void __launch_bounds__(256) resize_bilinear_kernel(Geo geo, int hi, i
                          : bilinear_align_corners([&](int y, int x) { return __ldg(base + (long long)y * wi + x); }, hi, wi,
                                                   s.ho, s.wo, s.Y, s.X);
   const int Xo = s.flip_x ? s.wo - 1 - s.X : s.X;
-  s.dst[(long long)s.Y * s.wo + Xo] = s.sc == 1.0f ? v : v * s.sc;
+  s.dst[s.transpose ? (long long)Xo * s.ho + s.Y : (long long)s.Y * s.wo + Xo] = s.sc == 1.0f ? v : v * s.sc;
 }
 
-// ---- video frames -> model input: uint8 [T,H,W,3] channel-last -> fp32 planar [T,3,ho,wo] -------------------------------
-// = resize_bilinear(frames.permute(0,3,1,2).float()), with the portrait transpose of evaluate_flow.py:713-717 (the source
-// is read as [3, W, H]) folded into the load.  One thread per output pixel, three planes written.
-__global__ void __launch_bounds__(256) frames_to_planar_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out,
-                                                               int H, int W, int transpose, int ho, int wo, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int X = (int)(i % wo);
-  const int Y = (int)((i / wo) % ho);
-  const long long t = i / ((long long)ho * wo);
-  const int hs = transpose ? W : H, ws = transpose ? H : W;     // source size as the resize sees it
-  const uint8_t* base = frames + t * (long long)H * W * 3;
-  const long long plane = (long long)ho * wo;
-  float* o = out + t * 3 * plane + (long long)Y * wo + X;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const auto load = [&](int y, int x) {
-      const long long pix = transpose ? (long long)x * W + y : (long long)y * W + x;
-      return (float)__ldg(base + pix * 3 + c);
-    };
-    o[c * plane] = bilinear_align_corners(load, hs, ws, ho, wo, Y, X);
-  }
-}
-
-// ---- depth frames -> model input: uint8 [T,H,W,3] -> ImageNet-normalised fp32 planar [T,3,ho,wo] ----------------------
-// = resize_bilinear of the frames normalised the way the depth data pipeline does it on the host
-// (dataloader/depth/augmentation.py:30, 56-61): every SOURCE sample is x / 255, then - mean_c, then / std_c, each one
-// correctly rounded fp32 operation in that order, and the normalised samples are resampled.  No transpose: the depth
-// drivers have no portrait rule.  `Geo` says where frame t lies and how large it is: one size for the whole batch
+// ---- frames -> model input: uint8 [T,H,W,3] channel-last -> fp32 planar [T,3,ho,wo] ------------------------------------
+// `Geo` says where frame t lies, how large it is and whether it is read transposed: one size for the whole batch
 // (FramesUniform), or each frame at its own offset and size in a packed buffer (FramesRagged); the output is uniform.
 struct FramePixel {
   const uint8_t* base;
-  int H, W;
+  int H, W, transpose;
   long long t;
   int Y, X;
 };
@@ -231,6 +205,7 @@ struct FramesUniform {
   const uint8_t* frames;
   int H, W, ho, wo;
   long long total;
+  int transpose;
   __device__ __forceinline__ bool pixel(FramePixel& p) const {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= total) return false;
@@ -239,6 +214,7 @@ struct FramesUniform {
     p.t = i / ((long long)ho * wo);
     p.base = frames + p.t * (long long)H * W * 3;
     p.H = H; p.W = W;
+    p.transpose = transpose;
     return true;
   }
 };
@@ -258,10 +234,37 @@ struct FramesRagged {
     p.Y = (int)(i / wo);
     p.base = frames + it.offset;
     p.H = it.h; p.W = it.w;
+    p.transpose = (it.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0;
     return true;
   }
 };
 
+// Flow frames, in [0, 255]: = resize_bilinear(frames.permute(0,3,1,2).float()), with the portrait transpose of
+// evaluate_flow.py:713-717 (the source is read as [3, W, H]) folded into the load.  One thread per output pixel, three
+// planes written.
+template <class Geo>
+__global__ void __launch_bounds__(256) frames_to_planar_kernel(Geo geo, float* __restrict__ out, int ho, int wo) {
+  FramePixel p;
+  if (!geo.pixel(p)) return;
+  const int H = p.H, W = p.W, X = p.X, Y = p.Y, transpose = p.transpose;
+  const int hs = transpose ? W : H, ws = transpose ? H : W;     // source size as the resize sees it
+  const uint8_t* base = p.base;
+  const long long plane = (long long)ho * wo;
+  float* o = out + p.t * 3 * plane + (long long)Y * wo + X;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const auto load = [&](int y, int x) {
+      const long long pix = transpose ? (long long)x * W + y : (long long)y * W + x;
+      return (float)__ldg(base + pix * 3 + c);
+    };
+    o[c * plane] = bilinear_align_corners(load, hs, ws, ho, wo, Y, X);
+  }
+}
+
+// Depth and stereo frames, ImageNet-normalised: = resize_bilinear of the frames normalised the way the depth data pipeline
+// does it on the host (dataloader/depth/augmentation.py:30, 56-61): every SOURCE sample is x / 255, then - mean_c, then
+// / std_c, each one correctly rounded fp32 operation in that order, and the normalised samples are resampled.  No
+// transpose: the depth and stereo drivers have no portrait rule.
 template <class Geo>
 __global__ void __launch_bounds__(256) frames_to_planar_normalized_kernel(Geo geo, float* __restrict__ out, int ho, int wo,
                                                                           float m0, float m1, float m2, float s0, float s1,
@@ -293,10 +296,61 @@ __device__ __forceinline__ bool flow_unknown(float u, float v) {
   return !(fabsf(u) <= 1e7f) || !(fabsf(v) <= 1e7f);        // also true for NaN
 }
 
-__global__ void __launch_bounds__(256) flow_maxrad_kernel(const float* __restrict__ flow, unsigned* __restrict__ maxbits,
-                                                          long long hw) {
+// Where flow image n and its picture lie: one size, contiguous flows and strided pictures (FlowUniform, grid x over all
+// pixels of the batch), or each flow [2, h, w] at its own offset in a packed buffer and its picture at its own byte offset
+// with 3w-byte rows (FlowRagged, grid x over the capacity's pixels, grid y the item).  A ragged item whose flow or picture
+// does not fit, or whose two sizes differ, has hw = 0: it reads and writes nothing.
+struct FlowImage {
+  const float* u;
+  uint8_t* img;
+  int w;
+  long long hw, row_stride;
+};
+
+struct FlowUniform {
+  const float* flow;
+  uint8_t* out;
+  int w;
+  long long hw, row_stride, image_stride, total;
+  __device__ __forceinline__ FlowImage image(long long n) const {
+    return FlowImage{flow + n * 2 * hw, out + n * image_stride, w, hw, row_stride};
+  }
+  __device__ __forceinline__ bool pixel(long long& n, long long& p) const {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= total) return false;
+    n = i / hw;
+    p = i - n * hw;
+    return true;
+  }
+};
+
+struct FlowRagged {
+  const float* flow;
+  uint8_t* out;
+  const um_ragged_item* flows;
+  const um_ragged_item* pics;
+  int h_max, w_max;
+  long long flow_numel, out_bytes;
+  __device__ __forceinline__ FlowImage image(long long n) const {
+    const um_ragged_item f = flows[n], q = pics[n];
+    const bool ok = f.h == q.h && f.w == q.w && ragged_ok(f, h_max, w_max, 2, flow_numel) &&
+                    ragged_ok(q, h_max, w_max, 3, out_bytes);
+    return FlowImage{flow + (ok ? f.offset : 0), out + (ok ? q.offset : 0), f.w, ok ? (long long)f.h * f.w : 0, 3LL * f.w};
+  }
+  __device__ __forceinline__ bool pixel(long long& n, long long& p) const {
+    n = blockIdx.y;
+    p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    return true;                                   // the kernel compares p with the image's hw
+  }
+};
+
+// grid (x: CTAs striding over the pixels of one image, y: image)
+template <class Geo>
+__global__ void __launch_bounds__(256) flow_maxrad_kernel(Geo geo, unsigned* __restrict__ maxbits) {
   const int n = blockIdx.y;
-  const float* u = flow + (long long)n * 2 * hw;
+  const FlowImage im = geo.image(n);
+  const long long hw = im.hw;
+  const float* u = im.u;
   const float* v = u + hw;
   float m = 0.f;
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
@@ -331,14 +385,15 @@ __device__ __forceinline__ int wheel(int k, int ch) {
   return ch == 0 ? r0 : ch == 1 ? 0 : 255 - s;
 }
 
-__global__ void __launch_bounds__(256) flow_color_kernel(const float* __restrict__ flow, const unsigned* __restrict__ maxbits,
-                                                         uint8_t* __restrict__ out, int w, long long hw, long long row_stride,
-                                                         long long image_stride, long long total) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const long long n = i / hw, p = i - n * hw;
-  const float uf = __ldg(flow + n * 2 * hw + p), vf = __ldg(flow + n * 2 * hw + hw + p);
-  uint8_t* o = out + n * image_stride + (p / w) * row_stride + (p % w) * 3;
+template <class Geo>
+__global__ void __launch_bounds__(256) flow_color_kernel(Geo geo, const unsigned* __restrict__ maxbits) {
+  long long n, p;
+  if (!geo.pixel(n, p)) return;
+  const FlowImage im = geo.image(n);
+  if (p >= im.hw) return;
+  const int w = im.w;
+  const float uf = __ldg(im.u + p), vf = __ldg(im.u + im.hw + p);
+  uint8_t* o = im.img + (p / w) * im.row_stride + (p % w) * 3;
   if (flow_unknown(uf, vf)) { o[0] = o[1] = o[2] = 0; return; }
   const double den = __dadd_rn((double)__uint_as_float(__ldg(maxbits + n)), 2.220446049250313e-16);   // maxrad + eps
   const double u = __ddiv_rn((double)uf, den), v = __ddiv_rn((double)vf, den);
@@ -833,9 +888,21 @@ int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h,
   UM_REQUIRE(frames && out && n > 0 && h > 0 && w > 0 && h_out > 0 && w_out > 0,
              "um_frames_to_planar: bad arguments (positive sizes, non-null buffers)");
   const long long total = (long long)n * h_out * w_out;
-  frames_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(frames, out, h, w, transpose ? 1 : 0,
-                                                                                           h_out, w_out, total);
+  const FramesUniform geo{frames, h, w, h_out, w_out, total, transpose ? 1 : 0};
+  frames_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, out, h_out, w_out);
   return um::check_launch("um_frames_to_planar");
+}
+
+int um_frames_to_planar_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out, int32_t n,
+                               int32_t h_max, int32_t w_max, int32_t h_out, int32_t w_out, void* stream) {
+  UM_REQUIRE(frames && items && out && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && h_out > 0 && w_out > 0 &&
+                 frames_bytes > 0,
+             "um_frames_to_planar_ragged: bad arguments (1-65535 frames, positive sizes, non-null buffers)");
+  const long long plane = (long long)h_out * w_out;
+  const FramesRagged geo{frames, items, h_max, w_max, h_out, w_out, frames_bytes};
+  frames_to_planar_kernel<<<dim3((unsigned)((plane + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(geo, out, h_out,
+                                                                                                            w_out);
+  return um::check_launch("um_frames_to_planar_ragged");
 }
 
 int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t h_out,
@@ -874,12 +941,32 @@ int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_
   long long bx = (hw + 255) / 256;
   const long long cap = (132LL * 8 + n - 1) / n;          // about 8 CTAs per SM over the whole batch, grid-stride beyond
   bx = bx < cap ? bx : cap;
-  flow_maxrad_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(flow, reinterpret_cast<unsigned*>(max_scratch), hw);
-  if (int rc = um::check_launch("um_flow_to_image")) return rc;
   const long long total = (long long)n * hw;
-  flow_color_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(flow, reinterpret_cast<const unsigned*>(max_scratch), out, w,
-                                                                     hw, row_stride, image_stride, total);
+  const FlowUniform geo{flow, out, w, hw, row_stride, image_stride, total};
+  flow_maxrad_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, reinterpret_cast<unsigned*>(max_scratch));
+  if (int rc = um::check_launch("um_flow_to_image")) return rc;
+  flow_color_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(geo, reinterpret_cast<const unsigned*>(max_scratch));
   return um::check_launch("um_flow_to_image");
+}
+
+int um_flow_to_image_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, uint8_t* out,
+                            int64_t out_bytes, const um_ragged_item* picture_items, float* max_scratch, int32_t n,
+                            int32_t h_max, int32_t w_max, void* stream) {
+  UM_REQUIRE(flow && flow_items && out && picture_items && max_scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 &&
+                 flow_numel > 0 && out_bytes > 0,
+             "um_flow_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long cap = (long long)h_max * w_max;      // the grids are sized for the largest image
+  if (cudaMemsetAsync(max_scratch, 0, sizeof(float) * n, st) != cudaSuccess) return um::check_launch("um_flow_to_image_ragged");
+  long long bx = (cap + 255) / 256;
+  const long long per_image = (132LL * 8 + n - 1) / n;
+  bx = bx < per_image ? bx : per_image;
+  const FlowRagged geo{flow, out, flow_items, picture_items, h_max, w_max, flow_numel, out_bytes};
+  flow_maxrad_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(geo, reinterpret_cast<unsigned*>(max_scratch));
+  if (int rc = um::check_launch("um_flow_to_image_ragged")) return rc;
+  flow_color_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)n), 256, 0, st>>>(
+      geo, reinterpret_cast<const unsigned*>(max_scratch));
+  return um::check_launch("um_flow_to_image_ragged");
 }
 
 int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,

@@ -32,6 +32,14 @@ batched by the size the model sees, and the input conversion, the resize back an
 from a device descriptor table (the `*_ragged` kernels), so one CUDA graph per inference size serves every pair that maps
 to it.  `disparity_to_image` is the reference's `vis_disparity` (min-max scaling, cv2's INFERNO map) on the device.
 Writing files (PNG, PFM) stays out of scope.
+
+Flow pairs of mixed sizes (`inference_flow`, evaluate_flow.py:686-799, which takes each pair at its own size and
+orientation): `MixedSizeFlowRunner` streams host uint8 (image1, image2) pairs of any size, landscape or portrait, batched by
+the size the model sees after the portrait transpose; the conversion, the resize back with the two component scales and the
+transpose back, the forward-backward occlusion check and the Middlebury colouring all read each pair's geometry from the
+device descriptor table (`um_frames_to_planar_ragged`, `um_resize_bilinear_ragged`, `um_fb_consistency_ragged`,
+`um_flow_to_image_ragged`).  It shares its buckets, graphs, packing and statistics with `MixedSizeStereoRunner`
+(`_MixedSizeRunner`).
 """
 import collections
 import itertools
@@ -709,66 +717,36 @@ def _ragged_step_layout(sizes, batch, size, pred_bidir_disp, pred_right_disp):
     return frames, outputs, off, used, results
 
 
-class MixedSizeStereoRunner(_PipelinedRunner):
-    """Streaming stereo inference over host (left, right) uint8 pairs of ANY size up to `max_frame_size`:
-    `inference_stereo` (evaluate_stereo.py:711-843), which takes each pair at its own size, as a stream.
+class _MixedSizeRunner(_PipelinedRunner):
+    """Streaming over host pairs of uint8 frames [h, w, 3] of ANY size up to `max_frame_size`, the part that does not depend
+    on the task: steps of up to `batch` pairs of one bucket (`_batches` with `max_open=max_buckets`); per staging slot one
+    pinned and one device buffer of packed uint8 frames and a descriptor table (`um_ragged_item`), of which a step uploads
+    the used bytes only; one CUDA graph per bucket and staging slot, captured when the bucket first appears, the least
+    recently used bucket's graphs and held buffers dropped when `max_buckets` buckets hold graphs; packed outputs of which
+    the used prefixes are downloaded; `(index, result)` in completion order; `stats`.
 
-    * buckets: a pair's bucket is the size the model sees, its size rounded up to a multiple of `padding_factor` or
-      `inference_size` (so with `inference_size` every pair shares one bucket); a step holds up to `batch` pairs of one
-      bucket, formed as the submission drivers form batches (`_batches`: one open step per bucket, sent when full; opening
-      more than `max_buckets` sends the oldest open step early; the open steps are sent at the end);
-    * upload: each slot has one pinned uint8 buffer of 2 * batch * H_max * W_max * 3 bytes and a small descriptor table
-      (`um_ragged_item`); a step packs its left frames, then its right frames, back to back and copies only the used bytes
-      and the table on a side stream while the previous step computes; a short step's fillers repeat its last pair
-      without uploading it again and their results are dropped;
-    * device work of a step, one CUDA graph per bucket and staging slot, captured when the bucket first appears (the least
-      recently used bucket's graphs and held buffers are dropped when `max_buckets` buckets hold graphs): the ragged
-      conversion (`um_frames_to_planar_normalized_ragged`: ImageNet normalisation and resize of every frame from its own
-      size to the bucket's), the hflip batching and forward of `infer_stereo`, the ragged resize back with the width
-      rescale and the flip back (`um_resize_bilinear_ragged`) and, with `visualize`, the ragged colouring
-      (`um_disparity_to_image_ragged`); the descriptors live in device memory, so a replay reads each step's geometry;
-    * download: only the used prefix of the packed disparities (and pictures).
+    A subclass provides `_bucket(pair)` (the size the model sees), `_frame_order(pairs)` (the step's frames in the order they
+    are packed), `_layout(sizes, size)` (the step's descriptor table as one record array, the used elements of each output
+    buffer, and per real pair its result views as (key, buffer, offset, shape)) and `_step(slot, size)` (the device work on
+    `dev_in[slot]` / `dev_desc[slot]`, returning {buffer: packed device tensor})."""
 
-    Sizes, padding, `inference_size` and the bidirectional / right-view semantics are those of `infer_stereo` on each pair.
-    `run(pairs)` takes an iterable of (left, right) host uint8 frames [h, w, 3] (numpy arrays or tensors, RGB as PIL decodes
-    them; both of a pair the same size) and yields (index, result) as steps complete -- completion order, not input order,
-    so a rare bucket does not hold back later results; `index` is the pair's position in the input, each exactly once.
-    `result` holds CPU views 'disp' [h, w] (+ 'disp_right') and, with `visualize`, the uint8 BGR pictures 'vis' [h, w, 3]
-    (+ 'vis_right'); `return_disp=False` with `visualize` sends back only the pictures.  The views point into reused pinned
-    staging -- copy what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
-
-    def __init__(self, model, max_frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
-                 pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, max_buckets=4, **model_kwargs):
-        if pred_bidir_disp and pred_right_disp:
-            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
-        if not return_disp and not visualize:
-            raise ValueError("nothing to return: return_disp=False needs visualize=True")
-        self.kw = dict(model_kwargs)
-        if self.kw.pop("task", "stereo") != "stereo":
-            raise ValueError("MixedSizeStereoRunner drives the stereo task only")
+    def _init_mixed(self, model, max_frame_size, batch, device, use_graph, max_buckets, n_desc, out_buffers):
+        """`n_desc`: items of a step's table; `out_buffers`: {buffer: (dtype, elements per pixel of capacity and pair)}"""
+        name = type(self).__name__
         self.model, self.batch, self.max_buckets = model, int(batch), int(max_buckets)
         if self.batch < 1 or self.max_buckets < 1:
-            raise ValueError("MixedSizeStereoRunner: batch and max_buckets must be positive")
+            raise ValueError("%s: batch and max_buckets must be positive" % name)
         self.hmax, self.wmax = int(max_frame_size[0]), int(max_frame_size[1])
         if self.hmax < 1 or self.wmax < 1 or self.hmax * self.wmax > 0x7fffffff:
-            raise ValueError("MixedSizeStereoRunner: max_frame_size must be positive, at most 2^31 - 1 pixels")
-        self.padding_factor, self.inference_size = padding_factor, inference_size
-        self.bidir, self.right = bool(pred_bidir_disp), bool(pred_right_disp)
-        self.visualize, self.return_disp = bool(visualize), bool(return_disp)
+            raise ValueError("%s: max_frame_size must be positive, at most 2^31 - 1 pixels" % name)
         self._init_pipeline(device, use_graph)
         cap = self.hmax * self.wmax
-        nout = (2 if self.bidir else 1) * self.batch
-        ndesc = 2 * self.batch + nout
         self.pin = [torch.empty((2 * self.batch * cap * 3,), dtype=torch.uint8).pin_memory() for _ in range(2)]
         self.dev_in = [torch.empty((2 * self.batch * cap * 3,), dtype=torch.uint8, device=self.dev) for _ in range(2)]
-        self.desc_pin = [torch.empty((ndesc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8).pin_memory() for _ in range(2)]
-        self.dev_desc = [torch.zeros((ndesc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8, device=self.dev) for _ in range(2)]
-        self.out_pin = [{} for _ in range(2)]
-        for pins in self.out_pin:
-            if self.return_disp:
-                pins["disp"] = torch.empty((nout * cap,)).pin_memory()
-            if self.visualize:
-                pins["vis"] = torch.empty((3 * nout * cap,), dtype=torch.uint8).pin_memory()
+        self.desc_pin = [torch.empty((n_desc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.dev_desc = [torch.zeros((n_desc, ops.RAGGED_ITEM_BYTES), dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.out_pin = [{k: torch.empty((per * self.batch * cap,), dtype=dt).pin_memory() for k, (dt, per) in out_buffers.items()}
+                        for _ in range(2)]
         self.meta = [None, None]                 # host layout of the step staged in each slot
         self.out_meta = [None, None]             # host layout of the step downloaded into each slot's pinned outputs
         self.buckets = collections.OrderedDict()  # inference size -> (graphs, outputs, held buffers), least recent first
@@ -776,35 +754,35 @@ class MixedSizeStereoRunner(_PipelinedRunner):
 
     # ---- host side
     def _pair(self, pair):
-        left, right = (torch.as_tensor(f) for f in pair)
-        for f in (left, right):
+        name = type(self).__name__
+        first, second = (torch.as_tensor(f) for f in pair)
+        for f in (first, second):
             if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                raise ValueError("MixedSizeStereoRunner: frames must be uint8 [h, w, 3]")
-        if left.shape != right.shape:
-            raise ValueError("MixedSizeStereoRunner: the left and right frames of a pair must have the same size")
-        if not (1 <= left.shape[0] <= self.hmax and 1 <= left.shape[1] <= self.wmax):
-            raise ValueError("MixedSizeStereoRunner: a %dx%d frame exceeds max_frame_size %dx%d"
-                             % (left.shape[0], left.shape[1], self.hmax, self.wmax))
-        return left, right
-
-    def _bucket(self, pair):
-        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+                raise ValueError("%s: frames must be uint8 [h, w, 3]" % name)
+        if first.shape != second.shape:
+            raise ValueError("%s: the two frames of a pair must have the same size" % name)
+        if not (1 <= first.shape[0] <= self.hmax and 1 <= first.shape[1] <= self.wmax):
+            raise ValueError("%s: a %dx%d frame exceeds max_frame_size %dx%d"
+                             % (name, first.shape[0], first.shape[1], self.hmax, self.wmax))
+        return first, second
 
     def _chunks(self, items):
         checked = ((i, self._pair(p)) for i, p in items)
         return _batches(checked, self.batch, lambda s: self._bucket(s[1]), self.max_buckets)
 
+    def _table(self, sizes, size):
+        table, used, results = self._layout(sizes, size)
+        return table.view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES), used, results
+
     def _stage_host(self, slot, chunk):
         """the step's packed frames and descriptor table into pinned memory, then their H2D copies (used bytes only)"""
         pairs = [p for _, p in chunk]
         size = self._bucket(pairs[0])
-        frames, outputs, nbytes, used, results = _ragged_step_layout([tuple(p[0].shape[:2]) for p in pairs], self.batch, size,
-                                                                     self.bidir, self.right)
-        off = 0
-        for f in [p[0] for p in pairs] + [p[1] for p in pairs]:
-            self.pin[slot][off:off + f.numel()].copy_(f.reshape(-1))
-            off += f.numel()
-        table = np.concatenate((frames, outputs)).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES)
+        table, used, results = self._table([tuple(p[0].shape[:2]) for p in pairs], size)
+        nbytes = 0
+        for f in self._frame_order(pairs):
+            self.pin[slot][nbytes:nbytes + f.numel()].copy_(f.reshape(-1))
+            nbytes += f.numel()
         self.desc_pin[slot].copy_(torch.from_numpy(table))
         self.dev_in[slot][:nbytes].copy_(self.pin[slot][:nbytes], non_blocking=True)
         self.dev_desc[slot].copy_(self.desc_pin[slot], non_blocking=True)
@@ -816,44 +794,19 @@ class MixedSizeStereoRunner(_PipelinedRunner):
     def _download(self, slot, out):
         meta = self.out_meta[slot] = self.meta[slot]
         for k, v in out.items():
-            n = meta["used"] * (3 if k == "vis" else 1)
+            n = meta["used"][k]
             self.out_pin[slot][k][:n].copy_(v[:n], non_blocking=True)
             self.stats["d2h_bytes"] += n * v.element_size()
 
     def _results(self, slot, n):
         pins = self.out_pin[slot]
-        for index, outs in self.out_meta[slot]["results"][:n]:
-            r = {}
-            for key, off, h, w in outs:
-                if self.return_disp:
-                    r[key] = pins["disp"][off:off + h * w].view(h, w)
-                if self.visualize:
-                    r[key.replace("disp", "vis")] = pins["vis"][3 * off:3 * (off + h * w)].view(h, w, 3)
-            yield index, r
+        for index, views in self.out_meta[slot]["results"][:n]:
+            yield index, {key: pins[buf][off:off + math.prod(shape)].view(shape) for key, buf, off, shape in views}
 
     # ---- device side
-    def _step(self, slot, size):
-        b, nf = self.batch, 2 * self.batch
-        items = self.dev_desc[slot]
-        planes = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:nf], self.hmax, self.wmax, int(size[0]),
-                                                         int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
-        disp = _stereo_forward(self.model, planes[:b], planes[b:], self.bidir, self.right, dict(self.kw))
-        out_items = items[nf:]
-        packed = _OPS.resize_bilinear_ragged(disp.contiguous(), out_items, self.hmax, self.wmax,
-                                             out_items.shape[0] * self.hmax * self.wmax)
-        out = {}
-        if self.return_disp:
-            out["disp"] = packed
-        if self.visualize:
-            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
-            _OPS.disparity_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
-        return out
-
     def _reset_inputs(self, slot):
         """zero frames and a full-capacity descriptor table: valid for any bucket"""
-        full = [(self.hmax, self.wmax)] * self.batch
-        frames, outputs, _, _, _ = _ragged_step_layout(full, self.batch, (self.hmax, self.wmax), self.bidir, self.right)
-        table = np.concatenate((frames, outputs)).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES)
+        table, _, _ = self._table([(self.hmax, self.wmax)] * self.batch, (self.hmax, self.wmax))
         self.dev_in[slot].zero_()
         self.dev_desc[slot].copy_(torch.from_numpy(table))
 
@@ -902,6 +855,237 @@ class MixedSizeStereoRunner(_PipelinedRunner):
     def run(self, pairs):
         with torch.cuda.device(self.dev):
             yield from self._pipeline(enumerate(pairs))
+
+
+class MixedSizeStereoRunner(_MixedSizeRunner):
+    """Streaming stereo inference over host (left, right) uint8 pairs of ANY size up to `max_frame_size`:
+    `inference_stereo` (evaluate_stereo.py:711-843), which takes each pair at its own size, as a stream.
+
+    * buckets: a pair's bucket is the size the model sees, its size rounded up to a multiple of `padding_factor` or
+      `inference_size` (so with `inference_size` every pair shares one bucket); a step holds up to `batch` pairs of one
+      bucket, formed as the submission drivers form batches (`_batches`: one open step per bucket, sent when full; opening
+      more than `max_buckets` sends the oldest open step early; the open steps are sent at the end);
+    * upload: each slot has one pinned uint8 buffer of 2 * batch * H_max * W_max * 3 bytes and a small descriptor table
+      (`um_ragged_item`); a step packs its left frames, then its right frames, back to back and copies only the used bytes
+      and the table on a side stream while the previous step computes; a short step's fillers repeat its last pair
+      without uploading it again and their results are dropped;
+    * device work of a step, one CUDA graph per bucket and staging slot, captured when the bucket first appears (the least
+      recently used bucket's graphs and held buffers are dropped when `max_buckets` buckets hold graphs): the ragged
+      conversion (`um_frames_to_planar_normalized_ragged`: ImageNet normalisation and resize of every frame from its own
+      size to the bucket's), the hflip batching and forward of `infer_stereo`, the ragged resize back with the width
+      rescale and the flip back (`um_resize_bilinear_ragged`) and, with `visualize`, the ragged colouring
+      (`um_disparity_to_image_ragged`); the descriptors live in device memory, so a replay reads each step's geometry;
+    * download: only the used prefix of the packed disparities (and pictures).
+
+    Sizes, padding, `inference_size` and the bidirectional / right-view semantics are those of `infer_stereo` on each pair.
+    `run(pairs)` takes an iterable of (left, right) host uint8 frames [h, w, 3] (numpy arrays or tensors, RGB as PIL decodes
+    them; both of a pair the same size) and yields (index, result) as steps complete -- completion order, not input order,
+    so a rare bucket does not hold back later results; `index` is the pair's position in the input, each exactly once.
+    `result` holds CPU views 'disp' [h, w] (+ 'disp_right') and, with `visualize`, the uint8 BGR pictures 'vis' [h, w, 3]
+    (+ 'vis_right'); `return_disp=False` with `visualize` sends back only the pictures.  The views point into reused pinned
+    staging -- copy what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
+
+    def __init__(self, model, max_frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
+                 pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, max_buckets=4, **model_kwargs):
+        if pred_bidir_disp and pred_right_disp:
+            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
+        if not return_disp and not visualize:
+            raise ValueError("nothing to return: return_disp=False needs visualize=True")
+        self.kw = dict(model_kwargs)
+        if self.kw.pop("task", "stereo") != "stereo":
+            raise ValueError("MixedSizeStereoRunner drives the stereo task only")
+        self.padding_factor, self.inference_size = padding_factor, inference_size
+        self.bidir, self.right = bool(pred_bidir_disp), bool(pred_right_disp)
+        self.visualize, self.return_disp = bool(visualize), bool(return_disp)
+        views = 2 if self.bidir else 1
+        buffers = {}
+        if self.return_disp:
+            buffers["disp"] = (torch.float32, views)
+        if self.visualize:
+            buffers["vis"] = (torch.uint8, 3 * views)
+        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), buffers)
+
+    # ---- host side
+    def _bucket(self, pair):
+        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+
+    @staticmethod
+    def _frame_order(pairs):
+        """the step's left frames, then its right frames"""
+        return [p[0] for p in pairs] + [p[1] for p in pairs]
+
+    def _layout(self, sizes, size):
+        frames, outputs, _, used, results = _ragged_step_layout(sizes, self.batch, size, self.bidir, self.right)
+        views = []
+        for outs in results:
+            views.append([])
+            for key, off, h, w in outs:
+                if self.return_disp:
+                    views[-1].append((key, "disp", off, (h, w)))
+                if self.visualize:
+                    views[-1].append((key.replace("disp", "vis"), "vis", 3 * off, (h, w, 3)))
+        return np.concatenate((frames, outputs)), {"disp": used, "vis": 3 * used}, views
+
+    # ---- device side
+    def _step(self, slot, size):
+        b, nf = self.batch, 2 * self.batch
+        items = self.dev_desc[slot]
+        planes = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:nf], self.hmax, self.wmax, int(size[0]),
+                                                         int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
+        disp = _stereo_forward(self.model, planes[:b], planes[b:], self.bidir, self.right, dict(self.kw))
+        out_items = items[nf:]
+        packed = _OPS.resize_bilinear_ragged(disp.contiguous(), out_items, self.hmax, self.wmax,
+                                             out_items.shape[0] * self.hmax * self.wmax)
+        out = {}
+        if self.return_disp:
+            out["disp"] = packed
+        if self.visualize:
+            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
+            _OPS.disparity_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
+        return out
+
+
+def _flow_step_layout(sizes, batch, size, pred_bidir_flow, fwd_bwd_consistency_check):
+    """Descriptor tables of one flow step of `batch` pairs at the inference size `size`, whose real pairs have the original
+    sizes `sizes` as stored (1 <= len <= batch; portrait pairs, h > w, carry RAGGED_TRANSPOSE: the model sees them
+    transposed).  Returns (frames, planes, flows, pictures, masks, frame_bytes, used, results):
+    * frames: 2*batch items over the packed uint8 frames -- the real pairs' first frames back to back, then their second
+      frames; the items of a short step's filler pairs point at its last pair's frames, so fillers upload nothing;
+    * planes: the resize back of the model's [D*batch, 2, H, W] flow (D = 2 with `pred_bidir_flow`: the forward flows, then
+      the backward ones) taken as 2*D*batch single-channel images -- the u plane, then the v plane of each flow, packed
+      back to back, so that a pair's flow is a contiguous planar [2, h, w]; scaled by the width and the height ratio of the
+      pair as the model sees it, rounded to fp32, when that size differs from `size` (1 otherwise, as `_flow_outputs`
+      does); fillers are empty items, which the kernels skip;
+    * flows / pictures: D*batch items, each flow [2, h, w] (offset in floats) and its RGB picture (offset in bytes);
+    * masks: with `fwd_bwd_consistency_check`, 2*batch items, the pairs' 'fwd_occ' [h, w], then their 'bwd_occ';
+    * frame_bytes: the used prefix of the packed frames; used: {'flow': floats, 'vis': bytes, 'occ': floats};
+    * results: per real pair, the (key, buffer, offset, shape) of each of its outputs."""
+    n = len(sizes)
+    frames = np.zeros(2 * batch, RAGGED_ITEM)
+    off = 0
+    for half in range(2):
+        for i, (h, w) in enumerate(sizes):
+            frames[half * batch + i] = (off, h, w, 1.0, ops.RAGGED_TRANSPOSE if h > w else 0)
+            off += 3 * h * w
+        frames[half * batch + n:(half + 1) * batch] = frames[half * batch + n - 1]
+    keys = ("flow", "flow_bwd") if pred_bidir_flow else ("flow",)
+    planes = np.zeros(2 * len(keys) * batch, RAGGED_ITEM)
+    flows, pictures = np.zeros(len(keys) * batch, RAGGED_ITEM), np.zeros(len(keys) * batch, RAGGED_ITEM)
+    masks = np.zeros(2 * batch if fwd_bwd_consistency_check else 0, RAGGED_ITEM)
+    results = [[] for _ in sizes]
+    used = 0                                                     # floats of flow so far; the pictures take 3 bytes per 2 floats
+    for d, key in enumerate(keys):
+        for i, (h, w) in enumerate(sizes):
+            transposed = h > w
+            ori = (w, h) if transposed else (h, w)                 # the pair as the model sees it
+            su, sv = (np.float32(ori[1] / size[1]), np.float32(ori[0] / size[0])) if ori != tuple(size) else (1.0, 1.0)
+            flags = ops.RAGGED_TRANSPOSE if transposed else 0
+            j = d * batch + i
+            planes[2 * j], planes[2 * j + 1] = (used, h, w, su, flags), (used + h * w, h, w, sv, flags)
+            flows[j], pictures[j] = (used, h, w, 1.0, 0), (3 * (used // 2), h, w, 1.0, 0)
+            results[i] += [(key, "flow", used, (2, h, w)), (key.replace("flow", "vis"), "vis", 3 * (used // 2), (h, w, 3))]
+            used += 2 * h * w
+    used_occ = 0
+    for k, key in enumerate(("fwd_occ", "bwd_occ") if fwd_bwd_consistency_check else ()):
+        for i, (h, w) in enumerate(sizes):
+            masks[k * batch + i] = (used_occ, h, w, 1.0, 0)
+            results[i].append((key, "occ", used_occ, (h, w)))
+            used_occ += h * w
+    return frames, planes, flows, pictures, masks, off, {"flow": used, "vis": 3 * (used // 2), "occ": used_occ}, results
+
+
+class MixedSizeFlowRunner(_MixedSizeRunner):
+    """Streaming optical flow over host (image1, image2) uint8 pairs of ANY size and either orientation up to
+    `max_frame_size`: `inference_flow` (evaluate_flow.py:686-799), which takes each pair at its own size, as a stream.
+
+    * buckets: a pair's bucket is the size the model sees -- the pair transposed when it is portrait (h > w,
+      evaluate_flow.py:713-717), then rounded up to a multiple of `padding_factor`, or `inference_size` -- so a 480x832 and
+      an 832x480 pair share a step; steps are formed as in `MixedSizeStereoRunner` (`_batches`, at most `max_buckets` open);
+    * upload: the step's first frames, then its second frames, packed back to back as uint8 (2.4 MB per 480x832 pair,
+      against 9.6 MB for two float32 images), the used bytes only, and the descriptor table, on a side stream while the
+      previous step computes; `pred_bwd_flow` (the reference's swap, evaluate_flow.py:735-736) only changes which frame of a
+      pair is packed first; a short step's fillers repeat its last pair without uploading it again;
+    * device work of a step, one CUDA graph per bucket and staging slot: `um_frames_to_planar_ragged` (uint8 -> float planes,
+      portrait transpose and resize of every frame from its own size to the bucket's), the forward (with
+      `pred_bidir_flow`), `um_resize_bilinear_ragged` back to each pair's own size and orientation with its two component
+      scales, `um_fb_consistency_ragged` on the flows at their original size with `fwd_bwd_consistency_check`, and
+      `um_flow_to_image_ragged` on 'flow' (and 'flow_bwd') with `visualize`;
+    * download: only the used prefixes of the packed flows, masks and pictures.
+
+    Sizes, transpose, rescale and bidirectional semantics are those of `infer_flow` on each pair.  `max_frame_size` bounds
+    the frames as stored, so (832, 832) admits both 480x832 and 832x480.  `run(pairs)` takes an iterable of (image1, image2)
+    host uint8 frames [h, w, 3] (numpy arrays or tensors; both of a pair the same size) and yields (index, result) as steps
+    complete -- completion order, not input order; `index` is the pair's position in the input, each exactly once.
+    `result` holds CPU views 'flow' [2, h, w] (+ 'flow_bwd'; 'fwd_occ' / 'bwd_occ' [h, w], 1 = occluded) and, with
+    `visualize`, the uint8 RGB pictures 'vis' [h, w, 3] (+ 'vis_bwd'); `return_flow=False` with `visualize` sends back only
+    the pictures.  The views point into reused pinned staging -- copy what you keep.  `stats` counts steps, pairs, captures
+    and the bytes copied each way."""
+
+    def __init__(self, model, max_frame_size, batch, device, padding_factor=32, inference_size=None, pred_bidir_flow=False,
+                 pred_bwd_flow=False, fwd_bwd_consistency_check=False, visualize=False, return_flow=True, use_graph=True,
+                 max_buckets=4, **model_kwargs):
+        self.kw = dict(model_kwargs)
+        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "MixedSizeFlowRunner")
+        if not return_flow and not visualize:
+            raise ValueError("nothing to return: return_flow=False needs visualize=True")
+        if not return_flow and fwd_bwd_consistency_check:
+            raise ValueError("return_flow=False sends back pictures only: it excludes fwd_bwd_consistency_check")
+        self.padding_factor, self.inference_size = padding_factor, inference_size
+        self.bidir, self.bwd, self.check = bool(pred_bidir_flow), bool(pred_bwd_flow), bool(fwd_bwd_consistency_check)
+        self.visualize, self.return_flow = bool(visualize), bool(return_flow)
+        dirs = 2 if self.bidir else 1
+        buffers = {}
+        if self.return_flow:
+            buffers["flow"] = (torch.float32, 2 * dirs)
+        if self.check:
+            buffers["occ"] = (torch.float32, 2)
+        if self.visualize:
+            buffers["vis"] = (torch.uint8, 3 * dirs)
+        if self.check and min(max_frame_size) < 2:
+            raise ValueError("MixedSizeFlowRunner: fwd_bwd_consistency_check needs frames of at least 2x2")
+        self.buffers = tuple(buffers)
+        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets,
+                         (2 + 4 * dirs + (2 if self.check else 0)) * int(batch), buffers)
+
+    # ---- host side
+    def _pair(self, pair):
+        first, second = super()._pair(pair)
+        if self.check and min(first.shape[:2]) < 2:
+            raise ValueError("MixedSizeFlowRunner: fwd_bwd_consistency_check needs frames of at least 2x2")
+        return first, second
+
+    def _bucket(self, pair):
+        return _frame_geometry(pair[0].shape[0], pair[0].shape[1], self.padding_factor, self.inference_size, "flow")[2]
+
+    def _frame_order(self, pairs):
+        """the step's first frames, then its second frames; `pred_bwd_flow` swaps the two of every pair"""
+        first, second = (1, 0) if self.bwd else (0, 1)
+        return [p[first] for p in pairs] + [p[second] for p in pairs]
+
+    def _layout(self, sizes, size):
+        *tables, _, used, results = _flow_step_layout(sizes, self.batch, size, self.bidir, self.check)
+        return np.concatenate(tables), used, [[v for v in views if v[1] in self.buffers] for views in results]
+
+    # ---- device side
+    def _step(self, slot, size):
+        b, cap = self.batch, self.hmax * self.wmax
+        nflow = (2 if self.bidir else 1) * b
+        frames, planes, flows, pictures, masks = torch.split(self.dev_desc[slot], [2 * b, 2 * nflow, nflow, nflow,
+                                                                                    2 * b if self.check else 0])
+        x = _OPS.frames_to_planar_ragged(self.dev_in[slot], frames, self.hmax, self.wmax, int(size[0]), int(size[1]))
+        flow = self.model(x[:b], x[b:], pred_bidir_flow=self.bidir, **self.kw)["flow_preds"][-1]      # [nflow, 2, H, W]
+        packed = _OPS.resize_bilinear_ragged(flow.contiguous().view(2 * nflow, 1, *flow.shape[-2:]), planes, self.hmax,
+                                             self.wmax, 2 * nflow * cap)
+        out = {}
+        if self.return_flow:
+            out["flow"] = packed
+        if self.check:
+            out["occ"] = torch.empty((2 * b * cap,), device=self.dev)
+            _OPS.fb_consistency_ragged(packed, flows, out["occ"], masks, self.hmax, self.wmax, 0.01, 0.5)
+        if self.visualize:
+            out["vis"] = torch.empty((3 * nflow * cap,), dtype=torch.uint8, device=self.dev)
+            _OPS.flow_to_image_ragged(packed, flows, out["vis"], pictures, self.hmax, self.wmax)
+        return out
 
 
 class _SequenceRunner(_PipelinedRunner):

@@ -70,7 +70,7 @@ class RaggedItem(ctypes.Structure):
                 ("flags", ctypes.c_int32)]
 
 
-RAGGED_FLIP_X = 1
+RAGGED_FLIP_X, RAGGED_TRANSPOSE = 1, 2
 RAGGED_ITEM_BYTES = ctypes.sizeof(RaggedItem)      # 24
 
 
@@ -101,6 +101,7 @@ _SIGNATURES = {
     "um_local_corr_volume": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_flow_warp": (_RC, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "um_fb_consistency": (_RC, [_P, _P, _F, _F, _P, _P, _I, _I, _I, _P]),
+    "um_fb_consistency_ragged": (_RC, [_P, _L, _P, _F, _F, _P, _L, _P, _I, _I, _I, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -108,11 +109,13 @@ _SIGNATURES = {
     "um_upsample2x": (_RC, [_P, _P, _I, _I, _I, _I, _F, _P]),
     "um_resize_bilinear": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _FP, _I, _P]),
     "um_frames_to_planar": (_RC, [_P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "um_frames_to_planar_ragged": (_RC, [_P, _L, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_frames_to_planar_normalized": (_RC, [_P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
     "um_frames_to_planar_normalized_ragged": (_RC, [_P, _L, _P, _P, _I, _I, _I, _I, _I, _FP, _FP, _P]),
     "um_resize_bilinear_ragged": (_RC, [_P, _P, _L, _P, _I, _I, _I, _I, _I, _P]),
     "um_disparity_to_image_ragged": (_RC, [_P, _L, _P, _P, _P, _I, _I, _I, _P]),
     "um_flow_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_flow_to_image_ragged": (_RC, [_P, _L, _P, _P, _L, _P, _P, _I, _I, _I, _P]),
     "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_depth_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_encode_submission": (_RC, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
@@ -536,6 +539,58 @@ def _disparity_to_image_ragged(disp, items, out, h_max, w_max):
 
 disparity_to_image_ragged = _define("disparity_to_image_ragged(Tensor disp, Tensor items, Tensor(a!) out, int h_max, int w_max) -> ()",
                                     _disparity_to_image_ragged)
+
+
+def _frames_to_planar_ragged(frames, items, h_max, w_max, h_out, w_out):
+    """frames: contiguous CUDA uint8, the packed frames (frame i [h_i, w_i, 3] at byte items[i].offset, read transposed with
+    RAGGED_TRANSPOSE) -> fp32 [n, 3, h_out, w_out] in [0, 255]"""
+    if not frames.is_cuda or frames.dtype != torch.uint8 or not frames.is_contiguous() or frames.numel() == 0:
+        raise RuntimeError("frames_to_planar_ragged: expected contiguous CUDA uint8 packed frames")
+    n = _ragged_items(items, "frames_to_planar_ragged")
+    out = torch.empty((n, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
+    _check(LIB.um_frames_to_planar_ragged(_p(frames), frames.numel(), _p(items), _p(out), n, h_max, w_max, h_out, w_out,
+                                          _stream()), "um_frames_to_planar_ragged")
+    return out
+
+
+frames_to_planar_ragged = _define(
+    "frames_to_planar_ragged(Tensor frames, Tensor items, int h_max, int w_max, int h_out, int w_out) -> Tensor",
+    _frames_to_planar_ragged)
+
+
+def _flow_to_image_ragged(flow, flow_items, out, picture_items, h_max, w_max):
+    """flow: contiguous fp32 packed planar flows (flow i [2, h_i, w_i] at float flow_items[i].offset); out: contiguous uint8,
+    picture i [h_i, w_i, 3] at byte picture_items[i].offset"""
+    _f32c(flow, "flow")
+    if out.dtype != torch.uint8 or not out.is_contiguous() or out.device != flow.device or out.numel() == 0:
+        raise RuntimeError("flow_to_image_ragged: out must be contiguous uint8 on the flow's device")
+    n = _ragged_items(flow_items, "flow_to_image_ragged")
+    if _ragged_items(picture_items, "flow_to_image_ragged") != n:
+        raise RuntimeError("flow_to_image_ragged: one picture item per flow item")
+    scratch = torch.empty((n,), device=flow.device, dtype=torch.float32)
+    _check(LIB.um_flow_to_image_ragged(_p(flow), flow.numel(), _p(flow_items), _p(out), out.numel(), _p(picture_items),
+                                       _p(scratch), n, h_max, w_max, _stream()), "um_flow_to_image_ragged")
+
+
+flow_to_image_ragged = _define(
+    "flow_to_image_ragged(Tensor flow, Tensor flow_items, Tensor(a!) out, Tensor picture_items, int h_max, int w_max) -> ()",
+    _flow_to_image_ragged)
+
+
+def _fb_consistency_ragged(flow, flow_items, occ, occ_items, h_max, w_max, alpha, beta):
+    """flow: contiguous fp32 packed planar flows; occ: contiguous fp32 packed masks; both tables hold 2n items, pair i's
+    forward flow (mask) at [i] and its backward one at [n + i]"""
+    _f32c(flow, "flow"), _f32c(occ, "occ")
+    n2 = _ragged_items(flow_items, "fb_consistency_ragged")
+    if _ragged_items(occ_items, "fb_consistency_ragged") != n2 or n2 % 2 or occ.device != flow.device:
+        raise RuntimeError("fb_consistency_ragged: two flow items and two mask items per pair, on one device")
+    _check(LIB.um_fb_consistency_ragged(_p(flow), flow.numel(), _p(flow_items), float(alpha), float(beta), _p(occ), occ.numel(),
+                                        _p(occ_items), n2 // 2, h_max, w_max, _stream()), "um_fb_consistency_ragged")
+
+
+fb_consistency_ragged = _define(
+    "fb_consistency_ragged(Tensor flow, Tensor flow_items, Tensor(a!) occ, Tensor occ_items, int h_max, int w_max, float alpha, "
+    "float beta) -> ()", _fb_consistency_ragged)
 
 DEPTH_TO_IMAGE_SCRATCH_WORDS = 2056      # per image, include/unimatch_sm100.h (um_depth_to_image)
 
