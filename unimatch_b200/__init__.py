@@ -35,13 +35,17 @@ _LAZY = {
     "validate_depth": (".evaluation", "validate_depth"),
     "create_flow_submission": (".submission", "create_flow_submission"),
     "create_stereo_submission": (".submission", "create_stereo_submission"),
+    "inference_flow": (".inference_io", "inference_flow"),
+    "inference_stereo": (".inference_io", "inference_stereo"),
+    "inference_depth": (".inference_io", "inference_depth"),
 }
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
            "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "MixedSizeStereoRunner", "MixedSizeFlowRunner",
            "disparity_to_image", "depth_to_image",
-           "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission"]
+           "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission",
+           "inference_flow", "inference_stereo", "inference_depth"]
 
 
 def __getattr__(name):

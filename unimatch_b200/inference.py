@@ -16,8 +16,8 @@ Video (`main_flow.py --inference_video`, evaluate_flow.py:642-831): `infer_flow_
 sequence with every frame encoded ONCE (pair (t, t+1) and pair (t+1, t+2) share frame t+1's feature pyramid; the encoder is
 per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 summation order), `VideoFlowRunner` streams host uint8 frames through the same
 path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
-colouring of utils/flow_viz.py on the device.  Decoding frames and writing videos (mp4) stay out of scope; the leaderboard
-files (.flo, PNG, PFM) are written by `submission.py`.
+colouring of utils/flow_viz.py on the device.  Writing videos (mp4) stays out of scope; the leaderboard files (.flo, PNG,
+PFM) are written by `submission.py`, and the plain inference commands' files (decoding included) by `inference_io.py`.
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
@@ -1171,6 +1171,9 @@ class VideoFlowRunner(_SequenceRunner):
     * download: the flow (and flow_bwd / fwd_occ / bwd_occ when asked) and, with `visualize`, the uint8 Middlebury picture
       (`flow_to_image`; with `concat_frame` the frame and its picture side by side, stacked as the reference's
       `concat_flow_img` does, evaluate_flow.py:818-825).  `return_flow=False` with `visualize` sends back only the picture.
+      `visualize_bwd` (with `pred_bidir_flow` and `visualize`) adds the backward flow's picture 'vis_bwd' [H,W,3];
+    * `pred_bwd_flow`: every pair runs in swapped order (evaluate_flow.py:735-736), as in `infer_flow_video`; a
+      `concat_frame` picture still shows the pair's first frame, as the reference's `concat_flow_img` does.
 
     Sizes, transpose and rescale semantics are those of `infer_flow_video` (and `infer_flow`); the flows equal
     `infer_flow_video` on the whole sequence up to fp32 summation order.  `run(frames)` takes an iterable of host uint8 frames
@@ -1181,20 +1184,25 @@ class VideoFlowRunner(_SequenceRunner):
 
     def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
                  visualize=False, concat_frame=False, pred_bidir_flow=False, fwd_bwd_consistency_check=False,
-                 return_flow=True, **model_kwargs):
+                 return_flow=True, pred_bwd_flow=False, visualize_bwd=False, **model_kwargs):
         self.kw = dict(model_kwargs)
         _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "VideoFlowRunner")
         if concat_frame and not visualize:
             raise ValueError("concat_frame needs visualize=True")
+        if visualize_bwd and not (visualize and pred_bidir_flow):
+            raise ValueError("visualize_bwd needs visualize=True and pred_bidir_flow=True")
         if not return_flow and not visualize:
             raise ValueError("nothing to return: return_flow=False needs visualize=True")
         self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.check = bool(pred_bidir_flow), bool(fwd_bwd_consistency_check)
         self.visualize, self.concat, self.return_flow = bool(visualize), bool(concat_frame), bool(return_flow)
+        self.bwd, self.visualize_bwd = bool(pred_bwd_flow), bool(visualize_bwd)
         self.concat_axis = 0 if self.h < self.w else 1                                  # evaluate_flow.py:822
         self.carry_frame = torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev)
 
     def _match(self, slot, first, second):
+        if self.bwd:
+            first, second = second, first
         flow = self.model.forward_encoded(first, second, pred_bidir_flow=self.bidir, **self.kw)["flow_preds"][-1]
         out = _flow_outputs(flow, self.ori, self.size, self.transposed, self.bidir, self.check)
         if self.visualize:
@@ -1208,8 +1216,12 @@ class VideoFlowRunner(_SequenceRunner):
                 pics = flow_half = torch.empty((b, h, w, 3), dtype=torch.uint8, device=self.dev)
             flow_to_image(out["flow"], flow_half)
             out["vis"] = pics
+            if self.visualize_bwd:
+                out["vis_bwd"] = flow_to_image(out["flow_bwd"])
             if not self.return_flow:
                 del out["flow"]
+                if self.visualize_bwd:
+                    del out["flow_bwd"]
         self.carry_frame.copy_(self.dev_in[slot][-1:])
         return out
 

@@ -55,9 +55,9 @@ def png_bytes(scanlines, h, w, bit_depth, colour_type):
 
 
 def picture_scanlines(rgb):
-    """uint8 [H, W, 3] RGB -> unfiltered scanlines (filter byte 0 on every row)."""
+    """uint8 [H, W, 3] RGB (or [H, W] grey) -> unfiltered scanlines (filter byte 0 on every row)."""
     h = rgb.shape[0]
-    rows = np.empty((h, 1 + rgb.shape[1] * 3), dtype=np.uint8)
+    rows = np.empty((h, 1 + rgb[0].size), dtype=np.uint8)
     rows[:, 0] = 0
     rows[:, 1:] = rgb.reshape(h, -1)
     return rows.tobytes()
