@@ -303,6 +303,15 @@ int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, i
 int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,
                       int32_t h, int32_t w, void* stream);
 
+/* um_depth_to_image per item: depth i = fp32 [h_i, w_i] at depth + items[i].offset (numel floats in all) -> its RGB picture
+ * at out + 3 * items[i].offset bytes, rows of 3 w_i bytes.  Picture i is bit-identical to um_depth_to_image of depth i
+ * alone: the radix select runs over the item's own N_i = h_i w_i pixels (k = floor(0.95 (N_i - 1))), and the NaN, constant
+ * and vmax <= vmin rules are the same.  scratch: DEVICE buffer of 2056 * n 32-bit words, reset inside the call.  One
+ * memset and nine kernels, grids sized by the capacity (h_max, w_max).  Replaces viz_depth_tensor on each predicted depth
+ * of inference_depth for frames of different sizes (evaluate_depth.py:338-417). */
+int um_depth_to_image_ragged(const float* depth, int64_t numel, const um_ragged_item* items, uint8_t* out, void* scratch,
+                             int32_t n, int32_t h_max, int32_t w_max, void* stream);
+
 /* ---- leaderboard submission payloads -------------------------------------------------------------------------
  * One launch from the model's planar output pred = DEVICE fp32 [batch, C, h, w] at the inference size (C = 2 flow, 1
  * disparity) to each sample's file payload, without the header: sample i at out + i * sample_stride (bytes).  Geometry:

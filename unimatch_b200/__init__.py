@@ -28,6 +28,7 @@ _LAZY = {
     "StereoRunner": (".inference", "StereoRunner"),
     "MixedSizeStereoRunner": (".inference", "MixedSizeStereoRunner"),
     "MixedSizeFlowRunner": (".inference", "MixedSizeFlowRunner"),
+    "MixedSizeDepthRunner": (".inference", "MixedSizeDepthRunner"),
     "disparity_to_image": (".inference", "disparity_to_image"),
     "depth_to_image": (".inference", "depth_to_image"),
     "validate_flow": (".evaluation", "validate_flow"),
@@ -43,7 +44,7 @@ _LAZY = {
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
            "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "MixedSizeStereoRunner", "MixedSizeFlowRunner",
-           "disparity_to_image", "depth_to_image",
+           "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth"]
 

@@ -465,9 +465,9 @@ __device__ const uint8_t kInferno[768] = {
     138, 246, 243, 142, 248, 244, 146, 249, 245, 150, 250, 246, 154, 251, 248, 157, 252, 249, 161, 253, 250, 164, 255, 252,
 };
 
-// Where disparity image n and its picture lie: one size, contiguous disparities and strided pictures (DispUniform), or each
-// image at its own offset and size in a packed buffer, its picture at 3 * offset bytes with 3w-byte rows (DispRagged).
-// A ragged item that does not fit (ragged_ok) has hw = 0: it reads and writes nothing.
+// Where disparity (or depth) image n and its picture lie: one size, contiguous images and strided pictures (DispUniform), or
+// each image at its own offset and size in a packed buffer, its picture at 3 * offset bytes with 3w-byte rows (DispRagged).
+// A ragged item that does not fit (ragged_ok) has hw = 0: it reads and writes nothing.  The depth kernels share both.
 struct DispImage {
   const float* d;
   uint8_t* img;
@@ -624,15 +624,16 @@ __device__ __forceinline__ double p95_index(int hw) { return __dmul_rn(0.95, (do
 // p > 0 histograms byte 3 - p of the keys whose top p bytes equal rank k's prefix (bins 0-255) or else rank k+1's (bins
 // 256-511).  The loop bound is warp-uniform, so that a warp's equal bins are counted by one shared atomic
 // (__match_any_sync): a smooth depth map puts most of a warp into one bin, which would otherwise serialise the atomics.
-template <bool kFirst>
-__global__ void __launch_bounds__(256) depth_hist_kernel(const float* __restrict__ depth, unsigned* __restrict__ scratch,
-                                                         int hw, int pass) {
+template <bool kFirst, class Geo>
+__global__ void __launch_bounds__(256) depth_hist_kernel(Geo geo, unsigned* __restrict__ scratch, int pass) {
   __shared__ unsigned hist[2 * kDvBins];
   for (int i = threadIdx.x; i < 2 * kDvBins; i += blockDim.x) hist[i] = 0;
   const int n = blockIdx.y, lane = threadIdx.x & 31;
   unsigned* img = scratch + (long long)n * kDvWords;
   unsigned* st = img + kDvHistWords;
-  const float* d = depth + (long long)n * hw;
+  const DispImage im = geo.image(n);
+  const float* d = im.d;
+  const int hw = im.hw;
   const int shift = 32 - 8 * pass;                           // pass > 0: the prefix is the key's top 8 * pass bits
   const unsigned pa = kFirst ? 0u : st[kDvPrefA], pb = kFirst ? 0u : st[kDvPrefB];
   __syncthreads();
@@ -681,8 +682,12 @@ __global__ void __launch_bounds__(256) depth_hist_kernel(const float* __restrict
 
 // one CTA of 256 threads per image, thread t owning bin t: a block-wide scan of the pass's histogram finds the bins that
 // hold ranks k and k+1 and appends them to both prefixes.  After the last pass the prefixes are the keys a and b, and
-// thread 0 forms vmax, the fp32 divisor and the image's mode, each float64 / fp32 operation rounded on its own.
-__global__ void __launch_bounds__(256) depth_select_kernel(unsigned* __restrict__ scratch, int hw, int pass) {
+// thread 0 forms vmax, the fp32 divisor and the image's mode, each float64 / fp32 operation rounded on its own.  A skipped
+// ragged item (hw = 0) selects nothing.
+template <class Geo>
+__global__ void __launch_bounds__(256) depth_select_kernel(Geo geo, unsigned* __restrict__ scratch, int pass) {
+  const int hw = geo.image(blockIdx.x).hw;
+  if (hw == 0) return;
   unsigned* img = scratch + (long long)blockIdx.x * kDvWords;
   unsigned* st = img + kDvHistWords;
   const unsigned* h = img + pass * 2 * kDvBins;
@@ -725,9 +730,8 @@ __global__ void __launch_bounds__(256) depth_select_kernel(unsigned* __restrict_
 }
 
 // grid (x: CTAs over the pixels of one image, y: image); the floor table is staged in shared memory as in disp_color_kernel
-__global__ void __launch_bounds__(256) depth_color_kernel(const float* __restrict__ depth, const unsigned* __restrict__ scratch,
-                                                          uint8_t* __restrict__ out, int w, int hw, long long row_stride,
-                                                          long long image_stride) {
+template <class Geo>
+__global__ void __launch_bounds__(256) depth_color_kernel(Geo geo, const unsigned* __restrict__ scratch) {
   __shared__ uint8_t lut[768];
   for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kPlasma[i];
   __syncthreads();
@@ -735,8 +739,11 @@ __global__ void __launch_bounds__(256) depth_color_kernel(const float* __restric
   const unsigned* st = scratch + (long long)n * kDvWords + kDvHistWords;
   const unsigned mode = __ldg(st + kDvMode);
   const float vmin = key_float(~__ldg(st + kDvLo)), range = __uint_as_float(__ldg(st + kDvRange));
-  const float* d = depth + (long long)n * hw;
-  uint8_t* img = out + n * image_stride;
+  const DispImage im = geo.image(n);
+  const int w = im.w, hw = im.hw;
+  const long long row_stride = im.row_stride;
+  const float* d = im.d;
+  uint8_t* img = im.img;
   for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
     int i = mode == kDvFlat ? 0 : -1;                          // colour index, -1 = black
     if (mode == kDvNormal) {
@@ -826,6 +833,29 @@ inline int ew_grid(long long n, int block = 256) {
   long long g = (n + block - 1) / block;
   const long long cap = 132LL * 16;      // 132 SMs (H100 SXM) x 16 resident CTAs, grid-stride beyond that
   return (int)(g < cap ? (g > 0 ? g : 1) : cap);
+}
+
+// The memset and nine launches of um_depth_to_image(_ragged); `hw` sizes the grid (the capacity for a ragged batch).
+template <class Geo>
+int depth_to_image_launch(const Geo& geo, void* scratch, int n, long long hw, cudaStream_t st, const char* name) {
+  static_assert(kDvWords == 2056, "the header states the scratch size");
+  unsigned* words = reinterpret_cast<unsigned*>(scratch);
+  if (cudaMemsetAsync(scratch, 0, sizeof(unsigned) * kDvWords * n, st) != cudaSuccess) return um::check_launch(name);
+  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
+  long long bx = (hw + 1023) / 1024;                                                // 4 pixels per thread and pass
+  bx = bx < per_image ? bx : per_image;
+  const dim3 grid((unsigned)(bx > 0 ? bx : 1), (unsigned)n);
+  for (int pass = 0; pass < 4; ++pass) {
+    if (pass == 0) depth_hist_kernel<true><<<grid, 256, 0, st>>>(geo, words, pass);
+    else depth_hist_kernel<false><<<grid, 256, 0, st>>>(geo, words, pass);
+    if (int rc = um::check_launch(name)) return rc;
+    depth_select_kernel<<<(unsigned)n, 256, 0, st>>>(geo, words, pass);
+    if (int rc = um::check_launch(name)) return rc;
+  }
+  long long cx = (hw + 255) / 256;
+  cx = cx < 2 * per_image ? cx : 2 * per_image;
+  depth_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, words);
+  return um::check_launch(name);
 }
 
 }  // namespace
@@ -1022,27 +1052,18 @@ int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int6
   UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_depth_to_image: an image has at most 2^31 - 1 pixels");
   UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
              "um_depth_to_image: row_stride must cover 3*w bytes and image_stride h rows");
-  static_assert(kDvWords == 2056, "the header states the scratch size");
-  cudaStream_t st = (cudaStream_t)stream;
   const int hw = h * w;
-  unsigned* words = reinterpret_cast<unsigned*>(scratch);
-  if (cudaMemsetAsync(scratch, 0, sizeof(unsigned) * kDvWords * n, st) != cudaSuccess)
-    return um::check_launch("um_depth_to_image");
-  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
-  long long bx = ((long long)hw + 1023) / 1024;                                     // 4 pixels per thread and pass
-  bx = bx < per_image ? bx : per_image;
-  const dim3 grid((unsigned)(bx > 0 ? bx : 1), (unsigned)n);
-  for (int pass = 0; pass < 4; ++pass) {
-    if (pass == 0) depth_hist_kernel<true><<<grid, 256, 0, st>>>(depth, words, hw, pass);
-    else depth_hist_kernel<false><<<grid, 256, 0, st>>>(depth, words, hw, pass);
-    if (int rc = um::check_launch("um_depth_to_image")) return rc;
-    depth_select_kernel<<<(unsigned)n, 256, 0, st>>>(words, hw, pass);
-    if (int rc = um::check_launch("um_depth_to_image")) return rc;
-  }
-  long long cx = ((long long)hw + 255) / 256;
-  cx = cx < 2 * per_image ? cx : 2 * per_image;
-  depth_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(depth, words, out, w, hw, row_stride, image_stride);
-  return um::check_launch("um_depth_to_image");
+  const DispUniform geo{depth, out, w, hw, row_stride, image_stride};
+  return depth_to_image_launch(geo, scratch, n, hw, (cudaStream_t)stream, "um_depth_to_image");
+}
+
+int um_depth_to_image_ragged(const float* depth, int64_t numel, const um_ragged_item* items, uint8_t* out, void* scratch,
+                             int32_t n, int32_t h_max, int32_t w_max, void* stream) {
+  UM_REQUIRE(depth && items && out && scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && numel > 0,
+             "um_depth_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
+  UM_REQUIRE((long long)h_max * w_max <= 0x7fffffffLL, "um_depth_to_image_ragged: an image has at most 2^31 - 1 pixels");
+  const DispRagged geo{depth, out, items, h_max, w_max, numel};
+  return depth_to_image_launch(geo, scratch, n, (long long)h_max * w_max, (cudaStream_t)stream, "um_depth_to_image_ragged");
 }
 
 int um_encode_submission(const float* pred, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t geometry,

@@ -17,11 +17,13 @@ until the single download at the end; the flow and stereo drivers issue no other
 synchronises once per batch for its `torch.inverse`).  The metrics are then formed on the host in float64, following each
 reference loop -- including its quirks, listed in each driver's docstring.
 """
+import os
+
 import numpy as np
 import torch
 
 from . import ops
-from .inference import InputPadder, _resize
+from .inference import InputPadder, _resize, depth_to_image
 
 _OPS = torch.ops.unimatch_sm100
 
@@ -54,10 +56,11 @@ def _download(table):
     return host.numpy()
 
 
-def _statistics(samples, batch, device, run, columns):
+def _statistics(samples, batch, device, run, columns, on_batch=None):
     """Per-sample statistics table [N, columns] (float64, dataset order) of `samples`, an iterable of tuples of CPU tensors
     (None for an absent optional tensor) grouped by the shape of their first tensor into batches of `batch`; `run(*tensors)`
-    gets each batch stacked on the device and returns its [n, columns] device table."""
+    gets each batch stacked on the device and returns its [n, columns] device table.  `on_batch(indices, table)`, when
+    given, follows each `run` with the batch's dataset indices and its device table."""
     if batch < 1:
         raise ValueError("batch must be positive")
     device = torch.device(device)
@@ -69,6 +72,8 @@ def _statistics(samples, batch, device, run, columns):
                   for k in range(len(items[0][1]))]
         tables.append(run(*fields))
         order.extend(i for i, _ in items)
+        if on_batch is not None:
+            on_batch([i for i, _ in items], tables[-1])
 
     for i, fields in enumerate(samples):
         fields = tuple(None if f is None else torch.as_tensor(f) for f in fields)
@@ -227,10 +232,34 @@ def _stereo_results(T, protocol):
 
 
 # --------------------------------------------------------------------------------------------------------------- depth
+class _DepthVisNames:
+    """The file names `save_vis_depth` gives the samples (evaluate_depth.py:133-138, :272-276): the reference's
+    `valid_samples` numbering, 1-based over the samples with a non-empty mask in dataset order, as `%04d_depth_pred.png`
+    (scannet) or `%04d.png` (demon).  Batches arrive grouped by size, so out of dataset order: `add(indices, counts)` takes
+    a batch's dataset indices and mask counts and returns the [(index, name)] whose number is now known, in dataset
+    order; an empty-mask sample gets no name."""
+
+    def __init__(self, protocol):
+        self.pattern = "%04d_depth_pred.png" if protocol == "scannet" else "%04d.png"
+        self.counts = {}
+        self.next_index = 0
+        self.valid_samples = 0
+
+    def add(self, indices, counts):
+        self.counts.update(zip(indices, counts))
+        named = []
+        while self.next_index in self.counts:
+            if self.counts.pop(self.next_index) > 0:
+                self.valid_samples += 1
+                named.append((self.next_index, self.pattern % self.valid_samples))
+            self.next_index += 1
+        return named
+
+
 @torch.no_grad()
 def validate_depth(model, dataset, *, protocol, batch=8, device="cuda", padding_factor=16, inference_size=None,
                    num_depth_candidates=64, eval_min_depth=0.5, eval_max_depth=10, min_depth=0.5, max_depth=10,
-                   **model_kwargs):
+                   save_vis_depth=False, save_dir=None, writers=4, **model_kwargs):
     """The results dict of evaluate_depth.py's `validate_<protocol>` on `dataset` (`protocol` 'scannet' or 'demon', the same
     loop): abs_rel, sq_rel, rmse, rmse_log, a1, a2, a3 of loss/depth_loss.py:compute_errors.  Inputs are padded with
     InputPadder mode 'kitti', or resized to `inference_size` with the depth resized back (not rescaled, as in the reference).
@@ -238,11 +267,20 @@ def validate_depth(model, dataset, *, protocol, batch=8, device="cuda", padding_
     their inverses.
 
     Kept quirk: samples with an empty mask are skipped, but the per-sample metrics are summed and divided by the number of
-    samples in the dataset, skipped ones included (evaluate_depth.py:148)."""
+    samples in the dataset, skipped ones included (evaluate_depth.py:148).
+
+    `save_vis_depth` writes, into `save_dir` (created if missing), the `viz_depth_tensor(1 / depth)` picture of every
+    sample with a non-empty mask, named as the reference names it (`_DepthVisNames`).  The pictures are painted on the
+    device (`depth_to_image`) from the unpadded or resized-back predictions the metrics are computed from, downloaded with
+    the batch's mask counts (one wait per batch) and written by `writers` threads.  Without it the driver does exactly what
+    it does otherwise."""
     if protocol not in _DEPTH_PROTOCOLS:
         raise ValueError("validate_depth: protocol must be one of %s" % list(_DEPTH_PROTOCOLS))
     if model_kwargs.setdefault("task", "depth") != "depth":
         raise ValueError("validate_depth drives the depth task only")
+    if save_vis_depth and save_dir is None:
+        raise ValueError("validate_depth: save_vis_depth needs save_dir")
+    pictures = []                                        # the last batch's device pictures, with save_vis_depth
 
     def run(img_ref, img_tgt, intrinsics, pose, depth, valid):
         ori = tuple(img_ref.shape[-2:])
@@ -255,10 +293,36 @@ def validate_depth(model, dataset, *, protocol, batch=8, device="cuda", padding_
         pred = model(img_ref, img_tgt, intrinsics=intrinsics, pose=pose, min_depth=1. / max_depth, max_depth=1. / min_depth,
                      num_depth_candidates=num_depth_candidates, **model_kwargs)["flow_preds"][-1]
         pred = padder.unpad(pred) if inference_size is None else _resize(pred.unsqueeze(1), ori).squeeze(1)
+        if save_vis_depth:
+            pictures[:] = [depth_to_image(pred)]
         return _OPS.eval_stats(pred, depth, valid, None, ops.EVAL_DEPTH, 0, 0.0, float(eval_min_depth), float(eval_max_depth))
 
     fields = ("img_ref", "img_tgt", "intrinsics", "pose", "depth", "valid")
-    T = _statistics((tuple(s[k] for k in fields) for s in dataset), batch, device, run, len(ops.EVAL_DEPTH_COLS))
+    samples = (tuple(s[k] for k in fields) for s in dataset)
+    if not save_vis_depth:
+        T = _statistics(samples, batch, device, run, len(ops.EVAL_DEPTH_COLS))
+        return _depth_results(T)
+    from .submission import _WriterPool, _write_picture
+    os.makedirs(save_dir, exist_ok=True)
+    names, held = _DepthVisNames(protocol), {}
+    pool = _WriterPool(writers, torch.device(device).type == "cuda")
+
+    def on_batch(indices, table):
+        slot, host, ready = pool.stage({"vis": pictures.pop(), "n": table[:, _col(ops.EVAL_DEPTH, "n")]})
+        if ready is not None:
+            ready.synchronize()
+        for i, n, pic in zip(indices, host["n"], host["vis"]):
+            if n > 0:
+                held[i] = pic.copy()                    # the staging slot is reused two batches later
+        for i, name in names.add(indices, host["n"]):
+            pool.submit(slot, None, _write_picture, os.path.join(save_dir, name), held.pop(i))
+
+    try:
+        T = _statistics(samples, batch, device, run, len(ops.EVAL_DEPTH_COLS), on_batch)
+    except BaseException as e:
+        pool.close(error=e)
+        raise
+    pool.close()
     return _depth_results(T)
 
 

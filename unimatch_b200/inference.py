@@ -16,8 +16,8 @@ Video (`main_flow.py --inference_video`, evaluate_flow.py:642-831): `infer_flow_
 sequence with every frame encoded ONCE (pair (t, t+1) and pair (t+1, t+2) share frame t+1's feature pyramid; the encoder is
 per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 summation order), `VideoFlowRunner` streams host uint8 frames through the same
 path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
-colouring of utils/flow_viz.py on the device.  Writing videos (mp4) stays out of scope; the leaderboard files (.flo, PNG,
-PFM) are written by `submission.py`, and the plain inference commands' files (decoding included) by `inference_io.py`.
+colouring of utils/flow_viz.py on the device.  The leaderboard files (.flo, PNG, PFM) are written by `submission.py`,
+and the plain inference commands' files (decoding and the `save_video` mp4 included) by `inference_io.py`.
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
@@ -40,6 +40,11 @@ transpose back, the forward-backward occlusion check and the Middlebury colourin
 device descriptor table (`um_frames_to_planar_ragged`, `um_resize_bilinear_ragged`, `um_fb_consistency_ragged`,
 `um_flow_to_image_ragged`).  It shares its buckets, graphs, packing and statistics with `MixedSizeStereoRunner`
 (`_MixedSizeRunner`).
+
+Posed depth pairs of mixed sizes (`inference_depth`, evaluate_depth.py:338-417, which takes each pair at its own size):
+`MixedSizeDepthRunner` streams host (frame t, frame t+1, relative pose) items, batched by frame t's inference size, through
+the same machinery; the conversion, the resize back and the colouring (`um_depth_to_image_ragged`) read each frame's size
+from the descriptor table.
 """
 import collections
 import itertools
@@ -726,7 +731,7 @@ class _MixedSizeRunner(_PipelinedRunner):
     the used prefixes are downloaded; `(index, result)` in completion order; `stats`.
 
     A subclass provides `_bucket(pair)` (the size the model sees), `_frame_order(pairs)` (the step's frames in the order they
-    are packed), `_layout(sizes, size)` (the step's descriptor table as one record array, the used elements of each output
+    are packed), `_layout(sizes, size)` (`sizes` as `_sizes(pairs)` gives them) (the step's descriptor table as one record array, the used elements of each output
     buffer, and per real pair its result views as (key, buffer, offset, shape)) and `_step(slot, size)` (the device work on
     `dev_in[slot]` / `dev_desc[slot]`, returning {buffer: packed device tensor})."""
 
@@ -770,6 +775,11 @@ class _MixedSizeRunner(_PipelinedRunner):
         checked = ((i, self._pair(p)) for i, p in items)
         return _batches(checked, self.batch, lambda s: self._bucket(s[1]), self.max_buckets)
 
+    @staticmethod
+    def _sizes(pairs):
+        """what `_layout` takes of each pair: its size (both frames of a pair share it)"""
+        return [tuple(p[0].shape[:2]) for p in pairs]
+
     def _table(self, sizes, size):
         table, used, results = self._layout(sizes, size)
         return table.view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES), used, results
@@ -778,7 +788,7 @@ class _MixedSizeRunner(_PipelinedRunner):
         """the step's packed frames and descriptor table into pinned memory, then their H2D copies (used bytes only)"""
         pairs = [p for _, p in chunk]
         size = self._bucket(pairs[0])
-        table, used, results = self._table([tuple(p[0].shape[:2]) for p in pairs], size)
+        table, used, results = self._table(self._sizes(pairs), size)
         nbytes = 0
         for f in self._frame_order(pairs):
             self.pin[slot][nbytes:nbytes + f.numel()].copy_(f.reshape(-1))
@@ -1300,3 +1310,171 @@ class DepthSequenceRunner(_SequenceRunner):
         self.pose_pin[slot].copy_(torch.from_numpy(_relative_poses(poses, self.bidir)))
         self.prev_pose = poses[-1]
         self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
+
+
+def _depth_step_layout(sizes, batch, pred_bidir_depth):
+    """Descriptor tables of one depth step of `batch` pairs, whose real pairs have the frame sizes `sizes` = [((h, w) of
+    frame t, (h, w) of frame t+1)] (1 <= len <= batch).  Returns (frames, outputs, frame_bytes, used, results):
+    * frames: 2*batch items over the packed uint8 frames -- the real pairs' frames t back to back, then their frames t+1,
+      each at its own size; the items of a short step's filler pairs point at its last pair's frames;
+    * outputs: batch items ('depth'), or 2*batch with `pred_bidir_depth` ('depth', then 'depth_bwd'), packed back to back,
+      each at the size of its pair's frame t with scale 1 (depth is not rescaled with the resize); fillers are empty items,
+      which the kernels skip;
+    * frame_bytes / used: the used prefixes of the packed frames and depths;
+    * results: per real pair, the (key, offset, h, w) of each of its outputs."""
+    n = len(sizes)
+    frames = np.zeros(2 * batch, RAGGED_ITEM)
+    off = 0
+    for k in range(2):
+        for i, pair in enumerate(sizes):
+            h, w = pair[k]
+            frames[k * batch + i] = (off, h, w, 1.0, 0)
+            off += 3 * h * w
+        frames[k * batch + n:(k + 1) * batch] = frames[k * batch + n - 1]
+    keys = ("depth", "depth_bwd") if pred_bidir_depth else ("depth",)
+    outputs = np.zeros(len(keys) * batch, RAGGED_ITEM)
+    results = [[] for _ in sizes]
+    used = 0
+    for k, key in enumerate(keys):
+        for i, ((h, w), _) in enumerate(sizes):
+            outputs[k * batch + i] = (used, h, w, 1.0, 0)
+            results[i].append((key, used, h, w))
+            used += h * w
+    return frames, outputs, off, used, results
+
+
+class MixedSizeDepthRunner(_MixedSizeRunner):
+    """Streaming depth over posed pairs of ANY size up to `max_frame_size`: `inference_depth` (evaluate_depth.py:338-417),
+    which takes each pair at its own size, as a stream.  Each item is one pair (uint8 frame t [h, w, 3], uint8 frame t+1
+    [h', w', 3], relative pose [4, 4]); the relative pose is the reference's host float32 `inv(pose[t+1]) @ pose[t]`, as
+    `_relative_poses` computes it, and with `pred_bidir_depth` its inverse is appended on the host.
+
+    * buckets: a pair's bucket is the size the model sees, frame t's size rounded up to a multiple of `padding_factor`, or
+      `inference_size` (depth has no portrait rule); steps are formed as in `MixedSizeStereoRunner` (`_batches`, at most
+      `max_buckets` open);
+    * upload: the step's frames t, then its frames t+1, packed back to back as uint8 (the used bytes only), the descriptor
+      table and the step's relative poses, on a side stream while the previous step computes;
+    * device work of a step, one CUDA graph per bucket and staging slot: `um_frames_to_planar_normalized_ragged` (every frame
+      normalised and resized from its own size to the bucket's, so frame t+1 follows frame t's inference size), the encoder
+      and the depth matching path, `um_resize_bilinear_ragged` back to frame t's size with scale 1, and with `visualize`
+      `um_depth_to_image_ragged`.  The intrinsics [3, 3] are not rescaled with the frames, as in the reference; the camera
+      operands are built once per staging slot before any capture, on static pose buffers the upload fills, and shared by
+      every bucket (they do not depend on the size);
+    * download: only the used prefixes of the packed depths and pictures.
+
+    Every pair encodes both of its frames: frame t+1 is seen at frame t's inference size and again at its own, so the
+    encode-once path of `DepthSequenceRunner` does not hold in general.  A directory of one frame size is better served
+    by that runner.  `run(items)` yields (index, result) as steps complete -- completion order, not input order; `index`
+    is the pair's position in the input, each exactly once.  `result` holds CPU views 'depth' [h, w] (+ 'depth_bwd') at
+    frame t's size and, with `visualize`, the uint8 RGB pictures 'vis' [h, w, 3] (+ 'vis_bwd') of `depth_to_image`;
+    `return_depth=False` with `visualize` sends back only the pictures.  The views point into reused pinned staging -- copy
+    what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
+
+    def __init__(self, model, max_frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None,
+                 min_depth=0.5, max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
+                 visualize=False, return_depth=True, use_graph=True, max_buckets=4, **model_kwargs):
+        if not return_depth and not visualize:
+            raise ValueError("nothing to return: return_depth=False needs visualize=True")
+        self.kw = _depth_task_kwargs(dict(model_kwargs), "MixedSizeDepthRunner")
+        K = _intrinsics33(intrinsics, "MixedSizeDepthRunner")
+        self.padding_factor, self.inference_size = padding_factor, inference_size
+        self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
+        self.visualize, self.return_depth = bool(visualize), bool(return_depth)
+        self.inv_range = (1.0 / max_depth, 1.0 / min_depth)                      # the model works on inverse depth
+        views = 2 if self.bidir else 1
+        buffers = {}
+        if self.return_depth:
+            buffers["depth"] = (torch.float32, views)
+        if self.visualize:
+            buffers["vis"] = (torch.uint8, 3 * views)
+        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), buffers)
+        npose = views * self.batch
+        self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
+        self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
+        Kb = K.to(self.dev)[None].repeat(self.batch, 1, 1)
+        # cams[slot]["pose"] IS pose_dev[slot] (a float32 pose of 2B matrices is taken as it is), so the upload updates it
+        self.cams = [model.depth_cameras(Kb, self.pose_dev[s], model.upsample_factor, *self.inv_range, num_depth_candidates,
+                                         self.bidir) for s in range(2)]
+
+    # ---- host side
+    def _pair(self, pair):
+        name = type(self).__name__
+        if len(pair) != 3:
+            raise ValueError("%s: an item is (frame t, frame t+1, relative pose)" % name)
+        frames = tuple(torch.as_tensor(f) for f in pair[:2])
+        for f in frames:
+            if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+                raise ValueError("%s: frames must be uint8 [h, w, 3]" % name)
+            if not (1 <= f.shape[0] <= self.hmax and 1 <= f.shape[1] <= self.wmax):
+                raise ValueError("%s: a %dx%d frame exceeds max_frame_size %dx%d"
+                                 % (name, f.shape[0], f.shape[1], self.hmax, self.wmax))
+        return frames + (_pose44(pair[2], name),)
+
+    def _bucket(self, pair):
+        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+
+    @staticmethod
+    def _sizes(pairs):
+        return [(tuple(p[0].shape[:2]), tuple(p[1].shape[:2])) for p in pairs]
+
+    @staticmethod
+    def _frame_order(pairs):
+        """the step's frames t, then its frames t+1"""
+        return [p[0] for p in pairs] + [p[1] for p in pairs]
+
+    def _layout(self, sizes, size):
+        frames, outputs, _, used, results = _depth_step_layout(sizes, self.batch, self.bidir)
+        views = []
+        for outs in results:
+            views.append([])
+            for key, off, h, w in outs:
+                if self.return_depth:
+                    views[-1].append((key, "depth", off, (h, w)))
+                if self.visualize:
+                    views[-1].append((key.replace("depth", "vis"), "vis", 3 * off, (h, w, 3)))
+        return np.concatenate((frames, outputs)), {"depth": used, "vis": 3 * used}, views
+
+    def _poses(self, pairs):
+        """the step's relative poses, a short step's last one repeated, then with `pred_bidir_depth` their inverses
+        (np.linalg.inv in float32, as `_relative_poses` forms them): float32 [views * batch, 4, 4]"""
+        rel = [pairs[min(i, len(pairs) - 1)][2] for i in range(self.batch)]
+        if self.bidir:
+            rel += [np.linalg.inv(r) for r in rel]
+        return np.stack(rel).astype(np.float32)
+
+    def _stage_host(self, slot, chunk):
+        """the packed frames and the table (`_MixedSizeRunner`), then the step's relative poses"""
+        super()._stage_host(slot, chunk)
+        self.pose_pin[slot].copy_(torch.from_numpy(self._poses([p for _, p in chunk])))
+        self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
+        self.stats["h2d_bytes"] += self.pose_pin[slot].nbytes
+
+    # ---- device side
+    def _reset_inputs(self, slot):
+        """zero frames, a full-capacity table and identity poses: valid for any bucket"""
+        cap = (self.hmax, self.wmax)
+        table, _, _ = self._table([(cap, cap)] * self.batch, cap)
+        self.dev_in[slot].zero_()
+        self.dev_desc[slot].copy_(torch.from_numpy(table))
+        self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
+
+    def _step(self, slot, size):
+        b = self.batch
+        items = self.dev_desc[slot]
+        x = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:2 * b], self.hmax, self.wmax, int(size[0]),
+                                                    int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
+        feats = self.model.encode_frames(x, task="depth")
+        depth = self.model.forward_encoded([f[:b] for f in feats], [f[b:] for f in feats], task="depth",
+                                           cameras=self.cams[slot], min_depth=self.inv_range[0], max_depth=self.inv_range[1],
+                                           depth_from_argmax=self.from_argmax, pred_bidir_depth=self.bidir,
+                                           **self.kw)["flow_preds"][-1]                     # [views * b, H, W]
+        out_items = items[2 * b:]
+        packed = _OPS.resize_bilinear_ragged(depth.contiguous().view(depth.shape[0], 1, *depth.shape[-2:]), out_items,
+                                             self.hmax, self.wmax, out_items.shape[0] * self.hmax * self.wmax)
+        out = {}
+        if self.return_depth:
+            out["depth"] = packed
+        if self.visualize:
+            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
+            _OPS.depth_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
+        return out

@@ -6,19 +6,23 @@ writing the same files, with the pairs streamed through the runners.
     main_flow.inference_flow = unimatch_b200.inference_flow     # then main_flow.main(args) as usual
 
 Each driver takes the reference function's keyword arguments (so `main_*.py` calls it unchanged) and a few of its own with
-defaults: `batch` (pairs per device step), `device`, `readers` (decode threads), `writers` (file-writer threads) and, for
-flow and stereo, `max_buckets` (inference sizes whose CUDA graphs are kept).  It returns a statistics dict (the reference
+defaults: `batch` (pairs per device step), `device`, `readers` (decode threads), `writers` (file-writer threads) and
+`max_buckets` (inference sizes whose CUDA graphs are kept).  It returns a statistics dict (the reference
 returns None): pairs, steps, bytes copied each way, and the summed busy seconds of the reader and writer threads.
 
 * Reading: files are listed exactly as the reference lists them and decoded as it decodes them, on `readers` threads in
   input order, up to `readers + 2 * batch` items ahead of the runner (PIL and cv2 release the GIL while decoding).  A video
   is decoded by cv2 on one reader thread, frame after frame.
 * Device work: `MixedSizeFlowRunner` (a directory: pairs of any size and orientation), `VideoFlowRunner` (a video: every
-  frame encoded once), `MixedSizeStereoRunner` and `DepthSequenceRunner`, each with its pictures painted on the device.
+  frame encoded once), `MixedSizeStereoRunner`, and `DepthSequenceRunner` (a depth directory of one frame size: every
+  frame encoded once) or `MixedSizeDepthRunner` (frames of several sizes), each with its pictures painted on the device.
 * Writing: the runners hand out views of pinned staging that later steps reuse, so the main thread copies each result into
   its file layout (PNG scanlines, `.flo` interleaved u / v, `.pfm` rows bottom to top) and the `submission._WriterPool`
   threads deflate and write.  Every `batch` pairs the pool waits for the jobs of the group before last, so at most two
   groups of copies are held; a writer's error is raised in the caller, and every file is complete when the driver returns.
+  `inference_flow(save_video=True)` encodes its mp4 with cv2's `mp4v` (MPEG-4 Part 2) on one ordered writer thread.  The
+  reference writes H.264 through imageio / libx264, which this package does not depend on (and cv2's own builds often
+  cannot encode H.264), so the video's pixels match the pictures up to the codec's loss, not the reference's bitstream.
 
 Deliberate difference: the reference's `inference_flow` never resets its transpose flag (evaluate_flow.py:675, :714-717,
 :757-758), so after the first portrait pair it transposes every later flow back, landscape ones included, and writes
@@ -35,8 +39,8 @@ import numpy as np
 import torch
 from PIL import Image
 
-from .inference import (DepthSequenceRunner, MixedSizeFlowRunner, MixedSizeStereoRunner, VideoFlowRunner, _flow_outputs,
-                        _inference_size, _resize, flow_to_image)
+from .inference import (DepthSequenceRunner, MixedSizeDepthRunner, MixedSizeFlowRunner, MixedSizeStereoRunner,
+                        VideoFlowRunner, _flow_outputs, _inference_size, _relative_poses, _resize, flow_to_image)
 from .submission import _WriterPool, _write, _write_png, flo_header, pfm_header, picture_scanlines
 
 # result key of the runner -> (file name suffix, encoding), in the order the reference writes them
@@ -224,9 +228,63 @@ def _job(path, x, encoding):
     return (_write_png, path, picture_scanlines(a), a.shape[0], a.shape[1], 8, colour)
 
 
-def _write_results(results, names, writers, group):
-    """Writes every (index, result) of `results`, `names(index)` giving {key: (path, encoding)}; returns the writers'
-    summed busy seconds."""
+def video_frame(rgb):
+    """A picture [H, W, 3] RGB as `cv2.VideoWriter` takes it: a BGR copy, with an odd height or width made even by
+    repeating the last row or column (mp4v drops an odd last row or column)."""
+    a = np.asarray(rgb)[..., ::-1]
+    h, w = a.shape[:2]
+    if h % 2 or w % 2:
+        a = np.pad(a, ((0, h % 2), (0, w % 2), (0, 0)), mode="edge")
+    return np.ascontiguousarray(a)
+
+
+def video_name(inference_video, concat_flow_img):
+    """The reference's video file name (evaluate_flow.py:815-816)."""
+    return os.path.basename(inference_video)[:-4] + ("_flow_img.mp4" if concat_flow_img else "_flow.mp4")
+
+
+class _VideoWriter:
+    """The frames of one mp4 (cv2.VideoWriter, fourcc mp4v, at `fps`), written in order by one thread.  `submit` copies
+    the picture (a view of reused staging) on the caller's thread; at most `ahead` frames wait for the writer."""
+
+    def __init__(self, path, fps, ahead=16):
+        self.path, self.fps, self.ahead = path, float(fps), int(ahead)
+        self.pool = ThreadPoolExecutor(1, thread_name_prefix="video-writer")
+        self.pending = collections.deque()
+        self.writer, self.busy_s, self.frames = None, 0.0, 0
+
+    def _write(self, frame):
+        t0 = time.perf_counter()
+        self.writer.write(frame)
+        return time.perf_counter() - t0
+
+    def submit(self, rgb):
+        import cv2
+        frame = video_frame(rgb)
+        if self.writer is None:
+            self.writer = cv2.VideoWriter(self.path, cv2.VideoWriter_fourcc(*"mp4v"), self.fps, (frame.shape[1], frame.shape[0]))
+            if not self.writer.isOpened():
+                raise RuntimeError("cannot open %s for writing with the mp4v codec" % self.path)
+        self.pending.append(self.pool.submit(self._write, frame))
+        self.frames += 1
+        while len(self.pending) > self.ahead:
+            self.busy_s += self.pending.popleft().result()
+
+    def close(self, error=None):
+        """Finish the file; re-raise a writer error unless the caller is already raising one."""
+        try:
+            if error is None:
+                while self.pending:
+                    self.busy_s += self.pending.popleft().result()
+        finally:
+            self.pool.shutdown(wait=True, cancel_futures=error is not None)
+            if self.writer is not None:
+                self.writer.release()
+
+
+def _write_results(results, names, writers, group, video=None):
+    """Writes every (index, result) of `results`, `names(index)` giving {key: (path, encoding)}, and with `video` each
+    result's 'vis' as the next frame of that `_VideoWriter`; returns the writers' summed busy seconds."""
     pool = _WriterPool(writers, False)
     slot = pool.stage({})[0]
     n = 0
@@ -234,13 +292,20 @@ def _write_results(results, names, writers, group):
         for index, r in results:
             for key, (path, encoding) in names(index).items():
                 pool.submit(slot, None, *_job(path, r[key], encoding))
+            if video is not None:
+                video.submit(r["vis"])
             n += 1
             if n % group == 0:
                 slot = pool.stage({})[0]       # waits for the jobs of the group before last
     except BaseException as e:
         pool.close(error=e)
+        if video is not None:
+            video.close(error=e)
         raise
     pool.close()
+    if video is not None:
+        video.close()
+        return pool.busy_s + video.busy_s
     return pool.busy_s
 
 
@@ -276,11 +341,14 @@ def inference_flow(model, inference_dir=None, inference_video=None, output_path=
     `_pred.flo` (+ `_pred_bwd.flo`); `<stem>` is the first frame's name without its extension.  Pictures are coloured from
     the flow as written, resized and transposed back.
 
-    `save_video` (an mp4 through imageio, which this package does not depend on) is refused; `concat_flow_img` only
-    shapes that video and is ignored.  Unlike the reference, a pair is transposed back only when it is itself portrait
-    (see the module docstring)."""
-    if save_video:
-        raise ValueError("inference_flow: save_video writes an mp4 through imageio, which unimatch_b200 does not depend on")
+    `save_video` (a video only) writes `<video name>_flow.mp4` instead of the `_flow.png` pictures, or with
+    `concat_flow_img` `<video name>_flow_img.mp4` of each pair's first frame and its picture side by side (stacked
+    vertically for landscape frames), at the input's frame rate; the other files are written as without it.  The mp4 is
+    encoded by cv2 with fourcc `mp4v` (MPEG-4 Part 2), not H.264 through imageio as the reference does, so its frames
+    equal the pictures up to that codec's loss; an odd height or width is made even by repeating the last row or column.
+    Unlike the reference, a pair is transposed back only when it is itself portrait (see the module docstring)."""
+    if save_video and inference_video is None:
+        raise ValueError("inference_flow: save_video needs inference_video")
     if fwd_bwd_consistency_check and not pred_bidir_flow:
         raise ValueError("inference_flow: fwd_bwd_consistency_check needs pred_bidir_flow=True")
     if (inference_dir is None) == (inference_video is None):
@@ -294,8 +362,13 @@ def inference_flow(model, inference_dir=None, inference_video=None, output_path=
     os.makedirs(output_path, exist_ok=True)
     if inference_video is not None:
         rd = _Readers(1, readers + 2 * batch)          # cv2 decodes a video frame after frame
+        video = None
+        if save_video:
+            keys.remove("vis")
+            video = (os.path.join(output_path, video_name(inference_video, concat_flow_img)), _video_fps(inference_video),
+                     bool(concat_flow_img))
         return _video_flow(model, _video_frames(inference_video, rd), output_path, keys, return_flow, pred_bwd_flow, batch,
-                           device, writers, kw, rd)
+                           device, writers, kw, rd, video)
     files = flow_inputs(inference_dir)
     if len(files) < 2:
         return _stats({"pairs": 0, "steps": 0, "h2d_bytes": 0, "d2h_bytes": 0}, rd, 0.0)
@@ -354,19 +427,36 @@ def _flow_pair_alone(model, file1, file2, device, pred_bwd_flow, kw, moved):
     return out
 
 
-def _video_flow(model, frames, output_path, keys, return_flow, pred_bwd_flow, batch, device, writers, kw, rd):
-    """The video branch of `inference_flow` on a stream of RGB uint8 frames [H, W, 3] (all of one size)."""
+def _video_fps(path):
+    """CAP_PROP_FPS of the video, as utils/file_io.py:203-210 reads it; read before any device work, so that `save_video`
+    on a video cv2 cannot open is refused at once"""
+    import cv2
+    cap = cv2.VideoCapture(path)
+    try:
+        if not cap.isOpened():
+            raise ValueError("inference_flow: save_video cannot open the video %s to read its frame rate (cv2 reads it, and "
+                             "cv2 with fourcc mp4v, not imageio as in the reference, writes the flow video)" % path)
+        return cap.get(cv2.CAP_PROP_FPS)
+    finally:
+        cap.release()
+
+
+def _video_flow(model, frames, output_path, keys, return_flow, pred_bwd_flow, batch, device, writers, kw, rd, video=None):
+    """The video branch of `inference_flow` on a stream of RGB uint8 frames [H, W, 3] (all of one size); `video`: (path,
+    fps, concat_flow_img) of the mp4 that `save_video` writes."""
     frames = iter(frames)
     first = next(frames, None)
     if first is None:
         return _stats({"pairs": 0, "steps": 0, "h2d_bytes": 0, "d2h_bytes": 0}, rd, 0.0)
     model.eval()
+    concat = video is not None and video[2]
     runner = VideoFlowRunner(model, first.shape[:2], batch, device, visualize=True, return_flow=return_flow,
-                             pred_bwd_flow=pred_bwd_flow, visualize_bwd=kw["pred_bidir_flow"], **kw)
+                             pred_bwd_flow=pred_bwd_flow, visualize_bwd=kw["pred_bidir_flow"], concat_frame=concat, **kw)
     names = _named(FLOW_FILES, keys, output_path, lambda t: flow_prefix(None, t, True))
     count = itertools.count()
     results = ((next(count), r) for r in runner.run(itertools.chain([first], frames)))
-    writer_s = _write_results(results, names, writers, batch)
+    writer = _VideoWriter(video[0], video[1], 2 * batch) if video is not None else None
+    writer_s = _write_results(results, names, writers, batch, writer)
     return _stats(_sequence_stats(runner, next(count)), rd, writer_s)
 
 
@@ -407,20 +497,27 @@ def inference_stereo(model, inference_dir=None, inference_dir_left=None, inferen
 def inference_depth(model, inference_dir=None, output_path="output", padding_factor=16, inference_size=None, attn_type="swin",
                     attn_splits_list=None, prop_radius_list=None, num_reg_refine=1, num_depth_candidates=64, min_depth=0.5,
                     max_depth=10, depth_from_argmax=False, pred_bidir_depth=False, batch=8, device="cuda", readers=4,
-                    writers=8):
+                    writers=8, max_buckets=4):
     """`evaluate_depth.inference_depth` on a ScanNet-layout directory: the consecutive pairs of color/*.jpg|png with the
-    relative poses of pose/*.txt and the first intrinsic/*.txt (4x4, its [:3, :3]), through
-    `DepthSequenceRunner(visualize=True, return_depth=False)`.  Writes `<stem>.png`, the `viz_depth_tensor(1 / depth)`
-    picture, and with `pred_bidir_depth` `<stem>_bwd.png`; `<stem>` is the reference frame's name without its extension.
-    The intrinsics are not rescaled when the frames are resized, as in the reference.  The runner takes one frame size,
-    so a directory whose frames differ in size is refused."""
+    relative poses of pose/*.txt and the first intrinsic/*.txt (4x4, its [:3, :3]).  Writes `<stem>.png`, the
+    `viz_depth_tensor(1 / depth)` picture, and with `pred_bidir_depth` `<stem>_bwd.png`; `<stem>` is the reference frame's
+    name without its extension.  The intrinsics are not rescaled when the frames are resized, as in the reference.
+
+    A directory of one frame size runs through `DepthSequenceRunner(visualize=True, return_depth=False)`, every frame
+    encoded once.  Frames of several sizes run pair by pair through `MixedSizeDepthRunner` (`max_frame_size` from the
+    image headers, at most `max_buckets` inference sizes holding graphs), as the reference takes each pair: both frames
+    resized to the inference size of the first, the depth resized back to the first frame's size.  The reference resizes
+    a pair only when its first frame is not already at the inference size (evaluate_depth.py:371-378), so a pair whose two
+    frames differ in size while the first needs no resize would give its model frames of two sizes; such a directory is
+    refused before any device work, as `inference_flow` refuses the same case."""
     if inference_dir is None:
         raise ValueError("inference_depth needs inference_dir")
     imgs, poses, intrinsics_file = depth_inputs(inference_dir)
-    sizes = {_header_size(f) for f in imgs}
-    if len(sizes) > 1:
-        raise ValueError("inference_depth: the frames under %s differ in size (%s); the depth driver takes one frame size"
-                         % (inference_dir, ", ".join("%dx%d" % s for s in sorted(sizes))))
+    sizes = [_header_size(f) for f in imgs]
+    for t in range(len(imgs) - 1):
+        if sizes[t] != sizes[t + 1] and _inference_size(sizes[t], padding_factor, inference_size) == sizes[t]:
+            raise ValueError("inference_depth: %s and %s differ in size and the first needs no resize, so the model would "
+                             "get frames of two sizes" % (imgs[t], imgs[t + 1]))
     keys = depth_keys(pred_bidir_depth)
     rd = _Readers(readers, readers + 2 * batch)
     os.makedirs(output_path, exist_ok=True)
@@ -428,13 +525,19 @@ def inference_depth(model, inference_dir=None, output_path="output", padding_fac
         return _stats({"pairs": 0, "steps": 0, "h2d_bytes": 0, "d2h_bytes": 0}, rd, 0.0)
     model.eval()
     K = np.loadtxt(intrinsics_file).astype(np.float32).reshape((4, 4))[:3, :3]
-    runner = DepthSequenceRunner(model, sizes.pop(), batch, device, K, padding_factor=padding_factor,
-                                 inference_size=inference_size, min_depth=min_depth, max_depth=max_depth,
-                                 num_depth_candidates=num_depth_candidates, depth_from_argmax=depth_from_argmax,
-                                 pred_bidir_depth=pred_bidir_depth, visualize=True, return_depth=False, attn_type=attn_type,
-                                 attn_splits_list=attn_splits_list, prop_radius_list=prop_radius_list,
-                                 num_reg_refine=num_reg_refine)
+    kw = dict(padding_factor=padding_factor, inference_size=inference_size, min_depth=min_depth, max_depth=max_depth,
+              num_depth_candidates=num_depth_candidates, depth_from_argmax=depth_from_argmax,
+              pred_bidir_depth=pred_bidir_depth, visualize=True, return_depth=False, attn_type=attn_type,
+              attn_splits_list=attn_splits_list, prop_radius_list=prop_radius_list, num_reg_refine=num_reg_refine)
     names = _named(DEPTH_FILES, keys, output_path, lambda i: _stem(imgs[i]))
     items = rd.map(lambda p: (_rgb_frame(p[0]), _pose(p[1])), zip(imgs, poses))
-    writer_s = _write_results(enumerate(runner.run(items)), names, writers, batch)
-    return _stats(_sequence_stats(runner, len(imgs) - 1, runner.pose_pin[0].nbytes), rd, writer_s)
+    if len(set(sizes)) == 1:
+        runner = DepthSequenceRunner(model, sizes[0], batch, device, K, **kw)
+        writer_s = _write_results(enumerate(runner.run(items)), names, writers, batch)
+        return _stats(_sequence_stats(runner, len(imgs) - 1, runner.pose_pin[0].nbytes), rd, writer_s)
+    cap = (max(h for h, _ in sizes), max(w for _, w in sizes))
+    runner = MixedSizeDepthRunner(model, cap, batch, device, K, max_buckets=max_buckets, **kw)
+    pairs = ((a[0], b[0], _relative_poses([a[1], b[1]], False)[0]) for a, b in _consecutive(items))
+    writer_s = _write_results(runner.run(pairs), names, writers, batch)
+    st = runner.stats
+    return _stats({k: st[k] for k in ("pairs", "steps", "h2d_bytes", "d2h_bytes")}, rd, writer_s)

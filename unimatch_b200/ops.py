@@ -118,6 +118,7 @@ _SIGNATURES = {
     "um_flow_to_image_ragged": (_RC, [_P, _L, _P, _P, _L, _P, _P, _I, _I, _I, _P]),
     "um_disparity_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
     "um_depth_to_image": (_RC, [_P, _P, _L, _L, _P, _I, _I, _I, _P]),
+    "um_depth_to_image_ragged": (_RC, [_P, _L, _P, _P, _P, _I, _I, _I, _P]),
     "um_encode_submission": (_RC, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
     "um_eval_stats": (_RC, [_P, _L, _L, _L, _L, _P, _P, _P, _I, _I, _F, _F, _F, _I, _I, _I, _P, _P, _P]),
     "um_conv2d_tc": (_RC, [ctypes.POINTER(ConvDesc), _P]),
@@ -610,6 +611,22 @@ def _depth_to_image(depth, out):
 
 
 depth_to_image = _define("depth_to_image(Tensor depth, Tensor(a!) out) -> ()", _depth_to_image)
+
+
+def _depth_to_image_ragged(depth, items, out, h_max, w_max):
+    """depth: contiguous fp32 packed depths (item i [h_i, w_i] at items[i].offset); out: contiguous uint8 of at least
+    3 depth.numel() bytes, RGB picture i at 3 items[i].offset"""
+    _f32c(depth, "depth")
+    if out.dtype != torch.uint8 or not out.is_contiguous() or out.device != depth.device or out.numel() < 3 * depth.numel():
+        raise RuntimeError("depth_to_image_ragged: out must be contiguous uint8 of 3 bytes per depth on its device")
+    n = _ragged_items(items, "depth_to_image_ragged")
+    scratch = torch.empty((DEPTH_TO_IMAGE_SCRATCH_WORDS * n,), device=depth.device, dtype=torch.int32)
+    _check(LIB.um_depth_to_image_ragged(_p(depth), depth.numel(), _p(items), _p(out), _p(scratch), n, h_max, w_max, _stream()),
+           "um_depth_to_image_ragged")
+
+
+depth_to_image_ragged = _define("depth_to_image_ragged(Tensor depth, Tensor items, Tensor(a!) out, int h_max, int w_max) -> ()",
+                                _depth_to_image_ragged)
 
 # include/unimatch_sm100.h (um_encode_submission)
 SUBMIT_CROP, SUBMIT_RESIZE = 0, 1
