@@ -269,6 +269,25 @@ int um_fb_consistency_ragged(const float* flow, int64_t flow_numel, const um_rag
                              float* occ, int64_t occ_numel, const um_ragged_item* occ_items, int32_t n, int32_t h_max,
                              int32_t w_max, void* stream);
 
+/* ---- dense point tracks ----------------------------------------------------------------------------------------
+ * Chains the forward flows of consecutive pairs from every pixel of a first frame (composition of flow_warp, geometry.py:65-72,
+ * with the fwd_occ of forward_backward_consistency_check, :75-96, as visibility).  Coordinates are pixels (x, y) at the
+ * flows' size.  State: pos [h, w, 2] (track positions) and vis [h, w] (uint8, 1 = visible), read and updated in place; the
+ * caller starts them at pos(y, x) = (x, y), vis = 1.  For each flow t = 0..n-1 in order, F = flow[t] (planar [2, h, w]) and
+ * O = occ[t] ([h, w]; occ NULL: O = 0, nothing occluded):
+ *   d = bilinear(F, p), o = bilinear(O, p);  p = p + d;
+ *   vis = vis && o < 0.5 && 0 <= p.x <= w-1 && 0 <= p.y <= h-1;
+ *   pos_out[t] = p, vis_out[t] = vis   (pos_out [n, h, w, 2], vis_out [n, h, w]).
+ * An invisible track stays invisible; its position is still advanced.  bilinear is bilinear_sample (geometry.py:41-62) in
+ * pixel coordinates: align_corners=True, zero padding.  fp32 order of operations, every step rounded on its own (no FMA):
+ *   x0 = floor(x), fx = x - x0 (exact), gx = 1 - fx, likewise y;  a corner outside [0, w-1] x [0, h-1] reads 0;
+ *   bilinear = gy (gx v00 + fx v01) + fy (gx v10 + fx v11);  a track with x <= -1, x >= w, y <= -1, y >= h or a NaN
+ *   coordinate samples 0 (it has no corner inside).
+ * One thread per track, one launch for the n flows; no host synchronisation (graph-capturable).  pos and pos_out are 8-byte
+ * aligned; the four state / output buffers do not overlap.  Frames of at least 2 x 2 (bilinear_sample divides by size - 1). */
+int um_chain_tracks(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, float* pos, uint8_t* vis,
+                    float* pos_out, uint8_t* vis_out, void* stream);
+
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the

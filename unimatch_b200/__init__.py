@@ -22,6 +22,8 @@ _LAZY = {
     "BatchedFlowRunner": (".inference", "BatchedFlowRunner"),
     "infer_flow_video": (".inference", "infer_flow_video"),
     "VideoFlowRunner": (".inference", "VideoFlowRunner"),
+    "VideoTrackRunner": (".inference", "VideoTrackRunner"),
+    "chain_tracks": (".inference", "chain_tracks"),
     "flow_to_image": (".inference", "flow_to_image"),
     "infer_depth_sequence": (".inference", "infer_depth_sequence"),
     "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
@@ -43,8 +45,8 @@ _LAZY = {
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner", "MixedSizeStereoRunner", "MixedSizeFlowRunner",
-           "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
+           "VideoTrackRunner", "chain_tracks", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
+           "MixedSizeStereoRunner", "MixedSizeFlowRunner", "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth"]
 

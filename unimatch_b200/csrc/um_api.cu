@@ -1,5 +1,5 @@
-// C-ABI glue: error reporting, launch accounting, and the attention entry points (argument checking + dispatch
-// between the tensor-core and the general CUDA-core kernels).  See include/unimatch_sm100.h.
+// C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
+// between the tensor-core and the general CUDA-core kernels) and the point-track entry (um_tracks.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -38,6 +38,13 @@ int softmax_expectation_tc(const float* q, const float* k, const float* values, 
 int softmax_expectation_simt(const float* q, const float* k, const float* values, float* out, int n_streams,
                              int n_total, int kv_shift, long long ldq, long long ldk, int vdim, int value_mode,
                              int post_op, const Geom& g, cudaStream_t st);
+int chain_tracks_launch(const float* flow, const float* occ, int n, int h, int w, float* pos, uint8_t* vis, float* pos_out,
+                        uint8_t* vis_out, cudaStream_t st);
+
+static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
+  const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
+  return x < y + (uintptr_t)bbytes && y < x + (uintptr_t)abytes;
+}
 
 }  // namespace um
 
@@ -139,6 +146,21 @@ int um_softmax_expectation(const float* q, const float* k, const float* values, 
   }
   return um::softmax_expectation_simt(q, k, values, out, n_streams, n_total, kv_shift, ldq, ldk, vdim, value_mode,
                                       post_op, g, (cudaStream_t)stream);
+}
+
+int um_chain_tracks(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, float* pos, uint8_t* vis,
+                    float* pos_out, uint8_t* vis_out, void* stream) {
+  UM_REQUIRE(flow && pos && vis && pos_out && vis_out, "um_chain_tracks: flow, state and outputs must not be NULL");
+  UM_REQUIRE(n > 0 && h > 1 && w > 1, "um_chain_tracks: bad shape (n >= 1 flows of at least 2 x 2)");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_chain_tracks: a frame has at most 2^31 - 1 pixels");
+  UM_REQUIRE(((reinterpret_cast<uintptr_t>(pos) | reinterpret_cast<uintptr_t>(pos_out)) & 7) == 0,
+             "um_chain_tracks: pos and pos_out must be 8-byte aligned");
+  const long long hw = (long long)h * w, p1 = 8 * hw, v1 = hw, pn = 8 * n * hw, vn = n * hw;
+  UM_REQUIRE(!um::overlap(pos, p1, vis, v1) && !um::overlap(pos, p1, pos_out, pn) && !um::overlap(pos, p1, vis_out, vn) &&
+                 !um::overlap(vis, v1, pos_out, pn) && !um::overlap(vis, v1, vis_out, vn) &&
+                 !um::overlap(pos_out, pn, vis_out, vn),
+             "um_chain_tracks: the state and output buffers must not overlap");
+  return um::chain_tracks_launch(flow, occ, n, h, w, pos, vis, pos_out, vis_out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -18,6 +18,10 @@ per-image, so the result is what `infer_flow` gives on the pairs, up to fp32 sum
 path with one upload per new frame and the previous step's last pyramid carried over, and `flow_to_image` is the Middlebury
 colouring of utils/flow_viz.py on the device.  The leaderboard files (.flo, PNG, PFM) are written by `submission.py`,
 and the plain inference commands' files (decoding and the `save_video` mp4 included) by `inference_io.py`.
+Dense point tracks over a video (composing the reference's `flow_warp` and `forward_backward_consistency_check`,
+geometry.py:41-96, frame after frame): `chain_tracks` chains device forward flows from every pixel of a first frame with the
+forward occlusion masks as visibility (`um_chain_tracks`), and `VideoTrackRunner` runs that launch inside the
+`VideoFlowRunner` step, so only the tracks are downloaded.
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
@@ -1238,6 +1242,83 @@ class VideoFlowRunner(_SequenceRunner):
     def _prime(self, frame):
         super()._prime(frame)
         self.carry_frame.copy_(frame)
+
+
+def _track_start(h, w, device):
+    """Tracks at every pixel of the first frame: pos [H,W,2] = (x, y), all visible."""
+    ys, xs = torch.meshgrid(torch.arange(h, device=device, dtype=torch.float32),
+                            torch.arange(w, device=device, dtype=torch.float32), indexing="ij")
+    return torch.stack((xs, ys), dim=-1).contiguous(), torch.ones((h, w), device=device, dtype=torch.uint8)
+
+
+@torch.no_grad()
+def chain_tracks(flows, occ=None, state=None):
+    """Dense point tracks through the forward flows of consecutive pairs, one `um_chain_tracks` launch.
+
+    `flows`: device planar [N,2,H,W], the forward flow of pair (t-1, t) at index t-1 in pixels at the frames' size (e.g.
+    `infer_flow_video(...)['flow']`); `occ`: its forward occlusion masks [N,H,W] (`'fwd_occ'`, 1 = occluded) or None
+    (nothing occluded).  `state`: (pos fp32 [H,W,2], vis uint8 [H,W]), contiguous on the flows' device and advanced in place,
+    or None: the tracks start at every pixel, pos(y, x) = (x, y), all visible.  Per flow, with F the flow and O the mask:
+    d = bilinear(F, p), o = bilinear(O, p) (the reference's `bilinear_sample`: pixel coordinates, align_corners=True, zero
+    padding), p = p + d, and the track stays visible while o < 0.5 and p lies in [0, W-1] x [0, H-1]; an invisible track stays
+    invisible and is still moved.  fp32, with the order of operations of include/unimatch_sm100.h.
+    Returns {'tracks': [N,H,W,2] fp32 (x, y), 'visible': [N,H,W] uint8}, the state after each flow.  To continue with the
+    flows that follow, pass state=(tracks[-1].clone(), visible[-1].clone())."""
+    if flows.dim() != 4 or flows.shape[1] != 2 or flows.shape[0] < 1:
+        raise ValueError("chain_tracks expects at least one planar flow [N,2,H,W]")
+    n, _, h, w = flows.shape
+    if occ is not None and tuple(occ.shape) != (n, h, w):
+        raise ValueError("chain_tracks: occ must be [N,H,W] like the flows")
+    if state is None:
+        state = _track_start(h, w, flows.device)
+    pos, vis = state
+    if tuple(pos.shape) != (h, w, 2) or tuple(vis.shape) != (h, w):
+        raise ValueError("chain_tracks: the state is (pos [H,W,2], vis [H,W]) at the flows' size")
+    tracks, visible = _OPS.chain_tracks(flows.float().contiguous(), None if occ is None else occ.float().contiguous(), pos,
+                                        vis)
+    return {"tracks": tracks, "visible": visible}
+
+
+class VideoTrackRunner(VideoFlowRunner):
+    """Dense point tracks over a video: where each pixel of the first frame of a `run()` is in every later frame, and whether
+    it is still visible, chained on the device inside the `VideoFlowRunner` step.
+
+    The step computes the forward and backward flows and the forward-backward occlusion masks (`pred_bidir_flow` and
+    `fwd_bwd_consistency_check` are always on) at the frames' original size and orientation, then one `um_chain_tracks`
+    launch advances every track through the step's `batch` forward flows in order (semantics: `chain_tracks`).  The track
+    state lives in device buffers that persist across steps and is reset at the start of each `run()`, so the tracks do
+    not depend on `batch` beyond the encoder's summation order in the flows themselves.
+    `run(frames)` yields, per frame t >= 1, 'tracks' fp32 [H,W,2] (x, y in pixels) and 'visible' uint8 [H,W]: 9 bytes per
+    pixel downloaded (3.6 MB per 480x832 frame), against 12 for the forward flow and its mask.  `return_flow=True` adds the
+    'flow', 'flow_bwd', 'fwd_occ' and 'bwd_occ' that `VideoFlowRunner(pred_bidir_flow=True, fwd_bwd_consistency_check=True)`
+    returns.  `pred_bwd_flow`, `visualize`, `concat_frame` and `visualize_bwd` are refused: the tracks run forward from the
+    first frame."""
+
+    def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
+                 return_flow=False, **model_kwargs):
+        for k in ("pred_bwd_flow", "visualize", "concat_frame", "visualize_bwd"):
+            if model_kwargs.pop(k, False):
+                raise ValueError("VideoTrackRunner: %s is not supported (tracks run forward from the first frame)" % k)
+        for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
+            if not model_kwargs.pop(k, True):
+                raise ValueError("VideoTrackRunner: %s is always on (the forward occlusion mask decides visibility)" % k)
+        super().__init__(model, frame_size, batch, device, padding_factor=padding_factor, inference_size=inference_size,
+                         use_graph=use_graph, pred_bidir_flow=True, fwd_bwd_consistency_check=True, **model_kwargs)
+        self.return_flow = bool(return_flow)
+        self.track_origin, self.track_vis = _track_start(self.h, self.w, self.dev)
+        self.track_pos = self.track_origin.clone()
+
+    def _match(self, slot, first, second):
+        out = super()._match(slot, first, second)
+        tracks, visible = _OPS.chain_tracks(out["flow"].contiguous(), out["fwd_occ"], self.track_pos, self.track_vis)
+        out = out if self.return_flow else {}
+        out["tracks"], out["visible"] = tracks, visible
+        return out
+
+    def _prime(self, frame):
+        super()._prime(frame)
+        self.track_pos.copy_(self.track_origin)
+        self.track_vis.fill_(1)
 
 
 class DepthSequenceRunner(_SequenceRunner):

@@ -102,6 +102,7 @@ _SIGNATURES = {
     "um_flow_warp": (_RC, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "um_fb_consistency": (_RC, [_P, _P, _F, _F, _P, _P, _I, _I, _I, _P]),
     "um_fb_consistency_ragged": (_RC, [_P, _L, _P, _F, _F, _P, _L, _P, _I, _I, _I, _P]),
+    "um_chain_tracks": (_RC, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -333,6 +334,33 @@ def _fb_consistency(fwd_flow, bwd_flow, alpha, beta):
 
 fb_consistency = _define("fb_consistency(Tensor fwd_flow, Tensor bwd_flow, float alpha, float beta) -> (Tensor, Tensor)",
                          _fb_consistency)
+
+
+def _chain_tracks(flow, occ, pos, vis):
+    """flow: contiguous fp32 [n, 2, h, w]; occ: contiguous fp32 [n, h, w] or None (nothing occluded); pos / vis: the running
+    state, contiguous fp32 [h, w, 2] and uint8 [h, w], advanced in place.  Returns the state after each flow, [n, h, w, 2]
+    and [n, h, w] (include/unimatch_sm100.h, um_chain_tracks)."""
+    _f32c(flow, "flow"), _f32c(pos, "pos")
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise RuntimeError("chain_tracks: expected planar flows [n, 2, h, w]")
+    n, _, h, w = flow.shape
+    if occ is not None:
+        _f32c(occ, "occ")
+        if tuple(occ.shape) != (n, h, w) or occ.device != flow.device:
+            raise RuntimeError("chain_tracks: occ must be [n, h, w] on the flows' device")
+    if tuple(pos.shape) != (h, w, 2) or pos.device != flow.device:
+        raise RuntimeError("chain_tracks: pos must be [h, w, 2] on the flows' device")
+    if vis.dtype != torch.uint8 or tuple(vis.shape) != (h, w) or not vis.is_contiguous() or vis.device != flow.device:
+        raise RuntimeError("chain_tracks: vis must be contiguous uint8 [h, w] on the flows' device")
+    pos_out = torch.empty((n, h, w, 2), device=flow.device, dtype=torch.float32)
+    vis_out = torch.empty((n, h, w), device=flow.device, dtype=torch.uint8)
+    _check(LIB.um_chain_tracks(_p(flow), _p(occ), n, h, w, _p(pos), _p(vis), _p(pos_out), _p(vis_out), _stream()),
+           "um_chain_tracks")
+    return pos_out, vis_out
+
+
+chain_tracks = _define("chain_tracks(Tensor flow, Tensor? occ, Tensor(a!) pos, Tensor(b!) vis) -> (Tensor, Tensor)",
+                       _chain_tracks)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
