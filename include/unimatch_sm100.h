@@ -288,6 +288,37 @@ int um_fb_consistency_ragged(const float* flow, int64_t flow_numel, const um_rag
 int um_chain_tracks(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, float* pos, uint8_t* vis,
                     float* pos_out, uint8_t* vis_out, void* stream);
 
+/* ---- query point tracks ----------------------------------------------------------------------------------------
+ * Tracks nq query points through a clip of nt frames, each forward and backward in time from the frame it is given at (the
+ * question TAP-Vid asks).  queries [nq, 3] = (t_q, y, x): t_q an integer frame index (stored as float), (x, y) pixels at the
+ * flows' size, pixel centres at integers.  Tables: tracks [nq, nt, 2] (x, y) and visible [nq, nt] (uint8, 1 = visible),
+ * row q holding query q's track in every frame.  Every step is um_chain_tracks's step with the same bilinear, the same fp32
+ * order of operations and no FMA:
+ *   frame t_q:          p = (x, y), visible;
+ *   forward, t > t_q:   pair (t-1, t), F its forward flow, O its fwd_occ:   p_t = p_{t-1} + bilinear(F, p_{t-1}),
+ *                       vis_t = vis_{t-1} && bilinear(O, p_{t-1}) < 0.5 && 0 <= p_t.x <= w-1 && 0 <= p_t.y <= h-1;
+ *   backward, t < t_q:  pair (t, t+1), B its backward flow (frame t+1 -> t), Ob its bwd_occ:   p_t = p_{t+1} +
+ *                       bilinear(B, p_{t+1}), vis_t = vis_{t+1} && bilinear(Ob, p_{t+1}) < 0.5 && p_t inside the frame.
+ * An invisible track still moves.  A masks pointer of NULL means nothing is occluded.  So for a query at an integer pixel
+ * the forward part is um_chain_tracks over the flows from pair t_q on, and the backward part um_chain_tracks over the
+ * backward flows of pairs t_q-1, ..., 0 in that order, bit for bit.
+ *
+ * um_track_points_forward: the n forward flows [n, 2, h, w] and masks [n, h, w] of pairs t0 .. t0+n-1, frames t0+1 .. t0+n
+ * of the table, which must exist (t0 + n < nt).  A stream is chained by launches over its pairs in order, the first at
+ * t0 = 0, each at the previous t0 + n: a query joins at pair t_q from the query itself, and otherwise continues from the
+ * state pos [nq, 2] / vis [nq] the previous launch left (read and written in place, never initialised by the caller).
+ * Writes the table entries t > t_q it reaches; a query whose t_q is not an integer in [0, nt) is skipped.
+ * um_track_points_backward: the n backward flows [n, 2, h, w] and masks [n, h, w] of pairs 0 .. n-1 (flow NULL when n = 0,
+ * n < nt), in one launch; writes entries 0 .. t_q of every row.  A query it cannot serve (t_q not an integer in
+ * [0, min(nt, n + 1))) gets NaN positions and visible = 0 in all nt entries.
+ * One thread per query; no host synchronisation.  flow, occ and queries 4-byte aligned, pos and tracks 8-byte aligned; the
+ * buffers a launch writes overlap nothing it reads or writes.  Frames of at least 2 x 2, nq >= 1. */
+int um_track_points_forward(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, int32_t t0,
+                            const float* queries, int32_t nq, int32_t nt, float* pos, uint8_t* vis, float* tracks,
+                            uint8_t* visible, void* stream);
+int um_track_points_backward(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, const float* queries,
+                             int32_t nq, int32_t nt, float* tracks, uint8_t* visible, void* stream);
+
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the

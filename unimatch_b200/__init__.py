@@ -24,6 +24,8 @@ _LAZY = {
     "VideoFlowRunner": (".inference", "VideoFlowRunner"),
     "VideoTrackRunner": (".inference", "VideoTrackRunner"),
     "chain_tracks": (".inference", "chain_tracks"),
+    "PointTrackRunner": (".inference", "PointTrackRunner"),
+    "track_points": (".inference", "track_points"),
     "flow_to_image": (".inference", "flow_to_image"),
     "infer_depth_sequence": (".inference", "infer_depth_sequence"),
     "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
@@ -36,6 +38,7 @@ _LAZY = {
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
+    "tapvid_metrics": (".evaluation", "tapvid_metrics"),
     "create_flow_submission": (".submission", "create_flow_submission"),
     "create_stereo_submission": (".submission", "create_stereo_submission"),
     "inference_flow": (".inference_io", "inference_flow"),
@@ -45,9 +48,9 @@ _LAZY = {
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "VideoTrackRunner", "chain_tracks", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
+           "VideoTrackRunner", "chain_tracks", "PointTrackRunner", "track_points", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
            "MixedSizeStereoRunner", "MixedSizeFlowRunner", "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
-           "validate_flow", "validate_stereo", "validate_depth", "create_flow_submission", "create_stereo_submission",
+           "validate_flow", "validate_stereo", "validate_depth", "tapvid_metrics", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth"]
 
 

@@ -1,8 +1,9 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
-// between the tensor-core and the general CUDA-core kernels) and the point-track entry (um_tracks.cu).  See include/unimatch_sm100.h.
+// between the tensor-core and the general CUDA-core kernels) and the point-track entries (um_tracks.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
+#include <initializer_list>
 
 #include <cuda_fp16.h>
 
@@ -40,11 +41,30 @@ int softmax_expectation_simt(const float* q, const float* k, const float* values
                              int post_op, const Geom& g, cudaStream_t st);
 int chain_tracks_launch(const float* flow, const float* occ, int n, int h, int w, float* pos, uint8_t* vis, float* pos_out,
                         uint8_t* vis_out, cudaStream_t st);
+int track_points_forward_launch(const float* flow, const float* occ, int n, int h, int w, int t0, const float* queries,
+                                int nq, int nt, float* pos, uint8_t* vis, float* tracks, uint8_t* visible, cudaStream_t st);
+int track_points_backward_launch(const float* flow, const float* occ, int n, int h, int w, const float* queries, int nq,
+                                 int nt, float* tracks, uint8_t* visible, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
   return x < y + (uintptr_t)bbytes && y < x + (uintptr_t)abytes;
 }
+
+// every written buffer (the first n_out of bufs) overlaps no other buffer; NULL entries are absent
+struct Span {
+  const void* p;
+  long long bytes;
+};
+static bool written_disjoint(std::initializer_list<Span> bufs, size_t n_out) {
+  const Span* b = bufs.begin();
+  for (size_t i = 0; i < n_out; ++i)
+    for (size_t j = 0; j < bufs.size(); ++j)
+      if (j != i && b[i].p && b[j].p && overlap(b[i].p, b[i].bytes, b[j].p, b[j].bytes)) return false;
+  return true;
+}
+
+static bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
 
 }  // namespace um
 
@@ -161,6 +181,46 @@ int um_chain_tracks(const float* flow, const float* occ, int32_t n, int32_t h, i
                  !um::overlap(pos_out, pn, vis_out, vn),
              "um_chain_tracks: the state and output buffers must not overlap");
   return um::chain_tracks_launch(flow, occ, n, h, w, pos, vis, pos_out, vis_out, (cudaStream_t)stream);
+}
+
+int um_track_points_forward(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, int32_t t0,
+                            const float* queries, int32_t nq, int32_t nt, float* pos, uint8_t* vis, float* tracks,
+                            uint8_t* visible, void* stream) {
+  UM_REQUIRE(flow && queries && pos && vis && tracks && visible,
+             "um_track_points_forward: flow, queries, state and tables must not be NULL");
+  UM_REQUIRE(n > 0 && h > 1 && w > 1 && nq > 0, "um_track_points_forward: bad shape (n >= 1 flows of at least 2 x 2, "
+             "nq >= 1 queries)");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_track_points_forward: a frame has at most 2^31 - 1 pixels");
+  UM_REQUIRE(t0 >= 0 && (long long)t0 + n < nt, "um_track_points_forward: frames t0 .. t0+n must lie inside the table "
+             "(t0 = %d, n = %d, nt = %d)", t0, n, nt);
+  UM_REQUIRE(um::aligned(flow, 4) && um::aligned(occ, 4) && um::aligned(queries, 4) && um::aligned(pos, 8) &&
+                 um::aligned(tracks, 8),
+             "um_track_points_forward: flow, occ and queries must be 4-byte aligned, pos and tracks 8-byte aligned");
+  const long long hw = (long long)h * w, tab = (long long)nq * nt;
+  UM_REQUIRE(um::written_disjoint({{pos, 8LL * nq}, {vis, nq}, {tracks, 8 * tab}, {visible, tab}, {queries, 12LL * nq},
+                                   {flow, 8LL * n * hw}, {occ, 4LL * n * hw}}, 4),
+             "um_track_points_forward: the state and tables must not overlap each other or the inputs");
+  return um::track_points_forward_launch(flow, occ, n, h, w, t0, queries, nq, nt, pos, vis, tracks, visible,
+                                         (cudaStream_t)stream);
+}
+
+int um_track_points_backward(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, const float* queries,
+                             int32_t nq, int32_t nt, float* tracks, uint8_t* visible, void* stream) {
+  UM_REQUIRE(queries && tracks && visible && (flow || n == 0),
+             "um_track_points_backward: queries, tables and (n > 0) flow must not be NULL");
+  UM_REQUIRE(n >= 0 && h > 1 && w > 1 && nq > 0, "um_track_points_backward: bad shape (n >= 0 flows of at least 2 x 2, "
+             "nq >= 1 queries)");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_track_points_backward: a frame has at most 2^31 - 1 pixels");
+  UM_REQUIRE(nt >= 2 && n < nt, "um_track_points_backward: the n stored pairs must lie inside a table of nt >= 2 frames "
+             "(n = %d, nt = %d)", n, nt);
+  UM_REQUIRE(um::aligned(flow, 4) && um::aligned(occ, 4) && um::aligned(queries, 4) && um::aligned(tracks, 8),
+             "um_track_points_backward: flow, occ and queries must be 4-byte aligned, tracks 8-byte aligned");
+  const long long hw = (long long)h * w, tab = (long long)nq * nt;
+  UM_REQUIRE(um::written_disjoint({{tracks, 8 * tab}, {visible, tab}, {queries, 12LL * nq}, {flow, 8LL * n * hw},
+                                   {occ, 4LL * n * hw}}, 2),
+             "um_track_points_backward: the tables must not overlap each other or the inputs");
+  return um::track_points_backward_launch(n > 0 ? flow : nullptr, n > 0 ? occ : nullptr, n, h, w, queries, nq, nt, tracks,
+                                          visible, (cudaStream_t)stream);
 }
 
 }  // extern "C"

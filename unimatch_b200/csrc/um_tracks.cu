@@ -1,11 +1,14 @@
-// Dense point tracks: the forward flows of consecutive pairs chained from every pixel of a first frame, with the forward
-// occlusion masks deciding visibility.  Semantics and the fp32 order of operations: include/unimatch_sm100.h
-// (um_chain_tracks); the float64 statement is tests/refops_tracks.py.
+// Point tracks chained through the flows of consecutive pairs.  Dense: the forward flows from every pixel of a first frame,
+// with the forward occlusion masks deciding visibility (um_chain_tracks).  Sparse: query points, each given at its own
+// frame, chained forward through the forward flows and backward through the backward flows (um_track_points_forward /
+// um_track_points_backward).  Semantics and the fp32 order of operations: include/unimatch_sm100.h; the float64
+// statements are tests/refops_tracks.py and tests/refops_points.py.
 #include "um_common.cuh"
 
 namespace {
 
 constexpr int TRACK_THREADS = 256;
+constexpr int POINT_THREADS = 128;
 
 // Bilinear taps of one axis at pixel coordinate c (align_corners=True): corners i0 = floor(c) and i0 + 1 with weights
 // (1 - f, f), f = c - i0 (exact in fp32); in0 / in1 tell which corners lie inside [0, n-1].
@@ -34,6 +37,22 @@ __device__ __forceinline__ float lerp2(const float* img, int w, const Axis& ax, 
   return __fadd_rn(__fmul_rn(ay.w0, top), __fmul_rn(ay.w1, bot));
 }
 
+// One step of a track through flow f (planar [2, h, w]) and mask o ([h, w] or NULL): the step every entry shares.
+__device__ __forceinline__ void track_step(float2& p, bool& v, const float* f, const float* o, int h, int w) {
+  const long long plane = (long long)h * w;
+  float dx = 0.f, dy = 0.f, m = 0.f;
+  // a track at least a pixel outside (or NaN) has no corner inside: the zero-padded samples are 0
+  if (p.x > -1.f && p.x < (float)w && p.y > -1.f && p.y < (float)h) {
+    const Axis ax = axis_taps(p.x, w), ay = axis_taps(p.y, h);
+    dx = lerp2(f, w, ax, ay);
+    dy = lerp2(f + plane, w, ax, ay);
+    if (o) m = lerp2(o, w, ax, ay);
+  }
+  p.x = __fadd_rn(p.x, dx);
+  p.y = __fadd_rn(p.y, dy);
+  v = v && m < 0.5f && p.x >= 0.f && p.x <= (float)(w - 1) && p.y >= 0.f && p.y <= (float)(h - 1);
+}
+
 // One thread owns track `pix` and advances it through the n flows in order; the state is read once and written once.
 __global__ void __launch_bounds__(TRACK_THREADS)
 chain_tracks_kernel(const float* __restrict__ flow, const float* __restrict__ occ, int n, int h, int w,
@@ -44,25 +63,78 @@ chain_tracks_kernel(const float* __restrict__ flow, const float* __restrict__ oc
   if (pix >= plane) return;
   float2 p = pos[pix];
   bool v = vis[pix] != 0;
-  const float xmax = (float)(w - 1), ymax = (float)(h - 1);
   for (int t = 0; t < n; ++t) {
-    const float* f = flow + (long long)t * 2 * plane;
-    float dx = 0.f, dy = 0.f, o = 0.f;
-    // a track at least a pixel outside (or NaN) has no corner inside: the zero-padded samples are 0
-    if (p.x > -1.f && p.x < (float)w && p.y > -1.f && p.y < (float)h) {
-      const Axis ax = axis_taps(p.x, w), ay = axis_taps(p.y, h);
-      dx = lerp2(f, w, ax, ay);
-      dy = lerp2(f + plane, w, ax, ay);
-      if (occ) o = lerp2(occ + (long long)t * plane, w, ax, ay);
-    }
-    p.x = __fadd_rn(p.x, dx);
-    p.y = __fadd_rn(p.y, dy);
-    v = v && o < 0.5f && p.x >= 0.f && p.x <= xmax && p.y >= 0.f && p.y <= ymax;
+    track_step(p, v, flow + (long long)t * 2 * plane, occ ? occ + (long long)t * plane : nullptr, h, w);
     pos_out[(long long)t * plane + pix] = p;
     vis_out[(long long)t * plane + pix] = v ? 1 : 0;
   }
   pos[pix] = p;
   vis[pix] = v ? 1 : 0;
+}
+
+// The query's frame t_q if it is an integer in [0, limit), else -1.
+__device__ __forceinline__ int query_frame(float t, int limit) {
+  return (t >= 0.f && t < (float)limit && t == floorf(t)) ? (int)t : -1;
+}
+
+// One thread owns query q and advances it through the launch's pairs t0 .. t0+n-1 that follow its frame: it joins at pair
+// t_q (from the query itself) or continues from the state an earlier launch left.
+__global__ void __launch_bounds__(POINT_THREADS)
+track_points_forward_kernel(const float* __restrict__ flow, const float* __restrict__ occ, int n, int h, int w, int t0,
+                            const float* __restrict__ queries, int nq, int nt, float2* __restrict__ pos,
+                            uint8_t* __restrict__ vis, float2* __restrict__ tracks, uint8_t* __restrict__ visible) {
+  const int q = blockIdx.x * POINT_THREADS + threadIdx.x;
+  if (q >= nq) return;
+  const int tq = query_frame(queries[3 * q], nt);
+  if (tq < 0 || tq >= t0 + n) return;
+  const long long plane = (long long)h * w, row = (long long)q * nt;
+  float2 p;
+  bool v;
+  int j = t0;
+  if (tq >= t0) {
+    p = make_float2(queries[3 * q + 2], queries[3 * q + 1]);
+    v = true;
+    j = tq;
+  } else {
+    p = pos[q];
+    v = vis[q] != 0;
+  }
+  for (; j < t0 + n; ++j) {
+    const long long i = j - t0;
+    track_step(p, v, flow + i * 2 * plane, occ ? occ + i * plane : nullptr, h, w);
+    tracks[row + j + 1] = p;
+    visible[row + j + 1] = v ? 1 : 0;
+  }
+  pos[q] = p;
+  vis[q] = v ? 1 : 0;
+}
+
+// One thread owns query q: frame t_q is the query itself, then pairs t_q-1 .. 0 of the backward flows in turn.  A query
+// that cannot be served (t_q not an integer in [0, nt) or past the n stored pairs) gets a NaN, invisible row.
+__global__ void __launch_bounds__(POINT_THREADS)
+track_points_backward_kernel(const float* __restrict__ flow, const float* __restrict__ occ, int n, int h, int w,
+                             const float* __restrict__ queries, int nq, int nt, float2* __restrict__ tracks,
+                             uint8_t* __restrict__ visible) {
+  const int q = blockIdx.x * POINT_THREADS + threadIdx.x;
+  if (q >= nq) return;
+  const int tq = query_frame(queries[3 * q], min(nt, n + 1));
+  const long long plane = (long long)h * w, row = (long long)q * nt;
+  if (tq < 0) {
+    for (int t = 0; t < nt; ++t) {
+      tracks[row + t] = make_float2(__int_as_float(0x7fffffff), __int_as_float(0x7fffffff));
+      visible[row + t] = 0;
+    }
+    return;
+  }
+  float2 p = make_float2(queries[3 * q + 2], queries[3 * q + 1]);
+  bool v = true;
+  tracks[row + tq] = p;
+  visible[row + tq] = 1;
+  for (int j = tq - 1; j >= 0; --j) {
+    track_step(p, v, flow + (long long)j * 2 * plane, occ ? occ + (long long)j * plane : nullptr, h, w);
+    tracks[row + j] = p;
+    visible[row + j] = v ? 1 : 0;
+  }
 }
 
 }  // namespace
@@ -76,6 +148,22 @@ int chain_tracks_launch(const float* flow, const float* occ, int n, int h, int w
   chain_tracks_kernel<<<(unsigned)((hw + TRACK_THREADS - 1) / TRACK_THREADS), TRACK_THREADS, 0, st>>>(
       flow, occ, n, h, w, reinterpret_cast<float2*>(pos), vis, reinterpret_cast<float2*>(pos_out), vis_out);
   return check_launch("um_chain_tracks");
+}
+
+// Arguments are checked by um_track_points_forward / um_track_points_backward (um_api.cu).
+int track_points_forward_launch(const float* flow, const float* occ, int n, int h, int w, int t0, const float* queries,
+                                int nq, int nt, float* pos, uint8_t* vis, float* tracks, uint8_t* visible, cudaStream_t st) {
+  track_points_forward_kernel<<<(unsigned)((nq + POINT_THREADS - 1) / POINT_THREADS), POINT_THREADS, 0, st>>>(
+      flow, occ, n, h, w, t0, queries, nq, nt, reinterpret_cast<float2*>(pos), vis, reinterpret_cast<float2*>(tracks),
+      visible);
+  return check_launch("um_track_points_forward");
+}
+
+int track_points_backward_launch(const float* flow, const float* occ, int n, int h, int w, const float* queries, int nq,
+                                 int nt, float* tracks, uint8_t* visible, cudaStream_t st) {
+  track_points_backward_kernel<<<(unsigned)((nq + POINT_THREADS - 1) / POINT_THREADS), POINT_THREADS, 0, st>>>(
+      flow, occ, n, h, w, queries, nq, nt, reinterpret_cast<float2*>(tracks), visible);
+  return check_launch("um_track_points_backward");
 }
 
 }  // namespace um

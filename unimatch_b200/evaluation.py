@@ -16,6 +16,8 @@ predictions to per-sample statistics with one `um_eval_stats` launch per batch. 
 until the single download at the end; the flow and stereo drivers issue no other host synchronisation (the depth model
 synchronises once per batch for its `torch.inverse`).  The metrics are then formed on the host in float64, following each
 reference loop -- including its quirks, listed in each driver's docstring.
+
+`tapvid_metrics` scores point tracks (e.g. `PointTrackRunner`'s) with TAP-Vid's metrics, in numpy on the host.
 """
 import os
 
@@ -337,3 +339,51 @@ def _depth_results(T):
                       c["a1"][i] / n, c["a2"][i] / n, c["a3"][i] / n]
     num_samples = T.shape[0]
     return {k: (float(v / num_samples) if num_samples else float("nan")) for k, v in zip(_DEPTH_NAMES, error_sum)}
+
+
+# ---------------------------------------------------------------------------------------------------------- point tracks
+TAPVID_THRESHOLDS = (1, 2, 4, 8, 16)
+
+
+def tapvid_metrics(query_points, gt_occluded, gt_tracks, pred_occluded, pred_tracks, query_mode):
+    """TAP-Vid's point-tracking metrics per video, in numpy (the arrays are tiny).
+
+    `query_points` [B,N,3] (t_q, y, x); `gt_occluded` / `pred_occluded` [B,N,T] bool; `gt_tracks` / `pred_tracks` [B,N,T,2]
+    (x, y).  Coordinates are compared as given: TAP-Vid's protocol rescales them to 256x256 first, which is the caller's job.
+    The evaluation points of a track are its frames t > t_q (`query_mode='first'`) or t != t_q (`'strided'`).
+      * occlusion_accuracy: share of evaluation points where the predicted and true occlusion agree;
+      * for d in 1, 2, 4, 8, 16 with within = |pred - gt|^2 < d^2 and vis = not occluded:
+        pts_within_d = sum(within & gt_vis & eval) / sum(gt_vis & eval),
+        jaccard_d = TP / (sum(gt_vis & eval) + FP), TP = sum(within & gt_vis & pred_vis & eval),
+        FP = sum((~gt_vis | ~within) & pred_vis & eval);
+      * average_pts_within_thresh and average_jaccard: their means over the five d.
+    Every value is float64 of shape [B]; 0 / 0 gives NaN."""
+    if query_mode not in ("first", "strided"):
+        raise ValueError("tapvid_metrics: query_mode is 'first' or 'strided'")
+    qp = np.asarray(query_points)
+    gt_occ, pred_occ = np.asarray(gt_occluded).astype(bool), np.asarray(pred_occluded).astype(bool)
+    gt, pred = np.asarray(gt_tracks, np.float64), np.asarray(pred_tracks, np.float64)
+    b, n, t = gt_occ.shape
+    if qp.shape != (b, n, 3) or pred_occ.shape != (b, n, t) or gt.shape != (b, n, t, 2) or pred.shape != (b, n, t, 2):
+        raise ValueError("tapvid_metrics: query_points [B,N,3], occlusions [B,N,T] and tracks [B,N,T,2] must agree")
+    tq = np.round(qp[..., 0]).astype(np.int64)[..., None]
+    frames = np.arange(t)[None, None]
+    evals = frames > tq if query_mode == "first" else frames != tq
+
+    def ratio(num, den):
+        with np.errstate(invalid="ignore", divide="ignore"):
+            return np.asarray(num, np.float64) / np.asarray(den, np.float64)
+
+    out = {"occlusion_accuracy": ratio(((gt_occ == pred_occ) & evals).sum((1, 2)), evals.sum((1, 2)))}
+    gt_vis, pred_vis = ~gt_occ, ~pred_occ
+    dist2 = ((pred - gt) ** 2).sum(-1)
+    visible = (gt_vis & evals).sum((1, 2))
+    for d in TAPVID_THRESHOLDS:
+        within = dist2 < d * d
+        out["pts_within_%d" % d] = ratio((within & gt_vis & evals).sum((1, 2)), visible)
+        tp = (within & gt_vis & pred_vis & evals).sum((1, 2))
+        fp = ((~gt_vis | ~within) & pred_vis & evals).sum((1, 2))
+        out["jaccard_%d" % d] = ratio(tp, visible + fp)
+    out["average_pts_within_thresh"] = np.mean([out["pts_within_%d" % d] for d in TAPVID_THRESHOLDS], axis=0)
+    out["average_jaccard"] = np.mean([out["jaccard_%d" % d] for d in TAPVID_THRESHOLDS], axis=0)
+    return out

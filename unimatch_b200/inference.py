@@ -21,7 +21,10 @@ and the plain inference commands' files (decoding and the `save_video` mp4 inclu
 Dense point tracks over a video (composing the reference's `flow_warp` and `forward_backward_consistency_check`,
 geometry.py:41-96, frame after frame): `chain_tracks` chains device forward flows from every pixel of a first frame with the
 forward occlusion masks as visibility (`um_chain_tracks`), and `VideoTrackRunner` runs that launch inside the
-`VideoFlowRunner` step, so only the tracks are downloaded.
+`VideoFlowRunner` step, so only the tracks are downloaded.  Query point tracks (TAP-Vid's question: N points, each given
+at its own frame, tracked forward and backward in time through every frame of the clip): `track_points` for device flows a
+caller holds, and `PointTrackRunner`, which chains them next to the `VideoFlowRunner` step and downloads only the tables
+(`um_track_points_forward` / `um_track_points_backward`).
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
@@ -1319,6 +1322,158 @@ class VideoTrackRunner(VideoFlowRunner):
         super()._prime(frame)
         self.track_pos.copy_(self.track_origin)
         self.track_vis.fill_(1)
+
+
+def _point_queries(queries, h, w, name):
+    """Host float32 [N,3] (t_q, y, x) of TAP-Vid's `query_points`, refused unless t_q is a non-negative integer and (x, y)
+    is finite and inside [0, W-1] x [0, H-1]."""
+    q = torch.as_tensor(queries).detach().to("cpu", torch.float32)
+    if q.dim() != 2 or q.shape[1] != 3 or q.shape[0] < 1:
+        raise ValueError("%s: queries must be [N, 3] (t_q, y, x) with N >= 1" % name)
+    bad = ~torch.isfinite(q).all(dim=1)
+    bad |= (q[:, 0] < 0) | (q[:, 0] != torch.floor(q[:, 0]))
+    bad |= (q[:, 1] < 0) | (q[:, 1] > h - 1) | (q[:, 2] < 0) | (q[:, 2] > w - 1)
+    if bad.any():
+        i = int(bad.nonzero()[0])
+        raise ValueError("%s: query %d (t_q, y, x) = %s needs a finite (x, y) inside the %dx%d frame and an integer "
+                         "t_q >= 0" % (name, i, tuple(q[i].tolist()), h, w))
+    return q
+
+
+def _late_query(q, nframes, name):
+    late = (q[:, 0] >= nframes).nonzero()
+    if len(late):
+        i = int(late[0])
+        raise ValueError("%s: query %d is given at frame %d of a clip of %d frames" % (name, i, int(q[i, 0]), nframes))
+
+
+@torch.no_grad()
+def track_points(flows, flows_bwd, fwd_occ, bwd_occ, queries):
+    """Query point tracks through device flows a caller already holds, forward and backward in time from each query's frame.
+
+    `flows` / `flows_bwd`: planar [T-1,2,H,W], the forward flow of pair (t, t+1) and its backward flow (frame t+1 -> t) at
+    index t, in pixels at the frames' size (e.g. `infer_flow_video(..., pred_bidir_flow=True,
+    fwd_bwd_consistency_check=True)`'s 'flow' and 'flow_bwd'); `fwd_occ` / `bwd_occ`: their occlusion masks [T-1,H,W]
+    (1 = occluded) or None (nothing occluded).  `queries`: [N,3] (t_q, y, x), TAP-Vid's `query_points` layout, t_q an integer
+    frame index and (x, y) pixels with pixel centres at integers, inside the frame.
+    At t_q a track is the query, visible.  Forward (t > t_q) it is `chain_tracks`'s step through pair (t-1, t)'s forward
+    flow and `fwd_occ`; backward (t < t_q) the same step through pair (t, t+1)'s backward flow and `bwd_occ`.  One
+    `um_track_points_forward` and one `um_track_points_backward` launch.
+    Returns {'tracks': [N,T,2] fp32 (x, y), 'visible': [N,T] uint8} on the flows' device."""
+    if flows.dim() != 4 or flows.shape[1] != 2 or flows.shape[0] < 1:
+        raise ValueError("track_points expects the forward flows of at least one pair, planar [T-1,2,H,W]")
+    n, _, h, w = flows.shape
+    if tuple(flows_bwd.shape) != tuple(flows.shape):
+        raise ValueError("track_points: flows_bwd must be [T-1,2,H,W] like the flows")
+    for name, occ in (("fwd_occ", fwd_occ), ("bwd_occ", bwd_occ)):
+        if occ is not None and tuple(occ.shape) != (n, h, w):
+            raise ValueError("track_points: %s must be [T-1,H,W] like the flows" % name)
+    q = _point_queries(queries, h, w, "track_points")
+    _late_query(q, n + 1, "track_points")
+    dev = flows.device
+    nq, tmax = q.shape[0], int(q[:, 0].max())
+    qd = q.to(dev)
+    tracks = torch.empty((nq, n + 1, 2), device=dev, dtype=torch.float32)
+    visible = torch.empty((nq, n + 1), device=dev, dtype=torch.uint8)
+    pos = torch.empty((nq, 2), device=dev, dtype=torch.float32)
+    vis = torch.empty((nq,), device=dev, dtype=torch.uint8)
+
+    def f32(t):
+        return None if t is None else t.float().contiguous()
+    _OPS.track_points_forward(f32(flows), f32(fwd_occ), 0, qd, pos, vis, tracks, visible)
+    _OPS.track_points_backward(f32(flows_bwd[:tmax]), None if bwd_occ is None else f32(bwd_occ[:tmax]), qd, tracks, visible)
+    return {"tracks": tracks, "visible": visible}
+
+
+class PointTrackRunner(VideoFlowRunner):
+    """Query point tracks over a video: for N query points, each given at its own frame t_q, where the point is in every
+    frame of the clip, before and after t_q, and whether it is visible there (TAP-Vid's question).
+
+    The step is `VideoFlowRunner`'s with `pred_bidir_flow` and `fwd_bwd_consistency_check` always on.  After each step's
+    device work (graph replay or eager), on the same stream and outside the graph because the frame offset changes every
+    step: one `um_track_points_forward` launch advances every query from its frame through the step's real pairs (the
+    repeats that fill a short last step are never chained), and the backward flows and masks of the step's pairs below
+    max(t_q) are copied into a device history.  When the stream ends, one `um_track_points_backward` launch walks every
+    query from t_q back to frame 0 through that history, and the tables are downloaded once: N x T x 9 bytes.  Semantics:
+    `track_points`, which gives the same tracks on the runner's own flows bit for bit.
+    The history holds max(t_q) x 12 x H x W bytes (4.8 MB per pair at 480x832), allocated when `track()` starts and
+    released when it ends; queries all at frame 0 need none.
+    `track(frames, queries)` takes an iterable of at least two host uint8 frames [H,W,3] and queries [N,3] (t_q, y, x) as in
+    `track_points`, and returns {'tracks': [N,T,2] fp32, 'visible': [N,T] uint8} on the host; `return_flow=True` adds the
+    per-pair 'flow', 'flow_bwd', 'fwd_occ' and 'bwd_occ' [T-1, ...] that `VideoFlowRunner` returns, stacked (for tests and
+    short clips).  `pred_bwd_flow`, `visualize`, `concat_frame` and `visualize_bwd` are refused."""
+
+    def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
+                 return_flow=False, **model_kwargs):
+        for k in ("pred_bwd_flow", "visualize", "concat_frame", "visualize_bwd"):
+            if model_kwargs.pop(k, False):
+                raise ValueError("PointTrackRunner: %s is not supported (the tracks need the forward and backward flows "
+                                 "of every pair)" % k)
+        for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
+            if not model_kwargs.pop(k, True):
+                raise ValueError("PointTrackRunner: %s is always on (the occlusion masks decide visibility)" % k)
+        super().__init__(model, frame_size, batch, device, padding_factor=padding_factor, inference_size=inference_size,
+                         use_graph=use_graph, pred_bidir_flow=True, fwd_bwd_consistency_check=True, **model_kwargs)
+        self.return_flow = bool(return_flow)
+        self._pts = None
+
+    def _reserve(self, nframes):
+        """grow the device tables to at least `nframes` columns (doubling), keeping what is written"""
+        s = self._pts
+        cap = s["tracks"].shape[1]
+        if nframes <= cap:
+            return
+        cap = max(nframes, 2 * cap)
+        for k, shape in (("tracks", (s["nq"], cap, 2)), ("visible", (s["nq"], cap))):
+            grown = torch.empty(shape, device=self.dev, dtype=s[k].dtype)
+            grown[:, :s[k].shape[1]].copy_(s[k])
+            s[k] = grown
+
+    def _device_step(self, slot, chunk):
+        s = self._pts
+        if s is None:
+            raise RuntimeError("PointTrackRunner: call track(frames, queries), not run(frames)")
+        out = super()._device_step(slot, chunk)
+        t0, n = s["pairs"], len(chunk)
+        self._reserve(t0 + n + 1)
+        keep = min(n, s["tmax"] - t0)
+        if keep > 0:                       # backward flows and masks of the pairs below max(t_q)
+            s["flow_bwd"][t0:t0 + keep].copy_(out["flow_bwd"][:keep])
+            s["bwd_occ"][t0:t0 + keep].copy_(out["bwd_occ"][:keep])
+        _OPS.track_points_forward(out["flow"][:n].contiguous(), out["fwd_occ"][:n].contiguous(), t0, s["queries"], s["pos"],
+                                  s["vis"], s["tracks"], s["visible"])
+        s["pairs"] = t0 + n
+        return out if self.return_flow else {}
+
+    @torch.no_grad()
+    def track(self, frames, queries):
+        q = _point_queries(queries, self.h, self.w, "PointTrackRunner")
+        it = iter(frames)
+        head = list(itertools.islice(it, 2))
+        if len(head) < 2:
+            raise ValueError("PointTrackRunner: a clip needs at least two frames")
+        nq, tmax = q.shape[0], int(q[:, 0].max())
+        size = len(frames) if hasattr(frames, "__len__") else 0
+        with torch.cuda.device(self.dev):
+            dev, hw = self.dev, (self.h, self.w)
+            self._pts = {"nq": nq, "tmax": tmax, "pairs": 0, "queries": q.to(dev),
+                         "pos": torch.empty((nq, 2), device=dev), "vis": torch.empty((nq,), device=dev, dtype=torch.uint8),
+                         "tracks": torch.empty((nq, max(size, tmax + 1, 2), 2), device=dev),
+                         "visible": torch.empty((nq, max(size, tmax + 1, 2)), device=dev, dtype=torch.uint8),
+                         "flow_bwd": torch.empty((tmax, 2) + hw, device=dev), "bwd_occ": torch.empty((tmax,) + hw, device=dev)}
+            try:
+                per_pair = [{k: v.clone() for k, v in r.items()} for r in self.run(itertools.chain(head, it))]
+                s = self._pts
+                nframes = s["pairs"] + 1
+                _late_query(q, nframes, "PointTrackRunner")
+                _OPS.track_points_backward(s["flow_bwd"], s["bwd_occ"], s["queries"], s["tracks"], s["visible"])
+                res = {"tracks": s["tracks"][:, :nframes].contiguous().cpu(),
+                       "visible": s["visible"][:, :nframes].contiguous().cpu()}
+            finally:
+                self._pts = None
+        if self.return_flow:
+            res.update({k: torch.stack([r[k] for r in per_pair]) for k in ("flow", "flow_bwd", "fwd_occ", "bwd_occ")})
+        return res
 
 
 class DepthSequenceRunner(_SequenceRunner):

@@ -103,6 +103,8 @@ _SIGNATURES = {
     "um_fb_consistency": (_RC, [_P, _P, _F, _F, _P, _P, _I, _I, _I, _P]),
     "um_fb_consistency_ragged": (_RC, [_P, _L, _P, _F, _F, _P, _L, _P, _I, _I, _I, _P]),
     "um_chain_tracks": (_RC, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "um_track_points_forward": (_RC, [_P, _P, _I, _I, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P]),
+    "um_track_points_backward": (_RC, [_P, _P, _I, _I, _I, _P, _I, _I, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -361,6 +363,64 @@ def _chain_tracks(flow, occ, pos, vis):
 
 chain_tracks = _define("chain_tracks(Tensor flow, Tensor? occ, Tensor(a!) pos, Tensor(b!) vis) -> (Tensor, Tensor)",
                        _chain_tracks)
+
+
+def _point_tables(queries, tracks, visible, device):
+    """queries: contiguous fp32 [nq, 3] (t_q, y, x); tracks / visible: contiguous fp32 [nq, nt, 2] and uint8 [nq, nt]"""
+    _f32c(queries, "queries"), _f32c(tracks, "tracks")
+    if queries.dim() != 2 or queries.shape[1] != 3 or queries.device != device:
+        raise RuntimeError("track_points: queries must be [nq, 3] on the flows' device")
+    nq = queries.shape[0]
+    if tracks.dim() != 3 or tracks.shape[0] != nq or tracks.shape[2] != 2 or tracks.device != device:
+        raise RuntimeError("track_points: tracks must be [nq, nt, 2] on the flows' device")
+    if (visible.dtype != torch.uint8 or tuple(visible.shape) != tuple(tracks.shape[:2]) or not visible.is_contiguous()
+            or visible.device != device):
+        raise RuntimeError("track_points: visible must be contiguous uint8 [nq, nt] on the flows' device")
+    return nq, tracks.shape[1]
+
+
+def _flows_and_masks(flow, occ, name):
+    _f32c(flow, name)
+    if flow.dim() != 4 or flow.shape[1] != 2:
+        raise RuntimeError("%s: expected planar flows [n, 2, h, w]" % name)
+    if occ is not None:
+        _f32c(occ, "occ")
+        if tuple(occ.shape) != (flow.shape[0],) + tuple(flow.shape[2:]) or occ.device != flow.device:
+            raise RuntimeError("%s: occ must be [n, h, w] on the flows' device" % name)
+    return flow.shape[0], flow.shape[2], flow.shape[3]
+
+
+def _track_points_forward(flow, occ, t0, queries, pos, vis, tracks, visible):
+    """flow / occ: the forward flows [n, 2, h, w] and masks [n, h, w] (or None) of pairs t0 .. t0+n-1; queries [nq, 3];
+    pos / vis: the running state, contiguous fp32 [nq, 2] and uint8 [nq]; tracks / visible: the tables, written in place
+    (include/unimatch_sm100.h, um_track_points_forward)."""
+    n, h, w = _flows_and_masks(flow, occ, "track_points_forward")
+    nq, nt = _point_tables(queries, tracks, visible, flow.device)
+    _f32c(pos, "pos")
+    if tuple(pos.shape) != (nq, 2) or pos.device != flow.device:
+        raise RuntimeError("track_points_forward: pos must be [nq, 2] on the flows' device")
+    if vis.dtype != torch.uint8 or tuple(vis.shape) != (nq,) or vis.device != flow.device:
+        raise RuntimeError("track_points_forward: vis must be uint8 [nq] on the flows' device")
+    _check(LIB.um_track_points_forward(_p(flow), _p(occ), n, h, w, int(t0), _p(queries), nq, nt, _p(pos), _p(vis),
+                                       _p(tracks), _p(visible), _stream()), "um_track_points_forward")
+
+
+track_points_forward = _define("track_points_forward(Tensor flow, Tensor? occ, int t0, Tensor queries, Tensor(a!) pos, "
+                               "Tensor(b!) vis, Tensor(c!) tracks, Tensor(d!) visible) -> ()", _track_points_forward)
+
+
+def _track_points_backward(flow, occ, queries, tracks, visible):
+    """flow / occ: the backward flows [n, 2, h, w] and masks [n, h, w] (or None) of pairs 0 .. n-1, n >= 0; queries [nq, 3];
+    tracks / visible: the tables, entries 0 .. t_q of every row written in place (include/unimatch_sm100.h,
+    um_track_points_backward)."""
+    n, h, w = _flows_and_masks(flow, occ, "track_points_backward")
+    nq, nt = _point_tables(queries, tracks, visible, flow.device)
+    _check(LIB.um_track_points_backward(_p(flow) if n else None, _p(occ) if n else None, n, h, w, _p(queries), nq, nt,
+                                        _p(tracks), _p(visible), _stream()), "um_track_points_backward")
+
+
+track_points_backward = _define("track_points_backward(Tensor flow, Tensor? occ, Tensor queries, Tensor(a!) tracks, "
+                                "Tensor(b!) visible) -> ()", _track_points_backward)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
