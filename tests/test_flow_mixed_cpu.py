@@ -10,7 +10,7 @@ import torch
 
 import refops_flow_ragged
 from oracle import flow_viz as OV
-from unimatch_b200 import MixedSizeFlowRunner, MixedSizeStereoRunner, UniMatch, ops
+from unimatch_b200 import MixedSizeDepthRunner, MixedSizeFlowRunner, MixedSizeStereoRunner, UniMatch, ops
 from unimatch_b200.inference import RAGGED_ITEM, _MixedSizeRunner, _flow_step_layout
 
 ONE = ctypes.c_void_p(1024)          # any non-null address: validation never dereferences it
@@ -104,8 +104,11 @@ def test_portrait_and_landscape_share_a_bucket_and_max_buckets_flushes():
 
 def test_both_mixed_runners_share_one_implementation():
     for name in ("_capture_bucket", "_device_step", "_prepare_graphs", "_chunks", "_stage_host", "_download", "_results",
-                 "_reset_inputs", "run"):
+                 "_reset_inputs", "run", "_capture_graphs", "_frame", "_sizes", "_table"):
         assert getattr(MixedSizeFlowRunner, name) is getattr(MixedSizeStereoRunner, name) is getattr(_MixedSizeRunner, name)
+    for name in ("_capture_bucket", "_device_step", "_chunks", "_download", "_results", "run", "_frame", "_bucket",
+                 "_frame_order", "_layout", "_resize_back", "_returned"):
+        assert getattr(MixedSizeDepthRunner, name) is getattr(MixedSizeStereoRunner, name) is getattr(_MixedSizeRunner, name)
 
 
 def test_runner_argument_errors():

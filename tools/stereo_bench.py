@@ -80,7 +80,7 @@ def run(args):
     runner = StereoRunner(model, (H, W), B, dev, padding_factor=pad, visualize=True, **call)
     runner.pin[0][:B].copy_(lefts)
     runner.pin[0][B:].copy_(rights)
-    runner._capture()
+    runner._prepare_graphs()
     static = runner.static_out[0]
     out_r = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in static.items()}
 

@@ -138,7 +138,8 @@ def infer_flow(model, image1, image2, *, padding_factor, inference_size=None, pr
     multiple of `padding_factor` (or to `inference_size`), the flow is resized back and its components rescaled.
     Returns {'flow': [B,2,H,W]} plus 'flow_bwd' when `pred_bidir_flow` and 'fwd_occ' / 'bwd_occ' ([B,H,W], 1 = occluded)
     when `fwd_bwd_consistency_check`.  `model_kwargs` are forwarded to `model(...)` (attn_type, attn_splits_list, ...)."""
-    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, "infer_flow")
+    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check)
+    model_kwargs = _task_kwargs(model_kwargs, "flow", "infer_flow")
     transposed = image1.size(-2) > image1.size(-1)
     if transposed:
         image1, image2 = image1.transpose(-2, -1), image2.transpose(-2, -1)
@@ -150,11 +151,28 @@ def infer_flow(model, image1, image2, *, padding_factor, inference_size=None, pr
     return _flow_outputs(flow, ori, size, transposed, pred_bidir_flow, fwd_bwd_consistency_check)
 
 
-def _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, name):
+def _task_kwargs(model_kwargs, task, name):
+    """A copy of the model keywords without 'task' (the model's own default is "flow"; the stereo and depth paths pass
+    their task themselves), refused unless it names `task`."""
+    model_kwargs = dict(model_kwargs)
+    if model_kwargs.pop("task", task) != task:
+        raise ValueError("%s drives the %s task only" % (name, task))
+    return model_kwargs
+
+
+def _check_returns(return_value, visualize, option, name):
+    if not return_value and not visualize:
+        raise ValueError("%s: nothing to return: %s=False needs visualize=True" % (name, option))
+
+
+def _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check):
     if fwd_bwd_consistency_check and not pred_bidir_flow:
         raise ValueError("fwd_bwd_consistency_check needs pred_bidir_flow=True (evaluate_flow.py:774-792)")
-    if model_kwargs.setdefault("task", "flow") != "flow":
-        raise ValueError("%s drives the flow task only" % name)
+
+
+def _check_stereo_views(pred_bidir_disp, pred_right_disp, name):
+    if pred_bidir_disp and pred_right_disp:
+        raise ValueError("%s: choose one of pred_bidir_disp / pred_right_disp" % name)
 
 
 def _flow_outputs(flow, ori, size, transposed, pred_bidir_flow, fwd_bwd_consistency_check):
@@ -230,7 +248,8 @@ def infer_flow_video(model, frames, *, padding_factor, inference_size=None, pred
     `infer_flow(model, frames[:-1], frames[1:], ...)` returns for the T-1 consecutive pairs, with every frame encoded once
     (equal up to fp32 summation order, see `UniMatch.encode_frames`).
     `pred_bwd_flow`: each pair runs in swapped order (evaluate_flow.py:735-736), i.e. the flow from frame t+1 to frame t."""
-    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, model_kwargs, "infer_flow_video")
+    _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check)
+    model_kwargs = _task_kwargs(model_kwargs, "flow", "infer_flow_video")
     h, w = _frames_hw(frames, "infer_flow_video")
     transposed, ori, size = _frame_geometry(h, w, padding_factor, inference_size, "flow")
     feats = model.encode_frames(_frames_to_model(frames, "flow", transposed, size))
@@ -249,8 +268,7 @@ def infer_stereo(model, left, right, *, padding_factor=16, inference_size=None, 
     `pred_bidir_disp`: the right-view disparity comes from the SAME network on the mirrored, swapped pair, batched with the
     original pair (hflip trick, :789-792) and mirrored back (:829-836); `pred_right_disp`: only that.  Returns
     {'disp': [B,H,W]} (+ 'disp_right' for the bidirectional case); disparities are rescaled by the width ratio."""
-    if pred_bidir_disp and pred_right_disp:
-        raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
+    _check_stereo_views(pred_bidir_disp, pred_right_disp, "infer_stereo")
     ori = tuple(left.shape[-2:])
     size = _inference_size(ori, padding_factor, inference_size)
     if size != ori:
@@ -306,17 +324,22 @@ def disparity_to_image(disp, out=None):
     for a batch: disparities [N,H,W] -> uint8 BGR pictures [N,H,W,3] (cv2's channel order, ready for cv2.imwrite), each image
     min-max scaled to 0..255 and coloured with cv2's INFERNO map; a single disparity [H,W] gives one picture [H,W,3].  `out`
     may be a view into larger pictures (3-byte pixels, any row / image stride).  One min / max pass and one colouring pass."""
-    if not torch.is_tensor(disp) or disp.dim() not in (2, 3) or not disp.dtype.is_floating_point or 0 in disp.shape:
-        raise ValueError("disparity_to_image expects float disparities [N,H,W] or [H,W]")
-    shape = tuple(disp.shape) + (3,)
+    return _to_image(disp, out, _OPS.disparity_to_image, "disparity_to_image", "disparities")
+
+
+def _to_image(x, out, op, name, what):
+    """float maps [N,H,W] or [H,W] -> uint8 pictures [..., 3] through the colouring op `op(maps [N,H,W], out [N,H,W,3])`"""
+    if not torch.is_tensor(x) or x.dim() not in (2, 3) or not x.dtype.is_floating_point or 0 in x.shape:
+        raise ValueError("%s expects float %s [N,H,W] or [H,W]" % (name, what))
+    shape = tuple(x.shape) + (3,)
     if out is None:
-        out = torch.empty(shape, device=disp.device, dtype=torch.uint8)
+        out = torch.empty(shape, device=x.device, dtype=torch.uint8)
     elif not torch.is_tensor(out) or tuple(out.shape) != shape or out.dtype != torch.uint8:
-        raise ValueError("disparity_to_image: out must be uint8 %s" % (list(shape),))
-    if disp.dim() == 2:
-        _OPS.disparity_to_image(disp[None].float().contiguous(), out[None])
+        raise ValueError("%s: out must be uint8 %s" % (name, list(shape)))
+    if x.dim() == 2:
+        op(x[None].float().contiguous(), out[None])
     else:
-        _OPS.disparity_to_image(disp.float().contiguous(), out)
+        op(x.float().contiguous(), out)
     return out
 
 
@@ -345,17 +368,16 @@ def depth_to_image(depth, out=None):
     matplotlib's `plasma`; a single depth [H,W] gives one picture [H,W,3].  `out` may be a view into larger pictures (3-byte
     pixels, any row / image stride).  A radix select of the two order statistics, then one colouring pass; see
     oracle/depth_viz.py for the arithmetic and the edge cases (NaN, zero or negative depths)."""
-    if not torch.is_tensor(depth) or depth.dim() not in (2, 3) or not depth.dtype.is_floating_point or 0 in depth.shape:
-        raise ValueError("depth_to_image expects float depths [N,H,W] or [H,W]")
-    shape = tuple(depth.shape) + (3,)
-    if out is None:
-        out = torch.empty(shape, device=depth.device, dtype=torch.uint8)
-    elif not torch.is_tensor(out) or tuple(out.shape) != shape or out.dtype != torch.uint8:
-        raise ValueError("depth_to_image: out must be uint8 %s" % (list(shape),))
-    if depth.dim() == 2:
-        _OPS.depth_to_image(depth[None].float().contiguous(), out[None])
-    else:
-        _OPS.depth_to_image(depth.float().contiguous(), out)
+    return _to_image(depth, out, _OPS.depth_to_image, "depth_to_image", "depths")
+
+
+def _colour_outputs(out, key, colour, keep):
+    """Adds the picture of every output in `out` (all named `key`*) as 'vis'* ('disp_right' -> 'vis_right'), colouring with
+    `colour`; the outputs themselves are dropped unless `keep`."""
+    for k in list(out):
+        out[k.replace(key, "vis")] = colour(out[k])
+        if not keep:
+            del out[k]
     return out
 
 
@@ -370,12 +392,6 @@ def _depth_outputs(depth, ori, size, pred_bidir_depth):
 
 
 # ---------------------------------------------------------------------------------------------- depth over posed sequences
-def _depth_task_kwargs(model_kwargs, name):
-    if model_kwargs.pop("task", "depth") != "depth":
-        raise ValueError("%s drives the depth task only" % name)
-    return model_kwargs
-
-
 def _intrinsics33(intrinsics, name):
     """The sequence's one intrinsics matrix (the reference reads one file per sequence, evaluate_depth.py:331, :343) as float32 [3,3]."""
     if not (torch.is_tensor(intrinsics) or isinstance(intrinsics, np.ndarray)) or tuple(intrinsics.shape) != (3, 3):
@@ -400,9 +416,13 @@ def _relative_poses(poses, bidir):
     reference's own expression, pair by pair (evaluate_depth.py:344-350): inv(pose[t+1]) @ pose[t] in numpy float32.  With
     `bidir` the inverses of those (np.linalg.inv) follow, for the backward streams: float32 [n,4,4] or [2n,4,4], the layout
     `UniMatch.depth_cameras` takes."""
-    rel = [np.linalg.inv(poses[t + 1]) @ poses[t] for t in range(len(poses) - 1)]
+    return _with_inverses([np.linalg.inv(poses[t + 1]) @ poses[t] for t in range(len(poses) - 1)], bidir)
+
+
+def _with_inverses(rel, bidir):
+    """Relative poses [4,4] stacked as float32 [n,4,4], followed with `bidir` by their inverses (np.linalg.inv)."""
     if bidir:
-        rel += [np.linalg.inv(r) for r in rel]
+        rel = rel + [np.linalg.inv(r) for r in rel]
     return np.stack(rel).astype(np.float32)
 
 
@@ -418,7 +438,7 @@ def infer_depth_sequence(model, frames, intrinsics, poses, *, padding_factor=16,
     inv(pose[t+1]) @ pose[t], computed on the host in numpy float32 as the reference does (and its inverse there too when
     `pred_bidir_depth`).  Returns what `infer_depth` returns on those pairs: {'depth': [T-1,H,W]} (+ 'depth_bwd'), equal up to
     fp32 summation order (see `UniMatch.encode_frames`)."""
-    model_kwargs = _depth_task_kwargs(model_kwargs, "infer_depth_sequence")
+    model_kwargs = _task_kwargs(model_kwargs, "depth", "infer_depth_sequence")
     h, w = _frames_hw(frames, "infer_depth_sequence")
     T = frames.shape[0]
     if len(poses) != T:
@@ -445,7 +465,7 @@ class _PipelinedRunner:
     returns a dict of device tensors whose first axis is the batch, the default `_download(slot, out)` (enqueue the D2H
     copies of a step's outputs into pinned buffers) and `_results(slot, n)` (one dict of host tensors per item) apply.
     Runners whose steps are not all one shape override `_chunks` (how items form steps), `_prepare_graphs` and
-    `_device_step` (which graph replays a step)."""
+    `_device_step` (which graph replays a step); all capture through `_capture_graphs`."""
 
     def _init_pipeline(self, device, use_graph):
         self.dev = torch.device(device)
@@ -467,26 +487,32 @@ class _PipelinedRunner:
         for i in range(n):
             yield {k: v[i] for k, v in self.out_pin[slot].items()}
 
-    def _capture(self):
+    def _capture_graphs(self, step, reset):
+        """One CUDA graph of `step(slot)` per staging slot, after the slots in `reset` are reset to valid inputs and two
+        eager warm-up rounds of both slots on a side stream (they build the module's cached operand planes outside the
+        capture).  Returns (graphs, outputs, held buffers): the graphs hold the raw addresses of the module's cached planes,
+        and calls at other shapes may evict them from the module's caches, so the runner keeps them alive for as long as
+        it may replay."""
         with torch.cuda.device(self.dev):
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):
-                for _ in range(2):            # eager warm-up: builds the module's cached operand planes outside the capture
+                for slot in reset:
+                    self._reset_inputs(slot)
+                for _ in range(2):
                     for slot in range(2):
-                        self._reset_inputs(slot)
-                        self._step(slot)
+                        step(slot)
             torch.cuda.current_stream().wait_stream(side)
             torch.cuda.synchronize()
+            graphs, outs = [], []
             for slot in range(2):
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    self.static_out[slot] = self._step(slot)
-                self.graphs[slot] = g
-            # the graphs hold the raw addresses of the module's cached planes; calls at other shapes may evict them from
-            # the module's caches, so the runner keeps them alive for as long as it may replay
-            self._held_buffers = self.model.cached_buffers()
+                    outs.append(step(slot))
+                graphs.append(g)
+            held = self.model.cached_buffers()
             torch.cuda.synchronize()
+        return graphs, outs, held
 
     def _stage(self, slot, chunk):
         """host side of one batch, then the H2D copies on the side stream; returns their completion event.  The slot's
@@ -504,7 +530,7 @@ class _PipelinedRunner:
     def _prepare_graphs(self):
         """Before the first step: the one-shape runners capture both slots' graphs here."""
         if self.use_graph and self.graphs[0] is None:
-            self._capture()
+            self.graphs, self.static_out, self._held_buffers = self._capture_graphs(self._step, (0, 1))
 
     def _chunks(self, items):
         """The steps' items: `self.batch` at a time, read as each step is staged."""
@@ -562,6 +588,11 @@ class _PipelinedRunner:
         done_ev.synchronize()
         yield from self._results(slot ^ 1, done_n)
 
+    @torch.no_grad()
+    def run(self, pairs):
+        with torch.cuda.device(self.dev):
+            yield from self._pipeline(pairs)
+
 
 class BatchedFlowRunner(_PipelinedRunner):
     """Fixed-bucket, double-buffered, graph-replayed flow inference for a stream of host frame pairs.
@@ -613,11 +644,6 @@ class BatchedFlowRunner(_PipelinedRunner):
         for i in range(n):
             yield self.padder.unpad(self.out_pin[slot][i])
 
-    @torch.no_grad()
-    def run(self, pairs):
-        with torch.cuda.device(self.dev):
-            yield from self._pipeline(pairs)
-
 
 class StereoRunner(_PipelinedRunner):
     """Streaming stereo inference over host (left, right) uint8 frame pairs: `inference_stereo` (evaluate_stereo.py:711-843)
@@ -641,13 +667,9 @@ class StereoRunner(_PipelinedRunner):
 
     def __init__(self, model, frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
                  pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, **model_kwargs):
-        if pred_bidir_disp and pred_right_disp:
-            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
-        if not return_disp and not visualize:
-            raise ValueError("nothing to return: return_disp=False needs visualize=True")
-        self.kw = dict(model_kwargs)
-        if self.kw.pop("task", "stereo") != "stereo":
-            raise ValueError("StereoRunner drives the stereo task only")
+        _check_stereo_views(pred_bidir_disp, pred_right_disp, "StereoRunner")
+        _check_returns(return_disp, visualize, "return_disp", "StereoRunner")
+        self.kw = _task_kwargs(model_kwargs, "stereo", "StereoRunner")
         self.model, self.batch = model, int(batch)
         if self.batch < 1:
             raise ValueError("StereoRunner: batch must be positive")
@@ -662,12 +684,7 @@ class StereoRunner(_PipelinedRunner):
 
     def _step(self, slot):
         out = _stereo_from_frames(self.model, self.dev_in[slot], **self.geometry, **self.kw)
-        if self.visualize:
-            for k in [k for k in ("disp", "disp_right") if k in out]:
-                out[k.replace("disp", "vis")] = disparity_to_image(out[k])
-                if not self.return_disp:
-                    del out[k]
-        return out
+        return _colour_outputs(out, "disp", disparity_to_image, self.return_disp) if self.visualize else out
 
     def _reset_inputs(self, slot):
         self.dev_in[slot].zero_()
@@ -686,15 +703,41 @@ class StereoRunner(_PipelinedRunner):
             self.pin[slot][self.batch + i].copy_(self._frame(right))
         self.dev_in[slot].copy_(self.pin[slot], non_blocking=True)
 
-    @torch.no_grad()
-    def run(self, pairs):
-        with torch.cuda.device(self.dev):
-            yield from self._pipeline(pairs)
-
 
 # um_ragged_item (include/unimatch_sm100.h) as a numpy record, for building descriptor tables on the host
 RAGGED_ITEM = np.dtype([("offset", "<i8"), ("h", "<i4"), ("w", "<i4"), ("scale", "<f4"), ("flags", "<i4")])
 assert RAGGED_ITEM.itemsize == ops.RAGGED_ITEM_BYTES
+
+
+def _frame_table(halves, batch, flags=None):
+    """The 2*batch items of a step's packed uint8 frames: `halves` = (sizes of the real pairs' first frames, sizes of their
+    second frames), packed back to back in that order, item i of each half with `flags[i]` (0 without `flags`).  The items
+    of a short step's filler pairs point at its last pair's frames, so fillers upload nothing.  Returns (items, bytes)."""
+    frames = np.zeros(2 * batch, RAGGED_ITEM)
+    off = 0
+    for half, sizes in enumerate(halves):
+        n = len(sizes)
+        for i, (h, w) in enumerate(sizes):
+            frames[half * batch + i] = (off, h, w, 1.0, flags[i] if flags else 0)
+            off += 3 * h * w
+        frames[half * batch + n:(half + 1) * batch] = frames[half * batch + n - 1]
+    return frames, off
+
+
+def _scalar_outputs(keys, sizes, batch, scales=None, flags=None):
+    """The len(keys)*batch items of a step's packed one-channel outputs: per key in turn, the real pairs' outputs of sizes
+    `sizes` back to back, output i with scale `scales[i]` (1 without `scales`) and flags `flags[k]` of its key (0 without
+    `flags`); fillers are empty items, which the kernels skip.  Returns (items, elements used, per real pair the
+    (key, offset, h, w) of each of its outputs)."""
+    outputs = np.zeros(len(keys) * batch, RAGGED_ITEM)
+    results = [[] for _ in sizes]
+    used = 0
+    for k, key in enumerate(keys):
+        for i, (h, w) in enumerate(sizes):
+            outputs[k * batch + i] = (used, h, w, scales[i] if scales else 1.0, flags[k] if flags else 0)
+            results[i].append((key, used, h, w))
+            used += h * w
+    return outputs, used, results
 
 
 def _ragged_step_layout(sizes, batch, size, pred_bidir_disp, pred_right_disp):
@@ -707,26 +750,12 @@ def _ragged_step_layout(sizes, batch, size, pred_bidir_disp, pred_right_disp):
       `_stereo_outputs` does), flipped for the right view; fillers are empty items, which the kernels skip;
     * frame_bytes / out_pixels: the used prefixes of the packed buffers;
     * results: per real pair, the (key, offset, h, w) of each of its outputs."""
-    n = len(sizes)
-    frames = np.zeros(2 * batch, RAGGED_ITEM)
-    off = 0
-    for side in range(2):
-        for i, (h, w) in enumerate(sizes):
-            frames[side * batch + i] = (off, h, w, 1.0, 0)
-            off += 3 * h * w
-        frames[side * batch + n:(side + 1) * batch] = frames[side * batch + n - 1]
+    frames, nbytes = _frame_table((sizes, sizes), batch)
     keys = ("disp", "disp_right") if pred_bidir_disp else ("disp",)
-    outputs = np.zeros(len(keys) * batch, RAGGED_ITEM)
-    results = [[] for _ in sizes]
-    used = 0
-    for k, key in enumerate(keys):
-        flags = ops.RAGGED_FLIP_X if (pred_right_disp or key == "disp_right") else 0
-        for i, (h, w) in enumerate(sizes):
-            scale = np.float32(w / float(size[1])) if (h, w) != tuple(size) else np.float32(1.0)
-            outputs[k * batch + i] = (used, h, w, scale, flags)
-            results[i].append((key, used, h, w))
-            used += h * w
-    return frames, outputs, off, used, results
+    scales = [np.float32(w / float(size[1])) if (h, w) != tuple(size) else np.float32(1.0) for h, w in sizes]
+    flags = [ops.RAGGED_FLIP_X if (pred_right_disp or key == "disp_right") else 0 for key in keys]
+    outputs, used, results = _scalar_outputs(keys, sizes, batch, scales, flags)
+    return frames, outputs, nbytes, used, results
 
 
 class _MixedSizeRunner(_PipelinedRunner):
@@ -737,13 +766,21 @@ class _MixedSizeRunner(_PipelinedRunner):
     recently used bucket's graphs and held buffers dropped when `max_buckets` buckets hold graphs; packed outputs of which
     the used prefixes are downloaded; `(index, result)` in completion order; `stats`.
 
-    A subclass provides `_bucket(pair)` (the size the model sees), `_frame_order(pairs)` (the step's frames in the order they
-    are packed), `_layout(sizes, size)` (`sizes` as `_sizes(pairs)` gives them) (the step's descriptor table as one record array, the used elements of each output
-    buffer, and per real pair its result views as (key, buffer, offset, shape)) and `_step(slot, size)` (the device work on
-    `dev_in[slot]` / `dev_desc[slot]`, returning {buffer: packed device tensor})."""
+    A subclass sets `value_key` (its value output, 'disp' / 'depth' / 'flow', of `value_planes` channels), stores its
+    `visualize` and `return_<value_key>` options (`_returned`) before `_init_mixed`, and provides
+    `_step(slot, size)` (the device work on `dev_in[slot]` / `dev_desc[slot]`, returning {buffer: packed device tensor}) and
+    either `_step_layout(sizes, size)` (the step's frame and one-channel output tables as `_ragged_step_layout` returns them;
+    `sizes` as `_sizes(pairs)` gives them) or its own `_layout(sizes, size)` (the step's descriptor table as one record
+    array, the used elements of each output buffer, and per real pair its result views as (key, buffer, offset, shape)).
+    The default `_bucket(pair)` (the size the model sees) is the first frame's inference size, and the default
+    `_frame_order(pairs)` packs the step's first frames, then its second frames."""
 
-    def _init_mixed(self, model, max_frame_size, batch, device, use_graph, max_buckets, n_desc, out_buffers):
-        """`n_desc`: items of a step's table; `out_buffers`: {buffer: (dtype, elements per pixel of capacity and pair)}"""
+    value_planes = 1
+
+    def _init_mixed(self, model, max_frame_size, batch, device, use_graph, max_buckets, n_desc, views, extra=None):
+        """`n_desc`: items of a step's table; `views`: outputs per pair and key (2 when bidirectional).  The output buffers,
+        each as (dtype, elements per pixel of capacity and pair): `value_key` when returned, then `extra`, then the uint8
+        RGB pictures 'vis' when returned."""
         name = type(self).__name__
         self.model, self.batch, self.max_buckets = model, int(batch), int(max_buckets)
         if self.batch < 1 or self.max_buckets < 1:
@@ -751,6 +788,13 @@ class _MixedSizeRunner(_PipelinedRunner):
         self.hmax, self.wmax = int(max_frame_size[0]), int(max_frame_size[1])
         if self.hmax < 1 or self.wmax < 1 or self.hmax * self.wmax > 0x7fffffff:
             raise ValueError("%s: max_frame_size must be positive, at most 2^31 - 1 pixels" % name)
+        out_buffers = {}
+        if self._returned(self.value_key):
+            out_buffers[self.value_key] = (torch.float32, self.value_planes * views)
+        out_buffers.update(extra or {})
+        if self._returned("vis"):
+            out_buffers["vis"] = (torch.uint8, 3 * views)
+        self.buffers = tuple(out_buffers)
         self._init_pipeline(device, use_graph)
         cap = self.hmax * self.wmax
         self.pin = [torch.empty((2 * self.batch * cap * 3,), dtype=torch.uint8).pin_memory() for _ in range(2)]
@@ -764,19 +808,36 @@ class _MixedSizeRunner(_PipelinedRunner):
         self.buckets = collections.OrderedDict()  # inference size -> (graphs, outputs, held buffers), least recent first
         self.stats = {"steps": 0, "pairs": 0, "captures": 0, "h2d_bytes": 0, "d2h_bytes": 0}
 
+    def _returned(self, buffer):
+        """whether the runner returns `buffer`: 'vis' with `visualize`, the value buffer unless its constructor option
+        `return_disp` / `return_flow` / `return_depth` is False"""
+        return self.visualize if buffer == "vis" else getattr(self, "return_" + buffer)
+
     # ---- host side
-    def _pair(self, pair):
+    def _frame(self, frame):
+        """a host frame as a uint8 [h, w, 3] tensor within the capacity"""
         name = type(self).__name__
-        first, second = (torch.as_tensor(f) for f in pair)
-        for f in (first, second):
-            if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                raise ValueError("%s: frames must be uint8 [h, w, 3]" % name)
-        if first.shape != second.shape:
-            raise ValueError("%s: the two frames of a pair must have the same size" % name)
-        if not (1 <= first.shape[0] <= self.hmax and 1 <= first.shape[1] <= self.wmax):
+        f = torch.as_tensor(frame)
+        if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
+            raise ValueError("%s: frames must be uint8 [h, w, 3]" % name)
+        if not (1 <= f.shape[0] <= self.hmax and 1 <= f.shape[1] <= self.wmax):
             raise ValueError("%s: a %dx%d frame exceeds max_frame_size %dx%d"
-                             % (name, first.shape[0], first.shape[1], self.hmax, self.wmax))
+                             % (name, f.shape[0], f.shape[1], self.hmax, self.wmax))
+        return f
+
+    def _pair(self, pair):
+        first, second = (self._frame(f) for f in pair)
+        if first.shape != second.shape:
+            raise ValueError("%s: the two frames of a pair must have the same size" % type(self).__name__)
         return first, second
+
+    def _bucket(self, pair):
+        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+
+    @staticmethod
+    def _frame_order(pairs):
+        """the step's first frames, then its second frames"""
+        return [p[0] for p in pairs] + [p[1] for p in pairs]
 
     def _chunks(self, items):
         checked = ((i, self._pair(p)) for i, p in items)
@@ -790,6 +851,16 @@ class _MixedSizeRunner(_PipelinedRunner):
     def _table(self, sizes, size):
         table, used, results = self._layout(sizes, size)
         return table.view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES), used, results
+
+    def _layout(self, sizes, size):
+        """the frame and output tables of `_step_layout`, with each output's value view and its picture's 'vis' view,
+        of the buffers the runner returns"""
+        frames, outputs, _, used, results = self._step_layout(sizes, size)
+        key = self.value_key
+        views = [[v for k, off, h, w in outs
+                  for v in ((k, key, off, (h, w)), (k.replace(key, "vis"), "vis", 3 * off, (h, w, 3)))
+                  if self._returned(v[1])] for outs in results]
+        return np.concatenate((frames, outputs)), {key: used, "vis": 3 * used}, views
 
     def _stage_host(self, slot, chunk):
         """the step's packed frames and descriptor table into pinned memory, then their H2D copies (used bytes only)"""
@@ -833,25 +904,9 @@ class _MixedSizeRunner(_PipelinedRunner):
     def _capture_bucket(self, slot, size):
         """Both slots' graphs of bucket `size`, while `slot` holds a staged step of that bucket (its inputs are used as they
         are for the eager warm-up) and the other slot is free (reset to valid descriptors)."""
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            self._reset_inputs(slot ^ 1)
-            for _ in range(2):                     # eager warm-up: builds the module's cached operand planes for this shape
-                for s in range(2):
-                    self._step(s, size)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        graphs, outs = [], []
-        for s in range(2):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                outs.append(self._step(s, size))
-            graphs.append(g)
-        held = self.model.cached_buffers()         # see _PipelinedRunner._capture
-        torch.cuda.synchronize()
+        entry = self._capture_graphs(lambda s: self._step(s, size), (slot ^ 1,))
         self.stats["captures"] += 1
-        return graphs, outs, held
+        return entry
 
     def _device_step(self, slot, chunk):
         size = self.meta[slot]["size"]
@@ -867,6 +922,20 @@ class _MixedSizeRunner(_PipelinedRunner):
         graphs, outs, _ = entry
         graphs[slot].replay()
         return outs[slot]
+
+    def _resize_back(self, values, items, colour):
+        """The model's one-channel outputs [N, 1, H, W] at the bucket size resized back into the packed `value_key`
+        buffer by their output `items` (`um_resize_bilinear_ragged`), and their pictures by the ragged colouring op
+        `colour` when 'vis' is returned."""
+        packed = _OPS.resize_bilinear_ragged(values.contiguous(), items, self.hmax, self.wmax,
+                                             items.shape[0] * self.hmax * self.wmax)
+        out = {}
+        if self._returned(self.value_key):
+            out[self.value_key] = packed
+        if self._returned("vis"):
+            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
+            colour(packed, items, out["vis"], self.hmax, self.wmax)
+        return out
 
     @torch.no_grad()
     def run(self, pairs):
@@ -902,64 +971,30 @@ class MixedSizeStereoRunner(_MixedSizeRunner):
     (+ 'vis_right'); `return_disp=False` with `visualize` sends back only the pictures.  The views point into reused pinned
     staging -- copy what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
 
+    value_key = "disp"
+
     def __init__(self, model, max_frame_size, batch, device, padding_factor=16, inference_size=None, pred_bidir_disp=False,
                  pred_right_disp=False, visualize=False, return_disp=True, use_graph=True, max_buckets=4, **model_kwargs):
-        if pred_bidir_disp and pred_right_disp:
-            raise ValueError("choose one of pred_bidir_disp / pred_right_disp")
-        if not return_disp and not visualize:
-            raise ValueError("nothing to return: return_disp=False needs visualize=True")
-        self.kw = dict(model_kwargs)
-        if self.kw.pop("task", "stereo") != "stereo":
-            raise ValueError("MixedSizeStereoRunner drives the stereo task only")
+        name = type(self).__name__
+        _check_stereo_views(pred_bidir_disp, pred_right_disp, name)
+        _check_returns(return_disp, visualize, "return_disp", name)
+        self.kw = _task_kwargs(model_kwargs, "stereo", name)
         self.padding_factor, self.inference_size = padding_factor, inference_size
         self.bidir, self.right = bool(pred_bidir_disp), bool(pred_right_disp)
         self.visualize, self.return_disp = bool(visualize), bool(return_disp)
         views = 2 if self.bidir else 1
-        buffers = {}
-        if self.return_disp:
-            buffers["disp"] = (torch.float32, views)
-        if self.visualize:
-            buffers["vis"] = (torch.uint8, 3 * views)
-        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), buffers)
+        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), views)
 
-    # ---- host side
-    def _bucket(self, pair):
-        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+    def _step_layout(self, sizes, size):
+        return _ragged_step_layout(sizes, self.batch, size, self.bidir, self.right)
 
-    @staticmethod
-    def _frame_order(pairs):
-        """the step's left frames, then its right frames"""
-        return [p[0] for p in pairs] + [p[1] for p in pairs]
-
-    def _layout(self, sizes, size):
-        frames, outputs, _, used, results = _ragged_step_layout(sizes, self.batch, size, self.bidir, self.right)
-        views = []
-        for outs in results:
-            views.append([])
-            for key, off, h, w in outs:
-                if self.return_disp:
-                    views[-1].append((key, "disp", off, (h, w)))
-                if self.visualize:
-                    views[-1].append((key.replace("disp", "vis"), "vis", 3 * off, (h, w, 3)))
-        return np.concatenate((frames, outputs)), {"disp": used, "vis": 3 * used}, views
-
-    # ---- device side
     def _step(self, slot, size):
         b, nf = self.batch, 2 * self.batch
         items = self.dev_desc[slot]
         planes = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:nf], self.hmax, self.wmax, int(size[0]),
                                                          int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
         disp = _stereo_forward(self.model, planes[:b], planes[b:], self.bidir, self.right, dict(self.kw))
-        out_items = items[nf:]
-        packed = _OPS.resize_bilinear_ragged(disp.contiguous(), out_items, self.hmax, self.wmax,
-                                             out_items.shape[0] * self.hmax * self.wmax)
-        out = {}
-        if self.return_disp:
-            out["disp"] = packed
-        if self.visualize:
-            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
-            _OPS.disparity_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
-        return out
+        return self._resize_back(disp, items[nf:], _OPS.disparity_to_image_ragged)
 
 
 def _flow_step_layout(sizes, batch, size, pred_bidir_flow, fwd_bwd_consistency_check):
@@ -977,15 +1012,8 @@ def _flow_step_layout(sizes, batch, size, pred_bidir_flow, fwd_bwd_consistency_c
     * masks: with `fwd_bwd_consistency_check`, 2*batch items, the pairs' 'fwd_occ' [h, w], then their 'bwd_occ';
     * frame_bytes: the used prefix of the packed frames; used: {'flow': floats, 'vis': bytes, 'occ': floats};
     * results: per real pair, the (key, buffer, offset, shape) of each of its outputs."""
-    n = len(sizes)
-    frames = np.zeros(2 * batch, RAGGED_ITEM)
-    off = 0
-    for half in range(2):
-        for i, (h, w) in enumerate(sizes):
-            frames[half * batch + i] = (off, h, w, 1.0, ops.RAGGED_TRANSPOSE if h > w else 0)
-            off += 3 * h * w
-        frames[half * batch + n:(half + 1) * batch] = frames[half * batch + n - 1]
-    keys = ("flow", "flow_bwd") if pred_bidir_flow else ("flow",)
+    frames, off = _frame_table((sizes, sizes), batch, [ops.RAGGED_TRANSPOSE if h > w else 0 for h, w in sizes])
+    keys =("flow", "flow_bwd") if pred_bidir_flow else ("flow",)
     planes = np.zeros(2 * len(keys) * batch, RAGGED_ITEM)
     flows, pictures = np.zeros(len(keys) * batch, RAGGED_ITEM), np.zeros(len(keys) * batch, RAGGED_ITEM)
     masks = np.zeros(2 * batch if fwd_bwd_consistency_check else 0, RAGGED_ITEM)
@@ -1038,31 +1066,26 @@ class MixedSizeFlowRunner(_MixedSizeRunner):
     the pictures.  The views point into reused pinned staging -- copy what you keep.  `stats` counts steps, pairs, captures
     and the bytes copied each way."""
 
+    value_key, value_planes = "flow", 2
+
     def __init__(self, model, max_frame_size, batch, device, padding_factor=32, inference_size=None, pred_bidir_flow=False,
                  pred_bwd_flow=False, fwd_bwd_consistency_check=False, visualize=False, return_flow=True, use_graph=True,
                  max_buckets=4, **model_kwargs):
-        self.kw = dict(model_kwargs)
-        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "MixedSizeFlowRunner")
-        if not return_flow and not visualize:
-            raise ValueError("nothing to return: return_flow=False needs visualize=True")
+        name = type(self).__name__
+        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check)
+        self.kw = _task_kwargs(model_kwargs, "flow", name)
+        _check_returns(return_flow, visualize, "return_flow", name)
         if not return_flow and fwd_bwd_consistency_check:
             raise ValueError("return_flow=False sends back pictures only: it excludes fwd_bwd_consistency_check")
         self.padding_factor, self.inference_size = padding_factor, inference_size
         self.bidir, self.bwd, self.check = bool(pred_bidir_flow), bool(pred_bwd_flow), bool(fwd_bwd_consistency_check)
         self.visualize, self.return_flow = bool(visualize), bool(return_flow)
         dirs = 2 if self.bidir else 1
-        buffers = {}
-        if self.return_flow:
-            buffers["flow"] = (torch.float32, 2 * dirs)
-        if self.check:
-            buffers["occ"] = (torch.float32, 2)
-        if self.visualize:
-            buffers["vis"] = (torch.uint8, 3 * dirs)
         if self.check and min(max_frame_size) < 2:
             raise ValueError("MixedSizeFlowRunner: fwd_bwd_consistency_check needs frames of at least 2x2")
-        self.buffers = tuple(buffers)
         self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets,
-                         (2 + 4 * dirs + (2 if self.check else 0)) * int(batch), buffers)
+                         (2 + 4 * dirs + (2 if self.check else 0)) * int(batch), dirs,
+                         {"occ": (torch.float32, 2)} if self.check else None)
 
     # ---- host side
     def _pair(self, pair):
@@ -1202,14 +1225,14 @@ class VideoFlowRunner(_SequenceRunner):
     def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
                  visualize=False, concat_frame=False, pred_bidir_flow=False, fwd_bwd_consistency_check=False,
                  return_flow=True, pred_bwd_flow=False, visualize_bwd=False, **model_kwargs):
-        self.kw = dict(model_kwargs)
-        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check, self.kw, "VideoFlowRunner")
+        name = type(self).__name__
+        _check_flow_args(pred_bidir_flow, fwd_bwd_consistency_check)
+        self.kw = _task_kwargs(model_kwargs, "flow", name)
         if concat_frame and not visualize:
             raise ValueError("concat_frame needs visualize=True")
         if visualize_bwd and not (visualize and pred_bidir_flow):
             raise ValueError("visualize_bwd needs visualize=True and pred_bidir_flow=True")
-        if not return_flow and not visualize:
-            raise ValueError("nothing to return: return_flow=False needs visualize=True")
+        _check_returns(return_flow, visualize, "return_flow", name)
         self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.check = bool(pred_bidir_flow), bool(fwd_bwd_consistency_check)
         self.visualize, self.concat, self.return_flow = bool(visualize), bool(concat_frame), bool(return_flow)
@@ -1252,6 +1275,17 @@ def _track_start(h, w, device):
     ys, xs = torch.meshgrid(torch.arange(h, device=device, dtype=torch.float32),
                             torch.arange(w, device=device, dtype=torch.float32), indexing="ij")
     return torch.stack((xs, ys), dim=-1).contiguous(), torch.ones((h, w), device=device, dtype=torch.uint8)
+
+
+def _track_flags(model_kwargs, name, reason):
+    """Takes out of a track runner's keywords the `VideoFlowRunner` flags it fixes: the ones that would change which
+    flows it chains are refused (`reason` says why), and the bidirectional flow with its occlusion masks is always on."""
+    for k in ("pred_bwd_flow", "visualize", "concat_frame", "visualize_bwd"):
+        if model_kwargs.pop(k, False):
+            raise ValueError("%s: %s is not supported (%s)" % (name, k, reason))
+    for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
+        if not model_kwargs.pop(k, True):
+            raise ValueError("%s: %s is always on (the occlusion masks decide visibility)" % (name, k))
 
 
 @torch.no_grad()
@@ -1299,12 +1333,7 @@ class VideoTrackRunner(VideoFlowRunner):
 
     def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
                  return_flow=False, **model_kwargs):
-        for k in ("pred_bwd_flow", "visualize", "concat_frame", "visualize_bwd"):
-            if model_kwargs.pop(k, False):
-                raise ValueError("VideoTrackRunner: %s is not supported (tracks run forward from the first frame)" % k)
-        for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
-            if not model_kwargs.pop(k, True):
-                raise ValueError("VideoTrackRunner: %s is always on (the forward occlusion mask decides visibility)" % k)
+        _track_flags(model_kwargs, "VideoTrackRunner", "tracks run forward from the first frame")
         super().__init__(model, frame_size, batch, device, padding_factor=padding_factor, inference_size=inference_size,
                          use_graph=use_graph, pred_bidir_flow=True, fwd_bwd_consistency_check=True, **model_kwargs)
         self.return_flow = bool(return_flow)
@@ -1405,13 +1434,7 @@ class PointTrackRunner(VideoFlowRunner):
 
     def __init__(self, model, frame_size, batch, device, padding_factor=32, inference_size=None, use_graph=True,
                  return_flow=False, **model_kwargs):
-        for k in ("pred_bwd_flow", "visualize", "concat_frame", "visualize_bwd"):
-            if model_kwargs.pop(k, False):
-                raise ValueError("PointTrackRunner: %s is not supported (the tracks need the forward and backward flows "
-                                 "of every pair)" % k)
-        for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
-            if not model_kwargs.pop(k, True):
-                raise ValueError("PointTrackRunner: %s is always on (the occlusion masks decide visibility)" % k)
+        _track_flags(model_kwargs, "PointTrackRunner", "the tracks need the forward and backward flows of every pair")
         super().__init__(model, frame_size, batch, device, padding_factor=padding_factor, inference_size=inference_size,
                          use_graph=use_graph, pred_bidir_flow=True, fwd_bwd_consistency_check=True, **model_kwargs)
         self.return_flow = bool(return_flow)
@@ -1476,7 +1499,37 @@ class PointTrackRunner(VideoFlowRunner):
         return res
 
 
-class DepthSequenceRunner(_SequenceRunner):
+class _PosedDepth:
+    """What the two depth runners share: per staging slot, the step's relative poses in a pinned and a device buffer of
+    views * batch [4,4] matrices, the camera operands built on them once, eagerly, before any capture (they depend on
+    the intrinsics only; `UniMatch.depth_cameras` takes a float32 pose of all the step's matrices as it is, so
+    `cams[slot]["pose"]` IS `pose_dev[slot]` and an upload updates the cameras), and the depth matching path on them.
+    The runner sets `model`, `batch`, `dev`, `kw`, `bidir`, `from_argmax` and `inv_range` first."""
+
+    def _init_poses(self, intrinsics, num_depth_candidates):
+        npose = (2 if self.bidir else 1) * self.batch
+        self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
+        self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
+        Kb = intrinsics.to(self.dev)[None].repeat(self.batch, 1, 1)
+        self.cams = [self.model.depth_cameras(Kb, self.pose_dev[s], self.model.upsample_factor, *self.inv_range,
+                                              num_depth_candidates, self.bidir) for s in range(2)]
+
+    def _reset_poses(self, slot):
+        self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
+
+    def _stage_poses(self, slot, rel):
+        """the step's relative poses, float32 [views * batch, 4, 4], into pinned memory, then their H2D copy"""
+        self.pose_pin[slot].copy_(torch.from_numpy(rel))
+        self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
+
+    def _depth(self, slot, first, second):
+        """the model's depths [views * batch, H, W] at the inference size, from the pairs' encoded features"""
+        return self.model.forward_encoded(first, second, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
+                                          max_depth=self.inv_range[1], depth_from_argmax=self.from_argmax,
+                                          pred_bidir_depth=self.bidir, **self.kw)["flow_preds"][-1]
+
+
+class DepthSequenceRunner(_PosedDepth, _SequenceRunner):
     """Streaming depth over a posed frame sequence: consecutive pairs of host (uint8 frame, absolute pose) items, every frame
     uploaded and encoded once -- the depth counterpart of `VideoFlowRunner`.
 
@@ -1500,21 +1553,14 @@ class DepthSequenceRunner(_SequenceRunner):
     def __init__(self, model, frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None, min_depth=0.5,
                  max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False, use_graph=True,
                  visualize=False, return_depth=True, **model_kwargs):
-        if not return_depth and not visualize:
-            raise ValueError("nothing to return: return_depth=False needs visualize=True")
-        self.kw = _depth_task_kwargs(dict(model_kwargs), "DepthSequenceRunner")
+        _check_returns(return_depth, visualize, "return_depth", "DepthSequenceRunner")
+        self.kw = _task_kwargs(model_kwargs, "depth", "DepthSequenceRunner")
         self.visualize, self.return_depth = bool(visualize), bool(return_depth)
         K = _intrinsics33(intrinsics, "DepthSequenceRunner")
         self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
         self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
         self.inv_range = (1.0 / max_depth, 1.0 / min_depth)                      # the model works on inverse depth
-        npose = (2 if self.bidir else 1) * self.batch
-        self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
-        self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
-        Kb = K.to(self.dev)[None].repeat(self.batch, 1, 1)
-        # cams[slot]["pose"] IS pose_dev[slot] (a float32 pose of 2B matrices is taken as it is), so the upload updates it
-        self.cams = [model.depth_cameras(Kb, self.pose_dev[s], model.upsample_factor, *self.inv_range, num_depth_candidates,
-                                         self.bidir) for s in range(2)]
+        self._init_poses(K, num_depth_candidates)
         self.prev_pose = None                              # last frame's absolute pose, float32 [4,4] on the host
 
     @staticmethod
@@ -1525,27 +1571,18 @@ class DepthSequenceRunner(_SequenceRunner):
         self.prev_pose = _pose44(first[1], "DepthSequenceRunner")
 
     def _match(self, slot, first, second):
-        depth = self.model.forward_encoded(first, second, task="depth", cameras=self.cams[slot], min_depth=self.inv_range[0],
-                                           max_depth=self.inv_range[1], depth_from_argmax=self.from_argmax,
-                                           pred_bidir_depth=self.bidir, **self.kw)["flow_preds"][-1]
-        out = _depth_outputs(depth, self.ori, self.size, self.bidir)
-        if self.visualize:
-            for k in [k for k in ("depth", "depth_bwd") if k in out]:
-                out[k.replace("depth", "vis")] = depth_to_image(out[k])
-                if not self.return_depth:
-                    del out[k]
-        return out
+        out = _depth_outputs(self._depth(slot, first, second), self.ori, self.size, self.bidir)
+        return _colour_outputs(out, "depth", depth_to_image, self.return_depth) if self.visualize else out
 
     def _reset_inputs(self, slot):
         super()._reset_inputs(slot)
-        self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
+        self._reset_poses(slot)
 
     def _stage_host(self, slot, chunk):
         """the frames, then the relative poses of the step's pairs, continuing from the carried pose"""
         poses = [self.prev_pose] + [_pose44(pose, "DepthSequenceRunner") for _, pose in super()._stage_host(slot, chunk)]
-        self.pose_pin[slot].copy_(torch.from_numpy(_relative_poses(poses, self.bidir)))
+        self._stage_poses(slot, _relative_poses(poses, self.bidir))
         self.prev_pose = poses[-1]
-        self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
 
 
 def _depth_step_layout(sizes, batch, pred_bidir_depth):
@@ -1558,28 +1595,13 @@ def _depth_step_layout(sizes, batch, pred_bidir_depth):
       which the kernels skip;
     * frame_bytes / used: the used prefixes of the packed frames and depths;
     * results: per real pair, the (key, offset, h, w) of each of its outputs."""
-    n = len(sizes)
-    frames = np.zeros(2 * batch, RAGGED_ITEM)
-    off = 0
-    for k in range(2):
-        for i, pair in enumerate(sizes):
-            h, w = pair[k]
-            frames[k * batch + i] = (off, h, w, 1.0, 0)
-            off += 3 * h * w
-        frames[k * batch + n:(k + 1) * batch] = frames[k * batch + n - 1]
+    frames, nbytes = _frame_table(tuple(zip(*sizes)), batch)
     keys = ("depth", "depth_bwd") if pred_bidir_depth else ("depth",)
-    outputs = np.zeros(len(keys) * batch, RAGGED_ITEM)
-    results = [[] for _ in sizes]
-    used = 0
-    for k, key in enumerate(keys):
-        for i, ((h, w), _) in enumerate(sizes):
-            outputs[k * batch + i] = (used, h, w, 1.0, 0)
-            results[i].append((key, used, h, w))
-            used += h * w
-    return frames, outputs, off, used, results
+    outputs, used, results = _scalar_outputs(keys, [t for t, _ in sizes], batch)
+    return frames, outputs, nbytes, used, results
 
 
-class MixedSizeDepthRunner(_MixedSizeRunner):
+class MixedSizeDepthRunner(_PosedDepth, _MixedSizeRunner):
     """Streaming depth over posed pairs of ANY size up to `max_frame_size`: `inference_depth` (evaluate_depth.py:338-417),
     which takes each pair at its own size, as a stream.  Each item is one pair (uint8 frame t [h, w, 3], uint8 frame t+1
     [h', w', 3], relative pose [4, 4]); the relative pose is the reference's host float32 `inv(pose[t+1]) @ pose[t]`, as
@@ -1606,83 +1628,46 @@ class MixedSizeDepthRunner(_MixedSizeRunner):
     `return_depth=False` with `visualize` sends back only the pictures.  The views point into reused pinned staging -- copy
     what you keep.  `stats` counts steps, pairs, captures and the bytes copied each way."""
 
+    value_key = "depth"
+
     def __init__(self, model, max_frame_size, batch, device, intrinsics, padding_factor=16, inference_size=None,
                  min_depth=0.5, max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
                  visualize=False, return_depth=True, use_graph=True, max_buckets=4, **model_kwargs):
-        if not return_depth and not visualize:
-            raise ValueError("nothing to return: return_depth=False needs visualize=True")
-        self.kw = _depth_task_kwargs(dict(model_kwargs), "MixedSizeDepthRunner")
-        K = _intrinsics33(intrinsics, "MixedSizeDepthRunner")
+        name = type(self).__name__
+        _check_returns(return_depth, visualize, "return_depth", name)
+        self.kw = _task_kwargs(model_kwargs, "depth", name)
+        K = _intrinsics33(intrinsics, name)
         self.padding_factor, self.inference_size = padding_factor, inference_size
         self.bidir, self.from_argmax = bool(pred_bidir_depth), bool(depth_from_argmax)
         self.visualize, self.return_depth = bool(visualize), bool(return_depth)
         self.inv_range = (1.0 / max_depth, 1.0 / min_depth)                      # the model works on inverse depth
         views = 2 if self.bidir else 1
-        buffers = {}
-        if self.return_depth:
-            buffers["depth"] = (torch.float32, views)
-        if self.visualize:
-            buffers["vis"] = (torch.uint8, 3 * views)
-        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), buffers)
-        npose = views * self.batch
-        self.pose_pin = [torch.empty((npose, 4, 4)).pin_memory() for _ in range(2)]
-        self.pose_dev = [torch.eye(4, device=self.dev).repeat(npose, 1, 1) for _ in range(2)]
-        Kb = K.to(self.dev)[None].repeat(self.batch, 1, 1)
-        # cams[slot]["pose"] IS pose_dev[slot] (a float32 pose of 2B matrices is taken as it is), so the upload updates it
-        self.cams = [model.depth_cameras(Kb, self.pose_dev[s], model.upsample_factor, *self.inv_range, num_depth_candidates,
-                                         self.bidir) for s in range(2)]
+        self._init_mixed(model, max_frame_size, batch, device, use_graph, max_buckets, (2 + views) * int(batch), views)
+        self._init_poses(K, num_depth_candidates)
 
     # ---- host side
     def _pair(self, pair):
         name = type(self).__name__
         if len(pair) != 3:
             raise ValueError("%s: an item is (frame t, frame t+1, relative pose)" % name)
-        frames = tuple(torch.as_tensor(f) for f in pair[:2])
-        for f in frames:
-            if f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3:
-                raise ValueError("%s: frames must be uint8 [h, w, 3]" % name)
-            if not (1 <= f.shape[0] <= self.hmax and 1 <= f.shape[1] <= self.wmax):
-                raise ValueError("%s: a %dx%d frame exceeds max_frame_size %dx%d"
-                                 % (name, f.shape[0], f.shape[1], self.hmax, self.wmax))
-        return frames + (_pose44(pair[2], name),)
-
-    def _bucket(self, pair):
-        return _inference_size(tuple(pair[0].shape[:2]), self.padding_factor, self.inference_size)
+        return self._frame(pair[0]), self._frame(pair[1]), _pose44(pair[2], name)
 
     @staticmethod
     def _sizes(pairs):
         return [(tuple(p[0].shape[:2]), tuple(p[1].shape[:2])) for p in pairs]
 
-    @staticmethod
-    def _frame_order(pairs):
-        """the step's frames t, then its frames t+1"""
-        return [p[0] for p in pairs] + [p[1] for p in pairs]
-
-    def _layout(self, sizes, size):
-        frames, outputs, _, used, results = _depth_step_layout(sizes, self.batch, self.bidir)
-        views = []
-        for outs in results:
-            views.append([])
-            for key, off, h, w in outs:
-                if self.return_depth:
-                    views[-1].append((key, "depth", off, (h, w)))
-                if self.visualize:
-                    views[-1].append((key.replace("depth", "vis"), "vis", 3 * off, (h, w, 3)))
-        return np.concatenate((frames, outputs)), {"depth": used, "vis": 3 * used}, views
+    def _step_layout(self, sizes, size):
+        return _depth_step_layout(sizes, self.batch, self.bidir)
 
     def _poses(self, pairs):
         """the step's relative poses, a short step's last one repeated, then with `pred_bidir_depth` their inverses
-        (np.linalg.inv in float32, as `_relative_poses` forms them): float32 [views * batch, 4, 4]"""
-        rel = [pairs[min(i, len(pairs) - 1)][2] for i in range(self.batch)]
-        if self.bidir:
-            rel += [np.linalg.inv(r) for r in rel]
-        return np.stack(rel).astype(np.float32)
+        (as `_relative_poses` forms them): float32 [views * batch, 4, 4]"""
+        return _with_inverses([pairs[min(i, len(pairs) - 1)][2] for i in range(self.batch)], self.bidir)
 
     def _stage_host(self, slot, chunk):
         """the packed frames and the table (`_MixedSizeRunner`), then the step's relative poses"""
         super()._stage_host(slot, chunk)
-        self.pose_pin[slot].copy_(torch.from_numpy(self._poses([p for _, p in chunk])))
-        self.pose_dev[slot].copy_(self.pose_pin[slot], non_blocking=True)
+        self._stage_poses(slot, self._poses([p for _, p in chunk]))
         self.stats["h2d_bytes"] += self.pose_pin[slot].nbytes
 
     # ---- device side
@@ -1692,7 +1677,7 @@ class MixedSizeDepthRunner(_MixedSizeRunner):
         table, _, _ = self._table([(cap, cap)] * self.batch, cap)
         self.dev_in[slot].zero_()
         self.dev_desc[slot].copy_(torch.from_numpy(table))
-        self.pose_dev[slot].copy_(torch.eye(4, device=self.dev).expand_as(self.pose_dev[slot]))
+        self._reset_poses(slot)
 
     def _step(self, slot, size):
         b = self.batch
@@ -1700,17 +1685,5 @@ class MixedSizeDepthRunner(_MixedSizeRunner):
         x = _OPS.frames_to_planar_normalized_ragged(self.dev_in[slot], items[:2 * b], self.hmax, self.wmax, int(size[0]),
                                                     int(size[1]), list(IMAGENET_MEAN), list(IMAGENET_STD))
         feats = self.model.encode_frames(x, task="depth")
-        depth = self.model.forward_encoded([f[:b] for f in feats], [f[b:] for f in feats], task="depth",
-                                           cameras=self.cams[slot], min_depth=self.inv_range[0], max_depth=self.inv_range[1],
-                                           depth_from_argmax=self.from_argmax, pred_bidir_depth=self.bidir,
-                                           **self.kw)["flow_preds"][-1]                     # [views * b, H, W]
-        out_items = items[2 * b:]
-        packed = _OPS.resize_bilinear_ragged(depth.contiguous().view(depth.shape[0], 1, *depth.shape[-2:]), out_items,
-                                             self.hmax, self.wmax, out_items.shape[0] * self.hmax * self.wmax)
-        out = {}
-        if self.return_depth:
-            out["depth"] = packed
-        if self.visualize:
-            out["vis"] = torch.empty((3 * packed.numel(),), dtype=torch.uint8, device=self.dev)
-            _OPS.depth_to_image_ragged(packed, out_items, out["vis"], self.hmax, self.wmax)
-        return out
+        depth = self._depth(slot, [f[:b] for f in feats], [f[b:] for f in feats])                 # [views * b, H, W]
+        return self._resize_back(depth.unsqueeze(1), items[2 * b:], _OPS.depth_to_image_ragged)
