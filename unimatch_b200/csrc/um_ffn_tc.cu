@@ -6,13 +6,23 @@
 // activation travels through HBM as fp16 (hi, lo) planes -- 4 KB per token row, 1.6 GB at 8 pairs of 480x832.  Here it
 // never leaves the registers: one CTA per 128-row tile, warp-specialised:
 //
-//   warp 8          TMA producer: the tile's [source | message] planes (128 KB, resident for the tile), then a 5-slot ring
-//                   of 16 KB weight tiles in the order the consumers use them: W1(c) as 4 K-slices, W2(c) as 2 row halves
-//   warpgroups 0-1  consumers, 64 rows each, for every 64-wide hidden chunk c:
-//                   H_c = X W1_c^T (48 wgmma 64x64x16, both operands in shared memory) into registers -> exact-erf GELU ->
-//                   (hi, lo) fp16 pairs, which are already the register A operand of O += P_c W2_c^T (24 wgmma 64x64x16);
-//                   after the last chunk: LayerNorm (two-pass statistics over the 4 threads of a row) + residual on O,
-//                   fp32 rows and / or fp16 planes out.
+//   warp 8          TMA producer: the tile's [source | message] planes (128 KB, resident for the tile), then a 3-slot ring
+//                   of 32 KB weight tiles in the order the consumers use them: W1(c) as 4 K-slices of 128 hidden rows,
+//                   W2(c) as 2 K-halves (64 hidden channels x 128 output rows); warps 9-11 only hand back their registers
+//   warpgroups 0-1  consumers, 64 rows each, for every 128-wide hidden chunk c:
+//                   H_c = X W1_c^T (48 wgmma 64x128x16, both operands in shared memory, one commit group per K-slice so
+//                   a slice is released while the next ones run) into 64 registers -> exact-erf GELU -> (hi, lo) fp16
+//                   pairs in the same registers, which are already the register A operand of O += P_c W2_c^T (24 wgmma
+//                   64x128x16, K = 128 as 8 k-steps, one commit group per half: the GELU of the second half runs under
+//                   the MMAs of the first); after the last chunk: LayerNorm (two-pass statistics over the 4 threads of a
+//                   row) + residual on O, fp32 rows and / or fp16 planes out.
+//                   The warpgroups take turns at issuing (named barriers 2 and 3), one slot's group per turn, so each
+//                   group runs on the tensor pipe in one piece and the warpgroups stay a group apart: one's GELU and
+//                   LayerNorm run under the other's MMAs.
+// A chunk of 128 (not 64) hidden channels halves the shared-memory bytes per MMA of H_c: a 64x64x16 MMA reads 4 KB of
+// operands in 32 tensor clocks, which with both warpgroups issuing is the whole 128 B/clk of the SM's shared memory.
+// Every output element is summed in the same order as with 64-wide chunks (K-slice, split term, k-step for H; 64-wide
+// hidden block, split term, k-step for O), so the result does not depend on the chunk width.
 #include "um_common.cuh"
 #include "um_tc.cuh"
 
@@ -22,14 +32,19 @@ using namespace tc;
 
 namespace {
 
-constexpr int NTHREADS = 288;                        // 2 consumer warpgroups (warps 0-7) + one TMA producer warp (warp 8)
+constexpr int NTHREADS = 384;                        // 2 consumer warpgroups (warps 0-7) + the TMA producer's warpgroup
 constexpr int PRODUCER = 8;
-constexpr int HC = 64;                               // hidden channels per chunk
+// per-thread registers of each role (setmaxnreg): 128 x 40 + 256 x 232 <= the 64 K register file.  A consumer holds O and
+// H_c / P_c (64 + 64) plus the operand addressing.
+constexpr int REGS_PRODUCER = 40, REGS_CONSUMER = 232;
+constexpr int TURN = 2;                              // named barriers 2 and 3: the consumer warpgroups' MMA turns
+constexpr int HC = 128;                              // hidden channels per chunk
 constexpr uint32_t X_BYTES = 4 * 32768;              // 4 K-slices x (hi, lo) x [128 rows x 64 ch]
-constexpr uint32_t SLOT_BYTES = 16384;               // (hi, lo) x [64 weight rows x 64 k]
-constexpr int NSLOT = 5;
+constexpr uint32_t SLOT_BYTES = 32768;               // (hi, lo) x [128 weight rows x 64 k]
+constexpr uint32_t PART_BYTES = SLOT_BYTES / 2;
+constexpr int NSLOT = 3;
 constexpr uint32_t OFF_RING = X_BYTES;
-constexpr uint32_t OFF_BAR = OFF_RING + NSLOT * SLOT_BYTES;        // 212992
+constexpr uint32_t OFF_BAR = OFF_RING + NSLOT * SLOT_BYTES;        // 229376
 constexpr uint32_t SMEM_BYTES = OFF_BAR + 256;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 
@@ -62,7 +77,9 @@ ffn_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant_
   }
   __syncthreads();
 
-  if (warp == PRODUCER) {
+  if (warp >= PRODUCER) {
+    setmaxnreg_dec<REGS_PRODUCER>();
+    if (warp != PRODUCER) return;
     if (elect_one()) {
       mbar_arrive_expect_tx(x_full, X_BYTES);
 #pragma unroll
@@ -82,8 +99,8 @@ ffn_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant_
           mbar_arrive_expect_tx(full + s, SLOT_BYTES);
 #pragma unroll
           for (int part = 0; part < 2; ++part) {
-            if (q < 4) tma_load_2d(slot + part * 8192, &map_w1, full + s, q * 64, part * p.hidden + c * HC);
-            else tma_load_2d(slot + part * 8192, &map_w2, full + s, c * HC, part * 128 + (q - 4) * 64);
+            if (q < 4) tma_load_2d(slot + part * PART_BYTES, &map_w1, full + s, q * 64, part * p.hidden + c * HC);
+            else tma_load_2d(slot + part * PART_BYTES, &map_w2, full + s, c * HC + (q - 4) * 64, part * 128);
           }
         }
         __syncwarp();
@@ -92,78 +109,102 @@ ffn_tc_kernel(const __grid_constant__ CUtensorMap map_x0, const __grid_constant_
   }
 
   // =============================== consumers ===============================
+  setmaxnreg_inc<REGS_CONSUMER>();
   const int wg = warp >> 2;
   const int fr = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows fr and fr + 8 (MMA fragment layout)
   const int fc = 2 * (lane & 3);                            // ... and columns 8 j + fc + {0, 1}
   const uint32_t x_base = smem_u32(smem) + wg * 8192;
+  const uint32_t ring = smem_u32(smem + OFF_RING);
   const int pa[3] = {1, 0, 0}, pb[3] = {0, 1, 0};          // lo*hi, hi*lo, hi*hi
+  // the slot of the ring position `it` and the parity its fill completes with
+  auto wait_full = [&](int it) {
+    const int s = it % NSLOT;
+    mbar_wait_inline(full + s, (it / NSLOT) & 1);
+    return ring + s * SLOT_BYTES;
+  };
+  auto release = [&](int it) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty + it % NSLOT);
+  };
+  // The two warpgroups take turns at issuing MMAs, one weight slot's group per turn, warpgroup 0 first: named barrier
+  // TURN + w is warpgroup w's turn.  Each group then runs on the tensor pipe in one piece, so the warpgroups stay a group
+  // apart and one's GELU (or LayerNorm) runs under the other's MMAs.  Warpgroup 0 does not wait for its first turn and
+  // warpgroup 1 does not pass on its last, so every arrive meets a sync.
+  const int last_turn = 6 * p.nchunk - 1;
+  auto turn_begin = [&](int it) {
+    if (wg == 0) {
+      if (it > 0) asm volatile("bar.sync %0, 256;" ::"n"(TURN) : "memory");
+    } else {
+      asm volatile("bar.sync %0, 256;" ::"n"(TURN + 1) : "memory");
+    }
+  };
+  auto turn_end = [&](int it) {
+    if (wg == 0) asm volatile("bar.arrive %0, 256;" ::"n"(TURN + 1) : "memory");
+    else if (it < last_turn) asm volatile("bar.arrive %0, 256;" ::"n"(TURN) : "memory");
+  };
   float o[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
   mbar_wait_inline(x_full, 0);
   int it = 0;
   for (int c = 0; c < p.nchunk; ++c) {
-    // ---- H_c = X W1_c^T: 64 rows x 64 hidden channels, K = 256 in 4 slots ----
-    float h[32];
-    int sl[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      sl[q] = (it + q) % NSLOT;
-      mbar_wait_inline(full + sl[q], ((it + q) / NSLOT) & 1);
-    }
+    // ---- H_c = X W1_c^T: 64 rows x 128 hidden channels, K = 256 in 4 slots.  A slot is released as soon as its
+    //      group has retired (wait<1> after the next group is issued), so the ring keeps filling under the MMAs ----
+    float h[64];
     fence_acc(h);
-    wgmma_fence();
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const uint32_t sb = smem_u32(smem + OFF_RING + sl[q] * SLOT_BYTES);
+      turn_begin(it + q);
+      const uint32_t sb = wait_full(it + q);
+      wgmma_fence();
 #pragma unroll
       for (int cc = 0; cc < 3; ++cc)
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks)
-          wgmma_ss<64>(h, desc_kmajor(x_base + (q * 2 + pa[cc]) * 16384 + ks * 32), desc_kmajor(sb + pb[cc] * 8192 + ks * 32),
-                       (q | cc | ks) != 0);
+          wgmma_ss<128>(h, desc_kmajor(x_base + (q * 2 + pa[cc]) * 16384 + ks * 32),
+                        desc_kmajor(sb + pb[cc] * PART_BYTES + ks * 32), (q | cc | ks) != 0);
+      wgmma_commit();
+      turn_end(it + q);
+      if (q > 0) {
+        wgmma_wait<1>();
+        release(it + q - 1);
+      }
     }
-    wgmma_commit();
     wgmma_wait<0>();
     fence_acc(h);
-    __syncwarp();
-    if (lane == 0)
-#pragma unroll
-      for (int q = 0; q < 4; ++q) mbar_arrive(empty + sl[q]);
+    release(it + 3);
     it += 4;
-    // ---- GELU -> fp16 (hi, lo) pairs in the A-operand layout of the next MMA ----
-    uint32_t ph[16], pl[16];
-#pragma unroll
-    for (int jj = 0; jj < 8; ++jj)
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-        split_f16x2(act_gelu(h[4 * jj + 2 * hh]), act_gelu(h[4 * jj + 2 * hh + 1]), &ph[2 * jj + hh], &pl[2 * jj + hh]);
-    // ---- O += P_c W2_c^T: output channels [0, 64) and [64, 128) from one slot each ----
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      sl[q] = (it + q) % NSLOT;
-      mbar_wait_inline(full + sl[q], ((it + q) / NSLOT) & 1);
-    }
+    // ---- O += P_c W2_c^T, hidden channels [0, 64) and [64, 128) of the chunk from one slot each.  P_c is GELU(H_c) as
+    //      fp16 (hi, lo) pairs in the A-operand layout, formed in place one half at a time: the second half's GELU runs
+    //      under the first half's MMAs ----
+    uint32_t ph[32], pl[32];
     fence_acc(o);
-    wgmma_fence();
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
-      const uint32_t sb = smem_u32(smem + OFF_RING + sl[q] * SLOT_BYTES);
-      float (&oq)[32] = *reinterpret_cast<float (*)[32]>(o + 32 * q);
+#pragma unroll
+      for (int jj = 8 * q; jj < 8 * q + 8; ++jj)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh)
+          split_f16x2(act_gelu(h[4 * jj + 2 * hh]), act_gelu(h[4 * jj + 2 * hh + 1]), &ph[2 * jj + hh], &pl[2 * jj + hh]);
+      turn_begin(it + q);
+      const uint32_t sb = wait_full(it + q);
+      wgmma_fence();
 #pragma unroll
       for (int cc = 0; cc < 3; ++cc)
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks) {
-          const uint32_t* pp = cc == 0 ? pl : ph;
-          const uint32_t a[4] = {pp[4 * ks], pp[4 * ks + 1], pp[4 * ks + 2], pp[4 * ks + 3]};
-          wgmma_rs_n64(oq, a, desc_kmajor(sb + (cc == 1 ? 8192 : 0) + ks * 32), true);
+          const uint32_t* pp = (cc == 0 ? pl : ph) + 16 * q + 4 * ks;
+          const uint32_t a[4] = {pp[0], pp[1], pp[2], pp[3]};
+          wgmma_rs_n128(o, a, desc_kmajor(sb + (cc == 1 ? PART_BYTES : 0) + ks * 32), true);
         }
+      wgmma_commit();
+      turn_end(it + q);
     }
-    wgmma_commit();
+    wgmma_wait<1>();
+    release(it);
     wgmma_wait<0>();
     fence_acc(o);
-    __syncwarp();
-    if (lane == 0) { mbar_arrive(empty + sl[0]); mbar_arrive(empty + sl[1]); }
+    release(it + 1);
     it += 2;
   }
 
@@ -234,8 +275,8 @@ int um_ffn_tc(const um_ffn_desc* d, void* stream) {
   int rc;
   if ((rc = make_map_4d_f16(&mx0, d->src[0], 128, 16, gh, 2, 1, (uint64_t)d->src_plane_stride))) return rc;
   if ((rc = make_map_4d_f16(&mx1, d->src[1], 128, 16, gh, 2, 1, (uint64_t)d->src_plane_stride))) return rc;
-  if ((rc = make_map_2d_f16(&mw1, d->w1, 2ull * d->hidden, 256, 64))) return rc;
-  if ((rc = make_map_2d_f16(&mw2, d->w2, 2ull * 128, (uint64_t)d->hidden, 64))) return rc;
+  if ((rc = make_map_2d_f16(&mw1, d->w1, 2ull * d->hidden, 256, HC))) return rc;
+  if ((rc = make_map_2d_f16(&mw2, d->w2, 2ull * 128, (uint64_t)d->hidden, 128))) return rc;
   FfnParams p{};
   p.nchunk = d->hidden / HC; p.hidden = d->hidden;
   p.residual = d->residual; p.ld_res = d->ld_res; p.gamma = d->gamma; p.beta = d->beta;
