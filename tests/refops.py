@@ -2,7 +2,8 @@
 (oracle/unimatch_oracle.py restates the reference functions; pinned by tests/golden).  Test infrastructure:
 
   * `-m gpu` parity tests compare each CUDA op with the function of the same name here on identical inputs;
-  * `register_cpu_kernels()` installs these functions as the ops' CPU kernels *inside the test process only*,
+  * `register_cpu_kernels()` installs these functions, and those of the other tests/refops_*.py modules (the table
+    `cpu_statements()`), as the ops' CPU kernels *inside the test process only*,
     so the host orchestration of `unimatch_b200.UniMatch` can be checked end to end against the oracle on a
     machine without a GPU.  The product never does this: outside tests the ops have no CPU kernel.
 """
@@ -322,18 +323,35 @@ def ffn_tc(src0, src1, w1, w2, residual, gamma, beta, out_f32, out_split, rows):
               gamma=gamma, beta=beta, rows=rows)
 
 
-ALL = ["split_planes", "conv7x7_small", "conv2d_tc", "ffn_tc", "instance_norm_stats", "instance_norm_apply", "window_attention", "window_attention_planes", "softmax_expectation", "local_corr_softmax", "local_corr_volume", "flow_warp", "fb_consistency",
-       "propagate_local", "depth_corr_softmax", "add_position", "convex_upsample", "upsample2x", "resize_bilinear"]
+def cpu_statements():
+    """{op name: CPU statement} of every unimatch_sm100 op that has one.  The statements of the video, depth, stereo, ragged
+    and evaluation ops live in modules that import this one, hence the imports here."""
+    import refops_depth
+    import refops_eval
+    import refops_flow_ragged
+    import refops_ragged
+    import refops_stereo
+    import refops_video
+    return {f.__name__: f for f in (
+        split_planes, conv7x7_small, conv2d_tc, ffn_tc, instance_norm_stats, instance_norm_apply, window_attention,
+        window_attention_planes, softmax_expectation, local_corr_softmax, local_corr_volume, flow_warp, fb_consistency,
+        propagate_local, depth_corr_softmax, add_position, convex_upsample, upsample2x, resize_bilinear,
+        refops_video.frames_to_planar, refops_video.flow_to_image, refops_depth.frames_to_planar_normalized,
+        refops_stereo.disparity_to_image, refops_ragged.frames_to_planar_normalized_ragged,
+        refops_ragged.resize_bilinear_ragged, refops_ragged.disparity_to_image_ragged,
+        refops_flow_ragged.frames_to_planar_ragged, refops_flow_ragged.flow_to_image_ragged,
+        refops_flow_ragged.fb_consistency_ragged, refops_eval.eval_stats)}
+
 
 _registered = []
 
 
 def register_cpu_kernels():
-    """Install the functions above as CPU kernels of the unimatch_sm100 ops (tests only)."""
+    """Install every statement of cpu_statements() as the CPU kernel of its op (tests only), all of them at the first call:
+    a test sees the same CPU kernels whichever tests ran before it in the process."""
     if _registered:
         return
     lib = torch.library.Library("unimatch_sm100", "IMPL", "CPU")
-    g = globals()
-    for name in ALL:
-        lib.impl(name, g[name])
+    for name, fn in cpu_statements().items():
+        lib.impl(name, fn)
     _registered.append(lib)

@@ -1,11 +1,7 @@
 """CPU statement of the depth-sequence op `frames_to_planar_normalized` (test infrastructure, like tests/refops.py and
-tests/refops_video.py): the `-m gpu` tests compare the CUDA op with it, and `register_cpu_kernels()` installs it -- together
-with every op of refops.py and refops_video.py -- as a CPU kernel inside the test process, so the host logic of the depth
-sequence drivers runs on a machine without a GPU."""
-import torch
-
+tests/refops_video.py): the `-m gpu` tests compare the CUDA op with it, and `refops.register_cpu_kernels()` installs it as a
+CPU kernel inside the test process, so the host logic of the depth sequence drivers runs on a machine without a GPU."""
 import refops
-import refops_video
 
 
 def normalize_frames(frames, mean, std):
@@ -22,18 +18,3 @@ def frames_to_planar_normalized(frames, h_out, w_out, mean, std):
     """uint8 [T,H,W,3] -> the normalised planar frames, resized (align_corners=True)."""
     return refops.resize_bilinear(normalize_frames(frames, mean, std).contiguous(), h_out, w_out, None, False)
 
-
-ALL = ["frames_to_planar_normalized"]
-
-_registered = []
-
-
-def register_cpu_kernels():
-    refops_video.register_cpu_kernels()
-    if _registered:
-        return
-    lib = torch.library.Library("unimatch_sm100", "IMPL", "CPU")
-    g = globals()
-    for name in ALL:
-        lib.impl(name, g[name])
-    _registered.append(lib)

@@ -1,12 +1,11 @@
 """CPU statement of the evaluation op `eval_stats` (test infrastructure, like tests/refops.py): the per-pixel fp32 torch / numpy
 expressions of the reference's validate_* loops (evaluate_flow.py, evaluate_stereo.py, loss/stereo_metric.py,
 loss/depth_loss.py:compute_errors), every operation correctly rounded, with the per-sample sums accumulated in float64.  The `-m gpu` tests compare the CUDA
-op with it, and `register_cpu_kernels()` installs it -- together with every op of refops.py -- as a CPU kernel inside the
-test process, so the validation drivers' host logic runs on a machine without a GPU."""
+op with it, and `refops.register_cpu_kernels()` installs it as a CPU kernel inside the test process, so the validation
+drivers' host logic runs on a machine without a GPU."""
 import numpy as np
 import torch
 
-import refops
 from unimatch_b200 import ops
 
 
@@ -100,18 +99,3 @@ def eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, e
         rows = _depth_rows(pred, gt, valid, eval_min, eval_max)
     return torch.tensor(rows, dtype=torch.float64).reshape(pred.shape[0], len(ops.EVAL_COLS[task]))
 
-
-ALL = ["eval_stats"]
-
-_registered = []
-
-
-def register_cpu_kernels():
-    refops.register_cpu_kernels()
-    if _registered:
-        return
-    lib = torch.library.Library("unimatch_sm100", "IMPL", "CPU")
-    g = globals()
-    for name in ALL:
-        lib.impl(name, g[name])
-    _registered.append(lib)

@@ -1,12 +1,11 @@
 """Statement of the ragged flow ops (test infrastructure, like tests/refops_ragged.py): every item of a ragged op is what
 the uniform op gives on that image alone, so each function below calls the uniform op once per item, on the inputs'
-device -- the CUDA op on a GPU, the CPU statements of refops_video / refops.py otherwise.  `register_cpu_kernels()`
+device -- the CUDA op on a GPU, the CPU statements of refops_video / refops.py otherwise.  `refops.register_cpu_kernels()`
 installs the three new ops as CPU kernels inside the test process; `resize_bilinear_ragged` here states the op with
-RAGGED_TRANSPOSE and is called directly (tests/refops_ragged.py registers the op's statement without the flag).
+RAGGED_TRANSPOSE and is called directly (the op's registered statement is tests/refops_ragged.py's, without the flag).
 `composed_flow_reference` states what `MixedSizeFlowRunner` computes, from existing functions only."""
 import torch
 
-import refops_video
 from refops_ragged import _fits, items_of
 from unimatch_b200 import ops
 
@@ -109,18 +108,3 @@ def composed_flow_reference(model, call, pairs, batch, max_buckets, padding_fact
                     res[index] = r
     return res
 
-
-ALL = ["frames_to_planar_ragged", "flow_to_image_ragged", "fb_consistency_ragged"]
-
-_registered = []
-
-
-def register_cpu_kernels():
-    refops_video.register_cpu_kernels()
-    if _registered:
-        return
-    lib = torch.library.Library("unimatch_sm100", "IMPL", "CPU")
-    g = globals()
-    for name in ALL:
-        lib.impl(name, g[name])
-    _registered.append(lib)

@@ -1,12 +1,12 @@
 """Statement of the ragged stereo ops (test infrastructure, like tests/refops_stereo.py): every item of a ragged op is what
 the uniform op gives on that image alone, so each function below calls the uniform op once per item, on the inputs'
 device -- the CUDA op on a GPU, the CPU statements of refops_depth / refops_stereo / refops.py otherwise.
-`register_cpu_kernels()` installs these as the CPU kernels of the ragged ops inside the test process.
+`refops.register_cpu_kernels()` installs these as the CPU kernels of the ragged ops inside the test process.
 `composed_stereo_reference` states what `MixedSizeStereoRunner` computes, from existing functions only."""
+import numpy as np
 import torch
 
 import refops_depth
-import refops_stereo
 from unimatch_b200 import ops
 from unimatch_b200.inference import RAGGED_ITEM
 
@@ -16,6 +16,13 @@ _OPS = torch.ops.unimatch_sm100
 def items_of(table):
     """uint8 [n, 24] descriptor table (any device) -> numpy records (offset, h, w, scale, flags)"""
     return table.cpu().contiguous().numpy().view(RAGGED_ITEM).reshape(-1)
+
+
+def table(recs, device=None):
+    """records (offset, h, w, scale, flags) -> uint8 [n, 24] descriptor table on `device`, a tensor that owns its memory: the
+    inverse of items_of"""
+    t = np.array(list(recs), RAGGED_ITEM).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES)
+    return torch.from_numpy(t.copy()).to(device)
 
 
 def _fits(it, h_max, w_max, per_pixel, numel):
@@ -97,18 +104,3 @@ def composed_stereo_reference(model, call, pairs, batch, max_buckets, padding_fa
                     res[index] = r
     return res
 
-
-ALL = ["frames_to_planar_normalized_ragged", "resize_bilinear_ragged", "disparity_to_image_ragged"]
-
-_registered = []
-
-
-def register_cpu_kernels():
-    refops_stereo.register_cpu_kernels()
-    if _registered:
-        return
-    lib = torch.library.Library("unimatch_sm100", "IMPL", "CPU")
-    g = globals()
-    for name in ALL:
-        lib.impl(name, g[name])
-    _registered.append(lib)

@@ -30,7 +30,7 @@ from bench import BENCH_WORKLOADS
 from oracle import unimatch_oracle as O
 from unimatch_b200 import UniMatch
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict
+from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict, workload_call
 
 FEAT_TOL = 3e-5          # encoder, warp: one pass of fp32-faithful arithmetic
 TRANSFORMER_TOL = 1e-4   # six blocks (24 GEMMs, 12 attention calls, 18 LayerNorms) in sequence
@@ -96,7 +96,7 @@ def run(dev, workload="gmflow-scale2-regrefine6", H=480, W=832, bidir=False, wei
     still sees the stages checked before it."""
     cfg = WORKLOADS[workload]
     task = cfg["model"]["task"]
-    call = dict(cfg["call"])
+    call = workload_call(workload)
     if bidir:
         assert task in ("flow", "depth"), "the stereo task has no bidirectional mode here"
         call["pred_bidir_flow" if task == "flow" else "pred_bidir_depth"] = True

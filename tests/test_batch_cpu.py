@@ -184,14 +184,12 @@ def run_batch_census(monkeypatch, dev, defect=None, B=3, size=CENSUS_SIZE):
     """One forward of every workload at batch B and `size` per task; returns the recorded stream patterns that are not rows of
     BATCH_TABLE (must be empty)."""
     import unimatch_b200.unimatch as um
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+    from unimatch_b200.synthetic import synthetic_model
     census = StreamCensus(um._OPS, B)
     monkeypatch.setattr(um, "_OPS", census if defect is None else OpsDefect(census, defect))
     for wl, cfg in WORKLOADS.items():
         task = cfg["model"]["task"]
-        m = UniMatch(**cfg["model"]).eval()
-        m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-        m = m.to(dev)
+        m = synthetic_model(wl, dev)
         inp = census_inputs(task, B, *size[task], dev)
         m(inp["img0"], inp["img1"], intrinsics=inp.get("intrinsics"), pose=inp.get("pose"), **cfg["call"])
     for p in sorted(census.patterns, key=str):

@@ -34,6 +34,8 @@ from test_batch_cpu import (ATTN, BATCH_TABLE, EXP, PLANES, VC, VT, OpsDefect, c
                             run_batch_census)
 from test_ref64_cpu import STEM_SCALE, STEM_SHIFT, stem_images
 from unimatch_b200 import UniMatch, ops
+from unimatch_b200.spec import WORKLOADS
+from unimatch_b200.synthetic import synthetic_model, workload_call
 
 pytestmark = pytest.mark.gpu
 OPS = torch.ops.unimatch_sm100
@@ -548,17 +550,8 @@ def test_batch_census_rejects_stereo_2b(monkeypatch):
 
 
 # ---- 2. every pair of every bench batch --------------------------------------------------------------------------------
-def _bench_model(wl):
-    from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
-    cfg = WORKLOADS[wl]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    return m.to(DEV), cfg
-
-
-def _fwd(m, cfg, d):
-    return m(d["img0"], d["img1"], intrinsics=d.get("intrinsics"), pose=d.get("pose"), **cfg["call"])["flow_preds"][-1]
+def _fwd(m, wl, d):
+    return m(d["img0"], d["img1"], intrinsics=d.get("intrinsics"), pose=d.get("pose"), **workload_call(wl))["flow_preds"][-1]
 
 
 def pair_tolerance(task):
@@ -571,15 +564,15 @@ def pair_tolerance(task):
 def test_every_pair_of_bench_batch(config):
     from unimatch_b200.synthetic import synthetic_batch
     wl, H, W, ppg = BENCH_WORKLOADS[config][:4]
-    m, cfg = _bench_model(wl)
-    task = cfg["model"]["task"]
+    m = synthetic_model(wl, DEV)
+    task = WORKLOADS[wl]["model"]["task"]
     tol_mean, tol_max = pair_tolerance(task)
     d = {k: v.to(DEV) for k, v in synthetic_batch(task, ppg, H, W).items()}
-    out = _fwd(m, cfg, d)
-    assert torch.equal(out, _fwd(m, cfg, d)), "%s: the same batched forward run twice differs" % config
+    out = _fwd(m, wl, d)
+    assert torch.equal(out, _fwd(m, wl, d)), "%s: the same batched forward run twice differs" % config
     worst = (0.0, 0.0, -1)
     for b in range(ppg):
-        one = _fwd(m, cfg, {k: v.to(DEV) for k, v in synthetic_batch(task, 1, H, W, first_index=b).items()})
+        one = _fwd(m, wl, {k: v.to(DEV) for k, v in synthetic_batch(task, 1, H, W, first_index=b).items()})
         mean, mx = cases.epe(out[b:b + 1].cpu(), one.cpu())
         worst = max(worst, (mean, mx, b))
         assert mean <= tol_mean and mx <= tol_max, "%s pair %d: batched vs alone mean %.3e max %.3e (tol %.0e / %.0e)" % (
@@ -648,8 +641,7 @@ def _pairs(n, H, W, seed):
 def graph_scenario(drop_refs=False, monkeypatch=None):
     from unimatch_b200.inference import BatchedFlowRunner
     from unimatch_b200.synthetic import synthetic_batch
-    m, cfg = _bench_model("gmflow-scale2")
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    m, call = synthetic_model("gmflow-scale2", DEV), workload_call("gmflow-scale2", drop=("task",))
     if drop_refs:
         monkeypatch.setattr(UniMatch, "cached_buffers", lambda self: [])
     bsz, H, W = FLOW_SHAPES[0]
@@ -663,7 +655,7 @@ def graph_scenario(drop_refs=False, monkeypatch=None):
     eager = []
     for n, h, w in FLOW_SHAPES[1:4]:
         d = {k: v.to(DEV) for k, v in synthetic_batch("flow", n, h, w).items()}
-        eager.append((d, _fwd(m, cfg, d).clone()))
+        eager.append((d, _fwd(m, "gmflow-scale2", d).clone()))
     assert not (captured_keys & set(m._attn_ws)), "the runner's planes were not evicted: the scenario was not reached"
     held = {t.data_ptr() for t in getattr(runner, "_held_buffers", [])}
     lost = sorted(p for p in captured if p not in held)
@@ -673,7 +665,7 @@ def graph_scenario(drop_refs=False, monkeypatch=None):
     for a, b in zip(r1, r2):
         assert torch.equal(a, b)
     d, first = eager[-1]
-    assert torch.equal(_fwd(m, cfg, d), first)
+    assert torch.equal(_fwd(m, "gmflow-scale2", d), first)
 
 
 def test_graph_runner_survives_other_shapes():
@@ -690,8 +682,8 @@ def test_graph_runner_check_rejects_dropped_references(monkeypatch):
 def test_depth_runner_survives_other_shapes():
     from unimatch_b200.inference import DepthSequenceRunner
     from unimatch_b200.synthetic import synthetic_batch, synthetic_posed_sequence
-    m, cfg = _bench_model("gmdepth-scale1-regrefine1")
-    kw = {k: v for k, v in cfg["call"].items() if k not in ("min_depth", "max_depth", "num_depth_candidates", "task")}
+    m = synthetic_model("gmdepth-scale1-regrefine1", DEV)
+    kw = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = synthetic_posed_sequence(5, 384, 512, seed=3)
     runner = DepthSequenceRunner(m, (384, 512), 2, DEV, K, use_graph=True, **kw)
     items = list(zip(frames.numpy(), poses.numpy()))
@@ -701,7 +693,7 @@ def test_depth_runner_survives_other_shapes():
     assert captured_keys
     for n, h, w in [(1, 384, 512), (3, 384, 512), (2, 320, 448), (1, 256, 384)]:
         d = {k: v.to(DEV) for k, v in synthetic_batch("depth", n, h, w).items()}
-        _fwd(m, cfg, d)
+        _fwd(m, "gmdepth-scale1-regrefine1", d)
     assert not (captured_keys & set(m._attn_ws)), "the runner's planes were not evicted: the scenario was not reached"
     held = {t.data_ptr() for t in getattr(runner, "_held_buffers", [])}
     assert captured <= held, "cached buffers the runner's graphs write are no longer referenced"
@@ -714,8 +706,8 @@ def test_shape_cycling_matches_fresh_model():
     """A model cycling through five (batch, size) combinations, its plane caches evicted on the way, gives at each of them
     the result of a fresh model bit for bit."""
     from unimatch_b200.synthetic import synthetic_batch
-    m, cfg = _bench_model("gmflow-scale2")
+    m = synthetic_model("gmflow-scale2", DEV)
     for n, h, w in FLOW_SHAPES + FLOW_SHAPES[:2]:
         d = {k: v.to(DEV) for k, v in synthetic_batch("flow", n, h, w).items()}
-        fresh, _ = _bench_model("gmflow-scale2")
-        assert torch.equal(_fwd(m, cfg, d), _fwd(fresh, cfg, d)), (n, h, w)
+        fresh = synthetic_model("gmflow-scale2", DEV)
+        assert torch.equal(_fwd(m, "gmflow-scale2", d), _fwd(fresh, "gmflow-scale2", d)), (n, h, w)

@@ -14,29 +14,17 @@ import torch
 from PIL import Image
 
 import refops_depth
+import refops_ragged
 from oracle import depth_viz as V
-from unimatch_b200 import MixedSizeDepthRunner, UniMatch, VideoFlowRunner
+from unimatch_b200 import MixedSizeDepthRunner, VideoFlowRunner
 from unimatch_b200 import inference_io as IO
 from unimatch_b200.evaluation import validate_depth
-from unimatch_b200.inference import RAGGED_ITEM, _relative_poses, _resize, depth_to_image, infer_depth
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_posed_sequence,
-                                     synthetic_state_dict, synthetic_video)
+from unimatch_b200.inference import _relative_poses, _resize, depth_to_image, infer_depth
+from unimatch_b200.synthetic import (IMAGENET_MEAN, IMAGENET_STD, synthetic_model, synthetic_posed_sequence, synthetic_video,
+                                     workload_call)
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
-
-
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k not in ("task", "min_depth", "max_depth", "num_depth_candidates")}
-    return m.cuda(), call
-
-
-def _table(recs):
-    return torch.from_numpy(np.array(recs, RAGGED_ITEM).view(np.uint8).reshape(-1, RAGGED_ITEM.itemsize).copy()).cuda()
 
 
 def _smooth(h, w, seed, lo=0.5, hi=10.0):
@@ -77,7 +65,7 @@ def test_depth_to_image_ragged_equals_uniform_and_oracle():
     skipped = [(0, 481, 4, 1.0, 0), (0, 0, 4, 1.0, 0), (flat.numel() - 3, 2, 2, 1.0, 0)]   # too tall, empty, past the end
     out = torch.full((3 * flat.numel(),), 0xAB, dtype=torch.uint8, device="cuda")
     before = out.clone()
-    _OPS.depth_to_image_ragged(flat, _table(recs + skipped), out, 480, 640)
+    _OPS.depth_to_image_ragged(flat, refops_ragged.table(recs + skipped, "cuda"), out, 480, 640)
     written = torch.zeros_like(out, dtype=torch.bool)
     for (o, h, w, _, _), d in zip(recs, depths):
         got = out[3 * o:3 * (o + h * w)].view(h, w, 3)
@@ -91,7 +79,7 @@ def test_depth_to_image_ragged_equals_uniform_and_oracle():
 def test_depth_to_image_ragged_graph_follows_its_table():
     depths = _items()
     flat, recs = _pack(depths)
-    table = _table(recs)
+    table = refops_ragged.table(recs, "cuda")
     out = torch.zeros((3 * flat.numel(),), dtype=torch.uint8, device="cuda")
     _OPS.depth_to_image_ragged(flat, table, out, 480, 640)                  # warm-up outside the capture
     torch.cuda.synchronize()
@@ -100,11 +88,11 @@ def test_depth_to_image_ragged_graph_follows_its_table():
         _OPS.depth_to_image_ragged(flat, table, out, 480, 640)
     # a different table: the items reversed in place, other sizes over the same packed floats
     recs2 = [(o, w, h, 1.0, 0) if h * w > 1 else (o, h, w, 1.0, 0) for (o, h, w, _, _) in reversed(recs)]
-    table.copy_(_table(recs2))
+    table.copy_(refops_ragged.table(recs2, "cuda"))
     out.zero_()
     g.replay()
     ref = torch.zeros_like(out)
-    _OPS.depth_to_image_ragged(flat, _table(recs2), ref, 480, 640)
+    _OPS.depth_to_image_ragged(flat, refops_ragged.table(recs2, "cuda"), ref, 480, 640)
     torch.cuda.synchronize()
     assert torch.equal(out, ref)
 
@@ -141,7 +129,8 @@ CASES = {"plain": dict(), "bidir": dict(pred_bidir_depth=True), "size": dict(inf
 def test_mixed_size_depth_runner(case):
     flags = CASES[case]
     bidir = flags.get("pred_bidir_depth", False)
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m = synthetic_model("gmdepth-scale1-regrefine1")
+    call = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = _frames_and_poses()
     pairs = [(frames[t], frames[t + 1], _relative_poses(poses[t:t + 2], False)[0]) for t in range(len(frames) - 1)]
     runner = MixedSizeDepthRunner(m, (90, 150), 2, "cuda", K, visualize=True, **flags, **call)
@@ -176,7 +165,8 @@ def _scannet_dir(root, frames, poses, K):
 
 @pytest.mark.parametrize("bidir", [False, True])
 def test_inference_depth_mixed_directory(tmp_path, bidir):
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m = synthetic_model("gmdepth-scale1-regrefine1")
+    call = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = _frames_and_poses(DIR_FRAMES)
     root = str(tmp_path / "scene")
     _scannet_dir(root, frames, poses, K)
@@ -241,7 +231,8 @@ def _read_video(path):
 
 @pytest.mark.parametrize("concat", [False, True])
 def test_inference_flow_save_video(tmp_path, concat):
-    m, call = _model("gmflow-scale1")
+    m = synthetic_model("gmflow-scale1")
+    call = workload_call("gmflow-scale1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     path, decoded = _mp4(tmp_path, synthetic_video(7, 96, 160, seed=23).numpy(), 10.0)
     flags = dict(pred_bidir_flow=True, save_flo_flow=True, padding_factor=16, batch=3)
     out, plain = str(tmp_path / "out"), str(tmp_path / "plain")
@@ -284,7 +275,8 @@ def _depth_samples():
 @pytest.mark.parametrize("protocol,size", [("scannet", None), ("demon", (64, 96))])
 def test_validate_depth_save_vis(tmp_path, monkeypatch, protocol, size):
     import unimatch_b200.evaluation as E
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m = synthetic_model("gmdepth-scale1-regrefine1")
+    call = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     samples = _depth_samples()
     plain = validate_depth(m, samples, protocol=protocol, batch=2, inference_size=size, **call)
     painted = []

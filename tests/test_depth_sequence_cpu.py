@@ -6,12 +6,10 @@ import numpy as np
 import pytest
 import torch
 
+import refops
 import refops_depth
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import DepthSequenceRunner, _relative_poses, infer_depth, infer_depth_sequence
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_posed_sequence,
-                                     synthetic_state_dict)
+from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_model, synthetic_posed_sequence, workload_call
 
 _WL = "gmdepth-scale1-regrefine1"
 
@@ -74,16 +72,8 @@ def test_runner_staging_uploads_reference_relative_poses(bidir):
     assert np.array_equal(r.prev_pose, poses[6])
 
 
-def _model():
-    cfg = WORKLOADS[_WL]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    kw = {k: v for k, v in cfg["call"].items() if k not in ("min_depth", "max_depth", "num_depth_candidates", "task")}
-    return m, kw
-
-
 def test_infer_depth_sequence_argument_errors():
-    m, kw = _model()
+    m, kw = synthetic_model(_WL, "cpu"), workload_call(_WL, drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = synthetic_posed_sequence(3, 32, 48)
     bad = [
         dict(frames=frames[:1], poses=poses[:1]),                                  # T < 2
@@ -115,8 +105,8 @@ def test_infer_depth_sequence_argument_errors():
 
 @pytest.mark.parametrize("size,bidir", [(None, True), ((48, 80), False)])
 def test_infer_depth_sequence_host_logic_cpu(size, bidir):
-    refops_depth.register_cpu_kernels()
-    m, kw = _model()
+    refops.register_cpu_kernels()
+    m, kw = synthetic_model(_WL, "cpu"), workload_call(_WL, drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = synthetic_posed_sequence(3, 40, 60, seed=7)
     got = infer_depth_sequence(m, frames, K, poses, padding_factor=16, inference_size=size, pred_bidir_depth=bidir, **kw)
     norm = refops_depth.normalize_frames(frames, IMAGENET_MEAN, IMAGENET_STD)

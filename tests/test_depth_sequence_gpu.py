@@ -12,11 +12,9 @@ import pytest
 import torch
 
 import refops_depth
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import DepthSequenceRunner, infer_depth, infer_depth_sequence
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_posed_sequence,
-                                     synthetic_state_dict)
+from unimatch_b200.synthetic import (IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_model, synthetic_posed_sequence,
+                                     workload_call)
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
@@ -34,17 +32,10 @@ def test_frames_to_planar_normalized_equals_resize(hw, size):
         assert torch.equal(got.cpu(), norm)
 
 
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    return m.cuda(), cfg["call"]
-
-
 @pytest.mark.parametrize("workload", ["gmdepth-scale1", "gmdepth-scale1-regrefine1"])
 @pytest.mark.parametrize("bidir", [False, True])
 def test_forward_encoded_depth_equals_forward(workload, bidir):
-    m, call = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload)
     d = {k: v.cuda() for k, v in synthetic_batch("depth", 2, 64, 96).items()}
     ref = m(d["img0"], d["img1"], intrinsics=d["intrinsics"], pose=d["pose"], pred_bidir_depth=bidir, **call)["flow_preds"]
     B = d["img0"].shape[0]
@@ -74,7 +65,7 @@ def _pairwise(m, kw, frames, K, poses, bidir, size=None):
 
 @pytest.mark.parametrize("size,bidir", [(None, False), (None, True), ((112, 176), False), ((112, 176), True)])
 def test_infer_depth_sequence_equals_pairwise(size, bidir):
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m, call = synthetic_model("gmdepth-scale1-regrefine1"), workload_call("gmdepth-scale1-regrefine1")
     kw = {k: v for k, v in call.items() if k not in _DEPTH_RANGE + ("task",)}
     frames, K, poses = synthetic_posed_sequence(7, 128, 192, seed=11)
     got = infer_depth_sequence(m, frames.cuda(), K, poses, padding_factor=16, inference_size=size, pred_bidir_depth=bidir, **kw)
@@ -88,7 +79,7 @@ def test_infer_depth_sequence_equals_pairwise(size, bidir):
 def test_depth_sequence_runner_eager_and_graph():
     """11 frames of 90x150 (inference size 96x160), batch 4: frame 0 primes the carried pyramid and pose, then three steps of
     4 / 4 / 2 (+2 repeats) new frames.  Graph replay and eager runs agree bit for bit."""
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m, call = synthetic_model("gmdepth-scale1-regrefine1"), workload_call("gmdepth-scale1-regrefine1")
     kw = {k: v for k, v in call.items() if k not in _DEPTH_RANGE + ("task",)}
     frames, K, poses = synthetic_posed_sequence(11, 90, 150, seed=21)
     ref = infer_depth_sequence(m, frames.cuda(), K, poses, pred_bidir_depth=True, **kw)

@@ -8,10 +8,8 @@ import pytest
 import torch
 
 from oracle import depth_viz as V
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import DepthSequenceRunner, depth_to_image
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_posed_sequence, synthetic_state_dict
+from unimatch_b200.synthetic import synthetic_model, synthetic_posed_sequence, workload_call
 
 pytestmark = pytest.mark.gpu
 
@@ -174,11 +172,8 @@ def test_depth_to_image_graph_replay():
 def test_depth_sequence_runner_pictures():
     """11 frames of 90x150, batch 4 (steps of 4 / 4 / 2 + 2 repeats), pred_bidir_depth: the pictures are the oracle's on the
     runner's own depths, graph replay equals eager bit for bit, and return_depth=False sends back the same pictures alone"""
-    cfg = WORKLOADS["gmdepth-scale1-regrefine1"]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    m = m.cuda()
-    kw = {k: v for k, v in cfg["call"].items() if k not in ("min_depth", "max_depth", "num_depth_candidates", "task")}
+    m = synthetic_model("gmdepth-scale1-regrefine1")
+    kw = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = synthetic_posed_sequence(11, 90, 150, seed=21)
     items = list(zip(frames.numpy(), poses.numpy()))
     runs = {}

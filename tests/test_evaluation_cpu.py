@@ -10,7 +10,7 @@ import torch
 
 import eval_samples as E
 import refloop_eval
-import refops_eval
+import refops
 from unimatch_b200 import evaluation, ops
 
 GOLDEN = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "golden_eval.pt"), weights_only=False)
@@ -34,7 +34,7 @@ def run_case(case, samples, **kw):
 
 @pytest.fixture(scope="module", autouse=True)
 def _cpu_kernels():
-    refops_eval.register_cpu_kernels()
+    refops.register_cpu_kernels()
 
 
 @pytest.mark.parametrize("case", GOLDEN, ids=[c["name"] for c in GOLDEN])

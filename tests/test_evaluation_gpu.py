@@ -10,9 +10,8 @@ import eval_samples as E
 import refloop_eval
 import refops_eval
 from test_evaluation_cpu import GOLDEN, check_results, run_case
-from unimatch_b200 import UniMatch, evaluation, ops
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+from unimatch_b200 import evaluation, ops
+from unimatch_b200.synthetic import synthetic_model, workload_call
 
 pytestmark = pytest.mark.gpu
 OPS = torch.ops.unimatch_sm100
@@ -122,18 +121,10 @@ def test_golden_protocols_on_device(case):
 
 
 # ------------------------------------------------------------------------------------------------ end to end, real module
-def _model(name):
-    cfg = WORKLOADS[name]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    kw = {k: v for k, v in cfg["call"].items() if k not in ("min_depth", "max_depth")}
-    return m.cuda(), kw
-
-
 def _e2e(task, workload, samples, opts):
     """The driver at batch 3 (short batches, two shapes) against the reference loop restated at batch 1 around the same module
     (tests/refloop_eval.py).  Batch composition changes `um_conv2d_tc`'s summation order, hence the tolerances."""
-    model, kw = _model(workload)
+    model, kw = synthetic_model(workload), workload_call(workload, drop=("min_depth", "max_depth"))
     want = refloop_eval.LOOPS[task](model, samples, **opts, **kw)
     driver = {"flow": evaluation.validate_flow, "stereo": evaluation.validate_stereo, "depth": evaluation.validate_depth}[task]
     got = driver(model, samples, batch=3, device="cuda", **opts, **kw)
@@ -164,8 +155,10 @@ def test_validate_depth_end_to_end(inference_size):
 
 
 def test_flow_and_stereo_drivers_do_not_synchronise():
-    flow_model, flow_kw = _model("gmflow-scale2-regrefine6")
-    stereo_model, stereo_kw = _model("gmstereo-scale2")
+    flow_model = synthetic_model("gmflow-scale2-regrefine6")
+    flow_kw = workload_call("gmflow-scale2-regrefine6", drop=("min_depth", "max_depth"))
+    stereo_model = synthetic_model("gmstereo-scale2")
+    stereo_kw = workload_call("gmstereo-scale2", drop=("min_depth", "max_depth"))
     flow = E.flow_samples(55, [(96, 128), (80, 112)], 5, sparse=True)
     stereo = E.stereo_samples(56, [(96, 128)], 4)
     runs = [lambda: evaluation.validate_flow(flow_model, flow, protocol="kitti", padding_factor=32, batch=3, **flow_kw),

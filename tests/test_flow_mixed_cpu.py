@@ -8,7 +8,9 @@ import numpy as np
 import pytest
 import torch
 
+import refops
 import refops_flow_ragged
+import refops_ragged
 from oracle import flow_viz as OV
 from unimatch_b200 import MixedSizeDepthRunner, MixedSizeFlowRunner, MixedSizeStereoRunner, UniMatch, ops
 from unimatch_b200.inference import RAGGED_ITEM, _MixedSizeRunner, _flow_step_layout
@@ -144,32 +146,29 @@ def test_runner_frame_errors():
         list(r._chunks(enumerate([(ok, ok), (ok, np.zeros((2, 2, 3), np.uint8))])))
 
 
-def _table(*recs):
-    return torch.from_numpy(np.array(list(recs), RAGGED_ITEM).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES))
-
-
 def test_ragged_flow_statements_equal_the_uniform_ops_cpu():
     """the CPU statements place every item where its descriptors say, as the uniform op computes it"""
-    refops_flow_ragged.register_cpu_kernels()
+    refops.register_cpu_kernels()
     g = torch.Generator().manual_seed(5)
     frames = torch.randint(0, 256, (3 * (4 * 5 + 9 * 6),), generator=g, dtype=torch.uint8)
-    fitems = _table((0, 4, 5, 1.0, 0), (60, 9, 6, 1.0, T))
+    fitems = refops_ragged.table([(0, 4, 5, 1.0, 0), (60, 9, 6, 1.0, T)])
     planes = _OPS.frames_to_planar_ragged(frames, fitems, 10, 10, 6, 9)
     assert torch.equal(planes[0], _OPS.frames_to_planar(frames[:60].view(1, 4, 5, 3), 6, 9, False)[0])
     assert torch.equal(planes[1], frames[60:].view(9, 6, 3).permute(2, 1, 0).float())        # exactly its transpose
     x = torch.randn((4, 1, 6, 9), generator=g)
-    items = _table((0, 4, 5, 1.25, 0), (20, 4, 5, 0.5, 0), (40, 9, 6, 1.0, T), (94, 9, 6, 1.0, T))
+    items = refops_ragged.table([(0, 4, 5, 1.25, 0), (20, 4, 5, 0.5, 0), (40, 9, 6, 1.0, T), (94, 9, 6, 1.0, T)])
     flow = refops_flow_ragged.resize_bilinear_ragged(x, items, 10, 10, 148)
     assert torch.equal(flow[:40].view(2, 4, 5), _OPS.resize_bilinear(x[:2].view(1, 2, 6, 9), 4, 5, [1.25, 0.5], False)[0])
     assert torch.equal(flow[40:].view(2, 9, 6), x[2:, 0].transpose(-2, -1))
-    fl, pic = _table((0, 4, 5, 1.0, 0), (40, 9, 6, 1.0, 0)), _table((0, 4, 5, 1.0, 0), (60, 9, 6, 1.0, 0))
+    fl = refops_ragged.table([(0, 4, 5, 1.0, 0), (40, 9, 6, 1.0, 0)])
+    pic = refops_ragged.table([(0, 4, 5, 1.0, 0), (60, 9, 6, 1.0, 0)])
     pics = torch.zeros((222,), dtype=torch.uint8)
     _OPS.flow_to_image_ragged(flow, fl, pics, pic, 10, 10)
     assert np.array_equal(pics[60:].view(9, 6, 3).numpy(), OV.flow_to_image_batch(flow[40:].view(1, 2, 9, 6).numpy())[0])
     both = torch.cat((flow[40:], -flow[40:]))
     occ = torch.full((2 * 54 + 3,), 7.0)
-    _OPS.fb_consistency_ragged(both, _table((0, 9, 6, 1.0, 0), (108, 9, 6, 1.0, 0)), occ,
-                               _table((0, 9, 6, 1.0, 0), (57, 9, 6, 1.0, 0)), 10, 10, 0.01, 0.5)
+    _OPS.fb_consistency_ragged(both, refops_ragged.table([(0, 9, 6, 1.0, 0), (108, 9, 6, 1.0, 0)]), occ,
+                               refops_ragged.table([(0, 9, 6, 1.0, 0), (57, 9, 6, 1.0, 0)]), 10, 10, 0.01, 0.5)
     ref = _OPS.fb_consistency(both[:108].view(1, 2, 9, 6), both[108:].view(1, 2, 9, 6), 0.01, 0.5)
     assert torch.equal(occ[:54].view(9, 6), ref[0][0]) and torch.equal(occ[57:111].view(9, 6), ref[1][0])
     assert (occ[54:57] == 7).all()

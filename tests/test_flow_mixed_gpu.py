@@ -8,20 +8,15 @@ import pytest
 import torch
 
 import refops_flow_ragged
-from unimatch_b200 import MixedSizeFlowRunner, UniMatch, infer_flow, ops
-from unimatch_b200.inference import RAGGED_ITEM, flow_to_image
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict, synthetic_video
+import refops_ragged
+from unimatch_b200 import MixedSizeFlowRunner, infer_flow, ops
+from unimatch_b200.inference import flow_to_image
+from unimatch_b200.synthetic import synthetic_batch, synthetic_model, synthetic_video, workload_call
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
 T = ops.RAGGED_TRANSPOSE
 KITTI = [(375, 1242), (370, 1226), (374, 1238), (376, 1241)]
-
-
-def _table(recs):
-    t = torch.from_numpy(np.array(list(recs), RAGGED_ITEM).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES))
-    return t.cuda()
 
 
 def _offsets(sizes, per_pixel, gap=0):
@@ -48,7 +43,7 @@ def test_frames_to_planar_ragged_equals_per_frame():
     packed = torch.cat([f.reshape(-1) for f in frames]).cuda()
     recs = [(o, h, w, 1.0, f) for o, (h, w), f in zip(offsets, sizes, flags)]
     recs += [(0, 1300, 10, 1.0, 0), (0, 0, 0, 1.0, 0), (total - 5, 2, 2, 1.0, 0)]     # too tall, empty, beyond the buffer
-    items = _table(recs)
+    items = refops_ragged.table(recs, "cuda")
     out = _OPS.frames_to_planar_ragged(packed, items, 1248, 1248, ho, wo)
     for i, (f, fl) in enumerate(zip(frames, flags)):
         one = _OPS.frames_to_planar(f[None].cuda().contiguous(), ho, wo, bool(fl))
@@ -94,13 +89,14 @@ def test_resize_bilinear_ragged_transposed_flow_equals_per_image():
     recs += [(0, 500, 10, 1.0, 0), (0, 0, 0, 1.0, 0)]                       # out of range and empty: skipped
     x = torch.cat((flow.view(-1, 1, *size), flow[:1].view(2, 1, *size)))
     out = torch.full((total,), -7.0, device="cuda")
-    _lib("um_resize_bilinear_ragged", x, out, total, _table(recs), len(recs), size[0], size[1], 400, 400)
+    _lib("um_resize_bilinear_ragged", x, out, total, refops_ragged.table(recs, "cuda"), len(recs), size[0], size[1], 400,
+         400)
     for i, (h, w) in enumerate(sizes):
         got, ref = out[offs[i]:offs[i] + 2 * h * w].view(2, h, w), _resize_back(flow[i:i + 1], h, w, size)
         assert torch.equal(got.isnan(), ref.isnan()) and torch.equal(got.nan_to_num(), ref.nan_to_num()), i
         assert (out[offs[i] + 2 * h * w:offs[i] + 2 * h * w + 3] == -7).all(), i        # the gaps between items are intact
     assert torch.equal(out[offs[3]:offs[3] + 2 * 96 * 312].view(2, 96, 312)[0], flow[3, 0])          # copied, inf included
-    ref = refops_flow_ragged.resize_bilinear_ragged(x, _table(recs), 400, 400, total)
+    ref = refops_flow_ragged.resize_bilinear_ragged(x, refops_ragged.table(recs, "cuda"), 400, 400, total)
     keep = out != -7
     assert torch.equal(out[keep].nan_to_num(), ref[keep].nan_to_num())
 
@@ -112,7 +108,7 @@ def test_captured_resize_follows_the_table():
     x = flow.view(4, 1, *size)
     first, _, _ = _flow_items([(50, 90), (96, 64)], size)
     second, offs, _ = _flow_items([(90, 50), (33, 77)], size)
-    items = _table(first)
+    items = refops_ragged.table(first, "cuda")
     side = torch.cuda.Stream()
     side.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(side):
@@ -123,7 +119,7 @@ def test_captured_resize_follows_the_table():
         out = _OPS.resize_bilinear_ragged(x, items, 128, 128, 4 * 128 * 128)
     graph.replay()
     assert torch.equal(out[:2 * 50 * 90].view(2, 50, 90), _resize_back(flow[:1], 50, 90, size))
-    items.copy_(_table(second))
+    items.copy_(refops_ragged.table(second, "cuda"))
     graph.replay()
     for i, (h, w) in enumerate([(90, 50), (33, 77)]):
         assert torch.equal(out[offs[i]:offs[i] + 2 * h * w].view(2, h, w), _resize_back(flow[i:i + 1], h, w, size)), i
@@ -149,7 +145,8 @@ def test_flow_to_image_ragged_equals_per_image():
     precs = [(o, h, w, 1.0, 0) for o, (h, w) in zip(poffs, sizes)] + [(0, 2000, 4, 1.0, 0), (0, 0, 0, 1.0, 0), (0, 9, 8, 1.0, 0)]
     pics = torch.full((ptotal,), 99, dtype=torch.uint8, device="cuda")
     for _ in range(2):
-        _OPS.flow_to_image_ragged(packed, _table(frecs), pics, _table(precs), 400, 1300)
+        _OPS.flow_to_image_ragged(packed, refops_ragged.table(frecs, "cuda"), pics, refops_ragged.table(precs, "cuda"), 400,
+                                  1300)
     for i, ((h, w), f) in enumerate(zip(sizes, flows)):
         if i > 0:                                  # item 0's slot is where the mismatched item points: still picture 0
             assert (pics[poffs[i] - 5:poffs[i]] == 99).all(), i
@@ -157,7 +154,8 @@ def test_flow_to_image_ragged_equals_per_image():
         assert torch.equal(pic, flow_to_image(f[None].cuda())[0]), i
     assert (pics[poffs[6]:poffs[6] + 3 * 17 * 19] == 255).all() and (pics[poffs[8]:poffs[8] + 243] == 0).all()
     ref = torch.full_like(pics, 99)
-    refops_flow_ragged.flow_to_image_ragged(packed, _table(frecs), ref, _table(precs), 400, 1300)
+    refops_flow_ragged.flow_to_image_ragged(packed, refops_ragged.table(frecs, "cuda"), ref,
+                                            refops_ragged.table(precs, "cuda"), 400, 1300)
     assert torch.equal(pics, ref)
 
 
@@ -169,8 +167,8 @@ def test_fb_consistency_ragged_equals_per_pair():
     foffs, ftotal = _offsets(sizes + sizes, 2)
     ooffs, ototal = _offsets(sizes + sizes, 1, gap=4)
     packed = torch.cat([f.reshape(-1) for f in fwd + bwd]).cuda()
-    fitems = _table((o, h, w, 1.0, 0) for o, (h, w) in zip(foffs, sizes + sizes))
-    oitems = _table((o, h, w, 1.0, 0) for o, (h, w) in zip(ooffs, sizes + sizes))
+    fitems = refops_ragged.table([(o, h, w, 1.0, 0) for o, (h, w) in zip(foffs, sizes + sizes)], "cuda")
+    oitems = refops_ragged.table([(o, h, w, 1.0, 0) for o, (h, w) in zip(ooffs, sizes + sizes)], "cuda")
     occ = torch.full((ototal,), -7.0, device="cuda")
     _OPS.fb_consistency_ragged(packed, fitems, occ, oitems, 400, 400, 0.01, 0.5)
     n = len(sizes)
@@ -188,14 +186,6 @@ def test_fb_consistency_ragged_equals_per_pair():
 
 
 # ---------------------------------------------------------------------------------------------------------------- the runner
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg
-
-
 # An interleaved mix; with padding 32 it falls into the (128, 256), (128, 224) and (64, 128) buckets: two portrait pairs
 # share the first with landscape ones, and one pair is at (128, 256) itself, so its flow is not resized back
 MIX = [(120, 250), (100, 220), (250, 120), (128, 256), (60, 100), (118, 245), (100, 220), (256, 128), (121, 249), (100, 60)]
@@ -228,7 +218,7 @@ CASES = {                    # sizes, batch, max_buckets, runner arguments
 def test_mixed_flow_runner_equals_composed_reference(workload, case):
     sizes, batch, max_buckets, kw = CASES[case]
     kw = dict(kw)
-    m, call, _ = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload, drop=("task",))
     pairs = _pairs(sizes, seed=40)
     return_flow = kw.get("return_flow", True)
     runner = MixedSizeFlowRunner(m, CAP, batch, "cuda", padding_factor=32, visualize=True, max_buckets=max_buckets, **kw,
@@ -262,7 +252,7 @@ def test_mixed_flow_runner_close_to_infer_flow_on_each_pair(workload):
     """the step's batch changes `um_conv2d_tc`'s summation order (README, video flow: 3e-6 of the largest flow at the bench
     sizes), and six refinement iterations on these small frames carry it a little further, so the pair alone agrees to 1e-5
     of its largest flow"""
-    m, call, _ = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload, drop=("task",))
     pairs = _pairs(MIX, seed=55)
     runner = MixedSizeFlowRunner(m, CAP, 2, "cuda", padding_factor=32, **BIDIR, **call)
     worst = 0.0
@@ -282,7 +272,7 @@ def test_mixed_flow_runner_close_to_infer_flow_on_each_pair(workload):
 def test_mixed_flow_runner_survives_other_shapes():
     """capture three buckets, evict the module's cached planes with forwards at other batch sizes and shapes, check that
     the runner still holds every buffer its graphs write, then replay bit for bit"""
-    m, call, cfg = _model("gmflow-scale2-regrefine6")
+    m, call = synthetic_model("gmflow-scale2-regrefine6"), workload_call("gmflow-scale2-regrefine6", drop=("task",))
     pairs = _pairs(MIX, seed=70)
     runner = MixedSizeFlowRunner(m, CAP, 2, "cuda", padding_factor=32, visualize=True, **call)
     r1 = {i: {k: v.clone() for k, v in r.items()} for i, r in runner.run(pairs)}
@@ -292,7 +282,7 @@ def test_mixed_flow_runner_survives_other_shapes():
     assert captured
     for n, h, w in [(1, 384, 512), (3, 384, 512), (2, 320, 448), (1, 256, 384), (4, 256, 384)]:
         d = {k: v.cuda() for k, v in synthetic_batch("flow", n, h, w).items()}
-        m(d["img0"], d["img1"], **cfg["call"])
+        m(d["img0"], d["img1"], **workload_call("gmflow-scale2-regrefine6"))
     assert captured_keys - (set(m._attn_ws) | set(m._pad_ws)), "the runner's planes were not evicted: the scenario was not reached"
     held = {t.data_ptr() for _, _, bufs in runner.buckets.values() for t in bufs}
     assert captured <= held, "cached buffers the runner's graphs write are no longer referenced"

@@ -8,21 +8,18 @@ import torch
 import cases
 import refops
 from cases import O
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import BatchedFlowRunner, infer_depth, infer_flow, infer_stereo
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict
+from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_model, synthetic_state_dict, workload_call
 
 
 def _setup(workload, b, h, w, dev):
     cfg = WORKLOADS[workload]
     sd = synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"])
     data = synthetic_batch(cfg["model"]["task"], b, h, w)
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(sd)
     mk = {k: cfg["model"][k] for k in ("num_scales", "upsample_factor", "reg_refine")}
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.to(dev), sd, {k: v.to(dev) for k, v in data.items()}, data, mk, call
+    call = workload_call(workload, drop=("task",))
+    return synthetic_model(workload, dev), sd, {k: v.to(dev) for k, v in data.items()}, data, mk, call
 
 
 def _stereo_check(dev, bidir, right, size):

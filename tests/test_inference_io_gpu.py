@@ -12,23 +12,14 @@ from PIL import Image
 from oracle import depth_viz as ODE
 from oracle import disp_viz as ODI
 from oracle import flow_viz as OF
-from unimatch_b200 import (DepthSequenceRunner, MixedSizeFlowRunner, MixedSizeStereoRunner, UniMatch, infer_depth_sequence,
-                           infer_flow, infer_flow_video)
+from unimatch_b200 import (DepthSequenceRunner, MixedSizeFlowRunner, MixedSizeStereoRunner, infer_depth_sequence, infer_flow,
+                           infer_flow_video)
 from unimatch_b200 import inference_io as IO
 from unimatch_b200.inference import _stereo_from_frames, flow_to_image
-from unimatch_b200.spec import WORKLOADS
 from unimatch_b200.submission import flo_header, pfm_header
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_posed_sequence, synthetic_state_dict, synthetic_video
+from unimatch_b200.synthetic import synthetic_model, synthetic_posed_sequence, synthetic_video, workload_call
 
 pytestmark = pytest.mark.gpu
-
-
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k not in ("task", "min_depth", "max_depth", "num_depth_candidates")}
-    return m.cuda(), call
 
 
 def _png(path):
@@ -83,7 +74,8 @@ FLOW_FLAGS = {"plain": dict(), "bidir_check_flo": dict(pred_bidir_flow=True, fwd
 @pytest.mark.parametrize("case", sorted(FLOW_FLAGS))
 def test_inference_flow_directory(tmp_path, case):
     flags = FLOW_FLAGS[case]
-    m, call = _model("gmflow-scale1")
+    m = synthetic_model("gmflow-scale1")
+    call = workload_call("gmflow-scale1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     d = _flow_dir(str(tmp_path))
     out = str(tmp_path / "out")
     stats = IO.inference_flow(m, inference_dir=d, output_path=out, padding_factor=16, batch=2, **flags, **call)
@@ -167,7 +159,8 @@ def _video_frames(tmp_path, frames):
 
 def test_inference_flow_video_bwd(tmp_path):
     """`pred_bwd_flow` on a video: each pair in swapped order, as `infer_flow_video(..., pred_bwd_flow=True)`"""
-    m, call = _model("gmflow-scale1")
+    m = synthetic_model("gmflow-scale1")
+    call = workload_call("gmflow-scale1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames = synthetic_video(8, 96, 160, seed=23).numpy()
     path, decoded = _video_frames(tmp_path, frames)
     out = str(tmp_path / "out")
@@ -211,7 +204,8 @@ STEREO_FLAGS = {"plain": dict(), "bidir_pfm": dict(pred_bidir_disp=True, save_pf
 @pytest.mark.parametrize("case", sorted(STEREO_FLAGS))
 def test_inference_stereo_directories(tmp_path, case):
     flags = STEREO_FLAGS[case]
-    m, call = _model("gmstereo-scale2")
+    m = synthetic_model("gmstereo-scale2")
+    call = workload_call("gmstereo-scale2", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     left_dir, right_dir = str(tmp_path / "left"), str(tmp_path / "right")
     os.makedirs(left_dir), os.makedirs(right_dir)
     for i, (h, w) in enumerate(STEREO_SIZES):
@@ -255,7 +249,8 @@ def test_inference_stereo_directories(tmp_path, case):
 # -------------------------------------------------------------------------------------------------------------------- depth
 @pytest.mark.parametrize("bidir", [False, True])
 def test_inference_depth_scannet(tmp_path, bidir):
-    m, call = _model("gmdepth-scale1-regrefine1")
+    m = synthetic_model("gmdepth-scale1-regrefine1")
+    call = workload_call("gmdepth-scale1-regrefine1", drop=("task", "min_depth", "max_depth", "num_depth_candidates"))
     frames, K, poses = synthetic_posed_sequence(7, 90, 150, seed=31)
     root = str(tmp_path / "scene")
     for sub in ("color", "pose", "intrinsic"):

@@ -474,16 +474,13 @@ def test_launch_census_of_bench_workloads(monkeypatch):
     """One pair of every workload in spec.WORKLOADS at its real resolution; every conv / attention / expectation /
     matching-path dispatch key it launches must be one the case tables here or in tests/test_matching_edges_gpu.py test."""
     import unimatch_b200.unimatch as um
-    from unimatch_b200 import UniMatch
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_batch, synthetic_state_dict
+    from unimatch_b200.synthetic import synthetic_batch, synthetic_model
     census = _Census(um._OPS)
     monkeypatch.setattr(um, "_OPS", census)
     for wl, cfg in WORKLOADS.items():
         H, W = CENSUS_RES[cfg["model"]["task"]]
-        model = UniMatch(**cfg["model"]).eval()
-        model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-        model = model.cuda()
+        model = synthetic_model(wl)
         inp = {k: v.cuda() for k, v in synthetic_batch(cfg["model"]["task"], 1, H, W).items()}
         with torch.no_grad():
             model(inp["img0"], inp["img1"], intrinsics=inp.get("intrinsics"), pose=inp.get("pose"), **cfg["call"])

@@ -70,3 +70,11 @@ def test_module_matches_reference_on_cpu(name):
     mean, mx = cases.epe(got, ref)
     assert mean <= cases.e2e_tolerance(name), (mean, mx)
 
+
+
+def test_cpu_statements_are_named_after_defined_ops():
+    """Every CPU statement of the registry is installed under the name of an op that unimatch_b200/ops.py defines, so a
+    misspelt or removed name fails here rather than only in a test that happens to call that op."""
+    from unimatch_b200 import ops  # noqa: F401  defines the unimatch_sm100 ops
+    unknown = [name for name in refops.cpu_statements() if not hasattr(torch.ops.unimatch_sm100, name)]
+    assert not unknown, unknown

@@ -9,10 +9,11 @@ import torch
 
 import refops_points as RP
 import refops_tracks as RT
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import (PointTrackRunner, VideoFlowRunner, chain_tracks, infer_flow_video, track_points)
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+from unimatch_b200.synthetic import synthetic_model, synthetic_video, workload_call
+
+_WL = "gmflow-scale1"
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
@@ -105,7 +106,8 @@ def test_forward_split_across_launches():
 
 
 def test_track_points_on_infer_flow_video():
-    m, call, pad = _model()
+    m, call = synthetic_model(_WL), workload_call(_WL, drop=("task",))
+    pad = WORKLOADS[_WL]["pad"]
     frames = synthetic_video(7, 64, 96, seed=12)
     ifv = infer_flow_video(m, frames.cuda(), padding_factor=pad, pred_bidir_flow=True, fwd_bwd_consistency_check=True,
                            **call)
@@ -116,14 +118,6 @@ def test_track_points_on_infer_flow_video():
     assert np.array_equal(tracks, emu["tracks"]) and np.array_equal(visible.astype(bool), emu["visible"])
 
 
-def _model(workload="gmflow-scale1"):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg["pad"]
-
-
 @pytest.mark.parametrize("batch,hw,use_graph,stream", [(1, (64, 96), True, False), (3, (64, 96), False, True),
                                                        (3, (80, 48), True, False), (8, (64, 96), True, True),
                                                        (8, (64, 96), False, False)])
@@ -132,7 +126,8 @@ def test_runner(batch, hw, use_graph, stream):
     generator of frames (the tables then grow as the stream goes).  The tracks are `track_points` on the runner's own flows
     bit for bit; the flows are VideoFlowRunner's bit for bit; a second call with other queries is independent of the
     first; return_flow=False returns the same tracks only; a query past the clip's end is refused, naming it"""
-    m, call, pad = _model()
+    m, call = synthetic_model(_WL), workload_call(_WL, drop=("task",))
+    pad = WORKLOADS[_WL]["pad"]
     h, w = hw
     frames = list(synthetic_video(11, h, w, seed=31).numpy())
     clip = (lambda: (f for f in frames)) if stream else (lambda: frames)

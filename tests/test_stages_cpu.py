@@ -11,7 +11,7 @@ import functools
 import pytest
 import torch
 
-import refops_stereo
+import refops
 import stage_checks
 import unimatch_b200.unimatch as um
 from unimatch_b200 import UniMatch
@@ -23,7 +23,7 @@ def small_shape(workload, bidir):
 
 
 def run_small(workload, bidir):
-    refops_stereo.register_cpu_kernels()
+    refops.register_cpu_kernels()
     res = stage_checks.run(torch.device("cpu"), workload, *small_shape(workload, bidir), bidir, report=lambda *_: None)
     assert "e2e" in res and all(v <= 1 for v in res.values())
 
@@ -115,7 +115,7 @@ DEFECTS = {
 @pytest.mark.parametrize("defect", sorted(DEFECTS))
 def test_stage_check_catches_defect_at_its_stage(monkeypatch, defect):
     workload, bidir, stage, before, patch = DEFECTS[defect]
-    refops_stereo.register_cpu_kernels()
+    refops.register_cpu_kernels()
     patch(monkeypatch)
     res = {}
     with pytest.raises(AssertionError) as e:

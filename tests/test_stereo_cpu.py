@@ -11,14 +11,15 @@ import numpy as np
 import pytest
 import torch
 
+import refops
 import refops_depth
-import refops_stereo
 from cases import O
 from oracle import disp_viz as OD
 from unimatch_b200 import UniMatch, ops
 from unimatch_b200.inference import StereoRunner, _stereo_from_frames, disparity_to_image
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_state_dict, synthetic_stereo_frames
+from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_model, synthetic_state_dict,
+                                     synthetic_stereo_frames, workload_call)
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 GOLD = torch.load(os.path.join(HERE, "golden", "golden_disp_vis.pt"))
@@ -57,7 +58,7 @@ def test_disparity_to_image_bad_arguments_are_reported_without_a_gpu():
 
 
 def test_disparity_to_image_shape_errors():
-    refops_stereo.register_cpu_kernels()
+    refops.register_cpu_kernels()
     for bad in (torch.zeros(5), torch.zeros((1, 1, 4, 5)), torch.zeros((2, 0, 5)), torch.zeros((4, 5), dtype=torch.int32)):
         with pytest.raises(ValueError):
             disparity_to_image(bad)
@@ -81,11 +82,8 @@ def test_synthetic_stereo_frames_is_seeded_uint8():
 def _stereo_setup():
     cfg = WORKLOADS["gmstereo-scale2"]
     sd = synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"])
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(sd)
     mk = {k: cfg["model"][k] for k in ("num_scales", "upsample_factor", "reg_refine")}
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m, sd, mk, call
+    return synthetic_model("gmstereo-scale2", "cpu"), sd, mk, workload_call("gmstereo-scale2", drop=("task",))
 
 
 @pytest.mark.parametrize("bidir,right,size", [(False, False, None), (False, False, (96, 160)), (True, False, None),
@@ -93,7 +91,7 @@ def _stereo_setup():
 def test_stereo_from_frames_host_logic_cpu(bidir, right, size):
     """2 pairs of 100x150, resized to 128x160 (padding 32) or to the inference size, against the oracle's infer_stereo on
     the frames normalised on the host as the reference's data pipeline does"""
-    refops_stereo.register_cpu_kernels()
+    refops.register_cpu_kernels()
     m, sd, mk, call = _stereo_setup()
     left, rightv = synthetic_stereo_frames(2, 100, 150, seed=9)
     got = _stereo_from_frames(m, torch.cat((left, rightv), 0), padding_factor=32, inference_size=size, pred_bidir_disp=bidir,

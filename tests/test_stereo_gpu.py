@@ -14,11 +14,9 @@ import torch
 
 import refops_depth
 from oracle import disp_viz as OD
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import StereoRunner, disparity_to_image, infer_stereo
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_state_dict,
-                                     synthetic_stereo_frames)
+from unimatch_b200.synthetic import (IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_model, synthetic_stereo_frames,
+                                     workload_call)
 
 pytestmark = pytest.mark.gpu
 GOLD = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "golden_disp_vis.pt"))
@@ -67,14 +65,6 @@ def test_disparity_to_image_strided_output():
     assert torch.equal(tall[:2, :37].cpu(), GOLD["odd_37x53"]["image"]) and not tall[:, 37:].any() and not tall[2].any()
 
 
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg
-
-
 def _reference(m, call, lefts, rights, batch, **kw):
     """infer_stereo on the runner's steps (short last step filled with its last pair), frames normalised on the host"""
     nl, nr = (refops_depth.normalize_frames(f, IMAGENET_MEAN, IMAGENET_STD) for f in (lefts, rights))
@@ -100,7 +90,7 @@ CASES = {                      # frame size, pairs, batch, runner / infer_stereo
 @pytest.mark.parametrize("case", sorted(CASES))
 def test_stereo_runner_equals_infer_stereo(workload, case):
     (h, w), n, batch, kw = CASES[case]
-    m, call, _ = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload, drop=("task",))
     lefts, rights = synthetic_stereo_frames(n, h, w, seed=13)
     runner = StereoRunner(m, (h, w), batch, "cuda", visualize=True, use_graph=case != "eager", **kw, **call)
     got = [{k: v.clone() for k, v in r.items()} for r in runner.run(zip(lefts.numpy(), rights.numpy()))]
@@ -118,7 +108,7 @@ def test_stereo_runner_equals_infer_stereo(workload, case):
 
 
 def test_stereo_runner_pictures_only():
-    m, call, _ = _model("gmstereo-scale2")
+    m, call = synthetic_model("gmstereo-scale2"), workload_call("gmstereo-scale2", drop=("task",))
     lefts, rights = synthetic_stereo_frames(3, 256, 384, seed=5)
     runner = StereoRunner(m, (256, 384), 2, "cuda", padding_factor=32, pred_bidir_disp=True, visualize=True, return_disp=False,
                           **call)
@@ -136,7 +126,7 @@ def test_stereo_runner_pictures_only():
 def test_stereo_runner_survives_other_shapes():
     """capture, evict the module's cached planes with forwards at other batch sizes and shapes, check that the runner still
     holds every buffer its graphs write, then replay bit for bit"""
-    m, call, cfg = _model("gmstereo-scale2")
+    m, call = synthetic_model("gmstereo-scale2"), workload_call("gmstereo-scale2", drop=("task",))
     lefts, rights = synthetic_stereo_frames(4, 384, 512, seed=3)
     runner = StereoRunner(m, (384, 512), 2, "cuda", **call)
     items = list(zip(lefts.numpy(), rights.numpy()))
@@ -146,7 +136,7 @@ def test_stereo_runner_survives_other_shapes():
     assert captured
     for n, h, w in [(1, 384, 512), (3, 384, 512), (2, 320, 448), (1, 256, 384), (4, 256, 384)]:
         d = {k: v.cuda() for k, v in synthetic_batch("stereo", n, h, w).items()}
-        m(d["img0"], d["img1"], **cfg["call"])
+        m(d["img0"], d["img1"], **workload_call("gmstereo-scale2"))
     assert captured_keys - (set(m._attn_ws) | set(m._pad_ws)), "the runner's planes were not evicted: the scenario was not reached"
     held = {t.data_ptr() for t in runner._held_buffers}
     assert captured <= held, "cached buffers the runner's graphs write are no longer referenced"

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import refops
 import refops_ragged
 from oracle import disp_viz as OD
 from unimatch_b200 import MixedSizeStereoRunner, UniMatch, ops, submission
@@ -71,16 +72,12 @@ def test_step_layout_right_views():
     assert list(outputs["flags"]) == [ops.RAGGED_FLIP_X] * 2
 
 
-def _table(*recs):
-    return torch.from_numpy(np.array(list(recs), RAGGED_ITEM).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES))
-
-
 def test_ragged_statements_equal_the_uniform_ops_cpu():
     """the CPU statements place every item where its descriptor says, as the uniform op computes it"""
-    refops_ragged.register_cpu_kernels()
+    refops.register_cpu_kernels()
     g = torch.Generator().manual_seed(5)
     x = torch.randn((3, 1, 6, 9), generator=g)
-    items = _table((0, 4, 5, 1.25, 0), (20, 6, 9, 1.0, 0), (74, 6, 9, 1.0, ops.RAGGED_FLIP_X))
+    items = refops_ragged.table([(0, 4, 5, 1.25, 0), (20, 6, 9, 1.0, 0), (74, 6, 9, 1.0, ops.RAGGED_FLIP_X)])
     out = torch.ops.unimatch_sm100.resize_bilinear_ragged(x, items, 8, 10, 128)
     assert torch.equal(out[:20].view(4, 5), torch.ops.unimatch_sm100.resize_bilinear(x[:1], 4, 5, [1.25], False)[0, 0])
     assert torch.equal(out[20:74].view(6, 9), x[1, 0])
@@ -90,7 +87,7 @@ def test_ragged_statements_equal_the_uniform_ops_cpu():
     assert torch.equal(pics[60:222].view(6, 9, 3), torch.from_numpy(OD.vis_disparity(x[1, 0].numpy())))
     assert torch.equal(pics[222:].view(6, 9, 3), torch.from_numpy(OD.vis_disparity(x[2, 0].flip(-1).numpy())))
     frames = torch.randint(0, 256, (3 * (4 * 5 + 6 * 9),), generator=g, dtype=torch.uint8)
-    fitems = _table((0, 4, 5, 1.0, 0), (60, 6, 9, 1.0, 0))
+    fitems = refops_ragged.table([(0, 4, 5, 1.0, 0), (60, 6, 9, 1.0, 0)])
     planes = torch.ops.unimatch_sm100.frames_to_planar_normalized_ragged(frames, fitems, 8, 10, 6, 9, [0.5] * 3, [0.25] * 3)
     assert torch.equal(planes[1], torch.ops.unimatch_sm100.frames_to_planar_normalized(frames[60:].view(1, 6, 9, 3), 6, 9,
                                                                                        [0.5] * 3, [0.25] * 3)[0])

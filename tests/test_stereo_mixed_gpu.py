@@ -13,20 +13,14 @@ import torch
 import refops_depth
 import refops_ragged
 from oracle import disp_viz as OD
-from unimatch_b200 import MixedSizeStereoRunner, UniMatch, ops
-from unimatch_b200.inference import RAGGED_ITEM, disparity_to_image
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import (BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_state_dict,
-                                     synthetic_stereo_frames)
+from unimatch_b200 import MixedSizeStereoRunner, ops
+from unimatch_b200.inference import disparity_to_image
+from unimatch_b200.synthetic import (IMAGENET_MEAN, IMAGENET_STD, synthetic_batch, synthetic_model, synthetic_stereo_frames,
+                                     workload_call)
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
 FLIP = ops.RAGGED_FLIP_X
-
-
-def _table(recs):
-    t = torch.from_numpy(np.array(list(recs), RAGGED_ITEM).view(np.uint8).reshape(-1, ops.RAGGED_ITEM_BYTES))
-    return t.cuda()
 
 
 def _packed(sizes):
@@ -44,7 +38,7 @@ def test_frames_to_planar_normalized_ragged_equals_per_frame():
     frames = [torch.randint(0, 256, (h, w, 3), generator=g, dtype=torch.uint8) for h, w in sizes]
     offsets, total = _packed(sizes)
     packed = torch.cat([f.reshape(-1) for f in frames]).cuda()
-    items = _table((3 * o, h, w, 1.0, 0) for o, (h, w) in zip(offsets, sizes))
+    items = refops_ragged.table([(3 * o, h, w, 1.0, 0) for o, (h, w) in zip(offsets, sizes)], "cuda")
     mean, std = list(IMAGENET_MEAN), list(IMAGENET_STD)
     out = _OPS.frames_to_planar_normalized_ragged(packed, items, 64, 80, 40, 56, mean, std)
     ref = refops_ragged.frames_to_planar_normalized_ragged(packed, items, 64, 80, 40, 56, mean, std)
@@ -69,7 +63,7 @@ def test_resize_bilinear_ragged_equals_per_image():
     flags = [0, FLIP, 0, FLIP, FLIP, 0]
     scales = [np.float32(53 / float(w)), np.float32(29 / float(w)), 1.0, 1.0, np.float32(77 / float(w)), 1.0]
     offsets, total = _packed(sizes)
-    items = _table((o, hh, ww, s, f) for o, (hh, ww), s, f in zip(offsets, sizes, scales, flags))
+    items = refops_ragged.table([(o, hh, ww, s, f) for o, (hh, ww), s, f in zip(offsets, sizes, scales, flags)], "cuda")
     out = _OPS.resize_bilinear_ragged(x, items, 64, 80, total)
     ref = refops_ragged.resize_bilinear_ragged(x, items, 64, 80, total)
     assert torch.equal(out.isnan(), ref.isnan()) and torch.equal(out.nan_to_num(), ref.nan_to_num())
@@ -93,7 +87,7 @@ def test_disparity_to_image_ragged_equals_per_image():
     disps[5][0, 0] = float("-inf")
     offsets, total = _packed(sizes)
     packed = torch.cat([d.reshape(-1) for d in disps]).cuda()
-    items = _table((o, h, w, 1.0, 0) for o, (h, w) in zip(offsets, sizes))
+    items = refops_ragged.table([(o, h, w, 1.0, 0) for o, (h, w) in zip(offsets, sizes)], "cuda")
     pics = torch.zeros((3 * total,), dtype=torch.uint8, device="cuda")
     for _ in range(2):
         _OPS.disparity_to_image_ragged(packed, items, pics, 48, 64)
@@ -107,14 +101,6 @@ def test_disparity_to_image_ragged_equals_per_image():
     for i in (1, 2, 3, 4, 5):
         assert (pics[3 * offsets[i]:3 * (offsets[i] + sizes[i][0] * sizes[i][1])].view(-1, 3).cpu() ==
                 torch.from_numpy(OD.INFERNO_BGR[0])).all(), i
-
-
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg
 
 
 # A KITTI-like interleaved mix (heights and widths a few pixels apart); with padding 32 they fall into the (128, 256) and
@@ -148,7 +134,7 @@ CASES = {                    # sizes, batch, max_buckets, runner arguments
 def test_mixed_runner_equals_composed_reference(workload, case):
     sizes, batch, max_buckets, kw = CASES[case]
     kw = dict(kw)
-    m, call, _ = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload, drop=("task",))
     pairs = _pairs(sizes, seed=40)
     return_disp = kw.get("return_disp", True)
     runner = MixedSizeStereoRunner(m, CAP, batch, "cuda", padding_factor=32, visualize=True, max_buckets=max_buckets, **kw,
@@ -177,7 +163,7 @@ def test_mixed_runner_equals_composed_reference(workload, case):
 def test_mixed_runner_survives_other_shapes():
     """capture two buckets, evict the module's cached planes with forwards at other batch sizes and shapes, check that the
     runner still holds every buffer its graphs write, then replay bit for bit"""
-    m, call, cfg = _model("gmstereo-scale2")
+    m, call = synthetic_model("gmstereo-scale2"), workload_call("gmstereo-scale2", drop=("task",))
     pairs = _pairs(MIX, seed=70)
     runner = MixedSizeStereoRunner(m, CAP, 2, "cuda", padding_factor=32, visualize=True, **call)
     r1 = {i: {k: v.clone() for k, v in r.items()} for i, r in runner.run(pairs)}
@@ -187,7 +173,7 @@ def test_mixed_runner_survives_other_shapes():
     assert captured
     for n, h, w in [(1, 384, 512), (3, 384, 512), (2, 320, 448), (1, 256, 384), (4, 256, 384)]:
         d = {k: v.cuda() for k, v in synthetic_batch("stereo", n, h, w).items()}
-        m(d["img0"], d["img1"], **cfg["call"])
+        m(d["img0"], d["img1"], **workload_call("gmstereo-scale2"))
     assert captured_keys - (set(m._attn_ws) | set(m._pad_ws)), "the runner's planes were not evicted: the scenario was not reached"
     held = {t.data_ptr() for _, _, bufs in runner.buckets.values() for t in bufs}
     assert captured <= held, "cached buffers the runner's graphs write are no longer referenced"

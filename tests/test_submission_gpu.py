@@ -9,10 +9,9 @@ import pytest
 import torch
 
 from oracle import submission_io as S
-from unimatch_b200 import UniMatch, ops, submission
+from unimatch_b200 import ops, submission
 from unimatch_b200.inference import InputPadder, _resize, disparity_to_image, flow_to_image
-from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+from unimatch_b200.synthetic import synthetic_model, workload_call
 
 pytestmark = pytest.mark.gpu
 OPS = torch.ops.unimatch_sm100
@@ -69,13 +68,6 @@ def test_encode_rejects_bad_arguments():
 
 
 # --------------------------------------------------------------------------------------------------- drivers end to end
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    return m.cuda(), {k: v for k, v in cfg["call"].items() if k != "task"}
-
-
 def _model_inputs(images, geom, padding_factor, mode):
     """The driver's model inputs for stacked device images, restated: InputPadder or the resize."""
     if geom[0] == "pad":
@@ -92,7 +84,7 @@ def _read(path):
 
 @torch.no_grad()
 def test_flow_drivers_end_to_end(tmp_path):
-    model, kw = _model("gmflow-scale1")
+    model, kw = synthetic_model("gmflow-scale1"), workload_call("gmflow-scale1", drop=("task",))
     g = torch.Generator().manual_seed(5)
     sizes = [(60, 90), (60, 90), (52, 100), (60, 90)]
     sintel = [(torch.rand((3, h, w), generator=g) * 255, torch.rand((3, h, w), generator=g) * 255, ("seq%d" % (i % 2), i))
@@ -128,7 +120,7 @@ def test_stereo_drivers_end_to_end(tmp_path):
             ("gmstereo-scale2", "eth3d", [(70, 100), (64, 96), (70, 100)], None, False),       # resize, then none
             ("gmstereo-scale2", "eth3d", [(70, 100)], None, True),
             ("gmstereo-scale2-regrefine3", "middlebury", [(70, 100), (70, 100), (70, 100)], None, False)):
-        model, kw = _model(workload)
+        model, kw = synthetic_model(workload), workload_call(workload, drop=("task",))
         data = [{"left": torch.randn((3, h, w), generator=g), "right": torch.randn((3, h, w), generator=g),
                  "left_name": "scenes/scene%d/im0.png" % i if protocol != "kitti" else "%06d_10.png" % i}
                 for i, (h, w) in enumerate(sizes)]

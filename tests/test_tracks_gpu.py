@@ -14,10 +14,11 @@ import pytest
 import torch
 
 import refops_tracks as RT
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import VideoFlowRunner, VideoTrackRunner, chain_tracks, infer_flow_video
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+from unimatch_b200.synthetic import synthetic_model, synthetic_video, workload_call
+
+_WL = "gmflow-scale1"
 
 pytestmark = pytest.mark.gpu
 _OPS = torch.ops.unimatch_sm100
@@ -117,14 +118,6 @@ def test_kernel_in_cuda_graph():
         assert torch.equal(out[0], ref["tracks"]) and torch.equal(out[1], ref["visible"])
 
 
-def _model(workload="gmflow-scale1"):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg["pad"]
-
-
 def _run(runner, frames):
     return [{k: v.clone() for k, v in r.items()} for r in runner.run(list(frames.numpy()))]
 
@@ -134,7 +127,8 @@ def test_runner_matches_statement(batch, hw):
     """10 frames: 9 steps of one pair, or steps of 4 / 4 / 1 (+3 repeats), or a portrait clip in steps of 3.  The tracks are
     the statement on the runner's own flows and masks bit for bit (fp32), and agree with the float64 statement on
     `infer_flow_video`'s flows and masks within the flows' difference (the encoder's summation order) carried along"""
-    m, call, pad = _model()
+    m, call = synthetic_model(_WL), workload_call(_WL, drop=("task",))
+    pad = WORKLOADS[_WL]["pad"]
     h, w = hw
     frames = synthetic_video(10, h, w, seed=31)
     runner = VideoTrackRunner(m, hw, batch, "cuda", padding_factor=pad, return_flow=True, **call)
@@ -172,7 +166,8 @@ def test_runner_matches_statement(batch, hw):
 def test_runner_graph_replay_and_reset():
     """tracks with and without graph replay; a second run starts again from the first frame; return_flow=False sends back
     the tracks only"""
-    m, call, pad = _model()
+    m, call = synthetic_model(_WL), workload_call(_WL, drop=("task",))
+    pad = WORKLOADS[_WL]["pad"]
     frames = synthetic_video(7, 64, 96, seed=8)
     out = {}
     for use_graph in (False, True):
@@ -196,7 +191,8 @@ def test_runner_graph_replay_and_reset():
 def test_runner_flows_equal_video_flow_runner(use_graph):
     """VideoTrackRunner(return_flow=True) returns what VideoFlowRunner(pred_bidir_flow=True, fwd_bwd_consistency_check=True)
     returns, bit for bit"""
-    m, call, pad = _model()
+    m, call = synthetic_model(_WL), workload_call(_WL, drop=("task",))
+    pad = WORKLOADS[_WL]["pad"]
     frames = synthetic_video(8, 64, 96, seed=9)
     tr = _run(VideoTrackRunner(m, (64, 96), 3, "cuda", padding_factor=pad, use_graph=use_graph, return_flow=True, **call),
               frames)

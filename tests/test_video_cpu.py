@@ -8,7 +8,7 @@ import pytest
 import torch
 
 import cases
-import refops_video
+import refops
 from cases import O
 from oracle import flow_viz as OV
 from unimatch_b200 import UniMatch
@@ -57,7 +57,7 @@ def _tiny_model():
     (3, (48, 64), None, False, True),                 # backward flow (pairs swapped)
 ])
 def test_infer_flow_video_host_logic_cpu(T, hw, size, bidir, bwd):
-    refops_video.register_cpu_kernels()
+    refops.register_cpu_kernels()
     m, sd, kw, mk = _tiny_model()
     frames = synthetic_video(T, *hw, seed=7)
     got = infer_flow_video(m, frames, padding_factor=16, inference_size=size, pred_bidir_flow=bidir, pred_bwd_flow=bwd,
@@ -83,7 +83,7 @@ def test_infer_flow_video_host_logic_cpu(T, hw, size, bidir, bwd):
 
 
 def test_infer_flow_video_argument_errors():
-    refops_video.register_cpu_kernels()
+    refops.register_cpu_kernels()
     m, _, kw, _ = _tiny_model()
     frames = synthetic_video(3, 32, 48)
     with pytest.raises(ValueError):

@@ -12,10 +12,9 @@ import pytest
 import torch
 
 from oracle import flow_viz as OV
-from unimatch_b200 import UniMatch
 from unimatch_b200.inference import VideoFlowRunner, flow_to_image, infer_flow, infer_flow_video
 from unimatch_b200.spec import WORKLOADS
-from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+from unimatch_b200.synthetic import synthetic_model, synthetic_video, workload_call
 
 pytestmark = pytest.mark.gpu
 GOLD_VIS = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "golden_vis.pt"))
@@ -89,14 +88,6 @@ def test_frames_to_planar_equals_resize(hw, size, transpose):
         assert torch.equal(got, x)
 
 
-def _model(workload):
-    cfg = WORKLOADS[workload]
-    m = UniMatch(**cfg["model"]).eval()
-    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]))
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
-    return m.cuda(), call, cfg["pad"]
-
-
 def _close(got, ref, what, rel=1e-4):
     err = (got.float() - ref.float()).abs().max().item()
     assert err <= rel * max(1.0, ref.abs().max().item()), (what, err)
@@ -104,7 +95,7 @@ def _close(got, ref, what, rel=1e-4):
 
 def test_encoder_is_per_frame():
     """a frame's pyramid does not depend on the batch it is encoded in (up to summation order); same batch: bit for bit"""
-    m, _, _ = _model("gmflow-scale2")
+    m = synthetic_model("gmflow-scale2")
     frames = synthetic_video(5, 64, 96, seed=2).cuda().permute(0, 3, 1, 2).float().contiguous()
     full = m.encode_frames(frames)
     assert all(torch.equal(a, b) for a, b in zip(full, m.encode_frames(frames)))
@@ -117,7 +108,8 @@ def test_encoder_is_per_frame():
 @pytest.mark.parametrize("workload,bidir,bwd", [("gmflow-scale1", False, False), ("gmflow-scale2-regrefine6", False, False),
                                                 ("gmflow-scale1", True, False), ("gmflow-scale2-regrefine6", False, True)])
 def test_infer_flow_video_equals_pairwise(workload, bidir, bwd):
-    m, call, pad = _model(workload)
+    m, call = synthetic_model(workload), workload_call(workload, drop=("task",))
+    pad = WORKLOADS[workload]["pad"]
     frames = synthetic_video(7, 128, 192, seed=11).cuda()
     got = infer_flow_video(m, frames, padding_factor=pad, pred_bidir_flow=bidir, pred_bwd_flow=bwd,
                            fwd_bwd_consistency_check=bidir, **call)
@@ -135,7 +127,8 @@ def test_infer_flow_video_equals_pairwise(workload, bidir, bwd):
 
 
 def test_infer_flow_video_portrait_resized_equals_pairwise():
-    m, call, pad = _model("gmflow-scale1")
+    m, call = synthetic_model("gmflow-scale1"), workload_call("gmflow-scale1", drop=("task",))
+    pad = WORKLOADS["gmflow-scale1"]["pad"]
     frames = synthetic_video(4, 100, 70, seed=12).cuda()
     got = infer_flow_video(m, frames, padding_factor=pad, inference_size=(64, 112), **call)
     planar = frames.permute(0, 3, 1, 2).float()
@@ -147,7 +140,8 @@ def test_infer_flow_video_portrait_resized_equals_pairwise():
 @pytest.mark.parametrize("use_graph", [False, True])
 def test_video_flow_runner_matches_infer_flow_video(use_graph):
     """11 frames, batch 4: frame 0 primes the carried pyramid, then three steps of 4 / 4 / 2 (+2 repeats) new frames."""
-    m, call, pad = _model("gmflow-scale1")
+    m, call = synthetic_model("gmflow-scale1"), workload_call("gmflow-scale1", drop=("task",))
+    pad = WORKLOADS["gmflow-scale1"]["pad"]
     frames = synthetic_video(11, 96, 160, seed=21)
     runner = VideoFlowRunner(m, (96, 160), 4, "cuda", padding_factor=pad, use_graph=use_graph, visualize=True,
                              pred_bidir_flow=True, **call)
@@ -165,7 +159,8 @@ def test_video_flow_runner_matches_infer_flow_video(use_graph):
 @pytest.mark.parametrize("hw,return_flow", [((64, 96), True), ((96, 64), True), ((64, 96), False)])
 def test_video_flow_runner_concat_layout(hw, return_flow):
     """concat_flow_img (evaluate_flow.py:818-825): frame above its picture when H < W, beside it otherwise."""
-    m, call, pad = _model("gmflow-scale1")
+    m, call = synthetic_model("gmflow-scale1"), workload_call("gmflow-scale1", drop=("task",))
+    pad = WORKLOADS["gmflow-scale1"]["pad"]
     h, w = hw
     frames = synthetic_video(6, h, w, seed=4)
     runner = VideoFlowRunner(m, hw, 4, "cuda", padding_factor=pad, visualize=True, concat_frame=True, return_flow=return_flow,

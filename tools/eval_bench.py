@@ -18,9 +18,7 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
-import time
 
 import torch
 
@@ -28,9 +26,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True
 
-from unimatch_b200 import UniMatch, evaluation  # noqa: E402
+from tools.common import card, timed  # noqa: E402
+from unimatch_b200 import evaluation  # noqa: E402
 from unimatch_b200.spec import WORKLOADS  # noqa: E402
-from unimatch_b200.synthetic import BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_state_dict  # noqa: E402
+from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_model, workload_call  # noqa: E402
 
 PROTOCOLS = {  # protocol -> (task, workload, shapes, padding factor, driver options)
     "sintel": ("flow", "gmflow-scale2-regrefine6", [(436, 1024)], 32, dict(protocol="sintel", with_speed_metric=True)),
@@ -62,14 +61,6 @@ def dataset(task, shapes, n, seed=0):
     return out
 
 
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        return "nvidia-smi unavailable (%s)" % e
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--protocol", required=True, choices=sorted(PROTOCOLS))
@@ -81,11 +72,8 @@ def main():
     sys.path.insert(0, os.path.join(ROOT, "tests"))
     import refloop_eval
     task, workload, shapes, pad, opts = PROTOCOLS[args.protocol]
-    cfg = WORKLOADS[workload]
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(**BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.cuda()
-    kw = {k: v for k, v in cfg["call"].items() if k not in ("min_depth", "max_depth")}
+    model = synthetic_model(workload)
+    kw = workload_call(workload, drop=("min_depth", "max_depth"))
     driver = {"flow": evaluation.validate_flow, "stereo": evaluation.validate_stereo, "depth": evaluation.validate_depth}[task]
     data = dataset(task, shapes, args.samples)
     warm = data[:len(shapes)]
@@ -96,15 +84,12 @@ def main():
     def batched(d):
         return driver(model, d, batch=args.batch, padding_factor=pad, **opts, **kw)
 
-    print("card:", card(), flush=True)
+    gpu = ", ".join(card().values())
+    print("card:", gpu, flush=True)
     times, results = {}, {}
     for name, fn in (("per_sample", loop), ("batched", batched)):
         fn(warm)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        results[name] = fn(data)
-        torch.cuda.synchronize()
-        times[name] = time.perf_counter() - t0
+        times[name], results[name] = timed(lambda: fn(data))
     want, got = results["per_sample"], results["batched"]
     worst_sum = worst_ratio = 0.0
     for k, v in want.items():
@@ -116,7 +101,7 @@ def main():
     res = dict(protocol=args.protocol, workload=workload, samples=args.samples, batch=args.batch,
                per_sample_samples_per_s=args.samples / times["per_sample"], batched_samples_per_s=args.samples / times["batched"],
                speedup=times["per_sample"] / times["batched"], max_rel_diff_sums=worst_sum, max_abs_diff_ratios=worst_ratio,
-               results=got, card=card())
+               results=got, card=gpu)
     print(json.dumps(res))
     if not (worst_sum <= 1e-4 and worst_ratio <= 1e-3) or any(math.isnan(v) for v in got.values()):
         sys.exit("batched results disagree with the per-sample loop")

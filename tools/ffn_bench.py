@@ -24,7 +24,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -32,17 +31,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tools.common import card  # noqa: E402
 from unimatch_b200 import ops  # noqa: E402
 
 PEAK_FP16_TFLOPS = 989.0
-
-
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        return "nvidia-smi unavailable (%s)" % e
 
 
 def operands(rows, hidden, dev, seed):
@@ -86,6 +78,7 @@ def lib_launcher(lib, t):
 
 
 def time_ms(launch, iters, warmup):
+    """mean device time of one launch, from CUDA events around `iters` back-to-back launches (common.timed is host time)"""
     for _ in range(warmup):
         launch()
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -118,7 +111,7 @@ def main():
         lib.um_ffn_tc.restype = ctypes.c_int
         lib.um_ffn_tc.argtypes = [ctypes.POINTER(ops.FfnDesc), ctypes.c_void_p]
         bases.append(("base%d" % i, path, lib))
-    gpu = card()
+    gpu = ", ".join(card().values())
     print("card: %s" % gpu, flush=True)
     result = {"card": gpu, "hidden": args.hidden, "iters": args.iters, "rounds": args.rounds,
               "baselines": {k: path for k, path, _ in bases}, "shapes": []}

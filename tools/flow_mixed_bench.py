@@ -26,7 +26,6 @@ import gc
 import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
@@ -35,7 +34,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from tools.stereo_bench import _power_limit  # noqa: E402
+from tools.common import card, timed  # noqa: E402
 
 KITTI_SIZES = [(375, 1242), (370, 1226), (374, 1238), (376, 1241)]
 SIZES = KITTI_SIZES + [(436, 1024), (832, 480)]
@@ -53,14 +52,6 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("flow_mixed_bench needs a CUDA device: nothing is measured without one")
     run(args)
-
-
-def _timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return time.perf_counter() - t0, out
 
 
 def _stream(n, seed=17):
@@ -123,9 +114,8 @@ def _kernel_times(batch, launches, dev):
 @torch.no_grad()
 def run(args):
     from oracle import flow_viz as OV
-    from unimatch_b200 import BatchedFlowRunner, MixedSizeFlowRunner, UniMatch, infer_flow
-    from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+    from unimatch_b200 import BatchedFlowRunner, MixedSizeFlowRunner, infer_flow
+    from unimatch_b200.synthetic import synthetic_model, workload_call
 
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
@@ -134,15 +124,12 @@ def run(args):
     floats = [tuple(torch.from_numpy(f).permute(2, 0, 1).float() for f in p) for p in pairs]     # arm 3's input format
     res = {"metric": "pairs/s of an interleaved mixed-size flow stream (%d pairs of %d sizes, batch %d, padding 32): "
                      "MixedSizeFlowRunner vs the per-pair host loop vs one BatchedFlowRunner per size" % (N, len(SIZES), B),
-           "device": torch.cuda.get_device_name(dev), "power_limit": _power_limit(), "pairs": N, "batch": B,
+           "device": torch.cuda.get_device_name(dev), "power_limit": card()["power_limit"], "pairs": N, "batch": B,
            "sizes": [list(s) for s in SIZES], "runs": {}}
 
     for name in args.models.split(","):
-        cfg = WORKLOADS[name]
-        model = UniMatch(**cfg["model"]).eval()
-        model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-        model = model.to(dev)
-        call = {k: v for k, v in cfg["call"].items() if k != "task"}
+        model = synthetic_model(name, dev)
+        call = workload_call(name, drop=("task",))
         groups = {s: [i for i in range(N) if sizes[i] == s] for s in SIZES if s in sizes}
         for pictures in (True, False):
             stats = {}
@@ -179,10 +166,10 @@ def run(args):
             for _ in range(args.reps):
                 for k, make in arms.items():
                     fn = make()
-                    cold[k].append(_timed(fn)[0])
+                    cold[k].append(timed(fn)[0])
                     if k == "mixed":
                         s0 = dict(stats["mixed"].stats)
-                    walls[k].append(_timed(fn)[0])
+                    walls[k].append(timed(fn)[0])
                     if k == "mixed":
                         mixed = stats.pop("mixed")
                         st = {key: mixed.stats[key] - s0[key] for key in mixed.stats}

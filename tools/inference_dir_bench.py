@@ -33,10 +33,8 @@ import argparse
 import json
 import os
 import shutil
-import subprocess
 import sys
 import tempfile
-import time
 
 import numpy as np
 import torch
@@ -45,18 +43,11 @@ from PIL import Image
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from tools.common import card, timed  # noqa: E402
+
 KITTI_SIZES = [(375, 1242), (370, 1226), (374, 1238), (376, 1241)]
 ETH3D_SIZES = [(489, 754), (455, 742), (501, 720), (480, 752)]
 SCANNET_MIXED = [(468, 624), (470, 630), (375, 500)]     # none already at its inference size (see inference_depth)
-
-
-def _gpu():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
 
 
 def _write_inputs(root, n_frames):
@@ -224,14 +215,6 @@ def _stereo_loop(model, dirs, output_path, padding_factor, inference_size, call)
                                                                              os.path.basename(name_l)[:-4] + "_disp.png"))
 
 
-def _timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return time.perf_counter() - t0, out
-
-
 @torch.no_grad()
 def main():
     ap = argparse.ArgumentParser()
@@ -244,19 +227,16 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("inference_dir_bench needs a CUDA device: nothing is measured without one")
-    from unimatch_b200 import UniMatch, inference_depth, inference_flow, inference_stereo
-    from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+    from unimatch_b200 import inference_depth, inference_flow, inference_stereo
+    from unimatch_b200.synthetic import synthetic_model, workload_call
 
     def model(name):
-        cfg = WORKLOADS[name]
-        m = UniMatch(**cfg["model"]).eval()
-        m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-        return m.cuda(), {k: v for k, v in cfg["call"].items() if k != "task"}
+        return synthetic_model(name), workload_call(name, drop=("task",))
 
     root = tempfile.mkdtemp(prefix="inference_dir_bench_")
     res = {"metric": "pairs/s from image files on disk to result files on disk: drop-in driver vs the reference's loop "
-                     "restated around the same module", "gpu": _gpu(), "device": torch.cuda.get_device_name(0),
+                     "restated around the same module", "gpu": "%(name)s, %(power_limit)s, %(max_sm_clock)s" % card(),
+           "device": torch.cuda.get_device_name(0),
            "batch": args.batch, "readers": args.readers, "writers": args.writers, "runs": {}}
     try:
         dirs = _write_inputs(root, args.frames)
@@ -310,7 +290,7 @@ def main():
                 for arm, fn in (("driver", driver), ("loop", loop)):
                     out = os.path.join(root, "out", name, arm, str(rep))
                     os.makedirs(out)
-                    wall, stats = _timed(lambda: fn(out))
+                    wall, stats = timed(lambda: fn(out))
                     if rep == 0:
                         run[arm]["first_pass_s"] = round(wall, 4)
                         continue

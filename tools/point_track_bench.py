@@ -22,7 +22,6 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
@@ -30,10 +29,9 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 from bench import BENCH_WORKLOADS  # noqa: E402
-from track_bench import _card  # noqa: E402
+from tools.common import card as read_card, timed  # noqa: E402
 
 
 def query_sets(n, nframes, h, w, seed=3):
@@ -86,7 +84,8 @@ def host_point_tracks(runner, frames, queries, h, w):
 
 
 def event_ms(fn, launches, reset=None):
-    """mean CUDA-event time of `fn` over `launches` launches (reset, outside the events, before each)"""
+    """mean CUDA-event time of `fn` over `launches` launches (reset, outside the events, before each); common.timed is the
+    host-clock time of a whole path"""
     for _ in range(5):
         fn()
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(launches)]
@@ -110,21 +109,18 @@ def main():
     ap.add_argument("--pairs-per-step", type=int, default=0, help="B (default: the workload's pairs per GPU in bench.py)")
     ap.add_argument("--kernel-launches", type=int, default=200)
     args = ap.parse_args()
-    from unimatch_b200 import UniMatch
     from unimatch_b200.inference import PointTrackRunner, VideoFlowRunner
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+    from unimatch_b200.synthetic import synthetic_model, synthetic_video, workload_call
     ops = torch.ops.unimatch_sm100
     wl_name, H, W, ppg, cfg_idx, _, _ = BENCH_WORKLOADS[args.workload]
     cfg = WORKLOADS[wl_name]
     B = args.pairs_per_step or ppg
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    card = _card()
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.to(dev)
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    card = read_card()
+    model = synthetic_model(wl_name, dev)
+    call = workload_call(wl_name, drop=("task",))
     frames = list(synthetic_video(1 + args.steps * B, H, W, seed=77).numpy())
     T, pairs = len(frames), len(frames) - 1
     sets = query_sets(args.queries, T, H, W)
@@ -150,11 +146,7 @@ def main():
     secs = {k: 0.0 for k, _ in paths}
     for _ in range(args.repeats):
         for k, fn in paths:
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            torch.cuda.synchronize()
-            secs[k] += time.perf_counter() - t0
+            secs[k] += timed(fn)[0]
 
     results = {}
     for s, q in sets.items():

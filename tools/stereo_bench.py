@@ -20,7 +20,6 @@ for bit identical.  Writes nothing to the tree.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -31,6 +30,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 from bench import BENCH_WORKLOADS  # noqa: E402
+from tools.common import card  # noqa: E402
 
 HBM_DATASHEET_GBS = 3350.0
 
@@ -46,33 +46,21 @@ def main():
     run(ap.parse_args())
 
 
-def _power_limit():
-    try:
-        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30)
-        return r.stdout.strip() or "unknown"
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
-
-
 @torch.no_grad()
 def run(args):
     import refops_depth
     from oracle import disp_viz as OD
-    from unimatch_b200 import UniMatch
     from unimatch_b200.inference import StereoRunner, disparity_to_image, infer_stereo
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_state_dict, synthetic_stereo_frames
+    from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_model, synthetic_stereo_frames, workload_call
     wl_name, H, W, ppg, cfg_idx, _, _ = BENCH_WORKLOADS[args.workload]
     name = args.model or wl_name
     cfg = WORKLOADS[name]
     B = args.pairs_per_step or ppg
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.to(dev)
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    model = synthetic_model(name, dev)
+    call = workload_call(name, drop=("task",))
     pad = cfg["pad"]
     lefts, rights = synthetic_stereo_frames(B, H, W, seed=77)
 
@@ -142,7 +130,7 @@ def run(args):
     res = {"metric": "pairs/s of %d stereo pairs @%dx%d %s per step: StereoRunner step (uint8 in, graph, disparity + picture "
                      "back) vs today's path (host-normalised float32 in, infer_stereo, disparity back, coloured on the CPU)"
                      % (B, H, W, name),
-           "device": torch.cuda.get_device_name(dev), "power_limit": _power_limit(),
+           "device": torch.cuda.get_device_name(dev), "power_limit": card()["power_limit"],
            "workload": "%s %dx%d, %d pairs per step (bench.py %s weights, BASELINE configs[%d])" % (name, H, W, B, args.workload,
                                                                                                     cfg_idx),
            "steps": args.steps, "warmup": max(args.warmup, 1), "data": "synthetic_stereo_frames seed 77",

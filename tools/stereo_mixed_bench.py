@@ -34,7 +34,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from tools.stereo_bench import _power_limit  # noqa: E402
+from tools.common import card, timed  # noqa: E402
 
 KITTI_SIZES = [(375, 1242), (370, 1226), (374, 1238), (376, 1241)]
 MODES = {"inference_size": dict(padding_factor=32, inference_size=(352, 1216)),
@@ -50,31 +50,19 @@ def main():
     run(ap.parse_args())
 
 
-def _timed(fn):
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    out = fn()
-    torch.cuda.synchronize()
-    return time.perf_counter() - t0, out
-
-
 @torch.no_grad()
 def run(args):
     import refops_depth
     import refops_ragged
     from oracle import disp_viz as OD
-    from unimatch_b200 import MixedSizeStereoRunner, StereoRunner, UniMatch
+    from unimatch_b200 import MixedSizeStereoRunner, StereoRunner
     from unimatch_b200.inference import infer_stereo
-    from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_state_dict, synthetic_stereo_frames
+    from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_model, synthetic_stereo_frames, workload_call
 
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    cfg = WORKLOADS[args.model]
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.to(dev)
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    model = synthetic_model(args.model, dev)
+    call = workload_call(args.model, drop=("task",))
     B, N = args.batch, args.pairs
     sizes = [KITTI_SIZES[i % len(KITTI_SIZES)] for i in range(N)]
     frames = {s: synthetic_stereo_frames(1, s[0], s[1], seed=90 + k) for k, s in enumerate(KITTI_SIZES)}
@@ -87,7 +75,7 @@ def run(args):
     checked_ok = True
     res = {"metric": "pairs/s of a KITTI-like mixed-size stereo stream (%d pairs of 4 sizes, %s, batch %d): "
                      "MixedSizeStereoRunner vs one StereoRunner per size vs the per-pair host loop" % (N, args.model, B),
-           "device": torch.cuda.get_device_name(dev), "power_limit": _power_limit(), "pairs": N, "batch": B,
+           "device": torch.cuda.get_device_name(dev), "power_limit": card()["power_limit"], "pairs": N, "batch": B,
            "sizes": [list(s) for s in KITTI_SIZES], "model": args.model, "modes": {}}
 
     for mode, geo in MODES.items():
@@ -110,9 +98,9 @@ def run(args):
         def mixed_pass():
             return {i: {k: v.clone() for k, v in r.items()} for i, r in mixed.run(pairs)}
 
-        cold_m, _ = _timed(mixed_pass)
+        cold_m, _ = timed(mixed_pass)
         s0 = dict(mixed.stats)
-        wall_m, got_m = _timed(mixed_pass)
+        wall_m, got_m = timed(mixed_pass)
         st = {k: mixed.stats[k] - s0[k] for k in mixed.stats}
 
         groups = {s: [i for i in range(N) if sizes[i] == s] for s in KITTI_SIZES}
@@ -125,8 +113,8 @@ def run(args):
                     out[i] = {k: v.clone() for k, v in r.items()}
             return out
 
-        cold_p, _ = _timed(pool_pass)
-        wall_p, got_p = _timed(pool_pass)
+        cold_p, _ = timed(pool_pass)
+        wall_p, got_p = timed(pool_pass)
         pool_steps = sum(-(-len(idx) // B) for idx in groups.values())
         pool_h2d = sum(-(-len(groups[s]) // B) * 2 * B * s[0] * s[1] * 3 for s in KITTI_SIZES)
         pool_d2h = sum(-(-len(groups[s]) // B) * B * s[0] * s[1] * 7 for s in KITTI_SIZES)
@@ -140,8 +128,8 @@ def run(args):
                 out[i] = {"disp": d, "vis": torch.from_numpy(OD.vis_disparity(d.numpy()))}
             return out
 
-        cold_l, _ = _timed(loop_pass)
-        wall_l, _ = _timed(loop_pass)
+        cold_l, _ = timed(loop_pass)
+        wall_l, _ = timed(loop_pass)
         loop_h2d = sum(2 * 3 * h * w * 4 for h, w in sizes)
         loop_d2h = sum(4 * h * w for h, w in sizes)
 

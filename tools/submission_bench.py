@@ -19,10 +19,8 @@ import argparse
 import json
 import os
 import shutil
-import subprocess
 import sys
 import tempfile
-import time
 
 import numpy as np
 import torch
@@ -31,10 +29,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True
 
-from unimatch_b200 import UniMatch, ops, submission  # noqa: E402
+from tools.common import card, timed  # noqa: E402
+from unimatch_b200 import ops, submission  # noqa: E402
 from unimatch_b200.inference import InputPadder  # noqa: E402
 from unimatch_b200.spec import WORKLOADS  # noqa: E402
-from unimatch_b200.synthetic import BENCH_WEIGHTS, IMAGENET_MEAN, IMAGENET_STD, synthetic_state_dict  # noqa: E402
+from unimatch_b200.synthetic import IMAGENET_MEAN, IMAGENET_STD, synthetic_model, workload_call  # noqa: E402
 
 PROTOCOLS = {  # protocol -> (task, workload, size, padding factor, InputPadder mode, format)
     "sintel": ("flow", "gmflow-scale2-regrefine6", (436, 1024), 32, "sintel", ops.SUBMIT_FLO),
@@ -111,14 +110,6 @@ def reference_loop(model, data, out, task, protocol, pad, mode, kw, cv2):
     return d2h
 
 
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
-                              capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError) as e:
-        return "nvidia-smi unavailable (%s)" % e
-
-
 def _count(root):
     return sum(len(fs) for _, _, fs in os.walk(root))
 
@@ -150,11 +141,8 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("submission_bench needs a CUDA device")
     task, workload, size, pad, mode, fmt = PROTOCOLS[args.protocol]
-    cfg = WORKLOADS[workload]
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(**BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.cuda()
-    kw = {k: v for k, v in cfg["call"].items() if k != "task"}
+    model = synthetic_model(workload)
+    kw = workload_call(workload, drop=("task",))
     data = dataset(task, args.protocol, size, args.samples)
     cv2 = _cv2()
     driver = submission.create_stereo_submission if task == "stereo" else submission.create_flow_submission
@@ -166,7 +154,8 @@ def main():
     def batched(d, out):
         return driver(model, d, protocol=proto, output_path=out, batch=args.batch, padding_factor=pad, writers=args.writers, **kw)
 
-    print("card:", card(), flush=True)
+    gpu = ", ".join(card().values())
+    print("card:", gpu, flush=True)
     root = tempfile.mkdtemp(prefix="submission_bench.")
     res = dict(protocol=args.protocol, workload=workload, size=list(size), samples=args.samples, batch=args.batch,
                writers=args.writers, reference_png_writer="cv2" if cv2 is not None else "numpy + stdlib zlib")
@@ -174,12 +163,8 @@ def main():
         files = {}
         for name, fn in (("reference_loop", loop), ("batched", batched)):
             fn(data[:args.batch], os.path.join(root, name + "_warm"))
-            torch.cuda.synchronize()
             out = os.path.join(root, name)
-            t0 = time.perf_counter()
-            stats = fn(data, out)
-            torch.cuda.synchronize()
-            wall = time.perf_counter() - t0
+            wall, stats = timed(lambda: fn(data, out))
             files[name] = _count(out)
             res[name + "_samples_per_s"] = args.samples / wall
             res[name + "_d2h_bytes_per_sample"] = stats["d2h_bytes"] / args.samples
@@ -190,7 +175,7 @@ def main():
         res["files"] = files
     finally:
         shutil.rmtree(root, ignore_errors=True)
-    res["card"] = card()
+    res["card"] = gpu
     print(json.dumps(res))
     if files["reference_loop"] != files["batched"] or files["batched"] != args.samples:
         sys.exit("the two paths wrote different numbers of files")

@@ -20,9 +20,7 @@ The card's name, power limit and maximum SM clock are read in the same run.  Pri
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
 import torch.nn.functional as F
@@ -31,19 +29,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from bench import BENCH_WORKLOADS  # noqa: E402
-
-
-def _card():
-    """name, power limit and maximum SM clock as nvidia-smi reports them (read-only query)"""
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=index,name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()
-        dev = torch.cuda.current_device()
-        row = [r for r in out if r.split(",")[0].strip() == str(dev)] or out
-        _, name, power, clock = [c.strip() for c in row[0].split(",")]
-        return {"name": name, "power_limit": power, "max_sm_clock": clock}
-    except (OSError, ValueError, IndexError, subprocess.SubprocessError) as e:
-        return {"name": torch.cuda.get_device_name(), "power_limit": "unknown (%s)" % e, "max_sm_clock": "unknown"}
+from tools.common import card as read_card, timed  # noqa: E402
 
 
 def host_tracks(h, w):
@@ -74,20 +60,17 @@ def main():
     ap.add_argument("--pairs-per-step", type=int, default=0, help="B (default: the workload's pairs per GPU in bench.py)")
     ap.add_argument("--kernel-launches", type=int, default=200)
     args = ap.parse_args()
-    from unimatch_b200 import UniMatch
     from unimatch_b200.inference import VideoFlowRunner, VideoTrackRunner, chain_tracks
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict, synthetic_video
+    from unimatch_b200.synthetic import synthetic_model, synthetic_video, workload_call
     wl_name, H, W, ppg, cfg_idx, _, _ = BENCH_WORKLOADS[args.workload]
     cfg = WORKLOADS[wl_name]
     B = args.pairs_per_step or ppg
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    card = _card()
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.to(dev)
-    call = {k: v for k, v in cfg["call"].items() if k != "task"}
+    card = read_card()
+    model = synthetic_model(wl_name, dev)
+    call = workload_call(wl_name, drop=("task",))
     frames = list(synthetic_video(1 + args.steps * B, H, W, seed=77).numpy())
     pairs = len(frames) - 1
     tr = VideoTrackRunner(model, (H, W), B, dev, padding_factor=cfg["pad"], **call)
@@ -116,11 +99,7 @@ def main():
     secs = {k: 0.0 for k, _ in paths}
     for _ in range(args.repeats):
         for k, fn in paths:
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            torch.cuda.synchronize()
-            secs[k] += time.perf_counter() - t0
+            secs[k] += timed(fn)[0]
 
     # parity of the device chain with the host loop on the last frame
     (tp, tv), (hp, hv) = last["tracks"], last["host"]

@@ -51,17 +51,15 @@ def run(args):
     """One runner step (B new synthetic uint8 frames uploaded from pinned memory, the previous step's last frame carried, B
     pairs, output back to pinned memory) against `UniMatch.forward` on the same B pairs as float32 images (uploaded and
     downloaded the same way), alternating step by step in one process, eager on both sides."""
-    from unimatch_b200 import UniMatch, ops
+    from unimatch_b200 import ops
     from unimatch_b200.spec import WORKLOADS
-    from unimatch_b200.synthetic import BENCH_WEIGHTS, synthetic_state_dict
+    from unimatch_b200.synthetic import synthetic_model
     wl_name, H, W, ppg, cfg_idx, _, _ = BENCH_WORKLOADS[args.workload]
     cfg = WORKLOADS[wl_name]
     B = args.pairs_per_step or ppg
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
-    model = UniMatch(**cfg["model"]).eval()
-    model.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg["model"]), strict=True)
-    model = model.to(dev)
+    model = synthetic_model(wl_name, dev)
     setup = _flow_steps if cfg["model"]["task"] == "flow" else _depth_steps
     video_step, pair_step, out_v, out_p, io, notes = setup(model, cfg, H, W, B, dev)
     vis_step, out_vis = _depth_picture_step(model, cfg, H, W, B, dev) if args.visualize else (None, None)

@@ -14,7 +14,7 @@ import math
 import torch
 import torch.nn.functional as F
 
-from .spec import param_spec
+from .spec import WORKLOADS, param_spec
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
@@ -64,6 +64,21 @@ def synthetic_state_dict(seed=326, damp=1.0, refine_gain=0.02, backbone_gain=1.0
             t = t * mask_gain           # logits of the convex-upsampling softmax (9 taps)
         sd[key] = t.float().contiguous()
     return sd
+
+
+def synthetic_model(workload, device="cuda"):
+    """`UniMatch` of `WORKLOADS[workload]` in eval mode with the BENCH_WEIGHTS state_dict (seed 326) loaded strictly, on
+    `device`: the model bench.py, the workload tests and the tools run."""
+    from .unimatch import UniMatch          # here, so that importing this module does not load the CUDA library
+    cfg = WORKLOADS[workload]["model"]
+    m = UniMatch(**cfg).eval()
+    m.load_state_dict(synthetic_state_dict(seed=326, **BENCH_WEIGHTS, **cfg), strict=True)
+    return m.to(device)
+
+
+def workload_call(workload, drop=()):
+    """A copy of the forward keywords of `WORKLOADS[workload]` without the keys named in `drop`."""
+    return {k: v for k, v in WORKLOADS[workload]["call"].items() if k not in drop}
 
 
 def _texture(g, h, w):
