@@ -134,6 +134,17 @@ int um_flow_warp(const float* f, const float* flow, float* out,
 int um_fb_consistency(const float* fwd_flow, const float* bwd_flow, float alpha, float beta, float* fwd_occ,
                       float* bwd_occ, int32_t batch, int32_t h, int32_t w, void* stream);
 
+/* um_fb_consistency plus the forward residual: fwd_occ and bwd_occ are bit-identical to um_fb_consistency's (the same
+ * kernel), and fwd_err [B,H,W] = | fwd + warp(bwd, fwd) |, the very fp32 value that the forward mask compares with
+ * alpha (|fwd| + |bwd|) + beta.  In fp32, with (u, v) = fwd[b,:,y,x] and s = size - 1 per axis: px = x + u,
+ * ix = ((2 px / s - 1) + 1) / 2 * s (likewise iy), x0 = floor(ix), the weights nw = (x0 + 1 - ix)(y0 + 1 - iy),
+ * ne = (ix - x0)(y0 + 1 - iy), sw = (x0 + 1 - ix)(iy - y0), se = (ix - x0)(iy - y0), and warp = fma(se, v11, fma(sw, v10,
+ * fma(ne, v01, nw v00))) over the corners inside the frame (zero padding); dx = u + warp.u, dy = v + warp.v,
+ * fwd_err = sqrt(fma(dx, dx, dy * dy)), every other operation correctly rounded on its own.  The uncertainty of the
+ * multi-flow tracks (um_multi_flow_tracks). */
+int um_fb_consistency_error(const float* fwd_flow, const float* bwd_flow, float alpha, float beta, float* fwd_occ,
+                            float* bwd_occ, float* fwd_err, int32_t batch, int32_t h, int32_t w, void* stream);
+
 /* out[b,y,x,:] = sum_{3x3 nb} softmax( q[b,y,x,:] . k[b,nb,:] / sqrt(128) ) flow[b,nb,:]; out-of-image
  * neighbours take part with logit 0 and value 0 (zero-padded unfold).
  * Replaces SelfAttnPropagation.forward_local_window_attn (attention.py:217-253). */
@@ -318,6 +329,35 @@ int um_track_points_forward(const float* flow, const float* occ, int32_t n, int3
                             uint8_t* visible, void* stream);
 int um_track_points_backward(const float* flow, const float* occ, int32_t n, int32_t h, int32_t w, const float* queries,
                              int32_t nq, int32_t nt, float* tracks, uint8_t* visible, void* stream);
+
+/* ---- multi-flow dense point tracks -----------------------------------------------------------------------------
+ * Every pixel of a first frame tracked through a clip, each new frame t reached from k candidate source frames (e.g.
+ * t-1, t-2, t-4, ... and frame 0: multi-flow tracking after MFT, Neoral, Serych and Matas, WACV 2024), keeping the most
+ * certain visible candidate, so a point occluded for a while comes back through a longer flow.  Coordinates are pixels
+ * (x, y) at the flows' size.  The state of every pixel p in frame s lives in one of r slots: pos [r, h, w, 2] (x, y),
+ * sig [r, h, w] (accumulated uncertainty sigma^2) and vis [r, h, w] (uint8, 1 = visible); the caller starts frame 0's slot
+ * at pos(y, x) = (x, y), sig = 0, vis = 1.
+ * Per frame t = 0..n-1 of the launch, in order, candidate j = 0..k-1 (c = t k + j) is pair c: F = flow[c] (planar
+ * [2, h, w], source -> frame), O = occ[c] (its fwd_occ, [h, w]) and E = err[c] (its fwd_err of um_fb_consistency_error),
+ * and src[t][j] the slot of its source frame's state; an entry outside [0, r) is absent and its pair is not read.
+ * From the source state (x_s, sigma2_s, v_s), with bilinear and its fp32 order of operations as for um_chain_tracks:
+ *   d = bilinear(F, x_s), o = bilinear(O, x_s), e = bilinear(E, x_s);  x = x_s + d;  sigma2 = sigma2_s + e * e;
+ *   valid = v_s && o < 0.5 && 0 <= x.x <= w-1 && 0 <= x.y <= h-1
+ * (each + and * rounded on its own, no FMA; x and v are exactly um_chain_tracks's step).  The frame takes the valid
+ * candidate of smallest sigma2, the first in j order on ties (a NaN never wins over an earlier candidate), visible; if no
+ * candidate is valid, the present candidate of smallest sigma2 under the same rule, invisible.  A frame without a present
+ * candidate is NaN, NaN, invisible.  The choice goes to tracks [n, h, w, 2], visible [n, h, w] and sigma [n, h, w], and
+ * into slot dst[t] (no state is written when dst[t] is outside [0, r)).
+ * src [n, k] and dst [n] are DEVICE int32 tables, read by the kernel, so a CUDA graph replay picks up whatever they hold.
+ * One thread per pixel walks the n frames in order, and pixel p of every slot is touched by that thread only: a later frame
+ * of the same launch may read the slot an earlier frame wrote, and then reads that frame's state.  Condition on the
+ * tables: dst[t] is no slot that a candidate of frame t' >= t reads for a frame other than t, i.e. a launch never
+ * overwrites a state one of its candidates still needs.  No host synchronisation (graph-capturable).  pos and tracks
+ * 8-byte aligned, the other buffers 4-byte aligned (vis and visible bytes); the six state and output buffers overlap
+ * nothing.  Frames of at least 2 x 2. */
+int um_multi_flow_tracks(const float* flow, const float* occ, const float* err, const int32_t* src, const int32_t* dst,
+                         int32_t n, int32_t k, int32_t h, int32_t w, int32_t r, float* pos, float* sig, uint8_t* vis,
+                         float* tracks, uint8_t* visible, float* sigma, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

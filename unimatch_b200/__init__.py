@@ -26,6 +26,9 @@ _LAZY = {
     "chain_tracks": (".inference", "chain_tracks"),
     "PointTrackRunner": (".inference", "PointTrackRunner"),
     "track_points": (".inference", "track_points"),
+    "MultiFlowTrackRunner": (".inference", "MultiFlowTrackRunner"),
+    "multi_flow_tracks": (".inference", "multi_flow_tracks"),
+    "multi_flow_sources": (".inference", "multi_flow_sources"),
     "flow_to_image": (".inference", "flow_to_image"),
     "infer_depth_sequence": (".inference", "infer_depth_sequence"),
     "DepthSequenceRunner": (".inference", "DepthSequenceRunner"),
@@ -48,7 +51,8 @@ _LAZY = {
 
 __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "InputPadder", "infer_flow", "infer_stereo",
            "infer_depth", "BatchedFlowRunner", "forward_backward_consistency_check", "infer_flow_video", "VideoFlowRunner",
-           "VideoTrackRunner", "chain_tracks", "PointTrackRunner", "track_points", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
+           "VideoTrackRunner", "chain_tracks", "PointTrackRunner", "track_points", "MultiFlowTrackRunner",
+           "multi_flow_tracks", "multi_flow_sources", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
            "MixedSizeStereoRunner", "MixedSizeFlowRunner", "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "tapvid_metrics", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth"]

@@ -45,6 +45,9 @@ int track_points_forward_launch(const float* flow, const float* occ, int n, int 
                                 int nq, int nt, float* pos, uint8_t* vis, float* tracks, uint8_t* visible, cudaStream_t st);
 int track_points_backward_launch(const float* flow, const float* occ, int n, int h, int w, const float* queries, int nq,
                                  int nt, float* tracks, uint8_t* visible, cudaStream_t st);
+int multi_flow_tracks_launch(const float* flow, const float* occ, const float* err, const int* src, const int* dst, int n,
+                             int k, int h, int w, int r, float* pos, float* sig, uint8_t* vis, float* tracks,
+                             uint8_t* visible, float* sigma, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -221,6 +224,28 @@ int um_track_points_backward(const float* flow, const float* occ, int32_t n, int
              "um_track_points_backward: the tables must not overlap each other or the inputs");
   return um::track_points_backward_launch(n > 0 ? flow : nullptr, n > 0 ? occ : nullptr, n, h, w, queries, nq, nt, tracks,
                                           visible, (cudaStream_t)stream);
+}
+
+int um_multi_flow_tracks(const float* flow, const float* occ, const float* err, const int32_t* src, const int32_t* dst,
+                         int32_t n, int32_t k, int32_t h, int32_t w, int32_t r, float* pos, float* sig, uint8_t* vis,
+                         float* tracks, uint8_t* visible, float* sigma, void* stream) {
+  UM_REQUIRE(flow && occ && err && src && dst && pos && sig && vis && tracks && visible && sigma,
+             "um_multi_flow_tracks: flows, masks, residuals, tables, state and outputs must not be NULL");
+  UM_REQUIRE(n > 0 && k > 0 && r > 0 && h > 1 && w > 1,
+             "um_multi_flow_tracks: bad shape (n >= 1 frames of k >= 1 candidates, r >= 1 slots, frames of at least 2 x 2)");
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL && (long long)n * k <= 0x7fffffffLL,
+             "um_multi_flow_tracks: a frame has at most 2^31 - 1 pixels, a launch at most 2^31 - 1 candidates");
+  UM_REQUIRE(um::aligned(flow, 4) && um::aligned(occ, 4) && um::aligned(err, 4) && um::aligned(src, 4) &&
+                 um::aligned(dst, 4) && um::aligned(pos, 8) && um::aligned(sig, 4) && um::aligned(tracks, 8) &&
+                 um::aligned(sigma, 4),
+             "um_multi_flow_tracks: pos and tracks must be 8-byte aligned, the other float and int32 buffers 4-byte aligned");
+  const long long hw = (long long)h * w, c = (long long)n * k * hw;
+  UM_REQUIRE(um::written_disjoint({{pos, 8 * r * hw}, {sig, 4 * r * hw}, {vis, r * hw}, {tracks, 8 * n * hw},
+                                   {visible, n * hw}, {sigma, 4 * n * hw}, {flow, 8 * c}, {occ, 4 * c}, {err, 4 * c},
+                                   {src, 4LL * n * k}, {dst, 4LL * n}}, 6),
+             "um_multi_flow_tracks: the state and outputs must not overlap each other or the inputs");
+  return um::multi_flow_tracks_launch(flow, occ, err, src, dst, n, k, h, w, r, pos, sig, vis, tracks, visible, sigma,
+                                      (cudaStream_t)stream);
 }
 
 }  // extern "C"

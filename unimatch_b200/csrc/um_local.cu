@@ -350,6 +350,7 @@ struct FbPixel {
   const float* bb;
   float* fwd_occ;
   float* bwd_occ;
+  float* fwd_err;
   int h, w, rem;
 };
 
@@ -358,6 +359,7 @@ struct FbUniform {
   const float* bwd;
   float* fwd_occ;
   float* bwd_occ;
+  float* fwd_err;                       // read only by the kErr instantiation
   int h, w;
   long long npix;
   __device__ __forceinline__ bool pixel(FbPixel& p) const {
@@ -370,6 +372,7 @@ struct FbUniform {
     p.bb = bwd + (long long)b * 2 * plane;
     p.fwd_occ = fwd_occ + (long long)b * plane;
     p.bwd_occ = bwd_occ + (long long)b * plane;
+    p.fwd_err = fwd_err + (long long)b * plane;
     p.h = h; p.w = w;
     return true;
   }
@@ -403,7 +406,8 @@ struct FbRagged {
   }
 };
 
-template <class Geo>
+// kErr: also store the forward residual |fwd + warp(bwd, fwd)| that the forward mask compares (um_fb_consistency_error).
+template <class Geo, bool kErr = false>
 __global__ void __launch_bounds__(256) fb_consistency_kernel(Geo geo, float alpha, float beta) {
   FbPixel p;
   if (!geo.pixel(p)) return;
@@ -419,8 +423,10 @@ __global__ void __launch_bounds__(256) fb_consistency_kernel(Geo geo, float alph
   const float2 wf = sample_flow(fb, plane, h, w, (float)x + bu, (float)y + bv);   // flow_warp(fwd, bwd)
   const float dfx = fu + wb.x, dfy = fv + wb.y, dbx = bu + wf.x, dby = bv + wf.y;
   const float thr = alpha * mag + beta;
-  p.fwd_occ[rem] = sqrtf(dfx * dfx + dfy * dfy) > thr ? 1.0f : 0.0f;
+  const float ef = sqrtf(dfx * dfx + dfy * dfy);
+  p.fwd_occ[rem] = ef > thr ? 1.0f : 0.0f;
   p.bwd_occ[rem] = sqrtf(dbx * dbx + dby * dby) > thr ? 1.0f : 0.0f;
+  if constexpr (kErr) p.fwd_err[rem] = ef;
 }
 
 }  // namespace
@@ -440,9 +446,19 @@ int um_fb_consistency(const float* fwd_flow, const float* bwd_flow, float alpha,
                       float* bwd_occ, int32_t batch, int32_t h, int32_t w, void* stream) {
   UM_REQUIRE(fwd_flow && bwd_flow && fwd_occ && bwd_occ && batch > 0 && h > 1 && w > 1, "um_fb_consistency: bad arguments");
   const long long npix = (long long)batch * h * w;
-  const FbUniform geo{fwd_flow, bwd_flow, fwd_occ, bwd_occ, h, w, npix};
+  const FbUniform geo{fwd_flow, bwd_flow, fwd_occ, bwd_occ, nullptr, h, w, npix};
   fb_consistency_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, alpha, beta);
   return um::check_launch("um_fb_consistency");
+}
+
+int um_fb_consistency_error(const float* fwd_flow, const float* bwd_flow, float alpha, float beta, float* fwd_occ,
+                            float* bwd_occ, float* fwd_err, int32_t batch, int32_t h, int32_t w, void* stream) {
+  UM_REQUIRE(fwd_flow && bwd_flow && fwd_occ && bwd_occ && fwd_err && batch > 0 && h > 1 && w > 1,
+             "um_fb_consistency_error: bad arguments");
+  const long long npix = (long long)batch * h * w;
+  const FbUniform geo{fwd_flow, bwd_flow, fwd_occ, bwd_occ, fwd_err, h, w, npix};
+  fb_consistency_kernel<FbUniform, true><<<(unsigned)((npix + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, alpha, beta);
+  return um::check_launch("um_fb_consistency_error");
 }
 
 int um_fb_consistency_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, float alpha, float beta,

@@ -1,8 +1,10 @@
 // Point tracks chained through the flows of consecutive pairs.  Dense: the forward flows from every pixel of a first frame,
 // with the forward occlusion masks deciding visibility (um_chain_tracks).  Sparse: query points, each given at its own
 // frame, chained forward through the forward flows and backward through the backward flows (um_track_points_forward /
-// um_track_points_backward).  Semantics and the fp32 order of operations: include/unimatch_sm100.h; the float64
-// statements are tests/refops_tracks.py and tests/refops_points.py.
+// um_track_points_backward).  Multi-flow: every pixel of a first frame, each new frame reached from several earlier
+// frames, keeping the most certain visible candidate (um_multi_flow_tracks).  Semantics and the fp32 order of operations:
+// include/unimatch_sm100.h; the float64 statements are tests/refops_tracks.py, tests/refops_points.py and
+// tests/refops_multiflow.py.
 #include "um_common.cuh"
 
 namespace {
@@ -137,6 +139,60 @@ track_points_backward_kernel(const float* __restrict__ flow, const float* __rest
   }
 }
 
+// One thread owns pixel `pix` of the first frame and walks the launch's n frames in order.  Frame t's candidates extend the
+// states in slots src[t][j] by the flow, mask and residual of pair (t, j); the choice goes to slot dst[t] and to the
+// outputs.  Only this thread touches pixel `pix` of any slot, so a later frame may read a slot an earlier one wrote.
+__global__ void __launch_bounds__(TRACK_THREADS)
+multi_flow_tracks_kernel(const float* __restrict__ flow, const float* __restrict__ occ, const float* __restrict__ err,
+                         const int* __restrict__ src, const int* __restrict__ dst, int n, int k, int h, int w, int r,
+                         float2* pos, float* sig, uint8_t* vis, float2* __restrict__ tracks,
+                         uint8_t* __restrict__ visible, float* __restrict__ sigma) {
+  const long long plane = (long long)h * w;
+  const long long pix = (long long)blockIdx.x * TRACK_THREADS + threadIdx.x;
+  if (pix >= plane) return;
+  const float nan = __int_as_float(0x7fffffff);
+  for (int t = 0; t < n; ++t) {
+    bool any = false, any_valid = false;
+    float2 bp = make_float2(nan, nan), vp = bp;
+    float bs = nan, vs = nan;
+    for (int j = 0; j < k; ++j) {
+      const int s = __ldg(src + t * k + j);
+      if (s < 0 || s >= r) continue;
+      const long long at = (long long)s * plane + pix, c = (long long)t * k + j;
+      float2 p = pos[at];
+      float s2 = sig[at];
+      bool v = vis[at] != 0;
+      float e = 0.f;                                 // the residual at the source position, sampled as track_step samples
+      if (p.x > -1.f && p.x < (float)w && p.y > -1.f && p.y < (float)h)
+        e = lerp2(err + c * plane, w, axis_taps(p.x, w), axis_taps(p.y, h));
+      track_step(p, v, flow + c * 2 * plane, occ + c * plane, h, w);
+      s2 = __fadd_rn(s2, __fmul_rn(e, e));
+      if (v && (!any_valid || s2 < vs)) {
+        any_valid = true;
+        vp = p;
+        vs = s2;
+      }
+      if (!any || s2 < bs) {
+        any = true;
+        bp = p;
+        bs = s2;
+      }
+    }
+    const float2 p = any_valid ? vp : bp;
+    const float s2 = any_valid ? vs : bs;
+    const int d = __ldg(dst + t);
+    if (d >= 0 && d < r) {
+      const long long at = (long long)d * plane + pix;
+      pos[at] = p;
+      sig[at] = s2;
+      vis[at] = any_valid ? 1 : 0;
+    }
+    tracks[(long long)t * plane + pix] = p;
+    sigma[(long long)t * plane + pix] = s2;
+    visible[(long long)t * plane + pix] = any_valid ? 1 : 0;
+  }
+}
+
 }  // namespace
 
 namespace um {
@@ -157,6 +213,17 @@ int track_points_forward_launch(const float* flow, const float* occ, int n, int 
       flow, occ, n, h, w, t0, queries, nq, nt, reinterpret_cast<float2*>(pos), vis, reinterpret_cast<float2*>(tracks),
       visible);
   return check_launch("um_track_points_forward");
+}
+
+// Arguments are checked by um_multi_flow_tracks (um_api.cu).
+int multi_flow_tracks_launch(const float* flow, const float* occ, const float* err, const int* src, const int* dst, int n,
+                             int k, int h, int w, int r, float* pos, float* sig, uint8_t* vis, float* tracks,
+                             uint8_t* visible, float* sigma, cudaStream_t st) {
+  const long long hw = (long long)h * w;
+  multi_flow_tracks_kernel<<<(unsigned)((hw + TRACK_THREADS - 1) / TRACK_THREADS), TRACK_THREADS, 0, st>>>(
+      flow, occ, err, src, dst, n, k, h, w, r, reinterpret_cast<float2*>(pos), sig, vis,
+      reinterpret_cast<float2*>(tracks), visible, sigma);
+  return check_launch("um_multi_flow_tracks");
 }
 
 int track_points_backward_launch(const float* flow, const float* occ, int n, int h, int w, const float* queries, int nq,

@@ -24,7 +24,10 @@ forward occlusion masks as visibility (`um_chain_tracks`), and `VideoTrackRunner
 `VideoFlowRunner` step, so only the tracks are downloaded.  Query point tracks (TAP-Vid's question: N points, each given
 at its own frame, tracked forward and backward in time through every frame of the clip): `track_points` for device flows a
 caller holds, and `PointTrackRunner`, which chains them next to the `VideoFlowRunner` step and downloads only the tables
-(`um_track_points_forward` / `um_track_points_backward`).
+(`um_track_points_forward` / `um_track_points_backward`).  Multi-flow dense tracks (each new frame matched against several
+earlier frames and the first, keeping the most certain visible candidate, so tracks come back after an occlusion):
+`multi_flow_tracks` for device flows a caller holds and `MultiFlowTrackRunner`, which encodes each frame once and gathers
+the source pyramids from a device ring (`um_fb_consistency_error`, `um_multi_flow_tracks`).
 
 Posed sequences (`inference_depth`, evaluate_depth.py:297-419): `infer_depth_sequence` runs the consecutive pairs of a frame
 sequence with absolute camera poses, every frame encoded once and the relative poses computed on the host as the reference
@@ -56,6 +59,7 @@ from the descriptor table.
 import collections
 import itertools
 import math
+import operator
 
 import numpy as np
 import torch
@@ -1497,6 +1501,195 @@ class PointTrackRunner(VideoFlowRunner):
         if self.return_flow:
             res.update({k: torch.stack([r[k] for r in per_pair]) for k in ("flow", "flow_bwd", "fwd_occ", "bwd_occ")})
         return res
+
+
+MULTI_FLOW_GAPS = (1, 2, 4, 8, 16, 32)
+
+
+def _multi_flow_gaps(gaps, anchor, name):
+    """(the gaps in increasing order, anchor), refused unless the gaps are distinct positive integers and some source
+    exists"""
+    try:
+        g = sorted(operator.index(x) for x in gaps)
+    except TypeError:
+        raise ValueError("%s: gaps must be integers, got %r" % (name, gaps)) from None
+    if any(x < 1 for x in g) or len(set(g)) != len(g):
+        raise ValueError("%s: gaps must be distinct positive integers, got %r" % (name, tuple(gaps)))
+    if not g and not anchor:
+        raise ValueError("%s: no source at all: give gaps or anchor=True" % name)
+    return tuple(g), bool(anchor)
+
+
+def multi_flow_sources(t, gaps=MULTI_FLOW_GAPS, anchor=True):
+    """The candidate source frames of frame t >= 1 of a multi-flow track, in candidate-slot order: frame t-g for each g in
+    `gaps` in increasing order (-1, absent, where t-g < 0), then frame 0 when `anchor`.  len(gaps) + anchor slots; frame 0
+    may appear twice (as gap t and as the anchor).  A frame without any present source is refused."""
+    gaps, anchor = _multi_flow_gaps(gaps, anchor, "multi_flow_sources")
+    t = operator.index(t)
+    if t < 1:
+        raise ValueError("multi_flow_sources: frame %d has no sources (frames t >= 1 have)" % t)
+    src = [t - g if t >= g else -1 for g in gaps] + ([0] if anchor else [])
+    if max(src) < 0:
+        raise ValueError("multi_flow_sources: frame %d has no source with gaps %r and anchor=False" % (t, gaps))
+    return src
+
+
+def _multi_flow_state(slots, h, w, device):
+    """The state ring (pos [R,H,W,2], sigma^2 [R,H,W], vis [R,H,W] uint8) with frame 0 in slot 0: every pixel at itself,
+    certain and visible"""
+    pos = torch.empty((slots, h, w, 2), device=device)
+    sig = torch.empty((slots, h, w), device=device)
+    vis = torch.empty((slots, h, w), device=device, dtype=torch.uint8)
+    pos[0], _ = _track_start(h, w, device)
+    sig[0] = 0
+    vis[0] = 1
+    return pos, sig, vis
+
+
+@torch.no_grad()
+def multi_flow_tracks(flows, flows_bwd, gaps=MULTI_FLOW_GAPS, anchor=True):
+    """Multi-flow dense point tracks through device flows a caller already holds: every pixel of frame 0, each frame t >= 1
+    reached from its sources (`multi_flow_sources(t, gaps, anchor)`: frames t-g and, with `anchor`, frame 0), keeping the
+    most certain candidate that is not occluded, so a point comes back after an occlusion (multi-flow tracking after MFT,
+    Neoral, Serych and Matas, WACV 2024).
+
+    `flows` / `flows_bwd`: planar [T-1,K,2,H,W], K = len(gaps) + anchor; entry (t-1, k) is the forward flow of pair
+    (source k of t, t) and its backward flow, in pixels at the frames' size (e.g. `infer_flow(..., pred_bidir_flow=True)` on
+    those pairs).  Entries of absent sources do not affect the result.  Per pair, O = `fwd_occ` of
+    `forward_backward_consistency_check` and E the forward residual that mask thresholds (`um_fb_consistency_error`).  From
+    source s's state (x_s, sigma2_s, v_s), with `chain_tracks`'s bilinear sampling: x = x_s + F(x_s), sigma2 = sigma2_s +
+    E(x_s)^2, valid = v_s and O(x_s) < 0.5 and x inside the frame.  Frame t takes the valid candidate of smallest sigma2
+    (the first on ties) and is visible; with none valid, the smallest sigma2 of all, invisible.  Frame 0: x = p,
+    sigma2 = 0, visible.  fp32 in the order of operations of include/unimatch_sm100.h.  One `um_fb_consistency_error`
+    call, one `um_multi_flow_tracks` launch, and a state of 13 x T x H x W bytes for the call.
+    Returns {'tracks': [T-1,H,W,2] fp32 (x, y), 'visible': [T-1,H,W] uint8, 'uncertainty': [T-1,H,W] fp32 sigma^2} for
+    frames 1 .. T-1."""
+    gaps, anchor = _multi_flow_gaps(gaps, anchor, "multi_flow_tracks")
+    k = len(gaps) + anchor
+    if flows.dim() != 5 or flows.shape[0] < 1 or flows.shape[1] != k or flows.shape[2] != 2:
+        raise ValueError("multi_flow_tracks expects planar flows [T-1,%d,2,H,W] (K = len(gaps) + anchor), got %s"
+                         % (k, tuple(flows.shape)))
+    if tuple(flows_bwd.shape) != tuple(flows.shape):
+        raise ValueError("multi_flow_tracks: flows_bwd must be [T-1,K,2,H,W] like the flows")
+    n, _, _, h, w = flows.shape
+    dev = flows.device
+    src = torch.tensor([multi_flow_sources(t, gaps, anchor) for t in range(1, n + 1)], dtype=torch.int32).to(dev)
+    dst = torch.arange(1, n + 1, dtype=torch.int32, device=dev)
+    fwd = flows.float().reshape(n * k, 2, h, w).contiguous()
+    occ, _, err = _OPS.fb_consistency_error(fwd, flows_bwd.float().reshape(n * k, 2, h, w).contiguous(), 0.01, 0.5)
+    pos, sig, vis = _multi_flow_state(n + 1, h, w, dev)
+    tracks, visible, sigma = _OPS.multi_flow_tracks(fwd.view(n, k, 2, h, w), occ.view(n, k, h, w), err.view(n, k, h, w),
+                                                    src, dst, pos, sig, vis)
+    return {"tracks": tracks, "visible": visible, "uncertainty": sigma}
+
+
+def _ring_slot(frame, slots):
+    """Slot of a frame in a ring of `slots`: frame 0 keeps slot 0, frames t >= 1 cycle through the others"""
+    return 0 if frame == 0 else 1 + (frame - 1) % (slots - 1)
+
+
+class MultiFlowTrackRunner(_SequenceRunner):
+    """Multi-flow dense point tracks over a video (semantics: `multi_flow_tracks`): where each pixel of the first frame of a
+    `run()` is in every later frame, whether it is visible, and how uncertain the estimate is.  Each new frame t is
+    matched against its K = len(gaps) + anchor sources (`multi_flow_sources`: t-1, t-2, t-4, ... and frame 0), so a point
+    hidden for a while comes back through a longer flow, and a track is a few links long however far the clip goes.
+
+    A step takes `batch` new frames, uploaded and encoded once, and runs batch x K pairs (2 x batch x K flows with
+    `pred_bidir_flow`), all inside one CUDA graph per staging slot:
+    * the new frames' pyramids go into a device feature ring; the first frame's pyramid has slot 0, never overwritten;
+    * the K source pyramids of every new frame are gathered from the ring with `index_select` on a small device table,
+      staged with the frames, so one graph serves every step; absent sources of a clip's first frames are filled with a
+      present pair and marked absent in the table;
+    * `forward_encoded(..., pred_bidir_flow=True)` on the pairs, resized back to the frames' size as `infer_flow` does,
+      then `um_fb_consistency_error` (masks and forward residuals) and one `um_multi_flow_tracks` launch over the step's
+      frames, whose states live in a device ring.
+    A short last step is filled with repeats of its last frame; they write no state and their results are dropped.
+    Memory held for the life of the runner: the feature ring of max(gaps) + batch + 1 pyramids (encode_frames' [h,w,128]
+    fp32 per scale: about 16 MB each for gmflow-scale2 at 480x832), and a state ring of as many slots, 13 bytes per pixel
+    each; plus the activations of a forward over batch x K pairs.
+    `run(frames)` resets the state and yields, per frame t >= 1 (frame 0 is not yielded), 'tracks' fp32 [H,W,2] (x, y),
+    'visible' uint8 [H,W] and 'uncertainty' fp32 [H,W] (sigma^2): 13 bytes per pixel.  `return_flow=True` adds the frame's
+    'flow' / 'flow_bwd' [K,2,H,W] and 'sources' [K] (frame indices, -1 absent).  `pred_bwd_flow`, `visualize`,
+    `concat_frame` and `visualize_bwd` are refused."""
+
+    task = "flow"
+
+    def __init__(self, model, frame_size, batch, device, gaps=MULTI_FLOW_GAPS, anchor=True, padding_factor=32,
+                 inference_size=None, use_graph=True, return_flow=False, **model_kwargs):
+        name = type(self).__name__
+        _track_flags(model_kwargs, name, "the tracks run forward from the first frame")
+        self.kw = _task_kwargs(model_kwargs, "flow", name)
+        self.gaps, self.anchor = _multi_flow_gaps(gaps, anchor, name)
+        self.k = len(self.gaps) + self.anchor
+        self._init_sequence(model, frame_size, batch, device, use_graph, padding_factor, inference_size)
+        self.return_flow = bool(return_flow)
+        self.slots = max(self.gaps, default=0) + self.batch + 1
+        with torch.cuda.device(self.dev):
+            probe = self._encode(torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev))
+        self.ring = [torch.empty((self.slots,) + tuple(f.shape[1:]), device=self.dev, dtype=f.dtype) for f in probe]
+        self.carry = [r[:1] for r in self.ring]            # _prime encodes the first frame into slot 0
+        self.pos, self.sig, self.vis = _multi_flow_state(self.slots, self.h, self.w, self.dev)
+        # per new frame: K feature slots to gather, K state slots (-1 absent), K source frames (-1 absent), the feature
+        # slot it is written to and its state slot (-1: a repeat, no state)
+        cols = 3 * self.k + 2
+        self.tab_pin = [torch.empty((self.batch, cols), dtype=torch.int64).pin_memory() for _ in range(2)]
+        self.tab_dev = [torch.empty((self.batch, cols), dtype=torch.int64, device=self.dev) for _ in range(2)]
+        self._next = 1
+
+    def _begin(self, first):
+        self._next = 1
+
+    def _prime(self, frame):
+        super()._prime(frame)
+        self.pos[0], _ = _track_start(self.h, self.w, self.dev)
+        self.sig[0] = 0
+        self.vis[0] = 1
+
+    def _step(self, slot):
+        b, k, h, w = self.batch, self.k, self.h, self.w
+        tab = self.tab_dev[slot]
+        new = self._encode(self.dev_in[slot])
+        for r, f in zip(self.ring, new):
+            r.index_copy_(0, tab[:, 3 * k], f)
+        gather = tab[:, :k].reshape(-1)
+        first = [r.index_select(0, gather) for r in self.ring]
+        second = [f[:, None].expand((b, k) + tuple(f.shape[1:])).reshape((b * k,) + tuple(f.shape[1:])) for f in new]
+        flow = self.model.forward_encoded(first, second, pred_bidir_flow=True, **self.kw)["flow_preds"][-1]
+        out = _flow_outputs(flow, self.ori, self.size, self.transposed, True, False)
+        fwd, bwd = out["flow"].contiguous(), out["flow_bwd"].contiguous()
+        occ, _, err = _OPS.fb_consistency_error(fwd, bwd, 0.01, 0.5)
+        src = tab[:, k:2 * k].to(torch.int32).contiguous()
+        dst = tab[:, 3 * k + 1].to(torch.int32).contiguous()
+        tracks, visible, sigma = _OPS.multi_flow_tracks(fwd.view(b, k, 2, h, w), occ.view(b, k, h, w),
+                                                        err.view(b, k, h, w), src, dst, self.pos, self.sig, self.vis)
+        res = {"tracks": tracks, "visible": visible, "uncertainty": sigma}
+        if self.return_flow:
+            res.update(flow=fwd.view(b, k, 2, h, w), flow_bwd=bwd.view(b, k, 2, h, w), sources=tab[:, 2 * k:3 * k])
+        return res
+
+    def _reset_inputs(self, slot):
+        super()._reset_inputs(slot)
+        k = self.k
+        t = self.tab_dev[slot]
+        t[:, :k] = 0
+        t[:, k:3 * k] = -1
+        t[:, 3 * k] = torch.arange(1, self.batch + 1, device=self.dev)
+        t[:, 3 * k + 1] = -1
+
+    def _stage_host(self, slot, chunk):
+        items = super()._stage_host(slot, chunk)
+        k, m, tab = self.k, len(chunk), self.tab_pin[slot]
+        for i in range(self.batch):
+            t = self._next + min(i, m - 1)
+            src = multi_flow_sources(t, self.gaps, self.anchor)
+            fill = next(s for s in src if s >= 0)
+            row = [_ring_slot(s if s >= 0 else fill, self.slots) for s in src]
+            row += [_ring_slot(s, self.slots) if s >= 0 else -1 for s in src] + src
+            row += [_ring_slot(t, self.slots), _ring_slot(t, self.slots) if i < m else -1]
+            tab[i] = torch.tensor(row, dtype=torch.int64)
+        self.tab_dev[slot].copy_(tab, non_blocking=True)
+        self._next += m
+        return items
 
 
 class _PosedDepth:

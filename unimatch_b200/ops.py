@@ -102,9 +102,11 @@ _SIGNATURES = {
     "um_flow_warp": (_RC, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "um_fb_consistency": (_RC, [_P, _P, _F, _F, _P, _P, _I, _I, _I, _P]),
     "um_fb_consistency_ragged": (_RC, [_P, _L, _P, _F, _F, _P, _L, _P, _I, _I, _I, _P]),
+    "um_fb_consistency_error": (_RC, [_P, _P, _F, _F, _P, _P, _P, _I, _I, _I, _P]),
     "um_chain_tracks": (_RC, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _P]),
     "um_track_points_forward": (_RC, [_P, _P, _I, _I, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P]),
     "um_track_points_backward": (_RC, [_P, _P, _I, _I, _I, _P, _I, _I, _P, _P, _P]),
+    "um_multi_flow_tracks": (_RC, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -338,6 +340,24 @@ fb_consistency = _define("fb_consistency(Tensor fwd_flow, Tensor bwd_flow, float
                          _fb_consistency)
 
 
+def _fb_consistency_error(fwd_flow, bwd_flow, alpha, beta):
+    """fb_consistency's masks plus the forward residual [B,H,W] they compare (include/unimatch_sm100.h,
+    um_fb_consistency_error)"""
+    _f32c(fwd_flow, "fwd_flow"), _f32c(bwd_flow, "bwd_flow")
+    if fwd_flow.dim() != 4 or fwd_flow.shape[1] != 2 or fwd_flow.shape != bwd_flow.shape:
+        raise ValueError("fb_consistency_error: flows must be planar [B,2,H,W] of equal shape")
+    b, _, h, w = fwd_flow.shape
+    fwd_occ = torch.empty((b, h, w), device=fwd_flow.device, dtype=torch.float32)
+    bwd_occ, fwd_err = torch.empty_like(fwd_occ), torch.empty_like(fwd_occ)
+    _check(LIB.um_fb_consistency_error(_p(fwd_flow), _p(bwd_flow), float(alpha), float(beta), _p(fwd_occ), _p(bwd_occ),
+                                       _p(fwd_err), b, h, w, _stream()), "um_fb_consistency_error")
+    return fwd_occ, bwd_occ, fwd_err
+
+
+fb_consistency_error = _define("fb_consistency_error(Tensor fwd_flow, Tensor bwd_flow, float alpha, float beta) -> "
+                               "(Tensor, Tensor, Tensor)", _fb_consistency_error)
+
+
 def _chain_tracks(flow, occ, pos, vis):
     """flow: contiguous fp32 [n, 2, h, w]; occ: contiguous fp32 [n, h, w] or None (nothing occluded); pos / vis: the running
     state, contiguous fp32 [h, w, 2] and uint8 [h, w], advanced in place.  Returns the state after each flow, [n, h, w, 2]
@@ -421,6 +441,42 @@ def _track_points_backward(flow, occ, queries, tracks, visible):
 
 track_points_backward = _define("track_points_backward(Tensor flow, Tensor? occ, Tensor queries, Tensor(a!) tracks, "
                                 "Tensor(b!) visible) -> ()", _track_points_backward)
+
+
+def _multi_flow_tracks(flow, occ, err, src, dst, pos, sig, vis):
+    """flow: contiguous fp32 [n, k, 2, h, w], candidate (t, j)'s pair; occ / err: its forward mask and residual, contiguous
+    fp32 [n, k, h, w]; src: device int32 [n, k], the state slot of each candidate's source (-1 absent); dst: device int32
+    [n], each frame's slot; pos / sig / vis: the state ring, contiguous fp32 [r, h, w, 2], fp32 [r, h, w] and uint8
+    [r, h, w], updated in place.  Returns tracks [n, h, w, 2], visible [n, h, w] and sigma^2 [n, h, w]
+    (include/unimatch_sm100.h, um_multi_flow_tracks)."""
+    _f32c(flow, "flow"), _f32c(occ, "occ"), _f32c(err, "err"), _f32c(pos, "pos"), _f32c(sig, "sig")
+    if flow.dim() != 5 or flow.shape[2] != 2:
+        raise RuntimeError("multi_flow_tracks: expected planar flows [n, k, 2, h, w]")
+    n, k, _, h, w = flow.shape
+    dev = flow.device
+    for name, t in (("occ", occ), ("err", err)):
+        if tuple(t.shape) != (n, k, h, w) or t.device != dev:
+            raise RuntimeError("multi_flow_tracks: %s must be [n, k, h, w] on the flows' device" % name)
+    for name, t, shape in (("src", src, (n, k)), ("dst", dst, (n,))):
+        if t.dtype != torch.int32 or tuple(t.shape) != shape or not t.is_contiguous() or t.device != dev:
+            raise RuntimeError("multi_flow_tracks: %s must be contiguous int32 %s on the flows' device" % (name, list(shape)))
+    r = pos.shape[0] if pos.dim() == 4 else -1
+    if tuple(pos.shape) != (r, h, w, 2) or pos.device != dev:
+        raise RuntimeError("multi_flow_tracks: pos must be [r, h, w, 2] on the flows' device")
+    if tuple(sig.shape) != (r, h, w) or sig.device != dev:
+        raise RuntimeError("multi_flow_tracks: sig must be [r, h, w] like pos")
+    if vis.dtype != torch.uint8 or tuple(vis.shape) != (r, h, w) or not vis.is_contiguous() or vis.device != dev:
+        raise RuntimeError("multi_flow_tracks: vis must be contiguous uint8 [r, h, w] like pos")
+    tracks = torch.empty((n, h, w, 2), device=dev, dtype=torch.float32)
+    visible = torch.empty((n, h, w), device=dev, dtype=torch.uint8)
+    sigma = torch.empty((n, h, w), device=dev, dtype=torch.float32)
+    _check(LIB.um_multi_flow_tracks(_p(flow), _p(occ), _p(err), _p(src), _p(dst), n, k, h, w, r, _p(pos), _p(sig), _p(vis),
+                                    _p(tracks), _p(visible), _p(sigma), _stream()), "um_multi_flow_tracks")
+    return tracks, visible, sigma
+
+
+multi_flow_tracks = _define("multi_flow_tracks(Tensor flow, Tensor occ, Tensor err, Tensor src, Tensor dst, Tensor(a!) pos, "
+                            "Tensor(b!) sig, Tensor(c!) vis) -> (Tensor, Tensor, Tensor)", _multi_flow_tracks)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
