@@ -88,17 +88,30 @@ def act_bound(y, e, name):
 
 
 def layernorm64(y, e, gamma, beta, res=None):
-    """LayerNorm over the last dim (128) of y with per-element input bound e -> (out, bound)."""
+    """LayerNorm over the last dim (n = 128) of y with per-element input bound e -> (out, bound).
+
+    The kernels take two-pass fp32 statistics: mean = fl(sum y) / n, then var = fl(sum (y - mean)^2) / n, then
+    out = (y - mean) * rsqrt(var + eps) * gamma + beta (+ residual).
+      * The fp32 sum of n terms, in any order, is off by at most (n - 1) u sum |y| (u = 2^-24), and / n is exact, so the
+        mean carries an absolute error dm <= n u mean|y| besides the input's em.  Every centred value moves by the same dm,
+        so the output moves by |gamma| rstd dm -- independently of |d|: a channel that sits exactly on the mean (a
+        constant row, the zero padding rows) still sees it.
+      * That shift changes the centred sum of squares by n dm^2 (the cross term sums to 0), i.e. rstd by at most
+        (dm rstd)^2 relative; the fp32 sum of squares adds n u relative, rsqrt and the products 2^-21.
+    Exact input (e = 0, a constant row of a value whose multiples up to n are exact in fp32) makes dm's actual value 0,
+    so the output is beta (+ residual) bit for bit."""
     g, b = gamma.double(), beta.double()
+    n = y.shape[-1]
     mean = y.mean(-1, keepdim=True)
     d = y - mean
     var = (d * d).mean(-1, keepdim=True)
     rstd = 1.0 / torch.sqrt(var + EPS_LN)
     out = d * rstd * g + b
     em = e.mean(-1, keepdim=True)
+    dm = n * U32 * y.abs().mean(-1, keepdim=True)
     rho = ((d.abs() * (e + em)).sum(-1, keepdim=True) / (d * d + EPS_LN).sum(-1, keepdim=True) + 2.0 ** -21 +
-           y.shape[-1] * U32 * (1 + mean.abs() * rstd))
-    bound = g.abs() * rstd * (e + em) + g.abs() * d.abs() * rstd * rho + 4 * U32 * (g.abs() * d.abs() * rstd + b.abs())
+           n * U32 + (dm * rstd) ** 2)
+    bound = g.abs() * rstd * (e + em + dm) + g.abs() * d.abs() * rstd * rho + 4 * U32 * (g.abs() * d.abs() * rstd + b.abs())
     if res is not None:
         out = out + res.double()
         bound = bound + U32 * out.abs()

