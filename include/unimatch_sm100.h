@@ -363,7 +363,7 @@ int um_multi_flow_tracks(const float* flow, const float* occ, const float* err, 
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the
  * maximum radius is a float32 reduction, the rest float64, as numpy evaluates the reference; zero flow is white.
- * max_scratch: DEVICE buffer of n floats (receives the per-image maximum radius).
+ * max_scratch: DEVICE buffer of n floats (receives the per-image maximum radius).  n <= 65535.
  * Replaces flow_to_image (utils/flow_viz.py:240-275; called at evaluate_flow.py:768 for videos). */
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
                      int32_t n, int32_t h, int32_t w, void* stream);
@@ -374,6 +374,7 @@ int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_
  * operation, truncated; the pixel is cv2's COLORMAP_INFERNO table at g.  A NaN normalised value gives g = 0, so a constant
  * image, a NaN anywhere in the image or +-inf in it paints the whole image INFERNO[0].
  * minmax_scratch: DEVICE buffer of 2n words (the per-image min / max keys; reset inside the call, graph-capturable).
+ * n <= 65535.
  * Replaces vis_disparity (utils/visualization.py:11-16), called on every predicted disparity by inference_stereo
  * (evaluate_stereo.py:820-841). */
 int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,
@@ -388,6 +389,7 @@ int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, i
  * black for a NaN t.  vmax <= vmin gives index 0 everywhere; a NaN in the image, or a NaN vmax, paints it all black.
  * scratch: DEVICE buffer of 2056 * n 32-bit words (per image four 512-bin radix-select histograms and the selection
  * state; reset inside the call).  One memset and nine kernels whatever the data, no host synchronisation: graph-capturable.
+ * n <= 65535.
  * Replaces viz_depth_tensor (utils/visualization.py:92-107), called on every predicted depth (and the backward one with
  * pred_bidir_depth) by inference_depth (evaluate_depth.py:403-417). */
 int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,

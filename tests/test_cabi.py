@@ -110,3 +110,12 @@ def test_conv7x7_validation_without_a_gpu():
                                       one, 64, None, 0, None)
         assert rc == -22, change
         assert b"um_conv7x7_small" in ops.LIB.um_last_error()
+
+
+def test_colouring_batches_over_65535_images_are_refused_without_a_gpu():
+    """The colouring kernels put the image on grid y (at most 65535 CTAs): a larger uniform batch is refused up front."""
+    one = ctypes.c_void_p(1024)
+    for name in ("um_flow_to_image", "um_disparity_to_image", "um_depth_to_image"):
+        rc = getattr(ops.LIB, name)(one, one, 12, 48, one, 65536, 4, 4, None)      # 4 x 4 pictures, 12-byte rows
+        assert rc == -22, name
+        assert name.encode() in ops.LIB.um_last_error()

@@ -60,6 +60,29 @@ inline int device_sm_count() {
   return sms[d];
 }
 
+// The per-image driver kernels put the image on grid y, which holds at most 65535 CTAs.  A batch of n images is launched
+// in chunks of at most that many: launch(first, count) launches images first .. first + count - 1, and each launch is
+// checked.  Every batch the drivers run is one chunk.
+constexpr long long kMaxGridY = 65535;
+template <class Launch>
+inline int launch_image_chunks(long long n, const char* what, Launch launch) {
+  for (long long first = 0; first < n; first += kMaxGridY) {
+    launch(first, (unsigned)(n - first < kMaxGridY ? n - first : kMaxGridY));
+    if (int rc = check_launch(what)) return rc;
+  }
+  return UM_OK;
+}
+
+// Runs body() in both arms of `if (ragged)`.  A driver kernel reads an image's geometry from a table or derives it from a
+// uniform shape; inlined into each arm, its body is compiled with the layout known, so the one instantiation holds a
+// uniform and a ragged version, and a thread outside its ragged image leaves without running the uniform version's
+// index arithmetic first (most CTAs of a grid sized by the capacity have no pixel).
+template <class Body>
+__device__ __forceinline__ void by_layout(bool ragged, Body body) {
+  if (ragged) body();
+  else body();
+}
+
 #define UM_REQUIRE(cond, ...)             \
   do {                                    \
     if (!(cond)) {                        \

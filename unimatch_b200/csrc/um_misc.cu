@@ -1,5 +1,7 @@
 // Small fused glue kernels on the matching path: position add, convex upsampling, x2 bilinear flow upsampling.
 // All channel-last, all bandwidth-bound, all vectorised (float4).
+#include <algorithm>
+
 #include "um_common.cuh"
 
 namespace {
@@ -110,180 +112,141 @@ __device__ __forceinline__ float bilinear_align_corners(const Load& load, int hi
 
 using um::ragged_ok;
 
-// One output sample of a planar resize: source plane (hi, wi), destination plane (ho, wo), scale and flip; `transpose`:
-// the destination plane is stored transposed, as [wo, ho].
-struct ResizeSample {
-  const float* src;
+// One destination image of a planar resize: stored as [h, w] at dst, written only if `ok` (a ragged item that fits),
+// scaled by sc, with UM_RAGGED_* flags; `may_copy`: an image at the input size without a flip is copied.  The kernel tests
+// its sample against (h, w) before `ok` and decodes the flags after both, as a thread past its image leaves first.
+struct ResizeImage {
   float* dst;
-  int ho, wo, Y, X;
+  int h, w;
   float sc;
-  int flip_x, copy, transpose;
+  int flags, may_copy, ok;
 };
 
-// Uniform batch [B, C, ho, wo]: one thread per output sample, channel c scaled by s_c.
-struct ResizeUniform {
-  const float* in;
-  float* out;
-  int C, hi, wi, ho, wo;
-  float s0, s1, s2;
-  int flip_x;
-  long long total;
-  __device__ __forceinline__ bool sample(ResizeSample& s) const {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return false;
-    s.X = (int)(i % wo);
-    s.Y = (int)((i / wo) % ho);
-    const long long bc = i / ((long long)ho * wo);
-    const int c = (int)(bc % C);
-    s.src = in + bc * (long long)hi * wi;
-    s.dst = out + bc * (long long)ho * wo;
-    s.ho = ho; s.wo = wo;
-    s.sc = c == 0 ? s0 : (c == 1 ? s1 : s2);
-    s.flip_x = flip_x;
-    s.copy = 0;
-    s.transpose = 0;
-    return true;
-  }
-};
-
-// Uniform single-channel batch [n, 1, hi, wi] -> item i at out + offset[i] at its own (h, w), scale and flip (grid y: item,
-// grid x: the capacity's pixels).  An item at the input size without a flip is copied as it is, as the stereo driver
-// leaves a disparity that needs no resize (the bilinear pass would turn a non-finite neighbour into NaN there).
-// UM_RAGGED_TRANSPOSE: the item's (h, w) is its size as stored; it is the transpose of the (w, h) resize of the source, so
-// the "at the input size" rule compares the swapped size.  Consecutive threads write consecutive stored samples.
-struct ResizeRagged {
+// Source planes [n, hi, wi].  Uniform batch (items null): destination planes [B, C, h, w], image n = b C + c scaled by
+// s_c, never copied (at equal sizes the bilinear pass still runs, and turns a non-finite neighbour into NaN).  Ragged
+// batch: image n at out + items[n].offset at its own size, scale and flags, (h, w) the capacity; an item that does not fit
+// writes nothing.  An item at the input size without a flip is copied as it is, as the stereo driver leaves a disparity that
+// needs no resize.  UM_RAGGED_TRANSPOSE: the item's (h, w) is its size as stored, so the "at the input size" rule compares
+// the swapped size.
+struct ResizeGeo {
   const float* in;
   float* out;
   const um_ragged_item* items;
-  int hi, wi, h_max, w_max;
+  int hi, wi, h, w, C;
+  float s0, s1, s2;
+  int flip_x;
   long long out_numel;
-  __device__ __forceinline__ bool sample(ResizeSample& s) const {
-    const int n = blockIdx.y;
+  __device__ __forceinline__ ResizeImage image(long long n) const {
+    if (!items) {
+      const int c = (int)(n % C);
+      return ResizeImage{out + n * h * w, h, w, c == 0 ? s0 : (c == 1 ? s1 : s2), flip_x ? UM_RAGGED_FLIP_X : 0, 0, 1};
+    }
     const um_ragged_item it = items[n];
-    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (!ragged_ok(it, h_max, w_max, 1, out_numel) || q >= (long long)it.h * it.w) return false;
-    s.transpose = (it.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0;
-    const int xs = (int)(q % it.w), ys = (int)(q / it.w);      // the sample as stored
-    s.X = s.transpose ? ys : xs;
-    s.Y = s.transpose ? xs : ys;
-    s.src = in + (long long)n * hi * wi;
-    s.dst = out + it.offset;
-    s.ho = s.transpose ? it.w : it.h;
-    s.wo = s.transpose ? it.h : it.w;
-    s.sc = it.scale;
-    s.flip_x = it.flags & UM_RAGGED_FLIP_X;
-    s.copy = !s.flip_x && s.ho == hi && s.wo == wi;
-    return true;
+    return ResizeImage{out + it.offset, it.h, it.w, it.scale, it.flags, 1, ragged_ok(it, h, w, 1, out_numel)};
   }
 };
 
 // out = scale * bilinear(in, ...).  `flip_x`: the OUTPUT is mirrored horizontally (torchvision hflip of
-// evaluate_stereo.py:789-796 folded into the same pass).
-template <class Geo>
-__global__ void __launch_bounds__(256) resize_bilinear_kernel(Geo geo, int hi, int wi) {
-  ResizeSample s;
-  if (!geo.sample(s)) return;
-  const float* base = s.src;
-  const float v = s.copy ? __ldg(base + (long long)s.Y * wi + s.X)
+// evaluate_stereo.py:789-796 folded into the same pass).  grid (x: the stored samples of one image, y: image - first);
+// consecutive threads write consecutive stored samples.
+__global__ void __launch_bounds__(256) resize_bilinear_kernel(ResizeGeo geo, long long first) {
+  um::by_layout(geo.items, [&] {
+    const long long n = first + blockIdx.y;
+    const ResizeImage im = geo.image(n);
+    const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= (long long)im.h * im.w || !im.ok) return;
+    const int transpose = (im.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0, flip_x = im.flags & UM_RAGGED_FLIP_X;
+    const int xs = (int)(q % im.w), ys = (int)(q / im.w);      // the sample as stored
+    const int X = transpose ? ys : xs, Y = transpose ? xs : ys;
+    const int ho = transpose ? im.w : im.h, wo = transpose ? im.h : im.w;
+    const int hi = geo.hi, wi = geo.wi;
+    const bool copy = im.may_copy && !flip_x && ho == hi && wo == wi;
+    const float* base = geo.in + n * hi * wi;
+    const float v = copy ? __ldg(base + (long long)Y * wi + X)
                          : bilinear_align_corners([&](int y, int x) { return __ldg(base + (long long)y * wi + x); }, hi, wi,
-                                                  s.ho, s.wo, s.Y, s.X);
-  const int Xo = s.flip_x ? s.wo - 1 - s.X : s.X;
-  s.dst[s.transpose ? (long long)Xo * s.ho + s.Y : (long long)s.Y * s.wo + Xo] = s.sc == 1.0f ? v : v * s.sc;
+                                                  ho, wo, Y, X);
+    const int Xo = flip_x ? wo - 1 - X : X;
+    im.dst[transpose ? (long long)Xo * ho + Y : (long long)Y * wo + Xo] = im.sc == 1.0f ? v : v * im.sc;
+  });
 }
 
 // ---- frames -> model input: uint8 [T,H,W,3] channel-last -> fp32 planar [T,3,ho,wo] ------------------------------------
-// `Geo` says where frame t lies, how large it is and whether it is read transposed: one size for the whole batch
-// (FramesUniform), or each frame at its own offset and size in a packed buffer (FramesRagged); the output is uniform.
-struct FramePixel {
+// Frame t [H, W, 3] at base (null: nothing to convert), read transposed with UM_RAGGED_TRANSPOSE in flags.
+struct FrameImage {
   const uint8_t* base;
-  int H, W, transpose;
-  long long t;
-  int Y, X;
+  int H, W, flags;
 };
 
-struct FramesUniform {
-  const uint8_t* frames;
-  int H, W, ho, wo;
-  long long total;
-  int transpose;
-  __device__ __forceinline__ bool pixel(FramePixel& p) const {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return false;
-    p.X = (int)(i % wo);
-    p.Y = (int)((i / wo) % ho);
-    p.t = i / ((long long)ho * wo);
-    p.base = frames + p.t * (long long)H * W * 3;
-    p.H = H; p.W = W;
-    p.transpose = transpose;
-    return true;
-  }
-};
-
-// grid (x: output pixels, y: frame)
-struct FramesRagged {
+// Uniform batch (items null): frames [n, h, w, 3], one transpose flag for all.  Ragged batch: frame t at frames +
+// items[t].offset at its own size, transposed with UM_RAGGED_TRANSPOSE, (h, w) the capacity.  The output is uniform.
+struct FramesGeo {
   const uint8_t* frames;
   const um_ragged_item* items;
-  int h_max, w_max, ho, wo;
+  int h, w, transpose;
   long long frames_bytes;
-  __device__ __forceinline__ bool pixel(FramePixel& p) const {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    p.t = blockIdx.y;
-    const um_ragged_item it = items[p.t];
-    if (i >= (long long)ho * wo || !ragged_ok(it, h_max, w_max, 3, frames_bytes)) return false;
-    p.X = (int)(i % wo);
-    p.Y = (int)(i / wo);
-    p.base = frames + it.offset;
-    p.H = it.h; p.W = it.w;
-    p.transpose = (it.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0;
-    return true;
+  __device__ __forceinline__ FrameImage image(long long t) const {
+    if (!items) return FrameImage{frames + t * h * w * 3, h, w, transpose ? UM_RAGGED_TRANSPOSE : 0};
+    const um_ragged_item it = items[t];
+    if (!ragged_ok(it, h, w, 3, frames_bytes)) return FrameImage{nullptr, 0, 0, 0};
+    return FrameImage{frames + it.offset, it.h, it.w, it.flags};
   }
 };
 
 // Flow frames, in [0, 255]: = resize_bilinear(frames.permute(0,3,1,2).float()), with the portrait transpose of
 // evaluate_flow.py:713-717 (the source is read as [3, W, H]) folded into the load.  One thread per output pixel, three
-// planes written.
-template <class Geo>
-__global__ void __launch_bounds__(256) frames_to_planar_kernel(Geo geo, float* __restrict__ out, int ho, int wo) {
-  FramePixel p;
-  if (!geo.pixel(p)) return;
-  const int H = p.H, W = p.W, X = p.X, Y = p.Y, transpose = p.transpose;
-  const int hs = transpose ? W : H, ws = transpose ? H : W;     // source size as the resize sees it
-  const uint8_t* base = p.base;
-  const long long plane = (long long)ho * wo;
-  float* o = out + p.t * 3 * plane + (long long)Y * wo + X;
+// planes written; grid (x: output pixels, y: frame - first).  No occupancy bound: 40 registers (6 CTAs per SM); at
+// __launch_bounds__(256, 8) it spills 8 bytes and a ragged step of 16 KITTI frames took 0.146 ms against 0.137 on an H100
+// 80GB HBM3 at 700 W (0.136 for the former ragged instantiation at 32 registers).
+__global__ void __launch_bounds__(256) frames_to_planar_kernel(FramesGeo geo, long long first, float* __restrict__ out, int ho,
+                                                               int wo) {
+  um::by_layout(geo.items, [&] {
+    const long long t = first + blockIdx.y;
+    const FrameImage f = geo.image(t);
+    const long long plane = (long long)ho * wo;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (!f.base || i >= plane) return;
+    const int H = f.H, W = f.W, X = (int)(i % wo), Y = (int)(i / wo), transpose = (f.flags & UM_RAGGED_TRANSPOSE) ? 1 : 0;
+    const int hs = transpose ? W : H, ws = transpose ? H : W;     // source size as the resize sees it
+    const uint8_t* base = f.base;
+    float* o = out + t * 3 * plane + (long long)Y * wo + X;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const auto load = [&](int y, int x) {
-      const long long pix = transpose ? (long long)x * W + y : (long long)y * W + x;
-      return (float)__ldg(base + pix * 3 + c);
-    };
-    o[c * plane] = bilinear_align_corners(load, hs, ws, ho, wo, Y, X);
-  }
+    for (int c = 0; c < 3; ++c) {
+      const auto load = [&](int y, int x) {
+        const long long pix = transpose ? (long long)x * W + y : (long long)y * W + x;
+        return (float)__ldg(base + pix * 3 + c);
+      };
+      o[c * plane] = bilinear_align_corners(load, hs, ws, ho, wo, Y, X);
+    }
+  });
 }
 
 // Depth and stereo frames, ImageNet-normalised: = resize_bilinear of the frames normalised the way the depth data pipeline
 // does it on the host (dataloader/depth/augmentation.py:30, 56-61): every SOURCE sample is x / 255, then - mean_c, then
 // / std_c, each one correctly rounded fp32 operation in that order, and the normalised samples are resampled.  No
-// transpose: the depth and stereo drivers have no portrait rule.
-template <class Geo>
-__global__ void __launch_bounds__(256) frames_to_planar_normalized_kernel(Geo geo, float* __restrict__ out, int ho, int wo,
-                                                                          float m0, float m1, float m2, float s0, float s1,
-                                                                          float s2) {
-  FramePixel p;
-  if (!geo.pixel(p)) return;
-  const int H = p.H, W = p.W, X = p.X, Y = p.Y;
-  const uint8_t* base = p.base;
-  const long long plane = (long long)ho * wo;
-  float* o = out + p.t * 3 * plane + (long long)Y * wo + X;
+// transpose: the depth and stereo drivers have no portrait rule.  6 CTAs per SM: 40 registers, no spills, the occupancy the
+// kernel had before its uniform and ragged versions shared one instantiation (46 registers without the bound).
+__global__ void __launch_bounds__(256, 6) frames_to_planar_normalized_kernel(FramesGeo geo, long long first,
+                                                                          float* __restrict__ out, int ho, int wo, float m0,
+                                                                          float m1, float m2, float s0, float s1, float s2) {
+  um::by_layout(geo.items, [&] {
+    const long long t = first + blockIdx.y;
+    const FrameImage f = geo.image(t);
+    const long long plane = (long long)ho * wo;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (!f.base || i >= plane) return;
+    const int H = f.H, W = f.W, X = (int)(i % wo), Y = (int)(i / wo);
+    const uint8_t* base = f.base;
+    float* o = out + t * 3 * plane + (long long)Y * wo + X;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    const float mean = c == 0 ? m0 : (c == 1 ? m1 : m2), std = c == 0 ? s0 : (c == 1 ? s1 : s2);
-    const auto load = [&](int y, int x) {
-      const float v = (float)__ldg(base + ((long long)y * W + x) * 3 + c);
-      return __fdiv_rn(__fsub_rn(__fdiv_rn(v, 255.0f), mean), std);
-    };
-    o[c * plane] = bilinear_align_corners(load, H, W, ho, wo, Y, X);
-  }
+    for (int c = 0; c < 3; ++c) {
+      const float mean = c == 0 ? m0 : (c == 1 ? m1 : m2), std = c == 0 ? s0 : (c == 1 ? s1 : s2);
+      const auto load = [&](int y, int x) {
+        const float v = (float)__ldg(base + ((long long)y * W + x) * 3 + c);
+        return __fdiv_rn(__fsub_rn(__fdiv_rn(v, 255.0f), mean), std);
+      };
+      o[c * plane] = bilinear_align_corners(load, H, W, ho, wo, Y, X);
+    }
+  });
 }
 
 // ---- Middlebury flow colouring: flow_to_image of utils/flow_viz.py:240-275 (the VCN variant) --------------------------
@@ -296,10 +259,10 @@ __device__ __forceinline__ bool flow_unknown(float u, float v) {
   return !(fabsf(u) <= 1e7f) || !(fabsf(v) <= 1e7f);        // also true for NaN
 }
 
-// Where flow image n and its picture lie: one size, contiguous flows and strided pictures (FlowUniform, grid x over all
-// pixels of the batch), or each flow [2, h, w] at its own offset in a packed buffer and its picture at its own byte offset
-// with 3w-byte rows (FlowRagged, grid x over the capacity's pixels, grid y the item).  A ragged item whose flow or picture
-// does not fit, or whose two sizes differ, has hw = 0: it reads and writes nothing.
+// Where flow image n and its picture lie.  Uniform batch (flows null): contiguous flows [n, 2, h, w] and strided pictures.
+// Ragged batch: each flow [2, h, w] at its own offset in a packed buffer and its picture at its own byte offset with
+// 3w-byte rows, (h, w) the capacity.  A ragged item whose flow or picture does not fit, or whose two sizes differ, has
+// hw = 0: it reads and writes nothing.
 struct FlowImage {
   const float* u;
   uint8_t* img;
@@ -307,65 +270,48 @@ struct FlowImage {
   long long hw, row_stride;
 };
 
-struct FlowUniform {
-  const float* flow;
-  uint8_t* out;
-  int w;
-  long long hw, row_stride, image_stride, total;
-  __device__ __forceinline__ FlowImage image(long long n) const {
-    return FlowImage{flow + n * 2 * hw, out + n * image_stride, w, hw, row_stride};
-  }
-  __device__ __forceinline__ bool pixel(long long& n, long long& p) const {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= total) return false;
-    n = i / hw;
-    p = i - n * hw;
-    return true;
-  }
-};
-
-struct FlowRagged {
+struct FlowGeo {
   const float* flow;
   uint8_t* out;
   const um_ragged_item* flows;
   const um_ragged_item* pics;
-  int h_max, w_max;
-  long long flow_numel, out_bytes;
+  int h, w;
+  long long row_stride, image_stride;                // uniform pictures
+  long long flow_numel, out_bytes;                   // ragged buffers
   __device__ __forceinline__ FlowImage image(long long n) const {
+    if (!flows) {
+      const long long hw = (long long)h * w;
+      return FlowImage{flow + n * 2 * hw, out + n * image_stride, w, hw, row_stride};
+    }
     const um_ragged_item f = flows[n], q = pics[n];
-    const bool ok = f.h == q.h && f.w == q.w && ragged_ok(f, h_max, w_max, 2, flow_numel) &&
-                    ragged_ok(q, h_max, w_max, 3, out_bytes);
+    const bool ok = f.h == q.h && f.w == q.w && ragged_ok(f, h, w, 2, flow_numel) && ragged_ok(q, h, w, 3, out_bytes);
     return FlowImage{flow + (ok ? f.offset : 0), out + (ok ? q.offset : 0), f.w, ok ? (long long)f.h * f.w : 0, 3LL * f.w};
-  }
-  __device__ __forceinline__ bool pixel(long long& n, long long& p) const {
-    n = blockIdx.y;
-    p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    return true;                                   // the kernel compares p with the image's hw
   }
 };
 
 // grid (x: CTAs striding over the pixels of one image, y: image)
-template <class Geo>
-__global__ void __launch_bounds__(256) flow_maxrad_kernel(Geo geo, unsigned* __restrict__ maxbits) {
-  const int n = blockIdx.y;
-  const FlowImage im = geo.image(n);
-  const long long hw = im.hw;
-  const float* u = im.u;
-  const float* v = u + hw;
-  float m = 0.f;
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
-    const float a = __ldg(u + p), b = __ldg(v + p);
-    if (flow_unknown(a, b)) continue;
-    m = fmaxf(m, __fsqrt_rn(__fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b))));
-  }
-  m = um::warp_max(m);
+__global__ void __launch_bounds__(256) flow_maxrad_kernel(FlowGeo geo, unsigned* __restrict__ maxbits) {
   __shared__ float part[8];
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < 8; ++i) m = fmaxf(m, part[i]);
-    atomicMax(maxbits + n, __float_as_uint(m));              // m >= 0: the bit patterns order like the values
-  }
+  um::by_layout(geo.flows, [&] {
+    const int n = blockIdx.y;
+    const FlowImage im = geo.image(n);
+    const long long hw = im.hw;
+    const float* u = im.u;
+    const float* v = u + hw;
+    float m = 0.f;
+    for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
+      const float a = __ldg(u + p), b = __ldg(v + p);
+      if (flow_unknown(a, b)) continue;
+      m = fmaxf(m, __fsqrt_rn(__fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b))));
+    }
+    m = um::warp_max(m);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int i = 1; i < 8; ++i) m = fmaxf(m, part[i]);
+      atomicMax(maxbits + n, __float_as_uint(m));              // m >= 0: the bit patterns order like the values
+    }
+  });
 }
 
 // Middlebury colour wheel (make_color_wheel, flow_viz.py:145-192): 55 hues, RY 15, YG 6, GC 4, CB 11, BM 13, MR 6.
@@ -385,31 +331,33 @@ __device__ __forceinline__ int wheel(int k, int ch) {
   return ch == 0 ? r0 : ch == 1 ? 0 : 255 - s;
 }
 
-template <class Geo>
-__global__ void __launch_bounds__(256) flow_color_kernel(Geo geo, const unsigned* __restrict__ maxbits) {
-  long long n, p;
-  if (!geo.pixel(n, p)) return;
-  const FlowImage im = geo.image(n);
-  if (p >= im.hw) return;
-  const int w = im.w;
-  const float uf = __ldg(im.u + p), vf = __ldg(im.u + im.hw + p);
-  uint8_t* o = im.img + (p / w) * im.row_stride + (p % w) * 3;
-  if (flow_unknown(uf, vf)) { o[0] = o[1] = o[2] = 0; return; }
-  const double den = __dadd_rn((double)__uint_as_float(__ldg(maxbits + n)), 2.220446049250313e-16);   // maxrad + eps
-  const double u = __ddiv_rn((double)uf, den), v = __ddiv_rn((double)vf, den);
-  const double rad = __dsqrt_rn(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v)));
-  const double a = __ddiv_rn(atan2(-v, -u), 3.141592653589793);
-  const double fk = __dadd_rn(__dmul_rn(__ddiv_rn(__dadd_rn(a, 1.0), 2.0), 54.0), 1.0);        // (a+1)/2*(ncols-1)+1
-  const int k0 = (int)floor(fk);
-  const int k1 = k0 + 1 == 56 ? 1 : k0 + 1;
-  const double f = __dsub_rn(fk, (double)k0);
+// grid (x: the pixels of one image, y: image)
+__global__ void __launch_bounds__(256) flow_color_kernel(FlowGeo geo, const unsigned* __restrict__ maxbits) {
+  um::by_layout(geo.flows, [&] {
+    const int n = blockIdx.y;
+    const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const FlowImage im = geo.image(n);
+    if (p >= im.hw) return;
+    const int w = im.w;
+    const float uf = __ldg(im.u + p), vf = __ldg(im.u + im.hw + p);
+    uint8_t* o = im.img + (p / w) * im.row_stride + (p % w) * 3;
+    if (flow_unknown(uf, vf)) { o[0] = o[1] = o[2] = 0; return; }
+    const double den = __dadd_rn((double)__uint_as_float(__ldg(maxbits + n)), 2.220446049250313e-16);   // maxrad + eps
+    const double u = __ddiv_rn((double)uf, den), v = __ddiv_rn((double)vf, den);
+    const double rad = __dsqrt_rn(__dadd_rn(__dmul_rn(u, u), __dmul_rn(v, v)));
+    const double a = __ddiv_rn(atan2(-v, -u), 3.141592653589793);
+    const double fk = __dadd_rn(__dmul_rn(__ddiv_rn(__dadd_rn(a, 1.0), 2.0), 54.0), 1.0);        // (a+1)/2*(ncols-1)+1
+    const int k0 = (int)floor(fk);
+    const int k1 = k0 + 1 == 56 ? 1 : k0 + 1;
+    const double f = __dsub_rn(fk, (double)k0);
 #pragma unroll
-  for (int ch = 0; ch < 3; ++ch) {
-    const double c0 = __ddiv_rn((double)wheel(k0 - 1, ch), 255.0), c1 = __ddiv_rn((double)wheel(k1 - 1, ch), 255.0);
-    double col = __dadd_rn(__dmul_rn(__dsub_rn(1.0, f), c0), __dmul_rn(f, c1));
-    col = rad <= 1.0 ? __dsub_rn(1.0, __dmul_rn(rad, __dsub_rn(1.0, col))) : __dmul_rn(col, 0.75);
-    o[ch] = (uint8_t)(int)floor(__dmul_rn(255.0, col));
-  }
+    for (int ch = 0; ch < 3; ++ch) {
+      const double c0 = __ddiv_rn((double)wheel(k0 - 1, ch), 255.0), c1 = __ddiv_rn((double)wheel(k1 - 1, ch), 255.0);
+      double col = __dadd_rn(__dmul_rn(__dsub_rn(1.0, f), c0), __dmul_rn(f, c1));
+      col = rad <= 1.0 ? __dsub_rn(1.0, __dmul_rn(rad, __dsub_rn(1.0, col))) : __dmul_rn(col, 0.75);
+      o[ch] = (uint8_t)(int)floor(__dmul_rn(255.0, col));
+    }
+  });
 }
 
 // ---- disparity colouring: vis_disparity of utils/visualization.py:11-16 ------------------------------------------------
@@ -465,9 +413,10 @@ __device__ const uint8_t kInferno[768] = {
     138, 246, 243, 142, 248, 244, 146, 249, 245, 150, 250, 246, 154, 251, 248, 157, 252, 249, 161, 253, 250, 164, 255, 252,
 };
 
-// Where disparity (or depth) image n and its picture lie: one size, contiguous images and strided pictures (DispUniform), or
-// each image at its own offset and size in a packed buffer, its picture at 3 * offset bytes with 3w-byte rows (DispRagged).
-// A ragged item that does not fit (ragged_ok) has hw = 0: it reads and writes nothing.  The depth kernels share both.
+// Where disparity (or depth) image n and its picture lie.  Uniform batch (items null): contiguous images [n, h, w] and
+// strided pictures.  Ragged batch: each image at its own offset and size in a packed buffer, its picture at 3 * offset
+// bytes with 3w-byte rows, (h, w) the capacity.  A ragged item that does not fit (ragged_ok) has hw = 0: it reads and
+// writes nothing.  The depth kernels share it.
 struct DispImage {
   const float* d;
   uint8_t* img;
@@ -475,92 +424,86 @@ struct DispImage {
   long long row_stride;
 };
 
-struct DispUniform {
-  const float* disp;
-  uint8_t* out;
-  int w, hw;
-  long long row_stride, image_stride;
-  __device__ __forceinline__ DispImage image(int n) const {
-    return DispImage{disp + (long long)n * hw, out + n * image_stride, w, hw, row_stride};
-  }
-};
-
-struct DispRagged {
+struct DispGeo {
   const float* disp;
   uint8_t* out;
   const um_ragged_item* items;
-  int h_max, w_max;
-  long long numel;
+  int h, w;
+  long long row_stride, image_stride;                // uniform pictures
+  long long numel;                                   // ragged buffer
   __device__ __forceinline__ DispImage image(int n) const {
+    if (!items) return DispImage{disp + (long long)n * h * w, out + n * image_stride, w, h * w, row_stride};
     const um_ragged_item it = items[n];
-    const bool ok = ragged_ok(it, h_max, w_max, 1, numel);
+    const bool ok = ragged_ok(it, h, w, 1, numel);
     return DispImage{disp + (ok ? it.offset : 0), out + 3 * (ok ? it.offset : 0), it.w, ok ? it.h * it.w : 0, 3LL * it.w};
   }
 };
 
 // grid (x: CTAs over the pixels of one image, y: image); 4 loads in flight per thread and step
-template <class Geo>
-__global__ void __launch_bounds__(256) disp_minmax_kernel(Geo geo, unsigned* __restrict__ lo, unsigned* __restrict__ hi) {
-  const int n = blockIdx.y;
-  const DispImage im = geo.image(n);
-  const float* d = im.d;
-  const int hw = im.hw;
-  unsigned l = 0, m = 0;
-  bool nan = false;
-  const int stride = gridDim.x * blockDim.x;
-  for (long long p0 = blockIdx.x * blockDim.x + threadIdx.x; p0 < hw; p0 += 4LL * stride) {
-    float v[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const long long p = p0 + (long long)k * stride;
-      v[k] = p < hw ? __ldg(d + p) : __ldg(d + p0);     // out of range: repeat a value of this thread's, no effect
-    }
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      nan |= v[k] != v[k];
-      const unsigned key = float_key(v[k]);
-      l = max(l, ~key);
-      m = max(m, key);
-    }
-  }
-  if (nan) m = kNanKey;
-  l = __reduce_max_sync(0xffffffffu, l);
-  m = __reduce_max_sync(0xffffffffu, m);
+__global__ void __launch_bounds__(256) disp_minmax_kernel(DispGeo geo, unsigned* __restrict__ lo, unsigned* __restrict__ hi) {
   __shared__ unsigned part[2][8];
-  if ((threadIdx.x & 31) == 0) { part[0][threadIdx.x >> 5] = l; part[1][threadIdx.x >> 5] = m; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < 8; ++i) { l = max(l, part[0][i]); m = max(m, part[1][i]); }
-    atomicMax(lo + n, l);
-    atomicMax(hi + n, m);
-  }
+  um::by_layout(geo.items, [&] {
+    const int n = blockIdx.y;
+    const DispImage im = geo.image(n);
+    const float* d = im.d;
+    const int hw = im.hw;
+    unsigned l = 0, m = 0;
+    bool nan = false;
+    const int stride = gridDim.x * blockDim.x;
+    for (long long p0 = blockIdx.x * blockDim.x + threadIdx.x; p0 < hw; p0 += 4LL * stride) {
+      float v[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const long long p = p0 + (long long)k * stride;
+        v[k] = p < hw ? __ldg(d + p) : __ldg(d + p0);     // out of range: repeat a value of this thread's, no effect
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        nan |= v[k] != v[k];
+        const unsigned key = float_key(v[k]);
+        l = max(l, ~key);
+        m = max(m, key);
+      }
+    }
+    if (nan) m = kNanKey;
+    l = __reduce_max_sync(0xffffffffu, l);
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0) { part[0][threadIdx.x >> 5] = l; part[1][threadIdx.x >> 5] = m; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int i = 1; i < 8; ++i) { l = max(l, part[0][i]); m = max(m, part[1][i]); }
+      atomicMax(lo + n, l);
+      atomicMax(hi + n, m);
+    }
+  });
 }
 
 // grid (x: CTAs over the pixels of one image, y: image); the LUT is staged in shared memory once per CTA, because every
 // warp indexes it divergently (a __constant__ table would serialise those reads)
-template <class Geo>
-__global__ void __launch_bounds__(256) disp_color_kernel(Geo geo, const unsigned* __restrict__ lo,
+__global__ void __launch_bounds__(256) disp_color_kernel(DispGeo geo, const unsigned* __restrict__ lo,
                                                          const unsigned* __restrict__ hi) {
   __shared__ uint8_t lut[768];
-  for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kInferno[i];
-  __syncthreads();
-  const int n = blockIdx.y;
-  const DispImage im = geo.image(n);
-  const int w = im.w, hw = im.hw;
-  const long long row_stride = im.row_stride;
-  const unsigned hkey = __ldg(hi + n);
-  const bool flagged = hkey == kNanKey;
-  const float mn = key_float(~__ldg(lo + n)), mx = key_float(hkey);
-  const float range = __fsub_rn(mx, mn);
-  const float* d = im.d;
-  uint8_t* img = im.img;
-  for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
-    const float q = __fmul_rn(__fdiv_rn(__fsub_rn(__ldg(d + p), mn), range), 255.0f);
-    const int g = (flagged || !(q >= 0.f)) ? 0 : min((int)q, 255);          // NaN -> 0; (int) truncates, as numpy's cast
-    const int y = (int)p / w, x = (int)p - y * w;
-    uint8_t* o = img + y * row_stride + 3LL * x;
-    o[0] = lut[3 * g]; o[1] = lut[3 * g + 1]; o[2] = lut[3 * g + 2];
-  }
+  um::by_layout(geo.items, [&] {
+    for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kInferno[i];
+    __syncthreads();
+    const int n = blockIdx.y;
+    const DispImage im = geo.image(n);
+    const int w = im.w, hw = im.hw;
+    const long long row_stride = im.row_stride;
+    const unsigned hkey = __ldg(hi + n);
+    const bool flagged = hkey == kNanKey;
+    const float mn = key_float(~__ldg(lo + n)), mx = key_float(hkey);
+    const float range = __fsub_rn(mx, mn);
+    const float* d = im.d;
+    uint8_t* img = im.img;
+    for (long long p = blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
+      const float q = __fmul_rn(__fdiv_rn(__fsub_rn(__ldg(d + p), mn), range), 255.0f);
+      const int g = (flagged || !(q >= 0.f)) ? 0 : min((int)q, 255);          // NaN -> 0; (int) truncates, as numpy's cast
+      const int y = (int)p / w, x = (int)p - y * w;
+      uint8_t* o = img + y * row_stride + 3LL * x;
+      o[0] = lut[3 * g]; o[1] = lut[3 * g + 1]; o[2] = lut[3 * g + 2];
+    }
+  });
 }
 
 // ---- depth colouring: viz_depth_tensor(1. / depth) of utils/visualization.py:92-107 ----------------------------------
@@ -624,8 +567,8 @@ __device__ __forceinline__ double p95_index(int hw) { return __dmul_rn(0.95, (do
 // p > 0 histograms byte 3 - p of the keys whose top p bytes equal rank k's prefix (bins 0-255) or else rank k+1's (bins
 // 256-511).  The loop bound is warp-uniform, so that a warp's equal bins are counted by one shared atomic
 // (__match_any_sync): a smooth depth map puts most of a warp into one bin, which would otherwise serialise the atomics.
-template <bool kFirst, class Geo>
-__global__ void __launch_bounds__(256) depth_hist_kernel(Geo geo, unsigned* __restrict__ scratch, int pass) {
+template <bool kFirst>
+__global__ void __launch_bounds__(256) depth_hist_kernel(DispGeo geo, unsigned* __restrict__ scratch, int pass) {
   __shared__ unsigned hist[2 * kDvBins];
   for (int i = threadIdx.x; i < 2 * kDvBins; i += blockDim.x) hist[i] = 0;
   const int n = blockIdx.y, lane = threadIdx.x & 31;
@@ -684,8 +627,7 @@ __global__ void __launch_bounds__(256) depth_hist_kernel(Geo geo, unsigned* __re
 // hold ranks k and k+1 and appends them to both prefixes.  After the last pass the prefixes are the keys a and b, and
 // thread 0 forms vmax, the fp32 divisor and the image's mode, each float64 / fp32 operation rounded on its own.  A skipped
 // ragged item (hw = 0) selects nothing.
-template <class Geo>
-__global__ void __launch_bounds__(256) depth_select_kernel(Geo geo, unsigned* __restrict__ scratch, int pass) {
+__global__ void __launch_bounds__(256) depth_select_kernel(DispGeo geo, unsigned* __restrict__ scratch, int pass) {
   const int hw = geo.image(blockIdx.x).hw;
   if (hw == 0) return;
   unsigned* img = scratch + (long long)blockIdx.x * kDvWords;
@@ -730,8 +672,7 @@ __global__ void __launch_bounds__(256) depth_select_kernel(Geo geo, unsigned* __
 }
 
 // grid (x: CTAs over the pixels of one image, y: image); the floor table is staged in shared memory as in disp_color_kernel
-template <class Geo>
-__global__ void __launch_bounds__(256) depth_color_kernel(Geo geo, const unsigned* __restrict__ scratch) {
+__global__ void __launch_bounds__(256) depth_color_kernel(DispGeo geo, const unsigned* __restrict__ scratch) {
   __shared__ uint8_t lut[768];
   for (int i = threadIdx.x; i < 768; i += blockDim.x) lut[i] = kPlasma[i];
   __syncthreads();
@@ -835,16 +776,65 @@ inline int ew_grid(long long n, int block = 256) {
   return (int)(g < cap ? (g > 0 ? g : 1) : cap);
 }
 
-// The memset and nine launches of um_depth_to_image(_ragged); `hw` sizes the grid (the capacity for a ragged batch).
-template <class Geo>
-int depth_to_image_launch(const Geo& geo, void* scratch, int n, long long hw, cudaStream_t st, const char* name) {
+// The launches of the uniform and the ragged entry of each driver op.  Grid x covers the pixels of the largest image: the
+// uniform size or the ragged capacity, geo.h x geo.w (for the frame conversion, the output size); grid y covers the images.
+// Passes that stride over an image take at most ~8 CTAs per SM over the batch.
+inline long long ctas_per_image(int n) { return ((long long)um::device_sm_count() * 8 + n - 1) / n; }
+
+int resize_launch(const ResizeGeo& geo, long long n, cudaStream_t st, const char* name) {
+  const unsigned gx = (unsigned)(((long long)geo.h * geo.w + 255) / 256);
+  return um::launch_image_chunks(n, name, [&](long long first, unsigned count) {
+    resize_bilinear_kernel<<<dim3(gx, count), 256, 0, st>>>(geo, first);
+  });
+}
+
+// mean null: the [0, 255] conversion; otherwise the ImageNet-normalised one with 3 means and stds
+int frames_launch(const FramesGeo& geo, int n, float* out, int ho, int wo, const float* mean, const float* std, cudaStream_t st,
+                  const char* name) {
+  const unsigned gx = (unsigned)(((long long)ho * wo + 255) / 256);
+  return um::launch_image_chunks(n, name, [&](long long first, unsigned count) {
+    if (mean)
+      frames_to_planar_normalized_kernel<<<dim3(gx, count), 256, 0, st>>>(geo, first, out, ho, wo, mean[0], mean[1], mean[2],
+                                                                          std[0], std[1], std[2]);
+    else
+      frames_to_planar_kernel<<<dim3(gx, count), 256, 0, st>>>(geo, first, out, ho, wo);
+  });
+}
+
+int flow_to_image_launch(const FlowGeo& geo, float* max_scratch, int n, cudaStream_t st, const char* name) {
+  const long long hw = (long long)geo.h * geo.w;
+  if (cudaMemsetAsync(max_scratch, 0, sizeof(float) * n, st) != cudaSuccess) return um::check_launch(name);
+  const long long bx = std::min((hw + 255) / 256, ctas_per_image(n));
+  flow_maxrad_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(geo, reinterpret_cast<unsigned*>(max_scratch));
+  if (int rc = um::check_launch(name)) return rc;
+  flow_color_kernel<<<dim3((unsigned)((hw + 255) / 256), (unsigned)n), 256, 0, st>>>(
+      geo, reinterpret_cast<const unsigned*>(max_scratch));
+  return um::check_launch(name);
+}
+
+int disparity_to_image_launch(const DispGeo& geo, float* minmax_scratch, int n, cudaStream_t st, const char* name) {
+  const long long hw = (long long)geo.h * geo.w;
+  unsigned* lo = reinterpret_cast<unsigned*>(minmax_scratch);
+  unsigned* hi = lo + n;
+  if (cudaMemsetAsync(minmax_scratch, 0, sizeof(float) * 2 * n, st) != cudaSuccess) return um::check_launch(name);
+  const long long per_image = ctas_per_image(n);
+  const long long bx = std::min((hw + 1023) / 1024, per_image);                    // 4 pixels per thread and pass
+  disp_minmax_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
+  if (int rc = um::check_launch(name)) return rc;
+  const long long cx = std::min((hw + 255) / 256, 2 * per_image);
+  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
+  return um::check_launch(name);
+}
+
+// The memset and nine launches of um_depth_to_image(_ragged).
+int depth_to_image_launch(const DispGeo& geo, void* scratch, int n, cudaStream_t st, const char* name) {
   static_assert(kDvWords == 2056, "the header states the scratch size");
+  const long long hw = (long long)geo.h * geo.w;
   unsigned* words = reinterpret_cast<unsigned*>(scratch);
   if (cudaMemsetAsync(scratch, 0, sizeof(unsigned) * kDvWords * n, st) != cudaSuccess) return um::check_launch(name);
-  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
-  long long bx = (hw + 1023) / 1024;                                                // 4 pixels per thread and pass
-  bx = bx < per_image ? bx : per_image;
-  const dim3 grid((unsigned)(bx > 0 ? bx : 1), (unsigned)n);
+  const long long per_image = ctas_per_image(n);
+  const long long bx = std::min((hw + 1023) / 1024, per_image);                    // 4 pixels per thread and pass
+  const dim3 grid((unsigned)bx, (unsigned)n);
   for (int pass = 0; pass < 4; ++pass) {
     if (pass == 0) depth_hist_kernel<true><<<grid, 256, 0, st>>>(geo, words, pass);
     else depth_hist_kernel<false><<<grid, 256, 0, st>>>(geo, words, pass);
@@ -852,8 +842,7 @@ int depth_to_image_launch(const Geo& geo, void* scratch, int n, long long hw, cu
     depth_select_kernel<<<(unsigned)n, 256, 0, st>>>(geo, words, pass);
     if (int rc = um::check_launch(name)) return rc;
   }
-  long long cx = (hw + 255) / 256;
-  cx = cx < 2 * per_image ? cx : 2 * per_image;
+  const long long cx = std::min((hw + 255) / 256, 2 * per_image);
   depth_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, words);
   return um::check_launch(name);
 }
@@ -895,32 +884,26 @@ int um_resize_bilinear(const float* in, float* out, int32_t batch, int32_t chann
                        int32_t h_out, int32_t w_out, const float* scale, int32_t flip_x, void* stream) {
   UM_REQUIRE(in && out && batch > 0 && channels > 0 && channels <= 3 && h_in > 0 && w_in > 0 && h_out > 0 && w_out > 0,
              "um_resize_bilinear: bad arguments (1-3 channels, positive sizes)");
-  const long long total = (long long)batch * channels * h_out * w_out;
   const float s0 = scale ? scale[0] : 1.0f, s1 = (scale && channels > 1) ? scale[1] : 1.0f,
               s2 = (scale && channels > 2) ? scale[2] : 1.0f;
-  const ResizeUniform geo{in, out, channels, h_in, w_in, h_out, w_out, s0, s1, s2, flip_x, total};
-  resize_bilinear_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, h_in, w_in);
-  return um::check_launch("um_resize_bilinear");
+  const ResizeGeo geo{in, out, nullptr, h_in, w_in, h_out, w_out, channels, s0, s1, s2, flip_x, 0};
+  return resize_launch(geo, (long long)batch * channels, (cudaStream_t)stream, "um_resize_bilinear");
 }
 
 int um_resize_bilinear_ragged(const float* in, float* out, int64_t out_numel, const um_ragged_item* items, int32_t n,
                               int32_t h_in, int32_t w_in, int32_t h_max, int32_t w_max, void* stream) {
   UM_REQUIRE(in && out && items && n > 0 && n <= 65535 && h_in > 0 && w_in > 0 && h_max > 0 && w_max > 0 && out_numel > 0,
              "um_resize_bilinear_ragged: bad arguments (1-65535 items, positive sizes, non-null buffers)");
-  const long long cap = (long long)h_max * w_max;
-  const ResizeRagged geo{in, out, items, h_in, w_in, h_max, w_max, out_numel};
-  resize_bilinear_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(geo, h_in, w_in);
-  return um::check_launch("um_resize_bilinear_ragged");
+  const ResizeGeo geo{in, out, items, h_in, w_in, h_max, w_max, 1, 1.0f, 1.0f, 1.0f, 0, out_numel};
+  return resize_launch(geo, n, (cudaStream_t)stream, "um_resize_bilinear_ragged");
 }
 
 int um_frames_to_planar(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t transpose,
                         int32_t h_out, int32_t w_out, void* stream) {
   UM_REQUIRE(frames && out && n > 0 && h > 0 && w > 0 && h_out > 0 && w_out > 0,
              "um_frames_to_planar: bad arguments (positive sizes, non-null buffers)");
-  const long long total = (long long)n * h_out * w_out;
-  const FramesUniform geo{frames, h, w, h_out, w_out, total, transpose ? 1 : 0};
-  frames_to_planar_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(geo, out, h_out, w_out);
-  return um::check_launch("um_frames_to_planar");
+  const FramesGeo geo{frames, nullptr, h, w, transpose ? 1 : 0, 0};
+  return frames_launch(geo, n, out, h_out, w_out, nullptr, nullptr, (cudaStream_t)stream, "um_frames_to_planar");
 }
 
 int um_frames_to_planar_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out, int32_t n,
@@ -928,22 +911,16 @@ int um_frames_to_planar_ragged(const uint8_t* frames, int64_t frames_bytes, cons
   UM_REQUIRE(frames && items && out && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && h_out > 0 && w_out > 0 &&
                  frames_bytes > 0,
              "um_frames_to_planar_ragged: bad arguments (1-65535 frames, positive sizes, non-null buffers)");
-  const long long plane = (long long)h_out * w_out;
-  const FramesRagged geo{frames, items, h_max, w_max, h_out, w_out, frames_bytes};
-  frames_to_planar_kernel<<<dim3((unsigned)((plane + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(geo, out, h_out,
-                                                                                                            w_out);
-  return um::check_launch("um_frames_to_planar_ragged");
+  const FramesGeo geo{frames, items, h_max, w_max, 0, frames_bytes};
+  return frames_launch(geo, n, out, h_out, w_out, nullptr, nullptr, (cudaStream_t)stream, "um_frames_to_planar_ragged");
 }
 
 int um_frames_to_planar_normalized(const uint8_t* frames, float* out, int32_t n, int32_t h, int32_t w, int32_t h_out,
                                    int32_t w_out, const float* mean, const float* std, void* stream) {
   UM_REQUIRE(frames && out && mean && std && n > 0 && h > 0 && w > 0 && h_out > 0 && w_out > 0,
              "um_frames_to_planar_normalized: bad arguments (positive sizes, non-null buffers, 3 means and stds)");
-  const long long total = (long long)n * h_out * w_out;
-  const FramesUniform geo{frames, h, w, h_out, w_out, total};
-  frames_to_planar_normalized_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      geo, out, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
-  return um::check_launch("um_frames_to_planar_normalized");
+  const FramesGeo geo{frames, nullptr, h, w, 0, 0};
+  return frames_launch(geo, n, out, h_out, w_out, mean, std, (cudaStream_t)stream, "um_frames_to_planar_normalized");
 }
 
 int um_frames_to_planar_normalized_ragged(const uint8_t* frames, int64_t frames_bytes, const um_ragged_item* items, float* out,
@@ -953,30 +930,18 @@ int um_frames_to_planar_normalized_ragged(const uint8_t* frames, int64_t frames_
                  w_out > 0 && frames_bytes > 0,
              "um_frames_to_planar_normalized_ragged: bad arguments (1-65535 frames, positive sizes, non-null buffers, 3 means "
              "and stds)");
-  const long long plane = (long long)h_out * w_out;
-  const FramesRagged geo{frames, items, h_max, w_max, h_out, w_out, frames_bytes};
-  frames_to_planar_normalized_kernel<<<dim3((unsigned)((plane + 255) / 256), (unsigned)n), 256, 0, (cudaStream_t)stream>>>(
-      geo, out, h_out, w_out, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
-  return um::check_launch("um_frames_to_planar_normalized_ragged");
+  const FramesGeo geo{frames, items, h_max, w_max, 0, frames_bytes};
+  return frames_launch(geo, n, out, h_out, w_out, mean, std, (cudaStream_t)stream, "um_frames_to_planar_normalized_ragged");
 }
 
 int um_flow_to_image(const float* flow, uint8_t* out, int64_t row_stride, int64_t image_stride, float* max_scratch,
                      int32_t n, int32_t h, int32_t w, void* stream) {
-  UM_REQUIRE(flow && out && max_scratch && n > 0 && h > 0 && w > 0, "um_flow_to_image: bad arguments");
+  UM_REQUIRE(flow && out && max_scratch && n > 0 && n <= 65535 && h > 0 && w > 0,
+             "um_flow_to_image: bad arguments (1-65535 images, positive sizes, non-null buffers)");
   UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
              "um_flow_to_image: row_stride must cover 3*w bytes and image_stride h rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long hw = (long long)h * w;
-  if (cudaMemsetAsync(max_scratch, 0, sizeof(float) * n, st) != cudaSuccess) return um::check_launch("um_flow_to_image");
-  long long bx = (hw + 255) / 256;
-  const long long cap = (132LL * 8 + n - 1) / n;          // about 8 CTAs per SM over the whole batch, grid-stride beyond
-  bx = bx < cap ? bx : cap;
-  const long long total = (long long)n * hw;
-  const FlowUniform geo{flow, out, w, hw, row_stride, image_stride, total};
-  flow_maxrad_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, reinterpret_cast<unsigned*>(max_scratch));
-  if (int rc = um::check_launch("um_flow_to_image")) return rc;
-  flow_color_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(geo, reinterpret_cast<const unsigned*>(max_scratch));
-  return um::check_launch("um_flow_to_image");
+  const FlowGeo geo{flow, out, nullptr, nullptr, h, w, row_stride, image_stride, 0, 0};
+  return flow_to_image_launch(geo, max_scratch, n, (cudaStream_t)stream, "um_flow_to_image");
 }
 
 int um_flow_to_image_ragged(const float* flow, int64_t flow_numel, const um_ragged_item* flow_items, uint8_t* out,
@@ -985,42 +950,19 @@ int um_flow_to_image_ragged(const float* flow, int64_t flow_numel, const um_ragg
   UM_REQUIRE(flow && flow_items && out && picture_items && max_scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 &&
                  flow_numel > 0 && out_bytes > 0,
              "um_flow_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long cap = (long long)h_max * w_max;      // the grids are sized for the largest image
-  if (cudaMemsetAsync(max_scratch, 0, sizeof(float) * n, st) != cudaSuccess) return um::check_launch("um_flow_to_image_ragged");
-  long long bx = (cap + 255) / 256;
-  const long long per_image = (132LL * 8 + n - 1) / n;
-  bx = bx < per_image ? bx : per_image;
-  const FlowRagged geo{flow, out, flow_items, picture_items, h_max, w_max, flow_numel, out_bytes};
-  flow_maxrad_kernel<<<dim3((unsigned)bx, (unsigned)n), 256, 0, st>>>(geo, reinterpret_cast<unsigned*>(max_scratch));
-  if (int rc = um::check_launch("um_flow_to_image_ragged")) return rc;
-  flow_color_kernel<<<dim3((unsigned)((cap + 255) / 256), (unsigned)n), 256, 0, st>>>(
-      geo, reinterpret_cast<const unsigned*>(max_scratch));
-  return um::check_launch("um_flow_to_image_ragged");
+  const FlowGeo geo{flow, out, flow_items, picture_items, h_max, w_max, 0, 0, flow_numel, out_bytes};
+  return flow_to_image_launch(geo, max_scratch, n, (cudaStream_t)stream, "um_flow_to_image_ragged");
 }
 
 int um_disparity_to_image(const float* disp, uint8_t* out, int64_t row_stride, int64_t image_stride, float* minmax_scratch,
                           int32_t n, int32_t h, int32_t w, void* stream) {
-  UM_REQUIRE(disp && out && minmax_scratch && n > 0 && h > 0 && w > 0, "um_disparity_to_image: bad arguments");
+  UM_REQUIRE(disp && out && minmax_scratch && n > 0 && n <= 65535 && h > 0 && w > 0,
+             "um_disparity_to_image: bad arguments (1-65535 images, positive sizes, non-null buffers)");
   UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_disparity_to_image: an image has at most 2^31 - 1 pixels");
   UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
              "um_disparity_to_image: row_stride must cover 3*w bytes and image_stride h rows");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int hw = h * w;
-  unsigned* lo = reinterpret_cast<unsigned*>(minmax_scratch);
-  unsigned* hi = lo + n;
-  if (cudaMemsetAsync(minmax_scratch, 0, sizeof(float) * 2 * n, st) != cudaSuccess)
-    return um::check_launch("um_disparity_to_image");
-  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;   // ~8 CTAs per SM over the batch
-  long long bx = ((long long)hw + 1023) / 1024;                                     // 4 pixels per thread and pass
-  bx = bx < per_image ? bx : per_image;
-  const DispUniform geo{disp, out, w, hw, row_stride, image_stride};
-  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, lo, hi);
-  if (int rc = um::check_launch("um_disparity_to_image")) return rc;
-  long long cx = ((long long)hw + 255) / 256;
-  cx = cx < 2 * per_image ? cx : 2 * per_image;
-  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
-  return um::check_launch("um_disparity_to_image");
+  const DispGeo geo{disp, out, nullptr, h, w, row_stride, image_stride, 0};
+  return disparity_to_image_launch(geo, minmax_scratch, n, (cudaStream_t)stream, "um_disparity_to_image");
 }
 
 int um_disparity_to_image_ragged(const float* disp, int64_t numel, const um_ragged_item* items, uint8_t* out,
@@ -1028,33 +970,19 @@ int um_disparity_to_image_ragged(const float* disp, int64_t numel, const um_ragg
   UM_REQUIRE(disp && items && out && minmax_scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && numel > 0,
              "um_disparity_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
   UM_REQUIRE((long long)h_max * w_max <= 0x7fffffffLL, "um_disparity_to_image_ragged: an image has at most 2^31 - 1 pixels");
-  cudaStream_t st = (cudaStream_t)stream;
-  const long long cap = (long long)h_max * w_max;      // the grid is sized for the largest image; smaller ones stride less
-  unsigned* lo = reinterpret_cast<unsigned*>(minmax_scratch);
-  unsigned* hi = lo + n;
-  if (cudaMemsetAsync(minmax_scratch, 0, sizeof(float) * 2 * n, st) != cudaSuccess)
-    return um::check_launch("um_disparity_to_image_ragged");
-  const long long per_image = ((long long)um::device_sm_count() * 8 + n - 1) / n;
-  long long bx = (cap + 1023) / 1024;
-  bx = bx < per_image ? bx : per_image;
-  const DispRagged geo{disp, out, items, h_max, w_max, numel};
-  disp_minmax_kernel<<<dim3((unsigned)(bx > 0 ? bx : 1), (unsigned)n), 256, 0, st>>>(geo, lo, hi);
-  if (int rc = um::check_launch("um_disparity_to_image_ragged")) return rc;
-  long long cx = (cap + 255) / 256;
-  cx = cx < 2 * per_image ? cx : 2 * per_image;
-  disp_color_kernel<<<dim3((unsigned)cx, (unsigned)n), 256, 0, st>>>(geo, lo, hi);
-  return um::check_launch("um_disparity_to_image_ragged");
+  const DispGeo geo{disp, out, items, h_max, w_max, 0, 0, numel};
+  return disparity_to_image_launch(geo, minmax_scratch, n, (cudaStream_t)stream, "um_disparity_to_image_ragged");
 }
 
 int um_depth_to_image(const float* depth, uint8_t* out, int64_t row_stride, int64_t image_stride, void* scratch, int32_t n,
                       int32_t h, int32_t w, void* stream) {
-  UM_REQUIRE(depth && out && scratch && n > 0 && h > 0 && w > 0, "um_depth_to_image: bad arguments");
+  UM_REQUIRE(depth && out && scratch && n > 0 && n <= 65535 && h > 0 && w > 0,
+             "um_depth_to_image: bad arguments (1-65535 images, positive sizes, non-null buffers)");
   UM_REQUIRE((long long)h * w <= 0x7fffffffLL, "um_depth_to_image: an image has at most 2^31 - 1 pixels");
   UM_REQUIRE(row_stride >= 3LL * w && image_stride >= row_stride * h,
              "um_depth_to_image: row_stride must cover 3*w bytes and image_stride h rows");
-  const int hw = h * w;
-  const DispUniform geo{depth, out, w, hw, row_stride, image_stride};
-  return depth_to_image_launch(geo, scratch, n, hw, (cudaStream_t)stream, "um_depth_to_image");
+  const DispGeo geo{depth, out, nullptr, h, w, row_stride, image_stride, 0};
+  return depth_to_image_launch(geo, scratch, n, (cudaStream_t)stream, "um_depth_to_image");
 }
 
 int um_depth_to_image_ragged(const float* depth, int64_t numel, const um_ragged_item* items, uint8_t* out, void* scratch,
@@ -1062,8 +990,8 @@ int um_depth_to_image_ragged(const float* depth, int64_t numel, const um_ragged_
   UM_REQUIRE(depth && items && out && scratch && n > 0 && n <= 65535 && h_max > 0 && w_max > 0 && numel > 0,
              "um_depth_to_image_ragged: bad arguments (1-65535 images, positive sizes, non-null buffers)");
   UM_REQUIRE((long long)h_max * w_max <= 0x7fffffffLL, "um_depth_to_image_ragged: an image has at most 2^31 - 1 pixels");
-  const DispRagged geo{depth, out, items, h_max, w_max, numel};
-  return depth_to_image_launch(geo, scratch, n, (long long)h_max * w_max, (cudaStream_t)stream, "um_depth_to_image_ragged");
+  const DispGeo geo{depth, out, items, h_max, w_max, 0, 0, numel};
+  return depth_to_image_launch(geo, scratch, n, (cudaStream_t)stream, "um_depth_to_image_ragged");
 }
 
 int um_encode_submission(const float* pred, int32_t batch, int32_t channels, int32_t h, int32_t w, int32_t geometry,

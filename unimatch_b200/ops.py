@@ -557,10 +557,15 @@ def _resize_bilinear(x, h_out, w_out, scale, flip_x):
 resize_bilinear = _define("resize_bilinear(Tensor x, int h_out, int w_out, float[]? scale, bool flip_x) -> Tensor", _resize_bilinear)
 
 
-def _frames_to_planar(frames, h_out, w_out, transpose):
+def _frames(frames, name):
+    """frames: contiguous CUDA uint8 [T, H, W, 3]; returns (T, H, W)"""
     if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3 or not frames.is_contiguous():
-        raise RuntimeError("frames_to_planar: expected contiguous CUDA uint8 frames [T, H, W, 3]")
-    t, h, w, _ = frames.shape
+        raise RuntimeError("%s: expected contiguous CUDA uint8 frames [T, H, W, 3]" % name)
+    return frames.shape[:3]
+
+
+def _frames_to_planar(frames, h_out, w_out, transpose):
+    t, h, w = _frames(frames, "frames_to_planar")
     out = torch.empty((t, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
     _check(LIB.um_frames_to_planar(_p(frames), _p(out), t, h, w, int(transpose), h_out, w_out, _stream()), "um_frames_to_planar")
     return out
@@ -571,11 +576,9 @@ frames_to_planar = _define("frames_to_planar(Tensor frames, int h_out, int w_out
 
 def _frames_to_planar_normalized(frames, h_out, w_out, mean, std):
     """mean / std: 3 per-channel constants each, passed to the kernel rounded to float32"""
-    if not frames.is_cuda or frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] != 3 or not frames.is_contiguous():
-        raise RuntimeError("frames_to_planar_normalized: expected contiguous CUDA uint8 frames [T, H, W, 3]")
+    t, h, w = _frames(frames, "frames_to_planar_normalized")
     if len(mean) != 3 or len(std) != 3:
         raise RuntimeError("frames_to_planar_normalized: expected 3 means and 3 stds")
-    t, h, w, _ = frames.shape
     out = torch.empty((t, 3, h_out, w_out), device=frames.device, dtype=torch.float32)
     m, s = (ctypes.c_float * 3)(*mean), (ctypes.c_float * 3)(*std)
     _check(LIB.um_frames_to_planar_normalized(_p(frames), _p(out), t, h, w, h_out, w_out, m, s, _stream()),
@@ -588,6 +591,14 @@ frames_to_planar_normalized = _define(
     _frames_to_planar_normalized)
 
 
+def _pictures(out, x, name, what):
+    """the pictures of x [N, ..., H, W]: uint8 [N, H, W, 3] on x's device with 3-byte pixels, rows and images may be strided"""
+    n, h, w = x.shape[0], x.shape[-2], x.shape[-1]
+    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
+            or out.device != x.device:
+        raise RuntimeError("%s: out must be uint8 [N, H, W, 3] on the %s's device with 3-byte pixels" % (name, what))
+
+
 def _flow_to_image(flow, out):
     """flow: planar [N, 2, H, W] fp32; out: uint8 [N, H, W, 3] whose pixels are 3 contiguous bytes -- rows and images may be
     strided (a view into a larger picture)."""
@@ -595,9 +606,7 @@ def _flow_to_image(flow, out):
     if flow.dim() != 4 or flow.shape[1] != 2:
         raise RuntimeError("flow_to_image: expected planar flow [N, 2, H, W]")
     n, _, h, w = flow.shape
-    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
-            or out.device != flow.device:
-        raise RuntimeError("flow_to_image: out must be uint8 [N, H, W, 3] on the flow's device with 3-byte pixels")
+    _pictures(out, flow, "flow_to_image", "flow")
     scratch = torch.empty((n,), device=flow.device, dtype=torch.float32)
     _check(LIB.um_flow_to_image(_p(flow), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
            "um_flow_to_image")
@@ -612,9 +621,7 @@ def _disparity_to_image(disp, out):
     if disp.dim() != 3:
         raise RuntimeError("disparity_to_image: expected disparities [N, H, W]")
     n, h, w = disp.shape
-    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
-            or out.device != disp.device:
-        raise RuntimeError("disparity_to_image: out must be uint8 [N, H, W, 3] on the disparity's device with 3-byte pixels")
+    _pictures(out, disp, "disparity_to_image", "disparity")
     scratch = torch.empty((2 * n,), device=disp.device, dtype=torch.float32)
     _check(LIB.um_disparity_to_image(_p(disp), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
            "um_disparity_to_image")
@@ -746,9 +753,7 @@ def _depth_to_image(depth, out):
     if depth.dim() != 3:
         raise RuntimeError("depth_to_image: expected depths [N, H, W]")
     n, h, w = depth.shape
-    if out.dtype != torch.uint8 or tuple(out.shape) != (n, h, w, 3) or out.stride(-1) != 1 or (w > 1 and out.stride(2) != 3) \
-            or out.device != depth.device:
-        raise RuntimeError("depth_to_image: out must be uint8 [N, H, W, 3] on the depth's device with 3-byte pixels")
+    _pictures(out, depth, "depth_to_image", "depth")
     scratch = torch.empty((DEPTH_TO_IMAGE_SCRATCH_WORDS * n,), device=depth.device, dtype=torch.int32)
     _check(LIB.um_depth_to_image(_p(depth), _p(out), out.stride(1), out.stride(0), _p(scratch), n, h, w, _stream()),
            "um_depth_to_image")
