@@ -29,7 +29,8 @@ extern "C" {
 
 #define UM_FEATURE_DIM 128
 
-/* ABI version and build info. */
+/* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
+ * tracks, the submission encoder, the scene-flow warp and statistics) leave existing callers working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
@@ -358,6 +359,55 @@ int um_track_points_backward(const float* flow, const float* occ, int32_t n, int
 int um_multi_flow_tracks(const float* flow, const float* occ, const float* err, const int32_t* src, const int32_t* dst,
                          int32_t n, int32_t k, int32_t h, int32_t w, int32_t r, float* pos, float* sig, uint8_t* vis,
                          float* tracks, uint8_t* visible, float* sigma, void* stream);
+
+/* ---- stereo scene flow -------------------------------------------------------------------------------------------
+ * The second disparity of scene flow (KITTI 2015's disp_1): the disparity at t+1 of the scene point seen at pixel p of the
+ * left frame at t, stored in frame t's grid.  disp_next [B, h, w] is the disparity of left frame t+1 and flow [B, 2, h, w]
+ * (planar) the optical flow from left frame t to left frame t+1, both contiguous at one size.  For pixel p = (x, y), in
+ * fp32 with each operation rounded on its own (no FMA), (u, v) = flow[b, :, y, x]:
+ *   q = (x + u, y + v);   in_frame[b, y, x] = 0 <= q.x <= w-1 && 0 <= q.y <= h-1   (uint8; a NaN coordinate gives 0);
+ *   c = (fminf(fmaxf(q.x, 0), w-1), fminf(fmaxf(q.y, 0), h-1))   (a NaN coordinate clamps to 0, as fmaxf does);
+ *   disp1[b, y, x] = bilinear(disp_next[b], c) with um_chain_tracks's bilinear and order of operations:
+ *     x0 = floor(c.x), fx = c.x - x0 (exact), gx = 1 - fx, likewise y;  gy (gx v00 + fx v01) + fy (gx v10 + fx v11),
+ *     a corner outside the frame (only ever at x0 + 1 = w or y0 + 1 = h, with weight 0) reads 0.
+ * That is grid_sample(disp_next, q, mode='bilinear', padding_mode='border', align_corners=True).  Decision: disp1 is
+ * dense.  A point that leaves the frame takes the nearest in-frame value rather than 0, because KITTI's disparity PNGs read
+ * 0 as "no estimate", and a dense map is scored without the server's background interpolation; in_frame says which pixels
+ * were sampled inside.  No occlusion handling: a point hidden at t+1 takes the disparity of whatever is in front of it.
+ * One thread per pixel, no host synchronisation (graph-capturable).  disp1 and in_frame overlap nothing.  Frames of at
+ * least 1 x 1, B <= 65535. */
+int um_warp_disparity(const float* disp_next, const float* flow, float* disp1, uint8_t* in_frame, int32_t batch, int32_t h,
+                      int32_t w, void* stream);
+
+/* KITTI 2015 scene-flow statistics (the devkit's D1, D2, Fl and SF outliers) of a batch at ground-truth resolution, on
+ * um_eval_stats's scaffold: UM_EVAL_PARTS CTAs per sample, each writing one partial row, then one ordered pass; no
+ * floating-point atomics, bit-reproducible.  Counts are kept per thread in 32-bit integers and converted at the reduction.
+ *   disp0, disp1: predictions [B, h, w]; flow: prediction [B, 2, h, w] (planar); all contiguous fp32;
+ *   gt_*: HOST arrays of 2 device pointers, gt_*[s] for s = UM_SF_OCC (all pixels) and UM_SF_NOC (non-occluded): disparities [B, h, w] (> 0 = valid, KITTI's PNG / 256),
+ *   flow [B, 2, h, w] and flow_valid [B, h, w] (>= 0.5 = valid); the UM_SF_NOC maps may all be NULL (that set then counts 0);
+ *   obj_map [B, h, w] or NULL: != 0 is foreground, NULL makes every pixel background;
+ *   scratch: DEVICE buffer of batch * UM_EVAL_PARTS * UM_SF_COLS doubles; out: DEVICE [batch, UM_SF_COLS] doubles.
+ * Per pixel and set, with um_eval_stats's fp32 expressions:
+ *   disparity (D1 on disp0, D2 on disp1): valid gt > 0, e = |gt - pred|, outlier e > 3 && e / gt > 0.05 (UM_EVS_D1);
+ *   flow (Fl): valid flow_valid >= 0.5, epe = sqrt(du du + dv dv), mag likewise of the gt, outlier epe > 3 && epe / mag > 0.05
+ *   (UM_EVF_OUTLIER);  SF: valid where all three are valid, an outlier where any of the three is.
+ * Column of (set, region, metric, kind) = UM_SF_COL(s, r, m, k). */
+#define UM_SF_OCC 0
+#define UM_SF_NOC 1
+#define UM_SF_BG 0
+#define UM_SF_FG 1
+#define UM_SF_D1 0
+#define UM_SF_D2 1
+#define UM_SF_FL 2
+#define UM_SF_SF 3
+#define UM_SF_N 0            /* valid pixels   */
+#define UM_SF_OUTLIERS 1     /* their outliers */
+#define UM_SF_COL(s, r, m, k) ((((s) * 2 + (r)) * 4 + (m)) * 2 + (k))
+#define UM_SF_COLS 32
+int um_scene_flow_stats(const float* disp0, const float* disp1, const float* flow, const float* const* gt_disp0,
+                        const float* const* gt_disp1, const float* const* gt_flow, const float* const* gt_flow_valid,
+                        const float* obj_map, int32_t batch, int32_t h, int32_t w, double* scratch, double* out,
+                        void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -38,6 +38,11 @@ _LAZY = {
     "MixedSizeDepthRunner": (".inference", "MixedSizeDepthRunner"),
     "disparity_to_image": (".inference", "disparity_to_image"),
     "depth_to_image": (".inference", "depth_to_image"),
+    "warp_disparity": (".inference", "warp_disparity"),
+    "infer_scene_flow": (".inference", "infer_scene_flow"),
+    "SceneFlowRunner": (".inference", "SceneFlowRunner"),
+    "validate_scene_flow": (".evaluation", "validate_scene_flow"),
+    "create_scene_flow_submission": (".submission", "create_scene_flow_submission"),
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
@@ -55,7 +60,8 @@ __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "In
            "multi_flow_tracks", "multi_flow_sources", "flow_to_image", "infer_depth_sequence", "DepthSequenceRunner", "StereoRunner",
            "MixedSizeStereoRunner", "MixedSizeFlowRunner", "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "tapvid_metrics", "create_flow_submission", "create_stereo_submission",
-           "inference_flow", "inference_stereo", "inference_depth"]
+           "inference_flow", "inference_stereo", "inference_depth", "warp_disparity", "infer_scene_flow", "SceneFlowRunner",
+           "validate_scene_flow", "create_scene_flow_submission"]
 
 
 def __getattr__(name):

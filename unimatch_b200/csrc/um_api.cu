@@ -1,5 +1,5 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
-// between the tensor-core and the general CUDA-core kernels) and the point-track entries (um_tracks.cu).  See include/unimatch_sm100.h.
+// between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -48,6 +48,8 @@ int track_points_backward_launch(const float* flow, const float* occ, int n, int
 int multi_flow_tracks_launch(const float* flow, const float* occ, const float* err, const int* src, const int* dst, int n,
                              int k, int h, int w, int r, float* pos, float* sig, uint8_t* vis, float* tracks,
                              uint8_t* visible, float* sigma, cudaStream_t st);
+int warp_disparity_launch(const float* disp_next, const float* flow, float* disp1, uint8_t* in_frame, int batch, int h, int w,
+                          cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -246,6 +248,20 @@ int um_multi_flow_tracks(const float* flow, const float* occ, const float* err, 
              "um_multi_flow_tracks: the state and outputs must not overlap each other or the inputs");
   return um::multi_flow_tracks_launch(flow, occ, err, src, dst, n, k, h, w, r, pos, sig, vis, tracks, visible, sigma,
                                       (cudaStream_t)stream);
+}
+
+int um_warp_disparity(const float* disp_next, const float* flow, float* disp1, uint8_t* in_frame, int32_t batch, int32_t h,
+                      int32_t w, void* stream) {
+  UM_REQUIRE(disp_next && flow && disp1 && in_frame, "um_warp_disparity: disp_next, flow, disp1 and in_frame must not be NULL");
+  UM_REQUIRE(batch > 0 && batch <= 65535 && h > 0 && w > 0, "um_warp_disparity: bad shape (batch %d, %d x %d)", batch, h, w);
+  UM_REQUIRE((long long)h * w <= 0x7fffffffLL && (long long)batch * h * w <= 0x7fffffffLL * 256,
+             "um_warp_disparity: a frame has at most 2^31 - 1 pixels, a batch at most 2^39 - 256");
+  UM_REQUIRE(um::aligned(disp_next, 4) && um::aligned(flow, 4) && um::aligned(disp1, 4),
+             "um_warp_disparity: disp_next, flow and disp1 must be 4-byte aligned");
+  const long long n = (long long)batch * h * w;
+  UM_REQUIRE(um::written_disjoint({{disp1, 4 * n}, {in_frame, n}, {disp_next, 4 * n}, {flow, 8 * n}}, 2),
+             "um_warp_disparity: disp1 and in_frame must not overlap each other or the inputs");
+  return um::warp_disparity_launch(disp_next, flow, disp1, in_frame, batch, h, w, (cudaStream_t)stream);
 }
 
 }  // extern "C"

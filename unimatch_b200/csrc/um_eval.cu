@@ -1,6 +1,6 @@
 // Evaluation statistics: predictions + ground truth of a batch -> a [B, S] float64 table of per-sample sufficient statistics
 // (counts and sums), from which the host forms the metrics of the reference's validate_* loops (evaluate_flow.py,
-// evaluate_stereo.py, evaluate_depth.py).
+// evaluate_stereo.py, evaluate_depth.py), and the KITTI 2015 scene-flow counts (um_scene_flow_stats) on the same scaffold.
 //
 // Arithmetic: every per-pixel value is computed with explicitly rounded fp32 intrinsics (no FMA contraction), in the order
 // the reference's torch / numpy expressions evaluate it, so each epe / error / ratio is the reference's fp32 value and every
@@ -15,10 +15,15 @@ namespace {
 
 constexpr int kThreads = 256;
 
+constexpr int kSceneFlow = 3;                        // um_scene_flow_stats: the task id of this file's scaffold only
+
+// Columns of a task's table and the per-thread accumulator type: fp64 sums, or 32-bit counts for the scene-flow table
+// (32 of them fit in registers where 32 doubles would spill; a thread counts at most hw / (UM_EVAL_PARTS * 256) pixels).
 template <int TASK> struct Cols;
-template <> struct Cols<UM_EVAL_FLOW> { static constexpr int n = UM_EVAL_FLOW_COLS; };
-template <> struct Cols<UM_EVAL_STEREO> { static constexpr int n = UM_EVAL_STEREO_COLS; };
-template <> struct Cols<UM_EVAL_DEPTH> { static constexpr int n = UM_EVAL_DEPTH_COLS; };
+template <> struct Cols<UM_EVAL_FLOW> { static constexpr int n = UM_EVAL_FLOW_COLS; using Acc = double; };
+template <> struct Cols<UM_EVAL_STEREO> { static constexpr int n = UM_EVAL_STEREO_COLS; using Acc = double; };
+template <> struct Cols<UM_EVAL_DEPTH> { static constexpr int n = UM_EVAL_DEPTH_COLS; using Acc = double; };
+template <> struct Cols<kSceneFlow> { static constexpr int n = UM_SF_COLS; using Acc = unsigned; };
 
 struct EvalArgs {
   const float* pred;
@@ -28,6 +33,18 @@ struct EvalArgs {
   const float* noc;                // contiguous [B, h, w] or NULL
   int mask_mode;
   float max_val, eval_min, eval_max;
+  int h, w;
+};
+
+struct SceneFlowArgs {
+  const float* disp0;              // contiguous [B, h, w]
+  const float* disp1;              // contiguous [B, h, w]
+  const float* flow;               // contiguous [B, 2, h, w]
+  const float* gt_disp0[2];        // per set (UM_SF_OCC, UM_SF_NOC): contiguous [B, h, w]; the NOC set NULL = absent
+  const float* gt_disp1[2];
+  const float* gt_flow[2];         // contiguous [B, 2, h, w]
+  const float* gt_valid[2];        // contiguous [B, h, w]
+  const float* obj;                // contiguous [B, h, w] or NULL
   int h, w;
 };
 
@@ -111,13 +128,55 @@ __device__ __forceinline__ void accumulate(const EvalArgs& a, int b, int y, int 
   }
 }
 
-// grid (UM_EVAL_PARTS, B): CTA p of sample b walks pixels p*256 + t, p*256 + t + PARTS*256, ... and writes one partial row.
+// A disparity outlier of the UM_EVS_D1 column: |gt - pred| > 3 and |gt - pred| / gt > 0.05.
+__device__ __forceinline__ bool disparity_outlier(float gt, float pred) {
+  const float e = fabsf(__fsub_rn(gt, pred));
+  return e > 3.f && __fdiv_rn(e, gt) > 0.05f;
+}
+
+// KITTI 2015 scene flow (devkit D1 / D2 / Fl / SF) at pixel (x, y): the valid and outlier counts of each set, in the
+// region (bg / fg) of the pixel.  Constant indices only: keeps `acc` in registers.
 template <int TASK>
-__global__ void __launch_bounds__(kThreads) eval_partial_kernel(EvalArgs a, double* __restrict__ partial) {
-  constexpr int S = Cols<TASK>::n;
-  double acc[S];
+__device__ __forceinline__ void accumulate(const SceneFlowArgs& a, int b, int y, int x, unsigned* acc) {
+  const long long hw = (long long)a.h * a.w, at = b * hw + (long long)y * a.w + x, fat = at + b * hw;
+  const float d0 = __ldg(a.disp0 + at), d1 = __ldg(a.disp1 + at);
+  const float u = __ldg(a.flow + fat), v = __ldg(a.flow + fat + hw);
+  const bool fg = a.obj && __ldg(a.obj + at) != 0.f;
 #pragma unroll
-  for (int c = 0; c < S; ++c) acc[c] = 0.0;
+  for (int s = 0; s < 2; ++s) {
+    if (!a.gt_disp0[s]) continue;
+    const float g0 = __ldg(a.gt_disp0[s] + at), g1 = __ldg(a.gt_disp1[s] + at);
+    const float gu = __ldg(a.gt_flow[s] + fat), gv = __ldg(a.gt_flow[s] + fat + hw);
+    const bool v0 = g0 > 0.f, v1 = g1 > 0.f, vf = __ldg(a.gt_valid[s] + at) >= 0.5f;
+    const bool o0 = v0 && disparity_outlier(g0, d0), o1 = v1 && disparity_outlier(g1, d1);
+    // the UM_EVF_OUTLIER expressions
+    const float du = __fsub_rn(u, gu), dv = __fsub_rn(v, gv);
+    const float epe = __fsqrt_rn(__fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv)));
+    const float mag = __fsqrt_rn(__fadd_rn(__fmul_rn(gu, gu), __fmul_rn(gv, gv)));
+    const bool of = vf && epe > 3.f && __fdiv_rn(epe, mag) > 0.05f;
+    const bool vs = v0 && v1 && vf, os = vs && (o0 || o1 || of);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const unsigned in = (fg == (r == UM_SF_FG)) ? 1u : 0u;
+      acc[UM_SF_COL(s, r, UM_SF_D1, UM_SF_N)] += in & v0;
+      acc[UM_SF_COL(s, r, UM_SF_D1, UM_SF_OUTLIERS)] += in & o0;
+      acc[UM_SF_COL(s, r, UM_SF_D2, UM_SF_N)] += in & v1;
+      acc[UM_SF_COL(s, r, UM_SF_D2, UM_SF_OUTLIERS)] += in & o1;
+      acc[UM_SF_COL(s, r, UM_SF_FL, UM_SF_N)] += in & vf;
+      acc[UM_SF_COL(s, r, UM_SF_FL, UM_SF_OUTLIERS)] += in & of;
+      acc[UM_SF_COL(s, r, UM_SF_SF, UM_SF_N)] += in & vs;
+      acc[UM_SF_COL(s, r, UM_SF_SF, UM_SF_OUTLIERS)] += in & os;
+    }
+  }
+}
+
+// grid (UM_EVAL_PARTS, B): CTA p of sample b walks pixels p*256 + t, p*256 + t + PARTS*256, ... and writes one partial row.
+template <int TASK, class Args>
+__global__ void __launch_bounds__(kThreads) eval_partial_kernel(Args a, double* __restrict__ partial) {
+  constexpr int S = Cols<TASK>::n;
+  typename Cols<TASK>::Acc acc[S];
+#pragma unroll
+  for (int c = 0; c < S; ++c) acc[c] = 0;
   const int b = blockIdx.y;
   const int hw = a.h * a.w;                          // < 2^31 (checked by the launcher): 32-bit index arithmetic
   for (int p = blockIdx.x * kThreads + threadIdx.x; p < hw; p += UM_EVAL_PARTS * kThreads) {
@@ -128,7 +187,7 @@ __global__ void __launch_bounds__(kThreads) eval_partial_kernel(EvalArgs a, doub
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int c = 0; c < S; ++c) {
-    double v = acc[c];
+    double v = (double)acc[c];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (lane == 0) red[warp][c] = v;
@@ -154,14 +213,14 @@ __global__ void __launch_bounds__(kThreads) eval_final_kernel(const double* __re
   out[i] = v;
 }
 
-template <int TASK>
-int launch(const EvalArgs& a, int batch, double* scratch, double* out, cudaStream_t st) {
+template <int TASK, class Args>
+int launch(const Args& a, int batch, double* scratch, double* out, cudaStream_t st, const char* what) {
   constexpr int S = Cols<TASK>::n;
   eval_partial_kernel<TASK><<<dim3(UM_EVAL_PARTS, (unsigned)batch), kThreads, 0, st>>>(a, scratch);
-  if (int rc = um::check_launch("um_eval_stats")) return rc;
+  if (int rc = um::check_launch(what)) return rc;
   const int total = batch * S;
   eval_final_kernel<<<(total + kThreads - 1) / kThreads, kThreads, 0, st>>>(scratch, out, S, total);
-  return um::check_launch("um_eval_stats");
+  return um::check_launch(what);
 }
 
 }  // namespace
@@ -189,9 +248,39 @@ int um_eval_stats(const float* pred, int64_t pred_sb, int64_t pred_sc, int64_t p
   }
   const EvalArgs a{pred, pred_sb, pred_sc, pred_sy, pred_sx, gt, valid, noc_valid, mask_mode, max_val, eval_min, eval_max, h, w};
   cudaStream_t st = (cudaStream_t)stream;
-  if (task == UM_EVAL_FLOW) return launch<UM_EVAL_FLOW>(a, batch, scratch, out, st);
-  if (task == UM_EVAL_STEREO) return launch<UM_EVAL_STEREO>(a, batch, scratch, out, st);
-  return launch<UM_EVAL_DEPTH>(a, batch, scratch, out, st);
+  if (task == UM_EVAL_FLOW) return launch<UM_EVAL_FLOW>(a, batch, scratch, out, st, "um_eval_stats");
+  if (task == UM_EVAL_STEREO) return launch<UM_EVAL_STEREO>(a, batch, scratch, out, st, "um_eval_stats");
+  return launch<UM_EVAL_DEPTH>(a, batch, scratch, out, st, "um_eval_stats");
+}
+
+int um_scene_flow_stats(const float* disp0, const float* disp1, const float* flow, const float* const* gt_disp0,
+                        const float* const* gt_disp1, const float* const* gt_flow, const float* const* gt_flow_valid,
+                        const float* obj_map, int32_t batch, int32_t h, int32_t w, double* scratch, double* out,
+                        void* stream) {
+  UM_REQUIRE(disp0 && disp1 && flow && scratch && out, "um_scene_flow_stats: predictions, scratch and out must be non-null");
+  UM_REQUIRE(gt_disp0 && gt_disp1 && gt_flow && gt_flow_valid,
+             "um_scene_flow_stats: the ground-truth pointer arrays must be non-null");
+  UM_REQUIRE(gt_disp0[UM_SF_OCC] && gt_disp1[UM_SF_OCC] && gt_flow[UM_SF_OCC] && gt_flow_valid[UM_SF_OCC],
+             "um_scene_flow_stats: the occ set needs disp0, disp1, flow and flow_valid");
+  const bool noc = gt_disp0[UM_SF_NOC] || gt_disp1[UM_SF_NOC] || gt_flow[UM_SF_NOC] || gt_flow_valid[UM_SF_NOC];
+  UM_REQUIRE(!noc || (gt_disp0[UM_SF_NOC] && gt_disp1[UM_SF_NOC] && gt_flow[UM_SF_NOC] && gt_flow_valid[UM_SF_NOC]),
+             "um_scene_flow_stats: the noc set takes all four maps or none");
+  UM_REQUIRE(batch > 0 && h > 0 && w > 0 && batch <= 65535 && (int64_t)h * w < ((int64_t)1 << 31) - UM_EVAL_PARTS * 256,
+             "um_scene_flow_stats: bad sizes (batch %d, %d x %d)", batch, h, w);
+  SceneFlowArgs a{};
+  a.disp0 = disp0;
+  a.disp1 = disp1;
+  a.flow = flow;
+  for (int s = 0; s < 2; ++s) {
+    a.gt_disp0[s] = gt_disp0[s];
+    a.gt_disp1[s] = gt_disp1[s];
+    a.gt_flow[s] = gt_flow[s];
+    a.gt_valid[s] = gt_flow_valid[s];
+  }
+  a.obj = obj_map;
+  a.h = h;
+  a.w = w;
+  return launch<kSceneFlow>(a, batch, scratch, out, (cudaStream_t)stream, "um_scene_flow_stats");
 }
 
 }  // extern "C"

@@ -4,7 +4,8 @@
 // um_track_points_backward).  Multi-flow: every pixel of a first frame, each new frame reached from several earlier
 // frames, keeping the most certain visible candidate (um_multi_flow_tracks).  Semantics and the fp32 order of operations:
 // include/unimatch_sm100.h; the float64 statements are tests/refops_tracks.py, tests/refops_points.py and
-// tests/refops_multiflow.py.
+// tests/refops_multiflow.py.  Scene flow: the second disparity warped through the flow with the same bilinear
+// (um_warp_disparity; statement tests/refops_sceneflow.py).
 #include "um_common.cuh"
 
 namespace {
@@ -193,6 +194,25 @@ multi_flow_tracks_kernel(const float* __restrict__ flow, const float* __restrict
   }
 }
 
+// One thread per pixel of the B frames: q = p + flow(p), then the bilinear sample of disp_next at q clamped into the frame
+// (grid_sample's border padding).  The clamped coordinate always lies inside, so only the weight-0 corner at x0 + 1 = w or
+// y0 + 1 = h can fall outside, and lerp2 reads 0 there.
+__global__ void __launch_bounds__(TRACK_THREADS)
+warp_disparity_kernel(const float* __restrict__ disp_next, const float* __restrict__ flow, float* __restrict__ disp1,
+                      uint8_t* __restrict__ in_frame, int h, int w, long long total) {
+  const long long i = (long long)blockIdx.x * TRACK_THREADS + threadIdx.x;
+  if (i >= total) return;
+  const long long plane = (long long)h * w;
+  const long long b = i / plane, pix = i - b * plane;
+  const int y = (int)(pix / w), x = (int)(pix - (long long)y * w);
+  const float* f = flow + 2 * b * plane + pix;
+  const float qx = __fadd_rn((float)x, __ldg(f)), qy = __fadd_rn((float)y, __ldg(f + plane));
+  const float mw = (float)(w - 1), mh = (float)(h - 1);
+  in_frame[i] = (qx >= 0.f && qx <= mw && qy >= 0.f && qy <= mh) ? 1 : 0;
+  const float cx = fminf(fmaxf(qx, 0.f), mw), cy = fminf(fmaxf(qy, 0.f), mh);
+  disp1[i] = lerp2(disp_next + b * plane, w, axis_taps(cx, w), axis_taps(cy, h));
+}
+
 }  // namespace
 
 namespace um {
@@ -224,6 +244,15 @@ int multi_flow_tracks_launch(const float* flow, const float* occ, const float* e
       flow, occ, err, src, dst, n, k, h, w, r, reinterpret_cast<float2*>(pos), sig, vis,
       reinterpret_cast<float2*>(tracks), visible, sigma);
   return check_launch("um_multi_flow_tracks");
+}
+
+// Arguments are checked by um_warp_disparity (um_api.cu).
+int warp_disparity_launch(const float* disp_next, const float* flow, float* disp1, uint8_t* in_frame, int batch, int h, int w,
+                          cudaStream_t st) {
+  const long long total = (long long)batch * h * w;
+  warp_disparity_kernel<<<(unsigned)((total + TRACK_THREADS - 1) / TRACK_THREADS), TRACK_THREADS, 0, st>>>(
+      disp_next, flow, disp1, in_frame, h, w, total);
+  return check_launch("um_warp_disparity");
 }
 
 int track_points_backward_launch(const float* flow, const float* occ, int n, int h, int w, const float* queries, int nq,

@@ -17,6 +17,9 @@ until the single download at the end; the flow and stereo drivers issue no other
 synchronises once per batch for its `torch.inverse`).  The metrics are then formed on the host in float64, following each
 reference loop -- including its quirks, listed in each driver's docstring.
 
+`validate_scene_flow` scores stereo scene flow (`infer_scene_flow`) with KITTI 2015's D1, D2, Fl and SF outliers
+(`um_scene_flow_stats`), on the same batching and single download.
+
 `tapvid_metrics` scores point tracks (e.g. `PointTrackRunner`'s) with TAP-Vid's metrics, in numpy on the host.
 """
 import os
@@ -25,7 +28,7 @@ import numpy as np
 import torch
 
 from . import ops
-from .inference import InputPadder, _resize, depth_to_image
+from .inference import InputPadder, _resize, depth_to_image, infer_scene_flow
 
 _OPS = torch.ops.unimatch_sm100
 
@@ -39,8 +42,10 @@ def _col(task, name):
     return ops.EVAL_COLS[task].index(name)
 
 
-def _upload(t, device):
-    t = t.float()
+def _upload(t, device, keep_uint8=False):
+    """A stacked host field on `device` through pinned memory, as float32 (uint8 kept as it is with `keep_uint8`)"""
+    if not (keep_uint8 and t.dtype == torch.uint8):
+        t = t.float()
     if device.type == "cuda":
         return t.pin_memory().to(device, non_blocking=True)
     return t.to(device)
@@ -58,11 +63,12 @@ def _download(table):
     return host.numpy()
 
 
-def _statistics(samples, batch, device, run, columns, on_batch=None):
+def _statistics(samples, batch, device, run, columns, on_batch=None, keep_uint8=False):
     """Per-sample statistics table [N, columns] (float64, dataset order) of `samples`, an iterable of tuples of CPU tensors
     (None for an absent optional tensor) grouped by the shape of their first tensor into batches of `batch`; `run(*tensors)`
     gets each batch stacked on the device and returns its [n, columns] device table.  `on_batch(indices, table)`, when
-    given, follows each `run` with the batch's dataset indices and its device table."""
+    given, follows each `run` with the batch's dataset indices and its device table.  With `keep_uint8`, uint8 fields (frames
+    as decoded) are uploaded as they are rather than as float32."""
     if batch < 1:
         raise ValueError("batch must be positive")
     device = torch.device(device)
@@ -70,7 +76,7 @@ def _statistics(samples, batch, device, run, columns, on_batch=None):
 
     def flush(shape):
         items = open_batches.pop(shape)
-        fields = [None if items[0][1][k] is None else _upload(torch.stack([it[1][k] for it in items]), device)
+        fields = [None if items[0][1][k] is None else _upload(torch.stack([it[1][k] for it in items]), device, keep_uint8)
                   for k in range(len(items[0][1]))]
         tables.append(run(*fields))
         order.extend(i for i, _ in items)
@@ -339,6 +345,97 @@ def _depth_results(T):
                       c["a1"][i] / n, c["a2"][i] / n, c["a3"][i] / n]
     num_samples = T.shape[0]
     return {k: (float(v / num_samples) if num_samples else float("nan")) for k, v in zip(_DEPTH_NAMES, error_sum)}
+
+
+# ---------------------------------------------------------------------------------------------------------- scene flow
+_SF_VIEWS = ("left0", "right0", "left1", "right1")
+_SF_GT = ("disp0", "disp1", "flow", "flow_valid")
+_SF_NOC = ("disp0_noc", "disp1_noc", "flow_noc", "flow_noc_valid")
+
+
+def _scene_flow_fields(s, index, noc, obj):
+    """The tensors of scene-flow sample `index` in the order `validate_scene_flow`'s batches take them, checked: four uint8
+    views [H,W,3] of one size, the ground truth at that size, the noc maps and obj_map when the dataset has them."""
+    if not isinstance(s, dict):
+        raise ValueError("validate_scene_flow: sample %d is not a dict" % index)
+    keys = _SF_VIEWS + _SF_GT + (_SF_NOC if noc else ()) + (("obj_map",) if obj else ())
+    if any(k in s for k in _SF_NOC) and not all(k in s for k in _SF_NOC):
+        raise ValueError("validate_scene_flow: sample %d has some of the noc maps %s but not all" % (index, list(_SF_NOC)))
+    missing = [k for k in keys if k not in s]
+    if missing:
+        raise ValueError("validate_scene_flow: sample %d lacks %s" % (index, missing))
+    if (all(k in s for k in _SF_NOC), "obj_map" in s) != (noc, obj):
+        raise ValueError("validate_scene_flow: sample %d differs from the first in its noc maps or obj_map" % index)
+    f = {k: torch.as_tensor(s[k]) for k in keys}
+    h, w = f["left0"].shape[:2] if f["left0"].dim() == 3 else (-1, -1)
+    for k in _SF_VIEWS:
+        if f[k].dtype != torch.uint8 or tuple(f[k].shape) != (h, w, 3):
+            raise ValueError("validate_scene_flow: sample %d: the views must be uint8 [H,W,3] of one size (%s is %s)"
+                             % (index, k, list(f[k].shape)))
+    for k in keys[4:]:
+        shape = (2, h, w) if k in ("flow", "flow_noc") else (h, w)
+        if tuple(f[k].shape) != shape:
+            raise ValueError("validate_scene_flow: sample %d: %s must be %s" % (index, k, list(shape)))
+    # the order `validate_scene_flow`'s run() takes: views, gt, the four noc maps or four Nones, obj_map or None
+    return (tuple(f[k] for k in _SF_VIEWS + _SF_GT) + (tuple(f[k] for k in _SF_NOC) if noc else (None,) * len(_SF_NOC))
+            + ((f["obj_map"],) if obj else (None,)))
+
+
+@torch.no_grad()
+def validate_scene_flow(stereo_model, flow_model, dataset, *, batch=8, device="cuda", stereo_kwargs=None, flow_kwargs=None,
+                        stereo_padding_factor=16, flow_padding_factor=32, stereo_inference_size=None,
+                        flow_inference_size=None):
+    """KITTI 2015 scene-flow results of `infer_scene_flow` on `dataset`: the devkit's D1, D2, Fl and SF outlier rates.
+
+    Samples are dicts with uint8 'left0', 'right0', 'left1', 'right1' [H,W,3] and the ground truth as float maps: 'disp0',
+    'disp1' [H,W] (KITTI's PNG / 256, 0 = no ground truth), 'flow' [2,H,W] and 'flow_valid' [H,W] (>= 0.5 = valid).  Optional,
+    in every sample or in none: 'disp0_noc', 'disp1_noc', 'flow_noc', 'flow_noc_valid' (the non-occluded set, the same
+    encoding) and 'obj_map' [H,W] (nonzero = foreground).
+    Per set (occ = all pixels, noc) and region: a disparity pixel is valid where its gt > 0 and an outlier where e > 3 and
+    e / gt > 0.05 (e = |gt - pred|; D1 on disp_0, D2 on disp_1); a flow pixel is valid where flow_valid >= 0.5 and an outlier
+    where epe > 3 and epe / |gt| > 0.05 (Fl); an SF pixel is valid where all three are and an outlier where any of the three
+    is.  Each value is 100 * outliers / valid pixels over the whole dataset, summed in float64 as the devkit sums them.
+    Returns `kitti_sf_{occ,noc}_{d1,d2,fl,sf}_{bg,fg,all}`; without noc maps there are no noc keys, without obj_map the fg
+    keys are NaN (every pixel is background), and an empty set gives NaN.
+
+    These are not comparable bit for bit with `validate_stereo(protocol='kitti15')` / `validate_flow(protocol='kitti')`:
+    those follow the reference's padding validators, this follows the inference geometry of `infer_scene_flow` (resize to a
+    multiple of the padding factor and back), the geometry the runner and the submission writer use.
+    Samples of one size form batches of `batch` (one open batch per size), one `um_scene_flow_stats` launch per batch, one
+    download at the end."""
+    first = {}
+
+    def samples():
+        for i, s in enumerate(dataset):
+            if not first:
+                first.update(noc=isinstance(s, dict) and all(k in s for k in _SF_NOC),
+                             obj=isinstance(s, dict) and "obj_map" in s)
+            yield _scene_flow_fields(s, i, first["noc"], first["obj"])
+
+    def run(left0, right0, left1, right1, disp0, disp1, flow, valid, nd0, nd1, nf, nv, obj):
+        out = infer_scene_flow(stereo_model, flow_model, left0, right0, left1, right1, stereo_kwargs=stereo_kwargs,
+                               flow_kwargs=flow_kwargs, stereo_padding_factor=stereo_padding_factor,
+                               flow_padding_factor=flow_padding_factor, stereo_inference_size=stereo_inference_size,
+                               flow_inference_size=flow_inference_size)
+        # the frames travel as uint8; a ground-truth map or obj_map given as uint8 is widened here, on the device
+        maps = [None if t is None else t.float() for t in (disp0, disp1, flow, valid, nd0, nd1, nf, nv, obj)]
+        return _OPS.scene_flow_stats(out["disp_0"], out["disp_1"], out["flow"], *maps)
+
+    T = _statistics(samples(), batch, device, run, ops.SF_COLS, keep_uint8=True)
+    return scene_flow_results(T.sum(axis=0) if len(T) else np.zeros(ops.SF_COLS), first.get("noc", False))
+
+
+def scene_flow_results(counts, noc):
+    """The results dict of a summed count table [SF_COLS] (columns `ops.sf_col`): 100 * outliers / valid per set, metric
+    and region, 'all' = bg + fg; NaN for an empty set; the noc keys only when `noc`."""
+    res = {}
+    for s, set_name in enumerate(ops.SF_SETS[:2 if noc else 1]):
+        for m, metric in enumerate(ops.SF_METRICS):
+            n = [counts[ops.sf_col(s, r, m, 0)] for r in range(2)]
+            o = [counts[ops.sf_col(s, r, m, 1)] for r in range(2)]
+            for key, num, den in (("bg", o[0], n[0]), ("fg", o[1], n[1]), ("all", o[0] + o[1], n[0] + n[1])):
+                res["kitti_sf_%s_%s_%s" % (set_name, metric, key)] = _ratio(100.0 * np.float64(num), den)
+    return res
 
 
 # ---------------------------------------------------------------------------------------------------------- point tracks

@@ -55,6 +55,12 @@ Posed depth pairs of mixed sizes (`inference_depth`, evaluate_depth.py:338-417, 
 `MixedSizeDepthRunner` streams host (frame t, frame t+1, relative pose) items, batched by frame t's inference size, through
 the same machinery; the conversion, the resize back and the colouring (`um_depth_to_image_ragged`) read each frame's size
 from the descriptor table.
+
+Stereo scene flow (KITTI 2015's disp_0 / disp_1 / flow, the stereo and flow networks together): `infer_scene_flow` runs one
+stereo forward over the 2B pairs of B stereo quadruples (left0, right0, left1, right1), one flow forward on (left0, left1)
+and one `um_warp_disparity`, which samples the disparity of frame t+1 where the flow carries each pixel of frame t;
+`warp_disparity` is that kernel for device tensors a caller holds, and `SceneFlowRunner` streams host stereo frames with
+each frame's stereo computed and its left view encoded once, in one CUDA graph per staging slot.
 """
 import collections
 import itertools
@@ -514,9 +520,13 @@ class _PipelinedRunner:
                 with torch.cuda.graph(g):
                     outs.append(step(slot))
                 graphs.append(g)
-            held = self.model.cached_buffers()
+            held = [b for m in self._graph_models() for b in m.cached_buffers()]
             torch.cuda.synchronize()
         return graphs, outs, held
+
+    def _graph_models(self):
+        """The modules a step calls, whose cached planes its graphs hold"""
+        return (self.model,)
 
     def _stage(self, slot, chunk):
         """host side of one batch, then the H2D copies on the side stream; returns their completion event.  The slot's
@@ -1880,3 +1890,172 @@ class MixedSizeDepthRunner(_PosedDepth, _MixedSizeRunner):
         feats = self.model.encode_frames(x, task="depth")
         depth = self._depth(slot, [f[:b] for f in feats], [f[b:] for f in feats])                 # [views * b, H, W]
         return self._resize_back(depth.unsqueeze(1), items[2 * b:], _OPS.depth_to_image_ragged)
+
+
+# ------------------------------------------------------------------------------------------------------ stereo scene flow
+@torch.no_grad()
+def warp_disparity(disp_next, flow):
+    """The second disparity of scene flow from device tensors a caller holds, one `um_warp_disparity` launch.
+
+    `disp_next`: [B,H,W], the disparity of left frame t+1; `flow`: planar [B,2,H,W], the optical flow from left frame t to
+    left frame t+1, in pixels at the same size.  Returns {'disp_1': [B,H,W] fp32, 'in_frame': [B,H,W] uint8}: disp_1 at pixel
+    p of frame t is the bilinear sample of disp_next at q = p + flow(p) clamped into the frame (grid_sample with
+    padding_mode='border', align_corners=True), so a point that leaves the frame takes the nearest in-frame value and the
+    map stays dense; in_frame is 1 where q lies inside [0, W-1] x [0, H-1].  fp32, with the order of operations of
+    include/unimatch_sm100.h.  No occlusion handling."""
+    if not torch.is_tensor(disp_next) or disp_next.dim() != 3:
+        raise ValueError("warp_disparity expects disparities [B,H,W]")
+    b, h, w = disp_next.shape
+    if not torch.is_tensor(flow) or tuple(flow.shape) != (b, 2, h, w):
+        raise ValueError("warp_disparity: flow must be planar [B,2,H,W] like the disparities")
+    disp1, in_frame = _OPS.warp_disparity(disp_next.float().contiguous(), flow.float().contiguous())
+    return {"disp_1": disp1, "in_frame": in_frame}
+
+
+def _stereo_quadruples(frames, name):
+    """(B, H, W) of the four device uint8 [B,H,W,3] views left0, right0, left1, right1, refused unless they agree"""
+    shape = None
+    for k, f in zip(("left0", "right0", "left1", "right1"), frames):
+        if not torch.is_tensor(f) or f.dtype != torch.uint8 or f.dim() != 4 or f.shape[-1] != 3 or f.shape[0] < 1:
+            raise ValueError("%s: %s must be uint8 frames [B,H,W,3] as decoded" % (name, k))
+        if shape is None:
+            shape = tuple(f.shape)
+        elif tuple(f.shape) != shape:
+            raise ValueError("%s: the four views must have one shape, %s is %s against %s" % (name, k, list(f.shape), list(shape)))
+    return shape[:3]
+
+
+def _flow_kwargs(flow_kwargs, name):
+    kw = _task_kwargs(flow_kwargs or {}, "flow", name)
+    for k in ("pred_bidir_flow", "fwd_bwd_consistency_check"):
+        if kw.pop(k, False):
+            raise ValueError("%s: %s is not supported (scene flow takes the forward flow only)" % (name, k))
+    return kw
+
+
+def _stereo_kwargs(stereo_kwargs, name):
+    kw = _task_kwargs(stereo_kwargs or {}, "stereo", name)
+    for k in ("pred_bidir_disp", "pred_right_disp"):
+        if kw.pop(k, False):
+            raise ValueError("%s: %s is not supported (scene flow takes the left disparity only)" % (name, k))
+    return kw
+
+
+@torch.no_grad()
+def infer_scene_flow(stereo_model, flow_model, left0, right0, left1, right1, *, stereo_kwargs=None, flow_kwargs=None,
+                     stereo_padding_factor=16, flow_padding_factor=32, stereo_inference_size=None, flow_inference_size=None):
+    """Stereo scene flow of B stereo quadruples: the disparity at time t, the disparity of the same pixels at t+1, and the
+    optical flow between the two left frames (what KITTI 2015's scene-flow benchmark scores).
+
+    `left0`, `right0` (time t) and `left1`, `right1` (time t+1) are device uint8 frames [B,H,W,3] as decoded.  Geometry is
+    that of `_stereo_from_frames` / `infer_stereo` for stereo and `infer_flow` for flow: each network resizes to a multiple of
+    its padding factor (or to its inference size), and its output is resized back and rescaled.  One stereo forward over the
+    2B pairs (left0, left1 then right0, right1), normalised on the device (`um_frames_to_planar_normalized`); one flow forward
+    on (left0, left1) (`um_frames_to_planar`); one `um_warp_disparity`.  `stereo_kwargs` / `flow_kwargs` go to the models
+    (attn_type, attn_splits_list, corr_radius_list, prop_radius_list, num_reg_refine).
+    Returns {'disp_0': [B,H,W], 'disp_1': [B,H,W], 'flow': [B,2,H,W], 'in_frame': [B,H,W] uint8} at the frames' size;
+    disp_1 and in_frame are `warp_disparity` of the disparity at t+1 and the flow."""
+    b, h, w = _stereo_quadruples((left0, right0, left1, right1), "infer_scene_flow")
+    skw, fkw = _stereo_kwargs(stereo_kwargs, "infer_scene_flow"), _flow_kwargs(flow_kwargs, "infer_scene_flow")
+    disp = _stereo_from_frames(stereo_model, torch.cat((left0, left1, right0, right1)), padding_factor=stereo_padding_factor,
+                               inference_size=stereo_inference_size, **skw)["disp"]
+    transposed, ori, size = _frame_geometry(h, w, flow_padding_factor, flow_inference_size, "flow")
+    planes = _frames_to_model(torch.cat((left0, left1)), "flow", transposed, size)
+    flow = flow_model(planes[:b], planes[b:], **fkw)["flow_preds"][-1]
+    flow = _flow_outputs(flow, ori, size, transposed, False, False)["flow"].contiguous()
+    out = {"disp_0": disp[:b].contiguous(), "flow": flow}
+    out["disp_1"], out["in_frame"] = _OPS.warp_disparity(disp[b:].contiguous(), flow)
+    return {k: out[k] for k in ("disp_0", "disp_1", "flow", "in_frame")}
+
+
+class SceneFlowRunner(_SequenceRunner):
+    """Streaming stereo scene flow over a stereo video: consecutive pairs of host (left, right) uint8 frames, each frame's
+    stereo computed once and each left frame encoded once for the flow.
+
+    * upload: each step copies `batch` NEW stereo frames in one pinned uint8 [2B,H,W,3] buffer (the B left frames, then the
+      B right ones, as `StereoRunner` packs them);
+    * device work of a step, captured once per staging slot in a CUDA graph: the stereo network on the B new pairs
+      (`_stereo_from_frames`), the flow encoder on the B new left frames and the flow matching path on the B pairs (previous
+      step's last frame, new frames) with the last pyramid carried, as `VideoFlowRunner` does, and `um_warp_disparity` of each
+      new frame's disparity through its pair's flow.  The last frame's disparity is carried to the next step as its first
+      pair's disp_0;
+    * download per consecutive pair (t, t+1): 'disp_0' [H,W] (frame t), 'disp_1' [H,W] (frame t+1's disparity in frame t's
+      grid), 'flow' [2,H,W] and 'in_frame' [H,W] uint8, 17 bytes per pixel; with `visualize` also 'vis_disp_0' / 'vis_disp_1'
+      (`disparity_to_image`, BGR) and 'vis_flow' (`flow_to_image`, RGB), painted inside the step's graph.
+
+    Sizes, semantics and keywords are those of `infer_scene_flow` (`stereo_padding_factor` / `stereo_inference_size` for
+    the stereo network, `flow_padding_factor` / `flow_inference_size` for the flow network); the outputs equal `infer_scene_flow` on the
+    consecutive quadruples up to the encoder's fp32 summation order.  One frame size per runner; a short last step is filled
+    with repeats of its last item and the extra results are dropped.  `run(items)` takes an iterable of (left, right) host
+    uint8 frames [H,W,3] and yields one dict of CPU tensors per consecutive pair (pinned staging reused -- copy what you
+    keep)."""
+
+    task = "flow"
+
+    def __init__(self, stereo_model, flow_model, frame_size, batch, device, *, stereo_kwargs=None, flow_kwargs=None,
+                 stereo_padding_factor=16, flow_padding_factor=32, stereo_inference_size=None, flow_inference_size=None,
+                 visualize=False, use_graph=True):
+        self.kw = _flow_kwargs(flow_kwargs, "SceneFlowRunner")
+        self.stereo_kw = _stereo_kwargs(stereo_kwargs, "SceneFlowRunner")
+        self.stereo_model = stereo_model
+        self.stereo_geometry = dict(padding_factor=stereo_padding_factor, inference_size=stereo_inference_size)
+        self.visualize = bool(visualize)
+        self._init_sequence(flow_model, frame_size, batch, device, use_graph, flow_padding_factor, flow_inference_size)
+        shape = (2 * self.batch, self.h, self.w, 3)
+        self.stereo_pin = [torch.empty(shape, dtype=torch.uint8).pin_memory() for _ in range(2)]
+        self.stereo_dev = [torch.empty(shape, dtype=torch.uint8, device=self.dev) for _ in range(2)]
+        self.pin = [p[:self.batch] for p in self.stereo_pin]          # the left frames, which the flow encoder reads
+        self.dev_in = [d[:self.batch] for d in self.stereo_dev]
+        self.carry_disp = torch.zeros((1, self.h, self.w), device=self.dev)
+        self.first_right = None
+
+    def _graph_models(self):
+        return (self.model, self.stereo_model)
+
+    def _item(self, item):
+        """(left, right) host uint8 frames [H,W,3] of one stereo frame"""
+        if not isinstance(item, (tuple, list)) or len(item) != 2:
+            raise ValueError("SceneFlowRunner: items are (left, right) stereo frames")
+        views = [torch.as_tensor(v) for v in item]
+        for v in views:
+            if v.dtype != torch.uint8 or tuple(v.shape) != (self.h, self.w, 3):
+                raise ValueError("SceneFlowRunner: frames must be uint8 [%d, %d, 3]" % (self.h, self.w))
+        return views
+
+    def _frame(self, item):
+        return self._item(item)[0]
+
+    def _begin(self, first):
+        self.first_right = self._item(first)[1]
+
+    def _disparity(self, frames_u8):
+        return _stereo_from_frames(self.stereo_model, frames_u8, **self.stereo_geometry, **self.stereo_kw)["disp"]
+
+    def _match(self, slot, first, second):
+        disp = self._disparity(self.stereo_dev[slot])
+        flow = self.model.forward_encoded(first, second, **self.kw)["flow_preds"][-1]
+        flow = _flow_outputs(flow, self.ori, self.size, self.transposed, False, False)["flow"].contiguous()
+        out = {"disp_0": torch.cat((self.carry_disp, disp[:-1])), "flow": flow}
+        out["disp_1"], out["in_frame"] = _OPS.warp_disparity(disp.contiguous(), flow)
+        self.carry_disp.copy_(disp[-1:])
+        if self.visualize:
+            out["vis_disp_0"], out["vis_disp_1"] = disparity_to_image(out["disp_0"]), disparity_to_image(out["disp_1"])
+            out["vis_flow"] = flow_to_image(flow)
+        return out
+
+    def _reset_inputs(self, slot):
+        self.stereo_dev[slot].zero_()
+
+    def _prime(self, frame):
+        """the first frame's pyramid and disparity (eagerly), carried into the first step"""
+        super()._prime(frame)
+        right = self.first_right.to(self.dev)[None]
+        self.carry_disp.copy_(self._disparity(torch.cat((frame, right))))
+
+    def _stage_host(self, slot, chunk):
+        """the step's left frames, then its right frames, into the pinned buffer; then their one H2D copy"""
+        for i in range(self.batch):
+            left, right = self._item(chunk[min(i, len(chunk) - 1)])
+            self.stereo_pin[slot][i].copy_(left)
+            self.stereo_pin[slot][self.batch + i].copy_(right)
+        self.stereo_dev[slot].copy_(self.stereo_pin[slot], non_blocking=True)

@@ -36,6 +36,15 @@ EVAL_FLOW_COLS = ("n", "epe", "1px", "3px", "5px", "outlier", "s0_10_n", "s0_10_
 EVAL_STEREO_COLS = ("n", "abs", "d1", "1px", "2px", "3px")
 EVAL_DEPTH_COLS = ("n", "abs_rel", "sq_rel", "sq", "log_sq", "a1", "a2", "a3")
 EVAL_COLS = {EVAL_FLOW: EVAL_FLOW_COLS, EVAL_STEREO: EVAL_STEREO_COLS, EVAL_DEPTH: EVAL_DEPTH_COLS}
+# the [B, 32] scene-flow table (include/unimatch_sm100.h, um_scene_flow_stats): column of (set, region, metric, kind)
+SF_SETS, SF_REGIONS, SF_METRICS, SF_KINDS = ("occ", "noc"), ("bg", "fg"), ("d1", "d2", "fl", "sf"), ("n", "outliers")
+SF_COLS = 32
+
+
+def sf_col(s, r, m, k):
+    """UM_SF_COL: column of set s (0 occ, 1 noc), region r (0 bg, 1 fg), metric m (0 D1, 1 D2, 2 Fl, 3 SF) and kind k
+    (0 valid pixels, 1 outliers)"""
+    return ((s * 2 + r) * 4 + m) * 2 + k
 
 
 ACT_NONE, ACT_RELU, ACT_TANH, ACT_SIGMOID, ACT_GELU = 0, 1, 2, 3, 4
@@ -84,6 +93,7 @@ class FfnDesc(ctypes.Structure):
 
 _P, _I, _L, _F = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
 _G, _FP, _RC = ctypes.POINTER(AttnGeom), ctypes.POINTER(ctypes.c_float), ctypes.c_int
+_PP = ctypes.POINTER(ctypes.c_void_p)
 
 # name -> (restype, argtypes) of every function include/unimatch_sm100.h declares
 _SIGNATURES = {
@@ -107,6 +117,8 @@ _SIGNATURES = {
     "um_track_points_forward": (_RC, [_P, _P, _I, _I, _I, _I, _P, _I, _I, _P, _P, _P, _P, _P]),
     "um_track_points_backward": (_RC, [_P, _P, _I, _I, _I, _P, _I, _I, _P, _P, _P]),
     "um_multi_flow_tracks": (_RC, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "um_warp_disparity": (_RC, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "um_scene_flow_stats": (_RC, [_P, _P, _P, _PP, _PP, _PP, _PP, _P, _I, _I, _I, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -477,6 +489,23 @@ def _multi_flow_tracks(flow, occ, err, src, dst, pos, sig, vis):
 
 multi_flow_tracks = _define("multi_flow_tracks(Tensor flow, Tensor occ, Tensor err, Tensor src, Tensor dst, Tensor(a!) pos, "
                             "Tensor(b!) sig, Tensor(c!) vis) -> (Tensor, Tensor, Tensor)", _multi_flow_tracks)
+
+
+def _warp_disparity(disp_next, flow):
+    """disp_next: contiguous fp32 [B, h, w], the disparity of left frame t+1; flow: contiguous fp32 [B, 2, h, w], left t ->
+    left t+1.  Returns (disp1 fp32 [B, h, w], in_frame uint8 [B, h, w]) (include/unimatch_sm100.h, um_warp_disparity)."""
+    _f32c(disp_next, "disp_next"), _f32c(flow, "flow")
+    if disp_next.dim() != 3 or flow.dim() != 4 or flow.shape[1] != 2 or tuple(flow.shape[2:]) != tuple(disp_next.shape[1:]) \
+            or flow.shape[0] != disp_next.shape[0] or flow.device != disp_next.device:
+        raise RuntimeError("warp_disparity: expected disp_next [B, h, w] and a planar flow [B, 2, h, w] on its device")
+    b, h, w = disp_next.shape
+    disp1 = torch.empty_like(disp_next)
+    in_frame = torch.empty((b, h, w), device=disp_next.device, dtype=torch.uint8)
+    _check(LIB.um_warp_disparity(_p(disp_next), _p(flow), _p(disp1), _p(in_frame), b, h, w, _stream()), "um_warp_disparity")
+    return disp1, in_frame
+
+
+warp_disparity = _define("warp_disparity(Tensor disp_next, Tensor flow) -> (Tensor, Tensor)", _warp_disparity)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
@@ -850,6 +879,46 @@ def _eval_stats(pred, gt, valid, noc_valid, task, mask_mode, max_val, eval_min, 
 eval_stats = _define(
     "eval_stats(Tensor pred, Tensor gt, Tensor? valid, Tensor? noc_valid, int task, int mask_mode, float max_val, "
     "float eval_min, float eval_max) -> Tensor", _eval_stats)
+
+
+def _scene_flow_stats(disp0, disp1, flow, gt_disp0, gt_disp1, gt_flow, gt_valid, noc_disp0, noc_disp1, noc_flow, noc_valid,
+                      obj_map):
+    """Predictions disp0 / disp1 [B, h, w] and flow [B, 2, h, w], the occ ground truth (disparities [B, h, w], flow
+    [B, 2, h, w], flow_valid [B, h, w]), the noc ground truth in the same shapes (all four or None) and obj_map [B, h, w] or
+    None, all contiguous fp32 on one device.  Returns the [B, SF_COLS] float64 count table (columns `sf_col`)."""
+    _f32c(disp0, "disp0")
+    if disp0.dim() != 3:
+        raise RuntimeError("scene_flow_stats: expected disparities [B, h, w]")
+    b, h, w = disp0.shape
+    noc = (noc_disp0, noc_disp1, noc_flow, noc_valid)
+    if any(t is None for t in noc) and any(t is not None for t in noc):
+        raise RuntimeError("scene_flow_stats: the noc set takes all four maps or none")
+    for t, name, shape in ((disp1, "disp1", (b, h, w)), (flow, "flow", (b, 2, h, w)), (gt_disp0, "gt_disp0", (b, h, w)),
+                           (gt_disp1, "gt_disp1", (b, h, w)), (gt_flow, "gt_flow", (b, 2, h, w)),
+                           (gt_valid, "gt_valid", (b, h, w)), (noc_disp0, "noc_disp0", (b, h, w)),
+                           (noc_disp1, "noc_disp1", (b, h, w)), (noc_flow, "noc_flow", (b, 2, h, w)),
+                           (noc_valid, "noc_valid", (b, h, w)), (obj_map, "obj_map", (b, h, w))):
+        if t is None:
+            continue
+        _f32c(t, name)
+        if tuple(t.shape) != shape or t.device != disp0.device:
+            raise RuntimeError("scene_flow_stats: %s must be %s on the predictions' device" % (name, list(shape)))
+
+    def pair(occ, noc_t):
+        return (ctypes.c_void_p * 2)(occ.data_ptr(), noc_t.data_ptr() if noc_t is not None else None)
+
+    scratch = torch.empty((b * EVAL_PARTS * SF_COLS,), device=disp0.device, dtype=torch.float64)
+    out = torch.empty((b, SF_COLS), device=disp0.device, dtype=torch.float64)
+    _check(LIB.um_scene_flow_stats(_p(disp0), _p(disp1), _p(flow), pair(gt_disp0, noc_disp0), pair(gt_disp1, noc_disp1),
+                                   pair(gt_flow, noc_flow), pair(gt_valid, noc_valid), _p(obj_map), b, h, w, _p(scratch),
+                                   _p(out), _stream()), "um_scene_flow_stats")
+    return out
+
+
+scene_flow_stats = _define(
+    "scene_flow_stats(Tensor disp0, Tensor disp1, Tensor flow, Tensor gt_disp0, Tensor gt_disp1, Tensor gt_flow, "
+    "Tensor gt_valid, Tensor? noc_disp0, Tensor? noc_disp1, Tensor? noc_flow, Tensor? noc_valid, Tensor? obj_map) -> Tensor",
+    _scene_flow_stats)
 
 
 # ---- tensor-core convolution / Linear ---------------------------------------------------------------------------

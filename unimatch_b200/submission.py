@@ -2,7 +2,8 @@
 batches, with each file's payload encoded on the device and the files written by a pool of host threads.
 
 `create_flow_submission` writes Sintel `.flo` files and KITTI 16-bit flow PNGs, `create_stereo_submission` KITTI 16-bit
-disparity PNGs and ETH3D / Middlebury `.pfm` files with their runtime files, in the reference's directory layout.  Samples
+disparity PNGs and ETH3D / Middlebury `.pfm` files with their runtime files, in the reference's directory layout.
+`create_scene_flow_submission` writes KITTI 2015's scene-flow layout (`disp_0/`, `disp_1/`, `flow/`) from `infer_scene_flow`.  Samples
 of equal size are grouped into batches of `batch` (one open batch per size, flushed when full and at the end, as the
 validation drivers do), padded with the reference's `InputPadder` mode or resized to `inference_size`, and run through the
 model.  One `um_encode_submission` launch per batch turns the model's output into every sample's file payload: the unpad
@@ -27,7 +28,7 @@ import torch
 
 from . import ops
 from .evaluation import _upload
-from .inference import InputPadder, _batches, _resize, disparity_to_image, flow_to_image
+from .inference import InputPadder, _batches, _resize, _stereo_quadruples, disparity_to_image, flow_to_image, infer_scene_flow
 
 _OPS = torch.ops.unimatch_sm100
 
@@ -361,3 +362,55 @@ def create_stereo_submission(model, dataset, *, protocol, output_path, batch=8, 
                 pool.submit(slot, ready, _write_runtime, os.path.join(d, "timeGMStereo.txt"), "", timer, n)
 
     return _run_batches(_batches(dataset, batch, lambda s: tuple(np.shape(s["left"]))), writers, device, run)
+
+
+SCENE_FLOW_VIEWS = ("left0", "right0", "left1", "right1")
+
+
+def scene_flow_name(sample, index):
+    """The file name (without '.png') of scene-flow sample `index`: its 'name', or KITTI's '%06d_10' numbering."""
+    name = sample.get("name") if isinstance(sample, dict) else None
+    return str(name) if name is not None else "%06d_10" % index
+
+
+@torch.no_grad()
+def create_scene_flow_submission(stereo_model, flow_model, dataset, *, output_path, batch=8, writers=8, device="cuda",
+                                 stereo_kwargs=None, flow_kwargs=None, stereo_padding_factor=16, flow_padding_factor=32,
+                                 stereo_inference_size=None, flow_inference_size=None):
+    """KITTI 2015's scene-flow submission of `infer_scene_flow` on `dataset`: `output_path/disp_0/<name>.png`,
+    `disp_1/<name>.png` (16-bit disparity PNGs, uint16(256 d)) and `flow/<name>.png` (16-bit flow PNGs, 64 u + 32768,
+    64 v + 32768, valid = 1).  Samples are dicts with uint8 'left0', 'right0', 'left1', 'right1' [H,W,3] and an optional
+    'name' (default '%06d_10' of the sample's index).  The files hold exactly what `infer_scene_flow` returns at the
+    frames' size (its geometry, keywords as there): disp_1 is dense, a point that leaves the frame taking the nearest
+    in-frame disparity.  Samples of one size form batches of `batch`; one `um_encode_submission` launch per file kind turns
+    a batch's outputs into the PNG scanlines, which are the only download; `writers` threads deflate and write them.
+    Returns {'samples', 'batches', 'd2h_bytes', 'writer_seconds'}."""
+    device = torch.device(device)
+    for d in ("disp_0", "disp_1", "flow"):
+        os.makedirs(os.path.join(output_path, d), exist_ok=True)
+
+    def shape_of(item):
+        i, s = item
+        if not isinstance(s, dict) or any(k not in s for k in SCENE_FLOW_VIEWS):
+            raise ValueError("create_scene_flow_submission: sample %d needs %s" % (i, list(SCENE_FLOW_VIEWS)))
+        return tuple(np.shape(s["left0"]))
+
+    def run(pool, items):
+        views = [torch.stack([torch.as_tensor(s[k]) for _, s in items]) for k in SCENE_FLOW_VIEWS]
+        views = [v.pin_memory().to(device, non_blocking=True) if device.type == "cuda" else v.to(device) for v in views]
+        n, h, w = _stereo_quadruples(views, "create_scene_flow_submission")
+        out = infer_scene_flow(stereo_model, flow_model, *views, stereo_kwargs=stereo_kwargs, flow_kwargs=flow_kwargs,
+                               stereo_padding_factor=stereo_padding_factor, flow_padding_factor=flow_padding_factor,
+                               stereo_inference_size=stereo_inference_size, flow_inference_size=flow_inference_size)
+        crop = (False, 0, 0)
+        payload = {"disp_0": _encode(out["disp_0"].unsqueeze(1), ops.SUBMIT_KITTI_DISP_PNG, (h, w), crop),
+                   "disp_1": _encode(out["disp_1"].unsqueeze(1), ops.SUBMIT_KITTI_DISP_PNG, (h, w), crop),
+                   "flow": _encode(out["flow"], ops.SUBMIT_KITTI_FLOW_PNG, (h, w), crop)}
+        slot, host, ready = pool.stage(payload)
+        for j, (i, s) in enumerate(items):
+            name = scene_flow_name(s, i) + ".png"
+            for kind, colour_type in (("disp_0", 0), ("disp_1", 0), ("flow", 2)):
+                pool.submit(slot, ready, _write_png, os.path.join(output_path, kind, name), host[kind][j], h, w, 16,
+                            colour_type)
+
+    return _run_batches(_batches(enumerate(dataset), batch, shape_of), writers, device, run)

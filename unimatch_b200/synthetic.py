@@ -146,6 +146,24 @@ def synthetic_stereo_frames(n, h, w, seed=1234):
     return torch.stack(lefts, 0).contiguous(), torch.stack(rights, 0).contiguous()
 
 
+def synthetic_stereo_video(T, h, w, seed=1234, step=3):
+    """A rectified stereo clip as decoded: left and right uint8 frames [T,H,W,3] (channel-last).  The left view is
+    `synthetic_video`'s moving crops of one box-blurred noise canvas; the right view is each left crop shifted by a seeded
+    whole-pixel disparity in [0, 32] of the whole clip (a fronto-parallel scene: disparity d everywhere, in every frame)."""
+    g = torch.Generator().manual_seed(seed)
+    m, d_max = step * max(T - 1, 0) + 1, 32
+    canvas = _texture(g, h + 2 * m, w + 2 * m + d_max)[0].round().clamp(0, 255).to(torch.uint8).permute(1, 2, 0)
+    moves = torch.randint(-step, step + 1, (max(T - 1, 0), 2), generator=g)
+    d = int(torch.randint(0, d_max + 1, (1,), generator=g))
+    y, x = m, m + d_max
+    lefts, rights = [], []
+    for dy, dx in [(0, 0)] + moves.tolist():
+        y, x = y + dy, x + dx
+        lefts.append(canvas[y:y + h, x:x + w])
+        rights.append(canvas[y:y + h, x - d:x - d + w])         # right view = left shifted by +d px
+    return torch.stack(lefts, 0).contiguous(), torch.stack(rights, 0).contiguous()
+
+
 def synthetic_posed_sequence(T, h, w, seed=1234, step=3, plane_depth=2.0):
     """A posed frame sequence for depth inference: T frames uint8 [T,H,W,3] of a fronto-parallel textured plane at depth
     `plane_depth`, the intrinsics K [3,3] (focal 0.9 W, centred principal point) and the absolute camera-to-world poses
