@@ -30,7 +30,8 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics) leave existing callers working and keep it. */
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion) leave existing callers working and
+ * keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
@@ -408,6 +409,46 @@ int um_scene_flow_stats(const float* disp0, const float* disp1, const float* flo
                         const float* const* gt_disp1, const float* const* gt_flow, const float* const* gt_flow_valid,
                         const float* obj_map, int32_t batch, int32_t h, int32_t w, double* scratch, double* out,
                         void* stream);
+
+/* ---- TSDF fusion of posed depth maps ---------------------------------------------------------------------------------
+ * A dense volume of X x Y x Z voxels (x fastest, at most 2^31 - 1 voxels, N = X Y Z), 20 bytes per voxel in three
+ * contiguous fp32 planes: tsdf [Z, Y, X], weight [Z, Y, X] and color [3, Z, Y, X] (R, G, B; channel offsets are 64-bit).
+ * origin is a HOST array of 3 floats; the centre of voxel (i, j, k) is, per axis, p = fma(idx + 0.5f, voxel_size, origin)
+ * (idx + 0.5f rounded first).  A zeroed volume is empty (weight 0 = never observed).
+ *
+ * Integration: depth [n, h, w] fp32 (metric z-depth), frames [n, h, w, 3] uint8 RGB at the same size, w2c [n, 3, 4] fp32
+ * row-major world-to-camera matrices M, and a DEVICE int32 n_valid: only frames 0 .. min(max(n_valid, 0), n) - 1 are
+ * fused, so one captured CUDA graph serves a short last step.  One thread per voxel walks those frames in order; per
+ * frame, in fp32 with every operation rounded on its own (__fmaf_rn, __fdiv_rn, ...):
+ *   c.x = fma(M02, p.z, fma(M01, p.y, fma(M00, p.x, M03))), likewise c.y (row 1) and c.z (row 2);  skip unless c.z > 0;
+ *   u = fma(fx, c.x / c.z, cx),  v = fma(fy, c.y / c.z, cy);  xi = floor(u + 0.5f), yi = floor(v + 0.5f);
+ *   skip unless 0 <= xi < w and 0 <= yi < h (a NaN is skipped);  d = depth[t, yi, xi];  skip unless d is finite and d > 0;
+ *   sdf = d - c.z;  skip if sdf < -trunc;  f = fminf(1, sdf / trunc);
+ *   W' = W + 1;  F' = fma(F, W, f) / W';  each colour channel C' = fma(C, W, frames[t, yi, xi, ch]) / W';  W = W'.
+ * The voxel's state is read at its first update and written once after its last, so voxels no frame reaches move no
+ * state bytes.  Because each voxel sees its frames in order, fusing frames in one launch or split over several gives the
+ * same volume bit for bit.  No atomics, no host synchronisation (graph-capturable).  voxel_size and trunc > 0 and finite;
+ * the volume planes overlap each other and the inputs nowhere; all fp32 buffers 4-byte aligned. */
+#define UM_TSDF_THREADS 256
+int um_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t X, int32_t Y, int32_t Z, const float* origin,
+                      float voxel_size, float trunc, const float* depth, const uint8_t* frames, const float* w2c, int32_t n,
+                      int32_t h, int32_t w, float fx, float fy, float cx, float cy, const int32_t* n_valid, void* stream);
+
+/* Surface extraction: the zero-crossing vertices of marching cubes, as coloured points.  Each voxel owns its +x, +y and +z
+ * edges that lie inside the grid; the edge from voxel 0 to voxel 1 emits a point iff weight0 > 0, weight1 > 0 and
+ * (F0 < 0) != (F1 < 0).  With s = F0 / (F0 - F1) the point is voxel 0's centre with fma(s, voxel_size, p0) on the edge's
+ * axis, and its colour per channel is __float2int_rn(fma(s, C1 - C0, C0)) clamped to 0..255.  Points are ordered by voxel
+ * linear index, then edge axis x, y, z.
+ * um_tsdf_surface_count writes offsets [nb + 1] (DEVICE int64, nb = ceil(N / UM_TSDF_THREADS)): offsets[b] the first
+ * point of block b (voxels b * UM_TSDF_THREADS ...), offsets[nb] the total P, which the caller reads to allocate
+ * points [P, 3] fp32 and colors [P, 3] uint8; um_tsdf_surface_points (n_points = P) then writes them, and with P = 0
+ * launches nothing.  A count pass, one ordered scan of
+ * the block counts and a write pass: no atomics, the output is the same from run to run. */
+int um_tsdf_surface_count(const float* tsdf, const float* weight, int32_t X, int32_t Y, int32_t Z, int64_t* offsets,
+                          void* stream);
+int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                           const float* origin, float voxel_size, const int64_t* offsets, int64_t n_points, float* points,
+                           uint8_t* colors, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

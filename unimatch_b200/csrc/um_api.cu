@@ -1,5 +1,6 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
-// between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu).  See include/unimatch_sm100.h.
+// between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu),
+// and TSDF fusion (um_fusion.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -50,6 +51,14 @@ int multi_flow_tracks_launch(const float* flow, const float* occ, const float* e
                              uint8_t* visible, float* sigma, cudaStream_t st);
 int warp_disparity_launch(const float* disp_next, const float* flow, float* disp1, uint8_t* in_frame, int batch, int h, int w,
                           cudaStream_t st);
+int tsdf_integrate_launch(float* tsdf, float* weight, float* color, int X, int Y, int Z, const float* origin,
+                          float voxel_size, float trunc, const float* depth, const uint8_t* frames, const float* w2c, int n,
+                          int h, int w, float fx, float fy, float cx, float cy, const int* n_valid, cudaStream_t st);
+int tsdf_surface_count_launch(const float* tsdf, const float* weight, int X, int Y, int Z, long long* offsets,
+                              cudaStream_t st);
+int tsdf_surface_points_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z,
+                               const float* origin, float voxel_size, const long long* offsets, float* points,
+                               uint8_t* colors, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -262,6 +271,68 @@ int um_warp_disparity(const float* disp_next, const float* flow, float* disp1, u
   UM_REQUIRE(um::written_disjoint({{disp1, 4 * n}, {in_frame, n}, {disp_next, 4 * n}, {flow, 8 * n}}, 2),
              "um_warp_disparity: disp1 and in_frame must not overlap each other or the inputs");
   return um::warp_disparity_launch(disp_next, flow, disp1, in_frame, batch, h, w, (cudaStream_t)stream);
+}
+
+// A TSDF volume of X x Y x Z voxels: every dimension positive, at most 2^31 - 1 voxels in all.
+static bool tsdf_dims(int32_t X, int32_t Y, int32_t Z) {
+  return X > 0 && Y > 0 && Z > 0 && (long long)X * Y * Z <= 0x7fffffffLL;
+}
+
+static bool positive_finite(float v) { return v > 0.f && v <= 3.402823466e38f; }
+
+int um_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t X, int32_t Y, int32_t Z, const float* origin,
+                      float voxel_size, float trunc, const float* depth, const uint8_t* frames, const float* w2c, int32_t n,
+                      int32_t h, int32_t w, float fx, float fy, float cx, float cy, const int32_t* n_valid, void* stream) {
+  UM_REQUIRE(tsdf && weight && color && origin && depth && frames && w2c && n_valid,
+             "um_tsdf_integrate: no pointer may be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_integrate: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(positive_finite(voxel_size) && positive_finite(trunc),
+             "um_tsdf_integrate: voxel_size and trunc must be positive and finite");
+  UM_REQUIRE(n > 0 && h > 0 && w > 0 && (long long)h * w <= 0x7fffffffLL, "um_tsdf_integrate: bad frames (%d x %d x %d)",
+             n, h, w);
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(color, 4) && um::aligned(depth, 4) &&
+                 um::aligned(w2c, 4) && um::aligned(n_valid, 4),
+             "um_tsdf_integrate: the fp32 and int32 buffers must be 4-byte aligned");
+  const long long nv = (long long)X * Y * Z, px = (long long)n * h * w;
+  UM_REQUIRE(um::written_disjoint({{tsdf, 4 * nv}, {weight, 4 * nv}, {color, 12 * nv}, {depth, 4 * px}, {frames, 3 * px},
+                                   {w2c, 48LL * n}, {n_valid, 4}},
+                                  3),
+             "um_tsdf_integrate: the volume planes must not overlap each other or the inputs");
+  return um::tsdf_integrate_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size, trunc, depth, frames, w2c, n, h, w, fx,
+                                   fy, cx, cy, n_valid, (cudaStream_t)stream);
+}
+
+int um_tsdf_surface_count(const float* tsdf, const float* weight, int32_t X, int32_t Y, int32_t Z, int64_t* offsets,
+                          void* stream) {
+  UM_REQUIRE(tsdf && weight && offsets, "um_tsdf_surface_count: no pointer may be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_surface_count: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(offsets, 8),
+             "um_tsdf_surface_count: tsdf and weight must be 4-byte aligned, offsets 8-byte aligned");
+  const long long nv = (long long)X * Y * Z, nb = (nv + UM_TSDF_THREADS - 1) / UM_TSDF_THREADS;
+  UM_REQUIRE(um::written_disjoint({{offsets, 8 * (nb + 1)}, {tsdf, 4 * nv}, {weight, 4 * nv}}, 1),
+             "um_tsdf_surface_count: offsets must not overlap the volume");
+  return um::tsdf_surface_count_launch(tsdf, weight, X, Y, Z, reinterpret_cast<long long*>(offsets), (cudaStream_t)stream);
+}
+
+int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                           const float* origin, float voxel_size, const int64_t* offsets, int64_t n_points, float* points,
+                           uint8_t* colors, void* stream) {
+  UM_REQUIRE(tsdf && weight && color && origin && offsets, "um_tsdf_surface_points: no input may be NULL");
+  UM_REQUIRE(n_points == 0 || (points && colors), "um_tsdf_surface_points: points and colors must not be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_surface_points: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(positive_finite(voxel_size), "um_tsdf_surface_points: voxel_size must be positive and finite");
+  const long long nv = (long long)X * Y * Z, nb = (nv + UM_TSDF_THREADS - 1) / UM_TSDF_THREADS;
+  UM_REQUIRE(n_points >= 0 && n_points <= 3 * nv, "um_tsdf_surface_points: bad point count %lld", (long long)n_points);
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(color, 4) && um::aligned(offsets, 8) &&
+                 um::aligned(points, 4),
+             "um_tsdf_surface_points: tsdf, weight, color and points must be 4-byte aligned, offsets 8-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{points, 12 * n_points}, {colors, 3 * n_points}, {tsdf, 4 * nv}, {weight, 4 * nv},
+                                   {color, 12 * nv}, {offsets, 8 * (nb + 1)}},
+                                  2),
+             "um_tsdf_surface_points: points and colors must not overlap each other, the volume or the offsets");
+  if (n_points == 0) return UM_OK;
+  return um::tsdf_surface_points_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size,
+                                        reinterpret_cast<const long long*>(offsets), points, colors, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,0 +1,153 @@
+"""TSDF fusion of posed depth maps on the device: a dense truncated-signed-distance volume (`TSDFVolume`), the integration of
+device depths and frames into it (`fuse_depths`, one `um_tsdf_integrate` launch), the zero-crossing points of its surface
+with their colours (`TSDFVolume.extract_points`) and a binary PLY writer for them (`write_ply`).  The kernels' arithmetic
+is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
+each step's CUDA graph."""
+import math
+
+import numpy as np
+import torch
+
+from .inference import _OPS, _intrinsics33, _pose44, _world_to_camera
+
+MAX_VOXELS = 2 ** 31 - 1
+
+
+def _f32(v):
+    """A Python float that is exactly the float32 the kernels receive"""
+    return float(np.float32(v))
+
+
+class TSDFVolume:
+    """A dense TSDF volume of dims = (X, Y, Z) voxels of `voxel_size` metres (x fastest), whose low corner is `origin`: voxel
+    (i, j, k) is centred at origin + (idx + 0.5) * voxel_size per axis.  Device planes, zeroed (empty): `tsdf` and `weight`
+    fp32 [Z, Y, X] and `color` fp32 [3, Z, Y, X] (RGB in 0..255), 20 bytes per voxel.  `trunc` (metres, default 4 voxel
+    sizes) is the truncation distance: the stored value is min(1, sdf / trunc), and a voxel more than `trunc` behind the
+    observed surface is not updated.  At most 2^31 - 1 voxels."""
+
+    def __init__(self, origin, voxel_size, dims, trunc=None, device="cuda"):
+        dims = tuple(int(d) for d in dims)
+        if len(dims) != 3 or min(dims) < 1:
+            raise ValueError("TSDFVolume: dims must be three positive voxel counts (X, Y, Z)")
+        if math.prod(dims) > MAX_VOXELS:
+            raise ValueError("TSDFVolume: %d x %d x %d voxels is more than 2^31 - 1" % dims)
+        if not (math.isfinite(voxel_size) and voxel_size > 0):
+            raise ValueError("TSDFVolume: voxel_size must be positive and finite")
+        trunc = 4.0 * _f32(voxel_size) if trunc is None else trunc
+        if not (math.isfinite(trunc) and trunc > 0):
+            raise ValueError("TSDFVolume: trunc must be positive and finite")
+        origin = [float(o) for o in origin]
+        if len(origin) != 3 or not all(math.isfinite(o) for o in origin):
+            raise ValueError("TSDFVolume: origin must be three finite coordinates")
+        self.origin = [_f32(o) for o in origin]
+        self.voxel_size, self.trunc, self.dims = _f32(voxel_size), _f32(trunc), dims
+        if torch.device(device).type != "cuda":
+            raise ValueError("TSDFVolume: the volume lives on a CUDA device")
+        X, Y, Z = dims
+        self.tsdf = torch.zeros((Z, Y, X), dtype=torch.float32, device=device)
+        self.weight = torch.zeros((Z, Y, X), dtype=torch.float32, device=device)
+        self.color = torch.zeros((3, Z, Y, X), dtype=torch.float32, device=device)
+        self.device = self.tsdf.device                   # with its index, as tensors on it report it
+
+    @classmethod
+    def covering(cls, intrinsics, poses, frame_size, max_depth, voxel_size, trunc=None, device="cuda"):
+        """The volume over the axis-aligned box of the cameras' view frusta from depth 0 to `max_depth`, padded by `trunc`
+        (default 4 voxel sizes) on every side: intrinsics [3,3] at `frame_size` = (H, W), host camera-to-world poses
+        [N,4,4] (see `covering_box`)."""
+        origin, dims, trunc = covering_box(intrinsics, poses, frame_size, max_depth, voxel_size, trunc)
+        return cls(origin, voxel_size, dims, trunc=trunc, device=device)
+
+    def reset(self):
+        """Empty the volume (every plane zeroed)"""
+        self.tsdf.zero_(), self.weight.zero_(), self.color.zero_()
+
+    def extract_points(self):
+        """The zero-crossing vertices of marching cubes on the observed voxels: points fp32 [P,3] (world coordinates) and
+        their colours uint8 [P,3], on the device, ordered by voxel index, then edge axis x, y, z.  One count pass, one scan,
+        one read of the count P by the host, one write pass; the result is the same from run to run."""
+        with torch.cuda.device(self.device):
+            offsets = _OPS.tsdf_surface_count(self.tsdf, self.weight)
+            n = int(offsets[-1].item())
+            return _OPS.tsdf_surface_points(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, offsets, n)
+
+    def _integrate(self, depths, frames, w2c, n_valid, K):
+        """One um_tsdf_integrate launch: frames 0 .. n_valid - 1 of device depths [n,H,W] and uint8 frames [n,H,W,3] with
+        their world-to-camera rows w2c [n,3,4] (device fp32) and the float32 intrinsics K [3,3] (host)."""
+        _OPS.tsdf_integrate(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, self.trunc, depths, frames, w2c,
+                            float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), n_valid)
+
+
+def covering_box(intrinsics, poses, frame_size, max_depth, voxel_size, trunc=None):
+    """(origin, dims, trunc) of `TSDFVolume.covering`: the axis-aligned box of every camera's frustum apex and the four far
+    corners of its frame (pixel corners (0, 0) .. (W, H) at depth `max_depth`), in float64, padded by `trunc` on every
+    side; origin is the box's low corner and dims = ceil(extent / voxel_size) per axis, so the voxels cover the box."""
+    K = _intrinsics33(intrinsics, "TSDFVolume.covering").double().numpy()
+    ps = [_pose44(p, "TSDFVolume.covering").astype(np.float64) for p in poses]
+    if not ps:
+        raise ValueError("TSDFVolume.covering: no poses")
+    if not (math.isfinite(max_depth) and max_depth > 0):
+        raise ValueError("TSDFVolume.covering: max_depth must be positive and finite")
+    if not (math.isfinite(voxel_size) and voxel_size > 0):
+        raise ValueError("TSDFVolume.covering: voxel_size must be positive and finite")
+    trunc = 4.0 * _f32(voxel_size) if trunc is None else float(trunc)
+    h, w = frame_size
+    corners = np.array([[0.0, 0.0], [w, 0.0], [0.0, h], [w, h]])
+    z = float(max_depth)
+    far = np.stack([(corners[:, 0] - K[0, 2]) / K[0, 0] * z, (corners[:, 1] - K[1, 2]) / K[1, 1] * z, np.full(4, z)], 1)
+    cam = np.concatenate([np.zeros((1, 3)), far], 0)                      # apex and the four far corners
+    pts = np.concatenate([cam @ p[:3, :3].T + p[:3, 3] for p in ps], 0)
+    lo, hi = pts.min(0) - trunc, pts.max(0) + trunc
+    dims = tuple(max(1, int(math.ceil((b - a) / voxel_size))) for a, b in zip(lo, hi))
+    return lo.tolist(), dims, trunc
+
+
+def _check_fusion_inputs(volume, depths, frames, name):
+    if not isinstance(volume, TSDFVolume):
+        raise ValueError("%s: volume must be a TSDFVolume" % name)
+    if not (torch.is_tensor(depths) and depths.is_cuda and depths.dtype == torch.float32 and depths.dim() == 3):
+        raise ValueError("%s: depths must be a device float32 tensor [N,H,W]" % name)
+    if not (torch.is_tensor(frames) and frames.is_cuda and frames.dtype == torch.uint8
+            and tuple(frames.shape) == tuple(depths.shape) + (3,)):
+        raise ValueError("%s: frames must be device uint8 [N,H,W,3] at the depths' size" % name)
+    if depths.device != volume.device or frames.device != volume.device:
+        raise ValueError("%s: depths and frames must be on the volume's device" % name)
+
+
+@torch.no_grad()
+def fuse_depths(volume, depths, frames, intrinsics, poses):
+    """Integrate N posed depth maps into `volume` with one `um_tsdf_integrate` launch: device depths [N,H,W] (metric, as
+    `infer_depth_sequence` returns them; zero, negative and non-finite depths are skipped), device uint8 frames [N,H,W,3]
+    (as `infer_depth_sequence` takes them), the intrinsics [3,3] at the frames' size and the host camera-to-world poses
+    [N,4,4].  Each voxel takes the frames in order and the nearest pixel of each, so fusing a sequence in one call or in
+    pieces gives the same volume bit for bit.  Returns the volume."""
+    _check_fusion_inputs(volume, depths, frames, "fuse_depths")
+    n = depths.shape[0]
+    if len(poses) != n:
+        raise ValueError("fuse_depths: %d depth maps need %d poses, got %d" % (n, n, len(poses)))
+    if n == 0:
+        return volume
+    K = _intrinsics33(intrinsics, "fuse_depths")
+    w2c = _world_to_camera([_pose44(p, "fuse_depths") for p in poses])
+    with torch.cuda.device(volume.device):
+        w2c_dev = torch.from_numpy(w2c).to(volume.device)
+        n_valid = torch.full((1,), n, dtype=torch.int32, device=volume.device)
+        volume._integrate(depths.contiguous(), frames.contiguous(), w2c_dev, n_valid, K)
+    return volume
+
+
+def write_ply(path, points, colors):
+    """A binary little-endian PLY of P coloured points: float x, y, z and uchar red, green, blue per vertex.  `points`
+    [P,3] and `colors` [P,3] uint8 are tensors (any device) or numpy arrays."""
+    pts = (points.detach().cpu().numpy() if torch.is_tensor(points) else np.asarray(points)).astype("<f4", copy=False)
+    col = colors.detach().cpu().numpy() if torch.is_tensor(colors) else np.asarray(colors)
+    if pts.ndim != 2 or pts.shape[1] != 3 or col.shape != pts.shape or col.dtype != np.uint8:
+        raise ValueError("write_ply: expected points [P,3] and uint8 colors [P,3]")
+    vertex = np.empty(len(pts), dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"),
+                                       ("blue", "u1")])
+    vertex["x"], vertex["y"], vertex["z"] = pts[:, 0], pts[:, 1], pts[:, 2]
+    vertex["red"], vertex["green"], vertex["blue"] = col[:, 0], col[:, 1], col[:, 2]
+    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
+              "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % len(pts))
+    with open(path, "wb") as f:
+        f.write(header.encode("ascii"))
+        f.write(vertex.tobytes())

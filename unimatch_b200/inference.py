@@ -429,6 +429,12 @@ def _relative_poses(poses, bidir):
     return _with_inverses([np.linalg.inv(poses[t + 1]) @ poses[t] for t in range(len(poses) - 1)], bidir)
 
 
+def _world_to_camera(poses):
+    """World-to-camera matrices of absolute float32 camera-to-world poses [4,4]: np.linalg.inv(pose) in numpy float32, the
+    path `_relative_poses` takes, as the float32 [n,3,4] rows `um_tsdf_integrate` reads."""
+    return np.ascontiguousarray(np.stack([np.linalg.inv(p) for p in poses]).astype(np.float32)[:, :3])
+
+
 def _with_inverses(rel, bidir):
     """Relative poses [4,4] stacked as float32 [n,4,4], followed with `bidir` by their inverses (np.linalg.inv)."""
     if bidir:
@@ -1784,8 +1790,81 @@ class DepthSequenceRunner(_PosedDepth, _SequenceRunner):
     def _stage_host(self, slot, chunk):
         """the frames, then the relative poses of the step's pairs, continuing from the carried pose"""
         poses = [self.prev_pose] + [_pose44(pose, "DepthSequenceRunner") for _, pose in super()._stage_host(slot, chunk)]
-        self._stage_poses(slot, _relative_poses(poses, self.bidir))
+        self._stage_step_poses(slot, poses, len(chunk))
         self.prev_pose = poses[-1]
+
+    def _stage_step_poses(self, slot, poses, n_real):
+        """the step's batch + 1 absolute poses (the carried one first; `n_real` real pairs) -> its relative poses"""
+        self._stage_poses(slot, _relative_poses(poses, self.bidir))
+
+
+class DepthFusionRunner(DepthSequenceRunner):
+    """`DepthSequenceRunner` that also fuses each pair's depth into a TSDF volume on the device (`fusion.TSDFVolume`), inside
+    the step's CUDA graph: after the depth of a step, one `um_tsdf_integrate` launch over its pairs' first frames t, with
+    the depth of frame t from pair (t, t+1), frame t's uint8 colours and its world-to-camera matrix.  The result is
+    `fuse_depths(volume, depths, frames, intrinsics, poses)` on the runner's own depths, bit for bit.
+
+    * frames t of a step are the carried previous frame and the new frames but the last: the runner keeps a device uint8
+      copy of the last frame next to the carried pyramid;
+    * the world-to-camera matrices (`_world_to_camera`, the host path of `fuse_depths`) and the number of real pairs are
+      staged with the relative poses, so the padding pairs of a short last step and the warm-up runs before a graph
+      capture (reset inputs: no pair) fuse nothing;
+    * only 'depth' is fused, so the last frame of a `run()` is not; `pred_bidir_depth` is refused, because the backward
+      depth of frame t+1 would count frame t+1 twice;
+    * the volume persists across `run()` calls, so a long scene can be fed in pieces (each piece's last frame is not fused);
+    * `return_depth=False` without `visualize` is allowed: the volume is the result, and `run()` then yields empty dicts
+      and downloads nothing.
+    The intrinsics are those of the frames' size, as for `DepthSequenceRunner`."""
+
+    def __init__(self, model, frame_size, batch, device, intrinsics, volume, padding_factor=16, inference_size=None,
+                 min_depth=0.5, max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
+                 use_graph=True, visualize=False, return_depth=True, **model_kwargs):
+        from .fusion import TSDFVolume
+        if pred_bidir_depth:
+            raise ValueError("DepthFusionRunner: pred_bidir_depth is refused: the backward depth of frame t+1 would fuse "
+                             "frame t+1 twice")
+        if not isinstance(volume, TSDFVolume):
+            raise ValueError("DepthFusionRunner: volume must be a TSDFVolume")
+        dev = torch.device(device)
+        if dev.type != "cuda" or (dev.index if dev.index is not None else torch.cuda.current_device()) != volume.device.index:
+            raise ValueError("DepthFusionRunner: the volume must be on the runner's device")
+        super().__init__(model, frame_size, batch, device, intrinsics, padding_factor=padding_factor,
+                         inference_size=inference_size, min_depth=min_depth, max_depth=max_depth,
+                         num_depth_candidates=num_depth_candidates, depth_from_argmax=depth_from_argmax,
+                         use_graph=use_graph, visualize=visualize, return_depth=True, **model_kwargs)
+        self.return_depth = bool(return_depth)
+        self.volume = volume
+        self.K = _intrinsics33(intrinsics, "DepthFusionRunner")
+        self.carry_frame = torch.zeros((1, self.h, self.w, 3), dtype=torch.uint8, device=self.dev)
+        self.w2c_pin = [torch.empty((self.batch, 3, 4)).pin_memory() for _ in range(2)]
+        self.w2c_dev = [torch.zeros((self.batch, 3, 4), device=self.dev) for _ in range(2)]
+        self.nvalid_pin = [torch.zeros((1,), dtype=torch.int32).pin_memory() for _ in range(2)]
+        self.nvalid_dev = [torch.zeros((1,), dtype=torch.int32, device=self.dev) for _ in range(2)]
+
+    def _match(self, slot, first, second):
+        out = _depth_outputs(self._depth(slot, first, second), self.ori, self.size, False)
+        frames = torch.cat((self.carry_frame, self.dev_in[slot][:-1]), dim=0)        # frame t of every pair
+        self.volume._integrate(out["depth"].contiguous(), frames, self.w2c_dev[slot], self.nvalid_dev[slot], self.K)
+        self.carry_frame.copy_(self.dev_in[slot][-1:])
+        if self.visualize:
+            return _colour_outputs(out, "depth", depth_to_image, self.return_depth)
+        return out if self.return_depth else {}
+
+    def _prime(self, frame):
+        super()._prime(frame)
+        self.carry_frame.copy_(frame)
+
+    def _reset_inputs(self, slot):
+        super()._reset_inputs(slot)
+        self.nvalid_dev[slot].zero_()
+
+    def _stage_step_poses(self, slot, poses, n_real):
+        """the relative poses, then the world-to-camera rows of the pairs' frames t and the number of real pairs"""
+        super()._stage_step_poses(slot, poses, n_real)
+        self.w2c_pin[slot].copy_(torch.from_numpy(_world_to_camera(poses[:-1])))
+        self.nvalid_pin[slot][0] = n_real
+        self.w2c_dev[slot].copy_(self.w2c_pin[slot], non_blocking=True)
+        self.nvalid_dev[slot].copy_(self.nvalid_pin[slot], non_blocking=True)
 
 
 def _depth_step_layout(sizes, batch, pred_bidir_depth):

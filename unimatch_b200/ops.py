@@ -119,6 +119,9 @@ _SIGNATURES = {
     "um_multi_flow_tracks": (_RC, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "um_warp_disparity": (_RC, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "um_scene_flow_stats": (_RC, [_P, _P, _P, _PP, _PP, _PP, _PP, _P, _I, _I, _I, _P, _P, _P]),
+    "um_tsdf_integrate": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _F, _P, _P, _P, _I, _I, _I, _F, _F, _F, _F, _P, _P]),
+    "um_tsdf_surface_count": (_RC, [_P, _P, _I, _I, _I, _P, _P]),
+    "um_tsdf_surface_points": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -506,6 +509,88 @@ def _warp_disparity(disp_next, flow):
 
 
 warp_disparity = _define("warp_disparity(Tensor disp_next, Tensor flow) -> (Tensor, Tensor)", _warp_disparity)
+
+
+# ---- TSDF fusion (include/unimatch_sm100.h, um_tsdf_*) -------------------------------------------------------------
+TSDF_THREADS = 256                                   # UM_TSDF_THREADS: voxels per block of the extraction's offsets
+
+
+def _tsdf_volume(tsdf, weight, color, name):
+    """The volume planes tsdf / weight [Z, Y, X] and color [3, Z, Y, X], contiguous fp32 on one device -> (X, Y, Z)"""
+    for t, n in ((tsdf, "tsdf"), (weight, "weight"), (color, "color")):
+        _f32c(t, "%s: %s" % (name, n))
+    if tsdf.dim() != 3 or tuple(weight.shape) != tuple(tsdf.shape) or tuple(color.shape) != (3,) + tuple(tsdf.shape) \
+            or weight.device != tsdf.device or color.device != tsdf.device:
+        raise RuntimeError("%s: expected tsdf and weight [Z, Y, X] and color [3, Z, Y, X] on one device" % name)
+    z, y, x = tsdf.shape
+    return x, y, z
+
+
+def _origin(origin, name):
+    if len(origin) != 3:
+        raise RuntimeError("%s: origin takes 3 coordinates" % name)
+    return (ctypes.c_float * 3)(*origin)
+
+
+def _tsdf_integrate(tsdf, weight, color, origin, voxel_size, trunc, depth, frames, w2c, fx, fy, cx, cy, n_valid):
+    """Fuses frames 0 .. n_valid - 1 of depth [n, h, w] (contiguous fp32), frames [n, h, w, 3] (contiguous uint8) and
+    world-to-camera matrices w2c [n, 3, 4] (contiguous fp32) into the volume, in place; n_valid: device int32 [1]."""
+    x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_integrate")
+    _f32c(depth, "depth"), _f32c(w2c, "w2c")
+    if depth.dim() != 3:
+        raise RuntimeError("tsdf_integrate: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    dev = tsdf.device
+    if frames.dtype != torch.uint8 or tuple(frames.shape) != (n, h, w, 3) or not frames.is_contiguous():
+        raise RuntimeError("tsdf_integrate: frames must be contiguous uint8 [n, h, w, 3] at the depths' size")
+    if tuple(w2c.shape) != (n, 3, 4):
+        raise RuntimeError("tsdf_integrate: w2c must be [n, 3, 4]")
+    if n_valid.dtype != torch.int32 or n_valid.numel() != 1:
+        raise RuntimeError("tsdf_integrate: n_valid must be one device int32")
+    if any(t.device != dev for t in (depth, frames, w2c, n_valid)):
+        raise RuntimeError("tsdf_integrate: every tensor must be on the volume's device")
+    _check(LIB.um_tsdf_integrate(_p(tsdf), _p(weight), _p(color), x, y, z, _origin(origin, "tsdf_integrate"), voxel_size,
+                                 trunc, _p(depth), _p(frames), _p(w2c), n, h, w, fx, fy, cx, cy, _p(n_valid), _stream()),
+           "um_tsdf_integrate")
+
+
+tsdf_integrate = _define(
+    "tsdf_integrate(Tensor(a!) tsdf, Tensor(b!) weight, Tensor(c!) color, float[] origin, float voxel_size, float trunc, "
+    "Tensor depth, Tensor frames, Tensor w2c, float fx, float fy, float cx, float cy, Tensor n_valid) -> ()", _tsdf_integrate)
+
+
+def _tsdf_surface_count(tsdf, weight):
+    """Returns the extraction's offsets, device int64 [ceil(X Y Z / TSDF_THREADS) + 1]: each block's first point, then
+    the number of points."""
+    _f32c(tsdf, "tsdf"), _f32c(weight, "weight")
+    if tsdf.dim() != 3 or tuple(weight.shape) != tuple(tsdf.shape) or weight.device != tsdf.device:
+        raise RuntimeError("tsdf_surface_count: expected tsdf and weight [Z, Y, X] on one device")
+    z, y, x = tsdf.shape
+    offsets = torch.empty((-(-tsdf.numel() // TSDF_THREADS) + 1,), device=tsdf.device, dtype=torch.int64)
+    _check(LIB.um_tsdf_surface_count(_p(tsdf), _p(weight), x, y, z, _p(offsets), _stream()), "um_tsdf_surface_count")
+    return offsets
+
+
+tsdf_surface_count = _define("tsdf_surface_count(Tensor tsdf, Tensor weight) -> Tensor", _tsdf_surface_count)
+
+
+def _tsdf_surface_points(tsdf, weight, color, origin, voxel_size, offsets, n_points):
+    """The surface's n_points points (fp32 [P, 3]) and colours (uint8 [P, 3]) from `tsdf_surface_count`'s offsets."""
+    x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_surface_points")
+    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-tsdf.numel() // TSDF_THREADS) + 1,) \
+            or offsets.device != tsdf.device:
+        raise RuntimeError("tsdf_surface_points: offsets must be tsdf_surface_count's device int64 table")
+    points = torch.empty((n_points, 3), device=tsdf.device, dtype=torch.float32)
+    colors = torch.empty((n_points, 3), device=tsdf.device, dtype=torch.uint8)
+    _check(LIB.um_tsdf_surface_points(_p(tsdf), _p(weight), _p(color), x, y, z, _origin(origin, "tsdf_surface_points"),
+                                      voxel_size, _p(offsets), n_points, _p(points) if n_points else None,
+                                      _p(colors) if n_points else None, _stream()), "um_tsdf_surface_points")
+    return points, colors
+
+
+tsdf_surface_points = _define(
+    "tsdf_surface_points(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, Tensor offsets, "
+    "int n_points) -> (Tensor, Tensor)", _tsdf_surface_points)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
