@@ -30,8 +30,8 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion) leave existing callers working and
- * keep it. */
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion and meshing) leave existing callers
+ * working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
@@ -449,6 +449,40 @@ int um_tsdf_surface_count(const float* tsdf, const float* weight, int32_t X, int
 int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
                            const float* origin, float voxel_size, const int64_t* offsets, int64_t n_points, float* points,
                            uint8_t* colors, void* stream);
+
+/* Mesh extraction: marching cubes' triangles over the same vertices, with per-vertex normals.
+ * Cubes: cube (i, j, k) has voxel (i, j, k) as its low corner, for i < X-1, j < Y-1, k < Z-1, and emits triangles only when
+ * all 8 corners have weight > 0.  Corner c = bx + 2 by + 4 bz; bit c of the cube's configuration is set when F(corner) < 0
+ * (the sign predicate of the point extraction: F == 0 counts as outside).
+ * Edges: edge e = 4 axis + b0 + 2 b1, where b0, b1 are the corner bits of the other two axes in increasing axis order, is
+ * the `axis` edge owned by voxel (i, j, k) + (those bits), so its vertex is the point um_tsdf_surface_points emits for
+ * that (voxel, axis): the mesh's vertices and colours are the point extraction's, bit for bit and in the same order.  A
+ * vertex on an edge whose cubes all have an unobserved corner is kept; no face references it.
+ * Triangles per configuration: unimatch_b200/csrc/um_mc_table.cuh, generated by um_mc_table.py (which states the rule):
+ * the crossing edges of each cube face are joined by segments that depend only on that face's four signs (an ambiguous
+ * face cuts each negative corner off), so neighbouring cubes meet without cracks; the segments are chained into loops and
+ * each loop fanned from its lowest edge id, loops in order of their lowest edge id.  At most 5 triangles per cube, each
+ * counter-clockwise seen from the F >= 0 (free-space) side.  Over observed cubes the mesh is closed (each edge in as many
+ * faces one way as the other); where both cubes at an ambiguous face fan a diagonal between the same two of its crossings,
+ * the two sheets touch along that edge.
+ * Faces: int32 [T, 3] vertex indices, ordered by cube linear index, then table order.
+ * Normals: fp32 [P, 3], from the TSDF gradient, in fp32 with every operation rounded on its own.  Per voxel v and axis,
+ * with v- and v+ the voxel's neighbours on that axis, each counted only inside the grid and observed (weight > 0):
+ *   g = (F(v+) - F(v-)) * 0.5f with both,  F(v+) - F(v) with only v+,  F(v) - F(v-) with only v-,  0 with neither.
+ * The vertex on the edge from voxel 0 to voxel 1 (s as for its point): n = fma(s, g1 - g0, g0) per component,
+ * l = sqrt(fma(n.z, n.z, fma(n.y, n.y, n.x * n.x))) (correctly rounded), normal = n / l, or (0, 0, 0) when l == 0.
+ * um_tsdf_mesh_count writes face_offsets [nb + 1] (DEVICE int64, as um_tsdf_surface_count's offsets): offsets[b] the
+ * first triangle of block b's cubes, offsets[nb] the total T.  um_tsdf_mesh takes both offset tables and both totals
+ * (n_points = P, n_faces = T, each at most 2^31 - 1) and writes points [P, 3] fp32, colors [P, 3] uint8 (as
+ * um_tsdf_surface_points), normals [P, 3] fp32 and faces [T, 3] int32, through first_vertex, caller-provided DEVICE scratch
+ * of N int32 (each voxel's first point).  Two launches: the vertex pass, then the face pass (none with T = 0); with P = 0
+ * nothing is launched.  No atomics, no host synchronisation (graph-capturable); the output is the same from run to run. */
+int um_tsdf_mesh_count(const float* tsdf, const float* weight, int32_t X, int32_t Y, int32_t Z, int64_t* face_offsets,
+                       void* stream);
+int um_tsdf_mesh(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                 const float* origin, float voxel_size, const int64_t* point_offsets, int64_t n_points,
+                 const int64_t* face_offsets, int64_t n_faces, int32_t* first_vertex, float* points, uint8_t* colors,
+                 float* normals, int32_t* faces, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -59,6 +59,10 @@ int tsdf_surface_count_launch(const float* tsdf, const float* weight, int X, int
 int tsdf_surface_points_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z,
                                const float* origin, float voxel_size, const long long* offsets, float* points,
                                uint8_t* colors, cudaStream_t st);
+int tsdf_mesh_count_launch(const float* tsdf, const float* weight, int X, int Y, int Z, long long* offsets, cudaStream_t st);
+int tsdf_mesh_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
+                     float voxel_size, const long long* point_offsets, const long long* face_offsets, long long n_faces,
+                     int* first_vertex, float* points, uint8_t* colors, float* normals, int* faces, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -333,6 +337,51 @@ int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* 
   if (n_points == 0) return UM_OK;
   return um::tsdf_surface_points_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size,
                                         reinterpret_cast<const long long*>(offsets), points, colors, (cudaStream_t)stream);
+}
+
+int um_tsdf_mesh_count(const float* tsdf, const float* weight, int32_t X, int32_t Y, int32_t Z, int64_t* face_offsets,
+                       void* stream) {
+  UM_REQUIRE(tsdf && weight && face_offsets, "um_tsdf_mesh_count: no pointer may be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_mesh_count: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(face_offsets, 8),
+             "um_tsdf_mesh_count: tsdf and weight must be 4-byte aligned, face_offsets 8-byte aligned");
+  const long long nv = (long long)X * Y * Z, nb = (nv + UM_TSDF_THREADS - 1) / UM_TSDF_THREADS;
+  UM_REQUIRE(um::written_disjoint({{face_offsets, 8 * (nb + 1)}, {tsdf, 4 * nv}, {weight, 4 * nv}}, 1),
+             "um_tsdf_mesh_count: face_offsets must not overlap the volume");
+  return um::tsdf_mesh_count_launch(tsdf, weight, X, Y, Z, reinterpret_cast<long long*>(face_offsets),
+                                    (cudaStream_t)stream);
+}
+
+int um_tsdf_mesh(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                 const float* origin, float voxel_size, const int64_t* point_offsets, int64_t n_points,
+                 const int64_t* face_offsets, int64_t n_faces, int32_t* first_vertex, float* points, uint8_t* colors,
+                 float* normals, int32_t* faces, void* stream) {
+  UM_REQUIRE(tsdf && weight && color && origin && point_offsets && face_offsets, "um_tsdf_mesh: no input may be NULL");
+  UM_REQUIRE(n_points == 0 || (first_vertex && points && colors && normals),
+             "um_tsdf_mesh: first_vertex, points, colors and normals must not be NULL");
+  UM_REQUIRE(n_faces == 0 || faces, "um_tsdf_mesh: faces must not be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_mesh: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(positive_finite(voxel_size), "um_tsdf_mesh: voxel_size must be positive and finite");
+  const long long nv = (long long)X * Y * Z, nb = (nv + UM_TSDF_THREADS - 1) / UM_TSDF_THREADS;
+  UM_REQUIRE(n_points >= 0 && n_points <= 3 * nv && n_points <= 0x7fffffffLL, "um_tsdf_mesh: bad point count %lld",
+             (long long)n_points);
+  UM_REQUIRE(n_faces >= 0 && n_faces <= 5 * nv && n_faces <= 0x7fffffffLL && (n_faces == 0 || n_points >= 3),
+             "um_tsdf_mesh: bad face count %lld (with %lld points)", (long long)n_faces, (long long)n_points);
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(color, 4) && um::aligned(point_offsets, 8) &&
+                 um::aligned(face_offsets, 8) && um::aligned(first_vertex, 4) && um::aligned(points, 4) &&
+                 um::aligned(normals, 4) && um::aligned(faces, 4),
+             "um_tsdf_mesh: the fp32 and int32 buffers must be 4-byte aligned, the offsets 8-byte aligned");
+  const long long P = n_points, T = n_faces;
+  UM_REQUIRE(um::written_disjoint({{points, 12 * P}, {colors, 3 * P}, {normals, 12 * P}, {first_vertex, P ? 4 * nv : 0},
+                                   {faces, 12 * T}, {tsdf, 4 * nv}, {weight, 4 * nv}, {color, 12 * nv},
+                                   {point_offsets, 8 * (nb + 1)}, {face_offsets, 8 * (nb + 1)}},
+                                  5),
+             "um_tsdf_mesh: the outputs and first_vertex must not overlap each other, the volume or the offsets");
+  if (n_points == 0) return UM_OK;
+  return um::tsdf_mesh_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size,
+                              reinterpret_cast<const long long*>(point_offsets),
+                              reinterpret_cast<const long long*>(face_offsets), n_faces, first_vertex, points, colors,
+                              normals, faces, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,7 +1,9 @@
-// TSDF fusion of posed depth maps into a dense voxel volume (um_tsdf_integrate) and the zero-crossing points of the fused
-// surface (um_tsdf_surface_count, um_tsdf_surface_points).  Semantics and the fp32 order of operations:
-// include/unimatch_sm100.h; the float32 and float64 statements are tests/refops_fusion.py.
+// TSDF fusion of posed depth maps into a dense voxel volume (um_tsdf_integrate), the zero-crossing points of the fused
+// surface (um_tsdf_surface_count, um_tsdf_surface_points) and its marching-cubes mesh (um_tsdf_mesh_count, um_tsdf_mesh).
+// Semantics and the fp32 order of operations: include/unimatch_sm100.h; the float32 and float64 statements are
+// tests/refops_fusion.py and tests/refops_mesh.py.
 #include "um_common.cuh"
+#include "um_mc_table.cuh"
 
 namespace {
 
@@ -175,11 +177,35 @@ __global__ void __launch_bounds__(FUSE_THREADS) tsdf_scan_kernel(long long* __re
   if (threadIdx.x == 0) offsets[nb] = carry;
 }
 
-// Pass 3: every voxel writes its points at its block's offset plus the points of the voxels before it in the block.
-__global__ void __launch_bounds__(FUSE_THREADS)
-tsdf_points_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, const float* __restrict__ color,
-                   Volume vol, long long total, const long long* __restrict__ offsets, float* __restrict__ points,
-                   uint8_t* __restrict__ colors) {
+// The gradient of F at voxel i (value F) along one axis, step voxels away in the layout: the central difference when both
+// neighbours are inside the grid (has_lo, has_hi) and observed, else the one-sided difference to the one that is, else 0.
+__device__ __forceinline__ float gradient(const float* __restrict__ tsdf, const float* __restrict__ weight, long long i,
+                                          long long step, bool has_lo, bool has_hi, float F) {
+  const bool lo = has_lo && __ldg(weight + i - step) > 0.f;
+  const bool hi = has_hi && __ldg(weight + i + step) > 0.f;
+  const float Fm = lo ? __ldg(tsdf + i - step) : 0.f, Fp = hi ? __ldg(tsdf + i + step) : 0.f;
+  if (lo && hi) return __fmul_rn(__fsub_rn(Fp, Fm), 0.5f);
+  if (hi) return __fsub_rn(Fp, F);
+  if (lo) return __fsub_rn(F, Fm);
+  return 0.f;
+}
+
+__device__ __forceinline__ void voxel_gradient(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                               const Volume& vol, long long i, int ii, int j, int k, float g[3]) {
+  const float F = __ldg(tsdf + i);
+  g[0] = gradient(tsdf, weight, i, 1, ii > 0, ii + 1 < vol.X, F);
+  g[1] = gradient(tsdf, weight, i, vol.X, j > 0, j + 1 < vol.Y, F);
+  g[2] = gradient(tsdf, weight, i, (long long)vol.X * vol.Y, k > 0, k + 1 < vol.Z, F);
+}
+
+// Every voxel writes its points at its block's offset plus the points of the voxels before it in the block.  kMesh also
+// writes each point's normal and the voxel's first point index (read by the face pass).
+template <bool kMesh>
+__device__ __forceinline__ void surface_points(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                               const float* __restrict__ color, const Volume& vol, long long total,
+                                               const long long* __restrict__ offsets, float* __restrict__ points,
+                                               uint8_t* __restrict__ colors, float* __restrict__ normals,
+                                               int* __restrict__ first_vertex) {
   const long long i = (long long)blockIdx.x * FUSE_THREADS + threadIdx.x;
   VoxelEdges v;
   int c = 0;
@@ -196,6 +222,11 @@ tsdf_points_kernel(const float* __restrict__ tsdf, const float* __restrict__ wei
   float c0[3];
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) c0[ch] = __ldg(color + ch * total + i);
+  float g0[3];
+  if constexpr (kMesh) {
+    first_vertex[i] = (int)o;
+    voxel_gradient(tsdf, weight, vol, i, v.ii, v.j, v.k, g0);
+  }
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     if (!v.e[a].hit) continue;
@@ -208,7 +239,113 @@ tsdf_points_kernel(const float* __restrict__ tsdf, const float* __restrict__ wei
       const int q = __float2int_rn(__fmaf_rn(s, __fsub_rn(c1, c0[ch]), c0[ch]));
       colors[3 * o + ch] = (uint8_t)min(max(q, 0), 255);
     }
+    if constexpr (kMesh) {
+      float g1[3], n[3];
+      voxel_gradient(tsdf, weight, vol, i + steps[a], v.ii + (a == 0), v.j + (a == 1), v.k + (a == 2), g1);
+#pragma unroll
+      for (int q = 0; q < 3; ++q) n[q] = __fmaf_rn(s, __fsub_rn(g1[q], g0[q]), g0[q]);
+      const float len = __fsqrt_rn(__fmaf_rn(n[2], n[2], __fmaf_rn(n[1], n[1], __fmul_rn(n[0], n[0]))));
+#pragma unroll
+      for (int q = 0; q < 3; ++q) normals[3 * o + q] = len == 0.f ? 0.f : __fdiv_rn(n[q], len);
+    }
     ++o;
+  }
+}
+
+// Pass 3 of the point extraction.
+__global__ void __launch_bounds__(FUSE_THREADS)
+tsdf_points_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, const float* __restrict__ color,
+                   Volume vol, long long total, const long long* __restrict__ offsets, float* __restrict__ points,
+                   uint8_t* __restrict__ colors) {
+  surface_points<false>(tsdf, weight, color, vol, total, offsets, points, colors, nullptr, nullptr);
+}
+
+// The mesh's vertex pass: the points of tsdf_points_kernel with their normals and each voxel's first point.
+__global__ void __launch_bounds__(FUSE_THREADS)
+tsdf_mesh_vertices_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, const float* __restrict__ color,
+                          Volume vol, long long total, const long long* __restrict__ offsets, float* __restrict__ points,
+                          uint8_t* __restrict__ colors, float* __restrict__ normals, int* __restrict__ first_vertex) {
+  surface_points<true>(tsdf, weight, color, vol, total, offsets, points, colors, normals, first_vertex);
+}
+
+// The case-table entry of the cube whose low corner is voxel i = (ii, j, k): 0 unless the cube lies inside the grid and
+// all 8 corners are observed; corner c = bx + 2 by + 4 bz sets bit c of the configuration when its F < 0.
+__device__ __forceinline__ unsigned long long cube_case(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                                        const Volume& vol, long long i, int ii, int j, int k) {
+  if (!(ii + 1 < vol.X && j + 1 < vol.Y && k + 1 < vol.Z)) return 0ull;
+  const long long xy = (long long)vol.X * vol.Y;
+  int cfg = 0;
+  bool seen = true;
+#pragma unroll
+  for (int c = 0; c < 8; ++c) {
+    const long long at = i + (c & 1) + ((c >> 1) & 1) * (long long)vol.X + (c >> 2) * xy;
+    seen &= __ldg(weight + at) > 0.f;
+    cfg |= (__ldg(tsdf + at) < 0.f) << c;
+  }
+  return seen ? __ldg(um_mc_table + cfg) : 0ull;
+}
+
+struct Coords {
+  int ii, j, k;
+};
+
+__device__ __forceinline__ Coords voxel_coords(const Volume& vol, long long i) {
+  const int xy = vol.X * vol.Y;
+  const int k = (int)(i / xy), r = (int)(i - (long long)k * xy);
+  const int j = r / vol.X;
+  return {r - j * vol.X, j, k};
+}
+
+// Mesh pass 1: the number of triangles of each block's cubes.
+__global__ void __launch_bounds__(FUSE_THREADS)
+tsdf_mesh_count_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, Volume vol, long long total,
+                       long long* __restrict__ block_counts) {
+  const long long i = (long long)blockIdx.x * FUSE_THREADS + threadIdx.x;
+  int n = 0;
+  if (i < total) {
+    const Coords c = voxel_coords(vol, i);
+    n = (int)(cube_case(tsdf, weight, vol, i, c.ii, c.j, c.k) >> 60);
+  }
+  int all;
+  block_exclusive_sum(n, &all);
+  if (threadIdx.x == 0) block_counts[blockIdx.x] = all;
+}
+
+// The point on edge e of the cube at voxel i = (ii, j, k): edge e = 4 axis + b0 + 2 b1 is the `axis` edge of the voxel
+// offset by b0, b1 on the other two axes, whose points come in axis order from its first one.
+__device__ __forceinline__ int edge_vertex(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                           const int* __restrict__ first_vertex, const Volume& vol, long long i, int ii,
+                                           int j, int k, int e) {
+  const int axis = e >> 2, b0 = e & 1, b1 = (e >> 1) & 1;
+  const int dx = axis == 0 ? 0 : b0, dy = axis == 0 ? b0 : axis == 1 ? 0 : b1, dz = axis == 2 ? 0 : b1;
+  const long long owner = i + dx + (long long)dy * vol.X + (long long)dz * vol.X * vol.Y;
+  int idx = __ldg(first_vertex + owner);
+  const float F0 = __ldg(tsdf + owner), W0 = __ldg(weight + owner);
+  if (axis > 0 && ii + dx + 1 < vol.X) idx += crossing(tsdf, weight, owner, 1, F0, W0).hit;
+  if (axis > 1 && j + dy + 1 < vol.Y) idx += crossing(tsdf, weight, owner, vol.X, F0, W0).hit;
+  return idx;
+}
+
+// Mesh pass 2: every cube writes its triangles at its block's offset plus the triangles of the cubes before it.
+__global__ void __launch_bounds__(FUSE_THREADS)
+tsdf_faces_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, Volume vol, long long total,
+                  const long long* __restrict__ offsets, const int* __restrict__ first_vertex, int* __restrict__ faces) {
+  const long long i = (long long)blockIdx.x * FUSE_THREADS + threadIdx.x;
+  Coords c = {0, 0, 0};
+  unsigned long long cs = 0ull;
+  if (i < total) {
+    c = voxel_coords(vol, i);
+    cs = cube_case(tsdf, weight, vol, i, c.ii, c.j, c.k);
+  }
+  const int n = (int)(cs >> 60);
+  int all;
+  const int before = block_exclusive_sum(n, &all);
+  if (n == 0) return;
+  long long o = __ldg(offsets + blockIdx.x) + before;
+  for (int t = 0; t < n; ++t, ++o) {
+#pragma unroll
+    for (int q = 0; q < 3; ++q)
+      faces[3 * o + q] = edge_vertex(tsdf, weight, first_vertex, vol, i, c.ii, c.j, c.k, (int)(cs >> (12 * t + 4 * q)) & 15);
   }
 }
 
@@ -243,6 +380,31 @@ int tsdf_surface_count_launch(const float* tsdf, const float* weight, int X, int
   if (int rc = check_launch("um_tsdf_surface_count")) return rc;
   tsdf_scan_kernel<<<1, FUSE_THREADS, 0, st>>>(offsets, (long long)nb);
   return check_launch("um_tsdf_surface_count");
+}
+
+int tsdf_mesh_count_launch(const float* tsdf, const float* weight, int X, int Y, int Z, long long* offsets, cudaStream_t st) {
+  const unsigned nb = volume_blocks(X, Y, Z);
+  const float origin[3] = {0.f, 0.f, 0.f};
+  tsdf_mesh_count_kernel<<<nb, FUSE_THREADS, 0, st>>>(tsdf, weight, make_volume(X, Y, Z, origin, 1.f),
+                                                      (long long)X * Y * Z, offsets);
+  if (int rc = check_launch("um_tsdf_mesh_count")) return rc;
+  tsdf_scan_kernel<<<1, FUSE_THREADS, 0, st>>>(offsets, (long long)nb);
+  return check_launch("um_tsdf_mesh_count");
+}
+
+// n_points > 0 (the entry point launches nothing for an empty surface).
+int tsdf_mesh_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
+                     float voxel_size, const long long* point_offsets, const long long* face_offsets, long long n_faces,
+                     int* first_vertex, float* points, uint8_t* colors, float* normals, int* faces, cudaStream_t st) {
+  const Volume vol = make_volume(X, Y, Z, origin, voxel_size);
+  const long long total = (long long)X * Y * Z;
+  tsdf_mesh_vertices_kernel<<<volume_blocks(X, Y, Z), FUSE_THREADS, 0, st>>>(tsdf, weight, color, vol, total, point_offsets,
+                                                                             points, colors, normals, first_vertex);
+  if (int rc = check_launch("um_tsdf_mesh")) return rc;
+  if (n_faces == 0) return UM_OK;
+  tsdf_faces_kernel<<<volume_blocks(X, Y, Z), FUSE_THREADS, 0, st>>>(tsdf, weight, vol, total, face_offsets, first_vertex,
+                                                                     faces);
+  return check_launch("um_tsdf_mesh");
 }
 
 int tsdf_surface_points_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z,

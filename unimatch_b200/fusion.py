@@ -1,6 +1,7 @@
 """TSDF fusion of posed depth maps on the device: a dense truncated-signed-distance volume (`TSDFVolume`), the integration of
 device depths and frames into it (`fuse_depths`, one `um_tsdf_integrate` launch), the zero-crossing points of its surface
-with their colours (`TSDFVolume.extract_points`) and a binary PLY writer for them (`write_ply`).  The kernels' arithmetic
+with their colours (`TSDFVolume.extract_points`), its marching-cubes mesh with per-vertex normals
+(`TSDFVolume.extract_mesh`) and a binary PLY writer for both (`write_ply`).  The kernels' arithmetic
 is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
@@ -11,6 +12,7 @@ import torch
 from .inference import _OPS, _intrinsics33, _pose44, _world_to_camera
 
 MAX_VOXELS = 2 ** 31 - 1
+MAX_MESH_INDEX = 2 ** 31 - 1                           # int32 face indices: at most this many vertices and faces
 
 
 def _f32(v):
@@ -69,6 +71,25 @@ class TSDFVolume:
             offsets = _OPS.tsdf_surface_count(self.tsdf, self.weight)
             n = int(offsets[-1].item())
             return _OPS.tsdf_surface_points(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, offsets, n)
+
+    def extract_mesh(self):
+        """Marching cubes on the observed voxels, on the device: points fp32 [P,3] and colors uint8 [P,3], which are
+        `extract_points()`'s bit for bit and in its order; normals fp32 [P,3], unit vectors along the TSDF gradient
+        (towards free space; (0, 0, 0) where the gradient vanishes); faces int32 [T,3] indices into the points,
+        counter-clockwise seen from free space, ordered by cube.  A cube (the 8 voxels from (i, j, k) to (i+1, j+1, k+1))
+        has faces only when all 8 of its voxels are observed, so a point whose cubes all touch an unobserved voxel is in
+        no face, and a volume with a dimension below 2 has none.  Count passes for points and faces, one host read of both
+        totals, then a vertex pass and a face pass; no atomics, the same result from run to run.  More than 2^31 - 1 points
+        or faces is refused before the outputs are allocated."""
+        with torch.cuda.device(self.device):
+            point_offsets = _OPS.tsdf_surface_count(self.tsdf, self.weight)
+            face_offsets = _OPS.tsdf_mesh_count(self.tsdf, self.weight)
+            n_points, n_faces = torch.stack((point_offsets[-1], face_offsets[-1])).tolist()
+            if max(n_points, n_faces) > MAX_MESH_INDEX:
+                raise ValueError("TSDFVolume.extract_mesh: %d points and %d faces; int32 faces hold at most 2^31 - 1 of "
+                                 "each" % (n_points, n_faces))
+            return _OPS.tsdf_mesh(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, point_offsets, n_points,
+                                  face_offsets, n_faces)
 
     def _integrate(self, depths, frames, w2c, n_valid, K):
         """One um_tsdf_integrate launch: frames 0 .. n_valid - 1 of device depths [n,H,W] and uint8 frames [n,H,W,3] with
@@ -135,19 +156,48 @@ def fuse_depths(volume, depths, frames, intrinsics, poses):
     return volume
 
 
-def write_ply(path, points, colors):
-    """A binary little-endian PLY of P coloured points: float x, y, z and uchar red, green, blue per vertex.  `points`
-    [P,3] and `colors` [P,3] uint8 are tensors (any device) or numpy arrays."""
-    pts = (points.detach().cpu().numpy() if torch.is_tensor(points) else np.asarray(points)).astype("<f4", copy=False)
-    col = colors.detach().cpu().numpy() if torch.is_tensor(colors) else np.asarray(colors)
+def _host(t):
+    return t.detach().cpu().numpy() if torch.is_tensor(t) else np.asarray(t)
+
+
+def write_ply(path, points, colors, normals=None, faces=None):
+    """A binary little-endian PLY of P coloured points: float x, y, z, then float nx, ny, nz when `normals` are given, and
+    uchar red, green, blue per vertex; with `faces`, an element face of T triangles (property list uchar int
+    vertex_indices).  `points` [P,3], `colors` [P,3] uint8, `normals` [P,3] and `faces` [T,3] (indices below P) are tensors
+    (any device) or numpy arrays, as `TSDFVolume.extract_points` / `extract_mesh` return them."""
+    pts = _host(points).astype("<f4", copy=False)
+    col = _host(colors)
     if pts.ndim != 2 or pts.shape[1] != 3 or col.shape != pts.shape or col.dtype != np.uint8:
         raise ValueError("write_ply: expected points [P,3] and uint8 colors [P,3]")
-    vertex = np.empty(len(pts), dtype=[("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("red", "u1"), ("green", "u1"),
-                                       ("blue", "u1")])
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    props = ["float x", "float y", "float z"]
+    if normals is not None:
+        nrm = _host(normals).astype("<f4", copy=False)
+        if nrm.shape != pts.shape:
+            raise ValueError("write_ply: expected normals [P,3]")
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+        props += ["float nx", "float ny", "float nz"]
+    fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+    props += ["uchar red", "uchar green", "uchar blue"]
+    vertex = np.empty(len(pts), dtype=fields)
     vertex["x"], vertex["y"], vertex["z"] = pts[:, 0], pts[:, 1], pts[:, 2]
+    if normals is not None:
+        vertex["nx"], vertex["ny"], vertex["nz"] = nrm[:, 0], nrm[:, 1], nrm[:, 2]
     vertex["red"], vertex["green"], vertex["blue"] = col[:, 0], col[:, 1], col[:, 2]
-    header = ("ply\nformat binary_little_endian 1.0\nelement vertex %d\nproperty float x\nproperty float y\n"
-              "property float z\nproperty uchar red\nproperty uchar green\nproperty uchar blue\nend_header\n" % len(pts))
+    header = "ply\nformat binary_little_endian 1.0\nelement vertex %d\n" % len(pts)
+    header += "".join("property %s\n" % p for p in props)
+    body = [vertex.tobytes()]
+    if faces is not None:
+        tri = _host(faces)
+        if tri.ndim != 2 or tri.shape[1] != 3 or tri.dtype.kind not in "iu" \
+                or (tri.size and (tri.min() < 0 or tri.max() >= len(pts))):
+            raise ValueError("write_ply: expected integer faces [T,3] indexing the points")
+        face = np.empty(len(tri), dtype=[("n", "u1"), ("v", "<i4", 3)])
+        face["n"], face["v"] = 3, tri
+        header += "element face %d\nproperty list uchar int vertex_indices\n" % len(tri)
+        body.append(face.tobytes())
+    header += "end_header\n"
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
-        f.write(vertex.tobytes())
+        for b in body:
+            f.write(b)

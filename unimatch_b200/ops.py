@@ -122,6 +122,8 @@ _SIGNATURES = {
     "um_tsdf_integrate": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _F, _P, _P, _P, _I, _I, _I, _F, _F, _F, _F, _P, _P]),
     "um_tsdf_surface_count": (_RC, [_P, _P, _I, _I, _I, _P, _P]),
     "um_tsdf_surface_points": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _P, _P]),
+    "um_tsdf_mesh_count": (_RC, [_P, _P, _I, _I, _I, _P, _P]),
+    "um_tsdf_mesh": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -591,6 +593,47 @@ def _tsdf_surface_points(tsdf, weight, color, origin, voxel_size, offsets, n_poi
 tsdf_surface_points = _define(
     "tsdf_surface_points(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, Tensor offsets, "
     "int n_points) -> (Tensor, Tensor)", _tsdf_surface_points)
+
+
+def _tsdf_mesh_count(tsdf, weight):
+    """Returns the mesh's face offsets, device int64 [ceil(X Y Z / TSDF_THREADS) + 1]: the first triangle of each block's
+    cubes, then the number of triangles."""
+    _f32c(tsdf, "tsdf"), _f32c(weight, "weight")
+    if tsdf.dim() != 3 or tuple(weight.shape) != tuple(tsdf.shape) or weight.device != tsdf.device:
+        raise RuntimeError("tsdf_mesh_count: expected tsdf and weight [Z, Y, X] on one device")
+    z, y, x = tsdf.shape
+    offsets = torch.empty((-(-tsdf.numel() // TSDF_THREADS) + 1,), device=tsdf.device, dtype=torch.int64)
+    _check(LIB.um_tsdf_mesh_count(_p(tsdf), _p(weight), x, y, z, _p(offsets), _stream()), "um_tsdf_mesh_count")
+    return offsets
+
+
+tsdf_mesh_count = _define("tsdf_mesh_count(Tensor tsdf, Tensor weight) -> Tensor", _tsdf_mesh_count)
+
+
+def _tsdf_mesh(tsdf, weight, color, origin, voxel_size, point_offsets, n_points, face_offsets, n_faces):
+    """The mesh's n_points vertices (fp32 [P, 3]), colours (uint8 [P, 3]) and normals (fp32 [P, 3]) and its n_faces
+    triangles (int32 [T, 3]) from `tsdf_surface_count`'s and `tsdf_mesh_count`'s offsets."""
+    x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_mesh")
+    nb = -(-tsdf.numel() // TSDF_THREADS) + 1
+    for t in (point_offsets, face_offsets):
+        if t.dtype != torch.int64 or tuple(t.shape) != (nb,) or t.device != tsdf.device:
+            raise RuntimeError("tsdf_mesh: the offsets must be tsdf_surface_count's and tsdf_mesh_count's device int64 tables")
+    dev = tsdf.device
+    points = torch.empty((n_points, 3), device=dev, dtype=torch.float32)
+    colors = torch.empty((n_points, 3), device=dev, dtype=torch.uint8)
+    normals = torch.empty((n_points, 3), device=dev, dtype=torch.float32)
+    faces = torch.empty((n_faces, 3), device=dev, dtype=torch.int32)
+    first = torch.empty((tsdf.numel() if n_points else 0,), device=dev, dtype=torch.int32)    # scratch
+    _check(LIB.um_tsdf_mesh(_p(tsdf), _p(weight), _p(color), x, y, z, _origin(origin, "tsdf_mesh"), voxel_size,
+                            _p(point_offsets), n_points, _p(face_offsets), n_faces, _p(first) if n_points else None,
+                            *(_p(t) if t.numel() else None for t in (points, colors, normals, faces)), _stream()),
+           "um_tsdf_mesh")
+    return points, colors, normals, faces
+
+
+tsdf_mesh = _define(
+    "tsdf_mesh(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, Tensor point_offsets, "
+    "int n_points, Tensor face_offsets, int n_faces) -> (Tensor, Tensor, Tensor, Tensor)", _tsdf_mesh)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
