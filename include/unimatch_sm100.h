@@ -30,7 +30,7 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion and meshing) leave existing callers
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing and ray casting) leave existing callers
  * working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
@@ -483,6 +483,41 @@ int um_tsdf_mesh(const float* tsdf, const float* weight, const float* color, int
                  const float* origin, float voxel_size, const int64_t* point_offsets, int64_t n_points,
                  const int64_t* face_offsets, int64_t n_faces, int32_t* first_vertex, float* points, uint8_t* colors,
                  float* normals, int32_t* faces, void* stream);
+
+/* Ray casting: the depth, colour and normal images of the fused surface seen by n pinhole cameras of h x w pixels with
+ * intrinsics fx, fy, cx, cy, from c2w [n, 3, 4] fp32 row-major camera-to-world rows M (DEVICE).  One thread per pixel
+ * (x, y) of view v, in fp32 with every operation rounded on its own (__fmaf_rn, __fdiv_rn, ...):
+ * Ray:  xc = (x - cx) / fx,  yc = (y - cy) / fy;  per axis a (x, y, z; origin o_a, voxel size vs, dims D_a):
+ *   d_a = fma(M_a0, xc, fma(M_a1, yc, M_a2))  (world direction, camera z-component 1, not normalised),
+ *   gd_a = d_a / vs,  go_a = (M_a3 - o_a) / vs - 0.5f;  the grid coordinate g_a(t) = fma(t, gd_a, go_a) puts voxel
+ *   centres on the integers, and t is the camera z-depth of the point at g(t).
+ * Range (slab test on the box of voxel centres, g_a in [0, D_a - 1]): t_lo = near, t_hi = far; per axis, if gd_a == 0 the
+ *   ray misses unless 0 <= go_a <= D_a - 1, else t0 = -go_a / gd_a, t1 = (D_a - 1 - go_a) / gd_a,
+ *   t_lo = fmaxf(t_lo, fminf(t0, t1)), t_hi = fminf(t_hi, fmaxf(t0, t1)).  The ray misses unless every gd_a and go_a is
+ *   finite, t_lo <= t_hi, t_hi is finite and every D_a >= 2 (a volume with a dimension below 2 has no cell).
+ * Sample at t: per axis g = fma(t, gd, go), i = clamp((int)floor(g), 0, D - 2), f = g - i.  Known iff all 8 voxels of the
+ *   cell have weight > 0 (the TSDF values are read only then).  F is trilinear with lerp(f, a, b) = fma(f, b - a, a) over
+ *   the corners c = bx + 2 by + 4 bz: along x (pairs 0-1, 2-3, 4-5, 6-7), then y, then z.  The sample is fine iff known and
+ *   F < 1 (an unknown sample, F >= 1 and NaN are coarse).
+ * March, with s_f = vs * 0.5f and s_c = trunc * 0.5f: A = the sample at t_a = t_lo; while t_a < t_hi:
+ *   t_b = fminf(t_a + (A fine ? s_f : s_c), t_hi), and t_b = t_hi if that is not > t_a;  B = the sample at t_b;
+ *   if A is coarse and B fine, the coarse step is taken back: t_b = fminf(t_a + s_f, t_hi) (t_hi if not > t_a), B = the
+ *   sample there;  if A and B are known and (F_a < 0) != (F_b < 0) the march ends: a hit if F_b < 0 (F == 0 counts as
+ *   outside, as in meshing), else a back face (a miss);  otherwise t_a = t_b, A = B.  t_a strictly increases and stays at
+ *   most t_hi, so the loop ends; every pair of consecutive samples ending in a fine sample is at most s_f apart, so each
+ *   sign change of F between known samples is bracketed by samples one fine step apart, at grazing angles too.
+ * Hit: s = F_a / (F_a - F_b);  depth = fma(s, t_b - t_a, t_a);  colour per channel __float2int_rn(lerp(s, C_a, C_b))
+ *   clamped to 0..255, C the trilinear colour at each sample;  n = lerp(s, G_a, G_b) per component, G the trilinear
+ *   interpolation (same order) of um_tsdf_mesh's per-voxel gradient, l = sqrt(fma(n.z, n.z, fma(n.y, n.y, n.x * n.x))),
+ *   normal = n / l (world coordinates, towards free space), (0, 0, 0) when l == 0.  A miss writes 0 to all three outputs.
+ * Outputs: depth [n, h, w] fp32, rgb [n, h, w, 3] uint8, normal [n, h, w, 3] fp32, every pixel written.  near finite and
+ * >= 0, far > near (+inf: the box alone limits the ray), voxel_size and trunc positive and finite, fx, fy finite and
+ * nonzero, cx, cy finite, n <= 65535; the outputs overlap each other, the volume and c2w nowhere.  Blocks of 16 x 8
+ * pixels; no atomics, no host synchronisation (graph-capturable). */
+int um_tsdf_raycast(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                    const float* origin, float voxel_size, float trunc, const float* c2w, int32_t n, int32_t h, int32_t w,
+                    float fx, float fy, float cx, float cy, float near, float far, float* depth, uint8_t* rgb,
+                    float* normal, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

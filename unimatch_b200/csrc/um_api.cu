@@ -63,6 +63,9 @@ int tsdf_mesh_count_launch(const float* tsdf, const float* weight, int X, int Y,
 int tsdf_mesh_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
                      float voxel_size, const long long* point_offsets, const long long* face_offsets, long long n_faces,
                      int* first_vertex, float* points, uint8_t* colors, float* normals, int* faces, cudaStream_t st);
+int tsdf_raycast_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
+                        float voxel_size, float trunc, const float* c2w, int n, int h, int w, float fx, float fy, float cx,
+                        float cy, float near, float far, float* depth, uint8_t* rgb, float* normal, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -283,6 +286,7 @@ static bool tsdf_dims(int32_t X, int32_t Y, int32_t Z) {
 }
 
 static bool positive_finite(float v) { return v > 0.f && v <= 3.402823466e38f; }
+static bool finite_value(float v) { return v >= -3.402823466e38f && v <= 3.402823466e38f; }
 
 int um_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t X, int32_t Y, int32_t Z, const float* origin,
                       float voxel_size, float trunc, const float* depth, const uint8_t* frames, const float* w2c, int32_t n,
@@ -382,6 +386,32 @@ int um_tsdf_mesh(const float* tsdf, const float* weight, const float* color, int
                               reinterpret_cast<const long long*>(point_offsets),
                               reinterpret_cast<const long long*>(face_offsets), n_faces, first_vertex, points, colors,
                               normals, faces, (cudaStream_t)stream);
+}
+
+int um_tsdf_raycast(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
+                    const float* origin, float voxel_size, float trunc, const float* c2w, int32_t n, int32_t h, int32_t w,
+                    float fx, float fy, float cx, float cy, float near, float far, float* depth, uint8_t* rgb,
+                    float* normal, void* stream) {
+  UM_REQUIRE(tsdf && weight && color && origin && c2w && depth && rgb && normal, "um_tsdf_raycast: no pointer may be NULL");
+  UM_REQUIRE(tsdf_dims(X, Y, Z), "um_tsdf_raycast: bad volume %d x %d x %d (at most 2^31 - 1 voxels)", X, Y, Z);
+  UM_REQUIRE(positive_finite(voxel_size) && positive_finite(trunc),
+             "um_tsdf_raycast: voxel_size and trunc must be positive and finite");
+  UM_REQUIRE(n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= 0x7fffffffLL,
+             "um_tsdf_raycast: bad views (%d x %d x %d; at most 65535 views of 2^31 - 1 pixels)", n, h, w);
+  UM_REQUIRE(fx != 0.f && fy != 0.f && finite_value(fx) && finite_value(fy) && finite_value(cx) && finite_value(cy),
+             "um_tsdf_raycast: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(near >= 0.f && finite_value(near) && far > near,
+             "um_tsdf_raycast: near must be finite and >= 0, far > near (+inf for no limit)");
+  UM_REQUIRE(um::aligned(tsdf, 4) && um::aligned(weight, 4) && um::aligned(color, 4) && um::aligned(c2w, 4) &&
+                 um::aligned(depth, 4) && um::aligned(normal, 4),
+             "um_tsdf_raycast: the fp32 buffers must be 4-byte aligned");
+  const long long nv = (long long)X * Y * Z, px = (long long)n * h * w;
+  UM_REQUIRE(um::written_disjoint({{depth, 4 * px}, {rgb, 3 * px}, {normal, 12 * px}, {tsdf, 4 * nv}, {weight, 4 * nv},
+                                   {color, 12 * nv}, {c2w, 48LL * n}},
+                                  3),
+             "um_tsdf_raycast: depth, rgb and normal must not overlap each other, the volume or c2w");
+  return um::tsdf_raycast_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size, trunc, c2w, n, h, w, fx, fy, cx, cy,
+                                 near, far, depth, rgb, normal, (cudaStream_t)stream);
 }
 
 }  // extern "C"

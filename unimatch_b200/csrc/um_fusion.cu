@@ -1,7 +1,8 @@
 // TSDF fusion of posed depth maps into a dense voxel volume (um_tsdf_integrate), the zero-crossing points of the fused
-// surface (um_tsdf_surface_count, um_tsdf_surface_points) and its marching-cubes mesh (um_tsdf_mesh_count, um_tsdf_mesh).
+// surface (um_tsdf_surface_count, um_tsdf_surface_points), its marching-cubes mesh (um_tsdf_mesh_count, um_tsdf_mesh)
+// and its ray-cast depth, colour and normal images (um_tsdf_raycast).
 // Semantics and the fp32 order of operations: include/unimatch_sm100.h; the float32 and float64 statements are
-// tests/refops_fusion.py and tests/refops_mesh.py.
+// tests/refops_fusion.py, tests/refops_mesh.py and tests/refops_render.py.
 #include "um_common.cuh"
 #include "um_mc_table.cuh"
 
@@ -349,6 +350,177 @@ tsdf_faces_kernel(const float* __restrict__ tsdf, const float* __restrict__ weig
   }
 }
 
+// ---- ray casting --------------------------------------------------------------------------------------------------------
+constexpr int RAY_TX = 16, RAY_TY = 8;          // a 2-D pixel tile per block: neighbouring rays read the same cache lines
+
+// A ray in grid coordinates: g(t) = fma(t, gd, go) per axis, where g = (p - origin) / voxel_size - 0.5 puts voxel centres
+// on the integers.
+struct Ray {
+  float gd[3], go[3];
+};
+
+// The trilinear cell of the sample at t: its low corner's linear index and the fractions along x, y, z.
+struct Cell {
+  long long base;
+  float f[3];
+};
+
+__device__ __forceinline__ Cell ray_cell(const Ray& r, const Volume& vol, float t) {
+  const int dims[3] = {vol.X, vol.Y, vol.Z};
+  int idx[3];
+  Cell c;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float g = __fmaf_rn(t, r.gd[a], r.go[a]);
+    idx[a] = min(max((int)floorf(g), 0), dims[a] - 2);
+    c.f[a] = __fsub_rn(g, (float)idx[a]);
+  }
+  c.base = ((long long)idx[2] * vol.Y + idx[1]) * vol.X + idx[0];
+  return c;
+}
+
+__device__ __forceinline__ float lerp(float f, float a, float b) { return __fmaf_rn(f, __fsub_rn(b, a), a); }
+
+// Trilinear interpolation of the 8 corner values v[c] (corner c = bx + 2 by + 4 bz): x, then y, then z.
+__device__ __forceinline__ float trilinear(const float v[8], const float f[3]) {
+  const float x00 = lerp(f[0], v[0], v[1]), x10 = lerp(f[0], v[2], v[3]);
+  const float x01 = lerp(f[0], v[4], v[5]), x11 = lerp(f[0], v[6], v[7]);
+  return lerp(f[2], lerp(f[1], x00, x10), lerp(f[1], x01, x11));
+}
+
+__device__ __forceinline__ long long corner(const Volume& vol, long long base, int c) {
+  return base + (c & 1) + ((c >> 1) & 1) * (long long)vol.X + (long long)(c >> 2) * vol.X * vol.Y;
+}
+
+// The sample at t: known iff all 8 corner weights are > 0 (the TSDF values are loaded only then), F the trilinear TSDF.
+struct Sample {
+  bool known;
+  float F;
+};
+
+__device__ __forceinline__ Sample ray_sample(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                             const Volume& vol, const Ray& r, float t) {
+  const Cell c = ray_cell(r, vol, t);
+  bool known = true;
+#pragma unroll
+  for (int q = 0; q < 8; ++q) known &= __ldg(weight + corner(vol, c.base, q)) > 0.f;
+  if (!known) return {false, 0.f};
+  float v[8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) v[q] = __ldg(tsdf + corner(vol, c.base, q));
+  return {true, trilinear(v, c.f)};
+}
+
+// Fine stepping applies after a known sample with F < 1 (NaN and F >= 1 step coarsely).
+__device__ __forceinline__ bool fine(Sample s) { return s.known && s.F < 1.f; }
+
+// The trilinear colour (3 channels) and TSDF gradient (3 components, um_tsdf_mesh's per-voxel gradient) at t.
+__device__ __forceinline__ void ray_shade(const float* __restrict__ tsdf, const float* __restrict__ weight,
+                                          const float* __restrict__ color, const Volume& vol, long long total,
+                                          const Ray& r, float t, float rgb[3], float grad[3]) {
+  const Cell c = ray_cell(r, vol, t);
+  float v[8];
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) v[q] = __ldg(color + ch * total + corner(vol, c.base, q));
+    rgb[ch] = trilinear(v, c.f);
+  }
+  const Coords lo = voxel_coords(vol, c.base);
+  const long long xy = (long long)vol.X * vol.Y;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const long long i = corner(vol, c.base, q);
+      const int at[3] = {lo.ii + (q & 1), lo.j + ((q >> 1) & 1), lo.k + (q >> 2)};
+      const int dims[3] = {vol.X, vol.Y, vol.Z};
+      v[q] = gradient(tsdf, weight, i, a == 0 ? 1 : a == 1 ? vol.X : xy, at[a] > 0, at[a] + 1 < dims[a], __ldg(tsdf + i));
+    }
+    grad[a] = trilinear(v, c.f);
+  }
+}
+
+// One thread per pixel of n views of h x w pixels; see include/unimatch_sm100.h (um_tsdf_raycast) for every operation.
+__global__ void __launch_bounds__(RAY_TX * RAY_TY)
+tsdf_raycast_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, const float* __restrict__ color,
+                    Volume vol, float trunc, const float* __restrict__ c2w, int h, int w, float fx, float fy, float cx,
+                    float cy, float near, float far, float* __restrict__ depth, uint8_t* __restrict__ rgb_out,
+                    float* __restrict__ normal) {
+  const int x = blockIdx.x * RAY_TX + threadIdx.x, y = blockIdx.y * RAY_TY + threadIdx.y, view = blockIdx.z;
+  if (x >= w || y >= h) return;
+  const long long px = ((long long)view * h + y) * w + x;
+  const float* m = c2w + 12 * view;
+  const float xc = __fdiv_rn(__fsub_rn((float)x, cx), fx), yc = __fdiv_rn(__fsub_rn((float)y, cy), fy);
+  const float origin[3] = {vol.ox, vol.oy, vol.oz};
+  const int dims[3] = {vol.X, vol.Y, vol.Z};
+  Ray r;
+  float t_lo = near, t_hi = far;
+  bool ok = vol.X >= 2 && vol.Y >= 2 && vol.Z >= 2;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const float d = __fmaf_rn(__ldg(m + 4 * a), xc, __fmaf_rn(__ldg(m + 4 * a + 1), yc, __ldg(m + 4 * a + 2)));
+    r.gd[a] = __fdiv_rn(d, vol.vs);
+    r.go[a] = __fsub_rn(__fdiv_rn(__fsub_rn(__ldg(m + 4 * a + 3), origin[a]), vol.vs), 0.5f);
+    ok &= isfinite(r.gd[a]) && isfinite(r.go[a]);
+    const float top = (float)(dims[a] - 1);
+    if (r.gd[a] == 0.f) {
+      ok &= r.go[a] >= 0.f && r.go[a] <= top;
+    } else {
+      const float t0 = __fdiv_rn(-r.go[a], r.gd[a]), t1 = __fdiv_rn(__fsub_rn(top, r.go[a]), r.gd[a]);
+      t_lo = fmaxf(t_lo, fminf(t0, t1));
+      t_hi = fminf(t_hi, fmaxf(t0, t1));
+    }
+  }
+  ok &= t_lo <= t_hi && isfinite(t_hi);
+  float out_d = 0.f, out_n[3] = {0.f, 0.f, 0.f};
+  int out_c[3] = {0, 0, 0};
+  bool hit = false;
+  if (ok) {
+    const float step_fine = __fmul_rn(vol.vs, 0.5f), step_coarse = __fmul_rn(trunc, 0.5f);
+    float ta = t_lo, tb = t_lo;
+    Sample A = ray_sample(tsdf, weight, vol, r, ta), B = A;
+    while (ta < t_hi) {
+      tb = fminf(__fadd_rn(ta, fine(A) ? step_fine : step_coarse), t_hi);
+      if (!(tb > ta)) tb = t_hi;
+      B = ray_sample(tsdf, weight, vol, r, tb);
+      if (!fine(A) && fine(B)) {                               // take the coarse step back: one fine step instead
+        tb = fminf(__fadd_rn(ta, step_fine), t_hi);
+        if (!(tb > ta)) tb = t_hi;
+        B = ray_sample(tsdf, weight, vol, r, tb);
+      }
+      if (A.known && B.known && (A.F < 0.f) != (B.F < 0.f)) {
+        hit = B.F < 0.f;                                       // a change to non-negative is a back face: a miss
+        break;
+      }
+      ta = tb, A = B;
+    }
+    if (hit) {
+      const float s = __fdiv_rn(A.F, __fsub_rn(A.F, B.F));
+      out_d = __fmaf_rn(s, __fsub_rn(tb, ta), ta);
+      const long long total = (long long)vol.X * vol.Y * vol.Z;
+      float ca[3], cb[3], ga[3], gb[3];
+      ray_shade(tsdf, weight, color, vol, total, r, ta, ca, ga);
+      ray_shade(tsdf, weight, color, vol, total, r, tb, cb, gb);
+#pragma unroll
+      for (int a = 0; a < 3; ++a) {
+        out_c[a] = min(max(__float2int_rn(lerp(s, ca[a], cb[a])), 0), 255);
+        out_n[a] = lerp(s, ga[a], gb[a]);
+      }
+      const float len =
+          __fsqrt_rn(__fmaf_rn(out_n[2], out_n[2], __fmaf_rn(out_n[1], out_n[1], __fmul_rn(out_n[0], out_n[0]))));
+#pragma unroll
+      for (int a = 0; a < 3; ++a) out_n[a] = len == 0.f ? 0.f : __fdiv_rn(out_n[a], len);
+    }
+  }
+  depth[px] = out_d;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    rgb_out[3 * px + a] = (uint8_t)out_c[a];
+    normal[3 * px + a] = out_n[a];
+  }
+}
+
 }  // namespace
 
 namespace um {
@@ -413,6 +585,15 @@ int tsdf_surface_points_launch(const float* tsdf, const float* weight, const flo
   tsdf_points_kernel<<<volume_blocks(X, Y, Z), FUSE_THREADS, 0, st>>>(
       tsdf, weight, color, make_volume(X, Y, Z, origin, voxel_size), (long long)X * Y * Z, offsets, points, colors);
   return check_launch("um_tsdf_surface_points");
+}
+
+int tsdf_raycast_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
+                        float voxel_size, float trunc, const float* c2w, int n, int h, int w, float fx, float fy, float cx,
+                        float cy, float near, float far, float* depth, uint8_t* rgb, float* normal, cudaStream_t st) {
+  const dim3 grid((unsigned)((w + RAY_TX - 1) / RAY_TX), (unsigned)((h + RAY_TY - 1) / RAY_TY), (unsigned)n);
+  tsdf_raycast_kernel<<<grid, dim3(RAY_TX, RAY_TY), 0, st>>>(tsdf, weight, color, make_volume(X, Y, Z, origin, voxel_size),
+                                                            trunc, c2w, h, w, fx, fy, cx, cy, near, far, depth, rgb, normal);
+  return check_launch("um_tsdf_raycast");
 }
 
 }  // namespace um

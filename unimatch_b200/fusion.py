@@ -1,7 +1,8 @@
 """TSDF fusion of posed depth maps on the device: a dense truncated-signed-distance volume (`TSDFVolume`), the integration of
 device depths and frames into it (`fuse_depths`, one `um_tsdf_integrate` launch), the zero-crossing points of its surface
 with their colours (`TSDFVolume.extract_points`), its marching-cubes mesh with per-vertex normals
-(`TSDFVolume.extract_mesh`) and a binary PLY writer for both (`write_ply`).  The kernels' arithmetic
+(`TSDFVolume.extract_mesh`), its ray-cast depth, colour and normal images from any camera (`TSDFVolume.render`, one
+`um_tsdf_raycast` launch) and a binary PLY writer for the points and meshes (`write_ply`).  The kernels' arithmetic
 is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
@@ -9,7 +10,7 @@ import math
 import numpy as np
 import torch
 
-from .inference import _OPS, _intrinsics33, _pose44, _world_to_camera
+from .inference import _OPS, _camera_to_world, _intrinsics33, _pose44, _world_to_camera
 
 MAX_VOXELS = 2 ** 31 - 1
 MAX_MESH_INDEX = 2 ** 31 - 1                           # int32 face indices: at most this many vertices and faces
@@ -90,6 +91,42 @@ class TSDFVolume:
                                  "each" % (n_points, n_faces))
             return _OPS.tsdf_mesh(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, point_offsets, n_points,
                                   face_offsets, n_faces)
+
+    @torch.no_grad()
+    def render(self, intrinsics, poses, frame_size, near=0.0, far=None):
+        """The fused surface seen by N pinhole cameras, ray-cast on the device in one `um_tsdf_raycast` launch: intrinsics
+        [3,3] at `frame_size` = (H, W), host camera-to-world poses [N,4,4] (as `fuse_depths` takes them).  Each pixel's ray
+        through its centre is marched over the box of voxel centres between camera z-depths `near` and `far` (None: the
+        box alone limits it) and ends at the first zero crossing of the trilinear TSDF from positive to negative between two
+        observed samples.  Returns {'depth': fp32 [N,H,W] camera z-depth, 'color': uint8 [N,H,W,3] RGB, 'normal': fp32
+        [N,H,W,3] unit world-space normals towards free space}, on the volume's device, all 0 where a ray finds no surface
+        (a depth of 0 is "no estimate" to `fuse_depths` and `depth_to_image`).  A ray that first crosses from negative to
+        positive (a camera inside a surface) misses.  No atomics and no host synchronisation after the one upload of the
+        poses; the same result from run to run."""
+        K = _intrinsics33(intrinsics, "TSDFVolume.render")
+        fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+        if not (all(math.isfinite(v) for v in (fx, fy, cx, cy)) and fx != 0 and fy != 0):
+            raise ValueError("TSDFVolume.render: fx, fy, cx and cy must be finite, fx and fy nonzero")
+        ps = [_pose44(p, "TSDFVolume.render") for p in poses]
+        if not all(np.isfinite(p).all() for p in ps):
+            raise ValueError("TSDFVolume.render: camera poses must be finite")
+        h, w = (int(v) for v in frame_size)
+        if h < 1 or w < 1 or h * w > MAX_VOXELS:
+            raise ValueError("TSDFVolume.render: frame_size must be (H, W) with at most 2^31 - 1 pixels")
+        if len(ps) > 65535:
+            raise ValueError("TSDFVolume.render: at most 65535 cameras per call")
+        near, far = _f32(near), math.inf if far is None else _f32(far)
+        if not (math.isfinite(near) and near >= 0 and far > near):
+            raise ValueError("TSDFVolume.render: near must be finite and >= 0, far None or greater than near")
+        if not ps:
+            return {"depth": torch.zeros((0, h, w), dtype=torch.float32, device=self.device),
+                    "color": torch.zeros((0, h, w, 3), dtype=torch.uint8, device=self.device),
+                    "normal": torch.zeros((0, h, w, 3), dtype=torch.float32, device=self.device)}
+        with torch.cuda.device(self.device):
+            c2w = torch.from_numpy(_camera_to_world(ps)).to(self.device)
+            depth, color, normal = _OPS.tsdf_raycast(self.tsdf, self.weight, self.color, self.origin, self.voxel_size,
+                                                     self.trunc, c2w, h, w, fx, fy, cx, cy, near, far)
+        return {"depth": depth, "color": color, "normal": normal}
 
     def _integrate(self, depths, frames, w2c, n_valid, K):
         """One um_tsdf_integrate launch: frames 0 .. n_valid - 1 of device depths [n,H,W] and uint8 frames [n,H,W,3] with

@@ -435,6 +435,11 @@ def _world_to_camera(poses):
     return np.ascontiguousarray(np.stack([np.linalg.inv(p) for p in poses]).astype(np.float32)[:, :3])
 
 
+def _camera_to_world(poses):
+    """The float32 [n,3,4] camera-to-world rows `um_tsdf_raycast` reads: the top three rows of absolute float32 poses [4,4]."""
+    return np.ascontiguousarray(np.stack([np.asarray(p, np.float32) for p in poses])[:, :3])
+
+
 def _with_inverses(rel, bidir):
     """Relative poses [4,4] stacked as float32 [n,4,4], followed with `bidir` by their inverses (np.linalg.inv)."""
     if bidir:

@@ -124,6 +124,7 @@ _SIGNATURES = {
     "um_tsdf_surface_points": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _P, _P]),
     "um_tsdf_mesh_count": (_RC, [_P, _P, _I, _I, _I, _P, _P]),
     "um_tsdf_mesh": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P]),
+    "um_tsdf_raycast": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _F, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -634,6 +635,29 @@ def _tsdf_mesh(tsdf, weight, color, origin, voxel_size, point_offsets, n_points,
 tsdf_mesh = _define(
     "tsdf_mesh(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, Tensor point_offsets, "
     "int n_points, Tensor face_offsets, int n_faces) -> (Tensor, Tensor, Tensor, Tensor)", _tsdf_mesh)
+
+
+def _tsdf_raycast(tsdf, weight, color, origin, voxel_size, trunc, c2w, h, w, fx, fy, cx, cy, near, far):
+    """The volume seen by n cameras of h x w pixels with camera-to-world rows c2w [n, 3, 4] (contiguous fp32): depth fp32
+    [n, h, w], colour uint8 [n, h, w, 3] and unit normals fp32 [n, h, w, 3], zero where a ray misses the surface."""
+    x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_raycast")
+    _f32c(c2w, "c2w")
+    if c2w.dim() != 3 or tuple(c2w.shape[1:]) != (3, 4) or c2w.device != tsdf.device:
+        raise RuntimeError("tsdf_raycast: c2w must be [n, 3, 4] on the volume's device")
+    n, dev = c2w.shape[0], tsdf.device
+    depth = torch.empty((n, h, w), device=dev, dtype=torch.float32)
+    rgb = torch.empty((n, h, w, 3), device=dev, dtype=torch.uint8)
+    normal = torch.empty((n, h, w, 3), device=dev, dtype=torch.float32)
+    _check(LIB.um_tsdf_raycast(_p(tsdf), _p(weight), _p(color), x, y, z, _origin(origin, "tsdf_raycast"), voxel_size, trunc,
+                               _p(c2w), n, h, w, fx, fy, cx, cy, near, far, _p(depth), _p(rgb), _p(normal), _stream()),
+           "um_tsdf_raycast")
+    return depth, rgb, normal
+
+
+tsdf_raycast = _define(
+    "tsdf_raycast(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, float trunc, Tensor c2w, "
+    "int h, int w, float fx, float fy, float cx, float cy, float near, float far) -> (Tensor, Tensor, Tensor)",
+    _tsdf_raycast)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
