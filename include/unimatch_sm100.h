@@ -30,7 +30,7 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing and ray casting) leave existing callers
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing, ray casting and ICP) leave existing callers
  * working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
@@ -518,6 +518,81 @@ int um_tsdf_raycast(const float* tsdf, const float* weight, const float* color, 
                     const float* origin, float voxel_size, float trunc, const float* c2w, int32_t n, int32_t h, int32_t w,
                     float fx, float fy, float cx, float cy, float near, float far, float* depth, uint8_t* rgb,
                     float* normal, void* stream);
+
+/* ---- tracking a camera against the fused volume: point-to-plane ICP (KinectFusion, Newcombe et al., ISMAR 2011) ------
+ * n frames (at most 65535), each a live depth map and an initial camera-to-world pose P_ref, are tracked independently
+ * in the same launches.  fp32 operations are each rounded on their own (__fmaf_rn, __fdiv_rn, ...); fp64 operations are
+ * __dmul_rn / __dadd_rn / __dsub_rn / __ddiv_rn / __dsqrt_rn, in the order written, except cos and sin (CUDA's).
+ * Depth pyramid (um_icp_downsample): level l+1 of an h x w map has floor(h/2) x floor(w/2) pixels; pixel (x, y) reads
+ *   the depths d0..d3 at (2x, 2y), (2x+1, 2y), (2x, 2y+1), (2x+1, 2y+1); a depth is valid iff finite and > 0.
+ *   lo = the fminf of the valid ones in that order; out = the fp32 sum, in that order from 0, of the valid d with
+ *   d - lo <= trunc, divided by their count (a float); 0 if none is valid.  The level's intrinsics are fx/2, fy/2,
+ *   (cx - 0.5f)/2 and (cy - 0.5f)/2 in fp32 (pixel x is centred at x on every level), computed by the caller.
+ * Live normals (um_icp_normals, written to a buffer [n, h, w, 3]): the vertex of depth d at pixel (x, y) is
+ *   v = (d * ((x - cx) / fx), d * ((y - cy) / fy), d).  With e1 = v(x+1, y) - v and e2 = v(x, y+1) - v (per component),
+ *   c_a = e1_b * e2_e - e1_e * e2_b for (a, b, e) = (x, y, z), (y, z, x), (z, x, y); l = sqrt(fma(c.z, c.z, fma(c.y, c.y,
+ *   c.x * c.x))), facing = fma(c.z, v.z, fma(c.y, v.y, c.x * v.x)); normal = c / (facing > 0 ? -l : l), so that n.v <= 0.
+ *   0 where x + 1 = w, y + 1 = h, one of the three depths is invalid, or l is 0 or not finite.
+ * Model maps: um_tsdf_raycast at the level's intrinsics from c2w_ref, the fp32 rows of P_ref, unchanged.  A model pixel is
+ *   valid iff its depth D > 0 and its normal m is not (0, 0, 0).
+ * State (um_icp_init; DEVICE fp64 [n, UM_ICP_STATE]): [0, 12) the estimate T = (R | t), [12, 24) P_ref, both [3, 4]
+ *   row-major camera-to-world; [24] the number of degenerate recorded solves.  Init, per frame f < n_valid:
+ *   P_ref = C * P (rows i < 3: (C_i0 P_0j + C_i1 P_1j) + C_i2 P_2j, plus C_i3 when j = 3) with the DEVICE fp64 [4, 4]
+ *   correction C, or P itself when C is NULL; T = P_ref; state[24] = 0; c2w_ref = (float)P_ref rows; w2c_ref = the rigid
+ *   inverse of P_ref: (R^T, -((R_0i t_0 + R_1i t_1) + R_2i t_2)) in fp64, each entry rounded to fp32.  poses: fp64
+ *   [n, 4, 4] row-major (the last row is not read).
+ * Association (um_icp_reduce), one thread per live pixel in 16 x 8 tiles, at the current T (rounded to fp32 rows):
+ *   skip unless d is valid and the live normal n is not 0;  p_a = fma(T_a2, v.z, fma(T_a1, v.y, fma(T_a0, v.x, T_a3))),
+ *   n_w,a = fma(T_a2, n.z, fma(T_a1, n.y, T_a0 * n.x));  c = w2c_ref applied to p exactly as um_tsdf_integrate projects
+ *   a voxel, and its nearest pixel (xi, yi) by integration's rule (c.z > 0, floor(u + 0.5f) inside the frame);  skip
+ *   unless the model pixel there is valid;  with xc = (xi - cx) / fx, yc = (yi - cy) / fy and M = c2w_ref:
+ *   dir_a = fma(M_a0, xc, fma(M_a1, yc, M_a2)) (the ray cast's), q_a = fma(D, dir_a, M_a3), e = p - q, pc = p - M_.3;
+ *   an inlier iff sqrt(fma(e.z, e.z, fma(e.y, e.y, e.x * e.x))) <= max_distance and fma(n_w.z, m.z, fma(n_w.y, m.y,
+ *   n_w.x * m.x)) >= cos_max_angle;  r = fma(m.z, e.z, fma(m.y, e.y, m.x * e.x));  a = (pc x m (as c above), m), the
+ *   Jacobian of r for dT applied on the left about the reference centre.
+ *   Terms (fp32 products, then exact conversion to fp64; 0 unless an inlier): k < 21 the upper triangle of a a^T row by
+ *   row (a_0 a_0 .. a_0 a_5, a_1 a_1, ..), 21 + i a_i r, 27 r r, 28 the inlier count (1), 29 the valid live pixel count
+ *   (1 for every pixel with valid d and n, inlier or not).  Sums, no atomics (the same result from run to run): per warp
+ *   v += shfl_down(v, o) for o = 16, 8, 4, 2, 1 (lane 0's: pixels outside the frame add 0), then the block's 4 warps in
+ *   order; partials [n, nb, UM_ICP_TERMS] fp64, nb = ceil(w/16) ceil(h/8), block b = by ceil(w/16) + bx.  um_icp_solve and
+ *   um_icp_accept sum a frame's partials with one warp of 32 lanes per term: lane l adds blocks l, l + 32, l + 64, ...
+ *   in order from 0.0, then v += shfl_down(v, o) for o = 16, 8, 4, 2, 1 gives lane 0 the sum.
+ * Solve (um_icp_solve, one block per frame): A (6 x 6, symmetric) and b from the sums.  Degenerate unless inliers >=
+ *   min_inliers and every Cholesky pivot of the Jacobi-scaled system is >= min_pivot (a NaN fails).  s_i = 1/sqrt(A_ii),
+ *   or 1 where A_ii is not > 0 (an unknown no residual constrains keeps its zero pivot);
+ *   Ahat_ij = (A_ij s_i) s_j;  for j = 0..5: pivot = Ahat_jj - L_j0^2 - .. - L_j,j-1^2 (subtracted in order), L_jj =
+ *   sqrt(pivot), L_ij = (Ahat_ij - L_i0 L_j0 - ..) / L_jj;  L z = -(b_i s_i), L^T y = z (back substitution from i = 5,
+ *   k ascending), x_i = y_i s_i.  A degenerate solve leaves T unchanged and, with `record` (the finest level), adds 1 to
+ *   state[24].  Otherwise x = (w, tau): th = sqrt((w0^2 + w1^2) + w2^2); dR = I if th == 0, else with k = w / th,
+ *   dR_ij = ((i == j ? cos th : 0) + sin th [k]x_ij) + ((1 - cos th) k_i) k_j;  R <- dR R, t <- ((dR (t - c)) + c) + tau
+ *   with c = P_ref's translation (matrix products summed (x0 + x1) + x2).
+ * Schedule (the caller's): for each level, coarse to fine, a fixed number of (um_icp_reduce, um_icp_solve) iterations;
+ *   fixed counts keep the launch sequence static, so it can be captured in a CUDA graph.
+ * Acceptance (um_icp_accept, after one more um_icp_reduce at level 0): tracked iff state[24] == 0 and inliers >=
+ *   min_inlier_fraction * valid (fp64).  A frame that is not tracked gets T = P_ref back.  Outputs: pose_out fp32
+ *   [n, 4, 4] ((float)T, last row 0 0 0 1), tracked uint8 [n], inliers int64 [n], rmse fp32 [n] ((float)sqrt(sum r^2 /
+ *   inliers), 0 without inliers) and w2c fp32 [n, 3, 4] (T's rigid inverse, as init's), the rows um_tsdf_integrate reads.
+ *   With a correction (n == 1, poses given), a tracked frame sets C = T P^-1, P^-1 = (R_P^T, -R_P^T t_P) in fp64 (rows
+ *   i < 3 as in init); a frame that is not tracked leaves C as it is.
+ * Every loop has a fixed trip count.  n_valid (DEVICE int32): frames >= min(max(n_valid, 0), n) are untouched by init,
+ * reduce, solve and accept, so one captured graph serves a short last step.  Pointers are fp32 unless stated; no output
+ * overlaps an input or another output. */
+#define UM_ICP_TERMS 30
+#define UM_ICP_STATE 32
+int um_icp_downsample(const float* src, float* dst, int32_t n, int32_t h, int32_t w, float trunc, void* stream);
+int um_icp_normals(const float* depth, float* normal, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx,
+                   float cy, void* stream);
+int um_icp_init(const double* poses, const double* correction, int32_t n, const int32_t* n_valid, double* state,
+                float* c2w, float* w2c, void* stream);
+int um_icp_reduce(const float* depth, const float* live_normal, const float* model_depth, const float* model_normal,
+                  const double* state, const float* c2w, const float* w2c, int32_t n, int32_t h, int32_t w, float fx,
+                  float fy, float cx, float cy, float max_distance, float cos_max_angle, const int32_t* n_valid,
+                  double* partials, void* stream);
+int um_icp_solve(const double* partials, int32_t nb, int32_t n, const int32_t* n_valid, double min_inliers,
+                 double min_pivot, int32_t record, double* state, void* stream);
+int um_icp_accept(const double* partials, int32_t nb, int32_t n, const int32_t* n_valid, double min_inlier_fraction,
+                  const double* poses, double* correction, double* state, float* pose_out, uint8_t* tracked,
+                  int64_t* inliers, float* rmse, float* w2c, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -1,6 +1,6 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
 // between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu),
-// and TSDF fusion (um_fusion.cu).  See include/unimatch_sm100.h.
+// TSDF fusion (um_fusion.cu) and ICP tracking against the volume (um_icp.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -66,6 +66,20 @@ int tsdf_mesh_launch(const float* tsdf, const float* weight, const float* color,
 int tsdf_raycast_launch(const float* tsdf, const float* weight, const float* color, int X, int Y, int Z, const float* origin,
                         float voxel_size, float trunc, const float* c2w, int n, int h, int w, float fx, float fy, float cx,
                         float cy, float near, float far, float* depth, uint8_t* rgb, float* normal, cudaStream_t st);
+int icp_downsample_launch(const float* src, float* dst, int n, int h, int w, float trunc, cudaStream_t st);
+int icp_normals_launch(const float* depth, float* normal, int n, int h, int w, float fx, float fy, float cx, float cy,
+                       cudaStream_t st);
+int icp_init_launch(const double* poses, const double* correction, int n, const int* n_valid, double* state, float* c2w,
+                    float* w2c, cudaStream_t st);
+int icp_reduce_launch(const float* depth, const float* live_normal, const float* model_depth, const float* model_normal,
+                      const double* state, const float* c2w, const float* w2c, int n, int h, int w, float fx, float fy,
+                      float cx, float cy, float max_distance, float cos_max_angle, const int* n_valid, double* partials,
+                      cudaStream_t st);
+int icp_solve_launch(const double* partials, int nb, int n, const int* n_valid, double min_inliers, double min_pivot,
+                     int record, double* state, cudaStream_t st);
+int icp_accept_launch(const double* partials, int nb, int n, const int* n_valid, double min_inlier_fraction,
+                      const double* poses, double* correction, double* state, float* pose_out, uint8_t* tracked,
+                      int64_t* inliers, float* rmse, float* w2c, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -412,6 +426,116 @@ int um_tsdf_raycast(const float* tsdf, const float* weight, const float* color, 
              "um_tsdf_raycast: depth, rgb and normal must not overlap each other, the volume or c2w");
   return um::tsdf_raycast_launch(tsdf, weight, color, X, Y, Z, origin, voxel_size, trunc, c2w, n, h, w, fx, fy, cx, cy,
                                  near, far, depth, rgb, normal, (cudaStream_t)stream);
+}
+
+
+// ---- ICP tracking against the volume (um_icp.cu) ----
+static bool icp_frames(int32_t n, int32_t h, int32_t w) {
+  return n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= 0x7fffffffLL;
+}
+
+static bool icp_intrinsics(float fx, float fy, float cx, float cy) {
+  return fx != 0.f && fy != 0.f && finite_value(fx) && finite_value(fy) && finite_value(cx) && finite_value(cy);
+}
+
+int um_icp_downsample(const float* src, float* dst, int32_t n, int32_t h, int32_t w, float trunc, void* stream) {
+  UM_REQUIRE(src && dst, "um_icp_downsample: no pointer may be NULL");
+  UM_REQUIRE(icp_frames(n, h, w) && h >= 2 && w >= 2,
+             "um_icp_downsample: bad depths (%d x %d x %d; at most 65535 maps of 2 x 2 to 2^31 - 1 pixels)", n, h, w);
+  UM_REQUIRE(positive_finite(trunc), "um_icp_downsample: trunc must be positive and finite");
+  UM_REQUIRE(um::aligned(src, 4) && um::aligned(dst, 4), "um_icp_downsample: src and dst must be 4-byte aligned");
+  const long long px = (long long)n * h * w, px2 = (long long)n * (h / 2) * (w / 2);
+  UM_REQUIRE(um::written_disjoint({{dst, 4 * px2}, {src, 4 * px}}, 1), "um_icp_downsample: dst must not overlap src");
+  return um::icp_downsample_launch(src, dst, n, h, w, trunc, (cudaStream_t)stream);
+}
+
+int um_icp_normals(const float* depth, float* normal, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx,
+                   float cy, void* stream) {
+  UM_REQUIRE(depth && normal, "um_icp_normals: no pointer may be NULL");
+  UM_REQUIRE(icp_frames(n, h, w), "um_icp_normals: bad depths (%d x %d x %d; at most 65535 maps of 2^31 - 1 pixels)", n,
+             h, w);
+  UM_REQUIRE(icp_intrinsics(fx, fy, cx, cy), "um_icp_normals: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(um::aligned(depth, 4) && um::aligned(normal, 4), "um_icp_normals: depth and normal must be 4-byte aligned");
+  const long long px = (long long)n * h * w;
+  UM_REQUIRE(um::written_disjoint({{normal, 12 * px}, {depth, 4 * px}}, 1), "um_icp_normals: normal must not overlap depth");
+  return um::icp_normals_launch(depth, normal, n, h, w, fx, fy, cx, cy, (cudaStream_t)stream);
+}
+
+int um_icp_init(const double* poses, const double* correction, int32_t n, const int32_t* n_valid, double* state,
+                float* c2w, float* w2c, void* stream) {
+  UM_REQUIRE(poses && n_valid && state && c2w && w2c, "um_icp_init: no pointer but correction may be NULL");
+  UM_REQUIRE(n > 0 && n <= 65535, "um_icp_init: bad frame count %d (1 .. 65535)", n);
+  UM_REQUIRE(um::aligned(poses, 8) && um::aligned(correction, 8) && um::aligned(state, 8) && um::aligned(n_valid, 4) &&
+                 um::aligned(c2w, 4) && um::aligned(w2c, 4),
+             "um_icp_init: the fp64 buffers must be 8-byte aligned, the fp32 and int32 buffers 4-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{state, 8LL * UM_ICP_STATE * n}, {c2w, 48LL * n}, {w2c, 48LL * n}, {poses, 128LL * n},
+                                   {correction, 128}, {n_valid, 4}},
+                                  3),
+             "um_icp_init: state, c2w and w2c must not overlap each other or the inputs");
+  return um::icp_init_launch(poses, correction, n, n_valid, state, c2w, w2c, (cudaStream_t)stream);
+}
+
+int um_icp_reduce(const float* depth, const float* live_normal, const float* model_depth, const float* model_normal,
+                  const double* state, const float* c2w, const float* w2c, int32_t n, int32_t h, int32_t w, float fx,
+                  float fy, float cx, float cy, float max_distance, float cos_max_angle, const int32_t* n_valid,
+                  double* partials, void* stream) {
+  UM_REQUIRE(depth && live_normal && model_depth && model_normal && state && c2w && w2c && n_valid && partials,
+             "um_icp_reduce: no pointer may be NULL");
+  UM_REQUIRE(icp_frames(n, h, w), "um_icp_reduce: bad frames (%d x %d x %d; at most 65535 frames of 2^31 - 1 pixels)", n,
+             h, w);
+  UM_REQUIRE(icp_intrinsics(fx, fy, cx, cy), "um_icp_reduce: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(positive_finite(max_distance) && finite_value(cos_max_angle) && cos_max_angle >= -1.f && cos_max_angle <= 1.f,
+             "um_icp_reduce: max_distance must be positive and finite, cos_max_angle in [-1, 1]");
+  UM_REQUIRE(um::aligned(depth, 4) && um::aligned(live_normal, 4) && um::aligned(model_depth, 4) &&
+                 um::aligned(model_normal, 4) && um::aligned(state, 8) && um::aligned(c2w, 4) && um::aligned(w2c, 4) &&
+                 um::aligned(n_valid, 4) && um::aligned(partials, 8),
+             "um_icp_reduce: the fp64 buffers must be 8-byte aligned, the fp32 and int32 buffers 4-byte aligned");
+  const long long px = (long long)n * h * w, nb = (long long)((w + 15) / 16) * ((h + 7) / 8);
+  UM_REQUIRE(um::written_disjoint({{partials, 8LL * UM_ICP_TERMS * nb * n}, {depth, 4 * px}, {live_normal, 12 * px},
+                                   {model_depth, 4 * px}, {model_normal, 12 * px}, {state, 8LL * UM_ICP_STATE * n},
+                                   {c2w, 48LL * n}, {w2c, 48LL * n}, {n_valid, 4}},
+                                  1),
+             "um_icp_reduce: partials must not overlap the inputs");
+  return um::icp_reduce_launch(depth, live_normal, model_depth, model_normal, state, c2w, w2c, n, h, w, fx, fy, cx, cy,
+                               max_distance, cos_max_angle, n_valid, partials, (cudaStream_t)stream);
+}
+
+static bool icp_partials(int32_t nb, int32_t n) { return n > 0 && n <= 65535 && nb > 0; }
+
+int um_icp_solve(const double* partials, int32_t nb, int32_t n, const int32_t* n_valid, double min_inliers,
+                 double min_pivot, int32_t record, double* state, void* stream) {
+  UM_REQUIRE(partials && n_valid && state, "um_icp_solve: no pointer may be NULL");
+  UM_REQUIRE(icp_partials(nb, n), "um_icp_solve: bad partials (%d frames of %d blocks)", n, nb);
+  UM_REQUIRE(min_inliers >= 0.0 && min_inliers <= 1e300 && min_pivot > 0.0 && min_pivot <= 1.0,
+             "um_icp_solve: min_inliers must be finite and >= 0, min_pivot in (0, 1]");
+  UM_REQUIRE(um::aligned(partials, 8) && um::aligned(state, 8) && um::aligned(n_valid, 4),
+             "um_icp_solve: partials and state must be 8-byte aligned, n_valid 4-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{state, 8LL * UM_ICP_STATE * n}, {partials, 8LL * UM_ICP_TERMS * nb * n}, {n_valid, 4}},
+                                  1),
+             "um_icp_solve: state must not overlap the inputs");
+  return um::icp_solve_launch(partials, nb, n, n_valid, min_inliers, min_pivot, record != 0, state, (cudaStream_t)stream);
+}
+
+int um_icp_accept(const double* partials, int32_t nb, int32_t n, const int32_t* n_valid, double min_inlier_fraction,
+                  const double* poses, double* correction, double* state, float* pose_out, uint8_t* tracked,
+                  int64_t* inliers, float* rmse, float* w2c, void* stream) {
+  UM_REQUIRE(partials && n_valid && state && pose_out && tracked && inliers && rmse && w2c,
+             "um_icp_accept: no pointer but poses and correction may be NULL");
+  UM_REQUIRE(icp_partials(nb, n), "um_icp_accept: bad partials (%d frames of %d blocks)", n, nb);
+  UM_REQUIRE(!correction || (poses && n == 1), "um_icp_accept: a correction takes the poses of exactly one frame");
+  UM_REQUIRE(min_inlier_fraction >= 0.0 && min_inlier_fraction <= 1.0,
+             "um_icp_accept: min_inlier_fraction must be in [0, 1]");
+  UM_REQUIRE(um::aligned(partials, 8) && um::aligned(state, 8) && um::aligned(poses, 8) && um::aligned(correction, 8) &&
+                 um::aligned(inliers, 8) && um::aligned(n_valid, 4) && um::aligned(pose_out, 4) && um::aligned(rmse, 4) &&
+                 um::aligned(w2c, 4),
+             "um_icp_accept: the fp64 and int64 buffers must be 8-byte aligned, the fp32 and int32 buffers 4-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{state, 8LL * UM_ICP_STATE * n}, {pose_out, 64LL * n}, {tracked, n}, {inliers, 8LL * n},
+                                   {rmse, 4LL * n}, {w2c, 48LL * n}, {correction, 128},
+                                   {partials, 8LL * UM_ICP_TERMS * nb * n}, {poses, 128LL * n}, {n_valid, 4}},
+                                  7),
+             "um_icp_accept: the outputs must not overlap each other or the inputs");
+  return um::icp_accept_launch(partials, nb, n, n_valid, min_inlier_fraction, poses, correction, state, pose_out, tracked,
+                               inliers, rmse, w2c, (cudaStream_t)stream);
 }
 
 }  // extern "C"

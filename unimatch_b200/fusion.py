@@ -2,7 +2,8 @@
 device depths and frames into it (`fuse_depths`, one `um_tsdf_integrate` launch), the zero-crossing points of its surface
 with their colours (`TSDFVolume.extract_points`), its marching-cubes mesh with per-vertex normals
 (`TSDFVolume.extract_mesh`), its ray-cast depth, colour and normal images from any camera (`TSDFVolume.render`, one
-`um_tsdf_raycast` launch) and a binary PLY writer for the points and meshes (`write_ply`).  The kernels' arithmetic
+`um_tsdf_raycast` launch), the tracking of cameras against it (`TSDFVolume.track`, point-to-plane ICP in the um_icp_*
+launches) and a binary PLY writer for the points and meshes (`write_ply`).  The kernels' arithmetic
 is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
@@ -11,6 +12,7 @@ import numpy as np
 import torch
 
 from .inference import _OPS, _camera_to_world, _intrinsics33, _pose44, _world_to_camera
+from .ops import ICP_STATE, ICP_TERMS, icp_blocks
 
 MAX_VOXELS = 2 ** 31 - 1
 MAX_MESH_INDEX = 2 ** 31 - 1                           # int32 face indices: at most this many vertices and faces
@@ -128,11 +130,147 @@ class TSDFVolume:
                                                      self.trunc, c2w, h, w, fx, fy, cx, cy, near, far)
         return {"depth": depth, "color": color, "normal": normal}
 
+    @torch.no_grad()
+    def track(self, depths, intrinsics, poses, *, levels=3, iterations=(4, 5, 10), max_distance=0.1, max_angle=20.0,
+              min_inlier_fraction=0.3):
+        """Track N cameras against the fused surface: frame-to-model point-to-plane ICP (KinectFusion) on the device.
+        depths: device fp32 [N,H,W] (metric z-depth; zero, negative and non-finite depths are invalid), intrinsics [3,3]
+        at (H, W), host camera-to-world initial poses [N,4,4] (as `fuse_depths` takes them).  Each frame is tracked on
+        its own, coarse to fine over a `levels`-level depth pyramid with `iterations[i]` Gauss-Newton steps on level
+        levels - 1 - i, against the volume ray-cast (`render`) at its initial pose; a pixel pairs with the model pixel
+        its point projects to when they are within `max_distance` metres and their normals within `max_angle` degrees.
+        A frame is tracked when no finest-level step was degenerate and at least `min_inlier_fraction` of its valid
+        pixels are inliers at the end; a frame that is not tracked gets its initial pose back unchanged.  The
+        arithmetic is stated in include/unimatch_sm100.h (um_icp_*).  One upload, a fixed launch sequence and one
+        download.  Returns {'pose': float32 [N,4,4] camera-to-world, 'tracked': bool [N], 'inliers': int64 [N],
+        'rmse': float32 [N] (the inliers' point-to-plane residual, metres)} on the host."""
+        name = "TSDFVolume.track"
+        if not (torch.is_tensor(depths) and depths.is_cuda and depths.dtype == torch.float32 and depths.dim() == 3):
+            raise ValueError("%s: depths must be a device float32 tensor [N,H,W]" % name)
+        if depths.device != self.device:
+            raise ValueError("%s: depths must be on the volume's device" % name)
+        n, h, w = depths.shape
+        K = _intrinsics33(intrinsics, name)
+        ps = [_pose44(p, name) for p in poses]
+        if len(ps) != n:
+            raise ValueError("%s: %d depth maps need %d poses, got %d" % (name, n, n, len(ps)))
+        if not all(np.isfinite(p).all() for p in ps):
+            raise ValueError("%s: camera poses must be finite" % name)
+        if n > 65535:
+            raise ValueError("%s: at most 65535 frames per call" % name)
+        icp = _ICP(self, K, n, h, w, levels, iterations, max_distance, max_angle, min_inlier_fraction, name)
+        out = {"pose": np.zeros((0, 4, 4), np.float32), "tracked": np.zeros(0, bool), "inliers": np.zeros(0, np.int64),
+               "rmse": np.zeros(0, np.float32)}
+        if n == 0:
+            return {k: torch.from_numpy(v) for k, v in out.items()}
+        with torch.cuda.device(self.device):
+            poses64 = torch.from_numpy(np.stack(ps).astype(np.float64)).to(self.device)
+            n_valid = torch.full((1,), n, dtype=torch.int32, device=self.device)
+            packed = torch.empty((77 * n,), dtype=torch.uint8, device=self.device)     # one download
+            views = (packed[:64 * n].view(torch.float32).view(n, 4, 4), packed[76 * n:],
+                     packed[64 * n:72 * n].view(torch.int64), packed[72 * n:76 * n].view(torch.float32))
+            icp.track(*icp.prepare(depths.contiguous()), poses64, n_valid, views)
+            host = packed.cpu().numpy()
+        return {"pose": torch.from_numpy(host[:64 * n].view(np.float32).reshape(n, 4, 4).copy()),
+                "tracked": torch.from_numpy(host[76 * n:].astype(bool)),
+                "inliers": torch.from_numpy(host[64 * n:72 * n].view(np.int64).copy()),
+                "rmse": torch.from_numpy(host[72 * n:76 * n].view(np.float32).copy())}
+
     def _integrate(self, depths, frames, w2c, n_valid, K):
         """One um_tsdf_integrate launch: frames 0 .. n_valid - 1 of device depths [n,H,W] and uint8 frames [n,H,W,3] with
         their world-to-camera rows w2c [n,3,4] (device fp32) and the float32 intrinsics K [3,3] (host)."""
         _OPS.tsdf_integrate(self.tsdf, self.weight, self.color, self.origin, self.voxel_size, self.trunc, depths, frames, w2c,
                             float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), n_valid)
+
+
+ICP_MIN_INLIERS = 36            # 6 x 6: at least as many inliers as the system has unknowns, times six
+ICP_MIN_PIVOT = 1e-2            # smallest Cholesky pivot of the Jacobi-scaled 6 x 6 system (see tests/test_icp_cpu.py)
+
+
+def icp_levels(K, h, w, levels):
+    """[(fx, fy, cx, cy, h, w)] of the depth pyramid's levels, finest first: float32 intrinsics (fx/2, fy/2, (cx - 0.5)/2,
+    (cy - 0.5)/2 per level, so pixel x is centred at x on every level) and floor-halved sizes."""
+    f32 = np.float32
+    fx, fy, cx, cy = (f32(K[0][0]), f32(K[1][1]), f32(K[0][2]), f32(K[1][2]))
+    out = [(fx, fy, cx, cy, h, w)]
+    for _ in range(levels - 1):
+        fx, fy = f32(fx * f32(0.5)), f32(fy * f32(0.5))
+        cx, cy = f32(f32(cx - f32(0.5)) * f32(0.5)), f32(f32(cy - f32(0.5)) * f32(0.5))
+        h, w = h // 2, w // 2
+        out.append((fx, fy, cx, cy, h, w))
+    return [(float(a), float(b), float(c), float(d), hh, ww) for a, b, c, d, hh, ww in out]
+
+
+class _ICP:
+    """The device buffers and the fixed launch sequence of tracking n frames of h x w against `volume`
+    (`TSDFVolume.track`, and `DepthFusionRunner(track=True)` one frame at a time)."""
+
+    def __init__(self, volume, K, n, h, w, levels, iterations, max_distance, max_angle, min_inlier_fraction, name):
+        if isinstance(levels, bool) or not isinstance(levels, int) or levels < 1:
+            raise ValueError("%s: levels must be a positive int" % name)
+        its = tuple(iterations)
+        if len(its) != levels or not all(isinstance(i, int) and not isinstance(i, bool) and i >= 0 for i in its) \
+                or its[-1] < 1:
+            raise ValueError("%s: iterations must give levels non-negative ints, coarse to fine, at least 1 on the finest"
+                             % name)
+        if h >> (levels - 1) < 2 or w >> (levels - 1) < 2 or h * w > MAX_VOXELS:
+            raise ValueError("%s: a %d x %d frame is too small for %d pyramid levels (2 x 2 on the coarsest)"
+                             % (name, h, w, levels))
+        with np.errstate(over="ignore"):
+            max_distance = _f32(max_distance) if math.isfinite(max_distance) else math.nan
+        if not (math.isfinite(max_distance) and max_distance > 0):                # the float32 value the kernel gets
+            raise ValueError("%s: max_distance must be positive and finite in float32" % name)
+        if not (math.isfinite(max_angle) and 0 < max_angle <= 180):
+            raise ValueError("%s: max_angle must be in (0, 180] degrees" % name)
+        if not (math.isfinite(min_inlier_fraction) and 0 <= min_inlier_fraction <= 1):
+            raise ValueError("%s: min_inlier_fraction must be in [0, 1]" % name)
+        fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+        if not (all(math.isfinite(v) for v in (fx, fy, cx, cy)) and fx != 0 and fy != 0):
+            raise ValueError("%s: fx, fy, cx and cy must be finite, fx and fy nonzero" % name)
+        self.volume, self.n = volume, n
+        self.levels = icp_levels(K.numpy(), h, w, levels)
+        self.iterations = its[::-1]                                       # per level, finest first
+        self.max_distance = max_distance
+        self.cos_max_angle = _f32(math.cos(math.radians(max_angle)))
+        self.min_inlier_fraction = float(min_inlier_fraction)
+        dev = volume.device
+        if n:
+            self.state = torch.zeros((n, ICP_STATE), dtype=torch.float64, device=dev)
+            rows = torch.eye(4, dtype=torch.float32, device=dev)[:3].repeat(n, 1, 1)
+            self.c2w, self.w2c = rows.clone(), rows.clone()                # the reference rows
+            self.w2c_out = rows.clone()                                    # the tracked poses' rows
+            self.partials = torch.empty((n * icp_blocks(h, w) * ICP_TERMS,), dtype=torch.float64, device=dev)
+
+    def prepare(self, depth):
+        """The pyramid of device depths [n, h, w] (contiguous fp32) and its live normals, finest first"""
+        pyramid = [depth]
+        for _ in self.levels[1:]:
+            pyramid.append(_OPS.icp_downsample(pyramid[-1], self.volume.trunc))
+        return pyramid, [_OPS.icp_normals(d, *lv[:4]) for d, lv in zip(pyramid, self.levels)]
+
+    def track(self, pyramid, normals, poses64, n_valid, outputs, correction=None):
+        """Launch the schedule for frames 0 .. n_valid - 1: fp64 initial poses [n, 4, 4] (corrected on the left by the fp64
+        [4, 4] `correction` when given, which a tracked frame then updates), outputs = (pose fp32 [n, 4, 4], tracked uint8
+        [n], inliers int64 [n], rmse fp32 [n]); the tracked poses' world-to-camera rows land in `w2c_out`."""
+        v = self.volume
+        _OPS.icp_init(poses64, correction, n_valid, self.state, self.c2w, self.w2c)
+        models = [_OPS.tsdf_raycast(v.tsdf, v.weight, v.color, v.origin, v.voxel_size, v.trunc, self.c2w, lv[4], lv[5],
+                                    *lv[:4], 0.0, math.inf) for lv in self.levels]
+
+        def reduce(level):
+            fx, fy, cx, cy, h, w = self.levels[level]
+            _OPS.icp_reduce(pyramid[level], normals[level], models[level][0], models[level][2], self.state, self.c2w,
+                            self.w2c, fx, fy, cx, cy, self.max_distance, self.cos_max_angle, n_valid, self.partials)
+            return icp_blocks(h, w)
+
+        for level in reversed(range(len(self.levels))):
+            for _ in range(self.iterations[level]):
+                nb = reduce(level)
+                _OPS.icp_solve(self.partials, nb, n_valid, float(ICP_MIN_INLIERS), ICP_MIN_PIVOT, level == 0, self.state)
+        nb = reduce(0)
+        pose, tracked, inliers, rmse = outputs
+        _OPS.icp_accept(self.partials, nb, n_valid, self.min_inlier_fraction, poses64 if correction is not None else None,
+                        correction, self.state, pose, tracked, inliers, rmse, self.w2c_out)
 
 
 def covering_box(intrinsics, poses, frame_size, max_depth, voxel_size, trunc=None):

@@ -1819,12 +1819,21 @@ class DepthFusionRunner(DepthSequenceRunner):
     * the volume persists across `run()` calls, so a long scene can be fed in pieces (each piece's last frame is not fused);
     * `return_depth=False` without `visualize` is allowed: the volume is the result, and `run()` then yields empty dicts
       and downloads nothing.
-    The intrinsics are those of the frames' size, as for `DepthSequenceRunner`."""
+    The intrinsics are those of the frames' size, as for `DepthSequenceRunner`.
+
+    With `track=True` the given poses are corrected before fusion (the network still takes the given relative poses).
+    Each step takes its pairs' frames t in order, inside the step's graph: the predicted pose is C P_t, with P_t the given
+    pose and C `pose_correction` (device fp64 [4,4], identity at first); frame t's depth is tracked against the volume
+    from there (`TSDFVolume.track`'s ICP with its defaults) and fused at the tracked pose, or at the predicted one when it
+    is not tracked; a tracked frame then sets C = T_t P_t^-1.  C persists across `run()` calls with the volume, as it
+    relates the given poses' frame to the volume's: reset both to start a new scene.  Each result gains 'pose' (float32
+    [4,4], the camera-to-world pose frame t was fused at) and 'tracked' (bool), which are all that is downloaded with
+    `return_depth=False` and no pictures."""
 
     def __init__(self, model, frame_size, batch, device, intrinsics, volume, padding_factor=16, inference_size=None,
                  min_depth=0.5, max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
-                 use_graph=True, visualize=False, return_depth=True, **model_kwargs):
-        from .fusion import TSDFVolume
+                 use_graph=True, visualize=False, return_depth=True, track=False, **model_kwargs):
+        from .fusion import TSDFVolume, _ICP
         if pred_bidir_depth:
             raise ValueError("DepthFusionRunner: pred_bidir_depth is refused: the backward depth of frame t+1 would fuse "
                              "frame t+1 twice")
@@ -1845,15 +1854,42 @@ class DepthFusionRunner(DepthSequenceRunner):
         self.w2c_dev = [torch.zeros((self.batch, 3, 4), device=self.dev) for _ in range(2)]
         self.nvalid_pin = [torch.zeros((1,), dtype=torch.int32).pin_memory() for _ in range(2)]
         self.nvalid_dev = [torch.zeros((1,), dtype=torch.int32, device=self.dev) for _ in range(2)]
+        self.track = bool(track)
+        if self.track:
+            self._icp = _ICP(volume, self.K, 1, self.h, self.w, 3, (4, 5, 10), 0.1, 20.0, 0.3, "DepthFusionRunner")
+            self.pose_correction = torch.eye(4, dtype=torch.float64, device=self.dev)
+            self.given_pin = [torch.empty((self.batch, 4, 4), dtype=torch.float64).pin_memory() for _ in range(2)]
+            self.given_dev = [torch.zeros((self.batch, 4, 4), dtype=torch.float64, device=self.dev) for _ in range(2)]
+            self.real_pin = [torch.zeros((self.batch,), dtype=torch.int32).pin_memory() for _ in range(2)]
+            self.real_dev = [torch.zeros((self.batch,), dtype=torch.int32, device=self.dev) for _ in range(2)]
 
     def _match(self, slot, first, second):
         out = _depth_outputs(self._depth(slot, first, second), self.ori, self.size, False)
         frames = torch.cat((self.carry_frame, self.dev_in[slot][:-1]), dim=0)        # frame t of every pair
-        self.volume._integrate(out["depth"].contiguous(), frames, self.w2c_dev[slot], self.nvalid_dev[slot], self.K)
+        poses = self._track_and_fuse(slot, out["depth"].contiguous(), frames) if self.track else {}
+        if not self.track:
+            self.volume._integrate(out["depth"].contiguous(), frames, self.w2c_dev[slot], self.nvalid_dev[slot], self.K)
         self.carry_frame.copy_(self.dev_in[slot][-1:])
         if self.visualize:
-            return _colour_outputs(out, "depth", depth_to_image, self.return_depth)
-        return out if self.return_depth else {}
+            return dict(_colour_outputs(out, "depth", depth_to_image, self.return_depth), **poses)
+        return dict(out, **poses) if self.return_depth else poses
+
+    def _track_and_fuse(self, slot, depth, frames):
+        """Frames t in order: track against the volume from C P_t, fuse at the result, update C; padding pairs (real
+        flag 0) are untouched.  Returns the step's 'pose' [batch,4,4] and 'tracked' [batch]."""
+        b = self.batch
+        pose = torch.empty((b, 4, 4), dtype=torch.float32, device=self.dev)
+        tracked = torch.empty((b,), dtype=torch.uint8, device=self.dev)
+        inliers = torch.empty((b,), dtype=torch.int64, device=self.dev)
+        rmse = torch.empty((b,), dtype=torch.float32, device=self.dev)
+        pyramid, normals = self._icp.prepare(depth)
+        for t in range(b):
+            real = self.real_dev[slot][t:t + 1]
+            self._icp.track([p[t:t + 1] for p in pyramid], [n[t:t + 1] for n in normals], self.given_dev[slot][t:t + 1],
+                            real, (pose[t:t + 1], tracked[t:t + 1], inliers[t:t + 1], rmse[t:t + 1]),
+                            correction=self.pose_correction)
+            self.volume._integrate(depth[t:t + 1], frames[t:t + 1], self._icp.w2c_out, real, self.K)
+        return {"pose": pose, "tracked": tracked.view(torch.bool)}
 
     def _prime(self, frame):
         super()._prime(frame)
@@ -1862,14 +1898,22 @@ class DepthFusionRunner(DepthSequenceRunner):
     def _reset_inputs(self, slot):
         super()._reset_inputs(slot)
         self.nvalid_dev[slot].zero_()
+        if self.track:
+            self.real_dev[slot].zero_()
 
     def _stage_step_poses(self, slot, poses, n_real):
-        """the relative poses, then the world-to-camera rows of the pairs' frames t and the number of real pairs"""
+        """the relative poses, then the world-to-camera rows of the pairs' frames t and the number of real pairs (with
+        `track`, also the frames' given poses in fp64 and a 0 / 1 flag per pair)"""
         super()._stage_step_poses(slot, poses, n_real)
         self.w2c_pin[slot].copy_(torch.from_numpy(_world_to_camera(poses[:-1])))
         self.nvalid_pin[slot][0] = n_real
         self.w2c_dev[slot].copy_(self.w2c_pin[slot], non_blocking=True)
         self.nvalid_dev[slot].copy_(self.nvalid_pin[slot], non_blocking=True)
+        if self.track:
+            self.given_pin[slot].copy_(torch.from_numpy(np.stack(poses[:-1]).astype(np.float64)))
+            self.real_pin[slot].copy_(torch.arange(self.batch) < n_real)
+            self.given_dev[slot].copy_(self.given_pin[slot], non_blocking=True)
+            self.real_dev[slot].copy_(self.real_pin[slot], non_blocking=True)
 
 
 def _depth_step_layout(sizes, batch, pred_bidir_depth):

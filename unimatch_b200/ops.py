@@ -91,7 +91,7 @@ class FfnDesc(ctypes.Structure):
                 ("split_plane_stride", ctypes.c_int64)]
 
 
-_P, _I, _L, _F = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float
+_P, _I, _L, _F, _D = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_float, ctypes.c_double
 _G, _FP, _RC = ctypes.POINTER(AttnGeom), ctypes.POINTER(ctypes.c_float), ctypes.c_int
 _PP = ctypes.POINTER(ctypes.c_void_p)
 
@@ -125,6 +125,12 @@ _SIGNATURES = {
     "um_tsdf_mesh_count": (_RC, [_P, _P, _I, _I, _I, _P, _P]),
     "um_tsdf_mesh": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _P, _L, _P, _L, _P, _P, _P, _P, _P, _P]),
     "um_tsdf_raycast": (_RC, [_P, _P, _P, _I, _I, _I, _FP, _F, _F, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _P, _P]),
+    "um_icp_downsample": (_RC, [_P, _P, _I, _I, _I, _F, _P]),
+    "um_icp_normals": (_RC, [_P, _P, _I, _I, _I, _F, _F, _F, _F, _P]),
+    "um_icp_init": (_RC, [_P, _P, _I, _P, _P, _P, _P, _P]),
+    "um_icp_reduce": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _P]),
+    "um_icp_solve": (_RC, [_P, _I, _I, _P, _D, _D, _I, _P, _P]),
+    "um_icp_accept": (_RC, [_P, _I, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -658,6 +664,143 @@ tsdf_raycast = _define(
     "tsdf_raycast(Tensor tsdf, Tensor weight, Tensor color, float[] origin, float voxel_size, float trunc, Tensor c2w, "
     "int h, int w, float fx, float fy, float cx, float cy, float near, float far) -> (Tensor, Tensor, Tensor)",
     _tsdf_raycast)
+
+
+# ---- ICP tracking against the TSDF volume (include/unimatch_sm100.h, um_icp_*) -------------------------------------
+ICP_TERMS = 30                                       # UM_ICP_TERMS: fp64 sums per frame and block of the association
+ICP_STATE = 32                                       # UM_ICP_STATE: fp64 state words per frame
+
+
+def icp_blocks(h, w):
+    """The association's blocks per frame at h x w pixels (16 x 8 tiles)"""
+    return -(-w // 16) * -(-h // 8)
+
+
+def _device_like(name, ref, *tensors):
+    if any(t.device != ref.device for t in tensors):
+        raise RuntimeError("%s: every tensor must be on one device" % name)
+
+
+def _icp_downsample(src, trunc):
+    """The next pyramid level of depths [n, h, w] (contiguous fp32): [n, h // 2, w // 2]"""
+    _f32c(src, "icp_downsample: src")
+    if src.dim() != 3:
+        raise RuntimeError("icp_downsample: expected depths [n, h, w]")
+    n, h, w = src.shape
+    dst = torch.empty((n, h // 2, w // 2), device=src.device, dtype=torch.float32)
+    _check(LIB.um_icp_downsample(_p(src), _p(dst), n, h, w, trunc, _stream()), "um_icp_downsample")
+    return dst
+
+
+icp_downsample = _define("icp_downsample(Tensor src, float trunc) -> Tensor", _icp_downsample)
+
+
+def _icp_normals(depth, fx, fy, cx, cy):
+    """The live normals fp32 [n, h, w, 3] of depths [n, h, w] (contiguous fp32), 0 where invalid"""
+    _f32c(depth, "icp_normals: depth")
+    if depth.dim() != 3:
+        raise RuntimeError("icp_normals: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    normal = torch.empty((n, h, w, 3), device=depth.device, dtype=torch.float32)
+    _check(LIB.um_icp_normals(_p(depth), _p(normal), n, h, w, fx, fy, cx, cy, _stream()), "um_icp_normals")
+    return normal
+
+
+icp_normals = _define("icp_normals(Tensor depth, float fx, float fy, float cx, float cy) -> Tensor", _icp_normals)
+
+
+def _icp_init(poses, correction, n_valid, state, c2w, w2c):
+    """Initialise the state fp64 [n, ICP_STATE] and the reference rows c2w / w2c fp32 [n, 3, 4] of fp64 poses [n, 4, 4]
+    (optionally corrected on the left by fp64 correction [4, 4]), in place; n_valid: device int32 [1]."""
+    n = poses.shape[0]
+    for t, shape, dt in ((poses, (n, 4, 4), torch.float64), (state, (n, ICP_STATE), torch.float64),
+                         (c2w, (n, 3, 4), torch.float32), (w2c, (n, 3, 4), torch.float32),
+                         (n_valid, (1,), torch.int32)) + (((correction, (4, 4), torch.float64),) if correction is not None else ()):
+        if tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous() or not t.is_cuda:
+            raise RuntimeError("icp_init: expected contiguous device %s %s" % (dt, list(shape)))
+    _device_like("icp_init", poses, state, c2w, w2c, n_valid, *([correction] if correction is not None else []))
+    _check(LIB.um_icp_init(_p(poses), _p(correction), n, _p(n_valid), _p(state), _p(c2w), _p(w2c), _stream()), "um_icp_init")
+
+
+icp_init = _define("icp_init(Tensor poses, Tensor? correction, Tensor n_valid, Tensor(a!) state, Tensor(b!) c2w, "
+                   "Tensor(c!) w2c) -> ()", _icp_init)
+
+
+def _icp_reduce(depth, live_normal, model_depth, model_normal, state, c2w, w2c, fx, fy, cx, cy, max_distance,
+                cos_max_angle, n_valid, partials):
+    """The association pass at one level: depth / model_depth [n, h, w], live_normal / model_normal [n, h, w, 3] (contiguous
+    fp32) -> the block partials, written to the first n * icp_blocks(h, w) * ICP_TERMS words of partials (fp64)."""
+    for t, nm in ((depth, "depth"), (live_normal, "live_normal"), (model_depth, "model_depth"),
+                  (model_normal, "model_normal"), (c2w, "c2w"), (w2c, "w2c")):
+        _f32c(t, "icp_reduce: " + nm)
+    if depth.dim() != 3:
+        raise RuntimeError("icp_reduce: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    if tuple(model_depth.shape) != (n, h, w) or tuple(live_normal.shape) != (n, h, w, 3) \
+            or tuple(model_normal.shape) != (n, h, w, 3) or tuple(c2w.shape) != (n, 3, 4) or tuple(w2c.shape) != (n, 3, 4):
+        raise RuntimeError("icp_reduce: the maps must be [n, h, w] / [n, h, w, 3] and the rows [n, 3, 4]")
+    if state.dtype != torch.float64 or tuple(state.shape) != (n, ICP_STATE) or partials.dtype != torch.float64 \
+            or not partials.is_contiguous() or partials.numel() < n * icp_blocks(h, w) * ICP_TERMS:
+        raise RuntimeError("icp_reduce: state must be fp64 [n, %d] and partials fp64 with room for the blocks" % ICP_STATE)
+    if n_valid.dtype != torch.int32 or n_valid.numel() != 1:
+        raise RuntimeError("icp_reduce: n_valid must be one device int32")
+    _device_like("icp_reduce", depth, live_normal, model_depth, model_normal, state, c2w, w2c, n_valid, partials)
+    _check(LIB.um_icp_reduce(_p(depth), _p(live_normal), _p(model_depth), _p(model_normal), _p(state), _p(c2w), _p(w2c), n,
+                             h, w, fx, fy, cx, cy, max_distance, cos_max_angle, _p(n_valid), _p(partials), _stream()),
+           "um_icp_reduce")
+
+
+icp_reduce = _define(
+    "icp_reduce(Tensor depth, Tensor live_normal, Tensor model_depth, Tensor model_normal, Tensor state, Tensor c2w, "
+    "Tensor w2c, float fx, float fy, float cx, float cy, float max_distance, float cos_max_angle, Tensor n_valid, "
+    "Tensor(a!) partials) -> ()", _icp_reduce)
+
+
+def _icp_partials(partials, state, n_valid, nb, name):
+    n = state.shape[0]
+    if state.dtype != torch.float64 or state.dim() != 2 or state.shape[1] != ICP_STATE or not state.is_contiguous():
+        raise RuntimeError("%s: state must be contiguous fp64 [n, %d]" % (name, ICP_STATE))
+    if partials.dtype != torch.float64 or not partials.is_contiguous() or partials.numel() < n * nb * ICP_TERMS or nb < 1:
+        raise RuntimeError("%s: partials must be contiguous fp64 with %d blocks per frame" % (name, nb))
+    if n_valid.dtype != torch.int32 or n_valid.numel() != 1:
+        raise RuntimeError("%s: n_valid must be one device int32" % name)
+    _device_like(name, state, partials, n_valid)
+    return n
+
+
+def _icp_solve(partials, nb, n_valid, min_inliers, min_pivot, record, state):
+    """One Gauss-Newton step per frame from the partials of nb blocks per frame, applied to state in place"""
+    n = _icp_partials(partials, state, n_valid, nb, "icp_solve")
+    _check(LIB.um_icp_solve(_p(partials), nb, n, _p(n_valid), min_inliers, min_pivot, int(record), _p(state), _stream()),
+           "um_icp_solve")
+
+
+icp_solve = _define("icp_solve(Tensor partials, int nb, Tensor n_valid, float min_inliers, float min_pivot, bool record, "
+                    "Tensor(a!) state) -> ()", _icp_solve)
+
+
+def _icp_accept(partials, nb, n_valid, min_inlier_fraction, poses, correction, state, pose_out, tracked, inliers, rmse, w2c):
+    """Acceptance of each frame from the last association pass: writes pose_out fp32 [n, 4, 4], tracked uint8 [n],
+    inliers int64 [n], rmse fp32 [n] and w2c fp32 [n, 3, 4]; with correction (fp64 [4, 4], n == 1) and poses (fp64
+    [n, 4, 4]) a tracked frame updates the correction."""
+    n = _icp_partials(partials, state, n_valid, nb, "icp_accept")
+    for t, shape, dt in ((pose_out, (n, 4, 4), torch.float32), (tracked, (n,), torch.uint8), (inliers, (n,), torch.int64),
+                         (rmse, (n,), torch.float32), (w2c, (n, 3, 4), torch.float32)):
+        if tuple(t.shape) != shape or t.dtype != dt or not t.is_contiguous():
+            raise RuntimeError("icp_accept: expected contiguous %s %s outputs" % (dt, list(shape)))
+    if correction is not None and (poses is None or tuple(correction.shape) != (4, 4) or correction.dtype != torch.float64
+                                   or tuple(poses.shape) != (n, 4, 4) or poses.dtype != torch.float64):
+        raise RuntimeError("icp_accept: a correction takes fp64 [4, 4] and the frame's fp64 poses [1, 4, 4]")
+    _device_like("icp_accept", state, pose_out, tracked, inliers, rmse, w2c,
+                 *[t for t in (poses, correction) if t is not None])
+    _check(LIB.um_icp_accept(_p(partials), nb, n, _p(n_valid), min_inlier_fraction, _p(poses), _p(correction), _p(state),
+                             _p(pose_out), _p(tracked), _p(inliers), _p(rmse), _p(w2c), _stream()), "um_icp_accept")
+
+
+icp_accept = _define(
+    "icp_accept(Tensor partials, int nb, Tensor n_valid, float min_inlier_fraction, Tensor? poses, Tensor(a!)? correction, "
+    "Tensor(b!) state, Tensor(c!) pose_out, Tensor(d!) tracked, Tensor(e!) inliers, Tensor(f!) rmse, Tensor(g!) w2c) -> ()",
+    _icp_accept)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
