@@ -30,8 +30,8 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing, ray casting and ICP) leave existing callers
- * working and keep it. */
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing, ray casting, ICP and the
+ * point-cloud ops) leave existing callers working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
@@ -593,6 +593,57 @@ int um_icp_solve(const double* partials, int32_t nb, int32_t n, const int32_t* n
 int um_icp_accept(const double* partials, int32_t nb, int32_t n, const int32_t* n_valid, double min_inlier_fraction,
                   const double* poses, double* correction, double* state, float* pose_out, uint8_t* tracked,
                   int64_t* inliers, float* rmse, float* w2c, void* stream);
+
+/* ---- point clouds: exact nearest neighbours, voxel down-sampling and the 3D metrics of a reconstruction -------------
+ * Points are fp32 [n, 3] (x, y, z), at most 2^31 - 1 per set.  fp64 operations are __dsub_rn / __ddiv_rn / ... in the
+ * order written.
+ * Grid (origin o, cell size c > 0, dims g[3] >= 1, all fp64 / int32 by value): the cell coordinate of a point along axis a
+ *   is t_a = ((double)p_a - o_a) / c, its cell k_a = floor(t_a) clamped to [0, g_a - 1], and its key
+ *   (k_z * g_y + k_y) * g_x + k_x (int64, x fastest).  um_cloud_keys writes the keys.
+ * Table (um_cloud_ranges): given the keys sorted stably with their input positions (order), start[c] / end[c] (int32
+ *   [g_x g_y g_z], zeroed by the entry) are the first and one-past-last sorted positions of cell c (0 and 0 for an empty
+ *   cell; keys outside the table are not entered), and sorted[i] = (x, y, z, bits of (int32) order[i]) fp32 [n, 4].
+ * Down-sampling (Open3D's VoxelDownSample): with v the voxel size, o = min_bound - v / 2 in fp64 (min_bound the set's
+ *   per-axis minimum) and g_a = floor((max_bound_a - o_a) / v) + 1 computed as t is, every point lies in the grid, so the
+ *   clamp never applies.  um_cloud_down_sample_count: per block of 256 sorted positions the number of runs of equal keys
+ *   that start in it, then one CTA's ordered exclusive scan in place, the total M at offsets[nb], nb = ceil(n / 256).
+ *   um_cloud_down_sample: run m (in key order) writes out[m] = (float)(s / count) per axis, s the fp64 sum from 0.0 of
+ *   (double)p over the run in sorted order, which a stable sort makes the input order.
+ * Nearest neighbour (um_cloud_nearest, one query q per thread) over the table of an indexed set P whose grid box holds
+ *   it (o at or below its minimum, g_a c at or above its extent): dx = q.x - p.x, dy, dz likewise (fp32), s =
+ *   fmaf(dz, dz, fmaf(dy, dy, dx * dx)); the neighbour is the p of least s, ties to the least input index; distance =
+ *   sqrtf(s) correctly rounded, index int64.  This equals a brute-force fp32 scan bit for bit whatever c is.
+ *   Search: cells of Chebyshev rings r = 0, 1, ... around the query's clamped cell j, clamped to the table.  Per axis the
+ *   gap of cell k is G_a(k) = max(0, max(k - t_a, t_a - (k + 1), 0) - (2^-20 + 2^-45 |t_a|)) * c (fp64).
+ *   Proof that a skipped cell cannot hold p with s <= best: a point of cell k has exact cell coordinate T in
+ *   [k - 2^-29, k + 1 + 2^-29] (two fp64 roundings of a value below 2^22 cells, the box holding the set); the query's
+ *   t_a = ((double)q_a - o_a) * rcp(c) (rcp correctly rounded: three roundings) is within 2^-51 |t| of its exact value, and the gap's own rounding is below 2^-31 + 2^-53 |t| cells, so the exact
+ *   |q_a - p_a| >= G_a(k).  The fp32 s is at least (1 - 5 * 2^-24) times the exact squared distance less 6 * 2^-150 (five
+ *   roundings, each within 2^-24 relative or 2^-150 absolute).  So a region whose fp64 bound B = sum of G_a^2 satisfies
+ *   B * (1 - 2^-20) - 2^-140 > best (the fp64 rounding of B is below 2^-50 relative) holds no p with s <= best.
+ *   A cell is skipped when its own B passes that test; the search stops before ring r when the bound of every cell at
+ *   Chebyshev distance >= r, min over axes a and sides +-1 with j_a +- r inside the table of G_a(j_a +- r)^2 + the
+ *   other two axes' G_b(j_b)^2 (G is monotone away from j and least at j), passes it, or when no such side is left (the
+ *   rings covered the table).  A query outside the box starts from its nearest box cell; its t carries its distance.
+ *   With distance / index, writes them [nq]; with partial_sum / partial_count (fp64 / int64 [ceil(nq / 256)]) instead,
+ *   per block of 256 queries the sum of (double)d (per warp a shfl_down tree 16, 8, 4, 2, 1 from lane 0, then the 8
+ *   warps in order) and the count of d < threshold (fp32, strict).
+ * Stats (um_cloud_stats, one warp): lane l adds the partials of blocks l, l + 32, ... in order from 0.0, then a
+ *   shfl_down tree (16, 8, 4, 2, 1); out[0] = the sum of d, out[1] = the count as a double (exact).  No atomics
+ *   anywhere: every result is the same from run to run.
+ * Every pointer is DEVICE memory; no output overlaps an input or another output. */
+int um_cloud_keys(const float* points, int64_t n, double ox, double oy, double oz, double cell, int32_t gx, int32_t gy,
+                  int32_t gz, int64_t* keys, void* stream);
+int um_cloud_ranges(const int64_t* sorted_keys, const int64_t* order, const float* points, int64_t n, int32_t gx,
+                    int32_t gy, int32_t gz, int32_t* start, int32_t* end, float* sorted_points, void* stream);
+int um_cloud_down_sample_count(const int64_t* sorted_keys, int64_t n, int64_t* offsets, void* stream);
+int um_cloud_down_sample(const int64_t* sorted_keys, const int64_t* order, const float* points, int64_t n,
+                         const int64_t* offsets, int64_t m, float* out, void* stream);
+int um_cloud_nearest(const float* queries, int64_t nq, const float* sorted_points, const int32_t* start,
+                     const int32_t* end, int64_t n, double ox, double oy, double oz, double cell, int32_t gx, int32_t gy,
+                     int32_t gz, float threshold, float* distance, int64_t* index, double* partial_sum,
+                     int64_t* partial_count, void* stream);
+int um_cloud_stats(const double* partial_sum, const int64_t* partial_count, int64_t nb, double* out, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -47,6 +47,10 @@ _LAZY = {
     "TSDFVolume": (".fusion", "TSDFVolume"),
     "fuse_depths": (".fusion", "fuse_depths"),
     "write_ply": (".fusion", "write_ply"),
+    "read_ply": (".fusion", "read_ply"),
+    "nearest_neighbors": (".fusion", "nearest_neighbors"),
+    "voxel_down_sample": (".fusion", "voxel_down_sample"),
+    "reconstruction_metrics": (".evaluation", "reconstruction_metrics"),
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
@@ -65,7 +69,8 @@ __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "In
            "MixedSizeStereoRunner", "MixedSizeFlowRunner", "MixedSizeDepthRunner", "disparity_to_image", "depth_to_image",
            "validate_flow", "validate_stereo", "validate_depth", "tapvid_metrics", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth", "warp_disparity", "infer_scene_flow", "SceneFlowRunner",
-           "validate_scene_flow", "create_scene_flow_submission", "DepthFusionRunner", "TSDFVolume", "fuse_depths", "write_ply"]
+           "validate_scene_flow", "create_scene_flow_submission", "DepthFusionRunner", "TSDFVolume", "fuse_depths", "write_ply",
+           "read_ply", "nearest_neighbors", "voxel_down_sample", "reconstruction_metrics"]
 
 
 def __getattr__(name):

@@ -1,6 +1,7 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
 // between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu),
-// TSDF fusion (um_fusion.cu) and ICP tracking against the volume (um_icp.cu).  See include/unimatch_sm100.h.
+// TSDF fusion (um_fusion.cu), ICP tracking against the volume (um_icp.cu) and the point-cloud ops (um_cloud.cu).  See
+// include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -80,6 +81,18 @@ int icp_solve_launch(const double* partials, int nb, int n, const int* n_valid, 
 int icp_accept_launch(const double* partials, int nb, int n, const int* n_valid, double min_inlier_fraction,
                       const double* poses, double* correction, double* state, float* pose_out, uint8_t* tracked,
                       int64_t* inliers, float* rmse, float* w2c, cudaStream_t st);
+int cloud_keys_launch(const float* points, long long n, const double* origin, double cell, const int* dims,
+                      long long* keys, cudaStream_t st);
+int cloud_ranges_launch(const long long* keys, const long long* order, const float* points, long long n, long long n_cells,
+                        int* start, int* end, float* sorted, cudaStream_t st);
+int cloud_down_sample_count_launch(const long long* keys, long long n, long long* offsets, cudaStream_t st);
+int cloud_down_sample_launch(const long long* keys, const long long* order, const float* points, long long n,
+                             const long long* offsets, float* out, cudaStream_t st);
+int cloud_nearest_launch(const float* queries, long long nq, const float* sorted, const int* start, const int* end,
+                         const double* origin, double cell, const int* dims, float threshold, float* distance,
+                         long long* index, double* partial_sum, long long* partial_count, cudaStream_t st);
+int cloud_stats_launch(const double* partial_sum, const long long* partial_count, long long nb, double* out,
+                       cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -536,6 +549,120 @@ int um_icp_accept(const double* partials, int32_t nb, int32_t n, const int32_t* 
              "um_icp_accept: the outputs must not overlap each other or the inputs");
   return um::icp_accept_launch(partials, nb, n, n_valid, min_inlier_fraction, poses, correction, state, pose_out, tracked,
                                inliers, rmse, w2c, (cudaStream_t)stream);
+}
+
+// ---- point clouds (um_cloud.cu) ----
+static const long long kCloudMax = 0x7fffffffLL;            // int32 input indices and table positions
+
+static long long cloud_blocks(long long n) { return (n + 255) / 256; }
+
+// A grid: a finite origin, a positive finite cell size and 1 .. 2^21 cells per axis.
+static bool cloud_grid(double ox, double oy, double oz, double cell, int32_t gx, int32_t gy, int32_t gz) {
+  const double lim = 1.7976931348623157e308;
+  return ox >= -lim && ox <= lim && oy >= -lim && oy <= lim && oz >= -lim && oz <= lim && cell > 0.0 && cell <= lim &&
+         gx >= 1 && gy >= 1 && gz >= 1 && gx <= (1 << 21) && gy <= (1 << 21) && gz <= (1 << 21);
+}
+
+int um_cloud_keys(const float* points, int64_t n, double ox, double oy, double oz, double cell, int32_t gx, int32_t gy,
+                  int32_t gz, int64_t* keys, void* stream) {
+  UM_REQUIRE(n >= 0 && n <= kCloudMax, "um_cloud_keys: bad point count %lld (0 .. 2^31 - 1)", (long long)n);
+  UM_REQUIRE(n == 0 || (points && keys), "um_cloud_keys: points and keys must not be NULL");
+  UM_REQUIRE(cloud_grid(ox, oy, oz, cell, gx, gy, gz),
+             "um_cloud_keys: bad grid (finite origin, positive finite cell, 1 .. 2^21 cells per axis)");
+  UM_REQUIRE(um::aligned(points, 4) && um::aligned(keys, 8), "um_cloud_keys: points 4-byte, keys 8-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{keys, 8 * n}, {points, 12 * n}}, 1), "um_cloud_keys: keys must not overlap points");
+  if (n == 0) return UM_OK;
+  const double o[3] = {ox, oy, oz};
+  const int g[3] = {gx, gy, gz};
+  return um::cloud_keys_launch(points, n, o, cell, g, reinterpret_cast<long long*>(keys), (cudaStream_t)stream);
+}
+
+int um_cloud_ranges(const int64_t* sorted_keys, const int64_t* order, const float* points, int64_t n, int32_t gx,
+                    int32_t gy, int32_t gz, int32_t* start, int32_t* end, float* sorted_points, void* stream) {
+  UM_REQUIRE(sorted_keys && order && points && start && end && sorted_points, "um_cloud_ranges: no pointer may be NULL");
+  UM_REQUIRE(n >= 1 && n <= kCloudMax, "um_cloud_ranges: bad point count %lld (1 .. 2^31 - 1)", (long long)n);
+  UM_REQUIRE(gx >= 1 && gy >= 1 && gz >= 1 && (long long)gx * gy * gz <= kCloudMax,
+             "um_cloud_ranges: bad table %d x %d x %d (at most 2^31 - 1 cells)", gx, gy, gz);
+  UM_REQUIRE(um::aligned(sorted_keys, 8) && um::aligned(order, 8) && um::aligned(points, 4) && um::aligned(start, 4) &&
+                 um::aligned(end, 4) && um::aligned(sorted_points, 16),
+             "um_cloud_ranges: keys and order 8-byte, points and tables 4-byte, sorted_points 16-byte aligned");
+  const long long c = (long long)gx * gy * gz;
+  UM_REQUIRE(um::written_disjoint({{start, 4 * c}, {end, 4 * c}, {sorted_points, 16 * n}, {sorted_keys, 8 * n},
+                                   {order, 8 * n}, {points, 12 * n}},
+                                  3),
+             "um_cloud_ranges: the tables and sorted_points must not overlap each other or the inputs");
+  return um::cloud_ranges_launch(reinterpret_cast<const long long*>(sorted_keys), reinterpret_cast<const long long*>(order),
+                                 points, n, c, start, end, sorted_points, (cudaStream_t)stream);
+}
+
+int um_cloud_down_sample_count(const int64_t* sorted_keys, int64_t n, int64_t* offsets, void* stream) {
+  UM_REQUIRE(sorted_keys && offsets, "um_cloud_down_sample_count: no pointer may be NULL");
+  UM_REQUIRE(n >= 1 && n <= kCloudMax, "um_cloud_down_sample_count: bad point count %lld (1 .. 2^31 - 1)", (long long)n);
+  UM_REQUIRE(um::aligned(sorted_keys, 8) && um::aligned(offsets, 8),
+             "um_cloud_down_sample_count: keys and offsets must be 8-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{offsets, 8 * (cloud_blocks(n) + 1)}, {sorted_keys, 8 * n}}, 1),
+             "um_cloud_down_sample_count: offsets must not overlap the keys");
+  return um::cloud_down_sample_count_launch(reinterpret_cast<const long long*>(sorted_keys), n,
+                                            reinterpret_cast<long long*>(offsets), (cudaStream_t)stream);
+}
+
+int um_cloud_down_sample(const int64_t* sorted_keys, const int64_t* order, const float* points, int64_t n,
+                         const int64_t* offsets, int64_t m, float* out, void* stream) {
+  UM_REQUIRE(sorted_keys && order && points && offsets && out, "um_cloud_down_sample: no pointer may be NULL");
+  UM_REQUIRE(n >= 1 && n <= kCloudMax && m >= 1 && m <= n, "um_cloud_down_sample: bad counts (%lld points, %lld cells)",
+             (long long)n, (long long)m);
+  UM_REQUIRE(um::aligned(sorted_keys, 8) && um::aligned(order, 8) && um::aligned(offsets, 8) && um::aligned(points, 4) &&
+                 um::aligned(out, 4),
+             "um_cloud_down_sample: keys, order and offsets 8-byte, points and out 4-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{out, 12 * m}, {sorted_keys, 8 * n}, {order, 8 * n}, {points, 12 * n},
+                                   {offsets, 8 * (cloud_blocks(n) + 1)}},
+                                  1),
+             "um_cloud_down_sample: out must not overlap the inputs");
+  return um::cloud_down_sample_launch(reinterpret_cast<const long long*>(sorted_keys),
+                                      reinterpret_cast<const long long*>(order), points, n,
+                                      reinterpret_cast<const long long*>(offsets), out, (cudaStream_t)stream);
+}
+
+int um_cloud_nearest(const float* queries, int64_t nq, const float* sorted_points, const int32_t* start,
+                     const int32_t* end, int64_t n, double ox, double oy, double oz, double cell, int32_t gx, int32_t gy,
+                     int32_t gz, float threshold, float* distance, int64_t* index, double* partial_sum,
+                     int64_t* partial_count, void* stream) {
+  UM_REQUIRE(nq >= 0 && nq <= kCloudMax && n >= 1 && n <= kCloudMax,
+             "um_cloud_nearest: bad counts (%lld queries, %lld points; 0 .. 2^31 - 1 queries, 1 .. 2^31 - 1 points)",
+             (long long)nq, (long long)n);
+  UM_REQUIRE(sorted_points && start && end && (nq == 0 || queries), "um_cloud_nearest: no input may be NULL");
+  UM_REQUIRE((distance && index && !partial_sum && !partial_count) || (!distance && !index && partial_sum && partial_count),
+             "um_cloud_nearest: give distance and index, or partial_sum and partial_count");
+  UM_REQUIRE(cloud_grid(ox, oy, oz, cell, gx, gy, gz) && (long long)gx * gy * gz <= kCloudMax,
+             "um_cloud_nearest: bad grid (finite origin, positive finite cell, 1 .. 2^21 cells per axis, at most 2^31 - 1)");
+  UM_REQUIRE(!partial_sum || (threshold > 0.f && threshold <= 3.402823466e38f),
+             "um_cloud_nearest: threshold must be positive and finite");
+  UM_REQUIRE(um::aligned(queries, 4) && um::aligned(sorted_points, 16) && um::aligned(start, 4) && um::aligned(end, 4) &&
+                 um::aligned(distance, 4) && um::aligned(index, 8) && um::aligned(partial_sum, 8) &&
+                 um::aligned(partial_count, 8),
+             "um_cloud_nearest: sorted_points 16-byte, index and partials 8-byte, the rest 4-byte aligned");
+  const long long c = (long long)gx * gy * gz, nb = cloud_blocks(nq);
+  UM_REQUIRE(um::written_disjoint({{distance, 4 * nq}, {index, 8 * nq}, {partial_sum, 8 * nb}, {partial_count, 8 * nb},
+                                   {queries, 12 * nq}, {sorted_points, 16 * n}, {start, 4 * c}, {end, 4 * c}},
+                                  4),
+             "um_cloud_nearest: the outputs must not overlap each other or the inputs");
+  if (nq == 0) return UM_OK;
+  const double o[3] = {ox, oy, oz};
+  const int g[3] = {gx, gy, gz};
+  return um::cloud_nearest_launch(queries, nq, sorted_points, start, end, o, cell, g, threshold, distance,
+                                  reinterpret_cast<long long*>(index), partial_sum,
+                                  reinterpret_cast<long long*>(partial_count), (cudaStream_t)stream);
+}
+
+int um_cloud_stats(const double* partial_sum, const int64_t* partial_count, int64_t nb, double* out, void* stream) {
+  UM_REQUIRE(out && (nb == 0 || (partial_sum && partial_count)), "um_cloud_stats: no pointer may be NULL");
+  UM_REQUIRE(nb >= 0 && nb <= cloud_blocks(kCloudMax), "um_cloud_stats: bad block count %lld", (long long)nb);
+  UM_REQUIRE(um::aligned(partial_sum, 8) && um::aligned(partial_count, 8) && um::aligned(out, 8),
+             "um_cloud_stats: the buffers must be 8-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{out, 16}, {partial_sum, 8 * nb}, {partial_count, 8 * nb}}, 1),
+             "um_cloud_stats: out must not overlap the partials");
+  return um::cloud_stats_launch(partial_sum, reinterpret_cast<const long long*>(partial_count), nb, out,
+                                (cudaStream_t)stream);
 }
 
 }  // extern "C"

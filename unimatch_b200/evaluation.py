@@ -21,7 +21,11 @@ reference loop -- including its quirks, listed in each driver's docstring.
 (`um_scene_flow_stats`), on the same batching and single download.
 
 `tapvid_metrics` scores point tracks (e.g. `PointTrackRunner`'s) with TAP-Vid's metrics, in numpy on the host.
+
+`reconstruction_metrics` scores a fused reconstruction against a reference surface with Atlas's 3D metrics (accuracy,
+completeness, precision, recall, F-score), from exact nearest neighbours on the device (`um_cloud_*`).
 """
+import math
 import os
 
 import numpy as np
@@ -484,3 +488,54 @@ def tapvid_metrics(query_points, gt_occluded, gt_tracks, pred_occluded, pred_tra
     out["average_pts_within_thresh"] = np.mean([out["pts_within_%d" % d] for d in TAPVID_THRESHOLDS], axis=0)
     out["average_jaccard"] = np.mean([out["jaccard_%d" % d] for d in TAPVID_THRESHOLDS], axis=0)
     return out
+
+
+_RECON_KEYS = ("acc", "comp", "chamfer", "prec", "recall", "fscore")
+
+
+@torch.no_grad()
+def reconstruction_metrics(pred, gt, *, threshold=0.05, down_sample=0.02, device="cuda"):
+    """Atlas's 3D metrics (Murez et al., ECCV 2020, `eval_mesh`) of a predicted point set against a ground-truth one,
+    on the device.  pred / gt: float32 [N,3] points in metres (device tensors, host tensors or numpy arrays; host sets
+    are uploaded once), e.g. `TSDFVolume.extract_points()` and a GT mesh's vertices (`read_ply`).  With `down_sample`
+    (metres; None skips it) both sets are first voxel down-sampled as `voxel_down_sample` does.  With d_pred the
+    distance of each predicted point to its nearest GT point and d_gt the reverse (exact float32 nearest neighbours,
+    `nearest_neighbors`): acc = mean(d_pred), comp = mean(d_gt), chamfer = (acc + comp) / 2, prec = mean(d_pred < t),
+    recall = mean(d_gt < t) (strict, t the float32 value of `threshold`) and fscore = 2 prec recall / (prec + recall),
+    0 when both are 0 (where Atlas gives NaN).  The sums are float64 in a fixed order (block partials, then one ordered
+    pass; no atomics), so the result is the same from run to run.  Returns a dict of Python floats, with n_pred and
+    n_gt the (down-sampled) set sizes; if either set is empty every metric is NaN.  Host reads: the bounding boxes,
+    the down-sampled counts and the final download.  Non-finite coordinates and down-sample grids of more than 2^21
+    cells per axis are refused with ValueError."""
+    from .fusion import _Table, _boxes, _check_voxel, _cloud, _down_sample_begin
+    name = "reconstruction_metrics"
+    if isinstance(threshold, bool) or not isinstance(threshold, (int, float)) or not math.isfinite(threshold):
+        raise ValueError("%s: threshold must be a positive finite number" % name)
+    t = float(np.float32(threshold))
+    if not t > 0:
+        raise ValueError("%s: threshold must be positive in float32" % name)
+    if down_sample is not None:
+        _check_voxel(down_sample, name)
+    dev = next((x.device for x in (pred, gt) if torch.is_tensor(x) and x.is_cuda), torch.device(device))
+    sets = [_cloud(pred, dev, name), _cloud(gt, dev, name)]
+    with torch.cuda.device(dev):
+        boxes = _boxes(sets, name)
+        if down_sample is not None:
+            begun = [_down_sample_begin(c, b, down_sample, name) if b is not None else None for c, b in zip(sets, boxes)]
+            live = [b for b in begun if b is not None]
+            counts = torch.stack([b[2][-1] for b in live]).tolist() if live else []
+            it = iter(counts)
+            sets = [_OPS.cloud_down_sample(b[0], b[1], c, b[2], next(it)) if b is not None else c
+                    for c, b in zip(sets, begun)]
+        n_pred, n_gt = (int(c.shape[0]) for c in sets)
+        out = {"n_pred": n_pred, "n_gt": n_gt}
+        if n_pred == 0 or n_gt == 0:
+            return dict({k: math.nan for k in _RECON_KEYS}, **out)
+        sums = torch.empty((2, 2), dtype=torch.float64, device=dev)
+        for row, (queries, points, box) in enumerate(((sets[0], sets[1], boxes[1]), (sets[1], sets[0], boxes[0]))):
+            _OPS.cloud_stats(*_Table(points, box).partials(queries, t), sums[row])
+        (s_pred, c_pred), (s_gt, c_gt) = sums.tolist()
+    acc, comp = s_pred / n_pred, s_gt / n_gt
+    prec, recall = c_pred / n_pred, c_gt / n_gt
+    fscore = 2 * prec * recall / (prec + recall) if prec + recall > 0 else 0.0
+    return dict(out, acc=acc, comp=comp, chamfer=(acc + comp) / 2, prec=prec, recall=recall, fscore=fscore)

@@ -3,7 +3,9 @@ device depths and frames into it (`fuse_depths`, one `um_tsdf_integrate` launch)
 with their colours (`TSDFVolume.extract_points`), its marching-cubes mesh with per-vertex normals
 (`TSDFVolume.extract_mesh`), its ray-cast depth, colour and normal images from any camera (`TSDFVolume.render`, one
 `um_tsdf_raycast` launch), the tracking of cameras against it (`TSDFVolume.track`, point-to-plane ICP in the um_icp_*
-launches) and a binary PLY writer for the points and meshes (`write_ply`).  The kernels' arithmetic
+launches), a binary PLY writer and reader for the points and meshes (`write_ply`, `read_ply`), and exact nearest
+neighbours and voxel down-sampling of point clouds (`nearest_neighbors`, `voxel_down_sample`, the um_cloud_* launches)
+that `evaluation.reconstruction_metrics` scores reconstructions with.  The kernels' arithmetic
 is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
@@ -376,3 +378,209 @@ def write_ply(path, points, colors, normals=None, faces=None):
         f.write(header.encode("ascii"))
         for b in body:
             f.write(b)
+
+
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2", "ushort": "u2",
+              "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4", "float": "f4", "float32": "f4",
+              "double": "f8", "float64": "f8"}
+
+
+def read_ply(path):
+    """The counterpart of `write_ply`: a binary little-endian PLY's vertices and triangles, as numpy arrays in a dict:
+    'points' float32 [P,3] (x, y, z), and when present 'colors' uint8 [P,3] (red, green, blue; alpha is dropped),
+    'normals' float32 [P,3] (nx, ny, nz) and 'faces' int32 [T,3].  Vertex properties may have any PLY scalar type; the
+    face element holds one list property of vertex indices, every face a triangle (ScanNet's `*_vh_clean_2.ply` and
+    `write_ply`'s output are both of this form).  ASCII and big-endian files, list properties elsewhere, other elements
+    and faces that are not triangles are refused with ValueError."""
+    with open(path, "rb") as f:
+        data = f.read()
+    end = data.find(b"end_header")
+    nl = data.find(b"\n", end)
+    if not data.startswith(b"ply") or end < 0 or nl < 0:
+        raise ValueError("read_ply: %s is not a PLY file (no 'ply' magic or no end_header)" % path)
+    lines = [ln.split() for ln in data[:end].decode("ascii", "replace").splitlines()[1:]]
+    elements, fmt = [], None
+    for ln in lines:
+        if not ln or ln[0] in ("comment", "obj_info"):
+            continue
+        if ln[0] == "format":
+            fmt = ln[1] if len(ln) > 1 else None
+        elif ln[0] == "element" and len(ln) == 3:
+            elements.append((ln[1], int(ln[2]), []))
+        elif ln[0] == "property" and elements:
+            elements[-1][2].append(ln[1:])
+        else:
+            raise ValueError("read_ply: unreadable header line %r" % " ".join(ln))
+    if fmt != "binary_little_endian":
+        raise ValueError("read_ply: only binary_little_endian PLY is read, not %s" % fmt)
+    out, offset = {}, nl + 1
+    for name, count, props in elements:
+        if name == "vertex":
+            if any(p[0] == "list" or p[0] not in _PLY_TYPES or len(p) != 2 for p in props):
+                raise ValueError("read_ply: vertex properties must be scalars of a PLY type")
+            dt = np.dtype([(p[1], "<" + _PLY_TYPES[p[0]]) for p in props])
+            v = np.frombuffer(data, dt, count, offset)
+            offset += dt.itemsize * count
+            if not all(k in dt.names for k in ("x", "y", "z")):
+                raise ValueError("read_ply: the vertex element has no x, y and z")
+            out["points"] = np.stack([v[k] for k in ("x", "y", "z")], 1).astype(np.float32)
+            if all(k in dt.names for k in ("nx", "ny", "nz")):
+                out["normals"] = np.stack([v[k] for k in ("nx", "ny", "nz")], 1).astype(np.float32)
+            if all(k in dt.names for k in ("red", "green", "blue")):
+                col = np.stack([v[k] for k in ("red", "green", "blue")], 1)
+                if col.dtype != np.uint8:
+                    raise ValueError("read_ply: colours must be uchar")
+                out["colors"] = col
+        elif name == "face":
+            if len(props) != 1 or props[0][0] != "list" or len(props[0]) != 4 or props[0][1] not in _PLY_TYPES \
+                    or props[0][2] not in _PLY_TYPES or _PLY_TYPES[props[0][2]][0] not in "iu":
+                raise ValueError("read_ply: the face element must hold one list of integer vertex indices")
+            dt = np.dtype([("n", "<" + _PLY_TYPES[props[0][1]]), ("v", "<" + _PLY_TYPES[props[0][2]], 3)])
+            first = np.frombuffer(data, "<" + _PLY_TYPES[props[0][1]], 1, offset) if count else np.zeros(1)
+            if count and first[0] != 3:
+                raise ValueError("read_ply: only triangle faces are read (a face has %d vertices)" % first[0])
+            f = np.frombuffer(data, dt, count, offset)       # with triangles only, the records are of one size
+            if (f["n"] != 3).any():
+                raise ValueError("read_ply: only triangle faces are read")
+            offset += dt.itemsize * count
+            out["faces"] = f["v"].astype(np.int32)
+        else:
+            raise ValueError("read_ply: element %r is not read (only vertex and face)" % name)
+    if "points" not in out:
+        raise ValueError("read_ply: no vertex element")
+    return out
+
+
+MAX_CLOUD_POINTS = 2 ** 31 - 1
+MAX_CELLS_PER_AXIS = 2 ** 21
+NN_CELLS_PER_POINT = 2                      # the nearest-neighbour table's cells per indexed point, at most
+NN_MAX_CELLS = 2 ** 26                      # and at most this many cells (two int32 tables of 256 MiB)
+
+
+def _cloud(points, device, name):
+    """A point set as contiguous device float32 [N,3] (one upload for host tensors and numpy arrays)"""
+    if not torch.is_tensor(points):
+        points = torch.from_numpy(np.ascontiguousarray(np.asarray(points)))
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError("%s: expected points [N,3], got %s" % (name, list(points.shape)))
+    if points.dtype != torch.float32:
+        raise ValueError("%s: expected float32 points, got %s" % (name, points.dtype))
+    if points.shape[0] > MAX_CLOUD_POINTS:
+        raise ValueError("%s: at most 2^31 - 1 points" % name)
+    return points.to(device).contiguous()
+
+
+def _boxes(clouds, name):
+    """The per-axis [min, max] of each non-empty set, read by the host in one read (None for an empty set); a
+    non-finite coordinate anywhere makes a bound non-finite and is refused"""
+    live = [c for c in clouds if c.shape[0]]
+    vals = torch.cat([torch.cat((c.amin(0), c.amax(0))) for c in live]).tolist() if live else []
+    if not all(math.isfinite(v) for v in vals):
+        raise ValueError("%s: point coordinates must be finite" % name)
+    boxes, k = [], 0
+    for c in clouds:
+        boxes.append((vals[k:k + 3], vals[k + 3:k + 6]) if c.shape[0] else None)
+        k += 6 if c.shape[0] else 0
+    return boxes
+
+
+def nn_grid(lo, hi, n):
+    """The nearest-neighbour table of n points in the box [lo, hi]: origin lo, the least cell size c (to a bisection's
+    precision) with prod(max(1, ceil(extent / c))) cells at most min(NN_CELLS_PER_POINT n, NN_MAX_CELLS) and at most 2^21
+    per axis, and dims.  A larger box (far floaters) gives larger cells, not a larger table; the search is exact for any."""
+    lo = [float(v) for v in lo]
+    ext = [max(0.0, float(b) - float(a)) for a, b in zip(lo, hi)]
+    m = max(ext)
+    if m == 0.0:
+        return lo, 1.0, (1, 1, 1)
+    cap = min(max(NN_CELLS_PER_POINT * n, 1), NN_MAX_CELLS)
+
+    def dims(c):
+        return tuple(max(1, math.ceil(e / c)) for e in ext)
+
+    a, b = m / MAX_CELLS_PER_AXIS * (1 + 1e-9), m
+    if math.prod(dims(a)) > cap:
+        for _ in range(64):
+            mid = math.sqrt(a * b)
+            a, b = (a, mid) if math.prod(dims(mid)) <= cap else (mid, b)
+        a = b
+    return lo, a, dims(a)
+
+
+class _Table:
+    """The cell table of an indexed point set on the device (um_cloud_keys, a stable sort, um_cloud_ranges)"""
+
+    def __init__(self, points, box):
+        self.origin, self.cell, self.dims = nn_grid(box[0], box[1], points.shape[0])
+        keys = _OPS.cloud_keys(points, self.origin, self.cell, self.dims)
+        skeys, order = torch.sort(keys, stable=True)
+        self.start, self.end, self.sorted = _OPS.cloud_ranges(skeys, order, points, self.dims)
+
+    def nearest(self, queries):
+        return _OPS.cloud_nearest(queries, self.sorted, self.start, self.end, self.origin, self.cell)
+
+    def partials(self, queries, threshold):
+        return _OPS.cloud_nearest_partials(queries, self.sorted, self.start, self.end, self.origin, self.cell, threshold)
+
+
+def down_sample_grid(box, voxel_size, name):
+    """Open3D's voxel grid of a set with bounds box = (min, max): origin min - v / 2 (float64), dims floor((max - origin)
+    / v) + 1; more than 2^21 cells on an axis is refused"""
+    v = float(voxel_size)
+    origin = [float(a) - v / 2 for a in box[0]]
+    dims = [math.floor((float(b) - o) / v) + 1 for b, o in zip(box[1], origin)]
+    if max(dims) > MAX_CELLS_PER_AXIS:
+        raise ValueError("%s: a %s-cell box at voxel size %g is more than 2^21 cells on an axis" % (name, dims, v))
+    return origin, v, dims
+
+
+def _down_sample_begin(points, box, voxel_size, name):
+    origin, v, dims = down_sample_grid(box, voxel_size, name)
+    skeys, order = torch.sort(_OPS.cloud_keys(points, origin, v, dims), stable=True)
+    return skeys, order, _OPS.cloud_down_sample_count(skeys)
+
+
+def _check_voxel(voxel_size, name):
+    if isinstance(voxel_size, bool) or not isinstance(voxel_size, (int, float)) \
+            or not (math.isfinite(voxel_size) and voxel_size > 0):
+        raise ValueError("%s: voxel size must be positive and finite" % name)
+
+
+@torch.no_grad()
+def voxel_down_sample(points, voxel_size, device="cuda"):
+    """Open3D's `VoxelDownSample` on the device: the points [N,3] (float32; a device tensor, a host tensor or a numpy
+    array, uploaded once) binned into cells of `voxel_size` whose grid starts half a cell below the set's minimum, each
+    occupied cell giving the mean of its points (float64 sums in input order, rounded to float32).  Returns float32 [M,3]
+    on the device, ordered by cell (x fastest).  Host reads: the bounding box and the cell count M.  Non-finite
+    coordinates and boxes of more than 2^21 cells per axis are refused with ValueError."""
+    name = "voxel_down_sample"
+    _check_voxel(voxel_size, name)
+    dev = points.device if torch.is_tensor(points) and points.is_cuda else torch.device(device)
+    p = _cloud(points, dev, name)
+    with torch.cuda.device(dev):
+        if p.shape[0] == 0:
+            return p.new_zeros((0, 3))
+        box, = _boxes([p], name)
+        skeys, order, offsets = _down_sample_begin(p, box, voxel_size, name)
+        return _OPS.cloud_down_sample(skeys, order, p, offsets, int(offsets[-1].item()))
+
+
+@torch.no_grad()
+def nearest_neighbors(queries, points, device="cuda"):
+    """The exact nearest neighbour of every query among `points`, on the device: (distance float32 [Q], index int64 [Q]).
+    The squared distance is float32 in one order, dx = q.x - p.x, ...; s = fmaf(dz, dz, fmaf(dy, dy, dx * dx)); the
+    neighbour is the point of least s, ties to the least index, and the distance is sqrtf(s) correctly rounded: a
+    brute-force float32 scan's result bit for bit, found by a ring search over a uniform grid whose pruning is proved
+    conservative under that rounding (include/unimatch_sm100.h).  Both sets are float32 [N,3] device tensors, host
+    tensors or numpy arrays (host sets are uploaded once).  Host reads: the bounding boxes (one read).  Empty `points`
+    and non-finite coordinates are refused with ValueError; no queries give empty outputs."""
+    name = "nearest_neighbors"
+    dev = points.device if torch.is_tensor(points) and points.is_cuda else torch.device(device)
+    q, p = _cloud(queries, dev, name), _cloud(points, dev, name)
+    with torch.cuda.device(dev):
+        if p.shape[0] == 0:
+            raise ValueError("%s: no points to search" % name)
+        _, box = _boxes([q, p], name)
+        if q.shape[0] == 0:
+            return q.new_zeros((0,)), torch.zeros((0,), dtype=torch.int64, device=dev)
+        return _Table(p, box).nearest(q)

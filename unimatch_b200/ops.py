@@ -131,6 +131,12 @@ _SIGNATURES = {
     "um_icp_reduce": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _P]),
     "um_icp_solve": (_RC, [_P, _I, _I, _P, _D, _D, _I, _P, _P]),
     "um_icp_accept": (_RC, [_P, _I, _I, _P, _D, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "um_cloud_keys": (_RC, [_P, _L, _D, _D, _D, _D, _I, _I, _I, _P, _P]),
+    "um_cloud_ranges": (_RC, [_P, _P, _P, _L, _I, _I, _I, _P, _P, _P, _P]),
+    "um_cloud_down_sample_count": (_RC, [_P, _L, _P, _P]),
+    "um_cloud_down_sample": (_RC, [_P, _P, _P, _L, _P, _L, _P, _P]),
+    "um_cloud_nearest": (_RC, [_P, _L, _P, _P, _P, _L, _D, _D, _D, _D, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
+    "um_cloud_stats": (_RC, [_P, _P, _L, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -801,6 +807,154 @@ icp_accept = _define(
     "icp_accept(Tensor partials, int nb, Tensor n_valid, float min_inlier_fraction, Tensor? poses, Tensor(a!)? correction, "
     "Tensor(b!) state, Tensor(c!) pose_out, Tensor(d!) tracked, Tensor(e!) inliers, Tensor(f!) rmse, Tensor(g!) w2c) -> ()",
     _icp_accept)
+
+
+# ---- point clouds (include/unimatch_sm100.h, um_cloud_*) -----------------------------------------------------------
+CLOUD_THREADS = 256                                  # queries and sorted positions per block of the cloud kernels
+
+
+def _cloud_points(t, name):
+    """A contiguous device fp32 [n, 3] point set"""
+    _f32c(t, name)
+    if t.dim() != 2 or t.shape[1] != 3:
+        raise RuntimeError("%s: expected points [n, 3]" % name)
+    return t.shape[0]
+
+
+def _cloud_grid(origin, cell, dims, name):
+    if len(origin) != 3 or len(dims) != 3:
+        raise RuntimeError("%s: origin and dims take 3 values" % name)
+    return [float(o) for o in origin] + [float(cell)] + [int(g) for g in dims]
+
+
+def _cloud_keys(points, origin, cell, dims):
+    """The int64 cell key of each point of points [n, 3] in the grid (origin, cell, dims) (x fastest)"""
+    n = _cloud_points(points, "cloud_keys: points")
+    keys = torch.empty((n,), device=points.device, dtype=torch.int64)
+    _check(LIB.um_cloud_keys(_p(points), n, *_cloud_grid(origin, cell, dims, "cloud_keys"), _p(keys), _stream()),
+           "um_cloud_keys")
+    return keys
+
+
+cloud_keys = _define("cloud_keys(Tensor points, float[] origin, float cell, int[] dims) -> Tensor", _cloud_keys)
+
+
+def _cloud_sorted(sorted_keys, order, points, name):
+    n = _cloud_points(points, name + ": points")
+    for t, nm in ((sorted_keys, "sorted_keys"), (order, "order")):
+        if t.dtype != torch.int64 or tuple(t.shape) != (n,) or not t.is_contiguous() or t.device != points.device:
+            raise RuntimeError("%s: %s must be contiguous int64 [n] on the points' device" % (name, nm))
+    return n
+
+
+def _cloud_ranges(sorted_keys, order, points, dims):
+    """The dense cell table of a point set from its stably sorted keys and their input positions: start / end int32
+    [gz, gy, gx] and the points in sorted order with their input index, fp32 [n, 4]"""
+    n = _cloud_sorted(sorted_keys, order, points, "cloud_ranges")
+    gx, gy, gz = (int(g) for g in dims)
+    start = torch.empty((gz, gy, gx), device=points.device, dtype=torch.int32)
+    end = torch.empty_like(start)
+    sorted_points = torch.empty((n, 4), device=points.device, dtype=torch.float32)
+    _check(LIB.um_cloud_ranges(_p(sorted_keys), _p(order), _p(points), n, gx, gy, gz, _p(start), _p(end), _p(sorted_points),
+                               _stream()), "um_cloud_ranges")
+    return start, end, sorted_points
+
+
+cloud_ranges = _define("cloud_ranges(Tensor sorted_keys, Tensor order, Tensor points, int[] dims) -> (Tensor, Tensor, Tensor)",
+                       _cloud_ranges)
+
+
+def _cloud_down_sample_count(sorted_keys):
+    """The down-sampling offsets, device int64 [ceil(n / CLOUD_THREADS) + 1]: each block's first output row, then the
+    number of occupied cells"""
+    if sorted_keys.dtype != torch.int64 or sorted_keys.dim() != 1 or not sorted_keys.is_contiguous():
+        raise RuntimeError("cloud_down_sample_count: sorted_keys must be contiguous int64 [n]")
+    n = sorted_keys.shape[0]
+    offsets = torch.empty((-(-n // CLOUD_THREADS) + 1,), device=sorted_keys.device, dtype=torch.int64)
+    _check(LIB.um_cloud_down_sample_count(_p(sorted_keys), n, _p(offsets), _stream()), "um_cloud_down_sample_count")
+    return offsets
+
+
+cloud_down_sample_count = _define("cloud_down_sample_count(Tensor sorted_keys) -> Tensor", _cloud_down_sample_count)
+
+
+def _cloud_down_sample(sorted_keys, order, points, offsets, m):
+    """The m occupied cells' mean points fp32 [m, 3], in key order"""
+    n = _cloud_sorted(sorted_keys, order, points, "cloud_down_sample")
+    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-n // CLOUD_THREADS) + 1,) \
+            or offsets.device != points.device:
+        raise RuntimeError("cloud_down_sample: offsets must be cloud_down_sample_count's device int64 table")
+    out = torch.empty((m, 3), device=points.device, dtype=torch.float32)
+    _check(LIB.um_cloud_down_sample(_p(sorted_keys), _p(order), _p(points), n, _p(offsets), m, _p(out), _stream()),
+           "um_cloud_down_sample")
+    return out
+
+
+cloud_down_sample = _define("cloud_down_sample(Tensor sorted_keys, Tensor order, Tensor points, Tensor offsets, int m) "
+                            "-> Tensor", _cloud_down_sample)
+
+
+def _cloud_nearest_args(queries, sorted_points, start, end, name):
+    nq = _cloud_points(queries, name + ": queries")
+    _f32c(sorted_points, name + ": sorted_points")
+    if sorted_points.dim() != 2 or sorted_points.shape[1] != 4:
+        raise RuntimeError("%s: sorted_points must be cloud_ranges' fp32 [n, 4]" % name)
+    if start.dtype != torch.int32 or end.dtype != torch.int32 or start.dim() != 3 or end.shape != start.shape \
+            or not start.is_contiguous() or not end.is_contiguous():
+        raise RuntimeError("%s: start and end must be cloud_ranges' int32 [gz, gy, gx] tables" % name)
+    if any(t.device != queries.device for t in (sorted_points, start, end)):
+        raise RuntimeError("%s: every tensor must be on one device" % name)
+    gz, gy, gx = start.shape
+    return nq, sorted_points.shape[0], (gx, gy, gz)
+
+
+def _cloud_nearest(queries, sorted_points, start, end, origin, cell):
+    """The exact fp32 nearest neighbour of each query among the table's points: distance fp32 [nq] and input index
+    int64 [nq]"""
+    nq, n, dims = _cloud_nearest_args(queries, sorted_points, start, end, "cloud_nearest")
+    distance = torch.empty((nq,), device=queries.device, dtype=torch.float32)
+    index = torch.empty((nq,), device=queries.device, dtype=torch.int64)
+    _check(LIB.um_cloud_nearest(_p(queries), nq, _p(sorted_points), _p(start), _p(end), n,
+                                *_cloud_grid(origin, cell, dims, "cloud_nearest"), 1.0, _p(distance), _p(index), None,
+                                None, _stream()), "um_cloud_nearest")
+    return distance, index
+
+
+cloud_nearest = _define("cloud_nearest(Tensor queries, Tensor sorted_points, Tensor start, Tensor end, float[] origin, "
+                        "float cell) -> (Tensor, Tensor)", _cloud_nearest)
+
+
+def _cloud_nearest_partials(queries, sorted_points, start, end, origin, cell, threshold):
+    """cloud_nearest's distances reduced per block of CLOUD_THREADS queries: the fp64 sum of d and the int64 count of
+    d < threshold, [ceil(nq / CLOUD_THREADS)] each"""
+    nq, n, dims = _cloud_nearest_args(queries, sorted_points, start, end, "cloud_nearest_partials")
+    nb = -(-nq // CLOUD_THREADS)
+    psum = torch.empty((nb,), device=queries.device, dtype=torch.float64)
+    pcount = torch.empty((nb,), device=queries.device, dtype=torch.int64)
+    _check(LIB.um_cloud_nearest(_p(queries), nq, _p(sorted_points), _p(start), _p(end), n,
+                                *_cloud_grid(origin, cell, dims, "cloud_nearest_partials"), threshold, None, None, _p(psum),
+                                _p(pcount), _stream()), "um_cloud_nearest")
+    return psum, pcount
+
+
+cloud_nearest_partials = _define(
+    "cloud_nearest_partials(Tensor queries, Tensor sorted_points, Tensor start, Tensor end, float[] origin, float cell, "
+    "float threshold) -> (Tensor, Tensor)", _cloud_nearest_partials)
+
+
+def _cloud_stats(partial_sum, partial_count, out):
+    """The fixed-order reduction of cloud_nearest_partials' partials into out (fp64 [2]): the sum of d, the count"""
+    nb = partial_sum.shape[0]
+    if partial_sum.dtype != torch.float64 or partial_count.dtype != torch.int64 or partial_sum.dim() != 1 \
+            or tuple(partial_count.shape) != (nb,) or not partial_sum.is_contiguous() or not partial_count.is_contiguous():
+        raise RuntimeError("cloud_stats: expected cloud_nearest_partials' fp64 and int64 [nb] partials")
+    if out.dtype != torch.float64 or tuple(out.shape) != (2,) or not out.is_contiguous():
+        raise RuntimeError("cloud_stats: out must be contiguous fp64 [2]")
+    _device_like("cloud_stats", out, partial_sum, partial_count)
+    _check(LIB.um_cloud_stats(_p(partial_sum), _p(partial_count), nb, _p(out), _stream()), "um_cloud_stats")
+
+
+cloud_stats = _define("cloud_stats(Tensor partial_sum, Tensor partial_count, Tensor(a!) out) -> ()", _cloud_stats)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
