@@ -30,8 +30,8 @@ extern "C" {
 #define UM_FEATURE_DIM 128
 
 /* ABI version and build info.  The version changes when an entry point changes or is removed; new entry points (the
- * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing, ray casting, ICP and the
- * point-cloud ops) leave existing callers working and keep it. */
+ * tracks, the submission encoder, the scene-flow warp and statistics, TSDF fusion, meshing, ray casting, ICP, the
+ * point-cloud ops and the mesh rasteriser) leave existing callers working and keep it. */
 #define UM_ABI_VERSION 4
 int um_abi_version(void);
 const char* um_build_info(void);
@@ -644,6 +644,86 @@ int um_cloud_nearest(const float* queries, int64_t nq, const float* sorted_point
                      int32_t gz, float threshold, float* distance, int64_t* index, double* partial_sum,
                      int64_t* partial_count, void* stream);
 int um_cloud_stats(const double* partial_sum, const int64_t* partial_count, int64_t nb, double* out, void* stream);
+
+/* ---- triangle meshes: rasterisation, visibility of points and the 2D depth metrics ----------------------------------
+ * A mesh is points fp32 [P, 3] and faces int32 [T, 3] (indices in [0, P), at most 2^31 - 1 faces), seen by n <= 65535
+ * pinhole cameras of h x w pixels (h w <= 2^31 - 1), intrinsics fx, fy (finite, nonzero), cx, cy (finite), through the
+ * fp32 world-to-camera rows w2c [n, 3, 4] (row-major, as um_tsdf_integrate reads them); near finite and > 0, far > near
+ * (+inf: no limit).  fp32 operations are each rounded on their own (__fmaf_rn, __fdiv_rn, ...), fp64 ones are __dadd_rn,
+ * __dsub_rn, __dmul_rn, __ddiv_rn, floor and ceil, in the order written.
+ * Per view and pixel (x, y), in fp32:
+ *   xc = (x - cx) / fx, yc = (y - cy) / fy: the ray through the pixel centre along d = (xc, yc, 1) in camera coordinates
+ *   (um_tsdf_raycast's convention); its parameter t along d is the camera z-depth.
+ *   Vertex V of point p: V.x = fma(M02, p.z, fma(M01, p.y, fma(M00, p.x, M03))), likewise V.y (row 1) and V.z (row 2).
+ *   Cross product a x b = (a.y b.z - a.z b.y, a.z b.x - a.x b.z, a.x b.y - a.y b.x), each product rounded, then the
+ *   difference.  Face (i0, i1, i2) with vertices A, B, C has edges AB (i0 -> i1), BC (i1 -> i2) and CA (i2 -> i0); the
+ *   edge i -> j has the canonical cross product K = V_lo x V_hi (lo, hi = i, j in ascending order) times +1 if i <= j,
+ *   else -1, so two faces that share an edge get exactly opposite edge values (the rasteriser is watertight by
+ *   construction).  E = fma(K.x, xc, fma(K.y, yc, K.z)) per edge (K the signed product).
+ *   Coverage: E_AB, E_BC, E_CA all >= 0 or all <= 0, and S = (E_AB + E_BC) + E_CA != 0.  Faces are two-sided (no
+ *   culling).  A face whose vertices coincide in camera space (a repeated index included) has S = 0 exactly and is never
+ *   hit.  A hit on the line of the ray behind the camera has t < 0 and fails the depth test.
+ *   Depth: det = fma(A.z, K_BC.z, fma(A.y, K_BC.y, A.x * K_BC.x)), t = det / S; a hit iff t is finite and
+ *   near <= t <= far.  The winner is the hit of least t; among equal t the least face index (a strict < over the
+ *   faces in ascending index).
+ *   Colour (when colors, uint8 [P, 3], is given): bA = E_BC / S, bB = E_CA / S, bC = E_AB / S (the 3D barycentrics of
+ *   the hit point, so perspective-correct); per channel fma(bC, col_C, fma(bB, col_B, bA * col_A)), __float2int_rn,
+ *   clamped to 0..255.
+ *   Outputs: depth fp32 [n, h, w] (t, 0 for a miss), face int32 [n, h, w] (-1 for a miss), rgb uint8 [n, h, w, 3] (0 for
+ *   a miss; optional).
+ * Rectangle (part of the definition: a face covers only the pixels of its rectangle), per (view, face) in fp64:
+ *   the vertices c = ((M_r0 p.x + M_r1 p.y) + M_r2 p.z) + M_r3 per row r (the fp32 entries and coordinates converted
+ *   exactly);  none if every vertex has c.z < near or every vertex has c.z > far;  else the triangle clipped to
+ *   c.z >= near: for each edge P -> Q (AB, BC, CA) keep P if P.z >= near, and if exactly one of P, Q has z >= near add
+ *   (P.x + s (Q.x - P.x), P.y + s (Q.y - P.y), near) with s = (near - P.z) / (Q.z - P.z);  each kept point projects to
+ *   u = fx (x / z) + cx, v = fy (y / z) + cy;  the rectangle is x in [floor(min u) - 1, ceil(max u) + 1] and y in
+ *   [floor(min v) - 1, ceil(max v) + 1] clamped to the frame (none if that is empty or a bound is NaN).  The exact hit
+ *   point of a ray with t >= near lies in the clipped triangle, so the rectangle holds every pixel whose exact ray hits
+ *   it; the 1-pixel margin absorbs the fp32 rounding of coverage and depth for the geometry tested
+ *   (tests/test_raster_cpu.py shows that dropping it changes no output there), but it is not proved for arbitrarily
+ *   degenerate geometry (slivers, vertices at extreme magnitudes, faces grazing the near plane).
+ * Launches (16 x 16 pixel tiles, tiles = ceil(h/16) ceil(w/16) per view):
+ *   um_mesh_bin_count: per (view, block of 256 faces) the number of tiles the faces' rectangles touch, then one CTA's
+ *   ordered exclusive int64 scan: offsets [n ceil(T/256) + 1] (DEVICE int64), view-major, the total E last.
+ *   um_mesh_bin (E entries): for each (view, face) in that order, per touched tile row by row, keys[e] = view tiles +
+ *   tile (int64) and values[e] = face << 16 | (x0 | x1 << 4 | y0 << 8 | y1 << 12), the rectangle within the tile.
+ *   The caller sorts keys stably with their positions (order), so each tile's entries stay in ascending face order.
+ *   um_mesh_ranges: start / end int32 [n tiles] (zeroed by the entry) hold the first and one-past-last sorted position
+ *   of each tile's entries.
+ *   um_mesh_raster: one CTA per (tile, view) and one thread per pixel; the entries values[order[e]] of the tile are
+ *   staged 256 at a time in shared memory (the signed canonical cross products, det, face and rectangle), and each thread
+ *   walks them in order.  Every pixel is written.
+ *   No atomics anywhere: every output is the same from run to run.
+ * Visibility (um_visible_points, one thread per point, views in order): the point is transformed and projected exactly as
+ *   um_tsdf_integrate projects a voxel centre (c.z > 0, nearest pixel floor(u + 0.5f) inside the frame); view t sees it
+ *   iff the depth D = depth[t, yi, xi] is finite, D > 0 and c.z <= D + tolerance (fp32).  visible[i] (uint8) = 1 iff some
+ *   view sees point i.
+ * Depth metrics (um_depth_metrics) of pred and gt fp32 [n, h, w]: a pixel is valid iff p is finite and > 0, masked iff
+ *   valid and g finite with 0 < g < max_depth.  Over masked pixels, with fp64 d = (double)p - (double)g: terms 0 count,
+ *   1 |d|, 2 |d| / g, 3 (d d) / g, 4 d d, 5 (log p - log g)^2 (CUDA's fp64 log of the fp32 values), 6..8 the count of
+ *   max(g / p, p / g) (fp32, correctly rounded divisions) < 1.25, 1.5625, 1.953125; term 9 the count of valid pixels
+ *   (masked or not).  Per block of 256 pixels of a frame, per term a shfl_down tree (16, 8, 4, 2, 1) per warp, then the
+ *   8 warps in order: partials fp64 [n, nb, UM_DEPTH_METRIC_TERMS], nb = ceil(h w / 256); then one warp per (frame,
+ *   term): lane l adds blocks l, l + 32, ... in order from 0.0, then a shfl_down tree: out fp64 [n, UM_DEPTH_METRIC_TERMS].
+ * Every pointer is DEVICE memory; no output overlaps an input or another output. */
+#define UM_DEPTH_METRIC_TERMS 10
+int um_mesh_bin_count(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const float* w2c,
+                      int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near, float far,
+                      int64_t* offsets, void* stream);
+int um_mesh_bin(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const float* w2c, int32_t n,
+                int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near, float far,
+                const int64_t* offsets, int64_t n_entries, int64_t* keys, int64_t* values, void* stream);
+int um_mesh_ranges(const int64_t* sorted_keys, int64_t n_entries, int32_t n, int32_t h, int32_t w, int32_t* start,
+                   int32_t* end, void* stream);
+int um_mesh_raster(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const uint8_t* colors,
+                   const float* w2c, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near,
+                   float far, const int64_t* order, const int64_t* values, int64_t n_entries, const int32_t* start,
+                   const int32_t* end, float* depth, int32_t* face, uint8_t* rgb, void* stream);
+int um_visible_points(const float* points, int64_t n_points, const float* depth, int32_t n, int32_t h, int32_t w,
+                      const float* w2c, float fx, float fy, float cx, float cy, float tolerance, uint8_t* visible,
+                      void* stream);
+int um_depth_metrics(const float* pred, const float* gt, int32_t n, int32_t h, int32_t w, float max_depth,
+                     double* partials, double* out, void* stream);
 
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger

@@ -51,6 +51,9 @@ _LAZY = {
     "nearest_neighbors": (".fusion", "nearest_neighbors"),
     "voxel_down_sample": (".fusion", "voxel_down_sample"),
     "reconstruction_metrics": (".evaluation", "reconstruction_metrics"),
+    "render_mesh": (".fusion", "render_mesh"),
+    "visible_points": (".fusion", "visible_points"),
+    "depth_metrics": (".evaluation", "depth_metrics"),
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
@@ -70,7 +73,8 @@ __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "In
            "validate_flow", "validate_stereo", "validate_depth", "tapvid_metrics", "create_flow_submission", "create_stereo_submission",
            "inference_flow", "inference_stereo", "inference_depth", "warp_disparity", "infer_scene_flow", "SceneFlowRunner",
            "validate_scene_flow", "create_scene_flow_submission", "DepthFusionRunner", "TSDFVolume", "fuse_depths", "write_ply",
-           "read_ply", "nearest_neighbors", "voxel_down_sample", "reconstruction_metrics"]
+           "read_ply", "nearest_neighbors", "voxel_down_sample", "reconstruction_metrics",
+           "render_mesh", "visible_points", "depth_metrics"]
 
 
 def __getattr__(name):

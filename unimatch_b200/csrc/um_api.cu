@@ -1,7 +1,7 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
 // between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu),
-// TSDF fusion (um_fusion.cu), ICP tracking against the volume (um_icp.cu) and the point-cloud ops (um_cloud.cu).  See
-// include/unimatch_sm100.h.
+// TSDF fusion (um_fusion.cu), ICP tracking against the volume (um_icp.cu), the point-cloud ops (um_cloud.cu) and the mesh
+// rasteriser, point visibility and depth metrics (um_raster.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -93,6 +93,22 @@ int cloud_nearest_launch(const float* queries, long long nq, const float* sorted
                          long long* index, double* partial_sum, long long* partial_count, cudaStream_t st);
 int cloud_stats_launch(const double* partial_sum, const long long* partial_count, long long nb, double* out,
                        cudaStream_t st);
+int mesh_bin_count_launch(const float* points, const int* faces, long long T, const float* w2c, int n, int h, int w,
+                          float fx, float fy, float cx, float cy, float near, float far, long long* offsets,
+                          cudaStream_t st);
+int mesh_bin_launch(const float* points, const int* faces, long long T, const float* w2c, int n, int h, int w, float fx,
+                    float fy, float cx, float cy, float near, float far, const long long* offsets, long long* keys,
+                    long long* values, cudaStream_t st);
+int mesh_ranges_launch(const long long* sorted_keys, long long total, long long n_bins, int* start, int* end,
+                       cudaStream_t st);
+int mesh_raster_launch(const float* points, const int* faces, const uint8_t* colors, const float* w2c, int n, int h,
+                       int w, float fx, float fy, float cx, float cy, float near, float far, const long long* order,
+                       const long long* values, const int* start, const int* end, float* depth, int* face,
+                       uint8_t* rgb, cudaStream_t st);
+int visible_points_launch(const float* points, long long P, const float* depth, int n, int h, int w, const float* w2c,
+                          float fx, float fy, float cx, float cy, float tolerance, uint8_t* visible, cudaStream_t st);
+int depth_metrics_launch(const float* pred, const float* gt, int n, int h, int w, float max_depth, double* partials,
+                         double* out, cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -663,6 +679,147 @@ int um_cloud_stats(const double* partial_sum, const int64_t* partial_count, int6
              "um_cloud_stats: out must not overlap the partials");
   return um::cloud_stats_launch(partial_sum, reinterpret_cast<const long long*>(partial_count), nb, out,
                                 (cudaStream_t)stream);
+}
+
+// ---- triangle meshes (um_raster.cu) ----
+static const long long kMeshMax = 0x7fffffffLL;             // int32 face indices, vertex indices and bin positions
+
+static long long mesh_tiles(int32_t h, int32_t w) { return (((long long)h + 15) / 16) * (((long long)w + 15) / 16); }
+
+// n views of h x w pixels and the camera: n 1 .. 65535, h w <= 2^31 - 1, fx fy finite nonzero, cx cy finite,
+// near finite > 0, far > near.
+static bool mesh_camera(int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near, float far) {
+  return n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= kMeshMax && fx != 0.f && fy != 0.f &&
+         finite_value(fx) && finite_value(fy) && finite_value(cx) && finite_value(cy) && near > 0.f &&
+         finite_value(near) && far > near;
+}
+
+static bool mesh_counts(int64_t n_points, int64_t n_faces) {
+  return n_points >= 1 && n_points <= kMeshMax && n_faces >= 1 && n_faces <= kMeshMax;
+}
+
+int um_mesh_bin_count(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const float* w2c,
+                      int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near, float far,
+                      int64_t* offsets, void* stream) {
+  UM_REQUIRE(points && faces && w2c && offsets, "um_mesh_bin_count: no pointer may be NULL");
+  UM_REQUIRE(mesh_counts(n_points, n_faces), "um_mesh_bin_count: bad mesh (%lld points, %lld faces; 1 .. 2^31 - 1 each)",
+             (long long)n_points, (long long)n_faces);
+  UM_REQUIRE(mesh_camera(n, h, w, fx, fy, cx, cy, near, far),
+             "um_mesh_bin_count: bad cameras (1 .. 65535 views of at most 2^31 - 1 pixels, fx fy finite nonzero, cx cy "
+             "finite, near finite > 0, far > near)");
+  UM_REQUIRE(um::aligned(points, 4) && um::aligned(faces, 4) && um::aligned(w2c, 4) && um::aligned(offsets, 8),
+             "um_mesh_bin_count: points, faces and w2c 4-byte, offsets 8-byte aligned");
+  const long long nb = (long long)n * ((n_faces + 255) / 256);
+  UM_REQUIRE(um::written_disjoint({{offsets, 8 * (nb + 1)}, {points, 12 * n_points}, {faces, 12 * n_faces},
+                                   {w2c, 48LL * n}},
+                                  1),
+             "um_mesh_bin_count: offsets must not overlap the inputs");
+  return um::mesh_bin_count_launch(points, faces, n_faces, w2c, n, h, w, fx, fy, cx, cy, near, far,
+                                   reinterpret_cast<long long*>(offsets), (cudaStream_t)stream);
+}
+
+int um_mesh_bin(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const float* w2c, int32_t n,
+                int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near, float far,
+                const int64_t* offsets, int64_t n_entries, int64_t* keys, int64_t* values, void* stream) {
+  UM_REQUIRE(points && faces && w2c && offsets && keys && values, "um_mesh_bin: no pointer may be NULL");
+  UM_REQUIRE(mesh_counts(n_points, n_faces), "um_mesh_bin: bad mesh (%lld points, %lld faces; 1 .. 2^31 - 1 each)",
+             (long long)n_points, (long long)n_faces);
+  UM_REQUIRE(mesh_camera(n, h, w, fx, fy, cx, cy, near, far), "um_mesh_bin: bad cameras (see um_mesh_bin_count)");
+  UM_REQUIRE(n_entries >= 1 && n_entries <= kMeshMax, "um_mesh_bin: bad entry count %lld (1 .. 2^31 - 1)",
+             (long long)n_entries);
+  UM_REQUIRE(um::aligned(points, 4) && um::aligned(faces, 4) && um::aligned(w2c, 4) && um::aligned(offsets, 8) &&
+                 um::aligned(keys, 8) && um::aligned(values, 8),
+             "um_mesh_bin: points, faces and w2c 4-byte, offsets, keys and values 8-byte aligned");
+  const long long nb = (long long)n * ((n_faces + 255) / 256);
+  UM_REQUIRE(um::written_disjoint({{keys, 8 * n_entries}, {values, 8 * n_entries}, {offsets, 8 * (nb + 1)},
+                                   {points, 12 * n_points}, {faces, 12 * n_faces}, {w2c, 48LL * n}},
+                                  2),
+             "um_mesh_bin: keys and values must not overlap each other or the inputs");
+  return um::mesh_bin_launch(points, faces, n_faces, w2c, n, h, w, fx, fy, cx, cy, near, far,
+                             reinterpret_cast<const long long*>(offsets), reinterpret_cast<long long*>(keys),
+                             reinterpret_cast<long long*>(values), (cudaStream_t)stream);
+}
+
+int um_mesh_ranges(const int64_t* sorted_keys, int64_t n_entries, int32_t n, int32_t h, int32_t w, int32_t* start,
+                   int32_t* end, void* stream) {
+  UM_REQUIRE(start && end && (n_entries == 0 || sorted_keys), "um_mesh_ranges: no pointer may be NULL");
+  UM_REQUIRE(n_entries >= 0 && n_entries <= kMeshMax, "um_mesh_ranges: bad entry count %lld (0 .. 2^31 - 1)",
+             (long long)n_entries);
+  UM_REQUIRE(n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= kMeshMax,
+             "um_mesh_ranges: bad views (%d x %d x %d; at most 65535 views of 2^31 - 1 pixels)", n, h, w);
+  UM_REQUIRE(um::aligned(sorted_keys, 8) && um::aligned(start, 4) && um::aligned(end, 4),
+             "um_mesh_ranges: keys 8-byte, tables 4-byte aligned");
+  const long long bins = n * mesh_tiles(h, w);
+  UM_REQUIRE(um::written_disjoint({{start, 4 * bins}, {end, 4 * bins}, {sorted_keys, 8 * n_entries}}, 2),
+             "um_mesh_ranges: the tables must not overlap each other or the keys");
+  return um::mesh_ranges_launch(reinterpret_cast<const long long*>(sorted_keys), n_entries, bins, start, end,
+                                (cudaStream_t)stream);
+}
+
+int um_mesh_raster(const float* points, int64_t n_points, const int32_t* faces, int64_t n_faces, const uint8_t* colors,
+                   const float* w2c, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy, float near,
+                   float far, const int64_t* order, const int64_t* values, int64_t n_entries, const int32_t* start,
+                   const int32_t* end, float* depth, int32_t* face, uint8_t* rgb, void* stream) {
+  UM_REQUIRE(points && faces && w2c && start && end && depth && face && (n_entries == 0 || (order && values)),
+             "um_mesh_raster: no pointer but colors and rgb may be NULL");
+  UM_REQUIRE(!colors == !rgb, "um_mesh_raster: give colors and rgb together");
+  UM_REQUIRE(mesh_counts(n_points, n_faces), "um_mesh_raster: bad mesh (%lld points, %lld faces; 1 .. 2^31 - 1 each)",
+             (long long)n_points, (long long)n_faces);
+  UM_REQUIRE(mesh_camera(n, h, w, fx, fy, cx, cy, near, far), "um_mesh_raster: bad cameras (see um_mesh_bin_count)");
+  UM_REQUIRE(n_entries >= 0 && n_entries <= kMeshMax, "um_mesh_raster: bad entry count %lld (0 .. 2^31 - 1)",
+             (long long)n_entries);
+  UM_REQUIRE(um::aligned(points, 4) && um::aligned(faces, 4) && um::aligned(w2c, 4) && um::aligned(order, 8) &&
+                 um::aligned(values, 8) && um::aligned(start, 4) && um::aligned(end, 4) && um::aligned(depth, 4) &&
+                 um::aligned(face, 4),
+             "um_mesh_raster: order and values 8-byte, the other int32 and fp32 buffers 4-byte aligned");
+  const long long px = (long long)n * h * w, bins = n * mesh_tiles(h, w);
+  UM_REQUIRE(um::written_disjoint({{depth, 4 * px}, {face, 4 * px}, {rgb, 3 * px}, {points, 12 * n_points},
+                                   {faces, 12 * n_faces}, {colors, 3 * n_points}, {w2c, 48LL * n},
+                                   {order, 8 * n_entries}, {values, 8 * n_entries}, {start, 4 * bins}, {end, 4 * bins}},
+                                  3),
+             "um_mesh_raster: depth, face and rgb must not overlap each other or the inputs");
+  return um::mesh_raster_launch(points, faces, colors, w2c, n, h, w, fx, fy, cx, cy, near, far,
+                                reinterpret_cast<const long long*>(order), reinterpret_cast<const long long*>(values),
+                                start, end, depth, face, rgb, (cudaStream_t)stream);
+}
+
+int um_visible_points(const float* points, int64_t n_points, const float* depth, int32_t n, int32_t h, int32_t w,
+                      const float* w2c, float fx, float fy, float cx, float cy, float tolerance, uint8_t* visible,
+                      void* stream) {
+  UM_REQUIRE(n_points >= 0 && n_points <= kMeshMax, "um_visible_points: bad point count %lld (0 .. 2^31 - 1)",
+             (long long)n_points);
+  UM_REQUIRE(n_points == 0 || (points && visible), "um_visible_points: points and visible must not be NULL");
+  UM_REQUIRE(n >= 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= kMeshMax,
+             "um_visible_points: bad views (%d x %d x %d; at most 65535 views of 2^31 - 1 pixels)", n, h, w);
+  UM_REQUIRE(n == 0 || (depth && w2c), "um_visible_points: depth and w2c must not be NULL");
+  UM_REQUIRE(fx != 0.f && fy != 0.f && finite_value(fx) && finite_value(fy) && finite_value(cx) && finite_value(cy),
+             "um_visible_points: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(finite_value(tolerance) && tolerance >= 0.f, "um_visible_points: tolerance must be finite and >= 0");
+  UM_REQUIRE(um::aligned(points, 4) && um::aligned(depth, 4) && um::aligned(w2c, 4),
+             "um_visible_points: the fp32 buffers must be 4-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{visible, n_points}, {points, 12 * n_points}, {depth, 4LL * n * h * w},
+                                   {w2c, 48LL * n}},
+                                  1),
+             "um_visible_points: visible must not overlap the inputs");
+  if (n_points == 0) return UM_OK;
+  return um::visible_points_launch(points, n_points, depth, n, h, w, w2c, fx, fy, cx, cy, tolerance, visible,
+                                   (cudaStream_t)stream);
+}
+
+int um_depth_metrics(const float* pred, const float* gt, int32_t n, int32_t h, int32_t w, float max_depth,
+                     double* partials, double* out, void* stream) {
+  UM_REQUIRE(pred && gt && partials && out, "um_depth_metrics: no pointer may be NULL");
+  UM_REQUIRE(n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= kMeshMax,
+             "um_depth_metrics: bad frames (%d x %d x %d; at most 65535 frames of 2^31 - 1 pixels)", n, h, w);
+  UM_REQUIRE(max_depth > 0.f, "um_depth_metrics: max_depth must be > 0");
+  UM_REQUIRE(um::aligned(pred, 4) && um::aligned(gt, 4) && um::aligned(partials, 8) && um::aligned(out, 8),
+             "um_depth_metrics: pred and gt 4-byte, partials and out 8-byte aligned");
+  const long long px = (long long)n * h * w, nb = ((long long)h * w + 255) / 256;
+  UM_REQUIRE(um::written_disjoint({{partials, 8LL * UM_DEPTH_METRIC_TERMS * n * nb}, {out, 8LL * UM_DEPTH_METRIC_TERMS * n},
+                                   {pred, 4 * px}, {gt, 4 * px}},
+                                  2),
+             "um_depth_metrics: partials and out must not overlap each other or the inputs");
+  return um::depth_metrics_launch(pred, gt, n, h, w, max_depth, partials, out, (cudaStream_t)stream);
 }
 
 }  // extern "C"

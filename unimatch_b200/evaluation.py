@@ -24,6 +24,10 @@ reference loop -- including its quirks, listed in each driver's docstring.
 
 `reconstruction_metrics` scores a fused reconstruction against a reference surface with Atlas's 3D metrics (accuracy,
 completeness, precision, recall, F-score), from exact nearest neighbours on the device (`um_cloud_*`).
+
+`depth_metrics` scores depth maps against reference depths with Atlas's 2D metrics (AbsRel, AbsDiff, SqRel, RMSE,
+LogRMSE, the delta thresholds and completeness), from fixed-order fp64 sums on the device (`um_depth_metrics`); the
+depths are typically `fusion.render_mesh` renderings of a predicted mesh at the input poses.
 """
 import math
 import os
@@ -539,3 +543,64 @@ def reconstruction_metrics(pred, gt, *, threshold=0.05, down_sample=0.02, device
     prec, recall = c_pred / n_pred, c_gt / n_gt
     fscore = 2 * prec * recall / (prec + recall) if prec + recall > 0 else 0.0
     return dict(out, acc=acc, comp=comp, chamfer=(acc + comp) / 2, prec=prec, recall=recall, fscore=fscore)
+
+
+DEPTH_METRIC_KEYS = ("AbsRel", "AbsDiff", "SqRel", "RMSE", "LogRMSE", "r1", "r2", "r3", "complete")
+
+
+@torch.no_grad()
+def depth_metrics(pred, gt, max_depth=10.0):
+    """Atlas's 2D depth metrics (Murez et al., ECCV 2020, `eval_depth`) of predicted depths against reference depths, on
+    the device: pred and gt device float32 [N,H,W] in metres (e.g. `render_mesh` of the predicted mesh at each input
+    pose, and the sensor depths).  Per frame, a pixel is masked in when pred is finite and > 0 and gt is finite with
+    0 < gt < max_depth; over the masked pixels AbsDiff = mean |p - g|, AbsRel = mean |p - g| / g, SqRel = mean
+    (p - g)^2 / g, RMSE = sqrt(mean (p - g)^2), LogRMSE = sqrt(mean (log p - log g)^2), and r1, r2, r3 the fractions
+    with max(g / p, p / g) < 1.25, 1.25^2, 1.25^3 (float32, correctly rounded divisions; the constants are exact);
+    complete = the fraction of all H W pixels with pred finite and > 0.  The scene value is the mean over frames, as
+    Atlas averages per-frame results; a frame with no masked pixel has NaN error metrics and is left out of their means
+    (its `complete` still counts).  Where this departs from Atlas: a non-finite prediction counts as "no estimate" (Atlas
+    masks only pred > 0), and the sums are float64 in a fixed order (per-block shuffle trees, then one ordered pass per
+    frame; no atomics, the same result from run to run) rather than numpy's float32 pairwise sums; the logs are CUDA's
+    float64 log of the float32 values.  Returns a dict of Python floats for DEPTH_METRIC_KEYS, 'n_frames' (the frames in
+    the error means) and 'per_frame', a dict of float64 numpy [N] arrays of the same keys plus 'n_masked' (the masked
+    pixel count).  One launch pair and one download; max_depth must be positive in float32."""
+    name = "depth_metrics"
+    for t, nm in ((pred, "pred"), (gt, "gt")):
+        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 3):
+            raise ValueError("%s: %s must be a device float32 tensor [N,H,W]" % (name, nm))
+    if pred.shape != gt.shape or pred.device != gt.device:
+        raise ValueError("%s: pred and gt must have one shape and one device" % name)
+    n, h, w = pred.shape
+    if n > 65535 or h * w > 2 ** 31 - 1:
+        raise ValueError("%s: at most 65535 frames of 2^31 - 1 pixels" % name)
+    if isinstance(max_depth, bool) or not isinstance(max_depth, (int, float)) or not math.isfinite(max_depth):
+        raise ValueError("%s: max_depth must be a positive finite number" % name)
+    md = float(np.float32(max_depth))
+    if not md > 0:
+        raise ValueError("%s: max_depth must be positive in float32" % name)
+    if n == 0 or h * w == 0:
+        sums = np.zeros((n, ops.DEPTH_METRIC_TERMS))
+    else:
+        with torch.cuda.device(pred.device):
+            sums = _OPS.depth_metrics(pred.contiguous(), gt.contiguous(), md).cpu().numpy()
+    return depth_metrics_from_sums(sums, h * w)
+
+
+def depth_metrics_from_sums(sums, pixels):
+    """The metrics of `depth_metrics` from the per-frame sums [N, 10] (count, |d|, |d|/g, d^2/g, d^2, (log p - log g)^2,
+    the three threshold counts, the valid prediction count) of frames of `pixels` pixels"""
+    sums = np.asarray(sums, np.float64).reshape(-1, ops.DEPTH_METRIC_TERMS)
+    c = sums[:, 0]
+    scored = c > 0
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mean = np.where(scored[:, None], sums / np.where(scored, c, 1.0)[:, None], np.nan)
+        per = {"AbsRel": mean[:, 2], "AbsDiff": mean[:, 1], "SqRel": mean[:, 3], "RMSE": np.sqrt(mean[:, 4]),
+               "LogRMSE": np.sqrt(mean[:, 5]), "r1": mean[:, 6], "r2": mean[:, 7], "r3": mean[:, 8],
+               "complete": sums[:, 9] / pixels if pixels else np.full(len(c), np.nan)}
+    out = {k: float(v[scored].mean()) if scored.any() else math.nan for k, v in per.items() if k != "complete"}
+    out["complete"] = float(per["complete"].mean()) if len(c) else math.nan
+    per["n_masked"] = c.copy()
+    out = {k: out[k] for k in DEPTH_METRIC_KEYS}
+    out["n_frames"] = int(scored.sum())
+    out["per_frame"] = {k: np.ascontiguousarray(v, np.float64) for k, v in per.items()}
+    return out

@@ -5,7 +5,10 @@ with their colours (`TSDFVolume.extract_points`), its marching-cubes mesh with p
 `um_tsdf_raycast` launch), the tracking of cameras against it (`TSDFVolume.track`, point-to-plane ICP in the um_icp_*
 launches), a binary PLY writer and reader for the points and meshes (`write_ply`, `read_ply`), and exact nearest
 neighbours and voxel down-sampling of point clouds (`nearest_neighbors`, `voxel_down_sample`, the um_cloud_* launches)
-that `evaluation.reconstruction_metrics` scores reconstructions with.  The kernels' arithmetic
+that `evaluation.reconstruction_metrics` scores reconstructions with, the rasterisation of triangle meshes from any camera
+into depth, face and colour images (`render_mesh`, the um_mesh_* launches) and the visibility of points in depth maps
+(`visible_points`, one `um_visible_points` launch), which culls both sets to what the cameras saw before scoring.  The
+kernels' arithmetic
 is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
@@ -584,3 +587,150 @@ def nearest_neighbors(queries, points, device="cuda"):
         if q.shape[0] == 0:
             return q.new_zeros((0,)), torch.zeros((0,), dtype=torch.int64, device=dev)
         return _Table(p, box).nearest(q)
+
+
+MAX_MESH_VIEWS = 65535
+MAX_BIN_ENTRIES = 2 ** 31 - 1
+
+
+def _camera(K, name):
+    fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
+    if not (all(math.isfinite(v) for v in (fx, fy, cx, cy)) and fx != 0 and fy != 0):
+        raise ValueError("%s: fx, fy, cx and cy must be finite, fx and fy nonzero" % name)
+    return fx, fy, cx, cy
+
+
+def _views(poses, name):
+    ps = [_pose44(p, name) for p in poses]
+    if not all(np.isfinite(p).all() for p in ps):
+        raise ValueError("%s: camera poses must be finite" % name)
+    if len(ps) > MAX_MESH_VIEWS:
+        raise ValueError("%s: at most 65535 cameras per call" % name)
+    return ps
+
+
+def _faces(faces, dev, name):
+    """Faces [T,3] of any integer type as a device tensor of that type (one upload for host data)"""
+    if not torch.is_tensor(faces):
+        faces = torch.from_numpy(np.ascontiguousarray(np.asarray(faces)))
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype.is_complex \
+            or faces.dtype == torch.bool:
+        raise ValueError("%s: expected integer faces [T,3], got %s %s" % (name, faces.dtype, list(faces.shape)))
+    if faces.shape[0] > MAX_MESH_INDEX:
+        raise ValueError("%s: at most 2^31 - 1 faces" % name)
+    return faces.to(dev)
+
+
+@torch.no_grad()
+def render_mesh(points, faces, intrinsics, poses, frame_size, colors=None, near=0.01, far=None, device="cuda"):
+    """Rasterise a triangle mesh on the device from N pinhole cameras: points float32 [P,3] and integer faces [T,3]
+    (device tensors, host tensors or numpy arrays, host data uploaded once; the form `TSDFVolume.extract_mesh` returns
+    and `read_ply` reads), intrinsics [3,3] at `frame_size` = (H, W), host camera-to-world poses [N,4,4] (as `render()`
+    and `fuse_depths` take them), optional uint8 vertex `colors` [P,3].  Pixel (x, y) casts the ray through its centre,
+    ((x - cx) / fx, (y - cy) / fy, 1) in camera coordinates; every face is two-sided, and the pixel takes the face hit at
+    the least camera z-depth t with near <= t <= far (None: no limit), ties to the least face index.  Edge functions are
+    evaluated from each edge's canonical vertex order, so faces sharing an edge leave no gap between them and a closed
+    mesh around the camera has no miss.  Every operation, the pixel rectangle a face is restricted to and the tie rule
+    are stated in include/unimatch_sm100.h (um_mesh_*); the result is the same from run to run.  Returns on the device
+    {'depth': float32 [N,H,W] camera z-depth, 0 for a miss (`render()`'s convention, which `fuse_depths`, `track` and
+    `depth_to_image` take), 'face': int32 [N,H,W] face index, -1 for a miss, and with `colors`, 'color': uint8 [N,H,W,3]
+    (the vertex colours at the hit's perspective-correct barycentrics)}.  An empty mesh gives all misses and no cameras
+    empty tensors.  Host reads: the vertices' bounds and the face-index range (one read), then the number of tile
+    entries (one read), so `render_mesh` cannot be captured in a CUDA graph.  Non-finite vertices, face indices outside
+    [0, P), bad intrinsics or poses, near <= 0 or far <= near, more than 65535 cameras, more than 2^31 - 1 pixels per
+    frame and more than 2^31 - 1 tile entries are refused with ValueError, before the outputs are allocated."""
+    name = "render_mesh"
+    dev = points.device if torch.is_tensor(points) and points.is_cuda else torch.device(device)
+    K = _intrinsics33(intrinsics, name)
+    fx, fy, cx, cy = _camera(K, name)
+    ps = _views(poses, name)
+    h, w = (int(v) for v in frame_size)
+    if h < 1 or w < 1 or h * w > MAX_VOXELS:
+        raise ValueError("%s: frame_size must be (H, W) with at most 2^31 - 1 pixels" % name)
+    with np.errstate(over="ignore"):
+        near = _f32(near) if math.isfinite(near) else math.nan
+        far = math.inf if far is None else (_f32(far) if not math.isnan(far) else math.nan)
+    if not (math.isfinite(near) and near > 0 and far > near):
+        raise ValueError("%s: near must be finite and > 0 in float32, far None or greater than near" % name)
+    p = _cloud(points, dev, name)
+    f = _faces(faces, dev, name)
+    col = None
+    if colors is not None:
+        col = colors if torch.is_tensor(colors) else torch.from_numpy(np.ascontiguousarray(np.asarray(colors)))
+        if col.dtype != torch.uint8 or tuple(col.shape) != (p.shape[0], 3):
+            raise ValueError("%s: colors must be uint8 [P,3], one per point" % name)
+        col = col.to(dev).contiguous()
+    n_points, n_faces, n = p.shape[0], f.shape[0], len(ps)
+    bounds = []
+    if n_points:
+        bounds += [p.amin(0).double(), p.amax(0).double()]
+    if n_faces:
+        bounds += [f.amin().double().reshape(1), f.amax().double().reshape(1)]
+    vals = torch.cat(bounds).tolist() if bounds else []                  # the one host read of the inputs
+    if n_points and not all(math.isfinite(v) for v in vals[:6]):
+        raise ValueError("%s: vertex coordinates must be finite" % name)
+    if n_faces and not (vals[-2] >= 0 and vals[-1] < n_points):
+        raise ValueError("%s: face indices must lie in [0, %d)" % (name, n_points))
+    if dev.type != "cuda":
+        raise ValueError("%s: the mesh is rendered on a CUDA device" % name)
+    with torch.cuda.device(dev):
+        if n == 0 or n_faces == 0:                                    # no camera, or every pixel a miss
+            out = {"depth": torch.zeros((n, h, w), dtype=torch.float32, device=dev),
+                   "face": torch.full((n, h, w), -1, dtype=torch.int32, device=dev)}
+            if col is not None:
+                out["color"] = torch.zeros((n, h, w, 3), dtype=torch.uint8, device=dev)
+            return out
+        fi = f.to(torch.int32).contiguous()
+        w2c = torch.from_numpy(_world_to_camera(ps)).to(dev)
+        cam = (h, w, fx, fy, cx, cy, near, far)
+        offsets = _OPS.mesh_bin_count(p, fi, w2c, *cam)
+        n_entries = int(offsets[-1].item())
+        if n_entries > MAX_BIN_ENTRIES:
+            raise ValueError("%s: %d tile entries is more than 2^31 - 1 (fewer cameras or faces per call)"
+                             % (name, n_entries))
+        if n_entries:
+            keys, values = _OPS.mesh_bin(p, fi, w2c, *cam, offsets, n_entries)
+            del offsets
+            keys, order = torch.sort(keys, stable=True)
+        else:
+            keys = order = values = torch.zeros((0,), dtype=torch.int64, device=dev)
+        start, end = _OPS.mesh_ranges(keys, n, h, w)
+        del keys
+        depth, face, rgb = _OPS.mesh_raster(p, fi, col, w2c, *cam, order, values, start, end)
+    out = {"depth": depth, "face": face}
+    if col is not None:
+        out["color"] = rgb
+    return out
+
+
+@torch.no_grad()
+def visible_points(points, depths, intrinsics, poses, tolerance=0.05):
+    """Which points some camera saw: bool [P] on the depths' device.  points float32 [P,3] (a device tensor, a host
+    tensor or a numpy array, uploaded once), depths device float32 [N,H,W] (e.g. `render_mesh` of a reference mesh,
+    sensor depths or `TSDFVolume.render`), intrinsics [3,3] at (H, W) and host camera-to-world poses [N,4,4].  Each view
+    in order transforms and projects the point exactly as `fuse_depths` projects a voxel (camera z > 0, the nearest pixel
+    inside the frame) and sees it iff that pixel's depth D is finite, D > 0 and z <= D + tolerance (float32).  A point
+    with a non-finite coordinate is seen by no view.  One thread per point, no atomics (um_visible_points).  Culling for
+    the 3D metrics is then plain indexing: `reconstruction_metrics(pred[vis_pred], gt[vis_gt])`.  The default tolerance
+    is the metrics' default threshold: an occluder closer in depth than that hardly moves them."""
+    name = "visible_points"
+    if not (torch.is_tensor(depths) and depths.is_cuda and depths.dtype == torch.float32 and depths.dim() == 3):
+        raise ValueError("%s: depths must be a device float32 tensor [N,H,W]" % name)
+    n, h, w = depths.shape
+    if h * w > MAX_VOXELS:
+        raise ValueError("%s: at most 2^31 - 1 pixels per depth map" % name)
+    K = _intrinsics33(intrinsics, name)
+    fx, fy, cx, cy = _camera(K, name)
+    ps = _views(poses, name)
+    if len(ps) != n:
+        raise ValueError("%s: %d depth maps need %d poses, got %d" % (name, n, n, len(ps)))
+    if isinstance(tolerance, bool) or not isinstance(tolerance, (int, float)) or not math.isfinite(tolerance) \
+            or tolerance < 0:
+        raise ValueError("%s: tolerance must be finite and >= 0" % name)
+    dev = depths.device
+    p = _cloud(points, dev, name)
+    with torch.cuda.device(dev):
+        if n == 0 or p.shape[0] == 0:
+            return torch.zeros((p.shape[0],), dtype=torch.bool, device=dev)
+        w2c = torch.from_numpy(_world_to_camera(ps)).to(dev)
+        return _OPS.visible_points(p, depths.contiguous(), w2c, fx, fy, cx, cy, _f32(tolerance))

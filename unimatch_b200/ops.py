@@ -137,6 +137,13 @@ _SIGNATURES = {
     "um_cloud_down_sample": (_RC, [_P, _P, _P, _L, _P, _L, _P, _P]),
     "um_cloud_nearest": (_RC, [_P, _L, _P, _P, _P, _L, _D, _D, _D, _D, _I, _I, _I, _F, _P, _P, _P, _P, _P]),
     "um_cloud_stats": (_RC, [_P, _P, _L, _P, _P]),
+    "um_mesh_bin_count": (_RC, [_P, _L, _P, _L, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P]),
+    "um_mesh_bin": (_RC, [_P, _L, _P, _L, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _L, _P, _P, _P]),
+    "um_mesh_ranges": (_RC, [_P, _L, _I, _I, _I, _P, _P, _P]),
+    "um_mesh_raster": (_RC, [_P, _L, _P, _L, _P, _P, _I, _I, _I, _F, _F, _F, _F, _F, _F, _P, _P, _L, _P, _P, _P, _P, _P,
+                             _P]),
+    "um_visible_points": (_RC, [_P, _L, _P, _I, _I, _I, _P, _F, _F, _F, _F, _F, _P, _P]),
+    "um_depth_metrics": (_RC, [_P, _P, _I, _I, _I, _F, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -955,6 +962,141 @@ def _cloud_stats(partial_sum, partial_count, out):
 
 
 cloud_stats = _define("cloud_stats(Tensor partial_sum, Tensor partial_count, Tensor(a!) out) -> ()", _cloud_stats)
+
+
+
+# ---- triangle meshes: rasterisation, point visibility, depth metrics (include/unimatch_sm100.h, um_mesh_* ...) -------
+MESH_TILE = 16                                       # pixels per side of the rasteriser's tiles
+DEPTH_METRIC_TERMS = 10                              # UM_DEPTH_METRIC_TERMS: fp64 sums per frame
+
+
+def mesh_tiles(h, w):
+    """The rasteriser's tiles per view of h x w pixels"""
+    return -(-h // MESH_TILE) * -(-w // MESH_TILE)
+
+
+def _mesh_args(points, faces, w2c, name):
+    """(P, T, n) of a contiguous device fp32 [P, 3] point set, int32 [T, 3] faces and fp32 [n, 3, 4] rows on one device"""
+    _f32c(points, name + ": points")
+    _f32c(w2c, name + ": w2c")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("%s: expected points [P, 3]" % name)
+    if faces.dtype != torch.int32 or faces.dim() != 2 or faces.shape[1] != 3 or not faces.is_contiguous():
+        raise RuntimeError("%s: expected contiguous int32 faces [T, 3]" % name)
+    if w2c.dim() != 3 or tuple(w2c.shape[1:]) != (3, 4):
+        raise RuntimeError("%s: expected world-to-camera rows [n, 3, 4]" % name)
+    _device_like(name, points, faces, w2c)
+    return points.shape[0], faces.shape[0], w2c.shape[0]
+
+
+def _mesh_bin_count(points, faces, w2c, h, w, fx, fy, cx, cy, near, far):
+    """The bin offsets, device int64 [n ceil(T / 256) + 1]: per (view, block of 256 faces) its first tile entry, then the
+    number of entries"""
+    p, t, n = _mesh_args(points, faces, w2c, "mesh_bin_count")
+    offsets = torch.empty((n * -(-t // 256) + 1,), device=points.device, dtype=torch.int64)
+    _check(LIB.um_mesh_bin_count(_p(points), p, _p(faces), t, _p(w2c), n, h, w, fx, fy, cx, cy, near, far, _p(offsets),
+                                 _stream()), "um_mesh_bin_count")
+    return offsets
+
+
+mesh_bin_count = _define("mesh_bin_count(Tensor points, Tensor faces, Tensor w2c, int h, int w, float fx, float fy, "
+                         "float cx, float cy, float near, float far) -> Tensor", _mesh_bin_count)
+
+
+def _mesh_bin(points, faces, w2c, h, w, fx, fy, cx, cy, near, far, offsets, n_entries):
+    """The n_entries tile entries: keys int64 (view * tiles + tile) and values int64 (face << 16 | in-tile rectangle)"""
+    p, t, n = _mesh_args(points, faces, w2c, "mesh_bin")
+    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (n * -(-t // 256) + 1,) or offsets.device != points.device:
+        raise RuntimeError("mesh_bin: offsets must be mesh_bin_count's device int64 table")
+    keys = torch.empty((n_entries,), device=points.device, dtype=torch.int64)
+    values = torch.empty_like(keys)
+    _check(LIB.um_mesh_bin(_p(points), p, _p(faces), t, _p(w2c), n, h, w, fx, fy, cx, cy, near, far, _p(offsets),
+                           n_entries, _p(keys), _p(values), _stream()), "um_mesh_bin")
+    return keys, values
+
+
+mesh_bin = _define("mesh_bin(Tensor points, Tensor faces, Tensor w2c, int h, int w, float fx, float fy, float cx, "
+                   "float cy, float near, float far, Tensor offsets, int n_entries) -> (Tensor, Tensor)", _mesh_bin)
+
+
+def _mesh_ranges(sorted_keys, n, h, w):
+    """The first and one-past-last sorted position of each (view, tile)'s entries: start / end int32 [n, tiles]"""
+    if sorted_keys.dtype != torch.int64 or sorted_keys.dim() != 1 or not sorted_keys.is_contiguous():
+        raise RuntimeError("mesh_ranges: sorted_keys must be contiguous int64 [E]")
+    start = torch.empty((n, mesh_tiles(h, w)), device=sorted_keys.device, dtype=torch.int32)
+    end = torch.empty_like(start)
+    _check(LIB.um_mesh_ranges(_p(sorted_keys), sorted_keys.shape[0], n, h, w, _p(start), _p(end), _stream()),
+           "um_mesh_ranges")
+    return start, end
+
+
+mesh_ranges = _define("mesh_ranges(Tensor sorted_keys, int n, int h, int w) -> (Tensor, Tensor)", _mesh_ranges)
+
+
+def _mesh_raster(points, faces, colors, w2c, h, w, fx, fy, cx, cy, near, far, order, values, start, end):
+    """depth fp32 [n, h, w] (0: miss), face int32 [n, h, w] (-1: miss) and, with colors (uint8 [P, 3]), rgb uint8
+    [n, h, w, 3]"""
+    p, t, n = _mesh_args(points, faces, w2c, "mesh_raster")
+    e = values.shape[0]
+    if order.dtype != torch.int64 or values.dtype != torch.int64 or tuple(order.shape) != (e,) or values.dim() != 1 \
+            or not order.is_contiguous() or not values.is_contiguous():
+        raise RuntimeError("mesh_raster: order and values must be contiguous int64 [E]")
+    if start.dtype != torch.int32 or tuple(start.shape) != (n, mesh_tiles(h, w)) or end.shape != start.shape \
+            or end.dtype != torch.int32 or not start.is_contiguous() or not end.is_contiguous():
+        raise RuntimeError("mesh_raster: start and end must be mesh_ranges' int32 [n, tiles] tables")
+    if colors is not None and (colors.dtype != torch.uint8 or tuple(colors.shape) != (p, 3) or not colors.is_contiguous()):
+        raise RuntimeError("mesh_raster: colors must be contiguous uint8 [P, 3]")
+    _device_like("mesh_raster", points, order, values, start, end, *([colors] if colors is not None else []))
+    dev = points.device
+    depth = torch.empty((n, h, w), device=dev, dtype=torch.float32)
+    face = torch.empty((n, h, w), device=dev, dtype=torch.int32)
+    rgb = torch.empty((n, h, w, 3) if colors is not None else (0,), device=dev, dtype=torch.uint8)
+    _check(LIB.um_mesh_raster(_p(points), p, _p(faces), t, _p(colors), _p(w2c), n, h, w, fx, fy, cx, cy, near, far,
+                              _p(order), _p(values), e, _p(start), _p(end), _p(depth), _p(face),
+                              _p(rgb) if colors is not None else None, _stream()), "um_mesh_raster")
+    return depth, face, rgb
+
+
+mesh_raster = _define("mesh_raster(Tensor points, Tensor faces, Tensor? colors, Tensor w2c, int h, int w, float fx, "
+                      "float fy, float cx, float cy, float near, float far, Tensor order, Tensor values, Tensor start, "
+                      "Tensor end) -> (Tensor, Tensor, Tensor)", _mesh_raster)
+
+
+def _visible_points(points, depth, w2c, fx, fy, cx, cy, tolerance):
+    """bool [P]: some view's depth map (fp32 [n, h, w]) sees the point (um_visible_points)"""
+    _f32c(points, "visible_points: points")
+    _f32c(depth, "visible_points: depth")
+    _f32c(w2c, "visible_points: w2c")
+    if points.dim() != 2 or points.shape[1] != 3 or depth.dim() != 3 or tuple(w2c.shape) != (depth.shape[0], 3, 4):
+        raise RuntimeError("visible_points: expected points [P, 3], depth [n, h, w] and w2c [n, 3, 4]")
+    _device_like("visible_points", points, depth, w2c)
+    n, h, w = depth.shape
+    visible = torch.empty((points.shape[0],), device=points.device, dtype=torch.bool)
+    _check(LIB.um_visible_points(_p(points), points.shape[0], _p(depth), n, h, w, _p(w2c), fx, fy, cx, cy, tolerance,
+                                 _p(visible), _stream()), "um_visible_points")
+    return visible
+
+
+visible_points = _define("visible_points(Tensor points, Tensor depth, Tensor w2c, float fx, float fy, float cx, float cy, "
+                         "float tolerance) -> Tensor", _visible_points)
+
+
+def _depth_metrics(pred, gt, max_depth):
+    """The per-frame sums of the depth metrics' terms, fp64 [n, DEPTH_METRIC_TERMS] (um_depth_metrics)"""
+    _f32c(pred, "depth_metrics: pred")
+    _f32c(gt, "depth_metrics: gt")
+    if pred.dim() != 3 or gt.shape != pred.shape:
+        raise RuntimeError("depth_metrics: expected pred and gt [n, h, w] of one shape")
+    _device_like("depth_metrics", pred, gt)
+    n, h, w = pred.shape
+    partials = torch.empty((n, -(-(h * w) // 256), DEPTH_METRIC_TERMS), device=pred.device, dtype=torch.float64)
+    out = torch.empty((n, DEPTH_METRIC_TERMS), device=pred.device, dtype=torch.float64)
+    _check(LIB.um_depth_metrics(_p(pred), _p(gt), n, h, w, max_depth, _p(partials), _p(out), _stream()),
+           "um_depth_metrics")
+    return out
+
+
+depth_metrics = _define("depth_metrics(Tensor pred, Tensor gt, float max_depth) -> Tensor", _depth_metrics)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
