@@ -123,23 +123,47 @@ def _c2(x, w, stride, pad):
     return torch.nn.functional.conv2d(x, w, None, stride=stride, padding=pad)
 
 
+def patches(x, kh, kw, stride, pad, pix):
+    """Input patches [P, c * kh * kw] (channel-major, the order of weight.flatten(1)) of the output pixels pix = (b, y, x) of
+    a convolution over the channel-last map x [B, H, W, c], zeros outside the image."""
+    b, yo, xo = pix
+    H, W = x.shape[1], x.shape[2]
+    Y = (yo[:, None] * stride - pad[0] + torch.arange(kh))[:, :, None].expand(-1, kh, kw)
+    X = (xo[:, None] * stride - pad[1] + torch.arange(kw))[:, None, :].expand(-1, kh, kw)
+    ok = (Y >= 0) & (Y < H) & (X >= 0) & (X < W)
+    v = x[b[:, None, None].expand_as(Y), Y.clamp(0, H - 1), X.clamp(0, W - 1)] * ok[..., None].to(x.dtype)
+    return v.permute(0, 3, 1, 2).reshape(b.numel(), -1)
+
+
 def conv64(xs, wt, bias=None, pad=(0, 0), stride=1, mode=CONV_LINEAR, act=0, aux0=None, aux1=None, gamma=None, beta=None,
-           pre=None):
+           pre=None, pix=None):
     """xs: channel-last fp32 sources [B, H, W, c_i] (concatenated along channels), wt: fp32 [cout, sum c_i, kh, kw].
-    Returns (out, bound) channel-last float64 [B, Ho, Wo, cout] of what um_conv2d_tc writes: GRU_ZR -> [z | r * h]."""
-    x32 = torch.cat([x.float() for x in xs], -1).permute(0, 3, 1, 2)
-    x, xh = x32.double(), split_sum(x32)
-    w, wh = wt.double(), split_sum(wt)
-    y = _c2(x, w, stride, pad)
-    a = _c2(x.abs(), w.abs(), stride, pad)
-    r = torch.sqrt(_c2(x * x, w * w, stride, pad))
-    rep = _c2((x - xh).abs(), w.abs(), stride, pad) + _c2(xh.abs(), (w - wh).abs(), stride, pad)
+    Returns (out, bound) channel-last float64 [B, Ho, Wo, cout] of what um_conv2d_tc writes: GRU_ZR -> [z | r * h].
+    pix = (b, y, x) output pixels: (out, bound) [P, cout] at those pixels only (aux0, aux1 and pre stay whole maps)."""
     kh, kw = wt.shape[2], wt.shape[3]
+    w, wh = wt.double(), split_sum(wt)
+    if pix is None:
+        x32 = torch.cat([x.float() for x in xs], -1).permute(0, 3, 1, 2)
+        x, xh = x32.double(), split_sum(x32)
+        y = _c2(x, w, stride, pad)
+        a = _c2(x.abs(), w.abs(), stride, pad)
+        r = torch.sqrt(_c2(x * x, w * w, stride, pad))
+        rep = _c2((x - xh).abs(), w.abs(), stride, pad) + _c2(xh.abs(), (w - wh).abs(), stride, pad)
+    else:
+        p32 = patches(torch.cat([x.float() for x in xs], -1), kh, kw, stride, pad, pix)
+        x, xh = p32.double(), split_sum(p32)
+        w, wh = w.flatten(1), wh.flatten(1)
+        y = x @ w.T
+        a = x.abs() @ w.abs().T
+        r = torch.sqrt((x * x) @ (w * w).T)
+        rep = (x - xh).abs() @ w.abs().T + xh.abs() @ (w - wh).abs().T
+        aux0, aux1, pre = (None if t is None else t[pix] for t in (aux0, aux1, pre))
     ktot = sum((c.shape[-1] + 63) // 64 * 64 for c in xs) * kh * kw
     nk = ktot // 64
     steps = 12 + nk if nk >= 8 else 12 * nk          # K >= 512: fresh accumulator per 64-wide stage, then fp32 adds
     e = G0 * a + steps * U_STEP * (y.abs() + WALK * r) + rep
-    y, e = y.permute(0, 2, 3, 1), e.permute(0, 2, 3, 1)
+    if pix is None:
+        y, e = y.permute(0, 2, 3, 1), e.permute(0, 2, 3, 1)
     if bias is not None:
         y = y + bias.double()
         e = e + U32 * y.abs()
@@ -238,29 +262,36 @@ def softmax_weighted(s, ds, vals, v_rep=None, tc_pv=True):
     return o, b
 
 
-def attention64(q, k, v, kv_shift, h, w, kh, kw, sh, sw, mask_mode, tc=True):
+def attention64(q, k, v, kv_shift, h, w, kh, kw, sh, sw, mask_mode, tc=True, rows=None):
     """softmax(Q K^T / sqrt(128) + Swin mask) V per window with the cyclic shift and the roll back; key / value stream of
-    stream n is (n + kv_shift) mod n_streams.  q, k, v: fp32 [n, h*w, 128].  Returns (out, bound, locate)."""
+    stream n is (n + kv_shift) mod n_streams.  q, k, v: fp32 [n, h*w, 128].  Returns (out, bound, locate), [n, h*w, 128],
+    or [n, R, 128] for the query tokens `rows` (sorted, distinct) only."""
     n = q.shape[0]
     tok, reg = window_layout(h, w, kh, kw, sh, sw)
     nwin, lw = tok.shape
-    out = torch.zeros((n, h * w, C), dtype=torch.float64)
+    rows = torch.arange(h * w) if rows is None else rows
+    slot = torch.full((h * w,), -1, dtype=torch.long)                  # token -> index into rows
+    slot[rows] = torch.arange(rows.numel())
+    out = torch.zeros((n, rows.numel(), C), dtype=torch.float64)
     bnd = torch.zeros_like(out)
-    for s_ in range(n):
-        ks = (s_ + kv_shift) % n
-        for wi in range(nwin):
-            t = tok[wi]
-            qw, kk, vv = q[s_, t], k[ks, t], v[ks, t]
+    for wi in range(nwin):
+        t = tok[wi]
+        sel = (slot[t] >= 0).nonzero().view(-1)                        # window positions of the queries evaluated
+        if sel.numel() == 0:
+            continue
+        m = reg[wi][sel][:, None] != reg[wi][None, :]
+        for s_ in range(n):
+            ks = (s_ + kv_shift) % n
+            qw, kk, vv = q[s_, t[sel]], k[ks, t], v[ks, t]
             s, e = _logit_bound(qw, kk)
             s, e = s / math.sqrt(C), e / math.sqrt(C)
             if mask_mode == MASK_SWIN:
-                m = reg[wi][:, None] != reg[wi][None, :]
                 s = s - 100.0 * m
                 e = e + U_STEP * 100.0 * m
             vd = vv.double()
             o, b = softmax_weighted(s, e, vd, (vd - split_sum(vv)).abs(), tc_pv=tc)
-            out[s_, t] = o
-            bnd[s_, t] = b
+            out[s_, slot[t[sel]]] = o
+            bnd[s_, slot[t[sel]]] = b
 
     pos = torch.empty(h * w, dtype=torch.long)
     win = torch.empty(h * w, dtype=torch.long)
@@ -269,7 +300,8 @@ def attention64(q, k, v, kv_shift, h, w, kh, kw, sh, sw, mask_mode, tc=True):
         win[tok[wi]] = wi
 
     def locate(idx):
-        st, t, c = idx
+        st, r, c = idx
+        t = rows[r]
         return "stream %d, window %d, query tile %d, row %d, channel %d" % (st, win[t], pos[t] // 128, pos[t] % 128, c)
     return out, bnd, locate
 
@@ -615,24 +647,29 @@ def add_position_ref(x, table, h, w):
     return x + table.repeat(h // wh, w // ww, 1)[None]
 
 
-def conv7x7_64(x, weight, bias, stride, relu, scale=None, shift=None):
+def conv7x7_64(x, weight, bias, stride, relu, scale=None, shift=None, pix=None):
     """The 7x7 stem / flow-encoder convolution, padding 3, on planar [N, cin, H, W] input: x * scale + shift per channel
     inside the image (the folded ImageNet normalisation), zeros outside, then + bias and ReLU.  The kernel is one fp32 FMA
-    chain of 49 cin products per output.  Returns (out, bound) channel-last [N, Ho, Wo, cout]."""
+    chain of 49 cin products per output.  Returns (out, bound) channel-last [N, Ho, Wo, cout], or [P, cout] at the output
+    pixels pix = (b, y, x)."""
     xd = x.double()
     if scale is not None:
         xd = xd * torch.tensor(scale, dtype=torch.float32).double().view(1, -1, 1, 1) + \
              torch.tensor(shift, dtype=torch.float32).double().view(1, -1, 1, 1)
     wd = weight.double()
-    y = torch.nn.functional.conv2d(xd, wd, None, stride=stride, padding=3)
-    a = torch.nn.functional.conv2d(xd.abs(), wd.abs(), None, stride=stride, padding=3)
+    if pix is None:
+        y = torch.nn.functional.conv2d(xd, wd, None, stride=stride, padding=3).permute(0, 2, 3, 1)
+        a = torch.nn.functional.conv2d(xd.abs(), wd.abs(), None, stride=stride, padding=3).permute(0, 2, 3, 1)
+    else:
+        p = patches(xd.permute(0, 2, 3, 1), 7, 7, stride, (3, 3), pix)
+        y, a = p @ wd.flatten(1).T, p.abs() @ wd.flatten(1).abs().T
     e = gamma(49 * x.shape[1] + 3) * a
     if bias is not None:
-        y = y + bias.double().view(1, -1, 1, 1)
-        e = e + gamma(49 * x.shape[1] + 3) * bias.double().abs().view(1, -1, 1, 1)
+        y = y + bias.double()
+        e = e + gamma(49 * x.shape[1] + 3) * bias.double().abs()
     if relu:
         y = torch.relu(y)
-    return y.permute(0, 2, 3, 1), e.permute(0, 2, 3, 1)
+    return y, e
 
 
 def pixel_subset(B, h, w, gen, seam_x=(), seam_y=(), n_seam=2000, n_rand=300):

@@ -37,6 +37,7 @@ ATTN_EDGE = [
     ("swin1d_shifted_lw256", 2, 4, 512, 4, 2, True, 1, 1.5),    # 1-D region mask on the tensor cores
     ("swin2d_lw390", 2, 30, 52, 2, 2, False, 1, 1.5),
     ("swin2d_first_tile_masked", 2, 32, 16, 2, 2, True, 1, 1.5),
+    ("swin2d_lw2304_cuda_cores", 1, 96, 96, 2, 2, False, 0, 1.5),  # windows > MAX_LP (Middlebury stereo at 1/8: 6144)
     ("swin1d_lw60_cuda_cores", 2, 4, 240, 4, 4, False, 1, 1.5),  # gmstereo-scale2's 1-D windows
     ("swin1d_lw60_shifted_cuda_cores", 2, 4, 240, 4, 4, True, 1, 1.5),
     ("three_streams_kvshift2", 3, 16, 24, 2, 2, True, 2, 1.5),
