@@ -725,6 +725,45 @@ int um_visible_points(const float* points, int64_t n_points, const float* depth,
 int um_depth_metrics(const float* pred, const float* gt, int32_t n, int32_t h, int32_t w, float max_depth,
                      double* partials, double* out, void* stream);
 
+/* ---- multi-view geometric consistency of depth maps, and valid depths as coloured world points ---------------------
+ * n depth maps depth fp32 [n, h, w] of one frame size with one pinhole camera fx, fy (finite, nonzero), cx, cy (finite);
+ * camera-to-world rows c2w and world-to-camera rows w2c fp32 [n, 3, 4] (row-major, as um_tsdf_raycast and
+ * um_tsdf_integrate read them).  A depth is valid iff it is finite and > 0.  fp32 operations are each rounded on their own
+ * (__fmaf_rn, __fdiv_rn, __fsqrt_rn, ...), in the order written.  Rows M applied to a point p:
+ *   M p = (fma(M02, p.z, fma(M01, p.y, fma(M00, p.x, M03))), likewise rows 1 and 2).
+ * Back-projection of pixel coordinates (u, v) at depth z: B(u, v, z) = ((u - cx) / fx * z, (v - cy) / fy * z, z), so pixel
+ * (x, y) is the ray through its centre (um_tsdf_raycast's and um_mesh_raster's convention).
+ * Consistency (um_depth_consistency): refs int32 [R] are the reference maps and sources int32 [R, S] their sources in
+ * order; an entry outside [0, n) is "no source" (and a reference outside [0, n) has no valid depth), so no table reads out
+ * of bounds.  One thread per reference pixel (x, y) of reference r with d = depth[r, y, x]; if d is valid, per source s:
+ *   c = w2c[s] (c2w[r] B(x, y, d));  the source does not count unless c.z > 0;
+ *   u = fma(fx, c.x / c.z, cx), v = fma(fy, c.y / c.z, cy);  it does not count unless 0 <= u <= w - 1 and
+ *   0 <= v <= h - 1 (a NaN does not count);
+ *   x0 = floor(u), y0 = floor(v), x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1), ax = u - x0, ay = v - y0 (exact);
+ *   the taps D00 = depth[s, y0, x0], D01 = [s, y0, x1], D10 = [s, y1, x0], D11 = [s, y1, x1] must all be valid;
+ *   top = fma(ax, D01 - D00, D00), bot = fma(ax, D11 - D10, D10), ds = fma(ay, bot - top, top)  (bilinear);
+ *   c' = w2c[r] (c2w[s] B(u, v, ds));  it does not count unless c'.z > 0;
+ *   u' = fma(fx, c'.x / c'.z, cx), v' = fma(fy, c'.y / c'.z, cy), dx = u' - x, dy = v' - y;
+ *   it is consistent iff sqrt(fma(dy, dy, dx * dx)) < max_pixel and |c'.z - d| / d < max_relative.
+ * views uint8 [R, h, w] = the number of consistent sources (0 for an invalid d); out fp32 [R, h, w] = d where
+ * views >= min_views, else 0.  S 1 .. 255, min_views 1 .. S, max_pixel and max_relative positive and finite, R 1 .. 65535.
+ * No atomics, no host synchronisation (graph-capturable); the same output from run to run.
+ * Points (um_depth_points_count, um_depth_points): every valid depth d = depth[t, y, x] gives the world point
+ * c2w[t] B(x, y, d) and the colour frames[t, y, x] (uint8 [n, h, w, 3]), ordered by frame, then row-major pixel.
+ * um_depth_points_count writes offsets [nb + 1] (DEVICE int64, nb = ceil(n h w / 256)): offsets[b] the first point of
+ * pixels b * 256 ... (frame-major), offsets[nb] the total P, which the caller reads to allocate points fp32 [P, 3] and
+ * colors uint8 [P, 3] (P <= 2^31 - 1); um_depth_points (n_points = P) writes them, and with P = 0 launches nothing.  A count
+ * pass, one ordered scan of the block counts and a write pass: no atomics.  n 1 .. 65535, h w <= 2^31 - 1, n h w <= 2^39.
+ * Every pointer is DEVICE memory; no output overlaps an input or another output. */
+int um_depth_consistency(const float* depth, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy,
+                         const float* c2w, const float* w2c, const int32_t* refs, int32_t r, const int32_t* sources,
+                         int32_t s, float max_pixel, float max_relative, int32_t min_views, uint8_t* views, float* out,
+                         void* stream);
+int um_depth_points_count(const float* depth, int32_t n, int32_t h, int32_t w, int64_t* offsets, void* stream);
+int um_depth_points(const float* depth, const uint8_t* frames, int32_t n, int32_t h, int32_t w, float fx, float fy,
+                    float cx, float cy, const float* c2w, const int64_t* offsets, int64_t n_points, float* points,
+                    uint8_t* colors, void* stream);
+
 /* Middlebury colour coding of n planar flows [n, 2, h, w] -> uint8 RGB pictures: pixel (y, x) of image i is written at
  * out + i * image_stride + y * row_stride + 3 * x (strides in BYTES; row_stride >= 3w), so a picture can land inside a larger
  * frame (e.g. next to the video frame).  Per image: |u| or |v| > 1e7 are unknown (black, excluded from the maximum), the

@@ -54,6 +54,9 @@ _LAZY = {
     "render_mesh": (".fusion", "render_mesh"),
     "visible_points": (".fusion", "visible_points"),
     "depth_metrics": (".evaluation", "depth_metrics"),
+    "sequence_sources": (".fusion", "sequence_sources"),
+    "filter_depths": (".fusion", "filter_depths"),
+    "depth_points": (".fusion", "depth_points"),
     "validate_flow": (".evaluation", "validate_flow"),
     "validate_stereo": (".evaluation", "validate_stereo"),
     "validate_depth": (".evaluation", "validate_depth"),
@@ -74,7 +77,7 @@ __all__ = ["UniMatch", "ops", "WORKLOADS", "BASELINE_CONFIGS", "param_spec", "In
            "inference_flow", "inference_stereo", "inference_depth", "warp_disparity", "infer_scene_flow", "SceneFlowRunner",
            "validate_scene_flow", "create_scene_flow_submission", "DepthFusionRunner", "TSDFVolume", "fuse_depths", "write_ply",
            "read_ply", "nearest_neighbors", "voxel_down_sample", "reconstruction_metrics",
-           "render_mesh", "visible_points", "depth_metrics"]
+           "render_mesh", "visible_points", "depth_metrics", "sequence_sources", "filter_depths", "depth_points"]
 
 
 def __getattr__(name):

@@ -1,7 +1,8 @@
 // C-ABI glue: error reporting, launch accounting, the attention entry points (argument checking + dispatch
 // between the tensor-core and the general CUDA-core kernels) the point-track entries and the disparity warp (um_tracks.cu),
 // TSDF fusion (um_fusion.cu), ICP tracking against the volume (um_icp.cu), the point-cloud ops (um_cloud.cu) and the mesh
-// rasteriser, point visibility and depth metrics (um_raster.cu).  See include/unimatch_sm100.h.
+// rasteriser, point visibility and depth metrics (um_raster.cu) and the multi-view consistency of depth maps and their
+// export as points (um_consistency.cu).  See include/unimatch_sm100.h.
 #include <stdarg.h>
 
 #include <atomic>
@@ -109,6 +110,14 @@ int visible_points_launch(const float* points, long long P, const float* depth, 
                           float fx, float fy, float cx, float cy, float tolerance, uint8_t* visible, cudaStream_t st);
 int depth_metrics_launch(const float* pred, const float* gt, int n, int h, int w, float max_depth, double* partials,
                          double* out, cudaStream_t st);
+int depth_consistency_launch(const float* depth, int N, int H, int W, float fx, float fy, float cx, float cy,
+                             const float* c2w, const float* w2c, const int* refs, int R, const int* src, int S,
+                             float max_pixel, float max_relative, int min_views, uint8_t* views, float* out,
+                             cudaStream_t st);
+int depth_points_count_launch(const float* depth, long long total, long long* offsets, cudaStream_t st);
+int depth_points_launch(const float* depth, const uint8_t* frames, int N, int H, int W, float fx, float fy, float cx,
+                        float cy, const float* c2w, const long long* offsets, float* points, uint8_t* colors,
+                        cudaStream_t st);
 
 static bool overlap(const void* a, long long abytes, const void* b, long long bbytes) {
   const uintptr_t x = reinterpret_cast<uintptr_t>(a), y = reinterpret_cast<uintptr_t>(b);
@@ -820,6 +829,75 @@ int um_depth_metrics(const float* pred, const float* gt, int32_t n, int32_t h, i
                                   2),
              "um_depth_metrics: partials and out must not overlap each other or the inputs");
   return um::depth_metrics_launch(pred, gt, n, h, w, max_depth, partials, out, (cudaStream_t)stream);
+}
+
+// ---- multi-view consistency of depth maps and their points (um_consistency.cu) ----
+static const long long kMaxDepthPixels = 1LL << 39;          // the point passes' blocks of 256 fit a 2^31 - 1 grid
+
+// n maps of h x w: n 1 .. 65535, h w <= 2^31 - 1, n h w <= 2^39
+static bool depth_maps(int32_t n, int32_t h, int32_t w) {
+  return n > 0 && n <= 65535 && h > 0 && w > 0 && (long long)h * w <= 0x7fffffffLL && (long long)n * h * w <= kMaxDepthPixels;
+}
+
+int um_depth_consistency(const float* depth, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy,
+                         const float* c2w, const float* w2c, const int32_t* refs, int32_t r, const int32_t* sources,
+                         int32_t s, float max_pixel, float max_relative, int32_t min_views, uint8_t* views, float* out,
+                         void* stream) {
+  UM_REQUIRE(depth && c2w && w2c && refs && sources && views && out, "um_depth_consistency: no pointer may be NULL");
+  UM_REQUIRE(depth_maps(n, h, w),
+             "um_depth_consistency: bad depths (%d x %d x %d; 1 .. 65535 maps of 1 .. 2^31 - 1 pixels, 2^39 in all)", n, h,
+             w);
+  UM_REQUIRE(r > 0 && r <= 65535, "um_depth_consistency: bad reference count %d (1 .. 65535)", r);
+  UM_REQUIRE(s > 0 && s <= 255, "um_depth_consistency: bad source count %d (1 .. 255: views is uint8)", s);
+  UM_REQUIRE(min_views >= 1 && min_views <= s, "um_depth_consistency: min_views %d outside [1, %d]", min_views, s);
+  UM_REQUIRE(positive_finite(max_pixel) && positive_finite(max_relative),
+             "um_depth_consistency: max_pixel and max_relative must be positive and finite");
+  UM_REQUIRE(icp_intrinsics(fx, fy, cx, cy), "um_depth_consistency: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(um::aligned(depth, 4) && um::aligned(c2w, 4) && um::aligned(w2c, 4) && um::aligned(refs, 4) &&
+                 um::aligned(sources, 4) && um::aligned(out, 4),
+             "um_depth_consistency: the fp32 and int32 buffers must be 4-byte aligned");
+  const long long hw = (long long)h * w, px = (long long)r * hw;
+  UM_REQUIRE(um::written_disjoint({{views, px}, {out, 4 * px}, {depth, 4 * n * hw}, {c2w, 48LL * n}, {w2c, 48LL * n},
+                                   {refs, 4LL * r}, {sources, 4LL * r * s}},
+                                  2),
+             "um_depth_consistency: views and out must not overlap each other or the inputs");
+  return um::depth_consistency_launch(depth, n, h, w, fx, fy, cx, cy, c2w, w2c, refs, r, sources, s, max_pixel,
+                                      max_relative, min_views, views, out, (cudaStream_t)stream);
+}
+
+int um_depth_points_count(const float* depth, int32_t n, int32_t h, int32_t w, int64_t* offsets, void* stream) {
+  UM_REQUIRE(depth && offsets, "um_depth_points_count: no pointer may be NULL");
+  UM_REQUIRE(depth_maps(n, h, w),
+             "um_depth_points_count: bad depths (%d x %d x %d; 1 .. 65535 maps of 1 .. 2^31 - 1 pixels, 2^39 in all)", n,
+             h, w);
+  UM_REQUIRE(um::aligned(depth, 4) && um::aligned(offsets, 8),
+             "um_depth_points_count: depth 4-byte, offsets 8-byte aligned");
+  const long long px = (long long)n * h * w, nb = (px + 255) / 256;
+  UM_REQUIRE(um::written_disjoint({{offsets, 8 * (nb + 1)}, {depth, 4 * px}}, 1),
+             "um_depth_points_count: offsets must not overlap depth");
+  return um::depth_points_count_launch(depth, px, reinterpret_cast<long long*>(offsets), (cudaStream_t)stream);
+}
+
+int um_depth_points(const float* depth, const uint8_t* frames, int32_t n, int32_t h, int32_t w, float fx, float fy,
+                    float cx, float cy, const float* c2w, const int64_t* offsets, int64_t n_points, float* points,
+                    uint8_t* colors, void* stream) {
+  UM_REQUIRE(depth && frames && c2w && offsets, "um_depth_points: no pointer may be NULL");
+  UM_REQUIRE(n_points == 0 || (points && colors), "um_depth_points: points and colors must not be NULL");
+  UM_REQUIRE(depth_maps(n, h, w),
+             "um_depth_points: bad depths (%d x %d x %d; 1 .. 65535 maps of 1 .. 2^31 - 1 pixels, 2^39 in all)", n, h, w);
+  const long long px = (long long)n * h * w, nb = (px + 255) / 256;
+  UM_REQUIRE(n_points >= 0 && n_points <= px && n_points <= 0x7fffffffLL,
+             "um_depth_points: bad point count %lld (0 .. min(pixels, 2^31 - 1))", (long long)n_points);
+  UM_REQUIRE(icp_intrinsics(fx, fy, cx, cy), "um_depth_points: fx and fy must be finite and nonzero, cx and cy finite");
+  UM_REQUIRE(um::aligned(depth, 4) && um::aligned(c2w, 4) && um::aligned(offsets, 8) && um::aligned(points, 4),
+             "um_depth_points: depth, c2w and points 4-byte, offsets 8-byte aligned");
+  UM_REQUIRE(um::written_disjoint({{points, 12 * n_points}, {colors, 3 * n_points}, {depth, 4 * px}, {frames, 3 * px},
+                                   {c2w, 48LL * n}, {offsets, 8 * (nb + 1)}},
+                                  2),
+             "um_depth_points: points and colors must not overlap each other or the inputs");
+  if (n_points == 0) return UM_OK;
+  return um::depth_points_launch(depth, frames, n, h, w, fx, fy, cx, cy, c2w, reinterpret_cast<const long long*>(offsets),
+                                 points, colors, (cudaStream_t)stream);
 }
 
 }  // extern "C"

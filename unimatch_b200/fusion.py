@@ -7,9 +7,10 @@ launches), a binary PLY writer and reader for the points and meshes (`write_ply`
 neighbours and voxel down-sampling of point clouds (`nearest_neighbors`, `voxel_down_sample`, the um_cloud_* launches)
 that `evaluation.reconstruction_metrics` scores reconstructions with, the rasterisation of triangle meshes from any camera
 into depth, face and colour images (`render_mesh`, the um_mesh_* launches) and the visibility of points in depth maps
-(`visible_points`, one `um_visible_points` launch), which culls both sets to what the cameras saw before scoring.  The
-kernels' arithmetic
-is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
+(`visible_points`, one `um_visible_points` launch), which culls both sets to what the cameras saw before scoring, and the
+multi-view geometric consistency filter of depth maps (`filter_depths` over a `sequence_sources` table, one
+`um_depth_consistency` launch) with the export of valid depths as coloured world points (`depth_points`).  The kernels'
+arithmetic is stated in include/unimatch_sm100.h; `DepthFusionRunner` (inference.py) fuses the depths of `DepthSequenceRunner` inside
 each step's CUDA graph."""
 import math
 
@@ -734,3 +735,128 @@ def visible_points(points, depths, intrinsics, poses, tolerance=0.05):
             return torch.zeros((p.shape[0],), dtype=torch.bool, device=dev)
         w2c = torch.from_numpy(_world_to_camera(ps)).to(dev)
         return _OPS.visible_points(p, depths.contiguous(), w2c, fx, fy, cx, cy, _f32(tolerance))
+
+
+MAX_CONSISTENCY_SOURCES = 255               # views is uint8
+
+
+def sequence_sources(n, before, after):
+    """The sources table of a clip of n frames for `filter_depths`: host int32 [n, before + after], row t listing frames
+    t - 1, ..., t - before, then t + 1, ..., t + after, with -1 (no source) beyond the ends of the clip."""
+    for v, nm in ((n, "n"), (before, "before"), (after, "after")):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0:
+            raise ValueError("sequence_sources: %s must be a non-negative int" % nm)
+    t = np.arange(n)[:, None]
+    offsets = np.array([-k for k in range(1, before + 1)] + list(range(1, after + 1)), np.int64)
+    src = t + offsets[None, :]
+    return np.where((src >= 0) & (src < n), src, -1).astype(np.int32).reshape(n, before + after)
+
+
+def _positive_f32(v, name, what):
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+        raise ValueError("%s: %s must be positive and finite" % (name, what))
+    with np.errstate(over="ignore"):
+        f = _f32(v)
+    if not (math.isfinite(f) and f > 0):
+        raise ValueError("%s: %s must be positive and finite in float32" % (name, what))
+    return f
+
+
+def _consistency_args(n, sources, max_pixel, max_relative, min_views, name):
+    """(sources int32 [n, S], max_pixel, max_relative, min_views) checked: S 1 .. 255, entries in [-1, n) and never the
+    row's own frame, thresholds positive and finite in float32, min_views an int in [1, S]"""
+    src = np.asarray(sources)
+    if src.ndim != 2 or src.shape[0] != n or src.dtype.kind not in "iu":
+        raise ValueError("%s: sources must be an integer table [N, S] with one row per depth map" % name)
+    s = src.shape[1]
+    if not 1 <= s <= MAX_CONSISTENCY_SOURCES:
+        raise ValueError("%s: %d sources per frame; 1 .. 255 (the counts are uint8)" % (name, s))
+    if src.size and (src.min() < -1 or src.max() >= n):
+        raise ValueError("%s: source indices must lie in [-1, %d)" % (name, n))
+    if (src == np.arange(n)[:, None]).any():
+        raise ValueError("%s: a frame cannot be its own source" % name)
+    if isinstance(min_views, bool) or not isinstance(min_views, (int, np.integer)) or not 1 <= min_views <= s:
+        raise ValueError("%s: min_views must be an int in [1, %d]" % (name, s))
+    return (src.astype(np.int32), _positive_f32(max_pixel, name, "max_pixel"),
+            _positive_f32(max_relative, name, "max_relative"), int(min_views))
+
+
+def _depth_stack(depths, name):
+    if not (torch.is_tensor(depths) and depths.is_cuda and depths.dtype == torch.float32 and depths.dim() == 3):
+        raise ValueError("%s: depths must be a device float32 tensor [N,H,W]" % name)
+    n, h, w = depths.shape
+    if h * w > MAX_VOXELS:
+        raise ValueError("%s: at most 2^31 - 1 pixels per depth map" % name)
+    if n > MAX_MESH_VIEWS:
+        raise ValueError("%s: at most 65535 depth maps per call" % name)
+    return n
+
+
+@torch.no_grad()
+def filter_depths(depths, intrinsics, poses, sources, max_pixel=1.0, max_relative=0.01, min_views=2):
+    """Multi-view geometric consistency of N depth maps (MVSNet's check), on the device: device depths [N,H,W] (metric
+    z-depth; zero, negative and non-finite depths are invalid), intrinsics [3,3] at (H, W), host camera-to-world poses
+    [N,4,4] (as `fuse_depths` takes them) and a host sources table [N,S] (e.g. `sequence_sources`; -1 is no source).
+    Every frame is a reference: each valid pixel is reprojected into each of its sources at its depth, the source depth
+    is sampled there bilinearly (all four taps valid, inside the frame), and that point is reprojected back; the source
+    is consistent when the pixel lands within `max_pixel` pixels of where it started and within `max_relative` of its
+    depth.  The arithmetic is stated in include/unimatch_sm100.h (um_depth_consistency).  Returns on the device
+    {'depth': fp32 [N,H,W], the depth where at least `min_views` sources are consistent and 0 (no estimate, which
+    `fuse_depths` skips) elsewhere, 'views': uint8 [N,H,W] the number of consistent sources}.  One upload and one
+    launch; no atomics, the same result from run to run.  A source equal to its own frame, indices outside [-1, N),
+    more than 255 sources, bad cameras, poses and thresholds are refused with ValueError."""
+    name = "filter_depths"
+    n = _depth_stack(depths, name)
+    _, h, w = depths.shape
+    K = _intrinsics33(intrinsics, name)
+    fx, fy, cx, cy = _camera(K, name)
+    ps = _views(poses, name)
+    if len(ps) != n:
+        raise ValueError("%s: %d depth maps need %d poses, got %d" % (name, n, n, len(ps)))
+    src, max_pixel, max_relative, min_views = _consistency_args(n, sources, max_pixel, max_relative, min_views, name)
+    dev = depths.device
+    if n == 0:
+        return {"depth": depths.new_zeros((0, h, w)), "views": torch.zeros((0, h, w), dtype=torch.uint8, device=dev)}
+    packed = np.concatenate([_camera_to_world(ps).view(np.uint8).ravel(), _world_to_camera(ps).view(np.uint8).ravel(),
+                             np.arange(n, dtype=np.int32).view(np.uint8), src.view(np.uint8).ravel()])
+    with torch.cuda.device(dev):
+        buf = torch.from_numpy(packed).to(dev)                              # the one upload
+        rows = buf[:96 * n].view(torch.float32).view(2, n, 3, 4)
+        refs = buf[96 * n:100 * n].view(torch.int32)
+        table = buf[100 * n:].view(torch.int32).view(n, src.shape[1])
+        views, depth = _OPS.depth_consistency(depths.contiguous(), rows[0], rows[1], refs, table, fx, fy, cx, cy,
+                                              max_pixel, max_relative, min_views)
+    return {"depth": depth, "views": views}
+
+
+@torch.no_grad()
+def depth_points(depths, frames, intrinsics, poses):
+    """The valid depths of N frames as a coloured world point cloud, on the device: device depths [N,H,W] (zero, negative
+    and non-finite depths are skipped, so `filter_depths`' output gives the kept pixels), device uint8 frames [N,H,W,3],
+    intrinsics [3,3] at (H, W) and host camera-to-world poses [N,4,4].  Each pixel is back-projected along the ray through
+    its centre, exactly as `filter_depths` does.  Returns (points fp32 [P,3], colors uint8 [P,3]), ordered by frame, then
+    row-major pixel: the form `write_ply` and `reconstruction_metrics` take.  A count pass, an ordered scan and a write
+    pass, with one host read of P; more than 2^31 - 1 points is refused with ValueError before the outputs are
+    allocated."""
+    name = "depth_points"
+    n = _depth_stack(depths, name)
+    _, h, w = depths.shape
+    if not (torch.is_tensor(frames) and frames.is_cuda and frames.dtype == torch.uint8
+            and tuple(frames.shape) == tuple(depths.shape) + (3,) and frames.device == depths.device):
+        raise ValueError("%s: frames must be device uint8 [N,H,W,3] at the depths' size, on their device" % name)
+    K = _intrinsics33(intrinsics, name)
+    fx, fy, cx, cy = _camera(K, name)
+    ps = _views(poses, name)
+    if len(ps) != n:
+        raise ValueError("%s: %d depth maps need %d poses, got %d" % (name, n, n, len(ps)))
+    dev = depths.device
+    with torch.cuda.device(dev):
+        if n == 0:
+            return depths.new_zeros((0, 3)), torch.zeros((0, 3), dtype=torch.uint8, device=dev)
+        d = depths.contiguous()
+        c2w = torch.from_numpy(_camera_to_world(ps)).to(dev)
+        offsets = _OPS.depth_points_count(d)
+        total = int(offsets[-1].item())
+        if total > MAX_CLOUD_POINTS:
+            raise ValueError("%s: %d valid depths is more than 2^31 - 1 points (fewer frames per call)" % (name, total))
+        return _OPS.depth_points(d, frames.contiguous(), c2w, fx, fy, cx, cy, offsets, total)

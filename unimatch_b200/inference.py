@@ -1828,12 +1828,32 @@ class DepthFusionRunner(DepthSequenceRunner):
     is not tracked; a tracked frame then sets C = T_t P_t^-1.  C persists across `run()` calls with the volume, as it
     relates the given poses' frame to the volume's: reset both to start a new scene.  Each result gains 'pose' (float32
     [4,4], the camera-to-world pose frame t was fused at) and 'tracked' (bool), which are all that is downloaded with
-    `return_depth=False` and no pictures."""
+    `return_depth=False` and no pictures.
+
+    With `consistency_views=k > 0` each frame t is checked against the previous k frames t before it is tracked and
+    fused: `fusion.filter_depths` with `max_pixel=1.0`, `max_relative=0.01` and `min_views=consistency_min_views` on the
+    network's depths, at the given poses (those the depths were computed with).  The check is causal, so streaming needs
+    no delay: the runner keeps a device ring of the raw depths of the last k frames t (all zeros when empty, so an empty
+    slot is never a consistent source) and the host keeps their given poses; each step stages the rows of the ring's
+    frames and its own, and one `um_depth_consistency` launch on the (k + batch) stack filters its frames inside the
+    step's graph.  The filtered depth is what is fused (and tracked), so the volume equals `fuse_depths(volume,
+    filter_depths(D, K, poses, sequence_sources(n, k, 0), min_views=m)['depth'], frames, K, poses)` on the runner's own
+    depths D.  The ring persists across `run()` calls with the volume (and `pose_correction`); `reset_scene()` empties
+    all three.  'depth' stays the network's depth, and each result gains 'views' (uint8 [H,W], the number of consistent
+    earlier frames), which is downloaded even with `return_depth=False`.  The first `consistency_min_views` frames of a
+    scene have fewer earlier frames than the count requires, so they are not fused.  `consistency_views=0` is the runner
+    without the check: no ring and no extra launch."""
 
     def __init__(self, model, frame_size, batch, device, intrinsics, volume, padding_factor=16, inference_size=None,
                  min_depth=0.5, max_depth=10.0, num_depth_candidates=64, depth_from_argmax=False, pred_bidir_depth=False,
-                 use_graph=True, visualize=False, return_depth=True, track=False, **model_kwargs):
-        from .fusion import TSDFVolume, _ICP
+                 use_graph=True, visualize=False, return_depth=True, track=False, consistency_views=0,
+                 consistency_min_views=2, **model_kwargs):
+        from .fusion import MAX_CONSISTENCY_SOURCES, TSDFVolume, _ICP
+        k, m = consistency_views, consistency_min_views
+        if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k <= MAX_CONSISTENCY_SOURCES:
+            raise ValueError("DepthFusionRunner: consistency_views must be an int in [0, 255]")
+        if k and (isinstance(m, bool) or not isinstance(m, int) or not 1 <= m <= k):
+            raise ValueError("DepthFusionRunner: consistency_min_views must be an int in [1, consistency_views]")
         if pred_bidir_depth:
             raise ValueError("DepthFusionRunner: pred_bidir_depth is refused: the backward depth of frame t+1 would fuse "
                              "frame t+1 twice")
@@ -1862,17 +1882,55 @@ class DepthFusionRunner(DepthSequenceRunner):
             self.given_dev = [torch.zeros((self.batch, 4, 4), dtype=torch.float64, device=self.dev) for _ in range(2)]
             self.real_pin = [torch.zeros((self.batch,), dtype=torch.int32).pin_memory() for _ in range(2)]
             self.real_dev = [torch.zeros((self.batch,), dtype=torch.int32, device=self.dev) for _ in range(2)]
+        self.consistency_views, self.consistency_min_views = k, m
+        if k:
+            b = self.batch
+            self.ring = torch.zeros((k, self.h, self.w), device=self.dev)
+            self.ring_poses = []                           # the given poses of the ring's frames, oldest first
+            # stack rows: the ring's k frames, oldest first, then the step's frames t; step row i is checked against
+            # stack rows k + i - 1, ..., i (the k frames before it)
+            self.cons_refs = torch.arange(k, k + b, dtype=torch.int32, device=self.dev)
+            self.cons_sources = (torch.arange(b)[:, None] + k - torch.arange(1, k + 1)[None, :]).to(torch.int32).to(self.dev)
+            self.rows_pin = [torch.empty((2, k + b, 3, 4)).pin_memory() for _ in range(2)]       # c2w, then w2c
+            self.rows_dev = [torch.eye(4, device=self.dev)[:3].repeat(2, k + b, 1, 1) for _ in range(2)]
+            self.ring_idx_pin = [torch.empty((k,), dtype=torch.int64).pin_memory() for _ in range(2)]
+            self.ring_idx_dev = [torch.arange(k, device=self.dev) for _ in range(2)]    # the stack rows the ring keeps
+
+    def reset_scene(self):
+        """Start a new scene: empty the volume, the consistency ring and `pose_correction`"""
+        self.volume.reset()
+        if self.track:
+            self.pose_correction.copy_(torch.eye(4, dtype=torch.float64, device=self.dev))
+        if self.consistency_views:
+            self.ring.zero_()
+            self.ring_poses = []
 
     def _match(self, slot, first, second):
         out = _depth_outputs(self._depth(slot, first, second), self.ori, self.size, False)
         frames = torch.cat((self.carry_frame, self.dev_in[slot][:-1]), dim=0)        # frame t of every pair
-        poses = self._track_and_fuse(slot, out["depth"].contiguous(), frames) if self.track else {}
+        depth, extra = out["depth"].contiguous(), {}
+        if self.consistency_views:
+            depth, extra["views"] = self._filter(slot, depth)
+        poses = self._track_and_fuse(slot, depth, frames) if self.track else {}
         if not self.track:
-            self.volume._integrate(out["depth"].contiguous(), frames, self.w2c_dev[slot], self.nvalid_dev[slot], self.K)
+            self.volume._integrate(depth, frames, self.w2c_dev[slot], self.nvalid_dev[slot], self.K)
         self.carry_frame.copy_(self.dev_in[slot][-1:])
+        extra.update(poses)
         if self.visualize:
-            return dict(_colour_outputs(out, "depth", depth_to_image, self.return_depth), **poses)
-        return dict(out, **poses) if self.return_depth else poses
+            return dict(_colour_outputs(out, "depth", depth_to_image, self.return_depth), **extra)
+        return dict(out, **extra) if self.return_depth else extra
+
+    def _filter(self, slot, depth):
+        """One um_depth_consistency launch on the ring and the step's depths, then the ring keeps the last k real rows of
+        that stack; returns the filtered depths [batch,H,W] and the counts"""
+        stack = torch.cat((self.ring, depth), dim=0)
+        rows = self.rows_dev[slot]
+        K = self.K
+        views, filtered = _OPS.depth_consistency(stack, rows[0], rows[1], self.cons_refs, self.cons_sources,
+                                                 float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]), 1.0,
+                                                 0.01, self.consistency_min_views)
+        self.ring.copy_(stack.index_select(0, self.ring_idx_dev[slot]))
+        return filtered, views
 
     def _track_and_fuse(self, slot, depth, frames):
         """Frames t in order: track against the volume from C P_t, fuse at the result, update C; padding pairs (real
@@ -1900,6 +1958,8 @@ class DepthFusionRunner(DepthSequenceRunner):
         self.nvalid_dev[slot].zero_()
         if self.track:
             self.real_dev[slot].zero_()
+        if self.consistency_views:                       # no real pair: the ring keeps its rows
+            self.ring_idx_dev[slot].copy_(torch.arange(self.consistency_views, device=self.dev))
 
     def _stage_step_poses(self, slot, poses, n_real):
         """the relative poses, then the world-to-camera rows of the pairs' frames t and the number of real pairs (with
@@ -1914,6 +1974,16 @@ class DepthFusionRunner(DepthSequenceRunner):
             self.real_pin[slot].copy_(torch.arange(self.batch) < n_real)
             self.given_dev[slot].copy_(self.given_pin[slot], non_blocking=True)
             self.real_dev[slot].copy_(self.real_pin[slot], non_blocking=True)
+        k = self.consistency_views
+        if k:
+            eye = np.eye(4, dtype=np.float32)
+            stack = [eye] * (k - len(self.ring_poses)) + self.ring_poses + list(poses[:-1])
+            self.rows_pin[slot][0].copy_(torch.from_numpy(_camera_to_world(stack)))
+            self.rows_pin[slot][1].copy_(torch.from_numpy(_world_to_camera(stack)))
+            self.ring_idx_pin[slot].copy_(torch.arange(n_real, n_real + k))
+            self.rows_dev[slot].copy_(self.rows_pin[slot], non_blocking=True)
+            self.ring_idx_dev[slot].copy_(self.ring_idx_pin[slot], non_blocking=True)
+            self.ring_poses = (self.ring_poses + list(poses[:n_real]))[-k:]
 
 
 def _depth_step_layout(sizes, batch, pred_bidir_depth):

@@ -144,6 +144,9 @@ _SIGNATURES = {
                              _P]),
     "um_visible_points": (_RC, [_P, _L, _P, _I, _I, _I, _P, _F, _F, _F, _F, _F, _P, _P]),
     "um_depth_metrics": (_RC, [_P, _P, _I, _I, _I, _F, _P, _P, _P]),
+    "um_depth_consistency": (_RC, [_P, _I, _I, _I, _F, _F, _F, _F, _P, _P, _P, _I, _P, _I, _F, _F, _I, _P, _P, _P]),
+    "um_depth_points_count": (_RC, [_P, _I, _I, _I, _P, _P]),
+    "um_depth_points": (_RC, [_P, _P, _I, _I, _I, _F, _F, _F, _F, _P, _P, _L, _P, _P, _P]),
     "um_propagate_local": (_RC, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _L, _L, _P]),
     "um_depth_corr_softmax": (_RC, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "um_add_position": (_RC, [_P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -1097,6 +1100,78 @@ def _depth_metrics(pred, gt, max_depth):
 
 
 depth_metrics = _define("depth_metrics(Tensor pred, Tensor gt, float max_depth) -> Tensor", _depth_metrics)
+
+
+# ---- multi-view consistency of depth maps and their points (include/unimatch_sm100.h, um_depth_*) -----------------
+def _rows34(t, n, name):
+    _f32c(t, name)
+    if tuple(t.shape) != (n, 3, 4):
+        raise RuntimeError("%s: expected rows [%d, 3, 4]" % (name, n))
+
+
+def _depth_consistency(depth, c2w, w2c, refs, sources, fx, fy, cx, cy, max_pixel, max_relative, min_views):
+    """views uint8 [R, h, w] (consistent sources per reference pixel) and the filtered depths fp32 [R, h, w] of depths
+    [n, h, w] with their rows c2w / w2c [n, 3, 4], int32 refs [R] and sources [R, S] (um_depth_consistency)"""
+    _f32c(depth, "depth_consistency: depth")
+    if depth.dim() != 3:
+        raise RuntimeError("depth_consistency: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    _rows34(c2w, n, "depth_consistency: c2w")
+    _rows34(w2c, n, "depth_consistency: w2c")
+    if refs.dtype != torch.int32 or refs.dim() != 1 or not refs.is_contiguous() or sources.dtype != torch.int32 \
+            or sources.dim() != 2 or sources.shape[0] != refs.shape[0] or not sources.is_contiguous():
+        raise RuntimeError("depth_consistency: refs must be contiguous int32 [R] and sources int32 [R, S]")
+    _device_like("depth_consistency", depth, c2w, w2c, refs, sources)
+    r, s = sources.shape
+    views = torch.empty((r, h, w), device=depth.device, dtype=torch.uint8)
+    out = torch.empty((r, h, w), device=depth.device, dtype=torch.float32)
+    _check(LIB.um_depth_consistency(_p(depth), n, h, w, fx, fy, cx, cy, _p(c2w), _p(w2c), _p(refs), r, _p(sources), s,
+                                    max_pixel, max_relative, min_views, _p(views), _p(out), _stream()),
+           "um_depth_consistency")
+    return views, out
+
+
+depth_consistency = _define("depth_consistency(Tensor depth, Tensor c2w, Tensor w2c, Tensor refs, Tensor sources, "
+                            "float fx, float fy, float cx, float cy, float max_pixel, float max_relative, int min_views) "
+                            "-> (Tensor, Tensor)", _depth_consistency)
+
+
+def _depth_points_count(depth):
+    """The point offsets of depths [n, h, w], device int64 [ceil(n h w / 256) + 1]: per block of 256 pixels its first
+    point, then the number of points"""
+    _f32c(depth, "depth_points_count: depth")
+    if depth.dim() != 3:
+        raise RuntimeError("depth_points_count: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    offsets = torch.empty((-(-(n * h * w) // 256) + 1,), device=depth.device, dtype=torch.int64)
+    _check(LIB.um_depth_points_count(_p(depth), n, h, w, _p(offsets), _stream()), "um_depth_points_count")
+    return offsets
+
+
+depth_points_count = _define("depth_points_count(Tensor depth) -> Tensor", _depth_points_count)
+
+
+def _depth_points(depth, frames, c2w, fx, fy, cx, cy, offsets, n_points):
+    """The n_points world points fp32 [P, 3] and colours uint8 [P, 3] of the valid depths (um_depth_points)"""
+    _f32c(depth, "depth_points: depth")
+    if depth.dim() != 3:
+        raise RuntimeError("depth_points: expected depths [n, h, w]")
+    n, h, w = depth.shape
+    _rows34(c2w, n, "depth_points: c2w")
+    if frames.dtype != torch.uint8 or tuple(frames.shape) != (n, h, w, 3) or not frames.is_contiguous():
+        raise RuntimeError("depth_points: frames must be contiguous uint8 [n, h, w, 3]")
+    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-(n * h * w) // 256) + 1,):
+        raise RuntimeError("depth_points: offsets must be depth_points_count's int64 table")
+    _device_like("depth_points", depth, frames, c2w, offsets)
+    points = torch.empty((n_points, 3), device=depth.device, dtype=torch.float32)
+    colors = torch.empty((n_points, 3), device=depth.device, dtype=torch.uint8)
+    _check(LIB.um_depth_points(_p(depth), _p(frames), n, h, w, fx, fy, cx, cy, _p(c2w), _p(offsets), n_points,
+                               _p(points), _p(colors), _stream()), "um_depth_points")
+    return points, colors
+
+
+depth_points = _define("depth_points(Tensor depth, Tensor frames, Tensor c2w, float fx, float fy, float cx, float cy, "
+                       "Tensor offsets, int n_points) -> (Tensor, Tensor)", _depth_points)
 
 
 def _propagate_local(q, k, flow, h, w, radius):
