@@ -434,16 +434,21 @@ int um_tsdf_integrate(float* tsdf, float* weight, float* color, int32_t X, int32
                       float voxel_size, float trunc, const float* depth, const uint8_t* frames, const float* w2c, int32_t n,
                       int32_t h, int32_t w, float fx, float fy, float cx, float cy, const int32_t* n_valid, void* stream);
 
+/* Offsets tables.  A count op (um_tsdf_surface_count, um_tsdf_mesh_count, um_cloud_down_sample_count, um_mesh_bin_count,
+ * um_depth_points_count) takes its items in blocks of UM_TSDF_THREADS in item order and writes offsets [nb + 1] (DEVICE
+ * int64, nb the number of blocks): offsets[b] the first output of block b, offsets[nb] the total, which the caller reads
+ * to allocate the outputs.  It launches a count pass, then one CTA's ordered exclusive int64 scan of the block counts in
+ * place.  Its fill op writes each item's outputs from its block's offset plus the outputs of the block's earlier items.
+ * No atomics: the output is the same from run to run. */
+
 /* Surface extraction: the zero-crossing vertices of marching cubes, as coloured points.  Each voxel owns its +x, +y and +z
  * edges that lie inside the grid; the edge from voxel 0 to voxel 1 emits a point iff weight0 > 0, weight1 > 0 and
  * (F0 < 0) != (F1 < 0).  With s = F0 / (F0 - F1) the point is voxel 0's centre with fma(s, voxel_size, p0) on the edge's
  * axis, and its colour per channel is __float2int_rn(fma(s, C1 - C0, C0)) clamped to 0..255.  Points are ordered by voxel
  * linear index, then edge axis x, y, z.
- * um_tsdf_surface_count writes offsets [nb + 1] (DEVICE int64, nb = ceil(N / UM_TSDF_THREADS)): offsets[b] the first
- * point of block b (voxels b * UM_TSDF_THREADS ...), offsets[nb] the total P, which the caller reads to allocate
- * points [P, 3] fp32 and colors [P, 3] uint8; um_tsdf_surface_points (n_points = P) then writes them, and with P = 0
- * launches nothing.  A count pass, one ordered scan of
- * the block counts and a write pass: no atomics, the output is the same from run to run. */
+ * um_tsdf_surface_count writes the offsets table (see Offsets tables) of the points over the N voxels,
+ * nb = ceil(N / UM_TSDF_THREADS), the total P; the caller allocates points [P, 3] fp32 and colors [P, 3] uint8, and
+ * um_tsdf_surface_points (n_points = P) writes them, and with P = 0 launches nothing. */
 int um_tsdf_surface_count(const float* tsdf, const float* weight, int32_t X, int32_t Y, int32_t Z, int64_t* offsets,
                           void* stream);
 int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* color, int32_t X, int32_t Y, int32_t Z,
@@ -471,8 +476,8 @@ int um_tsdf_surface_points(const float* tsdf, const float* weight, const float* 
  *   g = (F(v+) - F(v-)) * 0.5f with both,  F(v+) - F(v) with only v+,  F(v) - F(v-) with only v-,  0 with neither.
  * The vertex on the edge from voxel 0 to voxel 1 (s as for its point): n = fma(s, g1 - g0, g0) per component,
  * l = sqrt(fma(n.z, n.z, fma(n.y, n.y, n.x * n.x))) (correctly rounded), normal = n / l, or (0, 0, 0) when l == 0.
- * um_tsdf_mesh_count writes face_offsets [nb + 1] (DEVICE int64, as um_tsdf_surface_count's offsets): offsets[b] the
- * first triangle of block b's cubes, offsets[nb] the total T.  um_tsdf_mesh takes both offset tables and both totals
+ * um_tsdf_mesh_count writes face_offsets, the offsets table (see Offsets tables) of the triangles over the N cubes,
+ * nb as um_tsdf_surface_count's, the total T.  um_tsdf_mesh takes both offset tables and both totals
  * (n_points = P, n_faces = T, each at most 2^31 - 1) and writes points [P, 3] fp32, colors [P, 3] uint8 (as
  * um_tsdf_surface_points), normals [P, 3] fp32 and faces [T, 3] int32, through first_vertex, caller-provided DEVICE scratch
  * of N int32 (each voxel's first point).  Two launches: the vertex pass, then the face pass (none with T = 0); with P = 0
@@ -605,8 +610,8 @@ int um_icp_accept(const double* partials, int32_t nb, int32_t n, const int32_t* 
  *   cell; keys outside the table are not entered), and sorted[i] = (x, y, z, bits of (int32) order[i]) fp32 [n, 4].
  * Down-sampling (Open3D's VoxelDownSample): with v the voxel size, o = min_bound - v / 2 in fp64 (min_bound the set's
  *   per-axis minimum) and g_a = floor((max_bound_a - o_a) / v) + 1 computed as t is, every point lies in the grid, so the
- *   clamp never applies.  um_cloud_down_sample_count: per block of 256 sorted positions the number of runs of equal keys
- *   that start in it, then one CTA's ordered exclusive scan in place, the total M at offsets[nb], nb = ceil(n / 256).
+ *   clamp never applies.  um_cloud_down_sample_count writes the offsets table (see Offsets tables) of the
+ *   runs of equal keys over the n sorted positions a run can start at, nb = ceil(n / 256), the total M.
  *   um_cloud_down_sample: run m (in key order) writes out[m] = (float)(s / count) per axis, s the fp64 sum from 0.0 of
  *   (double)p over the run in sorted order, which a stable sort makes the input order.
  * Nearest neighbour (um_cloud_nearest, one query q per thread) over the table of an indexed set P whose grid box holds
@@ -683,8 +688,8 @@ int um_cloud_stats(const double* partial_sum, const int64_t* partial_count, int6
  *   (tests/test_raster_cpu.py shows that dropping it changes no output there), but it is not proved for arbitrarily
  *   degenerate geometry (slivers, vertices at extreme magnitudes, faces grazing the near plane).
  * Launches (16 x 16 pixel tiles, tiles = ceil(h/16) ceil(w/16) per view):
- *   um_mesh_bin_count: per (view, block of 256 faces) the number of tiles the faces' rectangles touch, then one CTA's
- *   ordered exclusive int64 scan: offsets [n ceil(T/256) + 1] (DEVICE int64), view-major, the total E last.
+ *   um_mesh_bin_count writes the offsets table (see Offsets tables) of the tiles the faces' rectangles
+ *   touch, over the (view, face) pairs in blocks of 256 faces of one view, view-major: nb = n ceil(T/256), the total E.
  *   um_mesh_bin (E entries): for each (view, face) in that order, per touched tile row by row, keys[e] = view tiles +
  *   tile (int64) and values[e] = face << 16 | (x0 | x1 << 4 | y0 << 8 | y1 << 12), the rectangle within the tile.
  *   The caller sorts keys stably with their positions (order), so each tile's entries stay in ascending face order.
@@ -750,10 +755,9 @@ int um_depth_metrics(const float* pred, const float* gt, int32_t n, int32_t h, i
  * No atomics, no host synchronisation (graph-capturable); the same output from run to run.
  * Points (um_depth_points_count, um_depth_points): every valid depth d = depth[t, y, x] gives the world point
  * c2w[t] B(x, y, d) and the colour frames[t, y, x] (uint8 [n, h, w, 3]), ordered by frame, then row-major pixel.
- * um_depth_points_count writes offsets [nb + 1] (DEVICE int64, nb = ceil(n h w / 256)): offsets[b] the first point of
- * pixels b * 256 ... (frame-major), offsets[nb] the total P, which the caller reads to allocate points fp32 [P, 3] and
- * colors uint8 [P, 3] (P <= 2^31 - 1); um_depth_points (n_points = P) writes them, and with P = 0 launches nothing.  A count
- * pass, one ordered scan of the block counts and a write pass: no atomics.  n 1 .. 65535, h w <= 2^31 - 1, n h w <= 2^39.
+ * um_depth_points_count writes the offsets table (see Offsets tables) of the points over the n h w pixels
+ * (frame-major), nb = ceil(n h w / 256), the total P; the caller allocates points fp32 [P, 3] and colors uint8 [P, 3]
+ * (P <= 2^31 - 1), and um_depth_points (n_points = P) writes them, and with P = 0 launches nothing.  n 1 .. 65535, h w <= 2^31 - 1, n h w <= 2^39.
  * Every pointer is DEVICE memory; no output overlaps an input or another output. */
 int um_depth_consistency(const float* depth, int32_t n, int32_t h, int32_t w, float fx, float fy, float cx, float cy,
                          const float* c2w, const float* w2c, const int32_t* refs, int32_t r, const int32_t* sources,

@@ -44,7 +44,7 @@ from tools.common import card, timed  # noqa: E402
 from tools.mesh_bench import _event_ms, _kernel_ms, build_volume  # noqa: E402
 from tools.render_bench import cameras  # noqa: E402
 
-NEW_KERNELS = ("mesh_bin_count_kernel", "mesh_scan_kernel", "mesh_bin_kernel", "mesh_ranges_kernel", "mesh_raster_kernel",
+NEW_KERNELS = ("mesh_bin_count_kernel", "offsets_scan_kernel", "mesh_bin_kernel", "mesh_ranges_kernel", "mesh_raster_kernel",
                "visible_points_kernel", "depth_metrics_kernel", "depth_metrics_sum_kernel")
 
 

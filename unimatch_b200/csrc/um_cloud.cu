@@ -5,11 +5,11 @@
 // tests/refops_recon.py.
 #include <limits.h>
 
-#include "um_common.cuh"
+#include "um_geometry.cuh"
 
 namespace {
 
-constexpr int CLOUD_THREADS = 256, CLOUD_WARPS = CLOUD_THREADS / 32;
+constexpr int CLOUD_THREADS = COMPACT_THREADS, CLOUD_WARPS = CLOUD_THREADS / 32;
 
 struct CloudGrid {
   double o[3], cell;
@@ -43,10 +43,7 @@ cloud_ranges_kernel(const long long* __restrict__ keys, const long long* __restr
   const long long i = (long long)blockIdx.x * CLOUD_THREADS + threadIdx.x;
   if (i >= n) return;
   const long long key = __ldg(keys + i), j = __ldg(order + i);
-  if (key >= 0 && key < n_cells) {
-    if (i == 0 || __ldg(keys + i - 1) != key) start[key] = (int)i;
-    if (i == n - 1 || __ldg(keys + i + 1) != key) end[key] = (int)(i + 1);
-  }
+  if (key >= 0 && key < n_cells) mark_run(keys, i, n, key, start, end);
   sorted[i] = make_float4(__ldg(p + 3 * j), __ldg(p + 3 * j + 1), __ldg(p + 3 * j + 2), __int_as_float((int)j));
 }
 
@@ -58,41 +55,9 @@ __device__ __forceinline__ bool run_head(const long long* __restrict__ keys, lon
 __global__ void __launch_bounds__(CLOUD_THREADS)
 cloud_heads_kernel(const long long* __restrict__ keys, long long n, long long* __restrict__ block_counts) {
   const long long i = (long long)blockIdx.x * CLOUD_THREADS + threadIdx.x;
-  const int c = __syncthreads_count(run_head(keys, i, n));
-  if (threadIdx.x == 0) block_counts[blockIdx.x] = c;
-}
-
-// Pass 2: one CTA turns the block counts into exclusive offsets in place, CLOUD_THREADS at a time, in order; the total
-// follows them at offsets[nb].
-__global__ void __launch_bounds__(CLOUD_THREADS) cloud_scan_kernel(long long* __restrict__ offsets, long long nb) {
-  __shared__ long long warp_sums[CLOUD_WARPS];
-  __shared__ long long carry;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (long long base = 0; base < nb; base += CLOUD_THREADS) {
-    const long long i = base + threadIdx.x;
-    const long long x = i < nb ? offsets[i] : 0;
-    long long incl = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) warp_sums[wid] = incl;
-    __syncthreads();
-    long long before = carry, all = 0;
-#pragma unroll
-    for (int q = 0; q < CLOUD_WARPS; ++q) {
-      before += q < wid ? warp_sums[q] : 0;
-      all += warp_sums[q];
-    }
-    if (i < nb) offsets[i] = before + incl - x;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += all;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[nb] = carry;
+  int all;
+  block_rank(run_head(keys, i, n), &all);
+  if (threadIdx.x == 0) block_counts[blockIdx.x] = all;
 }
 
 // Pass 3: the thread at the head of each run writes the run's mean, summed in fp64 in sorted (= input) order, to output
@@ -101,16 +66,12 @@ __global__ void __launch_bounds__(CLOUD_THREADS)
 cloud_down_sample_kernel(const long long* __restrict__ keys, const long long* __restrict__ order,
                          const float* __restrict__ p, long long n, const long long* __restrict__ offsets,
                          float* __restrict__ out) {
-  __shared__ int warp_heads[CLOUD_WARPS];
   const long long i = (long long)blockIdx.x * CLOUD_THREADS + threadIdx.x;
   const bool head = run_head(keys, i, n);
-  const unsigned b = __ballot_sync(0xffffffffu, head);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) warp_heads[wid] = __popc(b);
-  __syncthreads();
+  int all;
+  const int before = block_rank(head, &all);
   if (!head) return;
-  long long m = __ldg(offsets + blockIdx.x) + __popc(b & ((1u << lane) - 1u));
-  for (int q = 0; q < wid; ++q) m += warp_heads[q];
+  const long long m = __ldg(offsets + blockIdx.x) + before;
   const long long key = __ldg(keys + i);
   double s[3] = {0.0, 0.0, 0.0};
   long long c = 0;
@@ -222,9 +183,7 @@ cloud_nearest_kernel(const float* __restrict__ queries, long long nq, const floa
   __shared__ double warp_sum[CLOUD_WARPS];
   __shared__ int warp_count[CLOUD_WARPS];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  double v = i < nq ? (double)d : 0.0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = __dadd_rn(v, __shfl_down_sync(0xffffffffu, v, o));
+  const double v = warp_sum_ordered(i < nq ? (double)d : 0.0);
   const unsigned below = __ballot_sync(0xffffffffu, i < nq && d < threshold);
   if (lane == 0) warp_sum[wid] = v, warp_count[wid] = __popc(below);
   __syncthreads();
@@ -242,14 +201,11 @@ __global__ void __launch_bounds__(32)
 cloud_stats_kernel(const double* __restrict__ partial_sum, const long long* __restrict__ partial_count, long long nb,
                    double* __restrict__ out) {
   const int lane = threadIdx.x;
-  double s = 0.0;
+  const double s = partials_sum_ordered(partial_sum, nb, 1);
   long long c = 0;
-  for (long long b = lane; b < nb; b += 32) s = __dadd_rn(s, __ldg(partial_sum + b)), c += __ldg(partial_count + b);
+  for (long long b = lane; b < nb; b += 32) c += __ldg(partial_count + b);
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, o));
-    c += __shfl_down_sync(0xffffffffu, c, o);
-  }
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
   if (lane == 0) out[0] = s, out[1] = (double)c;
 }
 
@@ -274,12 +230,7 @@ int cloud_keys_launch(const float* points, long long n, const double* origin, do
 
 int cloud_ranges_launch(const long long* keys, const long long* order, const float* points, long long n, long long n_cells,
                         int* start, int* end, float* sorted, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(start, 0, 4 * n_cells, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(end, 0, 4 * n_cells, st);
-  if (e != cudaSuccess) {
-    set_error("um_cloud_ranges: %s", cudaGetErrorString(e));
-    return UM_ECUDA;
-  }
+  if (int rc = zero_runs(start, end, n_cells, "um_cloud_ranges", st)) return rc;
   cloud_ranges_kernel<<<cloud_blocks(n), CLOUD_THREADS, 0, st>>>(keys, order, points, n, n_cells, start, end,
                                                                  reinterpret_cast<float4*>(sorted));
   return check_launch("um_cloud_ranges");
@@ -289,8 +240,7 @@ int cloud_down_sample_count_launch(const long long* keys, long long n, long long
   const unsigned nb = cloud_blocks(n);
   cloud_heads_kernel<<<nb, CLOUD_THREADS, 0, st>>>(keys, n, offsets);
   if (int rc = check_launch("um_cloud_down_sample_count (heads)")) return rc;
-  cloud_scan_kernel<<<1, CLOUD_THREADS, 0, st>>>(offsets, (long long)nb);
-  return check_launch("um_cloud_down_sample_count (scan)");
+  return offsets_scan_launch(offsets, nb, "um_cloud_down_sample_count (scan)", st);
 }
 
 int cloud_down_sample_launch(const long long* keys, const long long* order, const float* points, long long n,

@@ -1,30 +1,11 @@
 // Multi-view geometric consistency of depth maps (um_depth_consistency) and the export of valid depths as coloured world
 // points (um_depth_points_count, um_depth_points).  Semantics and the order of operations: include/unimatch_sm100.h; the
 // numpy statement is tests/refops_consistency.py.
-#include "um_common.cuh"
+#include "um_geometry.cuh"
 
 namespace {
 
-constexpr int CONS_THREADS = 256, CONS_WARPS = CONS_THREADS / 32;
-
-struct Pinhole {
-  float fx, fy, cx, cy;
-};
-
-__device__ __forceinline__ bool valid_depth(float d) { return isfinite(d) && d > 0.f; }
-
-// rows m [3, 4] (row-major) applied to p, in um_tsdf_integrate's order
-__device__ __forceinline__ float3 apply_rows(const float* m, float3 p) {
-  return make_float3(__fmaf_rn(m[2], p.z, __fmaf_rn(m[1], p.y, __fmaf_rn(m[0], p.x, m[3]))),
-                     __fmaf_rn(m[6], p.z, __fmaf_rn(m[5], p.y, __fmaf_rn(m[4], p.x, m[7]))),
-                     __fmaf_rn(m[10], p.z, __fmaf_rn(m[9], p.y, __fmaf_rn(m[8], p.x, m[11]))));
-}
-
-// pixel coordinates (u, v) at camera z-depth d -> camera point ((u - cx) / fx * d, (v - cy) / fy * d, d)
-__device__ __forceinline__ float3 back_project(const Pinhole& k, float u, float v, float d) {
-  return make_float3(__fmul_rn(__fdiv_rn(__fsub_rn(u, k.cx), k.fx), d), __fmul_rn(__fdiv_rn(__fsub_rn(v, k.cy), k.fy), d),
-                     d);
-}
+constexpr int CONS_THREADS = COMPACT_THREADS;
 
 __device__ __forceinline__ void load_rows(float* dst, const float* __restrict__ rows, int i) {
 #pragma unroll
@@ -59,7 +40,8 @@ depth_consistency_kernel(const float* __restrict__ depth, int N, int H, int W, P
       load_rows(m, w2c, s);
       const float3 c = apply_rows(m, world);
       if (!(c.z > 0.f)) continue;
-      const float u = __fmaf_rn(k.fx, __fdiv_rn(c.x, c.z), k.cx), v = __fmaf_rn(k.fy, __fdiv_rn(c.y, c.z), k.cy);
+      const float2 uv = project(k, c);
+      const float u = uv.x, v = uv.y;
       if (!(u >= 0.f && u <= (float)(W - 1) && v >= 0.f && v <= (float)(H - 1))) continue;
       const float fx0 = floorf(u), fy0 = floorf(v);
       const int x0 = (int)fx0, y0 = (int)fy0, x1 = min(x0 + 1, W - 1), y1 = min(y0 + 1, H - 1);
@@ -73,9 +55,8 @@ depth_consistency_kernel(const float* __restrict__ depth, int N, int H, int W, P
       load_rows(m, c2w, s);
       const float3 back = apply_rows(w2c_r, apply_rows(m, back_project(k, u, v, ds)));
       if (!(back.z > 0.f)) continue;
-      const float u2 = __fmaf_rn(k.fx, __fdiv_rn(back.x, back.z), k.cx);
-      const float v2 = __fmaf_rn(k.fy, __fdiv_rn(back.y, back.z), k.cy);
-      const float dx = __fsub_rn(u2, xf), dy = __fsub_rn(v2, yf);
+      const float2 uv2 = project(k, back);
+      const float dx = __fsub_rn(uv2.x, xf), dy = __fsub_rn(uv2.y, yf);
       const float err = __fsqrt_rn(__fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
       const float rel = __fdiv_rn(fabsf(__fsub_rn(back.z, d)), d);
       if (err < max_pixel && rel < max_relative) ++count;
@@ -89,51 +70,10 @@ depth_consistency_kernel(const float* __restrict__ depth, int N, int H, int W, P
 // Pass 1: per block of 256 pixels (frame-major, then row-major), the number of valid depths.
 __global__ void __launch_bounds__(CONS_THREADS)
 depth_points_count_kernel(const float* __restrict__ depth, long long total, long long* __restrict__ block_counts) {
-  __shared__ int warp_counts[CONS_WARPS];
   const long long i = (long long)blockIdx.x * CONS_THREADS + threadIdx.x;
-  const bool ok = i < total && valid_depth(__ldg(depth + i));
-  const unsigned ballot = __ballot_sync(0xffffffffu, ok);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) warp_counts[wid] = __popc(ballot);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long s = 0;
-    for (int q = 0; q < CONS_WARPS; ++q) s += warp_counts[q];
-    block_counts[blockIdx.x] = s;
-  }
-}
-
-// Pass 2: one CTA turns the block counts into exclusive offsets in place, 256 at a time, in order; the total follows
-// them at offsets[nb].
-__global__ void __launch_bounds__(CONS_THREADS) depth_points_scan_kernel(long long* __restrict__ offsets, long long nb) {
-  __shared__ long long warp_sums[CONS_WARPS];
-  __shared__ long long carry;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (long long base = 0; base < nb; base += CONS_THREADS) {
-    const long long i = base + threadIdx.x;
-    const long long x = i < nb ? offsets[i] : 0;
-    long long incl = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) warp_sums[wid] = incl;
-    __syncthreads();
-    long long before = carry, all = 0;
-#pragma unroll
-    for (int q = 0; q < CONS_WARPS; ++q) {
-      before += q < wid ? warp_sums[q] : 0;
-      all += warp_sums[q];
-    }
-    if (i < nb) offsets[i] = before + incl - x;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += all;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[nb] = carry;
+  int all;
+  block_rank(i < total && valid_depth(__ldg(depth + i)), &all);
+  if (threadIdx.x == 0) block_counts[blockIdx.x] = all;
 }
 
 // Pass 3: each valid depth writes its world point and colour at offsets[block] + the valid depths before it in the block.
@@ -141,17 +81,13 @@ __global__ void __launch_bounds__(CONS_THREADS)
 depth_points_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ frames, int H, int W, Pinhole k,
                     const float* __restrict__ c2w, long long total, const long long* __restrict__ offsets,
                     float* __restrict__ points, uint8_t* __restrict__ colors) {
-  __shared__ int warp_counts[CONS_WARPS];
   const long long i = (long long)blockIdx.x * CONS_THREADS + threadIdx.x;
   const float d = i < total ? __ldg(depth + i) : 0.f;
   const bool ok = valid_depth(d);
-  const unsigned ballot = __ballot_sync(0xffffffffu, ok);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) warp_counts[wid] = __popc(ballot);
-  __syncthreads();
+  int all;
+  const int before = block_rank(ok, &all);
   if (!ok) return;
-  long long o = __ldg(offsets + blockIdx.x) + __popc(ballot & ((1u << lane) - 1u));
-  for (int q = 0; q < wid; ++q) o += warp_counts[q];
+  const long long o = __ldg(offsets + blockIdx.x) + before;
   const long long hw = (long long)H * W;
   const int t = (int)(i / hw);
   const long long pix = i - t * hw;
@@ -184,8 +120,7 @@ int depth_points_count_launch(const float* depth, long long total, long long* of
   const unsigned nb = pixel_blocks(total);
   depth_points_count_kernel<<<nb, CONS_THREADS, 0, st>>>(depth, total, offsets);
   if (int rc = check_launch("um_depth_points_count (count)")) return rc;
-  depth_points_scan_kernel<<<1, CONS_THREADS, 0, st>>>(offsets, (long long)nb);
-  return check_launch("um_depth_points_count (scan)");
+  return offsets_scan_launch(offsets, nb, "um_depth_points_count (scan)", st);
 }
 
 int depth_points_launch(const float* depth, const uint8_t* frames, int N, int H, int W, float fx, float fy, float cx,

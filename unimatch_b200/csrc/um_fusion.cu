@@ -3,13 +3,12 @@
 // and its ray-cast depth, colour and normal images (um_tsdf_raycast).
 // Semantics and the fp32 order of operations: include/unimatch_sm100.h; the float32 and float64 statements are
 // tests/refops_fusion.py, tests/refops_mesh.py and tests/refops_render.py.
-#include "um_common.cuh"
+#include "um_geometry.cuh"
 #include "um_mc_table.cuh"
 
 namespace {
 
-constexpr int FUSE_THREADS = UM_TSDF_THREADS;
-constexpr int FUSE_WARPS = FUSE_THREADS / 32;
+constexpr int FUSE_THREADS = COMPACT_THREADS;
 
 struct Volume {
   int X, Y, Z;
@@ -36,22 +35,20 @@ tsdf_integrate_kernel(float* __restrict__ tsdf, float* __restrict__ weight, floa
   const int xy = vol.X * vol.Y;
   const int k = (int)(i / xy), r = (int)(i - (long long)k * xy);
   const int j = r / vol.X, ii = r - j * vol.X;
-  const float px = centre(ii, vol.vs, vol.ox), py = centre(j, vol.vs, vol.oy), pz = centre(k, vol.vs, vol.oz);
+  const float3 p = make_float3(centre(ii, vol.vs, vol.ox), centre(j, vol.vs, vol.oy), centre(k, vol.vs, vol.oz));
+  const Pinhole cam = {fx, fy, cx, cy};
   const long long plane = (long long)h * w;
   bool loaded = false;
   float F = 0.f, Wt = 0.f, R = 0.f, G = 0.f, B = 0.f;
   for (int t = 0; t < nv; ++t) {
-    const float* m = w2c + 12 * t;
-    const float czz = __fmaf_rn(__ldg(m + 10), pz, __fmaf_rn(__ldg(m + 9), py, __fmaf_rn(__ldg(m + 8), px, __ldg(m + 11))));
+    const GlobalRows m = {w2c + 12 * t};
+    const float czz = apply_row(m, 2, p);
     if (!(czz > 0.f)) continue;
-    const float cxx = __fmaf_rn(__ldg(m + 2), pz, __fmaf_rn(__ldg(m + 1), py, __fmaf_rn(__ldg(m + 0), px, __ldg(m + 3))));
-    const float cyy = __fmaf_rn(__ldg(m + 6), pz, __fmaf_rn(__ldg(m + 5), py, __fmaf_rn(__ldg(m + 4), px, __ldg(m + 7))));
-    const float u = __fmaf_rn(fx, __fdiv_rn(cxx, czz), cx), v = __fmaf_rn(fy, __fdiv_rn(cyy, czz), cy);
-    const float xf = floorf(__fadd_rn(u, 0.5f)), yf = floorf(__fadd_rn(v, 0.5f));
-    if (!(xf >= 0.f && xf < (float)w && yf >= 0.f && yf < (float)h)) continue;      // NaN fails too
+    float xf, yf;
+    if (!nearest_pixel(project(cam, make_float3(apply_row(m, 0, p), apply_row(m, 1, p), czz)), w, h, xf, yf)) continue;
     const long long pix = (long long)yf * w + (long long)xf;
     const float d = __ldg(depth + t * plane + pix);
-    if (!(isfinite(d) && d > 0.f)) continue;
+    if (!valid_depth(d)) continue;
     const float sdf = __fsub_rn(d, czz);
     if (sdf < -trunc) continue;
     const float f = fminf(1.f, __fdiv_rn(sdf, trunc));
@@ -111,29 +108,6 @@ __device__ __forceinline__ VoxelEdges voxel_edges(const float* __restrict__ tsdf
   return v;
 }
 
-// Block-wide exclusive sum of one int per thread, in thread order; also returns the block's total.
-__device__ __forceinline__ int block_exclusive_sum(int x, int* total) {
-  __shared__ int warp_sums[FUSE_WARPS];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = x;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int y = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_sums[wid] = incl;
-  __syncthreads();
-  int before = 0, all = 0;
-#pragma unroll
-  for (int q = 0; q < FUSE_WARPS; ++q) {
-    const int s = warp_sums[q];
-    before += q < wid ? s : 0;
-    all += s;
-  }
-  *total = all;
-  return before + incl - x;
-}
-
 // Pass 1: the number of points each block of FUSE_THREADS voxels emits.
 __global__ void __launch_bounds__(FUSE_THREADS)
 tsdf_count_kernel(const float* __restrict__ tsdf, const float* __restrict__ weight, Volume vol, long long total,
@@ -143,39 +117,6 @@ tsdf_count_kernel(const float* __restrict__ tsdf, const float* __restrict__ weig
   int all;
   block_exclusive_sum(c, &all);
   if (threadIdx.x == 0) block_counts[blockIdx.x] = all;
-}
-
-// Pass 2: one CTA turns the block counts into exclusive offsets in place, FUSE_THREADS at a time, in order; the total
-// follows them at offsets[nb].
-__global__ void __launch_bounds__(FUSE_THREADS) tsdf_scan_kernel(long long* __restrict__ offsets, long long nb) {
-  __shared__ long long warp_sums[FUSE_WARPS];
-  __shared__ long long carry;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (long long base = 0; base < nb; base += FUSE_THREADS) {
-    const long long i = base + threadIdx.x;
-    const long long x = i < nb ? offsets[i] : 0;
-    long long incl = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) warp_sums[wid] = incl;
-    __syncthreads();
-    long long before = carry, all = 0;
-#pragma unroll
-    for (int q = 0; q < FUSE_WARPS; ++q) {
-      before += q < wid ? warp_sums[q] : 0;
-      all += warp_sums[q];
-    }
-    if (i < nb) offsets[i] = before + incl - x;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += all;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[nb] = carry;
 }
 
 // The gradient of F at voxel i (value F) along one axis, step voxels away in the layout: the central difference when both
@@ -550,8 +491,7 @@ int tsdf_surface_count_launch(const float* tsdf, const float* weight, int X, int
   tsdf_count_kernel<<<nb, FUSE_THREADS, 0, st>>>(tsdf, weight, make_volume(X, Y, Z, origin, 1.f),
                                                  (long long)X * Y * Z, offsets);
   if (int rc = check_launch("um_tsdf_surface_count")) return rc;
-  tsdf_scan_kernel<<<1, FUSE_THREADS, 0, st>>>(offsets, (long long)nb);
-  return check_launch("um_tsdf_surface_count");
+  return offsets_scan_launch(offsets, nb, "um_tsdf_surface_count", st);
 }
 
 int tsdf_mesh_count_launch(const float* tsdf, const float* weight, int X, int Y, int Z, long long* offsets, cudaStream_t st) {
@@ -560,8 +500,7 @@ int tsdf_mesh_count_launch(const float* tsdf, const float* weight, int X, int Y,
   tsdf_mesh_count_kernel<<<nb, FUSE_THREADS, 0, st>>>(tsdf, weight, make_volume(X, Y, Z, origin, 1.f),
                                                       (long long)X * Y * Z, offsets);
   if (int rc = check_launch("um_tsdf_mesh_count")) return rc;
-  tsdf_scan_kernel<<<1, FUSE_THREADS, 0, st>>>(offsets, (long long)nb);
-  return check_launch("um_tsdf_mesh_count");
+  return offsets_scan_launch(offsets, nb, "um_tsdf_mesh_count", st);
 }
 
 // n_points > 0 (the entry point launches nothing for an empty surface).

@@ -3,7 +3,7 @@
 // association with the per-block normal equations (um_icp_reduce), the Gauss-Newton step (um_icp_solve) and acceptance
 // (um_icp_accept).  The model maps come from um_tsdf_raycast (um_fusion.cu), unchanged.
 // Semantics and the order of operations: include/unimatch_sm100.h; the numpy statement is tests/refops_icp.py.
-#include "um_common.cuh"
+#include "um_geometry.cuh"
 
 namespace {
 
@@ -11,8 +11,6 @@ constexpr int ICP_TX = 16, ICP_TY = 8, ICP_THREADS = ICP_TX * ICP_TY, ICP_WARPS 
 constexpr int TERMS = UM_ICP_TERMS;
 constexpr int STATE = UM_ICP_STATE;
 constexpr int PIXEL_THREADS = 256;
-
-__device__ __forceinline__ bool valid_depth(float d) { return isfinite(d) && d > 0.f; }
 
 __device__ __forceinline__ int frames_valid(const int* __restrict__ n_valid, int n) {
   return min(max(__ldg(n_valid), 0), n);
@@ -41,13 +39,6 @@ icp_downsample_kernel(const float* __restrict__ src, float* __restrict__ dst, in
   dst[i] = any ? __fdiv_rn(sum, (float)c) : 0.f;
 }
 
-// The camera-frame vertex of depth d at pixel (x, y).
-__device__ __forceinline__ void vertex(float d, int x, int y, float fx, float fy, float cx, float cy, float v[3]) {
-  v[0] = __fmul_rn(d, __fdiv_rn(__fsub_rn((float)x, cx), fx));
-  v[1] = __fmul_rn(d, __fdiv_rn(__fsub_rn((float)y, cy), fy));
-  v[2] = d;
-}
-
 // One thread per pixel: the unit normal (v(x+1, y) - v) x (v(x, y+1) - v) facing the camera, 0 where not all three
 // depths are valid or the cross product vanishes.
 __global__ void __launch_bounds__(PIXEL_THREADS)
@@ -60,19 +51,19 @@ icp_normals_kernel(const float* __restrict__ depth, float* __restrict__ normal, 
   if (x + 1 < w && y + 1 < h) {
     const float d = __ldg(depth + i), dx = __ldg(depth + i + 1), dy = __ldg(depth + i + w);
     if (valid_depth(d) && valid_depth(dx) && valid_depth(dy)) {
-      float v[3], vx[3], vy[3], e1[3], e2[3], c[3];
-      vertex(d, x, y, fx, fy, cx, cy, v);
-      vertex(dx, x + 1, y, fx, fy, cx, cy, vx);
-      vertex(dy, x, y + 1, fx, fy, cx, cy, vy);
-#pragma unroll
-      for (int a = 0; a < 3; ++a) e1[a] = __fsub_rn(vx[a], v[a]), e2[a] = __fsub_rn(vy[a], v[a]);
+      const Pinhole k = {fx, fy, cx, cy};
+      const float3 v = back_project(k, (float)x, (float)y, d), vx = back_project(k, (float)(x + 1), (float)y, dx),
+                   vy = back_project(k, (float)x, (float)(y + 1), dy);
+      const float e1[3] = {__fsub_rn(vx.x, v.x), __fsub_rn(vx.y, v.y), __fsub_rn(vx.z, v.z)};
+      const float e2[3] = {__fsub_rn(vy.x, v.x), __fsub_rn(vy.y, v.y), __fsub_rn(vy.z, v.z)};
+      float c[3];
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
         const int b = (a + 1) % 3, e = (a + 2) % 3;
         c[a] = __fsub_rn(__fmul_rn(e1[b], e2[e]), __fmul_rn(e1[e], e2[b]));
       }
       const float len = __fsqrt_rn(__fmaf_rn(c[2], c[2], __fmaf_rn(c[1], c[1], __fmul_rn(c[0], c[0]))));
-      const float facing = __fmaf_rn(c[2], v[2], __fmaf_rn(c[1], v[1], __fmul_rn(c[0], v[0])));
+      const float facing = __fmaf_rn(c[2], v.z, __fmaf_rn(c[1], v.y, __fmul_rn(c[0], v.x)));
       if (len > 0.f && isfinite(len)) {
         const float s = facing > 0.f ? -len : len;
 #pragma unroll
@@ -149,22 +140,19 @@ __device__ __forceinline__ PixelTerms pixel_terms(const float* __restrict__ dept
   const float n[3] = {__ldg(live_normal + 3 * i), __ldg(live_normal + 3 * i + 1), __ldg(live_normal + 3 * i + 2)};
   if (!valid_depth(d) || (n[0] == 0.f && n[1] == 0.f && n[2] == 0.f)) return t;
   t.valid = true;
-  float v[3], p[3], nw[3];
-  vertex(d, x, y, fx, fy, cx, cy, v);
+  const Pinhole k = {fx, fy, cx, cy};
+  const float3 v = back_project(k, (float)x, (float)y, d);
+  float p[3], nw[3];
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    p[a] = __fmaf_rn(T[4 * a + 2], v[2], __fmaf_rn(T[4 * a + 1], v[1], __fmaf_rn(T[4 * a], v[0], T[4 * a + 3])));
+    p[a] = apply_row(T, a, v);
     nw[a] = __fmaf_rn(T[4 * a + 2], n[2], __fmaf_rn(T[4 * a + 1], n[1], __fmul_rn(T[4 * a], n[0])));
   }
   // projective association in the reference camera (world-to-camera rows V), integration's nearest-pixel rule
-  float c[3];
-#pragma unroll
-  for (int a = 0; a < 3; ++a)
-    c[a] = __fmaf_rn(V[4 * a + 2], p[2], __fmaf_rn(V[4 * a + 1], p[1], __fmaf_rn(V[4 * a], p[0], V[4 * a + 3])));
-  if (!(c[2] > 0.f)) return t;
-  const float u = __fmaf_rn(fx, __fdiv_rn(c[0], c[2]), cx), vv = __fmaf_rn(fy, __fdiv_rn(c[1], c[2]), cy);
-  const float xf = floorf(__fadd_rn(u, 0.5f)), yf = floorf(__fadd_rn(vv, 0.5f));
-  if (!(xf >= 0.f && xf < (float)w && yf >= 0.f && yf < (float)h)) return t;
+  const float3 c = apply_rows(V, make_float3(p[0], p[1], p[2]));
+  if (!(c.z > 0.f)) return t;
+  float xf, yf;
+  if (!nearest_pixel(project(k, c), w, h, xf, yf)) return t;
   const long long j = (long long)f * plane + (long long)yf * w + (long long)xf;
   const float D = __ldg(model_depth + j);
   const float m[3] = {__ldg(model_normal + 3 * j), __ldg(model_normal + 3 * j + 1), __ldg(model_normal + 3 * j + 2)};
@@ -192,10 +180,9 @@ __device__ __forceinline__ PixelTerms pixel_terms(const float* __restrict__ dept
   return t;
 }
 
-// One term of every thread's pixel summed over the warp (a shuffle tree; lane 0 holds the sum) into warp_sums[k].
+// One term of every thread's pixel summed over the warp (lane 0 holds the sum) into warp_sums[k].
 __device__ __forceinline__ void warp_term(double v, int k, int lane, double* warp_sums) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = da(v, __shfl_down_sync(0xffffffffu, v, o));
+  v = warp_sum_ordered(v);
   if (lane == 0) warp_sums[k] = v;
 }
 
@@ -252,11 +239,7 @@ constexpr int SUM_THREADS = 32 * (TERMS / 2);
 __device__ __forceinline__ void sum_partials(const double* __restrict__ partials, int nb, int f, double* sums) {
   const int lane = threadIdx.x & 31;
   for (int k = threadIdx.x >> 5; k < TERMS; k += TERMS / 2) {
-    double s = 0.0;
-    const double* p = partials + (long long)f * nb * TERMS + k;
-    for (int b = lane; b < nb; b += 32) s = da(s, __ldg(p + (long long)b * TERMS));
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s = da(s, __shfl_down_sync(0xffffffffu, s, o));
+    const double s = partials_sum_ordered(partials + (long long)f * nb * TERMS + k, nb, TERMS);
     if (lane == 0) sums[k] = s;
   }
   __syncthreads();

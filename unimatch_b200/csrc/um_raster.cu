@@ -3,11 +3,12 @@
 // rasteriser (um_mesh_raster), the visibility of points in depth maps (um_visible_points) and the per-frame sums of the
 // 2D depth metrics (um_depth_metrics).  Semantics and the order of operations: include/unimatch_sm100.h; the numpy
 // statement is tests/refops_raster.py.
-#include "um_common.cuh"
+#include "um_geometry.cuh"
 
 namespace {
 
 constexpr int RASTER_TILE = 16, RASTER_THREADS = RASTER_TILE * RASTER_TILE, RASTER_WARPS = RASTER_THREADS / 32;
+static_assert(RASTER_THREADS == COMPACT_THREADS, "the bin passes are compaction passes");
 constexpr int METRIC_TERMS = UM_DEPTH_METRIC_TERMS;
 
 struct RasterCam {
@@ -15,12 +16,9 @@ struct RasterCam {
   float fx, fy, cx, cy, near, far;
 };
 
-// camera coordinates of point i by the fp32 world-to-camera rows m, in um_tsdf_integrate's order
+// camera coordinates of point i by the fp32 world-to-camera rows m
 __device__ __forceinline__ float3 to_camera(const float* m, const float* __restrict__ p, long long i) {
-  const float x = __ldg(p + 3 * i), y = __ldg(p + 3 * i + 1), z = __ldg(p + 3 * i + 2);
-  return make_float3(__fmaf_rn(m[2], z, __fmaf_rn(m[1], y, __fmaf_rn(m[0], x, m[3]))),
-                     __fmaf_rn(m[6], z, __fmaf_rn(m[5], y, __fmaf_rn(m[4], x, m[7]))),
-                     __fmaf_rn(m[10], z, __fmaf_rn(m[9], y, __fmaf_rn(m[8], x, m[11]))));
+  return apply_rows(m, make_float3(__ldg(p + 3 * i), __ldg(p + 3 * i + 1), __ldg(p + 3 * i + 2)));
 }
 
 // ---- the fp64 pixel rectangle of one (view, face) ----------------------------------------------------------------
@@ -95,55 +93,14 @@ __global__ void __launch_bounds__(RASTER_THREADS)
 mesh_bin_count_kernel(const float* __restrict__ p, const int* __restrict__ faces, long long T,
                       const float* __restrict__ w2c, RasterCam cam, long long* __restrict__ block_counts) {
   __shared__ float m[12];
-  __shared__ long long warp_sums[RASTER_WARPS];
   load_rows(m, w2c, blockIdx.y);
   const long long f = (long long)blockIdx.x * RASTER_THREADS + threadIdx.x;
   long long c = 0;
   Rect r;
   if (f < T && face_rect(p, faces, f, m, cam, r)) c = rect_tiles(r);
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_down_sync(0xffffffffu, c, o);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (lane == 0) warp_sums[wid] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long s = 0;
-    for (int q = 0; q < RASTER_WARPS; ++q) s += warp_sums[q];
-    block_counts[(long long)blockIdx.y * gridDim.x + blockIdx.x] = s;
-  }
-}
-
-// Pass 2: one CTA turns the block counts into exclusive offsets in place, 256 at a time, in order; the total follows
-// them at offsets[nb].
-__global__ void __launch_bounds__(RASTER_THREADS) mesh_scan_kernel(long long* __restrict__ offsets, long long nb) {
-  __shared__ long long warp_sums[RASTER_WARPS];
-  __shared__ long long carry;
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (long long base = 0; base < nb; base += RASTER_THREADS) {
-    const long long i = base + threadIdx.x;
-    const long long x = i < nb ? offsets[i] : 0;
-    long long incl = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += y;
-    }
-    if (lane == 31) warp_sums[wid] = incl;
-    __syncthreads();
-    long long before = carry, all = 0;
-#pragma unroll
-    for (int q = 0; q < RASTER_WARPS; ++q) {
-      before += q < wid ? warp_sums[q] : 0;
-      all += warp_sums[q];
-    }
-    if (i < nb) offsets[i] = before + incl - x;
-    __syncthreads();
-    if (threadIdx.x == 0) carry += all;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) offsets[nb] = carry;
+  long long all;
+  block_exclusive_sum(c, &all);
+  if (threadIdx.x == 0) block_counts[(long long)blockIdx.y * gridDim.x + blockIdx.x] = all;
 }
 
 // Pass 3: each (view, face) writes its entries from offsets[block] + the entries of the block's earlier faces: per
@@ -153,24 +110,15 @@ mesh_bin_kernel(const float* __restrict__ p, const int* __restrict__ faces, long
                 RasterCam cam, const long long* __restrict__ offsets, long long* __restrict__ keys,
                 long long* __restrict__ values) {
   __shared__ float m[12];
-  __shared__ long long warp_sums[RASTER_WARPS];
   load_rows(m, w2c, blockIdx.y);
   const long long f = (long long)blockIdx.x * RASTER_THREADS + threadIdx.x;
   long long c = 0;
   Rect r;
   if (f < T && face_rect(p, faces, f, m, cam, r)) c = rect_tiles(r);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  long long incl = c;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const long long y = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_sums[wid] = incl;
-  __syncthreads();
+  long long all;
+  const long long before = block_exclusive_sum(c, &all);
   if (c == 0) return;
-  long long o = __ldg(offsets + (long long)blockIdx.y * gridDim.x + blockIdx.x) + incl - c;
-  for (int q = 0; q < wid; ++q) o += warp_sums[q];
+  long long o = __ldg(offsets + (long long)blockIdx.y * gridDim.x + blockIdx.x) + before;
   const long long view_base = (long long)blockIdx.y * cam.tiles_x * cam.tiles_y;
   for (int ty = r.y0 >> 4; ty <= r.y1 >> 4; ++ty) {
     const int y0 = max(r.y0, 16 * ty) - 16 * ty, y1 = min(r.y1, 16 * ty + 15) - 16 * ty;
@@ -187,9 +135,7 @@ __global__ void __launch_bounds__(RASTER_THREADS)
 mesh_ranges_kernel(const long long* __restrict__ keys, long long n, int* __restrict__ start, int* __restrict__ end) {
   const long long i = (long long)blockIdx.x * RASTER_THREADS + threadIdx.x;
   if (i >= n) return;
-  const long long key = __ldg(keys + i);
-  if (i == 0 || __ldg(keys + i - 1) != key) start[key] = (int)i;
-  if (i == n - 1 || __ldg(keys + i + 1) != key) end[key] = (int)(i + 1);
+  mark_run(keys, i, n, __ldg(keys + i), start, end);
 }
 
 // ---- the tile rasteriser -----------------------------------------------------------------------------------------
@@ -294,20 +240,18 @@ visible_points_kernel(const float* __restrict__ p, long long P, const float* __r
                       uint8_t* __restrict__ visible) {
   const long long i = (long long)blockIdx.x * RASTER_THREADS + threadIdx.x;
   if (i >= P) return;
-  const float px = __ldg(p + 3 * i), py = __ldg(p + 3 * i + 1), pz = __ldg(p + 3 * i + 2);
+  const float3 q = make_float3(__ldg(p + 3 * i), __ldg(p + 3 * i + 1), __ldg(p + 3 * i + 2));
+  const Pinhole cam = {fx, fy, cx, cy};
   const long long plane = (long long)h * w;
   bool seen = false;
   for (int t = 0; t < n && !seen; ++t) {
-    const float* m = w2c + 12 * t;
-    const float czz = __fmaf_rn(__ldg(m + 10), pz, __fmaf_rn(__ldg(m + 9), py, __fmaf_rn(__ldg(m + 8), px, __ldg(m + 11))));
+    const GlobalRows m = {w2c + 12 * t};
+    const float czz = apply_row(m, 2, q);
     if (!(czz > 0.f)) continue;
-    const float cxx = __fmaf_rn(__ldg(m + 2), pz, __fmaf_rn(__ldg(m + 1), py, __fmaf_rn(__ldg(m + 0), px, __ldg(m + 3))));
-    const float cyy = __fmaf_rn(__ldg(m + 6), pz, __fmaf_rn(__ldg(m + 5), py, __fmaf_rn(__ldg(m + 4), px, __ldg(m + 7))));
-    const float u = __fmaf_rn(fx, __fdiv_rn(cxx, czz), cx), v = __fmaf_rn(fy, __fdiv_rn(cyy, czz), cy);
-    const float xf = floorf(__fadd_rn(u, 0.5f)), yf = floorf(__fadd_rn(v, 0.5f));
-    if (!(xf >= 0.f && xf < (float)w && yf >= 0.f && yf < (float)h)) continue;
+    float xf, yf;
+    if (!nearest_pixel(project(cam, make_float3(apply_row(m, 0, q), apply_row(m, 1, q), czz)), w, h, xf, yf)) continue;
     const float d = __ldg(depth + t * plane + (long long)yf * w + (long long)xf);
-    seen = isfinite(d) && d > 0.f && czz <= __fadd_rn(d, tolerance);
+    seen = valid_depth(d) && czz <= __fadd_rn(d, tolerance);
   }
   visible[i] = seen ? 1 : 0;
 }
@@ -322,8 +266,8 @@ depth_metrics_kernel(const float* __restrict__ pred, const float* __restrict__ g
   const long long i = (long long)blockIdx.x * RASTER_THREADS + threadIdx.x;
   const long long at = (long long)blockIdx.y * hw + i;
   const float p = i < hw ? __ldg(pred + at) : 0.f, g = i < hw ? __ldg(gt + at) : 0.f;
-  const bool has = isfinite(p) && p > 0.f;
-  const bool in = has && isfinite(g) && g > 0.f && g < max_depth;
+  const bool has = valid_depth(p);
+  const bool in = has && valid_depth(g) && g < max_depth;
   double term[METRIC_TERMS];
 #pragma unroll
   for (int k = 0; k < METRIC_TERMS; ++k) term[k] = 0.0;
@@ -346,9 +290,7 @@ depth_metrics_kernel(const float* __restrict__ pred, const float* __restrict__ g
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
 #pragma unroll
   for (int k = 0; k < METRIC_TERMS; ++k) {
-    double s = term[k];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, o));
+    const double s = warp_sum_ordered(term[k]);
     if (lane == 0) warp_sums[wid][k] = s;
   }
   __syncthreads();
@@ -364,11 +306,7 @@ depth_metrics_kernel(const float* __restrict__ pred, const float* __restrict__ g
 __global__ void __launch_bounds__(32 * METRIC_TERMS)
 depth_metrics_sum_kernel(const double* __restrict__ partials, long long nb, double* __restrict__ out) {
   const int lane = threadIdx.x & 31, k = threadIdx.x >> 5, f = blockIdx.x;
-  const double* q = partials + (long long)f * nb * METRIC_TERMS + k;
-  double s = 0.0;
-  for (long long b = lane; b < nb; b += 32) s = __dadd_rn(s, __ldg(q + b * METRIC_TERMS));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) s = __dadd_rn(s, __shfl_down_sync(0xffffffffu, s, o));
+  const double s = partials_sum_ordered(partials + (long long)f * nb * METRIC_TERMS + k, nb, METRIC_TERMS);
   if (lane == 0) out[(long long)f * METRIC_TERMS + k] = s;
 }
 
@@ -396,8 +334,7 @@ int mesh_bin_count_launch(const float* points, const int* faces, long long T, co
     mesh_bin_count_kernel<<<dim3(fb, n), RASTER_THREADS, 0, st>>>(points, faces, T, w2c, cam, offsets);
     if (int rc = check_launch("um_mesh_bin_count (count)")) return rc;
   }
-  mesh_scan_kernel<<<1, RASTER_THREADS, 0, st>>>(offsets, (long long)fb * n);
-  return check_launch("um_mesh_bin_count (scan)");
+  return offsets_scan_launch(offsets, (long long)fb * n, "um_mesh_bin_count (scan)", st);
 }
 
 int mesh_bin_launch(const float* points, const int* faces, long long T, const float* w2c, int n, int h, int w, float fx,
@@ -410,12 +347,7 @@ int mesh_bin_launch(const float* points, const int* faces, long long T, const fl
 
 int mesh_ranges_launch(const long long* sorted_keys, long long total, long long n_bins, int* start, int* end,
                        cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(start, 0, 4 * n_bins, st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(end, 0, 4 * n_bins, st);
-  if (e != cudaSuccess) {
-    set_error("um_mesh_ranges: %s", cudaGetErrorString(e));
-    return UM_ECUDA;
-  }
+  if (int rc = zero_runs(start, end, n_bins, "um_mesh_ranges", st)) return rc;
   if (total == 0) return UM_OK;
   mesh_ranges_kernel<<<(unsigned)((total + RASTER_THREADS - 1) / RASTER_THREADS), RASTER_THREADS, 0, st>>>(
       sorted_keys, total, start, end);

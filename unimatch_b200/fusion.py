@@ -112,9 +112,7 @@ class TSDFVolume:
         positive (a camera inside a surface) misses.  No atomics and no host synchronisation after the one upload of the
         poses; the same result from run to run."""
         K = _intrinsics33(intrinsics, "TSDFVolume.render")
-        fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
-        if not (all(math.isfinite(v) for v in (fx, fy, cx, cy)) and fx != 0 and fy != 0):
-            raise ValueError("TSDFVolume.render: fx, fy, cx and cy must be finite, fx and fy nonzero")
+        fx, fy, cx, cy = _camera(K, "TSDFVolume.render")
         ps = [_pose44(p, "TSDFVolume.render") for p in poses]
         if not all(np.isfinite(p).all() for p in ps):
             raise ValueError("TSDFVolume.render: camera poses must be finite")
@@ -230,9 +228,7 @@ class _ICP:
             raise ValueError("%s: max_angle must be in (0, 180] degrees" % name)
         if not (math.isfinite(min_inlier_fraction) and 0 <= min_inlier_fraction <= 1):
             raise ValueError("%s: min_inlier_fraction must be in [0, 1]" % name)
-        fx, fy, cx, cy = (float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2]))
-        if not (all(math.isfinite(v) for v in (fx, fy, cx, cy)) and fx != 0 and fy != 0):
-            raise ValueError("%s: fx, fy, cx and cy must be finite, fx and fy nonzero" % name)
+        _camera(K, name)
         self.volume, self.n = volume, n
         self.levels = icp_levels(K.numpy(), h, w, levels)
         self.iterations = its[::-1]                                       # per level, finest first

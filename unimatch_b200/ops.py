@@ -536,8 +536,20 @@ def _warp_disparity(disp_next, flow):
 warp_disparity = _define("warp_disparity(Tensor disp_next, Tensor flow) -> (Tensor, Tensor)", _warp_disparity)
 
 
+# ---- offsets tables (include/unimatch_sm100.h) ---------------------------------------------------------------------
+BLOCK_THREADS = 256           # UM_TSDF_THREADS: items per block of the count ops' offsets tables and the block partials
+
+
+def _offsets_table(items, device, groups=1):
+    """A count op's offsets table, device int64 [groups ceil(items / BLOCK_THREADS) + 1]"""
+    return torch.empty((groups * -(-items // BLOCK_THREADS) + 1,), device=device, dtype=torch.int64)
+
+
+def _is_offsets_table(offsets, items, groups=1):
+    return offsets.dtype == torch.int64 and tuple(offsets.shape) == (groups * -(-items // BLOCK_THREADS) + 1,)
+
+
 # ---- TSDF fusion (include/unimatch_sm100.h, um_tsdf_*) -------------------------------------------------------------
-TSDF_THREADS = 256                                   # UM_TSDF_THREADS: voxels per block of the extraction's offsets
 
 
 def _tsdf_volume(tsdf, weight, color, name):
@@ -585,13 +597,13 @@ tsdf_integrate = _define(
 
 
 def _tsdf_surface_count(tsdf, weight):
-    """Returns the extraction's offsets, device int64 [ceil(X Y Z / TSDF_THREADS) + 1]: each block's first point, then
-    the number of points."""
+    """Returns the extraction's offsets table over the X Y Z voxels: each block's first point, then the number of
+    points."""
     _f32c(tsdf, "tsdf"), _f32c(weight, "weight")
     if tsdf.dim() != 3 or tuple(weight.shape) != tuple(tsdf.shape) or weight.device != tsdf.device:
         raise RuntimeError("tsdf_surface_count: expected tsdf and weight [Z, Y, X] on one device")
     z, y, x = tsdf.shape
-    offsets = torch.empty((-(-tsdf.numel() // TSDF_THREADS) + 1,), device=tsdf.device, dtype=torch.int64)
+    offsets = _offsets_table(tsdf.numel(), tsdf.device)
     _check(LIB.um_tsdf_surface_count(_p(tsdf), _p(weight), x, y, z, _p(offsets), _stream()), "um_tsdf_surface_count")
     return offsets
 
@@ -602,8 +614,7 @@ tsdf_surface_count = _define("tsdf_surface_count(Tensor tsdf, Tensor weight) -> 
 def _tsdf_surface_points(tsdf, weight, color, origin, voxel_size, offsets, n_points):
     """The surface's n_points points (fp32 [P, 3]) and colours (uint8 [P, 3]) from `tsdf_surface_count`'s offsets."""
     x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_surface_points")
-    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-tsdf.numel() // TSDF_THREADS) + 1,) \
-            or offsets.device != tsdf.device:
+    if not _is_offsets_table(offsets, tsdf.numel()) or offsets.device != tsdf.device:
         raise RuntimeError("tsdf_surface_points: offsets must be tsdf_surface_count's device int64 table")
     points = torch.empty((n_points, 3), device=tsdf.device, dtype=torch.float32)
     colors = torch.empty((n_points, 3), device=tsdf.device, dtype=torch.uint8)
@@ -619,13 +630,13 @@ tsdf_surface_points = _define(
 
 
 def _tsdf_mesh_count(tsdf, weight):
-    """Returns the mesh's face offsets, device int64 [ceil(X Y Z / TSDF_THREADS) + 1]: the first triangle of each block's
-    cubes, then the number of triangles."""
+    """Returns the mesh's face offsets table over the X Y Z voxels: the first triangle of each block's cubes, then the
+    number of triangles."""
     _f32c(tsdf, "tsdf"), _f32c(weight, "weight")
     if tsdf.dim() != 3 or tuple(weight.shape) != tuple(tsdf.shape) or weight.device != tsdf.device:
         raise RuntimeError("tsdf_mesh_count: expected tsdf and weight [Z, Y, X] on one device")
     z, y, x = tsdf.shape
-    offsets = torch.empty((-(-tsdf.numel() // TSDF_THREADS) + 1,), device=tsdf.device, dtype=torch.int64)
+    offsets = _offsets_table(tsdf.numel(), tsdf.device)
     _check(LIB.um_tsdf_mesh_count(_p(tsdf), _p(weight), x, y, z, _p(offsets), _stream()), "um_tsdf_mesh_count")
     return offsets
 
@@ -637,9 +648,8 @@ def _tsdf_mesh(tsdf, weight, color, origin, voxel_size, point_offsets, n_points,
     """The mesh's n_points vertices (fp32 [P, 3]), colours (uint8 [P, 3]) and normals (fp32 [P, 3]) and its n_faces
     triangles (int32 [T, 3]) from `tsdf_surface_count`'s and `tsdf_mesh_count`'s offsets."""
     x, y, z = _tsdf_volume(tsdf, weight, color, "tsdf_mesh")
-    nb = -(-tsdf.numel() // TSDF_THREADS) + 1
     for t in (point_offsets, face_offsets):
-        if t.dtype != torch.int64 or tuple(t.shape) != (nb,) or t.device != tsdf.device:
+        if not _is_offsets_table(t, tsdf.numel()) or t.device != tsdf.device:
             raise RuntimeError("tsdf_mesh: the offsets must be tsdf_surface_count's and tsdf_mesh_count's device int64 tables")
     dev = tsdf.device
     points = torch.empty((n_points, 3), device=dev, dtype=torch.float32)
@@ -820,7 +830,6 @@ icp_accept = _define(
 
 
 # ---- point clouds (include/unimatch_sm100.h, um_cloud_*) -----------------------------------------------------------
-CLOUD_THREADS = 256                                  # queries and sorted positions per block of the cloud kernels
 
 
 def _cloud_points(t, name):
@@ -875,12 +884,12 @@ cloud_ranges = _define("cloud_ranges(Tensor sorted_keys, Tensor order, Tensor po
 
 
 def _cloud_down_sample_count(sorted_keys):
-    """The down-sampling offsets, device int64 [ceil(n / CLOUD_THREADS) + 1]: each block's first output row, then the
-    number of occupied cells"""
+    """The down-sampling offsets table over the n sorted positions: each block's first output row, then the number of
+    occupied cells"""
     if sorted_keys.dtype != torch.int64 or sorted_keys.dim() != 1 or not sorted_keys.is_contiguous():
         raise RuntimeError("cloud_down_sample_count: sorted_keys must be contiguous int64 [n]")
     n = sorted_keys.shape[0]
-    offsets = torch.empty((-(-n // CLOUD_THREADS) + 1,), device=sorted_keys.device, dtype=torch.int64)
+    offsets = _offsets_table(n, sorted_keys.device)
     _check(LIB.um_cloud_down_sample_count(_p(sorted_keys), n, _p(offsets), _stream()), "um_cloud_down_sample_count")
     return offsets
 
@@ -891,8 +900,7 @@ cloud_down_sample_count = _define("cloud_down_sample_count(Tensor sorted_keys) -
 def _cloud_down_sample(sorted_keys, order, points, offsets, m):
     """The m occupied cells' mean points fp32 [m, 3], in key order"""
     n = _cloud_sorted(sorted_keys, order, points, "cloud_down_sample")
-    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-n // CLOUD_THREADS) + 1,) \
-            or offsets.device != points.device:
+    if not _is_offsets_table(offsets, n) or offsets.device != points.device:
         raise RuntimeError("cloud_down_sample: offsets must be cloud_down_sample_count's device int64 table")
     out = torch.empty((m, 3), device=points.device, dtype=torch.float32)
     _check(LIB.um_cloud_down_sample(_p(sorted_keys), _p(order), _p(points), n, _p(offsets), m, _p(out), _stream()),
@@ -935,10 +943,10 @@ cloud_nearest = _define("cloud_nearest(Tensor queries, Tensor sorted_points, Ten
 
 
 def _cloud_nearest_partials(queries, sorted_points, start, end, origin, cell, threshold):
-    """cloud_nearest's distances reduced per block of CLOUD_THREADS queries: the fp64 sum of d and the int64 count of
-    d < threshold, [ceil(nq / CLOUD_THREADS)] each"""
+    """cloud_nearest's distances reduced per block of BLOCK_THREADS queries: the fp64 sum of d and the int64 count of
+    d < threshold, [ceil(nq / BLOCK_THREADS)] each"""
     nq, n, dims = _cloud_nearest_args(queries, sorted_points, start, end, "cloud_nearest_partials")
-    nb = -(-nq // CLOUD_THREADS)
+    nb = -(-nq // BLOCK_THREADS)
     psum = torch.empty((nb,), device=queries.device, dtype=torch.float64)
     pcount = torch.empty((nb,), device=queries.device, dtype=torch.int64)
     _check(LIB.um_cloud_nearest(_p(queries), nq, _p(sorted_points), _p(start), _p(end), n,
@@ -993,10 +1001,10 @@ def _mesh_args(points, faces, w2c, name):
 
 
 def _mesh_bin_count(points, faces, w2c, h, w, fx, fy, cx, cy, near, far):
-    """The bin offsets, device int64 [n ceil(T / 256) + 1]: per (view, block of 256 faces) its first tile entry, then the
-    number of entries"""
+    """The bin offsets table over the T faces of each of the n views, view-major: per (view, block of faces) its first
+    tile entry, then the number of entries"""
     p, t, n = _mesh_args(points, faces, w2c, "mesh_bin_count")
-    offsets = torch.empty((n * -(-t // 256) + 1,), device=points.device, dtype=torch.int64)
+    offsets = _offsets_table(t, points.device, groups=n)
     _check(LIB.um_mesh_bin_count(_p(points), p, _p(faces), t, _p(w2c), n, h, w, fx, fy, cx, cy, near, far, _p(offsets),
                                  _stream()), "um_mesh_bin_count")
     return offsets
@@ -1009,7 +1017,7 @@ mesh_bin_count = _define("mesh_bin_count(Tensor points, Tensor faces, Tensor w2c
 def _mesh_bin(points, faces, w2c, h, w, fx, fy, cx, cy, near, far, offsets, n_entries):
     """The n_entries tile entries: keys int64 (view * tiles + tile) and values int64 (face << 16 | in-tile rectangle)"""
     p, t, n = _mesh_args(points, faces, w2c, "mesh_bin")
-    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (n * -(-t // 256) + 1,) or offsets.device != points.device:
+    if not _is_offsets_table(offsets, t, groups=n) or offsets.device != points.device:
         raise RuntimeError("mesh_bin: offsets must be mesh_bin_count's device int64 table")
     keys = torch.empty((n_entries,), device=points.device, dtype=torch.int64)
     values = torch.empty_like(keys)
@@ -1092,7 +1100,7 @@ def _depth_metrics(pred, gt, max_depth):
         raise RuntimeError("depth_metrics: expected pred and gt [n, h, w] of one shape")
     _device_like("depth_metrics", pred, gt)
     n, h, w = pred.shape
-    partials = torch.empty((n, -(-(h * w) // 256), DEPTH_METRIC_TERMS), device=pred.device, dtype=torch.float64)
+    partials = torch.empty((n, -(-(h * w) // BLOCK_THREADS), DEPTH_METRIC_TERMS), device=pred.device, dtype=torch.float64)
     out = torch.empty((n, DEPTH_METRIC_TERMS), device=pred.device, dtype=torch.float64)
     _check(LIB.um_depth_metrics(_p(pred), _p(gt), n, h, w, max_depth, _p(partials), _p(out), _stream()),
            "um_depth_metrics")
@@ -1137,13 +1145,13 @@ depth_consistency = _define("depth_consistency(Tensor depth, Tensor c2w, Tensor 
 
 
 def _depth_points_count(depth):
-    """The point offsets of depths [n, h, w], device int64 [ceil(n h w / 256) + 1]: per block of 256 pixels its first
+    """The point offsets table of depths [n, h, w] over the n h w pixels (frame-major): per block of pixels its first
     point, then the number of points"""
     _f32c(depth, "depth_points_count: depth")
     if depth.dim() != 3:
         raise RuntimeError("depth_points_count: expected depths [n, h, w]")
     n, h, w = depth.shape
-    offsets = torch.empty((-(-(n * h * w) // 256) + 1,), device=depth.device, dtype=torch.int64)
+    offsets = _offsets_table(n * h * w, depth.device)
     _check(LIB.um_depth_points_count(_p(depth), n, h, w, _p(offsets), _stream()), "um_depth_points_count")
     return offsets
 
@@ -1160,7 +1168,7 @@ def _depth_points(depth, frames, c2w, fx, fy, cx, cy, offsets, n_points):
     _rows34(c2w, n, "depth_points: c2w")
     if frames.dtype != torch.uint8 or tuple(frames.shape) != (n, h, w, 3) or not frames.is_contiguous():
         raise RuntimeError("depth_points: frames must be contiguous uint8 [n, h, w, 3]")
-    if offsets.dtype != torch.int64 or tuple(offsets.shape) != (-(-(n * h * w) // 256) + 1,):
+    if not _is_offsets_table(offsets, n * h * w):
         raise RuntimeError("depth_points: offsets must be depth_points_count's int64 table")
     _device_like("depth_points", depth, frames, c2w, offsets)
     points = torch.empty((n_points, 3), device=depth.device, dtype=torch.float32)
